@@ -1,7 +1,8 @@
-"""bench.py - headline benchmark of the B200 vocoder / synthesizer hot path (contract: see DESIGN.md section 6).
+"""bench.py - headline benchmark of the H100 vocoder / synthesizer hot path (contract: see DESIGN.md section 6).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--no-secondary] [--no-cpu-baseline]
                     [--workload hifigan_cfg2|fregan_cfg2|wavernn_cfg1|wavernn_cfg3|tacotron_cfg4|e2e_cfg5] [--precision ...]
+                    [--dump-outputs DIR]
 
 Prints ONE JSON line (rank 0).  The headline is BASELINE.json configs[1] (the config the metric is quoted on): HiFi-GAN
 Generator forward, batch 32 random mels of 256 frames x 80 bins per GPU; a "step" is one forward over one batch; under
@@ -11,7 +12,7 @@ torchrun every rank runs its own batch (weak scaling: utterance batches shard ac
              step ("burst" = the same K steps timed right after warm-up, reported beside it)
   e2e        same metric through the drop-in module surface hifigan.inference.infer_waveforms() with HOST numpy mels:
              pinned H2D of the batch and D2H of the waveforms inside the timed region, host sync every step
-  roofline   the tcgen05 conv kernel family: layer-granular algorithmic bytes / CUDA-event time of those launches
+  roofline   the tensor-core (wgmma) conv kernel: layer-granular algorithmic bytes / CUDA-event time of those launches
              (separate profiled pass) vs the measured HBM copy bandwidth; roofline_tensor: FLOPs vs the measured bf16 peak
              (burst peak for the burst figure, sustained peak for the soaked one)
   cpu_baseline  the oracle port of the reference forward on the host cores, bounded sample (rank 0, N = 1 only)
@@ -20,6 +21,10 @@ torchrun every rank runs its own batch (weak scaling: utterance batches shard ac
              tacotron_cfg4 (configs[3]), e2e_cfg5 (configs[4], weak: 128 utterances per GPU; strong: 1024 utterances
              over N GPUs), hifigan_fp32_equivalent (3-term split everywhere), and at N > 1 the fold-sharded cfg 3
 --impl reference: the CPU implementation (oracle port, all host threads) on the same config (rank 0 only).
+--dump-outputs DIR: after the timed steps of the selected workload, rank 0 writes what its last resident step returned as
+             DIR/<name>.npy (dump_outputs; at most 64 MB, a fixed seeded sample when larger): HiFi-GAN / Fre-GAN wav, WaveRNN indices,
+             Tacotron mel / linear / attention, e2e wav.  Inputs and weights are seeded, so two builds can be compared output for output.
+--steps K: the number of timed steps of the selected workload (the secondaries of the HiFi-GAN line use their own counts).
 """
 from __future__ import annotations
 
@@ -50,6 +55,7 @@ def parse():
     ap.add_argument("--soak-seconds", type=float, default=2.0)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true", help="headline workload only")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs as DIR/<name>.npy")
     ap.add_argument("--cpu-child", nargs=3, default=None, help=argparse.SUPPRESS)
     return ap.parse_args()
 
@@ -130,7 +136,7 @@ def run_reference(args):
 # ------------------------------------------------------------------------------------------------
 # ------------------------------------------------------------------------------------------------
 def measure_hifigan(ctx: Ctx, args, workload: str, precision: str, steps: int, warmup: int, soak_s: float, cpu: bool,
-                    roofline: bool = True):
+                    roofline: bool = True, dump: bool = False):
     """HiFi-GAN / Fre-GAN generator forward on the cfg-2 batch shape; returns the JSON dict (rank 0) or None."""
     import numpy as np
     import torch
@@ -161,7 +167,7 @@ def measure_hifigan(ctx: Ctx, args, workload: str, precision: str, steps: int, w
     produced = {"n": 0}
 
     def step_resident():
-        g(mel_dev)
+        ctx.outputs = {"wav": g(mel_dev)}
 
     def step_e2e():
         wavs = mod.infer_waveforms(mels_np, batch_size=B)   # host numpy in, host numpy out, host sync inside
@@ -173,6 +179,8 @@ def measure_hifigan(ctx: Ctx, args, workload: str, precision: str, steps: int, w
     launches_total = int(lib.mb_launch_count() - l0)
     launches = int(round(launches_total * steps / (max(3, warmup) + 2 * steps + r["soak_steps"])))
     log(f"resident: soaked {r['ms'] / steps:.3f} ms/step, burst {r['ms_burst'] / steps:.3f}; e2e pass")
+    if dump:
+        dump_outputs(ctx, args)
     e = ctx.timed(step_e2e, steps, 2, min(soak_s, 1.0), host_clock=True)
     assert produced["n"] == samples_per_step
     ms_step = r["ms"] / steps
@@ -201,7 +209,7 @@ def measure_hifigan(ctx: Ctx, args, workload: str, precision: str, steps: int, w
         total_flops = sum(v[1] for v in acc.values()) / reps
         if precision != "fp32":
             mma_mult = 3.0 if precision == "f16x3" else 1.0
-            roof_tensor = {"bound": "tensor", "kernel": f"tc_conv / tc_pair ({dom})", "unit": "TFLOP/s",
+            roof_tensor = {"bound": "tensor", "kernel": f"tc_conv ({dom})", "unit": "TFLOP/s",
                            "achieved_soaked": total_flops / (ms_step * 1e-3) / 1e12, "peak_sustained": pk["tflops_sustained"],
                            "frac_soaked": mma_mult * total_flops / (ms_step * 1e-3) / 1e12 / pk["tflops_sustained"],
                            "achieved_burst": total_flops / (ms_burst * 1e-3) / 1e12, "peak_burst": pk["tflops_burst"],
@@ -212,21 +220,16 @@ def measure_hifigan(ctx: Ctx, args, workload: str, precision: str, steps: int, w
             fam_ms = sum(acc[k][0] for k in fam) / reps
             fam_bytes = sum(acc[k][2] for k in fam) / reps
             fam_launches = sum(acc[k][3] for k in fam) / reps
-            traffic = None
-            tj = ROOT / "profiles" / "r02_hifigan_dram_traffic.json"
-            if tj.exists() and not fre and precision == "f16tc":
-                traffic = json.loads(tj.read_text())["tc_dram_bytes_per_launch"]
             gbs = fam_bytes / (fam_ms * 1e-3) / 1e9
-            roof = {"bound": "hbm", "kernel": "tc_conv_kernel + tc_pair_kernel (tcgen05 tap convs; all layers but conv_post)",
-                    "achieved": gbs, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": gbs / pk["hbm_gbs"], "traffic": traffic,
-                    "traffic_source": "ncu dram__bytes_read.sum + dram__bytes_write.sum per launch (profiles/)",
+            roof = {"bound": "hbm", "kernel": "tc_conv_kernel (wgmma tap convs; all layers but conv_post)",
+                    "achieved": gbs, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": gbs / pk["hbm_gbs"],
                     "plan_ops_per_step": fam_launches, "algorithmic_bytes_per_op": fam_bytes / max(fam_launches, 1),
                     "algorithmic_bytes_per_step": fam_bytes, "ms_per_step_in_kernel": fam_ms,
                     "share_of_step": fam_ms / ms_step, "peak_source": pk["source"] + ", HBM copy bandwidth",
                     "definition": "layer-granular fp32 bytes (inputs + outputs of every conv layer + weights once, SURVEY.md 8d) / "
                                   "event-timed duration of those launches (profiled pass, no PDL overlap)"}
         else:
-            peak = 72.0  # 148 SM x 128 lanes x 2 x ~1.9 GHz FP32 FFMA, nominal
+            peak = 67.0  # H100 SXM data sheet, FP32 (non-tensor), nominal
             roof = {"bound": "tensor", "kernel": f"tapconv_f32 ({dom})", "achieved": tf, "peak": peak, "unit": "TFLOP/s",
                     "frac": tf / peak, "traffic": None, "peak_source": "nominal fp32 FFMA (parity-anchor path)",
                     "launches_timed": cnt, "share_of_step": (t_ms / reps) / ms_step}
@@ -257,7 +260,7 @@ def measure_hifigan(ctx: Ctx, args, workload: str, precision: str, steps: int, w
         "config": {"workload": f"{workload}: Generator fwd, batch 32 x 256 frames x 80 mels per GPU",
                    "per_gpu_batch": B, "frames": T, "precision": precision, "precision_requested": requested,
                    "precision_calibration": g.calibration, "parallelism": f"dp{world}",
-                   "l2": "per-step working set (2.9 GB of activations) >> 126 MB L2; no explicit flush",
+                   "l2": "per-step working set (2.9 GB of activations) >> 50 MB L2; no explicit flush",
                    "weights": "random init, torch.manual_seed(0) order of the reference constructor"},
         "burst": {"value": world * samples_per_step / (ms_burst * 1e-3), "ms_per_step": ms_burst, "clocks": r["clocks_burst"]},
         "soak": {"seconds": r["soak_s"], "steps": r["soak_steps"], "clocks": r["clocks_soak"]},
@@ -268,6 +271,34 @@ def measure_hifigan(ctx: Ctx, args, workload: str, precision: str, steps: int, w
         "gpu_launches": launches, "clocks": r["clocks"], "roofline": roof, "roofline_tensor": roof_tensor,
         "roofline_hbm_step": roof_hbm, "step_tflops": step_tf, "cpu_baseline": cpu_d,
     }
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(ctx, args):
+    """--dump-outputs DIR: write what the last timed step of the selected workload returned (ctx.outputs) as DIR/<name>.npy,
+    float64 arrays as float64 and everything else as float32.  When the arrays exceed 64 MB together, each one is cut to a
+    fixed, seeded sample of its flattened elements (same positions every run) of its share of the budget."""
+    import numpy as np
+
+    if not args.dump_outputs or ctx.rank != 0:
+        return
+    if not ctx.outputs:
+        raise RuntimeError(f"--dump-outputs: workload {args.workload} recorded no outputs")
+    arrays = {}
+    for name, v in ctx.outputs.items():
+        a = v.detach().cpu().numpy() if hasattr(v, "detach") else np.asarray(v)
+        arrays[name] = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+    total = sum(a.nbytes for a in arrays.values())
+    out_dir = Path(args.dump_outputs)
+    out_dir.mkdir(parents=True, exist_ok=True)
+    for name, a in arrays.items():
+        if total > DUMP_BYTES:
+            keep = max(1, int(a.size * DUMP_BYTES / total))
+            pos = np.sort(np.random.default_rng(0).choice(a.size, size=keep, replace=False))
+            a = a.reshape(-1)[pos]
+        np.save(out_dir / f"{name}.npy", a)
 
 
 def _short(d, keys=("value", "unit", "ms_per_step", "burst", "e2e", "roofline", "cpu_baseline", "config", "dtype", "gpu_launches",
@@ -281,7 +312,7 @@ def run_ours(args):
     try:
         cpu = (not args.no_cpu_baseline) and ctx.world == 1
         if args.workload in ("hifigan_cfg2", "fregan_cfg2"):
-            line = measure_hifigan(ctx, args, args.workload, args.precision, args.steps, args.warmup, args.soak_seconds, cpu)
+            line = measure_hifigan(ctx, args, args.workload, args.precision, args.steps, args.warmup, args.soak_seconds, cpu, dump=True)
             secondary = {}
             if args.workload == "hifigan_cfg2" and not args.no_secondary:
                 import bench_e2e
@@ -319,11 +350,12 @@ def run_ours(args):
             import bench_tacotron
             import bench_wavernn
 
-            fn = {"wavernn_cfg1": lambda: bench_wavernn.measure_cfg1(ctx, args, cpu),
-                  "wavernn_cfg3": lambda: bench_wavernn.measure_cfg3(ctx, args, cpu, steps=max(3, min(args.steps, 5))),
-                  "tacotron_cfg4": lambda: bench_tacotron.measure(ctx, args, cpu, steps=max(1, min(args.steps, 10))),
-                  "e2e_cfg5": lambda: bench_e2e.measure(ctx, args, cpu, steps=max(1, min(args.steps, 5)))}[args.workload]
+            fn = {"wavernn_cfg1": lambda: bench_wavernn.measure_cfg1(ctx, args, cpu, steps=args.steps),
+                  "wavernn_cfg3": lambda: bench_wavernn.measure_cfg3(ctx, args, cpu, steps=args.steps),
+                  "tacotron_cfg4": lambda: bench_tacotron.measure(ctx, args, cpu, steps=args.steps),
+                  "e2e_cfg5": lambda: bench_e2e.measure(ctx, args, cpu, steps=args.steps)}[args.workload]
             line = fn()
+            dump_outputs(ctx, args)
             if ctx.rank == 0:
                 print(json.dumps(line), flush=True)
     finally:

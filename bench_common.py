@@ -67,7 +67,7 @@ def peaks():
         d = json.loads(p.read_text())
         return {"hbm_gbs": d["hbm_gbs"], "tflops_burst": d["bf16_tflops"],
                 "tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "tflops_burst": 1590.0, "tflops_sustained": 1400.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "tflops_burst": 989.0, "tflops_sustained": 989.0, "source": "H100 SXM data sheet (700 W), not measured"}
 
 
 class ClockSampler:
@@ -162,6 +162,7 @@ class Ctx:
         if self.world > 1 and not dist.is_initialized():
             dist.init_process_group("nccl", device_id=self.dev)
         self.sampler = ClockSampler(self.local).start()
+        self.outputs = {}  # name -> what the last resident (timed) step returned; bench.py --dump-outputs writes it
 
     def close(self):
         self.sampler.stop()

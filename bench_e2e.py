@@ -150,11 +150,14 @@ def measure(ctx, args, cpu: bool, steps: int = 2, strong_total: int = 0):
     def step_resident():
         emb = enc.reduce_partials(enc.forward(parts_dev), offsets)
         n = 0
+        wavs = []
         for bi, c in enumerate(chars_dev):
             _, lin, _ = taco.generate(c, emb[bi * TBATCH: bi * TBATCH + c.shape[0]], steps=STEPS, style_idx=-1, min_stop_token=10)
             for v in range(0, lin.shape[0], VBATCH):
-                n += gen(lin[v:v + VBATCH].contiguous()).numel()
+                wavs.append(gen(lin[v:v + VBATCH].contiguous()))
+                n += wavs[-1].numel()
         produced["samples"] = n
+        ctx.outputs = {"wav": torch.cat([w.reshape(w.shape[0], -1) for w in wavs])}
 
     def step_e2e():
         embeds = enc_inf.embed_utterances_frames(parts)

@@ -98,7 +98,8 @@ def measure(ctx, args, cpu: bool, steps: int = 3):
     shp.synthesis_batch_size = B  # one padded batch of 64 like the config (the reference default is 16)
 
     def step_resident():
-        model.generate(chars_dev, emb_dev, steps=STEPS, style_idx=-1, min_stop_token=10)
+        mel, linear, attn = model.generate(chars_dev, emb_dev, steps=STEPS, style_idx=-1, min_stop_token=10)
+        ctx.outputs = {"mel": mel, "linear": linear, "attn": attn}
 
     def step_e2e():
         syn.synthesize_from_sequences(seqs, embs, False, -1, 10, STEPS)
@@ -134,7 +135,7 @@ def measure(ctx, args, cpu: bool, steps: int = 3):
                 "h2d_bytes_per_step": int(B * TC * 8 + B * 256 * 4), "d2h_bytes_per_step": int(frames * 80 * 4),
                 "ms_per_step": e["ms"] / steps, "surface": "Synthesizer.synthesize_from_sequences (host ids / embeds -> host numpy mels)"},
         "gpu_launches": launches, "clocks": r["clocks"],
-        "roofline": {"bound": "tensor", "kernel": "tc_skinny / tc_gru / tc_big (tcgen05 GEMMs, 3-term fp16 split = 3 MMA flops per "
+        "roofline": {"bound": "tensor", "kernel": "tc_skinny / tc_gru / tc_big (wgmma GEMMs, 3-term fp16 split = 3 MMA flops per "
                                                    "useful flop, FP32-equivalent)",
                      "achieved": flops / (ms * 1e-3) / 1e12, "peak": pk["tflops_sustained"], "unit": "TFLOP/s",
                      "frac": 3.0 * flops / (ms * 1e-3) / 1e12 / pk["tflops_sustained"], "traffic": None,

@@ -129,7 +129,7 @@ def measure_cfg1(ctx, args, cpu: bool, steps: int = 3):
 
     def step_resident():
         torch.manual_seed(1234)
-        model.generate_indices(mel_dev, False, TARGET, OVERLAP, None)
+        ctx.outputs = {"indices": model.generate_indices(mel_dev, False, TARGET, OVERLAP, None)}
 
     r = ctx.timed(step_resident, steps, 1, 1.0, host_clock=True)
     e = ctx.timed(step_e2e, steps, 1, 0.0, host_clock=True)
@@ -164,21 +164,23 @@ def measure_cfg3(ctx, args, cpu: bool, steps: int = 3):
     out = {}
 
     def step_resident():
-        model.generate_indices(mel_dev, True, TARGET, OVERLAP, None)
+        ctx.outputs = {f"indices_{model.rng}": model.generate_indices(mel_dev, True, TARGET, OVERLAP, None)}
 
     def step_e2e():
         wav, _ = rnn_vocoder.infer_waveform(mel_np, batched=True, target=TARGET, overlap=OVERLAP, progress_callback=lambda *a: None)
         out["n"] = len(wav)
 
-    res = {}
+    res, outputs = {}, {}
     for mode in ("torch", "device"):
         model.rng = mode
         torch.manual_seed(1234)
         l0 = lib.mb_launch_count()
         r = ctx.timed(step_resident, steps, 1, 0.0, host_clock=True)
         launches = int(lib.mb_launch_count() - l0) * steps // (2 * steps + 1)
+        outputs.update(ctx.outputs)
         e = ctx.timed(step_e2e, steps, 1, 0.0, host_clock=True)
         res[mode] = (r, e, launches)
+    ctx.outputs = outputs
     model.rng = "torch"
     if ctx.rank != 0:
         return None

@@ -1,5 +1,5 @@
 /*
- * mockingbird_b200 - C ABI of the B200-native (sm_100a) vocoder / mel-synthesizer hot path.
+ * mockingbird_b200 - C ABI of the H100-native (sm_90a) vocoder / mel-synthesizer hot path.
  *
  * This is the drop-in boundary (SURVEY.md section 8b).  The reference (babysor/MockingBird) has no
  * FFI of its own: its callers talk to duck-typed Python module singletons.  The Python host layer
@@ -44,7 +44,7 @@ extern "C" {
 
 /* library-wide ----------------------------------------------------------------------------- */
 const char* mb_last_error(void);
-/* "mockingbird_b200 <ver> sm_100a"; never NULL */
+/* "mockingbird_b200 <ver> sm_90a"; never NULL */
 const char* mb_version(void);
 /* number of kernel launches issued by this library since load (all handles); used by bench.py
  * to report gpu_launches from a counter rather than from a guess */
@@ -61,9 +61,9 @@ uint64_t mb_launch_count(void);
 
 /* arithmetic of the channel-mixing convolutions */
 #define MB_PREC_FP32 0      /* FP32 FFMA everywhere (parity anchor, ~1e-6 of the reference)     */
-#define MB_PREC_F16TC 1     /* tcgen05 tensor cores: fp16 operands, fp32 accumulate, fp32
+#define MB_PREC_F16TC 1     /* wgmma tensor cores: fp16 operands, fp32 accumulate, fp32
                                residual stream; conv_post in fp32 (tolerance 1e-3, see DESIGN.md) */
-#define MB_PREC_F16X3 2     /* tcgen05 tensor cores with the 3-term fp16 split on EVERY layer
+#define MB_PREC_F16X3 2     /* wgmma tensor cores with the 3-term fp16 split on EVERY layer
                                (x*w = hi*hi + lo*hi + hi*lo, fp32 accumulate): FP32-equivalent results
                                (~1e-5 of the reference) at 3x the MMA work of MB_PREC_F16TC            */
 

@@ -1,4 +1,4 @@
-"""mockingbird_b200: B200-native (sm_100a) vocoder / mel-synthesizer inference hot path of
+"""mockingbird_b200: H100-native (sm_90a) vocoder / mel-synthesizer inference hot path of
 babysor/MockingBird behind the reference's own Python inference surfaces.
 
     from mockingbird_b200.vocoder.hifigan import inference as gan_vocoder

@@ -205,5 +205,5 @@ def require_cuda():
     import torch
 
     if not torch.cuda.is_available():
-        raise MbError("mockingbird_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise MbError("mockingbird_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
     return torch.device("cuda", torch.cuda.current_device())

@@ -1,4 +1,4 @@
-"""In-tree build of libmockingbird_b200.so (nvcc, sm_100a only).
+"""In-tree build of libmockingbird_b200.so (nvcc, sm_90a only).
 
 The shared library is the product's compute path; there is no CPU fallback.  The built .so is
 git-ignored but travels to the GPU box with the repo snapshot.
@@ -17,7 +17,7 @@ LIB_PATH = PKG_DIR / "libmockingbird_b200.so"
 STAMP = PKG_DIR / ".libmockingbird_b200.hash"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-fmad=false",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-fmad=false",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-O3", "-shared", "-lpthread",
 ]
 
@@ -94,7 +94,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     errs = [e for _, e in results if e]
     if errs:
         raise RuntimeError("nvcc failed:\n" + "\n".join(errs))
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(LIB_PATH), *[str(o) for o, _ in results],
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", str(LIB_PATH), *[str(o) for o, _ in results],
            "-lpthread"]
     proc = subprocess.run(cmd, cwd=str(CSRC), capture_output=True, text=True)
     if proc.returncode != 0:

@@ -1,4 +1,4 @@
-// DeepMind-style dual-softmax WaveRNN on the B200 (SURVEY.md 8f row N3; mb_deepmind_*).
+// DeepMind-style dual-softmax WaveRNN on the H100 (SURVEY.md 8f row N3; mb_deepmind_*).
 //   replaces  models/vocoder/wavernn/models/deepmind_version.py:75-162 (WaveRNN.generate): one unconditioned row, per sample two
 //             dependent half-steps (coarse 8 bits, then fine 8 bits given the coarse draw):
 //               R h (896 -> 2688, split coarse/fine x u,r,e) ; gates u,r = sigmoid, e = tanh(r * R_e + I_e + b_e) ;

@@ -1,4 +1,4 @@
-// Speaker encoder inference on B200 (mb_encoder_*): 3-layer LSTM over partial-utterance mel frames,
+// Speaker encoder inference on H100 (mb_encoder_*): 3-layer LSTM over partial-utterance mel frames,
 // last hidden state -> Linear -> ReLU -> L2 normalise; utterance embedding = L2(mean of partials).
 //
 // reference: models/encoder/model.py:41-61 (SpeakerEncoder.forward),

@@ -121,7 +121,7 @@ void touch(mb_gan* h, int buf, int c, int rate) {
 
 // Tensor-core path: internal tensors with fewer than 32 channels (Fre-GAN's full-rate stage has 16) are carried with
 // 32 channels, the extra ones identically zero (zero weight rows / columns and biases), so that the whole stage runs
-// on the C = 32 tcgen05 kernels instead of the FP32 FFMA kernels.  MB_GAN_PAD16=0 disables it.
+// on the C = 32 tensor-core kernels instead of the FP32 FFMA kernels.  MB_GAN_PAD16=0 disables it.
 int pad_channels(const mb_gan* h, int c) {
   static const bool env = [] {
     const char* e = getenv("MB_GAN_PAD16");

@@ -393,7 +393,7 @@ cudaError_t launch_add_inplace_f32(const TRef& dst32, const TRef& src32, const T
   const size_t n = (size_t)B * dst32.C * dst32.L;
   const int threads = 256;
   size_t blocks = (n + threads - 1) / threads;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (blocks == 0) return cudaSuccess;
   add_inplace_kernel<<<(unsigned)blocks, threads, 0, stream>>>(dst32, src32, dst16, slope, B);
   return cudaGetLastError();

@@ -1,11 +1,11 @@
-// Tensor-core execution of the GAN generator plan (MB_PREC_F16TC), sm_100a only.
+// Tensor-core execution of the GAN generator plan (MB_PREC_F16TC), sm_90a (Hopper warpgroup MMA).
 //
-// tc_conv_kernel: the tap conv (gan_kernels.h) as an implicit GEMM on tcgen05 tensor cores.
-//   D[128 rows x Cout] (fp32, TMEM) += A[128 rows x 16 ci] (fp16, smem) * B[Cout x 16 ci]^T (fp16, smem)
-//   * M = 128 consecutive time rows, N = Cout, K = (tap, input channel).
+// tc_conv_kernel: the tap conv (gan_kernels.h) as an implicit GEMM on the tensor cores (wgmma).
+//   D[64 rows x Cout] (fp32, registers) += A[64 rows x 16 ci] (fp16, smem) * B[Cout x 16 ci]^T (fp16, smem)
+//   * M = MT x 128 consecutive time rows per work item, N = Cout, K = (tap, input channel).
 //   * activations live in HBM as "F16B" planes [B][C/64][Lp][64] (already leaky-relu'd by the
 //     producer's epilogue) whose rows are stored PRE-SWIZZLED: the 16-byte chunks of every 128-byte
-//     row are XOR-permuted by (row & 7) exactly like the UMMA SWIZZLE_128B shared-memory layout
+//     row are XOR-permuted by (row & 7) exactly like the GMMA SWIZZLE_128B shared-memory layout
 //     (64-byte rows / SWIZZLE_64B when C = 32).  One bulk-TMA copy (cp.async.bulk) per 64-channel
 //     chunk fetches the rows [floor8(m0 + omin), ... + W) of a work item; because the copy starts at
 //     a row that is a multiple of 8 and lands 1024-byte aligned, it arrives in shared memory already
@@ -13,16 +13,12 @@
 //     The operand of tap t is the SAME buffer with the descriptor start address advanced by off_t
 //     rows (the swizzle is a function of absolute smem address bits, so no base-offset fix-up is needed): every tap, every dilation and every phase of a
 //     transposed conv reuse one window; zero padding comes from the zero pad rows of the plane.
-//     (A first version used the SWIZZLE_NONE 8x16 B core-matrix layout: correct, but the tensor core
-//     fetches such operands at 32 B/clk - 128 cycles per 128x16 A tile, profiles/r01_*swizzle_none*.)
 //   * weights: per (kernel index, 64-channel chunk) an fp16 image [Cout][64] with the same swizzle,
 //     streamed through a ring of shared-memory stages by bulk copies, or kept resident when the
 //     layer's whole weight set fits (all C<=64 layers).
-//   * warp roles: warp 0 = copy producer, warp 1 = MMA issuer (warp-uniform loop, one elected lane issues) + TMEM allocator,
-//     warps 2-9 = epilogue (TMEM -> registers -> bias/residual/MRF/leaky-relu -> fp32 F32B plane
-//     and/or fp16 F16B plane, fully coalesced 16 B per thread per 8 channels).
-//   * accumulators double-buffered in TMEM (2 x MT x Cout columns <= 512) so the epilogue of work
-//     item i overlaps the MMAs of item i+1; persistent CTAs, one per SM, static round-robin.
+//   * warp roles: warpgroup 0 = copy producer (one thread), warpgroups 1-2 = MMA and epilogue, each on half of the rows
+//     (registers -> shared-memory staging -> bias/residual/MRF/leaky-relu -> fp32 F32B plane and/or fp16 F16B plane,
+//     16 B per thread per 8 channels).  Persistent CTAs, one per SM, static round-robin.
 // reference semantics: hifigan/models.py:35-42 (ResBlock1), :134-150 (Generator.forward)
 #include "gan_tc.h"
 
@@ -40,10 +36,11 @@ namespace mb {
 
 namespace {
 
-__host__ __device__ constexpr int tc_threads(int ew) { return 64 + 32 * ew; }
+constexpr int kMmaGroups = 2;                      // MMA + epilogue warpgroups
+constexpr int kTcThreads = 128 * (1 + kMmaGroups);  // + the copy-producer warpgroup
 constexpr int kAStages = 2;
-constexpr int kAccStages = 2;
 constexpr int kMaxWStages = 16;
+constexpr uint32_t kStageBytes = kMmaGroups * 64 * tcdev::kStageLd * 4;  // epilogue staging: 64 rows x 32 columns per warpgroup
 constexpr uint32_t kSmemMax = 227 * 1024;
 constexpr size_t kPlaneSlack = 128 * 1024;
 
@@ -55,11 +52,10 @@ struct TcParams {
   int slab[kMaxPhases][kMaxTaps];
   int omin, W, MT;
   int cw, row_bytes, nk16, n_cchunks;   // channels per K-chunk (64 or 32), bytes per operand row
-  int layout_type;                     // UMMA layout: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B
   int baseoff_mode;                    // 1: descriptor base_offset = start address bits 7..9
   int slab_bytes, wstages, resident;
   int tiles_per_utt, n_work;
-  uint32_t a_stage_bytes, a_off, w_off, bias_off, bar_off;
+  uint32_t a_stage_bytes, a_off, w_off, bias_off, bar_off, stage_off;
   const __half* x16;
   int x_Lp;
   const __half* w16;
@@ -83,6 +79,16 @@ struct TcParams {
   float div;
   const int32_t* lengths;
   int len_mul_out;
+  int rows_item;                       // output rows per work item (MT x 128, or MT x 128 - 2 h2 for a fused pair)
+  // fused resblock pair (PAIR kernels): this launch's taps / weights are c1's, shifted by -h2 rows; c2 (k2 taps, dilation 1)
+  // reads c1's leaky-relu'd fp16 output from shared memory and owns bias / residual / outputs above
+  int k2, h2;
+  int off2[kMaxTaps];
+  const __half* w2;                    // c2's resident weight images [k2][Cout][cw]
+  const float* bias1;
+  float slope_mid;                     // leaky-relu between c1 and c2 (c2's in_slope)
+  int len_mul_mid;
+  uint32_t w2_off, mid_off, slab2_bytes;
 };
 
 using namespace tcdev;
@@ -94,19 +100,19 @@ __device__ __forceinline__ WorkItem decode_work(const TcParams& p, int work) {
   WorkItem w;
   w.r = work % p.stride;
   const int t = work / p.stride;
-  w.m0 = (t % p.tiles_per_utt) * (p.MT * 128);
+  w.m0 = (t % p.tiles_per_utt) * p.rows_item;
   w.b = t / p.tiles_per_utt;
   return w;
 }
 
-// N = Cout, MT = row tiles per work item, CW = channels per operand row (64: SWIZZLE_128B, 32: SWIZZLE_64B).
-// They are compile-time so that every MMA's descriptor is "base + immediate" (the single issuing
-// thread is otherwise the bottleneck: ~190 cycles per MMA with run-time address arithmetic).
-// EW epilogue warps (8, or 16 working on UC = 16-column units so that 576 threads fit the register file): see gan_tc_pair.cu.
-template <int N, int MT, int CW, int EW = 8, int UC = 32>
-__global__ void __launch_bounds__(tc_threads(EW), 1) tc_conv_kernel(const __grid_constant__ TcParams p) {
-  constexpr int kEpiWarps = EW;
-  constexpr int kTcThreads = tc_threads(EW);
+// N = Cout, MT = 128-row tiles per work item, CW = channels per operand row (64: SWIZZLE_128B, 32: SWIZZLE_64B).
+// They are compile-time so that the accumulators are register arrays and every descriptor is "base + immediate".
+// PAIR: fused resblock pair (see TcParams); c1's accumulators go through the bias / mask / leaky-relu epilogue into a swizzled fp16
+// operand in shared memory ("mid": row j = sequence row m0 - h2 + j) that c2's wgmmas read with a row shift per tap, so the
+// intermediate activation never reaches HBM.
+template <int N, int MT, int CW, bool PAIR = false>
+__global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(const __grid_constant__ TcParams p) {
+  constexpr int UC = 16;  // columns per epilogue thread and unit
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // swizzle atoms need 1024 B alignment
   uint8_t* a_base = smem + p.a_off;
@@ -117,9 +123,8 @@ __global__ void __launch_bounds__(tc_threads(EW), 1) tc_conv_kernel(const __grid
   uint64_t* a_empty = a_full + kAStages;
   uint64_t* w_full = a_empty + kAStages;
   uint64_t* w_empty = w_full + kMaxWStages;
-  uint64_t* acc_full = w_empty + kMaxWStages;
-  uint64_t* acc_empty = acc_full + kAccStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + kAccStages);
+  uint64_t* w2_full = w_empty + kMaxWStages;
+  float* stage_s = reinterpret_cast<float*>(smem + p.stage_off);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -127,41 +132,34 @@ __global__ void __launch_bounds__(tc_threads(EW), 1) tc_conv_kernel(const __grid
   if (threadIdx.x == 0) {
     for (int i = 0; i < kAStages; ++i) {
       mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 1);
+      mbar_init(&a_empty[i], kMmaGroups);
     }
     for (int i = 0; i < kMaxWStages; ++i) {
       mbar_init(&w_full[i], 1);
-      mbar_init(&w_empty[i], 1);
+      mbar_init(&w_empty[i], kMmaGroups);
     }
-    for (int i = 0; i < kAccStages; ++i) {
-      mbar_init(&acc_full[i], 1);
-      mbar_init(&acc_empty[i], 32 * kEpiWarps);
-    }
+    mbar_init(w2_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   for (int i = threadIdx.x; i < p.Cout; i += kTcThreads) bias_s[i] = p.bias ? p.bias[i] : 0.f;  // weights: never written by a kernel
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // Programmatic dependent launch: everything above (barrier init, TMEM allocation, bias) overlapped the
-  // tail of the previous layer's kernel; activations written by it may only be touched after this wait.
-  // Dependents of THIS kernel may begin their own prologue as soon as SMs free up.
+  // Programmatic dependent launch: everything above (barrier init, bias) overlapped the tail of the previous layer's kernel;
+  // activations written by it may only be touched after this wait.  Dependents of THIS kernel may begin their own prologue
+  // as soon as SMs free up.
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-
-  if (warp == 0) {
-    // ===================== copy producer =====================
-    if (lane == 0) {
+  if (warp < 4) {
+    // ===================== copy producer (warpgroup 0, one thread) =====================
+    regs_dec<40>();
+    if (warp == 0 && lane == 0) {
       int a_stage = 0, a_phase = 0, w_stage = 0, w_phase = 0;
       uint32_t resident_loaded = 0;
+      if constexpr (PAIR) {
+        mbar_expect_tx(w2_full, (uint32_t)p.k2 * p.slab2_bytes);
+        for (int t = 0; t < p.k2; ++t)
+          bulk_g2s(smem_u32(smem + p.w2_off + (size_t)t * p.slab2_bytes), p.w2 + (size_t)t * (p.slab2_bytes >> 1), p.slab2_bytes, w2_full);
+      }
       for (int work = blockIdx.x; work < p.n_work; work += gridDim.x) {
         const WorkItem wi = decode_work(p, work);
         for (int c = 0; c < p.n_cchunks; ++c) {
@@ -192,241 +190,268 @@ __global__ void __launch_bounds__(tc_threads(EW), 1) tc_conv_kernel(const __grid
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // The whole warp runs this loop in lock-step; one elected lane issues the tcgen05 instructions.
-    // Descriptors differ only in their low word (start address >> 4) and all per-MMA offsets are
-    // immediates.
-    {
-      constexpr uint32_t ROWB = CW * 2;
-      constexpr int NK16 = CW / 16;
-      constexpr uint32_t MT_STEP = (128u * ROWB) >> 4;
-      constexpr uint32_t idesc = (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      int a_stage = 0, a_phase = 0, w_stage = 0, w_phase = 0, acc_stage = 0, acc_phase = 0;
-      const uint64_t desc_hi = make_desc(0, 8u * ROWB, CW == 64 ? 2u : 4u, 0);  // everything but the address
-      const bool leader = elect_one();
-      uint32_t resident_seen = 0;  // resident weight images whose arrival has already been observed
-      for (int work = blockIdx.x; work < p.n_work; work += gridDim.x) {
-        const WorkItem wi = decode_work(p, work);
-        mbar_wait(&acc_empty[acc_stage], acc_phase ^ 1);
-        tc_fence_after();
-        const int delta = (kPadRows + wi.m0 + p.omin) & 7;  // rows the window start was rounded down by
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc_stage * MT * N);
-        const int nt = p.ntaps[wi.r];
-        bool first = true;
-        for (int c = 0; c < p.n_cchunks; ++c) {
-          mbar_wait(&a_full[a_stage], a_phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(a_base + (size_t)a_stage * p.a_stage_bytes);
-          for (int t = 0; t < nt; ++t) {
-            uint32_t w_addr;
-            if (p.resident) {
-              const int sid = p.slab[wi.r][t] * p.n_cchunks + c;
-              if (!(resident_seen & (1u << sid))) {
-                mbar_wait(&w_full[sid], 0);
-                tc_fence_after();
-                resident_seen |= 1u << sid;
-              }
-              w_addr = smem_u32(w_base + (size_t)sid * p.slab_bytes);
-            } else {
-              mbar_wait(&w_full[w_stage], w_phase);
-              tc_fence_after();
-              w_addr = smem_u32(w_base + (size_t)w_stage * p.slab_bytes);
-            }
-            const uint64_t a0 = desc_hi + (uint64_t)((a_addr + (uint32_t)(delta + p.off[wi.r][t] - p.omin) * ROWB) >> 4);
-            const uint64_t b0 = desc_hi + (uint64_t)(w_addr >> 4);
-            if (leader) {
-              if (first) {
-#pragma unroll
-                for (int s = 0; s < NK16; ++s)
-#pragma unroll
-                  for (int mt = 0; mt < MT; ++mt)
-                    tc_mma_f16(d_tmem + (uint32_t)(mt * N), a0 + (uint64_t)(2 * s + mt * MT_STEP), b0 + (uint64_t)(2 * s),
-                               idesc, s > 0 ? 1u : 0u);
-              } else {
-#pragma unroll
-                for (int s = 0; s < NK16; ++s)
-#pragma unroll
-                  for (int mt = 0; mt < MT; ++mt)
-                    tc_mma_f16(d_tmem + (uint32_t)(mt * N), a0 + (uint64_t)(2 * s + mt * MT_STEP), b0 + (uint64_t)(2 * s),
-                               idesc, 1u);
-              }
-              if (!p.resident) tc_commit(&w_empty[w_stage]);
-            }
-            first = false;
-            if (!p.resident) {
-              if (++w_stage == p.wstages) { w_stage = 0; w_phase ^= 1; }
-            }
-          }
-          if (leader) tc_commit(&a_empty[a_stage]);
-          if (++a_stage == kAStages) { a_stage = 0; a_phase ^= 1; }
-        }
-        if (leader) tc_commit(&acc_full[acc_stage]);
-        if (++acc_stage == kAccStages) { acc_stage = 0; acc_phase ^= 1; }
-      }
-    }
   } else {
-    // ===================== epilogue (warps 2..9) =====================
-    // Two groups of four warps; a group covers all four TMEM lane quarters and takes every other
-    // (row tile, 32-column) unit.  Per unit the residual / running-sum loads are issued FIRST (they do
-    // not depend on the accumulator, so for the first unit they overlap the MMAs of this work item),
-    // then the accumulator is read from TMEM, then everything is stored: 16 independent 16-byte
-    // loads in flight per thread instead of one.
-    const int quarter = warp & 3;  // TMEM lanes [32*quarter, 32*quarter+32)
-    const int grp = (warp - 2) >> 2;
-    const int row_in_tile = quarter * 32 + lane;
-    int acc_stage = 0, acc_phase = 0;
+    // ===================== MMA + epilogue (warpgroups 1 and 2) =====================
+    // Warpgroup g owns rows [g * MT * 64, (g + 1) * MT * 64) of the work item: MT accumulators of 64 rows x N columns.
+    // A (tap, K-chunk) step is one commit group of NK16 * MT wgmmas; a group's operand stages are released once the NEXT
+    // group is issued and this one has completed (wait_group 1), so two groups are in flight.
+    regs_inc<232>();
+    constexpr uint32_t ROWB = CW * 2;
+    constexpr int NK16 = CW / 16;
+    constexpr uint32_t MT_STEP = (64u * ROWB) >> 4;
+    const int g = warp / 4 - 1;
+    const int tid = threadIdx.x & 127;
+    const bool leader = tid == 0;
+    const uint64_t desc_hi = make_desc(0, 8u * ROWB, CW == 64 ? 1u : 2u, 0);  // everything but the address
+    float* stage = stage_s + g * 64 * kStageLd;
+    int a_stage = 0, a_phase = 0, w_stage = 0, w_phase = 0;
+    uint32_t resident_seen = 0;  // resident weight images whose arrival has already been observed
+    bool w2_seen = false;        // PAIR: c2's weights have arrived
+    float acc[MT][N / 2];
     const int C4 = p.Cout >> 2;
     const int ocw = f16_cw(p.Cout);  // output plane: channels per row chunk
-    const int units_per_tile = p.Cout / UC;
-    const int n_units = p.MT * units_per_tile;
-    constexpr int G = EW / 4;
     for (int work = blockIdx.x; work < p.n_work; work += gridDim.x) {
       const WorkItem wi = decode_work(p, work);
-      const int valid_out = p.lengths ? min(p.Lout, p.lengths[wi.b] * p.len_mul_out) : p.Lout;
-      bool waited = false;
-      for (int u = grp; u < n_units; u += G) {
-        const int mt = u / units_per_tile;
-        const int col0 = (u - mt * units_per_tile) * UC;
-        const int q = wi.m0 + mt * 128 + row_in_tile;
-        const int lo = q * p.stride + wi.r;
-        const bool inb = q < p.Lin;
-        const bool live = inb && lo < valid_out;
-        const size_t i32 = ((size_t)wi.b * C4 + (col0 >> 2)) * p.Lout + lo;  // + g * Lout per 4 channels
-        float4 rv[UC / 4], ov[UC / 4];
-        uint4 rh[UC / 8];
-        if (inb && p.res32) {
-#pragma unroll
-          for (int g = 0; g < UC / 4; ++g) rv[g] = reinterpret_cast<const float4*>(p.res32)[i32 + (size_t)g * p.Lout];
-        }
-        if (inb && p.res16) {  // (the lo halves of a hi/lo residual share rv's registers: res32 and res16 are exclusive)
-          const int rr = kPadRows + lo;
-          if (!p.res_hilo) {
-            const size_t rbase = (((size_t)wi.b * (p.Cout / ocw) + col0 / ocw) * p.res_Lp + rr) * (size_t)(ocw >> 3);
-            const int c0 = (col0 & (ocw - 1)) >> 3, sw = f16_swz(ocw, rr);
-#pragma unroll
-            for (int g = 0; g < UC / 8; ++g) rh[g] = reinterpret_cast<const uint4*>(p.res16)[rbase + (size_t)((c0 + g) ^ sw)];
+      const int delta = (kPadRows + wi.m0 + p.omin) & 7;  // rows the window start was rounded down by
+      const int nt = p.ntaps[wi.r];
+      int pend_a = -1, pend_w = -1;  // stages of the group in flight that is not yet released
+      bool first = true;
+      wgmma_fence();
+      for (int c = 0; c < p.n_cchunks; ++c) {
+        mbar_wait(&a_full[a_stage], a_phase);
+        const uint32_t a_addr = smem_u32(a_base + (size_t)a_stage * p.a_stage_bytes);
+        for (int t = 0; t < nt; ++t) {
+          uint32_t w_addr;
+          if (p.resident) {
+            const int sid = p.slab[wi.r][t] * p.n_cchunks + c;
+            if (!(resident_seen & (1u << sid))) {
+              mbar_wait(&w_full[sid], 0);
+              resident_seen |= 1u << sid;
+            }
+            w_addr = smem_u32(w_base + (size_t)sid * p.slab_bytes);
           } else {
-            // hi/lo plane: rows of 64 channels; hi block = channels [0, Cout), lo block = [Cout, 2 Cout)
-            const int nch = (2 * p.Cout) >> 6, sw = f16_swz(64, rr);
+            mbar_wait(&w_full[w_stage], w_phase);
+            w_addr = smem_u32(w_base + (size_t)w_stage * p.slab_bytes);
+          }
+          uint32_t a_row = a_addr + (uint32_t)(delta + p.off[wi.r][t] - p.omin) * ROWB;
+          const uint64_t a0 = desc_hi + (uint64_t)((a_row + (uint32_t)(g * MT) * 64u * ROWB) >> 4) +
+                              (p.baseoff_mode ? ((uint64_t)((a_row >> 7) & 7) << 49) : 0);
+          const uint64_t b0 = desc_hi + (uint64_t)(w_addr >> 4);
 #pragma unroll
-            for (int g = 0; g < UC / 8; ++g) {
-              const int ch = col0 + 8 * g, cl = ch + p.Cout;
-              rh[g] = reinterpret_cast<const uint4*>(p.res16)[(((size_t)wi.b * nch + (ch >> 6)) * p.res_Lp + rr) * 8 + (size_t)(((ch & 63) >> 3) ^ sw)];
-              rv[g] = reinterpret_cast<const float4*>(p.res16)[(((size_t)wi.b * nch + (cl >> 6)) * p.res_Lp + rr) * 8 + (size_t)(((cl & 63) >> 3) ^ sw)];
-            }
+          for (int mt = 0; mt < MT; ++mt) fence_acc(acc[mt]);
+          wgmma_fence();
+#pragma unroll
+          for (int s = 0; s < NK16; ++s)
+#pragma unroll
+            for (int mt = 0; mt < MT; ++mt)
+              wgmma_f16<N>(acc[mt], a0 + (uint64_t)(2 * s + mt * MT_STEP), b0 + (uint64_t)(2 * s), (first && s == 0) ? 0u : 1u);
+          wgmma_commit();
+          first = false;
+          wgmma_wait<1>();
+#pragma unroll
+          for (int mt = 0; mt < MT; ++mt) fence_acc(acc[mt]);
+          if (leader) {
+            if (pend_w >= 0) mbar_arrive(&w_empty[pend_w]);
+            if (pend_a >= 0) mbar_arrive(&a_empty[pend_a]);
+          }
+          pend_w = p.resident ? -1 : w_stage;
+          pend_a = (t == nt - 1) ? a_stage : -1;
+          if (!p.resident) {
+            if (++w_stage == p.wstages) { w_stage = 0; w_phase ^= 1; }
           }
         }
-        if (inb && p.mode != EPI_STORE && !p.red_add) {
+        if (++a_stage == kAStages) { a_stage = 0; a_phase ^= 1; }
+      }
+      wgmma_wait<0>();
 #pragma unroll
-          for (int g = 0; g < UC / 4; ++g) ov[g] = reinterpret_cast<const float4*>(p.y32)[i32 + (size_t)g * p.Lout];
-        }
-        if (!waited) {
-          mbar_wait(&acc_full[acc_stage], acc_phase);
-          tc_fence_after();
-          waited = true;
-        }
-        uint32_t raw[UC];
-        tmem_ld<UC>(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)((acc_stage * p.MT + mt) * p.Cout + col0), raw);
-        if (!inb) continue;
-        float v[UC];
+      for (int mt = 0; mt < MT; ++mt) fence_acc(acc[mt]);
+      if (leader) {
+        if (pend_w >= 0) mbar_arrive(&w_empty[pend_w]);
+        if (pend_a >= 0) mbar_arrive(&a_empty[pend_a]);
+      }
+      if constexpr (PAIR) {
+        // ---- c1 epilogue -> mid (fp16, swizzled like the operand planes); rows outside [0, valid) are c2's zero padding
+        uint8_t* mid = smem + p.mid_off;
+        const int valid_mid = p.lengths ? min(p.Lin, p.lengths[wi.b] * p.len_mul_mid) : p.Lin;
+        group_sync(3, 128 * kMmaGroups);  // both warpgroups are done reading the previous item's mid
+        const int w = tid >> 5, l = tid & 31;
 #pragma unroll
-        for (int i = 0; i < UC; ++i) v[i] = __uint_as_float(raw[i]) * p.acc_scale + bias_s[col0 + i];
-        if (p.res32) {
+        for (int mt = 0; mt < MT; ++mt) {
 #pragma unroll
-          for (int g = 0; g < UC / 4; ++g) {
-            v[4 * g + 0] += rv[g].x; v[4 * g + 1] += rv[g].y; v[4 * g + 2] += rv[g].z; v[4 * g + 3] += rv[g].w;
-          }
-        }
-        if (p.res16) {
+          for (int h = 0; h < 2; ++h) {
+            const int r = (g * MT + mt) * 64 + 16 * w + (l >> 2) + 8 * h;
+            const int sq = wi.m0 - p.h2 + r;
+            const bool live = sq >= 0 && sq < valid_mid;
+            const int sw = f16_swz(CW, r);
 #pragma unroll
-          for (int g = 0; g < UC / 8; ++g) {
-            if (p.res_hilo) add_res16_hilo(&v[8 * g], rh[g], *reinterpret_cast<const uint4*>(&rv[g]), p.res_inv);
-            else add_res16(&v[8 * g], rh[g], p.res_inv);
-          }
-        }
-        if (p.mode != EPI_STORE && !p.red_add) {
-#pragma unroll
-          for (int g = 0; g < UC / 4; ++g) {
-            v[4 * g + 0] += ov[g].x; v[4 * g + 1] += ov[g].y; v[4 * g + 2] += ov[g].z; v[4 * g + 3] += ov[g].w;
-          }
-          if (p.mode == EPI_ADD_DIV) {
-#pragma unroll
-            for (int i = 0; i < UC; ++i) v[i] /= p.div;
-          }
-        }
-        if (!live) {
-#pragma unroll
-          for (int i = 0; i < UC; ++i) v[i] = 0.f;
-        }
-        if (p.red_add) {  // MRF sum of a middle resblock: S += v by vector reductions in L2 (rows past the length add nothing)
-          if (live) {
-#pragma unroll
-            for (int g = 0; g < UC / 4; ++g)
-              red_add_f32x4(p.y32 + (i32 + (size_t)g * p.Lout) * 4, v[4 * g + 0], v[4 * g + 1], v[4 * g + 2], v[4 * g + 3]);
-          }
-        } else if (p.y32) {
-#pragma unroll
-          for (int g = 0; g < UC / 4; ++g)
-            reinterpret_cast<float4*>(p.y32)[i32 + (size_t)g * p.Lout] =
-                make_float4(v[4 * g + 0], v[4 * g + 1], v[4 * g + 2], v[4 * g + 3]);
-        }
-        if (p.y16) {
-          const int rr = kPadRows + lo;
-          const int ysw = f16_swz(p.y_cw, rr);
-          const int ycw8 = p.y_cw >> 3;
-#pragma unroll
-          for (int g = 0; g < UC / 8; ++g) {
-            float a[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) a[e] = lrelu(v[8 * g + e], p.out_slope);
-            __half2 h[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) h[e] = __floats2half2_rn(a[2 * e], a[2 * e + 1]);
-            uint4 pk;
-            pk.x = *reinterpret_cast<uint32_t*>(&h[0]);
-            pk.y = *reinterpret_cast<uint32_t*>(&h[1]);
-            pk.z = *reinterpret_cast<uint32_t*>(&h[2]);
-            pk.w = *reinterpret_cast<uint32_t*>(&h[3]);
-            const int ct = p.y_c0 + col0 + 8 * g;  // channel of the (hi) block
-            const int chunk = ct / p.y_cw, cc = ct - chunk * p.y_cw;
-            const size_t i16 = (((size_t)wi.b * p.y_nchunks + chunk) * p.y_Lp + rr) * (size_t)ycw8 + (size_t)((cc >> 3) ^ ysw);
-            reinterpret_cast<uint4*>(p.y16)[i16] = pk;
-            if (p.y_lo_c >= 0) {
-              __half2 l2[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float2 hf = __half22float2(h[e]);
-                l2[e] = __floats2half2_rn(a[2 * e] - hf.x, a[2 * e + 1] - hf.y);
+            for (int jj = 0; jj < N / 8; ++jj) {
+              const int col = 8 * jj + 2 * (l & 3);
+              float a0 = 0.f, a1 = 0.f;
+              if (live) {
+                a0 = lrelu(acc[mt][4 * jj + 2 * h + 0] + p.bias1[col], p.slope_mid);
+                a1 = lrelu(acc[mt][4 * jj + 2 * h + 1] + p.bias1[col + 1], p.slope_mid);
               }
-              uint4 pl;
-              pl.x = *reinterpret_cast<uint32_t*>(&l2[0]);
-              pl.y = *reinterpret_cast<uint32_t*>(&l2[1]);
-              pl.z = *reinterpret_cast<uint32_t*>(&l2[2]);
-              pl.w = *reinterpret_cast<uint32_t*>(&l2[3]);
-              const int ctl = ct + p.y_lo_c;
-              const int chl = ctl / p.y_cw, ccl = ctl - chl * p.y_cw;
-              const size_t j16 = (((size_t)wi.b * p.y_nchunks + chl) * p.y_Lp + rr) * (size_t)ycw8 + (size_t)((ccl >> 3) ^ ysw);
-              reinterpret_cast<uint4*>(p.y16)[j16] = pl;
+              *reinterpret_cast<__half2*>(mid + (size_t)r * ROWB + ((jj ^ sw) << 4) + (col & 7) * 2) = __floats2half2_rn(a0, a1);
+            }
+          }
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> wgmma operand reads
+        group_sync(3, 128 * kMmaGroups);
+        if (!w2_seen) {
+          mbar_wait(w2_full, 0);
+          w2_seen = true;
+        }
+        // ---- c2: output row i reads mid rows i + h2 + off2[t]
+        const uint32_t mid_addr = smem_u32(mid) + (uint32_t)(g * MT) * 64u * ROWB;
+        for (int t = 0; t < p.k2; ++t) {
+          const uint64_t a0 = desc_hi + (uint64_t)((mid_addr + (uint32_t)(p.h2 + p.off2[t]) * ROWB) >> 4);
+          const uint64_t b0 = desc_hi + (uint64_t)(smem_u32(smem + p.w2_off + (size_t)t * p.slab2_bytes) >> 4);
+#pragma unroll
+          for (int mt = 0; mt < MT; ++mt) fence_acc(acc[mt]);
+          wgmma_fence();
+#pragma unroll
+          for (int s = 0; s < NK16; ++s)
+#pragma unroll
+            for (int mt = 0; mt < MT; ++mt)
+              wgmma_f16<N>(acc[mt], a0 + (uint64_t)(2 * s + mt * MT_STEP), b0 + (uint64_t)(2 * s), (t == 0 && s == 0) ? 0u : 1u);
+          wgmma_commit();
+        }
+        wgmma_wait<0>();
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt) fence_acc(acc[mt]);
+      }
+      // ---- epilogue: per (row tile, 32-column unit) the slice goes through shared memory so that a thread owns one row and
+      // 16 consecutive columns (the fp16 plane stores 8 channels and the F32B plane 4 channels per 16-byte access)
+      const int valid_out = p.lengths ? min(p.Lout, p.lengths[wi.b] * p.len_mul_out) : p.Lout;
+      const int row_in_tile = tid & 63;
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+        for (int u = 0; u < N / 32; ++u) {
+          const int col0 = u * 32 + (tid >> 6) * UC;
+          const int q = wi.m0 + (g * MT + mt) * 64 + row_in_tile;
+          const int lo = q * p.stride + wi.r;
+          const bool inb = q < p.Lin && (g * MT + mt) * 64 + row_in_tile < p.rows_item;
+          const bool live = inb && lo < valid_out;
+          const size_t i32 = ((size_t)wi.b * C4 + (col0 >> 2)) * p.Lout + lo;  // + g * Lout per 4 channels
+          float4 rv[UC / 4], ov[UC / 4];
+          uint4 rh[UC / 8];
+          if (inb && p.res32) {
+#pragma unroll
+            for (int j = 0; j < UC / 4; ++j) rv[j] = reinterpret_cast<const float4*>(p.res32)[i32 + (size_t)j * p.Lout];
+          }
+          if (inb && p.res16) {  // (the lo halves of a hi/lo residual share rv's registers: res32 and res16 are exclusive)
+            const int rr = kPadRows + lo;
+            if (!p.res_hilo) {
+              const size_t rbase = (((size_t)wi.b * (p.Cout / ocw) + col0 / ocw) * p.res_Lp + rr) * (size_t)(ocw >> 3);
+              const int c0 = (col0 & (ocw - 1)) >> 3, sw = f16_swz(ocw, rr);
+#pragma unroll
+              for (int j = 0; j < UC / 8; ++j) rh[j] = reinterpret_cast<const uint4*>(p.res16)[rbase + (size_t)((c0 + j) ^ sw)];
+            } else {
+              // hi/lo plane: rows of 64 channels; hi block = channels [0, Cout), lo block = [Cout, 2 Cout)
+              const int nch = (2 * p.Cout) >> 6, sw = f16_swz(64, rr);
+#pragma unroll
+              for (int j = 0; j < UC / 8; ++j) {
+                const int ch = col0 + 8 * j, cl = ch + p.Cout;
+                rh[j] = reinterpret_cast<const uint4*>(p.res16)[(((size_t)wi.b * nch + (ch >> 6)) * p.res_Lp + rr) * 8 + (size_t)(((ch & 63) >> 3) ^ sw)];
+                rv[j] = reinterpret_cast<const float4*>(p.res16)[(((size_t)wi.b * nch + (cl >> 6)) * p.res_Lp + rr) * 8 + (size_t)(((cl & 63) >> 3) ^ sw)];
+              }
+            }
+          }
+          if (inb && p.mode != EPI_STORE && !p.red_add) {
+#pragma unroll
+            for (int j = 0; j < UC / 4; ++j) ov[j] = reinterpret_cast<const float4*>(p.y32)[i32 + (size_t)j * p.Lout];
+          }
+          group_sync(1 + g, 128);  // the previous unit's rows have been read
+          stage_acc32(stage, &acc[mt][u * 16], tid);
+          group_sync(1 + g, 128);
+          if (!inb) continue;
+          float v[UC];
+          const float* srow = stage + row_in_tile * kStageLd + (tid >> 6) * UC;
+#pragma unroll
+          for (int i = 0; i < UC; ++i) v[i] = srow[i] * p.acc_scale + bias_s[col0 + i];
+          if (p.res32) {
+#pragma unroll
+            for (int j = 0; j < UC / 4; ++j) {
+              v[4 * j + 0] += rv[j].x; v[4 * j + 1] += rv[j].y; v[4 * j + 2] += rv[j].z; v[4 * j + 3] += rv[j].w;
+            }
+          }
+          if (p.res16) {
+#pragma unroll
+            for (int j = 0; j < UC / 8; ++j) {
+              if (p.res_hilo) add_res16_hilo(&v[8 * j], rh[j], *reinterpret_cast<const uint4*>(&rv[j]), p.res_inv);
+              else add_res16(&v[8 * j], rh[j], p.res_inv);
+            }
+          }
+          if (p.mode != EPI_STORE && !p.red_add) {
+#pragma unroll
+            for (int j = 0; j < UC / 4; ++j) {
+              v[4 * j + 0] += ov[j].x; v[4 * j + 1] += ov[j].y; v[4 * j + 2] += ov[j].z; v[4 * j + 3] += ov[j].w;
+            }
+            if (p.mode == EPI_ADD_DIV) {
+#pragma unroll
+              for (int i = 0; i < UC; ++i) v[i] /= p.div;
+            }
+          }
+          if (!live) {
+#pragma unroll
+            for (int i = 0; i < UC; ++i) v[i] = 0.f;
+          }
+          if (p.red_add) {  // MRF sum of a middle resblock: S += v by vector reductions in L2 (rows past the length add nothing)
+            if (live) {
+#pragma unroll
+              for (int j = 0; j < UC / 4; ++j)
+                red_add_f32x4(p.y32 + (i32 + (size_t)j * p.Lout) * 4, v[4 * j + 0], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+            }
+          } else if (p.y32) {
+#pragma unroll
+            for (int j = 0; j < UC / 4; ++j)
+              reinterpret_cast<float4*>(p.y32)[i32 + (size_t)j * p.Lout] =
+                  make_float4(v[4 * j + 0], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+          }
+          if (p.y16) {
+            const int rr = kPadRows + lo;
+            const int ysw = f16_swz(p.y_cw, rr);
+            const int ycw8 = p.y_cw >> 3;
+#pragma unroll
+            for (int j = 0; j < UC / 8; ++j) {
+              float a[8];
+#pragma unroll
+              for (int e = 0; e < 8; ++e) a[e] = lrelu(v[8 * j + e], p.out_slope);
+              __half2 h[4];
+#pragma unroll
+              for (int e = 0; e < 4; ++e) h[e] = __floats2half2_rn(a[2 * e], a[2 * e + 1]);
+              uint4 pk;
+              pk.x = *reinterpret_cast<uint32_t*>(&h[0]);
+              pk.y = *reinterpret_cast<uint32_t*>(&h[1]);
+              pk.z = *reinterpret_cast<uint32_t*>(&h[2]);
+              pk.w = *reinterpret_cast<uint32_t*>(&h[3]);
+              const int ct = p.y_c0 + col0 + 8 * j;  // channel of the (hi) block
+              const int chunk = ct / p.y_cw, cc = ct - chunk * p.y_cw;
+              const size_t i16 = (((size_t)wi.b * p.y_nchunks + chunk) * p.y_Lp + rr) * (size_t)ycw8 + (size_t)((cc >> 3) ^ ysw);
+              reinterpret_cast<uint4*>(p.y16)[i16] = pk;
+              if (p.y_lo_c >= 0) {
+                __half2 l2[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                  const float2 hf = __half22float2(h[e]);
+                  l2[e] = __floats2half2_rn(a[2 * e] - hf.x, a[2 * e + 1] - hf.y);
+                }
+                uint4 pl;
+                pl.x = *reinterpret_cast<uint32_t*>(&l2[0]);
+                pl.y = *reinterpret_cast<uint32_t*>(&l2[1]);
+                pl.z = *reinterpret_cast<uint32_t*>(&l2[2]);
+                pl.w = *reinterpret_cast<uint32_t*>(&l2[3]);
+                const int ctl = ct + p.y_lo_c;
+                const int chl = ctl / p.y_cw, ccl = ctl - chl * p.y_cw;
+                const size_t j16 = (((size_t)wi.b * p.y_nchunks + chl) * p.y_Lp + rr) * (size_t)ycw8 + (size_t)((ccl >> 3) ^ ysw);
+                reinterpret_cast<uint4*>(p.y16)[j16] = pl;
+              }
             }
           }
         }
       }
-      if (!waited) {
-        mbar_wait(&acc_full[acc_stage], acc_phase);
-        tc_fence_after();
-      }
-      tc_fence_before();
-      mbar_arrive(&acc_empty[acc_stage]);
-      if (++acc_stage == kAccStages) { acc_stage = 0; acc_phase ^= 1; }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
   }
 }
 
@@ -558,15 +583,16 @@ bool tc_capable(const TapConv& t) {
   return true;
 }
 
-// row tiles per work item: as many as TMEM (2 x MT x Cout <= 512 columns) and shared memory allow
+// row tiles per work item: MT x Cout <= 256 accumulator columns (128 registers per MMA thread), and as shared memory allows
 int pick_mt_max(int Cout) { return Cout >= 256 ? 1 : (Cout >= 128 ? 2 : (Cout >= 64 ? 4 : 8)); }
 
 struct SmemPlan {
-  uint32_t a_stage_bytes, a_off, w_off, bias_off, bar_off, total;
+  uint32_t a_stage_bytes, a_off, w_off, bias_off, bar_off, stage_off, ex_off, total;
   int wstages, resident, W, omin;
 };
 
-bool plan_smem(const TapConv& t, const TcLayer& tc, int total_slabs, SmemPlan* sp) {
+// `extra`: bytes of a 1024-aligned region after everything else (fused pair: c2's weights and the intermediate rows)
+bool plan_smem(const TapConv& t, const TcLayer& tc, int total_slabs, SmemPlan* sp, uint32_t extra = 0) {
   int omin = 0x7fffffff, omax = -0x7fffffff;
   for (int r = 0; r < t.stride; ++r)
     for (int i = 0; i < t.ntaps[r]; ++i) {
@@ -580,7 +606,7 @@ bool plan_smem(const TapConv& t, const TcLayer& tc, int total_slabs, SmemPlan* s
   sp->a_stage_bytes = (uint32_t)align_up((size_t)sp->W * row_bytes, 1024);
   sp->a_off = 0;
   sp->w_off = sp->a_off + kAStages * sp->a_stage_bytes;
-  const uint32_t tail = (uint32_t)align_up((size_t)t.Cout * 4, 128) + 1024;
+  const uint32_t tail = (uint32_t)align_up((size_t)t.Cout * 4, 128) + 1024 + kStageBytes + (extra ? 1024 + extra : 0);
   const uint32_t usable = kSmemMax - 1024;  // the kernel aligns its base to 1024 B
   if (sp->w_off + tail + 2 * tc.slab_bytes > usable) return false;
   int ws = (int)((usable - sp->w_off - tail) / tc.slab_bytes);
@@ -589,7 +615,9 @@ bool plan_smem(const TapConv& t, const TcLayer& tc, int total_slabs, SmemPlan* s
   sp->wstages = sp->resident ? total_slabs : ws;
   sp->bias_off = sp->w_off + (uint32_t)sp->wstages * (uint32_t)tc.slab_bytes;
   sp->bar_off = sp->bias_off + (uint32_t)align_up((size_t)t.Cout * 4, 128);
-  sp->total = sp->bar_off + 1024;
+  sp->stage_off = sp->bar_off + 1024;
+  sp->ex_off = (uint32_t)align_up((size_t)sp->stage_off + kStageBytes, 1024);
+  sp->total = extra ? sp->ex_off + extra : sp->stage_off + kStageBytes;
   return sp->total <= usable;
 }
 
@@ -600,7 +628,7 @@ int kernel_count(const TapConv& t) {
   return k;
 }
 
-// MB_TC_FUSE=0 disables the fused resblock-pair kernel (gan_tc_pair.cu) for A/B measurements
+// MB_TC_FUSE=0: resblock pairs as two tc_conv launches instead of one fused launch
 bool tc_fuse_enabled() {
   static int on = -1;
   if (on < 0) {
@@ -608,6 +636,39 @@ bool tc_fuse_enabled() {
     on = e ? atoi(e) : 1;
   }
   return on != 0;
+}
+
+// fused resblock pair: c1's taps shifted by -h2 rows (the launch computes c1 on rows m0 - h2 ...), the row tiles per item and
+// the shared-memory plan with c2's weights and the intermediate rows in the extra region
+struct PairPlan {
+  TapConv t1;
+  int mt, h2;
+  SmemPlan sp;
+  uint32_t w2_off, mid_off;
+};
+bool pair_plan(const TcOp& c1, const TcOp& c2, PairPlan* pl) {
+  const int C = c1.taps.Cout;
+  if (!(C == 32 || C == 64) || c1.tc.n_cchunks != 1 || c2.tc.n_cchunks != 1) return false;
+  const int k2 = c2.taps.ntaps[0];
+  pl->h2 = (k2 - 1) / 2;
+  pl->t1 = c1.taps;
+  for (int i = 0; i < pl->t1.ntaps[0]; ++i) pl->t1.off[0][i] -= pl->h2;
+  const int rowb = c1.tc.kc * 2;
+  const int mts[2] = {C == 64 ? 2 : 8, C == 64 ? 1 : 4};  // kernel instances
+  for (int mt : mts) {
+    TcLayer tc = c1.tc;
+    tc.mt = mt;
+    const uint32_t w2_bytes = (uint32_t)align_up((size_t)k2 * c2.tc.slab_bytes, 1024);
+    const uint32_t mid_bytes = (uint32_t)align_up((size_t)((mt * 128 + 2 * pl->h2 + 7) & ~7) * rowb, 1024);
+    if (mt * 128 <= 2 * pl->h2) continue;
+    if (plan_smem(pl->t1, tc, kernel_count(c1.taps), &pl->sp, w2_bytes + mid_bytes)) {
+      pl->mt = mt;
+      pl->w2_off = pl->sp.ex_off;
+      pl->mid_off = pl->sp.ex_off + w2_bytes;
+      return true;
+    }
+  }
+  return false;
 }
 
 // MB_TC_RES16=0 keeps an fp32 residual plane in every stage (default: only in the full-rate stage; the
@@ -632,16 +693,6 @@ bool tc_x3_res16_enabled() {
   return on != 0;
 }
 
-// MB_TC_PAIR32=0 disables the fp32-input pair kernel of the full-rate stage (falls back to the fp16-plane pair)
-bool tc_pair32_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("MB_TC_PAIR32");
-    on = e ? atoi(e) : 1;
-  }
-  return on != 0;
-}
-
 // MB_TC_SPLIT3=0 keeps conv_pre on the FP32 FFMA kernel
 bool tc_split3_enabled() {
   static int on = -1;
@@ -653,9 +704,9 @@ bool tc_split3_enabled() {
 }
 
 // how the A descriptor encodes a start address that is not 1024-byte aligned (row-shifted taps).
-// Measured on B200 (tests/test_gan_tc_layers.py under MB_TC_BASEOFF=0/1): the operand fetch applies the
-// swizzle XOR on absolute shared-memory address bits, so the matrix-base-offset field must stay 0
-// (mode 0, default); mode 1 (field = address bits 7..9) double-counts the phase and is wrong.
+// The operand fetch applies the swizzle XOR on absolute shared-memory address bits, so the matrix-base-offset field stays 0
+// (mode 0, default; tests/test_gan_tc_layers.py checks every layer shape against torch); mode 1 (field = address bits 7..9)
+// is kept for A/B checks of that assumption.
 int tc_baseoff_mode() {
   static int mode = -1;
   if (mode < 0) {
@@ -673,8 +724,10 @@ size_t f32_plane_bytes(size_t B, size_t T, size_t cr) { return align_up(4 * B * 
 
 int launch_tc(const TcOp& op, const char* tc_arena, const TRef& x16, const TRef& res32, const TRef& res16, float res_slope,
               const TRef& y32, const TRef& y16, float out_slope, const int32_t* lengths, int B, int Lin, cudaStream_t st,
-              int y_c0 = 0, const float* bias_override = nullptr) {
-  const TapConv& t = op.taps;
+              int y_c0 = 0, const float* bias_override = nullptr, const TcOp* c2 = nullptr) {
+  PairPlan pl;
+  if (c2 && !pair_plan(op, *c2, &pl)) return fail(MB_ERR_INVALID, "tc_pair(%s): no shared-memory plan", op.name);
+  const TapConv& t = c2 ? pl.t1 : op.taps;
   TcParams p;
   memset(&p, 0, sizeof(p));
   p.B = B;
@@ -688,26 +741,28 @@ int launch_tc(const TcOp& op, const char* tc_arena, const TRef& x16, const TRef&
   memcpy(p.slab, t.slab, sizeof(p.slab));
   SmemPlan sp;
   const int total_slabs = kernel_count(t) * op.tc.n_cchunks;
-  if (!plan_smem(t, op.tc, total_slabs, &sp)) return fail(MB_ERR_INVALID, "tc_conv(%s): shared memory plan failed", op.name);
+  if (c2) sp = pl.sp;
+  else if (!plan_smem(t, op.tc, total_slabs, &sp)) return fail(MB_ERR_INVALID, "tc_conv(%s): shared memory plan failed", op.name);
   p.omin = sp.omin;
   p.W = sp.W;
-  p.MT = op.tc.mt;
+  p.MT = c2 ? pl.mt : op.tc.mt;
   p.cw = op.tc.kc;
   p.row_bytes = op.tc.kc * 2;
-  p.layout_type = (op.tc.kc == 64) ? 2 : 4;
   p.baseoff_mode = tc_baseoff_mode();
   p.nk16 = op.tc.kc / 16;
   p.n_cchunks = op.tc.n_cchunks;
   p.slab_bytes = (int)op.tc.slab_bytes;
   p.wstages = sp.wstages;
   p.resident = sp.resident;
-  p.tiles_per_utt = (Lin + p.MT * 128 - 1) / (p.MT * 128);
+  p.rows_item = p.MT * 128 - (c2 ? 2 * pl.h2 : 0);
+  p.tiles_per_utt = (Lin + p.rows_item - 1) / p.rows_item;
   p.n_work = B * p.tiles_per_utt * p.stride;
   p.a_stage_bytes = sp.a_stage_bytes;
   p.a_off = sp.a_off;
   p.w_off = sp.w_off;
   p.bias_off = sp.bias_off;
   p.bar_off = sp.bar_off;
+  p.stage_off = sp.stage_off;
   p.x16 = reinterpret_cast<const __half*>(x16.p);
   p.x_Lp = f16_lp(x16.L);
   p.x_pchunks = op.tc.x3 ? op.tc.x_pchunks : op.tc.n_cchunks;
@@ -735,26 +790,35 @@ int launch_tc(const TcOp& op, const char* tc_arena, const TRef& x16, const TRef&
   p.div = t.div;
   p.lengths = lengths;
   p.len_mul_out = t.len_mul_out;
+  if (c2) {  // c2 owns bias, accumulate mode and outputs; c1's bias and slope go to the intermediate
+    const TapConv& u = c2->taps;
+    p.k2 = u.ntaps[0];
+    p.h2 = pl.h2;
+    for (int i = 0; i < p.k2; ++i) p.off2[i] = u.off[0][i];
+    p.w2 = reinterpret_cast<const __half*>(tc_arena + c2->tc.w16_off);
+    p.slab2_bytes = (uint32_t)c2->tc.slab_bytes;
+    p.w2_off = pl.w2_off;
+    p.mid_off = pl.mid_off;
+    p.bias1 = op.b32;
+    p.bias = c2->b32;
+    p.slope_mid = u.in_slope;
+    p.len_mul_mid = op.taps.len_mul_out;
+    p.mode = u.mode;
+    p.div = u.div;
+    p.len_mul_out = u.len_mul_out;
+    p.red_add = (p.mode == EPI_ADD && !y16.p && y32.p && tc_red_add_enabled()) ? 1 : 0;
+  }
   if (res16.p && !res16.hilo && res16.C != t.Cout) return fail(MB_ERR_INVALID, "tc_conv(%s): fp16 residual plane geometry", op.name);
   if (res16.p && res16.hilo && res16.C != (t.Cout >= 64 ? 2 * t.Cout : 64)) return fail(MB_ERR_INVALID, "tc_conv(%s): hi/lo residual plane geometry", op.name);
   if (y_c0 != 0 && (p.y32 || p.res32 || p.res16)) return fail(MB_ERR_INVALID, "tc_conv(%s): channel-offset launch supports the fp16 plane only", op.name);
   if (p.mode != EPI_STORE && !p.y32) return fail(MB_ERR_INVALID, "tc_conv(%s): accumulate mode without fp32 plane", op.name);
   void (*kern)(const TcParams) = nullptr;
-  static const int ew16 = [] {
-    const char* e = getenv("MB_TC_CONV_EW16");  // A/B switch: 1 = sixteen epilogue warps on 16-column units
-    return e ? atoi(e) : 0;
-  }();
-  int threads = tc_threads(8);
-  if (ew16) {
-    threads = tc_threads(16);
-    if (p.Cout == 256 && p.MT == 1 && p.cw == 64) kern = tc_conv_kernel<256, 1, 64, 16, 16>;
-    else if (p.Cout == 128 && p.MT == 2 && p.cw == 64) kern = tc_conv_kernel<128, 2, 64, 16, 16>;
-    else if (p.Cout == 128 && p.MT == 1 && p.cw == 64) kern = tc_conv_kernel<128, 1, 64, 16, 16>;
-    else if (p.Cout == 64 && p.MT == 4 && p.cw == 64) kern = tc_conv_kernel<64, 4, 64, 16, 16>;
-    else if (p.Cout == 32 && p.MT == 4 && p.cw == 64) kern = tc_conv_kernel<32, 4, 64, 16, 16>;
-    else threads = tc_threads(8);
-  }
-  if (kern) {
+  if (c2) {
+    if (p.Cout == 64 && p.MT == 2 && p.cw == 64) kern = tc_conv_kernel<64, 2, 64, true>;
+    else if (p.Cout == 64 && p.MT == 1 && p.cw == 64) kern = tc_conv_kernel<64, 1, 64, true>;
+    else if (p.Cout == 32 && p.MT == 8 && p.cw == 32) kern = tc_conv_kernel<32, 8, 32, true>;
+    else if (p.Cout == 32 && p.MT == 4 && p.cw == 32) kern = tc_conv_kernel<32, 4, 32, true>;
+    else return fail(MB_ERR_INVALID, "tc_pair(%s): no kernel instance for C=%d MT=%d cw=%d", op.name, p.Cout, p.MT, p.cw);
   } else if (p.Cout == 256 && p.MT == 1 && p.cw == 64) kern = tc_conv_kernel<256, 1, 64>;
   else if (p.Cout == 128 && p.MT == 2 && p.cw == 64) kern = tc_conv_kernel<128, 2, 64>;
   else if (p.Cout == 128 && p.MT == 1 && p.cw == 64) kern = tc_conv_kernel<128, 1, 64>;
@@ -767,16 +831,16 @@ int launch_tc(const TcOp& op, const char* tc_arena, const TRef& x16, const TRef&
   else if (p.Cout == 32 && p.MT == 4 && p.cw == 32) kern = tc_conv_kernel<32, 4, 32>;
   else return fail(MB_ERR_INVALID, "tc_conv(%s): no kernel instance for Cout=%d MT=%d cw=%d", op.name, p.Cout, p.MT, p.cw);
   MB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemMax));
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int dev = 0, sms = 0;
+  MB_CUDA_CHECK(cudaGetDevice(&dev));
+  MB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int grid = std::min(p.n_work, sms);
   if (grid <= 0) return MB_OK;
-  // always claim the whole shared memory: one CTA per SM, so the 512-column TMEM allocation never contends
+  // always claim the whole shared memory: one persistent CTA per SM
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(threads);
+  cfg.blockDim = dim3(kTcThreads);
   cfg.dynamicSmemBytes = kSmemMax;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
@@ -918,12 +982,10 @@ int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, 
     p32[i] = ws;
     ws += f32_plane_bytes(B, T, bufs[i].cr);
   }
-  // buffer -> fp16 plane storage.  The fused pair kernel must not write the fp16 plane it is still reading
-  // halos from (other CTAs), so it ping-pongs between the buffer's storage and the unused storage of the
-  // pair's intermediate buffer; map16 tracks where each buffer's current fp16 plane lives.
+  // buffer -> fp16 / fp32 plane storage (identity: every layer writes its own buffer's planes)
   std::vector<int> map16(nb);
   for (int i = 0; i < nb; ++i) map16[i] = i;
-  std::vector<int> map32(nb);  // same indirection for the fp32 planes (fp32-input pair kernel, in-place pairs)
+  std::vector<int> map32(nb);
   for (int i = 0; i < nb; ++i) map32[i] = i;
   std::vector<float> plane_slope(nb, 1.f);  // leaky-relu slope each fp16 storage was written with
   const int n = (int)ops.size();
@@ -945,17 +1007,13 @@ int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, 
     }
     return false;
   };
-  // ---- pre-pass: which (c1, c2) op pairs run as ONE fused kernel (gan_tc_pair.cu)?
-  //   kind 1: fp16-plane input;  kind 2: fp32-plane input (full-rate stage, residual = the pair's input)
-  std::vector<int> fuse_kind(n, 0);
-  std::vector<TcPairParams> pair_plan(n);
+  // ---- pre-pass: which (c1, c2) op pairs run as ONE fused launch (tc_conv_kernel<..., PAIR = true>)?
+  std::vector<char> fuse_next(n, 0);
   for (int i = 0; i + 1 < n; ++i) {
-    memset(&pair_plan[i], 0, sizeof(TcPairParams));
     const TcOp& op = ops[i];
-    if (!tc_fuse_enabled() || !op.is_conv || !op.tc.use_tc || !ops[i + 1].is_conv || !ops[i + 1].tc.use_tc) continue;
-    if (op.tc.x3 || ops[i + 1].tc.x3) continue;                 // 3-term-split layers run unfused (tc_conv_kernel)
-    if (wants_hilo(ops[i + 1].dst, i + 2) && op.cout != 64) continue;  // the pair kernel writes hi/lo planes for C = 64 only
     const TcOp& c2 = ops[i + 1];
+    if (!tc_fuse_enabled() || !op.is_conv || !op.tc.use_tc || !c2.is_conv || !c2.tc.use_tc) continue;
+    if (op.tc.x3 || c2.tc.x3 || op.tc.split3 || c2.tc.split3) continue;  // 3-term-split layers run unfused
     const TapConv& t1 = op.taps;
     const TapConv& t2 = c2.taps;
     const int k = t1.ntaps[0];
@@ -973,13 +1031,12 @@ int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, 
       if (c.src == op.dst || (c.is_conv && (c.res == op.dst || c.dst2 == op.dst))) ok = false;
       if (c.is_conv && c.dst == op.dst && c.taps.mode == EPI_STORE) break;
     }
-    if (!ok) continue;
-    const bool want32 = tc_pair32_enabled() && c2.res == op.src && !res16_ok(c2);
-    if (want32 && tc_pair_plan(op.cin, k, d1, true, &pair_plan[i])) fuse_kind[i] = 2;
-    else if (tc_pair_plan(op.cin, k, d1, false, &pair_plan[i])) fuse_kind[i] = 1;
-    if (fuse_kind[i]) ++i;  // c2 belongs to this pair
+    PairPlan pl;
+    if (ok && pair_plan(op, c2, &pl)) {
+      fuse_next[i] = 1;
+      ++i;  // c2 belongs to this pair
+    }
   }
-  auto reads_f32 = [&](int j) { return fuse_kind[j] == 2; };  // op j (a c1) takes its operand from the fp32 plane
   for (int i = 0; i < n; ++i) {
     const TcOp& op = ops[i];
     if (events) MB_CUDA_CHECK(cudaEventRecord(events[i], st));
@@ -990,7 +1047,7 @@ int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, 
       bool need16 = false;
       float slope16 = 1.f;
       for (int j = i + 1; j < n; ++j) {
-        if (ops[j].is_conv && ops[j].src == op.dst && ops[j].tc.use_tc && !reads_f32(j)) { need16 = true; slope16 = ops[j].taps.in_slope; }
+        if (ops[j].is_conv && ops[j].src == op.dst && ops[j].tc.use_tc) { need16 = true; slope16 = ops[j].taps.in_slope; }
         if (ops[j].is_conv && ops[j].dst == op.dst) break;
       }
       TRef d32 = make_ref(p32[map32[op.dst]], LAYOUT_F32B, op.cout, Lout);
@@ -1012,11 +1069,9 @@ int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, 
       count_launch();
       continue;
     }
-    // ---- fused resblock pair (c1 -> T -> c2), decided in the pre-pass above
-    TcPairParams pp = pair_plan[i];
-    const bool fuse = fuse_kind[i] != 0;
+    const bool fuse = fuse_next[i] != 0;
     const TcOp& oop = fuse ? ops[i + 1] : op;  // the op whose outputs this launch produces
-    const char* fused_x16 = fuse ? p16[map16[op.src]] : nullptr;
+    const int x16_idx = (op.src >= 0 && op.src < nb) ? map16[op.src] : -1;  // storage of the input plane (before any swap)
     const bool use_res16 = res16_ok(oop);
     TRef res16 = use_res16 ? make_ref(p16[map16[oop.res]], LAYOUT_F16B, oop.cout, Lout) : TRef{};
     if (use_res16 && cur16[map16[oop.res]].hilo) {  // the residual buffer currently holds a hi/lo plane (3-term-split consumers)
@@ -1025,9 +1080,9 @@ int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, 
     }
     const float res_slope = use_res16 ? plane_slope[map16[oop.res]] : 1.f;
     const TRef res32 = (oop.res >= 0 && !use_res16) ? make_ref(p32[map32[oop.res]], LAYOUT_F32B, oop.cout, Lout) : TRef{};
-    const char* fused_x32 = (fuse_kind[i] == 2) ? p32[map32[op.src]] : nullptr;
-    if (fuse_kind[i] == 2 && oop.dst == op.src) std::swap(map32[oop.dst], map32[op.dst]);  // write the other fp32 storage
-    if (fuse && oop.dst == op.src) std::swap(map16[oop.dst], map16[op.dst]);  // write the other storage
+    // a fused pair must not write the fp16 plane other CTAs still read halos from: an in-place pair (c2 writes c1's input buffer)
+    // writes the storage of the (dead) intermediate buffer instead
+    if (fuse && oop.dst == op.src) std::swap(map16[oop.dst], map16[op.dst]);
     const int scan_from = fuse ? i + 2 : i + 1;
     // ---- which planes must this op produce? (scan the consumers of dst until it is overwritten)
     bool need16 = false, need32 = false;
@@ -1038,9 +1093,7 @@ int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, 
         const TcOp& c = ops[j];
         if (c.is_conv) {
           if (c.src == buf) {
-            if (reads_f32(j)) {
-              n32 = true;
-            } else if (c.tc.use_tc) {
+            if (c.tc.use_tc) {
               if (hs && s16 != c.taps.in_slope) return fail(MB_ERR_INVALID, "tc_forward: consumers of one buffer disagree on slope");
               n16 = true;
               s16 = c.taps.in_slope;
@@ -1100,39 +1153,6 @@ int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, 
         plane_slope[map16[oop.dst2]] = y2_slope;
       }
     }
-    if (fuse) {
-      const TcOp& c2 = ops[i + 1];
-      pp.L = Lin;
-      pp.x16 = reinterpret_cast<const __half*>(fused_x16);
-      pp.x32 = reinterpret_cast<const float*>(fused_x32);
-      pp.slope_in = op.taps.in_slope;
-      pp.x_Lp = f16_lp(Lin);
-      pp.w1 = reinterpret_cast<const __half*>(tc_arena + op.tc.w16_off);
-      pp.w2 = reinterpret_cast<const __half*>(tc_arena + c2.tc.w16_off);
-      pp.bias1 = op.b32;
-      pp.bias2 = c2.b32;
-      pp.slope_mid = c2.taps.in_slope;
-      pp.res32 = reinterpret_cast<const float*>(res32.p);
-      pp.res16 = reinterpret_cast<const __half*>(res16.p);
-      pp.res_Lp = f16_lp(Lout);
-      pp.res_inv = 1.f / res_slope;
-      pp.y32 = reinterpret_cast<float*>(y32.p);
-      pp.y16 = reinterpret_cast<__half*>(y16.p);
-      pp.y_Lp = f16_lp(Lout);
-      pp.y_hilo = y16.hilo;
-      if (y16.hilo && c2.cout != 64) return fail(MB_ERR_INVALID, "tc_pair(%s): hi/lo output needs C = 64", c2.name);
-      pp.out_slope = slope16;
-      pp.mode = c2.taps.mode;
-      pp.div = c2.taps.div;
-      pp.lengths = lengths;
-      pp.len_mul = c2.taps.len_mul_out;
-      if (pp.mode != EPI_STORE && !pp.y32) return fail(MB_ERR_INVALID, "tc_pair(%s): accumulate mode without fp32 plane", c2.name);
-      int rc = launch_tc_pair(pp, B, st);
-      if (rc != MB_OK) return rc;
-      if (events) MB_CUDA_CHECK(cudaEventRecord(events[i + 1], st));
-      ++i;  // c2 is done as well
-      continue;
-    }
     if (op.tc.split3 && op.src == BUF_IN && y16.p && !y32.p && op.res < 0 && op.dst2 < 0) {
       // conv_pre on the tensor cores, fp32-accurate: split the fp32 input into fp16 hi/lo planes (scratch = any
       // other buffer's fp16 storage; all planes are dead at this point of the forward)
@@ -1164,12 +1184,17 @@ int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, 
       }
     } else if (op.tc.use_tc) {
       if (op.src < 0 || op.src >= nb) return fail(MB_ERR_INVALID, "tc_forward: tensor-core layer %s reads an external buffer", op.name);
-      TRef x16 = make_ref(p16[map16[op.src]], LAYOUT_F16B, op.tc.x3 ? 64 * op.tc.x_pchunks : op.cin, Lin);
+      TRef x16 = make_ref(p16[x16_idx], LAYOUT_F16B, op.tc.x3 ? 64 * op.tc.x_pchunks : op.cin, Lin);
       x16.hilo = op.tc.x3;
-      if (cur16[map16[op.src]].hilo != x16.hilo)
+      if (cur16[x16_idx].hilo != x16.hilo)
         return fail(MB_ERR_INVALID, "tc_forward: %s expects a %s input plane", op.name, x16.hilo ? "hi/lo" : "plain");
-      int rc = launch_tc(op, tc_arena, x16, res32, res16, res_slope, y32, y16, slope16, lengths, B, Lin, st);
+      int rc = launch_tc(op, tc_arena, x16, res32, res16, res_slope, y32, y16, slope16, lengths, B, Lin, st, 0, nullptr,
+                         fuse ? &ops[i + 1] : nullptr);
       if (rc != MB_OK) return rc;
+      if (fuse) {
+        if (events) MB_CUDA_CHECK(cudaEventRecord(events[i + 1], st));
+        ++i;  // c2 is done as well
+      }
     } else {
       TapConv p = op.taps;
       p.B = B;

@@ -1,4 +1,4 @@
-// Tensor-core (tcgen05 / TMEM / bulk-TMA) execution of the GAN generator plan (MB_PREC_F16TC).
+// Tensor-core (wgmma / bulk-TMA) execution of the GAN generator plan (MB_PREC_F16TC).
 // Host-side interface used by gan_api.cu; the kernels live in gan_tc.cu.
 #pragma once
 #include <cuda_runtime.h>
@@ -12,10 +12,10 @@ namespace mb {
 
 // per-layer packing decision, filled by tc_plan_layers
 struct TcLayer {
-  int use_tc = 0;        // 1: tcgen05 kernel, 0: FP32 kernel on blocked layouts
+  int use_tc = 0;        // 1: tensor-core kernel, 0: FP32 kernel on blocked layouts
   int kc = 0;            // input channels per K-chunk (<= 64, multiple of 16)
   int n_cchunks = 0;     // Cin / kc
-  int mt = 1;            // 128-row accumulator tiles per work item
+  int mt = 1;            // 128-row tiles per work item
   size_t slab_bytes = 0; // one (kernel index, chunk) weight image: [kc/8][Cout][8] fp16
   size_t w16_off = 0;    // byte offset of this layer's images in the tensor-core arena section
   int x3 = 0;            // 1: FP32-equivalent 3-term fp16 split of a layer whose input is an internal "hi/lo" plane
@@ -64,54 +64,8 @@ int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, 
                const float* mel, const int32_t* lengths, int B, int T, int num_mels, int hop, float* wav,
                void* workspace, cudaStream_t stream, cudaEvent_t* events /* nullptr or [ops+1] */);
 
-// fused resblock pair (gan_tc_pair.cu): c1 (k taps, dilation d1) -> lrelu -> c2 (k taps, dilation 1)
-struct TcPairParams {
-  int L, C, k, d1, h1, h2;
-  int MT, M_out, W1, W2;
-  int a1_stages, a2_stages;
-  int tiles_per_utt, n_work;
-  uint32_t a1_stage_bytes, a2_bytes, a1_off, a2_off, w1_off, w2_off, bias_off, bar_off;
-  int epi_split;             // 1: epilogue warps 2-5 do E1, 6-9 do E2 (decoupled); 0: all eight do E1 then E2 (round 1)
-  int f32in;                 // 1: the input is the fp32 F32B plane x32 (converted on the fly), no fp16 input plane
-  uint32_t s32_stage_bytes, s32_off;
-  int s32_stages;
-  int s32_pieces;            // row pieces of the fp32 staging window (one mbarrier each): 2 or 4
-  int s32_r0;                // > 0: two UNEQUAL pieces, window rows [0, s32_r0) and [s32_r0, W1) (RT kernels: piece = halo + whole row tiles)
-  int wstream, wstages;      // 1: both weight sets are streamed tap by tap through a ring of wstages slabs (C = 64, k >= 7: they do not fit beside
-                             // double-buffered operands); 0: both resident for the whole kernel
-  int rt;                    // 1: residual preloaded into the second accumulator by the converter warps (tc_pair_kernel<..., RT = true>)
-  const float* x32;
-  float slope_in;            // leaky-relu applied to the input by the converter (c1's in_slope)
-  const __half* x16;
-  int x_Lp;
-  const __half* w1;
-  const __half* w2;
-  const float* bias1;
-  const float* bias2;
-  float slope_mid;
-  const float* res32;
-  const __half* res16;  // residual from an activated fp16 plane: x = y >= 0 ? y : y * res_inv
-  int res_Lp;
-  float res_inv;
-  float* y32;
-  __half* y16;
-  int y_Lp;
-  int y_hilo;                // 1: y16 is a hi/lo plane (C == 64 only: chunk 0 = hi, chunk 1 = lo = fp16(v - hi))
-  float out_slope;
-  int mode;
-  int red_add;               // 1: mode == EPI_ADD without an fp16 output: the epilogue accumulates with red.global.add.v4.f32 (no read of y32)
-  float div;
-  const int32_t* lengths;
-  int len_mul;
-  long long* trace;          // debug (MB_TC_PAIR_TRACE): clock64 stamps of CTA 0's roles, [role 4][item 64][event 8]
-};
-bool tc_pair_plan(int C, int k, int d1, bool f32in, TcPairParams* p);
-// MB_TC_RED_ADD=0: accumulate-mode epilogues read, add and store the running sum themselves (round 2)
+// MB_TC_RED_ADD=0: accumulate-mode epilogues read, add and store the running sum themselves
 bool tc_red_add_enabled();
-int launch_tc_pair(TcPairParams& p, int B, cudaStream_t st);
-// gan_tc_pair32s.cu: fp32-input pair with the residual / result rows kept in shared memory (bulk-TMA in, bulk-TMA out)
-bool tc_pair32s_eligible(const TcPairParams& p);
-int launch_tc_pair32s(const TcPairParams& p, int B, cudaStream_t st, bool* done);
 
 int tc_debug_layer(const TcOp& op, const char* tc_arena, const float* x, const float* residual, int B, int Lin,
                    float* y, void* workspace, size_t workspace_bytes, cudaStream_t stream);

@@ -31,7 +31,7 @@ extern "C" {
 
 const char* mb_last_error(void) { return mb::g_err; }
 
-const char* mb_version(void) { return "mockingbird_b200 0.1 sm_100a"; }
+const char* mb_version(void) { return "mockingbird_b200 0.1 sm_90a"; }
 
 uint64_t mb_launch_count(void) { return mb::g_launches.load(std::memory_order_relaxed); }
 

@@ -1,4 +1,4 @@
-// Mel-spectrogram front-ends on B200 (mb_melspec_*): SURVEY.md section 8f rows N1 / N2.
+// Mel-spectrogram front-ends on H100 (mb_melspec_*): SURVEY.md section 8f rows N1 / N2.
 //
 //   N2  models/encoder/audio.py:53-65      wav_to_mel_spectrogram = librosa.feature.melspectrogram(y, sr=16000,
 //       n_fft=400, hop_length=160, n_mels=40) (power spectrogram, no log), transposed to [frames][40]

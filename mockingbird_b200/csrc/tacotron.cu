@@ -1,4 +1,4 @@
-// Tacotron inference on B200 (mb_tacotron_*): encoder (embedding, PreNet, CBHG), global style token,
+// Tacotron inference on H100 (mb_tacotron_*): encoder (embedding, PreNet, CBHG), global style token,
 // attention decoder loop and postnet CBHG, lowered onto the FP32 kernels of tacotron_kernels.cu plus
 // the location-sensitive-attention step kernel below.
 //

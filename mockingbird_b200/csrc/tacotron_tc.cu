@@ -1,19 +1,19 @@
-// Tensor-core GEMMs of the Tacotron decoder step (sm_100a: tcgen05 / TMEM / bulk-TMA), FP32-accurate.
+// Tensor-core GEMMs of the Tacotron decoder step (sm_90a: wgmma / bulk-TMA / mbarrier), FP32-accurate.
 //
 // The decoder's LSTM cells (tacotron.py:118-127: two LSTMCell(1024) with residuals) are 84 % of the
 // per-step MACs with only batch-many (<= 128) rows: Y[M][4H] = [x | h] . [W_ih | W_hh]^T.  FP32 FFMA
 // kernels are compute-bound there at ~7 TFLOP/s; the tensor cores need fp16 operands, which alone would
 // break the 1e-3 parity bar after 200 recurrent steps.  So every product is computed as a 3-term split
 //     a*w ~= hi(a)*hi(w) + lo(a)*hi(w) + hi(a)*lo(w),   hi(v) = fp16(v), lo(v) = fp16(v - hi(v))
-// with FP32 accumulation in TMEM: ~2^-21 relative per product, i.e. FP32-equivalent (weights are
+// with FP32 accumulation in registers: ~2^-21 relative per product, i.e. FP32-equivalent (weights are
 // pre-scaled by a power of two so that their lo parts stay out of the fp16 subnormal range).
 //
 //   grid      : one CTA per 32 output columns (LSTM: the 4 gates of 8 hidden units, interleaved at pack
 //               time, so the cell update c' = f*c + i*g, h' = o*tanh(c') runs in the epilogue)
 //   operands  : K-major SWIZZLE_128B tiles of 64 k: activations [K/64][rows_pad][64] (hi and lo, written
 //               by act_split_kernel), weights [tile][K/64][hi|lo][32][64]; each tile is one bulk copy
-//   pipeline  : warp 0 producer (4-stage ring), warp 1 MMA issuer (12 MMAs M128 x N32 x K16 per stage),
-//               warps 2-5 epilogue (TMEM lane = batch row)
+//   pipeline  : warp 0 producer (4-stage ring), warpgroups 1-2 MMA (12 wgmmas M64 x N32 x K16 per stage, 64 batch rows
+//               each; the second only for more than 64 rows) and epilogue (one batch row per thread)
 #include <cuda_fp16.h>
 
 #include <cstdlib>
@@ -31,7 +31,8 @@ using namespace tcdev;
 
 constexpr int kStages = 4;          // ring depth of the 32-column kernels (5 stages measured no faster: 37.8 vs 36.0 ms on cfg 4)
 constexpr int kBigStages = 3;       // ring depth of the 128-column kernel (64 KB per stage)
-constexpr int kThreads = 192;
+constexpr int kThreads = 384;    // copy-producer warpgroup + two MMA / epilogue warpgroups (64 rows each)
+constexpr size_t kEpiStageBytes = 2 * 64 * kStageLd * 4;
 constexpr uint32_t kATile = 16384;  // 128 rows x 128 B (rows >= rows_pad stay zero)
 constexpr uint32_t kWTile = 4096;   // 32 rows x 128 B
 constexpr uint32_t kStageBytes = 2 * kATile + 2 * kWTile;
@@ -63,13 +64,6 @@ __device__ __forceinline__ void bulk_g2s_mc(uint32_t dst_smem, const void* src, 
       "l"(src), "r"(bytes), "r"(smem_u32(bar)), "h"(mask)
       : "memory");
 }
-// tcgen05.commit arriving on the mbarrier at this offset in every CTA of `mask`
-__device__ __forceinline__ void tc_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-               "h"(mask)
-               : "memory");
-}
-
 // Shared main loop: operands for output tile `tile` stream through the ring; `epi(m, v)` is called by the
 // epilogue warps with the 32 accumulator columns (already scaled, bias added) of row m.
 template <int NT, int STAGES, typename Epi>
@@ -77,10 +71,8 @@ __device__ __forceinline__ void skinny_body_t(const __half* a_hi_g, const __half
                                               int n_valid, int KB, int M, int rows_pad, float inv_scale, int tile, Epi epi,
                                               size_t a_kb_stride = 0, int kb0 = 0, int KBw = 0, bool compact = false) {
   constexpr uint32_t kWTile = w_tile_bytes<NT>();
-  // `compact` (32-column kernels with <= 64 rows, MB_TACO_RING8): an activation slot is 8 KB instead of 16 - the M = 128 MMA still reads
-  // 128 rows, i.e. runs 8 KB into the following slot (A_lo resp. the weight tiles of the same stage: finite fp16 values), and the
-  // accumulator rows 64-127 it produces from them are never read (epilogue: m < M).  A stage shrinks from 40 to 24 KB, so the ring
-  // holds 8 k-blocks instead of 4: half as many dependent L2 round trips per launch, and no zero fill of the unused rows.
+  // `compact` (32-column kernels with <= 64 rows, MB_TACO_RING8): an activation slot is 8 KB (64 rows) instead of 16, so a stage
+  // shrinks from 40 to 24 KB and the ring holds 8 k-blocks instead of 4: half as many dependent L2 round trips per launch.
   const int kStages = compact ? 2 * STAGES : STAGES;
   const uint32_t kASlot = compact ? kATile / 2 : kATile;
   const uint32_t kStageBytes = 2 * kASlot + 2 * kWTile;
@@ -89,59 +81,42 @@ __device__ __forceinline__ void skinny_body_t(const __half* a_hi_g, const __half
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)kStages * kStageBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + kStages;
-  uint64_t* acc_full = bars + 2 * kStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 1);
-  float* bias_s = reinterpret_cast<float*>(bars + 2 * kStages + 2);
+  float* bias_s = reinterpret_cast<float*>(bars + 2 * kStages);
+
+  float* stage_s = reinterpret_cast<float*>(smem + (size_t)kStages * kStageBytes + 1024);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t a_bytes = (uint32_t)rows_pad * 128u;
   if (a_kb_stride == 0) a_kb_stride = a_bytes;  // bytes between the k-blocks of the activation tiles
   // Optionally launched as clusters of `csize` CTAs (launch_tc_skinny, MB_TACO_MC; off by default, see there): the activation tiles are
-  // the same for every output tile, so each CTA fetches 1 / csize of a tile and multicasts it to the whole cluster (L2 -> SM traffic of a
-  // decoder LSTM launch: 98 -> 41 MB).
-  // A stage is refilled only when ALL CTAs of the cluster have consumed it: every CTA's commit arrives on every CTA's `empty` barrier.
+  // the same for every output tile, so each CTA fetches 1 / csize of a tile and multicasts it to the whole cluster.
+  // A stage is refilled only when ALL CTAs of the cluster have consumed it: every consumer arrives on every CTA's `empty` barrier.
   const uint32_t csize = cluster_nctaid_x();
   const uint32_t crank = cluster_ctarank();
   const bool mc = csize > 1;
   const uint16_t cmask = (uint16_t)((1u << csize) - 1u);
+  // warpgroup g (1, 2) multiplies rows [64 (g - 1), 64 g); the second one only when there are more than 64 rows
+  const uint32_t n_mma_groups = M > 64 ? 2u : 1u;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], mc ? csize : 1u);
+      mbar_init(&empty[i], n_mma_groups * (mc ? csize : 1u));
     }
-    mbar_init(acc_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(NT)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   if (threadIdx.x < NT) bias_s[threadIdx.x] = (bias && tile * NT + (int)threadIdx.x < n_valid) ? bias[tile * NT + threadIdx.x] : 0.f;
-  if (rows_pad < 128 && !compact) {
-    // rows [rows_pad, 128) of every A slot are never written by the copies: zero them once
-    const int nst = KB < kStages ? KB : kStages;
-    for (int s = 0; s < 2 * nst; ++s) {
-      uint8_t* slot = smem + (size_t)(s >> 1) * kStageBytes + (size_t)(s & 1) * kASlot + a_bytes;
-      for (uint32_t i = threadIdx.x * 16u; i < kATile - a_bytes; i += kThreads * 16u)
-        *reinterpret_cast<uint4*>(slot + i) = make_uint4(0u, 0u, 0u, 0u);
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  if (mc) cluster_sync_all();  // every CTA's barriers are initialised before a peer's multicast / commit can reach them
-  const uint32_t tmem_base = *tmem_slot;
-  // Programmatic dependent launch: everything above (barriers, TMEM allocation, bias, zero fill) touched no tensor
-  // another kernel writes and may overlap the tail of the previous launch (recurrences are chains of these
-  // kernels); its outputs are only read below.  A plain launch makes both instructions no-ops.
+  if (mc) cluster_sync_all();  // every CTA's barriers are initialised before a peer's multicast / arrive can reach them
+  // Programmatic dependent launch: everything above (barriers, bias) touched no tensor another kernel writes and may overlap
+  // the tail of the previous launch (recurrences are chains of these kernels); its outputs are only read below.  A plain
+  // launch makes both instructions no-ops.
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    regs_dec<40>();
+    if (warp == 0 && lane == 0) {
       const uint8_t* wt = reinterpret_cast<const uint8_t*>(w_g) + (size_t)tile * (KBw > 0 ? KBw : KB) * (2 * kWTile);
       for (int kb = 0; kb < KB; ++kb) {
         const int s = kb % kStages, ph = (kb / kStages) & 1;
@@ -161,55 +136,67 @@ __device__ __forceinline__ void skinny_body_t(const __half* a_hi_g, const __half
         bulk_g2s(smem_u32(st + 2 * kASlot), wt + kg * (2 * kWTile), 2 * kWTile, &full[s]);
       }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = (1u << 4) | ((uint32_t)(NT >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    const uint64_t desc_hi = make_desc(0, 1024u, 2u, 0);
-    const bool leader = elect_one();
-    for (int kb = 0; kb < KB; ++kb) {
-      const int s = kb % kStages, ph = (kb / kStages) & 1;
-      mbar_wait(&full[s], ph);
-      tc_fence_after();
-      const uint32_t base = smem_u32(smem + (size_t)s * kStageBytes);
-      const uint64_t ah = desc_hi + (uint64_t)(base >> 4);
-      const uint64_t al = desc_hi + (uint64_t)((base + kASlot) >> 4);
-      const uint64_t wh = desc_hi + (uint64_t)((base + 2 * kASlot) >> 4);
-      const uint64_t wl = desc_hi + (uint64_t)((base + 2 * kASlot + kWTile) >> 4);
-      if (leader) {
+  } else {
+    regs_inc<232>();
+    const int g = warp / 4 - 1;
+    const int tid = threadIdx.x & 127;
+    if ((uint32_t)g < n_mma_groups) {
+      // one commit group per stage (12 wgmmas: 4 k-steps x 3 split terms); a stage is released once the next one is issued
+      // and it has completed (wait_group 1)
+      const uint64_t desc_hi = make_desc(0, 1024u, 1u, 0);
+      const uint32_t row_off = (uint32_t)g * 64u * 128u;
+      float acc[NT / 2];
+      auto release = [&](int s) {
+        if (tid != 0) return;
+        if (mc) {
+          for (uint32_t c = 0; c < csize; ++c) mbar_arrive_cluster(&empty[s], c);
+        } else {
+          mbar_arrive(&empty[s]);
+        }
+      };
+      wgmma_fence();
+      for (int kb = 0; kb < KB; ++kb) {
+        const int s = kb % kStages, ph = (kb / kStages) & 1;
+        mbar_wait(&full[s], ph);
+        const uint32_t base = smem_u32(smem + (size_t)s * kStageBytes);
+        const uint64_t ah = desc_hi + (uint64_t)((base + row_off) >> 4);
+        const uint64_t al = desc_hi + (uint64_t)((base + kASlot + row_off) >> 4);
+        const uint64_t wh = desc_hi + (uint64_t)((base + 2 * kASlot) >> 4);
+        const uint64_t wl = desc_hi + (uint64_t)((base + 2 * kASlot + kWTile) >> 4);
+        fence_acc(acc);
+        wgmma_fence();
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          tc_mma_f16(tmem_base, ah + (uint64_t)(2 * k), wh + (uint64_t)(2 * k), idesc, (kb | k) ? 1u : 0u);
-          tc_mma_f16(tmem_base, al + (uint64_t)(2 * k), wh + (uint64_t)(2 * k), idesc, 1u);
-          tc_mma_f16(tmem_base, ah + (uint64_t)(2 * k), wl + (uint64_t)(2 * k), idesc, 1u);
+          wgmma_f16<NT>(acc, ah + (uint64_t)(2 * k), wh + (uint64_t)(2 * k), (kb | k) ? 1u : 0u);
+          wgmma_f16<NT>(acc, al + (uint64_t)(2 * k), wh + (uint64_t)(2 * k), 1u);
+          wgmma_f16<NT>(acc, ah + (uint64_t)(2 * k), wl + (uint64_t)(2 * k), 1u);
         }
-        if (mc) tc_commit_mc(&empty[s], cmask);
-        else tc_commit(&empty[s]);
+        wgmma_commit();
+        wgmma_wait<1>();
+        fence_acc(acc);
+        if (kb > 0) release((kb - 1) % kStages);
       }
-    }
-    if (leader) tc_commit(acc_full);
-  } else {
-    const int quarter = warp & 3;
-    const int m = quarter * 32 + lane;
-    mbar_wait(acc_full, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int c0 = 0; c0 < NT; c0 += 32) {
-      uint32_t raw[32];
-      tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)c0, raw);
-      if (m < M) {
-        float v[32];
+      wgmma_wait<0>();
+      fence_acc(acc);
+      release((KB - 1) % kStages);
+      // epilogue: 32-column slices through shared memory, one row per thread of the first two warps
+      float* stage = stage_s + g * 64 * kStageLd;
+      const int m = g * 64 + tid;
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(raw[i]) * inv_scale + bias_s[c0 + i];
-        epi(m, v, c0);
+      for (int c0 = 0; c0 < NT; c0 += 32) {
+        group_sync(1 + g, 128);
+        stage_acc32(stage, &acc[c0 / 2], tid);
+        group_sync(1 + g, 128);
+        if (tid < 64 && m < M) {
+          float v[32];
+#pragma unroll
+          for (int i = 0; i < 32; ++i) v[i] = stage[tid * kStageLd + i] * inv_scale + bias_s[c0 + i];
+          epi(m, v, c0);
+        }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (mc) cluster_sync_all();  // no CTA leaves while a peer's commit may still arrive on its barriers
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(NT) : "memory");
-  }
+  if (mc) cluster_sync_all();  // no CTA leaves while a peer's arrive may still reach its barriers
 }
 
 // the 32-column instance used by the recurrent kernels (bias already in tile order, all 32 columns valid)
@@ -574,7 +561,7 @@ size_t tc_skinny_act_bytes(int M, int K) {
 }
 
 cudaError_t tc_skinny_absmax(const float* w, size_t n, unsigned int* dev_out, cudaStream_t st) {
-  absmax_kernel<<<148, 256, 0, st>>>(w, n, dev_out);
+  absmax_kernel<<<132, 256, 0, st>>>(w, n, dev_out);
   return cudaGetLastError();
 }
 
@@ -620,7 +607,7 @@ cudaError_t launch_pack_big_w(const TcBigPack& q, __half* dst, cudaStream_t st) 
 
 cudaError_t launch_tc_big(const TcBigArgs& a, cudaStream_t st) {
   if (a.M <= 0 || a.N <= 0 || a.N % 4 || a.KB <= 0 || a.rows_total % 128 || a.rows_total < a.M) return cudaErrorInvalidValue;
-  constexpr size_t smem = kBigStages * stage_bytes<128>() + 1024 + 1024;
+  constexpr size_t smem = kBigStages * stage_bytes<128>() + 1024 + 1024 + kEpiStageBytes;
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(tc_big_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -632,7 +619,7 @@ cudaError_t launch_tc_big(const TcBigArgs& a, cudaStream_t st) {
 
 cudaError_t launch_tc_lstm_seq(const TcLstmSeqArgs& a, cudaStream_t st) {
   if (a.M <= 0 || a.H <= 0 || a.H % 8 || a.KB <= 0 || a.rows_total % 128 || a.rows_total < a.M) return cudaErrorInvalidValue;
-  constexpr size_t smem = kStages * kStageBytes + 1024 + 1024;
+  constexpr size_t smem = kStages * kStageBytes + 1024 + 1024 + kEpiStageBytes;
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(tc_lstm_seq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -646,7 +633,7 @@ cudaError_t launch_tc_gru(const TcGruArgs& a, cudaStream_t st) {
   if (a.M <= 0 || a.M > 128 || a.H <= 0 || a.H % 8 || a.KB <= 0 || a.ndir < 1 || a.ndir > 2) return cudaErrorInvalidValue;
   TcGruArgs p = a;
   p.rows_pad = a.M <= 64 ? 64 : 128;
-  constexpr size_t smem = kStages * kStageBytes + 1024 + 1024;
+  constexpr size_t smem = kStages * kStageBytes + 1024 + 1024 + kEpiStageBytes;
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(tc_gru_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -665,7 +652,7 @@ cudaError_t launch_tc_skinny(const TcSkinnyArgs& a, cudaStream_t st) {
     return e ? atoi(e) != 0 : true;
   }();
   p.compact = (ring8 && p.rows_pad == 64) ? 1 : 0;
-  constexpr size_t smem = (kStages * kStageBytes > 2 * kStages * (kATile + 2 * kWTile) ? kStages * kStageBytes : 2 * kStages * (kATile + 2 * kWTile)) + 1024 + 1024;
+  constexpr size_t smem = (kStages * kStageBytes > 2 * kStages * (kATile + 2 * kWTile) ? kStages * kStageBytes : 2 * kStages * (kATile + 2 * kWTile)) + 1024 + 1024 + kEpiStageBytes;
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(tc_skinny_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

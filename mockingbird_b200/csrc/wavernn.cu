@@ -1,4 +1,4 @@
-// fatchord WaveRNN on B200: conditioning network + the persistent, weight-stationary sample loop.
+// fatchord WaveRNN on H100: conditioning network + the persistent, weight-stationary sample loop.
 //
 // reference: models/vocoder/wavernn/models/fatchord_version.py
 //   UpsampleNetwork / MelResNet :27-85, sample loop of WaveRNN.generate :176-234

@@ -1,1 +1,1 @@
-"""Speaker encoder on the B200 path (reference: models/encoder)."""
+"""Speaker encoder on the H100 path (reference: models/encoder)."""

@@ -1,7 +1,7 @@
 """Encoder audio front-end (reference: models/encoder/audio.py:53-65), SURVEY.md §8f row N2.
 
 ``wav_to_mel_spectrogram(wav)``: 40-channel mel POWER spectrogram (25 ms window, 10 ms step, not log) as float32
-[n_frames, 40], computed on the B200 (mb_melspec_*).  The reference calls librosa.feature.melspectrogram; librosa is
+[n_frames, 40], computed on the H100 (mb_melspec_*).  The reference calls librosa.feature.melspectrogram; librosa is
 unpinned there, and its centered-frame padding changed from "reflect" (<= 0.9) to "constant" (>= 0.10):
 ``pad_mode`` selects which (default "reflect", the behaviour of the librosa releases contemporary with the reference).
 Volume normalisation / VAD trimming (preprocess_wav, webrtcvad) are host-side preprocessing and out of scope."""

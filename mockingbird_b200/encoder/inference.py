@@ -1,6 +1,6 @@
 """Drop-in for ``models/encoder/inference.py`` (reference :15-172): module-global model,
 ``load_model`` / ``set_model`` / ``is_loaded`` / ``embed_frames_batch`` / ``compute_partial_slices`` /
-``embed_utterance``.  The network runs on the B200 (mb_encoder_*); outputs are host numpy like the
+``embed_utterance``.  The network runs on the H100 (mb_encoder_*); outputs are host numpy like the
 reference.  Extension: ``embed_utterances_frames`` embeds many utterances' partial stacks in one batch.
 """
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""``SpeakerEncoder`` on the B200 path (reference: models/encoder/model.py:12-61).
+"""``SpeakerEncoder`` on the H100 path (reference: models/encoder/model.py:12-61).
 
 Same constructor ``SpeakerEncoder(device, loss_device)`` and ``forward(utterances[B, n_frames, 40]) ->
 embeds[B, 256]``; the 3-layer LSTM, the Linear+ReLU and the L2 normalisation run in the CUDA library

@@ -2,7 +2,7 @@
 
 ``melspectrogram(wav, hparams)``: pre-emphasis -> STFT -> 80-band mel of the magnitudes -> dB - ref_level_db ->
 symmetric normalisation to [-max_abs_value, max_abs_value]; float32 [num_mels, n_frames] like the reference, computed on
-the B200 (mb_melspec_*).  ``pad_mode`` as in mockingbird_b200.encoder.audio."""
+the H100 (mb_melspec_*).  ``pad_mode`` as in mockingbird_b200.encoder.audio."""
 from __future__ import annotations
 
 import numpy as np

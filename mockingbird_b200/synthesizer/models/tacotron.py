@@ -1,4 +1,4 @@
-"""``Tacotron`` on the B200 path (reference: models/synthesizer/models/tacotron.py:140-298).
+"""``Tacotron`` on the H100 path (reference: models/synthesizer/models/tacotron.py:140-298).
 
 Same constructor arguments and ``generate(x, speaker_embedding, steps=2000, style_idx=0,
 min_stop_token=5) -> (mel_outputs, linear, attn_scores)`` surface; ``r`` property backed by the loaded

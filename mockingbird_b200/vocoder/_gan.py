@@ -49,7 +49,7 @@ class GanGenerator:
         self.h = h
         if _cfg_get(h, "sampling_rate", 16000) == 24000 and self.KIND == _lib.MB_GAN_HIFIGAN:
             raise NotImplementedError("the 24 kHz InterpolationBlock variant (hifigan/models.py:105-117) "
-                                      "is not part of the B200 path")
+                                      "is not part of the H100 path")
         rates = list(_cfg_get(h, "upsample_rates"))
         kernels = list(_cfg_get(h, "upsample_kernel_sizes"))
         rks = list(_cfg_get(h, "resblock_kernel_sizes"))

@@ -1,4 +1,4 @@
-"""Fre-GAN ``FreGAN`` generator on the B200 path (reference: models/vocoder/fregan/generator.py:79-179)."""
+"""Fre-GAN ``FreGAN`` generator on the H100 path (reference: models/vocoder/fregan/generator.py:79-179)."""
 from __future__ import annotations
 
 from ... import _lib

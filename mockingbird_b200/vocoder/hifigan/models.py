@@ -1,4 +1,4 @@
-"""HiFi-GAN ``Generator`` on the B200 path (reference: models/vocoder/hifigan/models.py:96-162)."""
+"""HiFi-GAN ``Generator`` on the H100 path (reference: models/vocoder/hifigan/models.py:96-162)."""
 from __future__ import annotations
 
 from ... import _lib
@@ -25,7 +25,7 @@ class Generator(GanGenerator):
     """``Generator(h)``; ``forward(mel[B,80,T]) -> wav[B,1,200*T]`` (models.py:134-150).
 
     ``precision``: "auto" (default; picks "f16tc" when a load-time probe shows it within 5e-4 of "f16x3" for this
-    checkpoint, else "f16x3"), "f16tc" (tcgen05, fp16 operands / fp32 accumulate, 3-term split on the serial layers),
-    "f16x3" (tcgen05, 3-term fp16 split everywhere: FP32-equivalent) or "fp32" (FFMA everywhere, ~1e-6)."""
+    checkpoint, else "f16x3"), "f16tc" (wgmma, fp16 operands / fp32 accumulate, 3-term split on the serial layers),
+    "f16x3" (wgmma, 3-term fp16 split everywhere: FP32-equivalent) or "fp32" (FFMA everywhere, ~1e-6)."""
 
     KIND = _lib.MB_GAN_HIFIGAN

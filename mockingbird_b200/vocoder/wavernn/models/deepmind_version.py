@@ -1,4 +1,4 @@
-"""DeepMind-style dual-softmax ``WaveRNN`` on the B200 path (reference: models/vocoder/wavernn/models/deepmind_version.py).
+"""DeepMind-style dual-softmax ``WaveRNN`` on the H100 path (reference: models/vocoder/wavernn/models/deepmind_version.py).
 
 Same constructor and ``generate(seq_len) -> (output, coarse, fine)`` surface (``output = coarse * 256 + fine - 2**15``,
 wavernn/audio.py:34-35).  The whole sample loop - R h, the coarse and the dependent fine gate / MLP / 256-way draw - runs in one

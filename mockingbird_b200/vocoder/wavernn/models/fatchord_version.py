@@ -1,4 +1,4 @@
-"""fatchord ``WaveRNN`` on the B200 path (reference: models/vocoder/wavernn/models/fatchord_version.py:88-257).
+"""fatchord ``WaveRNN`` on the H100 path (reference: models/vocoder/wavernn/models/fatchord_version.py:88-257).
 
 Same constructor and ``generate(mels, batched, target, overlap, mu_law, progress_callback)`` surface.
 The conditioning network and the whole sample loop run in the CUDA library (mb_wavernn_*); the host

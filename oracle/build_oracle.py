@@ -41,7 +41,11 @@ def build_ref(force: bool = False):
     """compile the reference's own monotonic_align/core.pyx into oracle/_ref (container only: needs /root/reference)"""
     import sysconfig
 
-    if not REF_PYX.is_file():
+    try:
+        have_ref = REF_PYX.is_file()
+    except OSError:  # a parent directory this user may not traverse: the reference is absent
+        have_ref = False
+    if not have_ref:
         return ref_so()
     if not force and ref_so() is not None:
         return ref_so()

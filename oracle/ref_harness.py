@@ -26,7 +26,10 @@ REFERENCE_ROOT = Path(os.environ.get("MOCKINGBIRD_REFERENCE", "/root/reference")
 
 
 def reference_available() -> bool:
-    return (REFERENCE_ROOT / "models" / "vocoder" / "hifigan" / "models.py").is_file()
+    try:
+        return (REFERENCE_ROOT / "models" / "vocoder" / "hifigan" / "models.py").is_file()
+    except OSError:  # a parent directory this user may not traverse: the reference is absent
+        return False
 
 
 class _Stub(types.ModuleType):

@@ -11,7 +11,7 @@ sys.path.insert(0, str(ROOT / "synth_weights"))  # seeded random-init weights (n
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
     config.addinivalue_line("markers", "reference: needs /root/reference (build container only)")
 
 

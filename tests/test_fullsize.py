@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import torch
 
+import golden_io
 import ref_init as ri
 import wavernn_oracle as wo
 
@@ -65,7 +66,7 @@ def test_twin_cfg3_three_folds_all_8800_draws(twin, golden_dir):
     """configs[2]: folds 0, 29 and 57 (the last one runs past the end of the conditioning) free running for all
     8 800 steps == the reference; the post-processing restatement reproduces the reference waveform from the
     golden integers"""
-    z = np.load(golden_dir / "wavernn_cfg3.npz")
+    z = golden_io.load(golden_dir / "wavernn_cfg3.npz")
     nf, starts = wo.fold_geometry(2400 * 200, 8000, 400)
     assert nf == 58 and z["idx"].shape == (58, 8800)
     rows = [0, 29, 57]
@@ -85,7 +86,7 @@ def test_tacotron_oracle_cfg4_rows(golden_dir):
     the four stored utterances as their own batch; rows of a batch are independent in eval mode)"""
     import tacotron_oracle as to
 
-    z = np.load(golden_dir / "tacotron_cfg4.npz")
+    z = golden_io.load(golden_dir / "tacotron_cfg4.npz")
     rows = [int(r) for r in z["rows"]]
     chars = torch.from_numpy(z["chars"].astype(np.int64))
     emb = torch.from_numpy(z["emb"])
@@ -124,7 +125,7 @@ def test_gpu_wavernn_cfg1_identical(wmodel, golden_dir):
 def test_gpu_wavernn_cfg3_identical(wmodel, golden_dir):
     """all 58 x 8 800 = 510 400 draws integer-identical to the reference's CPU run under torch.manual_seed(1234);
     a mismatch reports the first diverging step and rows"""
-    z = np.load(golden_dir / "wavernn_cfg3.npz")
+    z = golden_io.load(golden_dir / "wavernn_cfg3.npz")
     torch.manual_seed(1234)
     idx = wmodel.generate_indices(MEL3(), True, 8000, 400, None)
     assert idx.shape == (58, 8800)
@@ -144,7 +145,7 @@ def test_gpu_tacotron_cfg4(golden_dir):
     stored rows within 1e-3 (max-norm relative, asserted at 5e-4), every row's float64 sums, attention argmax path"""
     from mockingbird_b200.synthesizer.inference import Synthesizer
 
-    z = np.load(golden_dir / "tacotron_cfg4.npz")
+    z = golden_io.load(golden_dir / "tacotron_cfg4.npz")
     model = Synthesizer("unused.pt", verbose=False).load_state(ri.tacotron_state_dict(0, r=2, randomize_bn=True))
     chars = torch.from_numpy(z["chars"].astype(np.int64))
     emb = torch.from_numpy(z["emb"])
@@ -202,7 +203,7 @@ def test_torch_oracle_prefix_matches_reference(wsd, golden_dir):
     torch.manual_seed(1234)
     idx, _ = wt.generate_indices(wsd, MEL1(), False, 8000, 400, max_steps=400)
     assert np.array_equal(idx, z1["idx"][:, :400])
-    z3 = np.load(golden_dir / "wavernn_cfg3.npz")
+    z3 = golden_io.load(golden_dir / "wavernn_cfg3.npz")
     torch.manual_seed(1234)
     idx, _ = wt.generate_indices(wsd, MEL3(), True, 8000, 400, max_steps=40)
     assert np.array_equal(idx, z3["idx"][:, :40])

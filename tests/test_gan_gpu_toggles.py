@@ -1,5 +1,5 @@
-"""The f16tc path has run-time switches for A/B measurements (MB_TC_FUSE, MB_TC_RES16, MB_TC_PAIR32, MB_TC_PAIR32S, MB_TC_PAIR_RT, MB_TC_PAIR_WSTREAM, MB_TC_RED_ADD,
-MB_TC_SPLIT3, MB_TC_UPS_X3; read once per process).  Every combination a user can select must stay inside the 1e-3
+"""The f16tc path has run-time switches for A/B measurements (MB_TC_FUSE, MB_TC_RES16, MB_TC_X3_RES16, MB_TC_RED_ADD, MB_TC_SPLIT3,
+MB_TC_UPS_X3, MB_POST_TILE, MB_POST_ROWS; read once per process).  Every combination a user can select must stay inside the 1e-3
 tolerance: each setting runs the golden comparison in a fresh interpreter."""
 import json
 import os
@@ -43,8 +43,9 @@ out["tail"] = tail
 print(json.dumps(out))
 """
 
-ENVS = [{}, {"MB_TC_UPS_X3": "0", "MB_TC_RES16": "0"}, {"MB_TC_FUSE": "0"}, {"MB_TC_RES16": "0"}, {"MB_TC_PAIR32": "0"}, {"MB_TC_PAIR32S": "1"}, {"MB_TC_PAIR_WSTREAM": "1", "MB_TC_PAIR_RT": "1"}, {"MB_TC_PAIR_RT": "0"}, {"MB_TC_RED_ADD": "0"}, {"MB_POST_TILE": "1"}, {"MB_TC_SPLIT3": "0"},
-        {"MB_TC_RES16": "0", "MB_TC_PAIR32": "0", "MB_TC_FUSE": "0"}]
+ENVS = [{}, {"MB_TC_UPS_X3": "0", "MB_TC_RES16": "0"}, {"MB_TC_FUSE": "0"}, {"MB_TC_RES16": "0", "MB_TC_FUSE": "0"}, {"MB_TC_UPS_X3": "0"}, {"MB_TC_RES16": "0"}, {"MB_TC_X3_RES16": "0"},
+        {"MB_POST_ROWS": "1"}, {"MB_POST_ROWS": "4"}, {"MB_TC_RED_ADD": "0"}, {"MB_POST_TILE": "1"}, {"MB_TC_SPLIT3": "0"},
+        {"MB_TC_RES16": "0", "MB_TC_RED_ADD": "0", "MB_TC_SPLIT3": "0"}]
 
 
 @pytest.mark.parametrize("env", ENVS, ids=lambda e: ",".join(f"{k}={v}" for k, v in e.items()) or "default")

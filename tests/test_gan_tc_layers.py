@@ -1,4 +1,4 @@
-"""GPU tests of the tcgen05 tap-conv kernel, one layer at a time (mb_gan_debug_layer).
+"""GPU tests of the tensor-core (wgmma) tap-conv kernel, one layer at a time (mb_gan_debug_layer).
 
 Reference for each layer = torch-CPU conv on operands rounded to fp16 exactly as the kernel rounds
 them (fp16 x fp16 products are exact in the fp32 accumulator), so the only difference left is the

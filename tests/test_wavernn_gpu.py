@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import torch
 
+import golden_io
 import ref_init as ri
 import wavernn_oracle as wo
 
@@ -140,7 +141,7 @@ def test_device_postprocess_matches_reference(model, gold, golden_dir):
     assert w1.dtype == np.float64 and w1.shape == gold["wav1"].shape and np.abs(w1 - gold["wav1"]).max() <= 1e-12
     w2 = model.postprocess_device(torch.from_numpy(gold["idx2"]).cuda(), 30, True, 1000, 100, True)
     assert w2.shape == gold["wav2"].shape and np.abs(w2 - gold["wav2"]).max() <= 1e-12
-    z = np.load(golden_dir / "wavernn_cfg3.npz")
+    z = golden_io.load(golden_dir / "wavernn_cfg3.npz")
     w3 = model.postprocess_device(torch.from_numpy(z["idx"]).cuda(), 2400, True, 8000, 400, True)
     st = int(json.loads(str(z["meta"]))["wav_stride"])
     assert len(w3) == int(z["wav_len"])
