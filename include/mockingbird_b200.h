@@ -134,6 +134,41 @@ int32_t mb_gan_num_layers(const mb_gan* h);
 /* fills a short description "name Cin Cout k dil stride" for layer i; returns 0 on success */
 int mb_gan_layer_info(const mb_gan* h, int32_t layer_index, char* buf, size_t buflen);
 
+/* Host-only (no GPU needed, like mb_gan_create): how the tensor-core forward runs op i of a
+ * MB_PREC_F16TC / MB_PREC_F16X3 handle, as "name key=value ...":
+ *   use_tc x3 split3 kc n_cchunks mt rows_item resident wstages omin omax   (the op launched alone)
+ *   fuse_next fused_prev             1: first / second op of a resblock pair run as ONE fused launch
+ *   pair_mt pair_rows_item pair_resident pair_wstages pair_omin   (fuse_next: the pair's launch)
+ *   kernel=N,MT,CW,PAIR              the tc_conv_kernel instance this op launches (0,0,0,0: none) */
+int mb_gan_tc_plan_info(const mb_gan* h, int32_t op_index, char* buf, size_t buflen);
+
+/* test hook: one tensor-core launch of the plan with caller-chosen epilogue inputs and outputs.
+ * All tensors are device memory; x [B, Cin, L], residual / y [B, Cout, L*stride], y16 [B, C16, L*stride]
+ * fp32 NCL.  The layers run at one input row per frame (lengths count input rows). */
+typedef struct mb_gan_debug_spec {
+  int32_t layer_index;
+  int32_t pair;        /* 0: layer alone; 1: layers (i, i+1) as one fused launch (error if the
+                          forward does not fuse them); 2: the same pair as two launches */
+  int32_t mode;        /* epilogue of the (last) layer: 0 store, 1 y += v, 2 y = (y + v) / div */
+  float div;
+  int32_t red_add;     /* 1: mode 1 without fp16 output accumulates by red.global.add */
+  int32_t res_kind;    /* residual: 0 none, 1 fp32 plane, 2 activated fp16 plane, 3 hi/lo plane */
+  float res_slope;     /* leaky-relu slope of the fp16 residual planes */
+  int32_t out16;       /* fp16 output plane: 0 none, 1 plain, 2 hi/lo */
+  float out_slope;     /* leaky-relu slope of the fp16 output plane */
+  int32_t batch, frames_in;
+  const float* x;
+  const float* residual;
+  const int32_t* lengths; /* [B] or NULL */
+  float* y;            /* running sum in (modes 1, 2), result out; may be NULL in mode 0 */
+  float* y16;          /* out16: the plane read back, C16 = Cout (plain) or the hi/lo plane's
+                          channels (2 Cout, at least 64): hi channels first, then lo */
+} mb_gan_debug_spec;
+/* writes one line per kernel launch into `report`:
+ * "kernel=N,MT,CW,PAIR rows_item= resident= wstages= n_work= grid= red_add=" */
+int mb_gan_debug_launch(mb_gan* h, const mb_gan_debug_spec* spec, void* workspace, size_t workspace_bytes,
+                        void* stream, char* report, size_t report_len);
+
 /* ---------------------------------------------------------------------------------------------
  * fatchord WaveRNN
  *   replaces  models/vocoder/wavernn/models/fatchord_version.py:88-257 (WaveRNN.generate and the

@@ -43,6 +43,27 @@ class GanConfig(C.Structure):
     ]
 
 
+class GanDebugSpec(C.Structure):
+    _fields_ = [
+        ("layer_index", C.c_int32),
+        ("pair", C.c_int32),
+        ("mode", C.c_int32),
+        ("div", C.c_float),
+        ("red_add", C.c_int32),
+        ("res_kind", C.c_int32),
+        ("res_slope", C.c_float),
+        ("out16", C.c_int32),
+        ("out_slope", C.c_float),
+        ("batch", C.c_int32),
+        ("frames_in", C.c_int32),
+        ("x", C.c_void_p),
+        ("residual", C.c_void_p),
+        ("lengths", C.c_void_p),
+        ("y", C.c_void_p),
+        ("y16", C.c_void_p),
+    ]
+
+
 class WaveRNNConfig(C.Structure):
     _fields_ = [
         ("rnn_dims", C.c_int32),
@@ -100,6 +121,9 @@ SIGNATURES = {
                                      C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_gan_num_layers": (C.c_int32, [C.c_void_p]),
     "mb_gan_layer_info": (C.c_int, [C.c_void_p, C.c_int32, C.c_char_p, C.c_size_t]),
+    "mb_gan_tc_plan_info": (C.c_int, [C.c_void_p, C.c_int32, C.c_char_p, C.c_size_t]),
+    "mb_gan_debug_launch": (C.c_int, [C.c_void_p, C.POINTER(GanDebugSpec), C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p,
+                                      C.c_size_t]),
     "mb_wavernn_create": (C.c_int, [C.POINTER(WaveRNNConfig), C.POINTER(C.c_void_p)]),
     "mb_wavernn_destroy": (None, [C.c_void_p]),
     "mb_wavernn_arena_bytes": (C.c_size_t, [C.c_void_p]),

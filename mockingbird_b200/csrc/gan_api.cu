@@ -370,6 +370,31 @@ TRef ncl(const void* p, int C, int L) {
   return t;
 }
 
+TcOp tc_op(const mb_gan* h, const Layer& L) {
+  TcOp o{};
+  o.is_conv = (L.kind == OP_CONV);
+  o.taps = L.taps;
+  o.tc = L.tc;
+  o.name = L.name.c_str();
+  o.src = L.src;
+  o.dst = L.dst;
+  o.res = L.res;
+  o.dst2 = L.dst2;
+  o.cin = L.cin;
+  o.cout = L.cout;
+  o.rate_in = L.rate_in;
+  o.rate_out = L.rate_out;
+  o.w32 = h->arena ? h->arena + L.w_off : nullptr;  // (the plan query runs before an arena is set)
+  o.b32 = h->arena ? h->arena + L.b_off : nullptr;
+  return o;
+}
+
+std::vector<TcOp> tc_ops(const mb_gan* h) {
+  std::vector<TcOp> ops;
+  for (const Layer& L : h->layers) ops.push_back(tc_op(h, L));
+  return ops;
+}
+
 int run_layer_f32(mb_gan* h, const Layer& L, const float* src, const float* res, float* dst, float* dst2,
                   const int32_t* lengths, int B, int T, cudaStream_t st) {
   if (L.kind == OP_ADD) {
@@ -532,25 +557,7 @@ static int gan_forward_impl(mb_gan* h, const float* mel, const int32_t* lengths,
     return fail(MB_ERR_WORKSPACE, "mb_gan_forward: workspace %zu < %zu bytes", workspace_bytes, need);
   cudaStream_t st = (cudaStream_t)stream;
   if (h->cfg.precision != MB_PREC_FP32) {
-    std::vector<TcOp> ops;
-    for (const Layer& L : h->layers) {
-      TcOp o{};
-      o.is_conv = (L.kind == OP_CONV);
-      o.taps = L.taps;
-      o.tc = L.tc;
-      o.name = L.name.c_str();
-      o.src = L.src;
-      o.dst = L.dst;
-      o.res = L.res;
-      o.dst2 = L.dst2;
-      o.cin = L.cin;
-      o.cout = L.cout;
-      o.rate_in = L.rate_in;
-      o.rate_out = L.rate_out;
-      o.w32 = h->arena + L.w_off;
-      o.b32 = h->arena + L.b_off;
-      ops.push_back(o);
-    }
+    const std::vector<TcOp> ops = tc_ops(h);
     std::vector<TcBufReq> req;
     for (size_t i = 0; i < h->buf_cr.size(); ++i) req.push_back({h->buf_cr[i]});
     char* tcbase = (char*)h->arena + align_up(h->f32_floats * sizeof(float), 256);
@@ -655,6 +662,94 @@ int mb_gan_debug_layer(mb_gan* h, int32_t i, const float* x, const float* residu
     return tc_debug_layer(o, tcbase, x, residual, batch, frames_in, y, workspace, workspace_bytes, st);
   }
   return run_layer_f32(h, L, x, residual, y, nullptr, nullptr, batch, frames_in, st);
+}
+
+int mb_gan_tc_plan_info(const mb_gan* h, int32_t i, char* buf, size_t buflen) {
+  if (!h || !buf || i < 0 || i >= (int32_t)h->layers.size()) return fail(MB_ERR_INVALID, "mb_gan_tc_plan_info: bad index");
+  if (h->cfg.precision == MB_PREC_FP32) return fail(MB_ERR_INVALID, "mb_gan_tc_plan_info: fp32 handle has no tensor-core plan");
+  const std::vector<TcOp> ops = tc_ops(h);
+  const std::vector<char> fuse = tc_fusion_plan(ops, (int)h->buf_cr.size());
+  TcOpPlan p;
+  int rc = tc_op_plan(ops, fuse, i, &p);
+  if (rc != MB_OK) return rc;
+  snprintf(buf, buflen,
+           "%s use_tc=%d x3=%d split3=%d kc=%d n_cchunks=%d mt=%d rows_item=%d resident=%d wstages=%d omin=%d omax=%d "
+           "fuse_next=%d fused_prev=%d pair_mt=%d pair_rows_item=%d pair_resident=%d pair_wstages=%d pair_omin=%d "
+           "kernel=%d,%d,%d,%d",
+           h->layers[i].name.c_str(), p.use_tc, p.x3, p.split3, p.kc, p.n_cchunks, p.mt, p.rows_item, p.resident, p.wstages,
+           p.omin, p.omax, p.fuse_next, p.fused_prev, p.pair_mt, p.pair_rows_item, p.pair_resident, p.pair_wstages, p.pair_omin,
+           p.kn, p.kmt, p.kcw, p.kpair);
+  return MB_OK;
+}
+
+int mb_gan_debug_launch(mb_gan* h, const mb_gan_debug_spec* s, void* workspace, size_t workspace_bytes, void* stream,
+                        char* report, size_t report_len) {
+  if (!h || !s || !workspace || !s->x) return fail(MB_ERR_INVALID, "mb_gan_debug_launch: null argument");
+  const int32_t i = s->layer_index;
+  const int32_t n = (int32_t)h->layers.size();
+  if (h->cfg.precision == MB_PREC_FP32) return fail(MB_ERR_INVALID, "mb_gan_debug_launch: fp32 handle has no tensor-core layers");
+  if (i < 0 || i >= n || s->pair < 0 || s->pair > 2 || (s->pair && i + 1 >= n))
+    return fail(MB_ERR_INVALID, "mb_gan_debug_launch: bad layer %d / pair %d", i, s->pair);
+  if (s->mode < EPI_STORE || s->mode > EPI_ADD_DIV) return fail(MB_ERR_INVALID, "mb_gan_debug_launch: bad mode %d", s->mode);
+  if (s->batch <= 0 || s->frames_in <= 0) return fail(MB_ERR_INVALID, "mb_gan_debug_launch: empty batch");
+  const int nl = s->pair ? 2 : 1;
+  for (int k = 0; k < nl; ++k) {
+    const Layer& L = h->layers[i + k];
+    if (L.kind != OP_CONV) return fail(MB_ERR_INVALID, "mb_gan_debug_launch: layer %d is not a conv", i + k);
+    if (!L.w_set || !L.b_set) return fail(MB_ERR_STATE, "mb_gan_debug_launch: weights of %s not set", L.name.c_str());
+  }
+  if (s->pair) {
+    const std::vector<char> fuse = tc_fusion_plan(tc_ops(h), (int)h->buf_cr.size());
+    if (!fuse[i])
+      return fail(MB_ERR_INVALID, "mb_gan_debug_launch: %s and %s are not a fused pair", h->layers[i].name.c_str(),
+                  h->layers[i + 1].name.c_str());
+  }
+  // run at rate_in = 1 (frames_in = input rows); the last op takes the requested accumulate mode
+  TcOp o[2];
+  for (int k = 0; k < nl; ++k) {
+    const Layer& L = h->layers[i + k];
+    o[k] = tc_op(h, L);
+    const int mult = L.rate_out / L.rate_in;
+    o[k].rate_in = 1;
+    o[k].rate_out = mult;
+    o[k].taps.len_mul_in = 1;
+    o[k].taps.len_mul_out = mult;
+  }
+  o[nl - 1].taps.mode = s->mode;
+  o[nl - 1].taps.div = s->div;
+  TcDebugSpec d;
+  d.B = s->batch;
+  d.Lin = s->frames_in;
+  d.x = s->x;
+  d.res = s->residual;
+  d.res_kind = s->res_kind;
+  d.res_slope = s->res_slope;
+  d.lengths = s->lengths;
+  d.red_add = s->red_add != 0;
+  d.y = s->y;
+  d.out16 = s->out16;
+  d.out_slope = s->out_slope;
+  d.y16 = s->y16;
+  d.two_launches = s->pair == 2;
+  char* tcbase = (char*)h->arena + align_up(h->f32_floats * sizeof(float), 256);
+  TcLaunchInfo info[2];
+  int launches = 0;
+  int rc = tc_debug_launch(o[0], s->pair ? &o[1] : nullptr, d, tcbase, workspace, workspace_bytes, (cudaStream_t)stream, info,
+                           &launches);
+  if (rc != MB_OK) return rc;
+  if (report && report_len) {
+    size_t used = 0;
+    report[0] = 0;
+    for (int k = 0; k < launches && used < report_len; ++k) {
+      const TcLaunchInfo& f = info[k];
+      const int w = snprintf(report + used, report_len - used,
+                             "kernel=%d,%d,%d,%d rows_item=%d resident=%d wstages=%d n_work=%d grid=%d red_add=%d\n", f.n, f.mt,
+                             f.cw, f.pair, f.rows_item, f.resident, f.wstages, f.n_work, f.grid, f.red_add);
+      if (w < 0) break;
+      used += (size_t)w;
+    }
+  }
+  return MB_OK;
 }
 
 }  // extern "C"

@@ -716,15 +716,45 @@ int tc_baseoff_mode() {
   return mode;
 }
 
+// every compiled tc_conv_kernel instance <N, MT, CW, PAIR>; launch_tc and the plan query pick from this list.  tc_plan_layers
+// never picks <32, 2, 64>, <32, 4, 32> or <64, 1, 64> for a layer launched alone (a C = 32 fp16 layer's weights are resident at
+// MT = 8, a C = 64 layer always fits MT >= 2), so those are not compiled.
+struct TcInstance {
+  int n, mt, cw;
+  bool pair;
+  void (*kern)(const TcParams);
+};
+const TcInstance kTcInstances[] = {
+    {256, 1, 64, false, tc_conv_kernel<256, 1, 64>},
+    {128, 2, 64, false, tc_conv_kernel<128, 2, 64>},
+    {128, 1, 64, false, tc_conv_kernel<128, 1, 64>},
+    {64, 4, 64, false, tc_conv_kernel<64, 4, 64>},
+    {64, 2, 64, false, tc_conv_kernel<64, 2, 64>},
+    {32, 8, 32, false, tc_conv_kernel<32, 8, 32>},
+    {32, 4, 64, false, tc_conv_kernel<32, 4, 64>},
+    {64, 2, 64, true, tc_conv_kernel<64, 2, 64, true>},
+    {64, 1, 64, true, tc_conv_kernel<64, 1, 64, true>},
+    {32, 8, 32, true, tc_conv_kernel<32, 8, 32, true>},
+    {32, 4, 32, true, tc_conv_kernel<32, 4, 32, true>},
+};
+const TcInstance* find_instance(int n, int mt, int cw, bool pair) {
+  for (const TcInstance& k : kTcInstances)
+    if (k.n == n && k.mt == mt && k.cw == cw && k.pair == pair) return &k;
+  return nullptr;
+}
+
 size_t f16_plane_bytes(size_t B, size_t T, size_t cr) {
   // rows are padded to Lp = ceil8(L + 2*kPadRows) <= L + 2*kPadRows + 7 for at most 512 channels
   return align_up(2 * B * T * cr + 2 * B * 1024 * (2 * kPadRows + 7) + kPlaneSlack, 1024);  // pad rows of <= 1024 channels (hi/lo of 512)
 }
 size_t f32_plane_bytes(size_t B, size_t T, size_t cr) { return align_up(4 * B * T * cr + 256, 1024); }
 
+// red_add: an EPI_ADD launch without fp16 output may accumulate by red.global.add (else read-add-store).
+// info (optional): what was launched.
 int launch_tc(const TcOp& op, const char* tc_arena, const TRef& x16, const TRef& res32, const TRef& res16, float res_slope,
               const TRef& y32, const TRef& y16, float out_slope, const int32_t* lengths, int B, int Lin, cudaStream_t st,
-              int y_c0 = 0, const float* bias_override = nullptr, const TcOp* c2 = nullptr) {
+              bool red_add, int y_c0 = 0, const float* bias_override = nullptr, const TcOp* c2 = nullptr,
+              TcLaunchInfo* info = nullptr) {
   PairPlan pl;
   if (c2 && !pair_plan(op, *c2, &pl)) return fail(MB_ERR_INVALID, "tc_pair(%s): no shared-memory plan", op.name);
   const TapConv& t = c2 ? pl.t1 : op.taps;
@@ -786,7 +816,7 @@ int launch_tc(const TcOp& op, const char* tc_arena, const TRef& x16, const TRef&
   p.y_lo_c = (y16.p && y16.hilo) ? (y16.C >> 1) : -1;
   p.out_slope = out_slope;
   p.mode = t.mode;
-  p.red_add = (p.mode == EPI_ADD && !y16.p && y32.p && tc_red_add_enabled()) ? 1 : 0;
+  p.red_add = (p.mode == EPI_ADD && !y16.p && y32.p && red_add) ? 1 : 0;
   p.div = t.div;
   p.lengths = lengths;
   p.len_mul_out = t.len_mul_out;
@@ -806,35 +836,35 @@ int launch_tc(const TcOp& op, const char* tc_arena, const TRef& x16, const TRef&
     p.mode = u.mode;
     p.div = u.div;
     p.len_mul_out = u.len_mul_out;
-    p.red_add = (p.mode == EPI_ADD && !y16.p && y32.p && tc_red_add_enabled()) ? 1 : 0;
+    p.red_add = (p.mode == EPI_ADD && !y16.p && y32.p && red_add) ? 1 : 0;
   }
   if (res16.p && !res16.hilo && res16.C != t.Cout) return fail(MB_ERR_INVALID, "tc_conv(%s): fp16 residual plane geometry", op.name);
   if (res16.p && res16.hilo && res16.C != (t.Cout >= 64 ? 2 * t.Cout : 64)) return fail(MB_ERR_INVALID, "tc_conv(%s): hi/lo residual plane geometry", op.name);
   if (y_c0 != 0 && (p.y32 || p.res32 || p.res16)) return fail(MB_ERR_INVALID, "tc_conv(%s): channel-offset launch supports the fp16 plane only", op.name);
   if (p.mode != EPI_STORE && !p.y32) return fail(MB_ERR_INVALID, "tc_conv(%s): accumulate mode without fp32 plane", op.name);
-  void (*kern)(const TcParams) = nullptr;
-  if (c2) {
-    if (p.Cout == 64 && p.MT == 2 && p.cw == 64) kern = tc_conv_kernel<64, 2, 64, true>;
-    else if (p.Cout == 64 && p.MT == 1 && p.cw == 64) kern = tc_conv_kernel<64, 1, 64, true>;
-    else if (p.Cout == 32 && p.MT == 8 && p.cw == 32) kern = tc_conv_kernel<32, 8, 32, true>;
-    else if (p.Cout == 32 && p.MT == 4 && p.cw == 32) kern = tc_conv_kernel<32, 4, 32, true>;
-    else return fail(MB_ERR_INVALID, "tc_pair(%s): no kernel instance for C=%d MT=%d cw=%d", op.name, p.Cout, p.MT, p.cw);
-  } else if (p.Cout == 256 && p.MT == 1 && p.cw == 64) kern = tc_conv_kernel<256, 1, 64>;
-  else if (p.Cout == 128 && p.MT == 2 && p.cw == 64) kern = tc_conv_kernel<128, 2, 64>;
-  else if (p.Cout == 128 && p.MT == 1 && p.cw == 64) kern = tc_conv_kernel<128, 1, 64>;
-  else if (p.Cout == 64 && p.MT == 4 && p.cw == 64) kern = tc_conv_kernel<64, 4, 64>;
-  else if (p.Cout == 64 && p.MT == 2 && p.cw == 64) kern = tc_conv_kernel<64, 2, 64>;
-  else if (p.Cout == 64 && p.MT == 1 && p.cw == 64) kern = tc_conv_kernel<64, 1, 64>;
-  else if (p.Cout == 32 && p.MT == 8 && p.cw == 32) kern = tc_conv_kernel<32, 8, 32>;
-  else if (p.Cout == 32 && p.MT == 2 && p.cw == 64) kern = tc_conv_kernel<32, 2, 64>;
-  else if (p.Cout == 32 && p.MT == 4 && p.cw == 64) kern = tc_conv_kernel<32, 4, 64>;
-  else if (p.Cout == 32 && p.MT == 4 && p.cw == 32) kern = tc_conv_kernel<32, 4, 32>;
-  else return fail(MB_ERR_INVALID, "tc_conv(%s): no kernel instance for Cout=%d MT=%d cw=%d", op.name, p.Cout, p.MT, p.cw);
+  const TcInstance* inst = find_instance(p.Cout, p.MT, p.cw, c2 != nullptr);
+  if (!inst)
+    return fail(MB_ERR_INVALID, "%s(%s): no kernel instance for Cout=%d MT=%d cw=%d", c2 ? "tc_pair" : "tc_conv", op.name, p.Cout,
+                p.MT, p.cw);
+  void (*kern)(const TcParams) = inst->kern;
   MB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemMax));
   int dev = 0, sms = 0;
   MB_CUDA_CHECK(cudaGetDevice(&dev));
   MB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int grid = std::min(p.n_work, sms);
+  if (info) {
+    *info = TcLaunchInfo{};
+    info->n = inst->n;
+    info->mt = inst->mt;
+    info->cw = inst->cw;
+    info->pair = inst->pair ? 1 : 0;
+    info->rows_item = p.rows_item;
+    info->resident = p.resident;
+    info->wstages = p.wstages;
+    info->n_work = p.n_work;
+    info->grid = grid;
+    info->red_add = p.red_add;
+  }
   if (grid <= 0) return MB_OK;
   // always claim the whole shared memory: one persistent CTA per SM
   cudaLaunchConfig_t cfg;
@@ -966,6 +996,90 @@ size_t tc_workspace_bytes(const std::vector<TcBufReq>& bufs, int B, int T, int n
   return total;
 }
 
+std::vector<char> tc_fusion_plan(const std::vector<TcOp>& ops, int nb) {
+  const int n = (int)ops.size();
+  std::vector<char> fuse_next(n, 0);
+  for (int i = 0; i + 1 < n; ++i) {
+    const TcOp& op = ops[i];
+    const TcOp& c2 = ops[i + 1];
+    if (!tc_fuse_enabled() || !op.is_conv || !op.tc.use_tc || !c2.is_conv || !c2.tc.use_tc) continue;
+    if (op.tc.x3 || c2.tc.x3 || op.tc.split3 || c2.tc.split3) continue;  // 3-term-split layers run unfused
+    const TapConv& t1 = op.taps;
+    const TapConv& t2 = c2.taps;
+    const int k = t1.ntaps[0];
+    const int d1 = k > 1 ? t1.off[0][1] - t1.off[0][0] : 1;
+    bool ok = op.cin == op.cout && c2.cin == c2.cout && op.cin == c2.cin && t1.stride == 1 && t2.stride == 1 &&
+              t2.ntaps[0] == k && (k & 1) && op.res < 0 && op.dst2 < 0 && c2.dst2 < 0 && t1.mode == EPI_STORE &&
+              op.dst == c2.src && op.dst >= 0 && op.dst < nb && op.src >= 0 && op.src < nb && c2.res != op.dst &&
+              op.rate_in == c2.rate_in;
+    for (int t = 0; ok && t < k; ++t)
+      ok = (t1.off[0][t] == t * d1 - d1 * (k - 1) / 2) && (t2.off[0][t] == t - (k - 1) / 2) && t1.slab[0][t] == t &&
+           t2.slab[0][t] == t;
+    // the intermediate buffer must not be read by anything but c2 before it is overwritten
+    for (int j = i + 2; ok && j < n; ++j) {
+      const TcOp& c = ops[j];
+      if (c.src == op.dst || (c.is_conv && (c.res == op.dst || c.dst2 == op.dst))) ok = false;
+      if (c.is_conv && c.dst == op.dst && c.taps.mode == EPI_STORE) break;
+    }
+    PairPlan pl;
+    if (ok && pair_plan(op, c2, &pl)) {
+      fuse_next[i] = 1;
+      ++i;  // c2 belongs to this pair
+    }
+  }
+  return fuse_next;
+}
+
+int tc_op_plan(const std::vector<TcOp>& ops, const std::vector<char>& fuse_next, int i, TcOpPlan* out) {
+  *out = TcOpPlan{};
+  const TcOp& op = ops[i];
+  if (!op.is_conv) return MB_OK;
+  out->use_tc = op.tc.use_tc;
+  out->x3 = op.tc.x3;
+  out->split3 = op.tc.split3;
+  out->fuse_next = fuse_next[i];
+  out->fused_prev = i > 0 && fuse_next[i - 1];
+  if (!op.tc.use_tc && !op.tc.split3) return MB_OK;
+  // the geometry launch_tc runs: conv_pre's split as 256-channel halves, everything else as planned
+  TcOp o = op;
+  if (op.tc.split3) {
+    o.taps.Cin = 256;
+    o.taps.Cout = 256;
+  }
+  const TapConv& t = o.taps;
+  out->kc = o.tc.kc;
+  out->n_cchunks = o.tc.n_cchunks;
+  out->mt = o.tc.mt;
+  SmemPlan sp;
+  if (!plan_smem(t, o.tc, kernel_count(t) * o.tc.n_cchunks, &sp))
+    return fail(MB_ERR_INVALID, "tc_plan(%s): shared memory plan failed", op.name);
+  out->resident = sp.resident;
+  out->wstages = sp.wstages;
+  out->omin = sp.omin;
+  out->omax = -0x7fffffff;
+  for (int r = 0; r < t.stride; ++r)
+    for (int k = 0; k < t.ntaps[r]; ++k) out->omax = std::max(out->omax, t.off[r][k]);
+  out->rows_item = o.tc.mt * 128;
+  const TcInstance* inst = find_instance(t.Cout, o.tc.mt, o.tc.kc, false);
+  if (out->fuse_next) {
+    PairPlan pl;
+    if (!pair_plan(op, ops[i + 1], &pl)) return fail(MB_ERR_INVALID, "tc_plan(%s): fused pair without a plan", op.name);
+    out->pair_mt = pl.mt;
+    out->pair_rows_item = pl.mt * 128 - 2 * pl.h2;
+    out->pair_resident = pl.sp.resident;
+    out->pair_wstages = pl.sp.wstages;
+    out->pair_omin = pl.sp.omin;
+    inst = find_instance(t.Cout, pl.mt, o.tc.kc, true);
+  }
+  if (out->fused_prev) return MB_OK;  // launched by the previous op
+  if (!inst) return fail(MB_ERR_INVALID, "tc_plan(%s): no kernel instance", op.name);
+  out->kn = inst->n;
+  out->kmt = inst->mt;
+  out->kcw = inst->cw;
+  out->kpair = inst->pair ? 1 : 0;
+  return MB_OK;
+}
+
 int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, const char* tc_arena,
                const float* mel, const int32_t* lengths, int B, int T, int num_mels, int hop, float* wav,
                void* workspace, cudaStream_t st, cudaEvent_t* events) {
@@ -1007,36 +1121,7 @@ int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, 
     }
     return false;
   };
-  // ---- pre-pass: which (c1, c2) op pairs run as ONE fused launch (tc_conv_kernel<..., PAIR = true>)?
-  std::vector<char> fuse_next(n, 0);
-  for (int i = 0; i + 1 < n; ++i) {
-    const TcOp& op = ops[i];
-    const TcOp& c2 = ops[i + 1];
-    if (!tc_fuse_enabled() || !op.is_conv || !op.tc.use_tc || !c2.is_conv || !c2.tc.use_tc) continue;
-    if (op.tc.x3 || c2.tc.x3 || op.tc.split3 || c2.tc.split3) continue;  // 3-term-split layers run unfused
-    const TapConv& t1 = op.taps;
-    const TapConv& t2 = c2.taps;
-    const int k = t1.ntaps[0];
-    const int d1 = k > 1 ? t1.off[0][1] - t1.off[0][0] : 1;
-    bool ok = op.cin == op.cout && c2.cin == c2.cout && op.cin == c2.cin && t1.stride == 1 && t2.stride == 1 &&
-              t2.ntaps[0] == k && (k & 1) && op.res < 0 && op.dst2 < 0 && c2.dst2 < 0 && t1.mode == EPI_STORE &&
-              op.dst == c2.src && op.dst >= 0 && op.dst < nb && op.src >= 0 && op.src < nb && c2.res != op.dst &&
-              op.rate_in == c2.rate_in;
-    for (int t = 0; ok && t < k; ++t)
-      ok = (t1.off[0][t] == t * d1 - d1 * (k - 1) / 2) && (t2.off[0][t] == t - (k - 1) / 2) && t1.slab[0][t] == t &&
-           t2.slab[0][t] == t;
-    // the intermediate buffer must not be read by anything but c2 before it is overwritten
-    for (int j = i + 2; ok && j < n; ++j) {
-      const TcOp& c = ops[j];
-      if (c.src == op.dst || (c.is_conv && (c.res == op.dst || c.dst2 == op.dst))) ok = false;
-      if (c.is_conv && c.dst == op.dst && c.taps.mode == EPI_STORE) break;
-    }
-    PairPlan pl;
-    if (ok && pair_plan(op, c2, &pl)) {
-      fuse_next[i] = 1;
-      ++i;  // c2 belongs to this pair
-    }
-  }
+  const std::vector<char> fuse_next = tc_fusion_plan(ops, nb);
   for (int i = 0; i < n; ++i) {
     const TcOp& op = ops[i];
     if (events) MB_CUDA_CHECK(cudaEventRecord(events[i], st));
@@ -1178,8 +1263,8 @@ int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, 
         half.taps.Cin = 256;
         half.taps.Cout = 256;
         half.tc.w16_off = op.tc.w16_off + (size_t)hf * kernel_count(op.taps) * 4 * op.tc.slab_bytes;
-        int rc = launch_tc(half, tc_arena, xs, TRef{}, TRef{}, 1.f, TRef{}, y16, slope16, lengths, B, Lin, st, hf * 256,
-                           op.b32 ? op.b32 + hf * 256 : nullptr);
+        int rc = launch_tc(half, tc_arena, xs, TRef{}, TRef{}, 1.f, TRef{}, y16, slope16, lengths, B, Lin, st,
+                           tc_red_add_enabled(), hf * 256, op.b32 ? op.b32 + hf * 256 : nullptr);
         if (rc != MB_OK) return rc;
       }
     } else if (op.tc.use_tc) {
@@ -1188,8 +1273,8 @@ int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, 
       x16.hilo = op.tc.x3;
       if (cur16[x16_idx].hilo != x16.hilo)
         return fail(MB_ERR_INVALID, "tc_forward: %s expects a %s input plane", op.name, x16.hilo ? "hi/lo" : "plain");
-      int rc = launch_tc(op, tc_arena, x16, res32, res16, res_slope, y32, y16, slope16, lengths, B, Lin, st, 0, nullptr,
-                         fuse ? &ops[i + 1] : nullptr);
+      int rc = launch_tc(op, tc_arena, x16, res32, res16, res_slope, y32, y16, slope16, lengths, B, Lin, st,
+                         tc_red_add_enabled(), 0, nullptr, fuse ? &ops[i + 1] : nullptr);
       if (rc != MB_OK) return rc;
       if (fuse) {
         if (events) MB_CUDA_CHECK(cudaEventRecord(events[i + 1], st));
@@ -1261,11 +1346,92 @@ int tc_debug_layer(const TcOp& op, const char* tc_arena, const float* x, const f
     e = launch_convert_layout(make_ref(const_cast<float*>(residual), LAYOUT_NCL, t.Cout, Lout), r32, B, 1.f, st);
     if (e != cudaSuccess) return fail(MB_ERR_CUDA, "convert: %s", cudaGetErrorString(e));
   }
-  int rc = launch_tc(op, tc_arena, x16, r32, TRef{}, 1.f, y32, TRef{}, 1.f, nullptr, B, Lin, st);
+  int rc = launch_tc(op, tc_arena, x16, r32, TRef{}, 1.f, y32, TRef{}, 1.f, nullptr, B, Lin, st, tc_red_add_enabled());
   if (rc != MB_OK) return rc;
   e = launch_convert_layout(y32, yn, B, 1.f, st);
   if (e != cudaSuccess) return fail(MB_ERR_CUDA, "convert: %s", cudaGetErrorString(e));
   count_launch(3);
+  return MB_OK;
+}
+
+int tc_debug_launch(const TcOp& op, const TcOp* c2, const TcDebugSpec& s, const char* tc_arena, void* workspace,
+                    size_t workspace_bytes, cudaStream_t st, TcLaunchInfo* info, int* n_launches) {
+  *n_launches = 0;
+  const TcOp& last = c2 ? *c2 : op;  // the op whose outputs the launch produces
+  if (!op.tc.use_tc || !last.tc.use_tc) return fail(MB_ERR_INVALID, "tc_debug_launch(%s): not a tensor-core layer", op.name);
+  const int B = s.B, Lin = s.Lin, Lout = Lin * op.taps.stride;
+  const int Cout = last.taps.Cout;
+  const int xC = op.tc.x3 ? 64 * op.tc.x_pchunks : op.taps.Cin;
+  const int hlC = Cout >= 64 ? 2 * Cout : 64;  // hi/lo plane of Cout channels
+  const int y16C = s.out16 == 2 ? hlC : Cout;
+  auto f16b = [&](int C, int L) { return align_up((size_t)B * C * f16_lp(L) * 2 + kPlaneSlack, 1024); };
+  const size_t b_x16 = f16b(xC, Lin), b_mid = c2 ? f16b(Cout, Lin) : 0, b_res = f16b(hlC, Lout),
+               b_r32 = align_up((size_t)B * Cout * Lout * 4, 1024), b_y16 = f16b(y16C, Lout);
+  const size_t need = b_x16 + b_mid + b_res + 2 * b_r32 + b_y16 + 1024;
+  if (workspace_bytes < need) return fail(MB_ERR_WORKSPACE, "tc_debug_launch: workspace %zu < %zu bytes", workspace_bytes, need);
+  char* ws = (char*)(((uintptr_t)workspace + 1023) & ~(uintptr_t)1023);
+  MB_CUDA_CHECK(cudaMemsetAsync(ws, 0, need - 1024, st));  // zero pad rows of every fp16 plane
+  char* p_mid = ws + b_x16;
+  char* p_res = p_mid + b_mid;
+  char* p_r32 = p_res + b_res;
+  char* p_y32 = p_r32 + b_r32;
+  char* p_y16 = p_y32 + b_r32;
+  TRef x16 = make_ref(ws, LAYOUT_F16B, xC, Lin);
+  x16.hilo = op.tc.x3;
+  cudaError_t e = launch_convert_layout(make_ref(const_cast<float*>(s.x), LAYOUT_NCL, op.taps.Cin, Lin), x16, B, op.taps.in_slope, st);
+  if (e != cudaSuccess) return fail(MB_ERR_CUDA, "convert: %s", cudaGetErrorString(e));
+  TRef res32, res16;
+  const TRef res_ncl = make_ref(const_cast<float*>(s.res), LAYOUT_NCL, Cout, Lout);
+  if (s.res_kind != 0 && !s.res) return fail(MB_ERR_INVALID, "tc_debug_launch: residual kind %d without residual", s.res_kind);
+  if (s.res_kind == 1) {
+    res32 = make_ref(p_r32, LAYOUT_F32B, Cout, Lout);
+    e = launch_convert_layout(res_ncl, res32, B, 1.f, st);
+  } else if (s.res_kind == 2 || s.res_kind == 3) {
+    res16 = make_ref(p_res, LAYOUT_F16B, s.res_kind == 3 ? hlC : Cout, Lout);
+    res16.hilo = s.res_kind == 3;
+    e = launch_convert_layout(res_ncl, res16, B, s.res_slope, st);
+  } else if (s.res_kind != 0) {
+    return fail(MB_ERR_INVALID, "tc_debug_launch: residual kind %d", s.res_kind);
+  }
+  if (e != cudaSuccess) return fail(MB_ERR_CUDA, "convert: %s", cudaGetErrorString(e));
+  const TRef y_ncl = make_ref(s.y, LAYOUT_NCL, Cout, Lout);
+  const TRef y32 = s.y ? make_ref(p_y32, LAYOUT_F32B, Cout, Lout) : TRef{};
+  if (s.y) {  // the running sum of the accumulate modes
+    e = launch_convert_layout(y_ncl, y32, B, 1.f, st);
+    if (e != cudaSuccess) return fail(MB_ERR_CUDA, "convert: %s", cudaGetErrorString(e));
+  }
+  TRef y16;
+  if (s.out16 == 1 || s.out16 == 2) {
+    if (!s.y16) return fail(MB_ERR_INVALID, "tc_debug_launch: fp16 output plane without destination");
+    y16 = make_ref(p_y16, LAYOUT_F16B, y16C, Lout);
+    y16.hilo = s.out16 == 2;
+  } else if (s.out16 != 0) {
+    return fail(MB_ERR_INVALID, "tc_debug_launch: fp16 output kind %d", s.out16);
+  }
+  int rc;
+  if (c2 && s.two_launches) {
+    // c1 -> activated fp16 intermediate plane (what tc_forward does for an unfused pair), then c2 reads it
+    const TRef mid = make_ref(p_mid, LAYOUT_F16B, Cout, Lin);
+    rc = launch_tc(op, tc_arena, x16, TRef{}, TRef{}, 1.f, TRef{}, mid, c2->taps.in_slope, s.lengths, B, Lin, st, s.red_add, 0,
+                   nullptr, nullptr, &info[0]);
+    if (rc != MB_OK) return rc;
+    rc = launch_tc(*c2, tc_arena, mid, res32, res16, s.res_slope, y32, y16, s.out_slope, s.lengths, B, Lin, st, s.red_add, 0,
+                   nullptr, nullptr, &info[1]);
+    *n_launches = 2;
+  } else {
+    rc = launch_tc(op, tc_arena, x16, res32, res16, s.res_slope, y32, y16, s.out_slope, s.lengths, B, Lin, st, s.red_add, 0,
+                   nullptr, c2, &info[0]);
+    *n_launches = 1;
+  }
+  if (rc != MB_OK) return rc;
+  if (s.y) {
+    e = launch_convert_layout(y32, y_ncl, B, 1.f, st);
+    if (e != cudaSuccess) return fail(MB_ERR_CUDA, "convert: %s", cudaGetErrorString(e));
+  }
+  if (y16.p) {
+    e = launch_convert_layout(y16, make_ref(s.y16, LAYOUT_NCL, y16C, Lout), B, 1.f, st);
+    if (e != cudaSuccess) return fail(MB_ERR_CUDA, "convert: %s", cudaGetErrorString(e));
+  }
   return MB_OK;
 }
 

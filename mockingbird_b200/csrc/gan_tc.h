@@ -70,4 +70,42 @@ bool tc_red_add_enabled();
 int tc_debug_layer(const TcOp& op, const char* tc_arena, const float* x, const float* residual, int B, int Lin,
                    float* y, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
+// which (c1, c2) op pairs tc_forward runs as ONE fused launch (tc_conv_kernel<..., PAIR = true>): fuse_next[i] = 1 for ops
+// (i, i + 1).  nbufs = number of plan buffers.
+std::vector<char> tc_fusion_plan(const std::vector<TcOp>& ops, int nbufs);
+
+// how tc_forward runs op i (host-only)
+struct TcOpPlan {
+  int use_tc, x3, split3;
+  int kc, n_cchunks, mt, rows_item, resident, wstages, omin, omax;  // the op launched on its own
+  int fuse_next, fused_prev;                                         // first / second op of a fused pair
+  int pair_mt, pair_rows_item, pair_resident, pair_wstages, pair_omin;  // fuse_next: the pair's launch
+  int kn, kmt, kcw, kpair;  // kernel instance <N, MT, CW, PAIR> this op launches (kn = 0: none of its own)
+};
+int tc_op_plan(const std::vector<TcOp>& ops, const std::vector<char>& fuse_next, int i, TcOpPlan* out);
+
+// what one tc_conv launch ran
+struct TcLaunchInfo {
+  int n, mt, cw, pair, rows_item, resident, wstages, n_work, grid, red_add;
+};
+
+// test hook: one tensor-core layer, or a resblock pair (c2 != nullptr) fused or as two launches, with the epilogue inputs and
+// outputs chosen by the caller.  The accumulate mode is op's (c2's) taps.mode / div.
+struct TcDebugSpec {
+  int B = 0, Lin = 0;
+  const float* x = nullptr;           // NCL [B][Cin][Lin] (not activated)
+  const float* res = nullptr;         // NCL [B][Cout][Lout]
+  int res_kind = 0;                   // 0 none, 1 fp32 plane, 2 activated fp16 plane, 3 hi/lo plane
+  float res_slope = 1.f;              // slope the fp16 residual planes are activated with
+  const int32_t* lengths = nullptr;   // device [B], in input rows
+  bool red_add = false;               // EPI_ADD by red.global.add where the epilogue allows it
+  float* y = nullptr;                 // NCL [B][Cout][Lout]: running sum in (accumulate modes), fp32 result out
+  int out16 = 0;                      // 0 none, 1 plain fp16 plane, 2 hi/lo plane
+  float out_slope = 1.f;
+  float* y16 = nullptr;               // NCL [B][C16][Lout]: the fp16 plane read back (hi channels, then lo channels)
+  bool two_launches = false;          // pair: c1 into an fp16 plane, then c2 (what an unfused pair does)
+};
+int tc_debug_launch(const TcOp& op, const TcOp* c2, const TcDebugSpec& spec, const char* tc_arena, void* workspace,
+                    size_t workspace_bytes, cudaStream_t stream, TcLaunchInfo* info /* [2] */, int* n_launches);
+
 }  // namespace mb

@@ -289,6 +289,63 @@ class GanGenerator:
                                                  C.c_void_p(stream)))
         return y
 
+    def tc_plan_info(self, i: int) -> Dict[str, object]:
+        """how the tensor-core forward runs op i (mb_gan_tc_plan_info): {"name": ..., key: int, "kernel": (N, MT, CW, PAIR)}"""
+        buf = C.create_string_buffer(512)
+        _lib.check(_lib.lib().mb_gan_tc_plan_info(self._handle, i, buf, 512))
+        return _parse_report(buf.value.decode())
+
+    EPI_MODES = {"store": 0, "add": 1, "add_div": 2}
+    RES_KINDS = {None: 0, "f32": 1, "f16": 2, "hilo": 3}
+    OUT16_KINDS = {None: 0, "f16": 1, "hilo": 2}
+
+    def debug_launch(self, i: int, x: torch.Tensor, *, pair: int = 0, mode: str = "store", div: float = 1.0,
+                     red_add: bool = False, y_init: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None,
+                     res_kind: Optional[str] = None, res_slope: float = 1.0, out16: Optional[str] = None,
+                     out_slope: float = 1.0, lengths: Optional[torch.Tensor] = None):
+        """one tensor-core launch of layer i, or of the fused pair (i, i + 1) (pair=1) or that pair as two launches (pair=2),
+        through mb_gan_debug_launch.  x [B, Cin, L] (not activated), residual [B, Cout, L*stride], y_init the running sum of the
+        accumulate modes, lengths int32 [B] in input rows.  Returns (y, y16_hi, y16_lo, launches): fp32 NCL tensors (the fp16
+        ones None when not requested) and one dict per kernel launch ({"kernel": (N, MT, CW, PAIR), "rows_item": ...})."""
+        if not self._ready:
+            self._upload()
+        x = x.contiguous().float()
+        B, cin, L = x.shape
+        last = self.layer_info(i + (1 if pair else 0))
+        cout = int(last.split("cout=")[1].split()[0])
+        stride = int(last.split("stride=")[1].split()[0]) if not pair else 1
+        Lout = L * stride
+        dev = x.device
+        y = (y_init.contiguous().float().clone() if y_init is not None
+             else torch.zeros(B, cout, Lout, dtype=torch.float32, device=dev))
+        c16 = (max(2 * cout, 64) if out16 == "hilo" else cout)
+        y16 = torch.zeros(B, c16, Lout, dtype=torch.float32, device=dev) if out16 else None
+        res = residual.contiguous().float() if residual is not None else None
+        lens = lengths.to(device=dev, dtype=torch.int32).contiguous() if lengths is not None else None
+        spec = _lib.GanDebugSpec()
+        spec.layer_index, spec.pair, spec.mode, spec.div = i, pair, self.EPI_MODES[mode], div
+        spec.red_add = int(red_add)
+        spec.res_kind, spec.res_slope = self.RES_KINDS[res_kind], res_slope
+        spec.out16, spec.out_slope = self.OUT16_KINDS[out16], out_slope
+        spec.batch, spec.frames_in = B, L
+        spec.x = x.data_ptr()
+        spec.residual = res.data_ptr() if res is not None else None
+        spec.lengths = lens.data_ptr() if lens is not None else None
+        spec.y = y.data_ptr()
+        spec.y16 = y16.data_ptr() if y16 is not None else None
+        plane = B * 2 * max(cin, cout, 64) * (max(L, Lout) + 88) * 4 + (128 << 10) + 2048  # >= any plane of the launch
+        ws = torch.empty(6 * plane + (1 << 20), dtype=torch.uint8, device=dev)
+        report = C.create_string_buffer(1024)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        _lib.check(_lib.lib().mb_gan_debug_launch(self._handle, C.byref(spec), C.c_void_p(ws.data_ptr()), ws.numel(),
+                                                  C.c_void_p(stream), report, 1024))
+        launches = [_parse_report(line) for line in report.value.decode().splitlines() if line]
+        hi = lo = None
+        if y16 is not None:
+            hi = y16[:, :cout]
+            lo = y16[:, c16 // 2:c16 // 2 + cout] if out16 == "hilo" else None
+        return y, hi, lo, launches
+
     def __del__(self):
         try:
             if getattr(self, "_handle", None) is not None and self._handle.value:
@@ -296,6 +353,18 @@ class GanGenerator:
                 self._handle = C.c_void_p()
         except Exception:
             pass
+
+
+def _parse_report(text: str) -> Dict[str, object]:
+    """"[name] key=int ... kernel=N,MT,CW,PAIR" -> dict"""
+    out: Dict[str, object] = {}
+    for tok in text.split():
+        if "=" not in tok:
+            out["name"] = tok
+            continue
+        k, v = tok.split("=", 1)
+        out[k] = tuple(int(p) for p in v.split(",")) if "," in v else int(v)
+    return out
 
 
 _pinned: Dict[str, torch.Tensor] = {}
