@@ -429,6 +429,58 @@ int32_t mb_melspec_num_frames(const mb_melspec* h, int32_t n_samples);   /* 1 + 
 /* wav fp32 [n_samples] (device) -> out fp32 [frames][n_mels] or [n_mels][frames] (device) */
 int mb_melspec_forward(mb_melspec* h, const float* wav, int32_t n_samples, float* out, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Voice-conversion mel decoder (ppg2mel)
+ *   replaces  models/ppg2mel/__init__.py:166-192 (MelDecoderMOLv2.inference: PPG / pitch encoder, reduce_proj with the
+ *             normalised speaker embedding), models/ppg2mel/rnn_decoder_mol.py:267-315 (Decoder.inference: PreNet with
+ *             dropout always on, attention LSTMCell, MoL attention, decoder LSTMCell, projection + stop layer) and
+ *             models/ppg2mel/utils/cnn_postnet.py (Postnet, eval BatchNorm)
+ * ------------------------------------------------------------------------------------------- */
+typedef struct mb_ppg2mel_config {
+  int32_t bottle_neck_feature_dim;     /* 144 PPG dim (any 1..1024) */
+  int32_t spk_embed_dim;               /* 256 (any 1..1024) */
+  int32_t encoder_dim;                 /* 256 */
+  int32_t encoder_downsample_rates[2]; /* 2, 2 */
+  int32_t attention_rnn_dim;           /* 512 */
+  int32_t decoder_rnn_dim;             /* 512 */
+  int32_t num_decoder_rnn_layer;       /* 1 */
+  int32_t concat_context_to_last;      /* 1 */
+  int32_t prenet_dims[2];              /* 256, 128 */
+  int32_t num_mixtures;                /* 5 */
+  int32_t frames_per_step;             /* 2 */
+  int32_t num_mels;                    /* 80 */
+} mb_ppg2mel_config;
+
+typedef struct mb_ppg2mel mb_ppg2mel;
+
+/* every field but the two input dims must hold the value shown (the kernels specialise on them): MB_ERR_INVALID else */
+int mb_ppg2mel_create(const mb_ppg2mel_config* cfg, mb_ppg2mel** out);
+void mb_ppg2mel_destroy(mb_ppg2mel* h);
+size_t mb_ppg2mel_arena_bytes(const mb_ppg2mel* h);
+int mb_ppg2mel_set_arena(mb_ppg2mel* h, void* arena, size_t bytes);
+/* tensors of ckpt['model'] under their reference names (decoder.prenet_pitch.* is accepted and ignored; the postnet's
+ * num_batches_tracked is ignored); finalize repacks them and folds the postnet BatchNorm into its convolutions */
+int mb_ppg2mel_set_weight(mb_ppg2mel* h, const char* name, const float* w, const int64_t* dims, int32_t ndim,
+                          void* stream);
+int mb_ppg2mel_finalize(mb_ppg2mel* h, void* stream);
+size_t mb_ppg2mel_workspace_bytes(const mb_ppg2mel* h, int32_t batch, int32_t frames);
+
+/* MelDecoderMOLv2.inference for a padded batch of 1..128 rows, each row computed as its own B = 1 call:
+ *   ppg fp32 [B][frames][bottle_neck_feature_dim], lf0_uv fp32 [B][frames][2], spk fp32 [B][spk_embed_dim] (device)
+ *   lengths int32 [B] (host): valid PPG frames of each row, 4 <= lengths[b] <= frames; T_enc[b] = lengths[b] / 4
+ *   mask1 uint8 [S][B][256], mask2 uint8 [S][B][128] (device): PreNet keep flags of decoder step s, S = 2 * (frames / 4);
+ *     both NULL -> drawn on the device from `seed` (Philox, keyed by step, row and unit)
+ *   outputs (device, zero-filled past each row's end): mel / mel_post fp32 [B][2 S][80], align fp32 [B][S][frames / 4],
+ *     stop fp32 [B][S] (stop logits, may be NULL); steps_host int32 [B] (host): decoder steps n of each row (2 n mel
+ *     frames, n alignment rows).
+ * Row b stops after step n when sigmoid(stop) > 0.5 and n >= 2 T_enc[b] - 5, or when n = 2 T_enc[b]; a finished row
+ * is frozen while the others run on.  The decoder steps are replayed from a CUDA graph of 16 steps on an internal
+ * stream ordered after `stream` (events); the host polls the finished rows once per graph replay. */
+int mb_ppg2mel_inference(mb_ppg2mel* h, const float* ppg, const float* lf0_uv, const float* spk, const int32_t* lengths,
+                         int32_t batch, int32_t frames, const uint8_t* mask1, const uint8_t* mask2, uint64_t seed,
+                         float* mel, float* mel_post, float* align, float* stop, int32_t* steps_host, void* workspace,
+                         size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

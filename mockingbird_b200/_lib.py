@@ -89,6 +89,14 @@ class EncoderConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("mel_n_channels", "hidden_size", "num_layers", "embedding_size")]
 
 
+class Ppg2MelConfig(C.Structure):
+    _fields_ = [("bottle_neck_feature_dim", C.c_int32), ("spk_embed_dim", C.c_int32), ("encoder_dim", C.c_int32),
+                ("encoder_downsample_rates", C.c_int32 * 2), ("attention_rnn_dim", C.c_int32),
+                ("decoder_rnn_dim", C.c_int32), ("num_decoder_rnn_layer", C.c_int32), ("concat_context_to_last", C.c_int32),
+                ("prenet_dims", C.c_int32 * 2), ("num_mixtures", C.c_int32), ("frames_per_step", C.c_int32),
+                ("num_mels", C.c_int32)]
+
+
 class MelSpecConfig(C.Structure):
     _fields_ = [("sample_rate", C.c_int32), ("n_fft", C.c_int32), ("hop_length", C.c_int32), ("win_length", C.c_int32),
                 ("n_mels", C.c_int32), ("fmin", C.c_float), ("fmax", C.c_float), ("pad_mode", C.c_int32),
@@ -190,6 +198,16 @@ SIGNATURES = {
     "mb_melspec_set_arena": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_melspec_num_frames": (C.c_int32, [C.c_void_p, C.c_int32]),
     "mb_melspec_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "mb_ppg2mel_create": (C.c_int, [C.POINTER(Ppg2MelConfig), C.POINTER(C.c_void_p)]),
+    "mb_ppg2mel_destroy": (None, [C.c_void_p]),
+    "mb_ppg2mel_arena_bytes": (C.c_size_t, [C.c_void_p]),
+    "mb_ppg2mel_set_arena": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "mb_ppg2mel_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int32, C.c_void_p]),
+    "mb_ppg2mel_finalize": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "mb_ppg2mel_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.c_int32]),
+    "mb_ppg2mel_inference": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32,
+                                       C.c_int32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 _lib: Optional[C.CDLL] = None

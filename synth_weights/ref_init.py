@@ -394,3 +394,70 @@ def deepmind_state_dict(seed: int = 0, bias_scale: float = 0.1) -> Dict[str, tor
         for b in ("bias_u", "bias_r", "bias_e"):
             sd[b] = torch.randn(H) * bias_scale
     return sd
+
+
+# ---- ppg2mel MelDecoderMOLv2 (models/ppg2mel/__init__.py:20-118, rnn_decoder_mol.py:24-107) ----------------------
+PPG2MEL_CONFIG = dict(num_speakers=1, spk_embed_dim=256, bottle_neck_feature_dim=144, encoder_dim=256,
+                      encoder_downsample_rates=[2, 2], attention_rnn_dim=512, decoder_rnn_dim=512, num_decoder_rnn_layer=1,
+                      concat_context_to_last=True, prenet_dims=[256, 128], num_mixtures=5, frames_per_step=2,
+                      mask_padding=True)
+
+
+def ppg2mel_state_dict(seed: int = 0, randomize_bn: bool = True) -> Dict[str, torch.Tensor]:
+    """``torch.manual_seed(seed); MelDecoderMOLv2(**PPG2MEL_CONFIG)`` state_dict rebuilt from stock torch layers in the
+    constructor's order.  The reference's ``Linear`` / ``Conv1d`` wrappers (utils/basic_layers.py:27-56) build the
+    torch layer (default init) and then redraw the weight with xavier_uniform_; MOLAttention.initialize_bias
+    (utils/mol_attention.py:41-54) overwrites the sigma / Delta biases with constants (r = 2/4 < 1: Delta = -0.432).
+    ``randomize_bn`` replaces the postnet BatchNorm statistics and affines (identity in a fresh module) by seeded draws."""
+    nn = torch.nn
+    gain = nn.init.calculate_gain
+    torch.manual_seed(seed)
+    sd: Dict[str, torch.Tensor] = {}
+
+    def put(name, m):
+        for n, p in m.state_dict().items():
+            sd[f"{name}.{n}"] = p.detach().clone()
+
+    for branch, cin in (("bnf_prenet", 144), ("pitch_convs", 2)):
+        put(f"{branch}.0", nn.Conv1d(cin, 256, 1, bias=False))
+        put(f"{branch}.3", nn.Conv1d(256, 256, 4, 2, 1))
+        put(f"{branch}.6", nn.Conv1d(256, 256, 4, 2, 1))
+    put("reduce_proj", nn.Linear(512, 256))
+
+    def xlinear(name, i, o, bias=True, g="linear"):
+        m = nn.Linear(i, o, bias=bias)
+        nn.init.xavier_uniform_(m.weight, gain=gain(g))
+        put(name + ".linear_layer", m)
+
+    for pre in ("prenet", "prenet_pitch"):
+        xlinear(f"decoder.{pre}.layers.0", 80, 256, bias=False)
+        xlinear(f"decoder.{pre}.layers.1", 256, 128, bias=False)
+    put("decoder.attention_rnn", nn.LSTMCell(384, 512))
+    q0, q2 = nn.Linear(512, 256), nn.Linear(256, 15)
+    with torch.no_grad():
+        q2.bias[5:10] = 1.0
+        q2.bias[10:15] = -0.432
+    put("decoder.attention_layer.query_layer.0", q0)
+    put("decoder.attention_layer.query_layer.2", q2)
+    put("decoder.decoder_rnn_layers.0", nn.LSTMCell(768, 512))
+    xlinear("decoder.linear_projection", 768, 160)
+    xlinear("decoder.stop_layer", 768, 1, g="sigmoid")
+    chans = [80, 512, 512, 512, 512, 80]
+    for i in range(5):
+        c = nn.Conv1d(chans[i], chans[i + 1], 5, 1, 2)
+        nn.init.xavier_uniform_(c.weight, gain=gain("tanh" if i < 4 else "linear"))
+        put(f"postnet.convolutions.{i}.0.conv", c)
+        put(f"postnet.convolutions.{i}.1", nn.BatchNorm1d(chans[i + 1]))
+    if randomize_bn:
+        g2 = torch.Generator().manual_seed(30_000 + seed)
+        for k in sorted(sd):
+            if k.startswith("postnet.") and ".1." in k:
+                if k.endswith(".running_var"):
+                    sd[k] = torch.rand(sd[k].shape, generator=g2) * 1.5 + 0.25
+                elif k.endswith(".running_mean"):
+                    sd[k] = torch.randn(sd[k].shape, generator=g2) * 0.3
+                elif k.endswith(".weight"):
+                    sd[k] = torch.rand(sd[k].shape, generator=g2) + 0.5
+                elif k.endswith(".bias"):
+                    sd[k] = torch.randn(sd[k].shape, generator=g2) * 0.2
+    return sd
