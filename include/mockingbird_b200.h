@@ -58,6 +58,10 @@ uint64_t mb_launch_count(void);
  * ------------------------------------------------------------------------------------------- */
 #define MB_GAN_HIFIGAN 0
 #define MB_GAN_FREGAN 1
+/* HiFi-GAN as the reference builds it for h.sampling_rate == 24000 (models.py:107-118): each upsampling layer is
+ * InterpolationBlock(u) (nearest) + Conv1d(k, padding=(k-1)//2), checkpoint keys "ups.{i}.1.*"; k must be odd.  Lowered
+ * to a polyphase tap conv with folded weights (DESIGN.md 3.6); same mb_gan_config fields as MB_GAN_HIFIGAN. */
+#define MB_GAN_HIFIGAN_INTERP 2
 
 /* arithmetic of the channel-mixing convolutions */
 #define MB_PREC_FP32 0      /* FP32 FFMA everywhere (parity anchor, ~1e-6 of the reference)     */
@@ -68,7 +72,7 @@ uint64_t mb_launch_count(void);
                                (~1e-5 of the reference) at 3x the MMA work of MB_PREC_F16TC            */
 
 typedef struct mb_gan_config {
-  int32_t kind;                 /* MB_GAN_HIFIGAN | MB_GAN_FREGAN                                  */
+  int32_t kind;                 /* MB_GAN_HIFIGAN | MB_GAN_FREGAN | MB_GAN_HIFIGAN_INTERP          */
   int32_t num_mels;             /* 80 (models.py:99 hard-codes 80)                                 */
   int32_t upsample_initial_channel;
   int32_t num_upsamples;        /* len(h.upsample_rates) <= 8                                      */

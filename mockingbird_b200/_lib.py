@@ -14,6 +14,7 @@ from . import build as _build
 MB_OK = 0
 MB_GAN_HIFIGAN = 0
 MB_GAN_FREGAN = 1
+MB_GAN_HIFIGAN_INTERP = 2  # 24 kHz HiFi-GAN: nearest upsample + Conv1d per stage (hifigan/models.py:107-118)
 MB_PREC_FP32 = 0
 MB_PREC_F16TC = 1
 MB_PREC_F16X3 = 2

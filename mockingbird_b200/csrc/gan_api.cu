@@ -1,6 +1,7 @@
 // GAN generator plan + C ABI (mb_gan_*): HiFi-GAN Generator.forward (hifigan/models.py:134-150) and
 // FreGAN.forward (fregan/generator.py:137-166) lowered to a list of tap-conv ops over a handful of
 // workspace buffers.  See include/mockingbird_b200.h for the contract.
+#include <algorithm>
 #include <cstdlib>
 #include <cstring>
 #include <string>
@@ -26,7 +27,7 @@ struct Layer {
   int cin = 0, cout = 0, k = 1, dil = 1, stride = 1;
   int cin_w = 0, cout_w = 0;  // channel counts of the checkpoint tensors (cin / cout may be zero-padded, see pad_channels)
   bool transposed = false;
-  int nearest = 1;  // nearest-neighbour upsample factor in front of a 1x1 conv (Fre-GAN res_output)
+  int nearest = 1;  // nearest-neighbour upsample factor in front of an odd-k conv (Fre-GAN res_output: k = 1; 24 kHz ups.*.1)
   float in_slope = 1.f;
   int src = BUF_NONE, dst = BUF_NONE, res = BUF_NONE, dst2 = BUF_NONE;
   int mode = EPI_STORE;
@@ -37,7 +38,26 @@ struct Layer {
   bool w_set = false, b_set = false;
   TapConv taps{};                 // static part (B, Lin, Lout, lengths filled per call)
   TcLayer tc{};                   // tensor-core packing info (MB_PREC_F16TC)
+  FoldTable fold{};               // nearest > 1: kernel taps summed into each slab
 };
+
+int floor_div(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
+
+// nearest-upsample by u + Conv1d(k, padding=(k-1)/2): output phase r reads input rows q + d, d = floor((r + j - p) / u) for
+// kernel tap j, p = (k-1)/2.  First and last d of phase r:
+void fold_range(int u, int k, int r, int* dlo, int* dhi) {
+  const int p = (k - 1) / 2;
+  *dlo = floor_div(r - p, u);
+  *dhi = floor_div(r + k - 1 - p, u);
+}
+
+// weight slabs a layer's taps refer to
+int slab_count(const TapConv& t) {
+  int n = 0;
+  for (int r = 0; r < t.stride; ++r)
+    for (int i = 0; i < t.ntaps[r]; ++i) n = std::max(n, t.slab[r][i] + 1);
+  return n;
+}
 
 void build_taps(Layer& L) {
   TapConv& t = L.taps;
@@ -67,12 +87,31 @@ void build_taps(Layer& L) {
       t.ntaps[r] = n;
     }
   } else if (L.nearest > 1) {
-    // nn.Upsample(scale_factor=u, 'nearest') + 1x1 conv: out[q*u + r] = W x[q]
-    t.stride = L.nearest;
-    for (int r = 0; r < L.nearest; ++r) {
-      t.ntaps[r] = 1;
-      t.off[r][0] = 0;
-      t.slab[r][0] = 0;
+    // nearest upsample by u + Conv1d(k, padding=p=(k-1)/2), k odd (24 kHz InterpolationBlock, hifigan/models.py:107-118; Fre-GAN
+    // res_output: k = 1):  y[q*u + r] = sum_j W_j x[q + floor((r + j - p)/u)] = sum_d V[r][d] x[q + d], where V[r][d] sums the
+    // consecutive taps j = jlo .. jhi with floor((r + j - p)/u) == d.  Slabs are numbered in (r, ascending d) order; a run (jlo, jhi)
+    // that an earlier phase already has reuses its slab (k = 1: every phase reads slab 0 at offset 0)
+    const int u = L.nearest, k = L.k, p = (k - 1) / 2;
+    t.stride = u;
+    L.fold.nslabs = 0;
+    for (int r = 0; r < u; ++r) {
+      int dlo, dhi;
+      fold_range(u, k, r, &dlo, &dhi);
+      int n = 0;
+      for (int d = dlo; d <= dhi; ++d) {
+        const int jlo = std::max(0, d * u - r + p), jhi = std::min(k - 1, d * u + u - 1 - r + p);
+        int s = 0;
+        while (s < L.fold.nslabs && !(L.fold.jlo[s] == jlo && L.fold.jhi[s] == jhi)) ++s;
+        if (s == L.fold.nslabs) {
+          L.fold.jlo[s] = jlo;
+          L.fold.jhi[s] = jhi;
+          ++L.fold.nslabs;
+        }
+        t.off[r][n] = d;
+        t.slab[r][n] = s;
+        ++n;
+      }
+      t.ntaps[r] = n;
     }
   } else {
     // Conv1d(k, dilation=d, padding=get_padding(k,d)=(k*d-d)/2) (utils/util.py:60-61)
@@ -224,9 +263,28 @@ int build_plan(mb_gan* h) {
       if ((c.resblock_kernel_sizes[j] - 1) * c.resblock_dilation_sizes[j][m] > 96)
         return fail(MB_ERR_INVALID, "mb_gan_create: receptive field of resblock kernel %d dilation %d too wide",
                     c.resblock_kernel_sizes[j], c.resblock_dilation_sizes[j][m]);
+  const bool interp = c.kind == MB_GAN_HIFIGAN_INTERP;
   for (int i = 0; i < c.num_upsamples; ++i) {
     const int u = c.upsample_rates[i], k = c.upsample_kernel_sizes[i];
     if (u < 1 || u > kMaxPhases) return fail(MB_ERR_INVALID, "mb_gan_create: upsample rate %d unsupported", u);
+    if (interp) {
+      // nearest upsample by u + Conv1d(k, padding=(k-1)/2) (hifigan/models.py:107-118), folded into u phases
+      if (k < 1 || k % 2 == 0)
+        return fail(MB_ERR_INVALID,
+                    "mb_gan_create: interpolation upsample kernel size %d unsupported: with an even k, Conv1d(k, padding=(k-1)//2) "
+                    "emits u*L-1 samples per stage, so no hop describes the output",
+                    k);
+      for (int r = 0; r < u; ++r) {
+        int dlo, dhi;
+        fold_range(u, k, r, &dlo, &dhi);
+        if (dhi - dlo + 1 > kMaxTaps)
+          return fail(MB_ERR_INVALID, "mb_gan_create: interpolation upsample (k=%d,u=%d) folds to %d taps per phase (max %d)", k, u,
+                      dhi - dlo + 1, kMaxTaps);
+        if (-dlo > kPadRows || dhi > kPadRows)
+          return fail(MB_ERR_INVALID, "mb_gan_create: interpolation upsample (k=%d,u=%d) reads rows beyond +-%d", k, u, kPadRows);
+      }
+      continue;
+    }
     // output length (L-1)u - 2p + k + op must equal u*L
     if (k - 2 * (u / 2 + u % 2) + (u % 2) != u)
       return fail(MB_ERR_INVALID, "mb_gan_create: upsample (k=%d,u=%d) does not produce u*L samples", k, u);
@@ -234,14 +292,18 @@ int build_plan(mb_gan* h) {
   const int T = new_buf(h), X = new_buf(h), R = new_buf(h), S = new_buf(h);
   const int C0 = c.upsample_initial_channel;
   int rate = 1;
-  if (c.kind == MB_GAN_HIFIGAN) {
+  if (c.kind == MB_GAN_HIFIGAN || interp) {
     add_conv(h, "conv_pre", c.num_mels, C0, 7, 1, 1, false, 1, 1.f, BUF_IN, T, BUF_NONE, 1);
     int cur = T;
     int ch = C0;
     for (int i = 0; i < c.num_upsamples; ++i) {
       const int u = c.upsample_rates[i];
-      add_conv(h, "ups." + std::to_string(i), ch, ch / 2, c.upsample_kernel_sizes[i], 1, u, true, 1, 0.1f, cur, X,
-               BUF_NONE, rate);
+      if (interp)  // ups[i] = Sequential(InterpolationBlock(u), Conv1d): the conv's checkpoint keys are "ups.{i}.1.*"
+        add_conv(h, "ups." + std::to_string(i) + ".1", ch, ch / 2, c.upsample_kernel_sizes[i], 1, 1, false, u, 0.1f, cur, X,
+                 BUF_NONE, rate);
+      else
+        add_conv(h, "ups." + std::to_string(i), ch, ch / 2, c.upsample_kernel_sizes[i], 1, u, true, 1, 0.1f, cur, X,
+                 BUF_NONE, rate);
       ch /= 2;
       rate *= u;
       add_mrf(h, i, ch, rate, X, R, T, S);
@@ -329,7 +391,7 @@ int build_plan(mb_gan* h) {
     if (L.kind != OP_CONV) continue;
     build_taps(L);
     L.w_off = off;
-    off += (size_t)L.k * L.cin * L.cout;
+    off += (size_t)slab_count(L.taps) * L.cin * L.cout;
     off = align_up(off, 64);
     L.b_off = off;
     off += (size_t)L.cout;
@@ -443,15 +505,18 @@ int mb_gan_create(const mb_gan_config* cfg, mb_gan** out) {
       // Fre-GAN res_output: the first one reads S, which `ups` reads through leaky-relu (one fp16 plane cannot serve both): FP32
       // kernel.  The later ones read the running `output` buffer, which nothing else consumes: they run on the tensor cores with
       // the 3-term split over an un-activated hi/lo plane written by the preceding "output += x" op (MB_GAN_NEAREST_TC=0: FP32).
-      const bool nearest_f32 = L.nearest > 1 && (L.name.rfind("res_output.0.", 0) == 0 || !env_flag("MB_GAN_NEAREST_TC", true));
+      // (the 24 kHz HiFi-GAN's folded upsampling layers "ups.{i}.1" read the same leaky-relu plane as a transposed `ups` would)
+      const bool res_output = L.name.rfind("res_output.", 0) == 0;
+      const bool nearest_f32 = res_output && (L.name.rfind("res_output.0.", 0) == 0 || !env_flag("MB_GAN_NEAREST_TC", true));
       d.force_f32 = (L.dst2 != BUF_NONE) || nearest_f32;
       // 3-term split (FP32-equivalent operands): every layer in MB_PREC_F16X3; in MB_PREC_F16TC the serial layers nothing
-      // downstream averages out - the transposed convs `ups.*` / `cond_up.*` (DESIGN.md 3.4; MB_TC_UPS_X3=0 disables)
+      // downstream averages out - the upsampling layers `ups.*` (transposed or folded interpolation) / `cond_up.*` (DESIGN.md 3.4;
+      // MB_TC_UPS_X3=0 disables)
       d.want_x3 = cfg->precision == MB_PREC_F16X3 ||
                   (env_flag("MB_TC_UPS_X3", true) &&
-                   (L.name.rfind("ups.", 0) == 0 || L.name.rfind("cond_up.", 0) == 0 || L.name.rfind("res_output.", 0) == 0));
+                   (L.name.rfind("ups.", 0) == 0 || L.name.rfind("cond_up.", 0) == 0 || res_output));
       d.taps = &L.taps;
-      d.k = L.k;
+      d.k = slab_count(L.taps);  // weight slabs (the checkpoint's k, except for folded nearest-upsample layers)
       d.tc = &L.tc;
       descs.push_back(d);
     }
@@ -505,7 +570,9 @@ int mb_gan_set_weight(mb_gan* h, const char* name, const float* w, const int64_t
       if (ndim != 3 || dims[0] != d0 || dims[1] != d1 || dims[2] != L.k)
         return fail(MB_ERR_INVALID, "mb_gan_set_weight: %s expects [%lld,%lld,%d]", name, (long long)d0,
                     (long long)d1, L.k);
-      cudaError_t e = launch_pack_slabs_f32(w, h->arena + L.w_off, L.cout_w, L.cin_w, L.k, L.transposed, st, L.cout, L.cin);
+      cudaError_t e = L.nearest > 1
+                          ? launch_fold_slabs_f32(w, h->arena + L.w_off, L.cout_w, L.cin_w, L.k, L.fold, L.cout, L.cin, st)
+                          : launch_pack_slabs_f32(w, h->arena + L.w_off, L.cout_w, L.cin_w, L.k, L.transposed, st, L.cout, L.cin);
       if (e != cudaSuccess) return fail(MB_ERR_CUDA, "pack_slabs: %s", cudaGetErrorString(e));
       count_launch();
       if (h->cfg.precision != MB_PREC_FP32) {
@@ -607,8 +674,14 @@ int mb_gan_layer_work(const mb_gan* h, int32_t i, int32_t batch, int32_t frames,
   const Layer& L = h->layers[i];
   const double rows_in = (double)batch * frames * L.rate_in, rows_out = (double)batch * frames * L.rate_out;
   if (L.kind == OP_CONV) {
-    // every output row receives k/stride taps of Cin x Cout (transposed), or k taps (conv)
-    const double taps = L.transposed ? (double)L.k / L.stride : (double)L.k;
+    // every output row receives k/stride taps of Cin x Cout (transposed), the folded taps of its phase (nearest upsample + conv:
+    // on average sum_r ntaps[r] / u), or k taps (conv)
+    double taps = L.transposed ? (double)L.k / L.stride : (double)L.k;
+    if (L.nearest > 1) {
+      int n = 0;
+      for (int r = 0; r < L.taps.stride; ++r) n += L.taps.ntaps[r];
+      taps = (double)n / L.nearest;
+    }
     if (macs) *macs = rows_out * taps * L.cin_w * L.cout_w;  // algorithmic work: the checkpoint's channel counts
     if (bytes) *bytes = 4.0 * (rows_in * L.cin_w + rows_out * L.cout_w);
   } else {

@@ -335,6 +335,24 @@ __global__ void pack_slabs_kernel(const float* __restrict__ w, float* __restrict
   dst[((size_t)k * Cin_p + ci) * Cout_p + co] = w[src];
 }
 
+// one thread per element of the padded destination [nslabs][Cin_p][Cout_p]
+__global__ void fold_slabs_kernel(const float* __restrict__ w, float* __restrict__ dst, int Cout, int Cin, int K,
+                                  FoldTable fold, int Cout_p, int Cin_p) {
+  const size_t n = (size_t)fold.nslabs * Cin_p * Cout_p;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int co = (int)(i % Cout_p);
+  const int ci = (int)((i / Cout_p) % Cin_p);
+  const int s = (int)(i / ((size_t)Cout_p * Cin_p));
+  float v = 0.f;
+  if (co < Cout && ci < Cin) {
+    const float* row = w + ((size_t)co * Cin + ci) * K;
+    v = row[fold.jlo[s]];
+    for (int j = fold.jlo[s] + 1; j <= fold.jhi[s]; ++j) v += row[j];
+  }
+  dst[i] = v;
+}
+
 }  // namespace
 
 cudaError_t launch_tapconv_f32(const TapConv& p, const TapConvIO& io, const float* w, const float* bias,
@@ -423,6 +441,16 @@ cudaError_t launch_pack_slabs_f32(const float* w, float* dst, int Cout, int Cin,
     if (e != cudaSuccess) return e;
   }
   pack_slabs_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(w, dst, Cout, Cin, K, transposed ? 1 : 0, Cout_p, Cin_p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_fold_slabs_f32(const float* w, float* dst, int Cout, int Cin, int K, const FoldTable& fold, int Cout_p,
+                                  int Cin_p, cudaStream_t stream) {
+  if (Cout_p < Cout) Cout_p = Cout;
+  if (Cin_p < Cin) Cin_p = Cin;
+  const size_t n = (size_t)fold.nslabs * Cin_p * Cout_p;
+  if (n == 0) return cudaSuccess;
+  fold_slabs_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(w, dst, Cout, Cin, K, fold, Cout_p, Cin_p);
   return cudaGetLastError();
 }
 

@@ -112,4 +112,17 @@ cudaError_t launch_convert_layout(const TRef& src, const TRef& dst, int B, float
 cudaError_t launch_pack_slabs_f32(const float* w, float* dst, int Cout, int Cin, int K, bool transposed,
                                   cudaStream_t stream, int Cout_p = 0, int Cin_p = 0);
 
+// Nearest-neighbour upsample by u followed by Conv1d(k, padding=(k-1)/2), folded into a polyphase tap conv: slab s of the
+// layer is the sum of the kernel taps W_j, j = jlo[s] .. jhi[s] (one run of consecutive j that all read the same input row).
+constexpr int kMaxSlabs = kMaxPhases * kMaxTaps;
+struct FoldTable {
+  int nslabs;
+  int jlo[kMaxSlabs], jhi[kMaxSlabs];
+};
+
+// weight fold + repack: Conv1d weight [Cout][Cin][K] -> slabs [nslabs][Cin_p][Cout_p], slab s = sum_{j = jlo[s]}^{jhi[s]} w[:, :, j]
+// accumulated in fp32 in ascending j; every element of dst is written (padded channels = 0)
+cudaError_t launch_fold_slabs_f32(const float* w, float* dst, int Cout, int Cin, int K, const FoldTable& fold, int Cout_p,
+                                  int Cin_p, cudaStream_t stream);
+
 }  // namespace mb

@@ -47,15 +47,16 @@ class GanGenerator:
 
     def __init__(self, h, precision: str = "auto", top_k: int = 4):
         self.h = h
-        if _cfg_get(h, "sampling_rate", 16000) == 24000 and self.KIND == _lib.MB_GAN_HIFIGAN:
-            raise NotImplementedError("the 24 kHz InterpolationBlock variant (hifigan/models.py:105-117) "
-                                      "is not part of the H100 path")
+        # the reference's own rule (hifigan/models.py:107): at 24 kHz every upsampling layer is nearest upsample + Conv1d
+        self.kind = self.KIND
+        if self.KIND == _lib.MB_GAN_HIFIGAN and _cfg_get(h, "sampling_rate", 16000) == 24000:
+            self.kind = _lib.MB_GAN_HIFIGAN_INTERP
         rates = list(_cfg_get(h, "upsample_rates"))
         kernels = list(_cfg_get(h, "upsample_kernel_sizes"))
         rks = list(_cfg_get(h, "resblock_kernel_sizes"))
         rds = [list(d) for d in _cfg_get(h, "resblock_dilation_sizes")]
         cfg = _lib.GanConfig()
-        cfg.kind = self.KIND
+        cfg.kind = self.kind
         cfg.num_mels = 80  # hifigan/models.py:99 hard-codes 80 input channels
         cfg.upsample_initial_channel = int(_cfg_get(h, "upsample_initial_channel"))
         cfg.num_upsamples = len(rates)

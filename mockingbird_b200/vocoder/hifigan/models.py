@@ -22,7 +22,10 @@ DEFAULT_CONFIG_16K = {
 
 
 class Generator(GanGenerator):
-    """``Generator(h)``; ``forward(mel[B,80,T]) -> wav[B,1,200*T]`` (models.py:134-150).
+    """``Generator(h)``; ``forward(mel[B,80,T]) -> wav[B,1,hop*T]`` (models.py:134-150), hop = prod(h.upsample_rates).
+
+    Like the reference (models.py:107-123), ``h.sampling_rate == 24000`` selects nearest-upsample + Conv1d upsampling layers
+    (checkpoint keys ``ups.{i}.1.*``, odd kernel sizes only), every other rate ConvTranspose1d layers.
 
     ``precision``: "auto" (default; picks "f16tc" when a load-time probe shows it within 5e-4 of "f16x3" for this
     checkpoint, else "f16x3"), "f16tc" (wgmma, fp16 operands / fp32 accumulate, 3-term split on the serial layers),

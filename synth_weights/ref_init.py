@@ -70,16 +70,23 @@ def _resblocks(sd, cfg, n_stages: int) -> None:
 
 
 def hifigan_state_dict(cfg: dict, seed: int = 0) -> Dict[str, torch.Tensor]:
-    """Folded (weight-norm removed) generator weights of ``torch.manual_seed(seed); Generator(h)``."""
+    """Folded (weight-norm removed) generator weights of ``torch.manual_seed(seed); Generator(h)``.  At
+    ``sampling_rate == 24000`` each upsampling layer is ``Sequential(InterpolationBlock(u), Conv1d(k))`` (models.py:107-118):
+    its conv is ``ups.{i}.1`` and consumes the RNG where the ConvTranspose1d would."""
     torch.manual_seed(seed)
     sd: Dict[str, torch.Tensor] = {}
     C0 = cfg["upsample_initial_channel"]
     _put(sd, "conv_pre", torch.nn.Conv1d(80, C0, 7))
+    interp = cfg.get("sampling_rate") == 24000
     ups = []
     for i, (u, k) in enumerate(zip(cfg["upsample_rates"], cfg["upsample_kernel_sizes"])):
-        m = torch.nn.ConvTranspose1d(C0 // (2 ** i), C0 // (2 ** (i + 1)), k, u)
+        if interp:
+            m = torch.nn.Conv1d(C0 // (2 ** i), C0 // (2 ** (i + 1)), k)
+            _put(sd, f"ups.{i}.1", m)
+        else:
+            m = torch.nn.ConvTranspose1d(C0 // (2 ** i), C0 // (2 ** (i + 1)), k, u)
+            _put(sd, f"ups.{i}", m)
         ups.append(m)
-        _put(sd, f"ups.{i}", m)
     _resblocks(sd, cfg, len(ups))
     post = torch.nn.Conv1d(C0 // (2 ** len(ups)), 1, 7)
     _put(sd, "conv_post", post)
@@ -130,6 +137,26 @@ HIFIGAN_CONFIG_16K = {
     "upsample_initial_channel": 512, "resblock_kernel_sizes": [3, 7, 11],
     "resblock_dilation_sizes": [[1, 3, 5], [1, 3, 5], [1, 3, 5]],
     "num_mels": 80, "hop_size": 200, "sampling_rate": 16000,
+}
+
+# 24 kHz HiFi-GAN (nearest upsample + Conv1d per stage, hop 240 = 10 ms frames).  A STAND-IN: the json of the released 24 kHz
+# checkpoint (run.py:46, vocoder/saved_models/24k/) is not part of the reference tree, so these are plausible values with
+# prod(upsample_rates) == hop_size and odd kernel sizes; the library itself takes every value from the caller's config.
+HIFIGAN_CONFIG_24K = {
+    "resblock": "1", "seed": 1234,
+    "upsample_rates": [5, 4, 3, 2, 2], "upsample_kernel_sizes": [11, 9, 7, 5, 5],
+    "upsample_initial_channel": 512, "resblock_kernel_sizes": [3, 7, 11],
+    "resblock_dilation_sizes": [[1, 3, 5], [1, 3, 5], [1, 3, 5]],
+    "num_mels": 80, "hop_size": 240, "sampling_rate": 24000,
+}
+
+# test-only second 24 kHz config: upsample rate 8, a kernel (17) wider than the tap conv's 11 taps before folding, ResBlock2
+HIFIGAN_CONFIG_24K_U8 = {
+    "resblock": "2", "seed": 1234,
+    "upsample_rates": [8, 5, 3, 2], "upsample_kernel_sizes": [17, 11, 7, 5],
+    "upsample_initial_channel": 256, "resblock_kernel_sizes": [3, 7, 11],
+    "resblock_dilation_sizes": [[1, 3], [1, 3], [1, 3]],
+    "num_mels": 80, "hop_size": 240, "sampling_rate": 24000,
 }
 
 FREGAN_CONFIG = {
