@@ -364,6 +364,63 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
                          const uint8_t* dec_masks, uint64_t seed, float* mel, float* linear, float* attn,
                          int32_t* frames_out_host, void* workspace, size_t workspace_bytes, void* stream);
 
+/* test hook: ONE launch of a 3-term-split tensor-core GEMM of the Tacotron / speaker-encoder family on caller-provided fp32
+ * device tensors (no model handle), through the functions the forward uses, in its order: tc_skinny_absmax -> tc_weight_scale ->
+ * tc_skinny_pack / pack_big_w -> act_split / im2col_split -> launch_tc_{skinny,gru,lstm_seq,big}.  Tensors are row-major. */
+#define MB_TACO_TC_SKINNY_PLAIN 0 /* y[M][N] = [x0 | x1] . [w0 | w1]^T + b0 + b1 (+ pre), at y + step * y_step                   */
+#define MB_TACO_TC_SKINNY_LSTM 1  /* gates of [x0 | x1] . [w0 | w1]^T + b0 + b1, w [4H][K] (i|f|g|o): c in/out, h out, xres += h */
+#define MB_TACO_TC_GRU 2          /* per direction d: gh = h_d . w[d]^T + b[d] (w [3H][H]), GRU cell with gi[d]: hst[d] in/out, out[d] */
+#define MB_TACO_TC_LSTM_SEQ 3     /* gates = x0 . w0^T + gi[0] (w0 [4H][H], x0 = h_{t-1}, any M): c in/out, h_t -> out[0] */
+#define MB_TACO_TC_BIG 4          /* y = res + BN(act(sum_s x_s[row + shift_s] . W_s^T + b0)), W_s[n][k] = w0[n*ldw + w_off_s + k*w_stride_s] */
+typedef struct mb_taco_tc_debug_spec {
+  int32_t kind;              /* MB_TACO_TC_* */
+  int32_t M, N, H;           /* rows; output columns (PLAIN, BIG); hidden units (LSTM, GRU, LSTM_SEQ) */
+  int32_t K0, K1;            /* SKINNY: the two K segments (K1 may be 0); GRU / LSTM_SEQ: K0 = H; BIG: K of every segment */
+  const float* w[2];         /* SKINNY: w0 [rows][K0], w1 [rows][K1]; GRU: W_hh of direction d; LSTM_SEQ / BIG: w[0] */
+  const float* b[2];         /* SKINNY: biases summed (either may be NULL); GRU: b_hh of direction d; BIG: b[0] [N] or NULL */
+  int32_t ldw;               /* BIG */
+  int32_t nseg, T;           /* BIG: segments (taps, <= 5), rows per sequence (shift bounds) */
+  const float* x[5];         /* SKINNY: x0 [M][ldx0], x1; GRU: h_{t-1} of direction d; LSTM_SEQ: x[0]; BIG: segment inputs */
+  int32_t ldx[5], shift[5], w_off[5], w_stride[5];
+  int32_t kb0, kb_count;     /* SKINNY: only k-blocks [kb0, kb0 + kb_count) of the image (kb_count 0: all) */
+  const float* pre;          /* SKINNY: partial sum [M][ldpre] in tile column order, or NULL */
+  int32_t ldpre;
+  const int32_t* step_ptr;   /* PLAIN: output slab step = (*step_ptr or 0) + step_j */
+  int32_t step_j;
+  int64_t y_step;
+  float* y;                  /* PLAIN / BIG output, row stride ldy */
+  int32_t ldy;
+  float* c;                  /* LSTM / LSTM_SEQ cell state [M][H] */
+  float* h;                  /* LSTM: h' out [M][H] */
+  float* xres;               /* LSTM: residual stream [M][H] in/out */
+  const float* gi[2];        /* GRU / LSTM_SEQ: input projections, row m at gi[d] + m * ldgi */
+  int32_t ldgi;
+  float* hst[2];             /* GRU: state [M][H] in/out of direction d */
+  float* out[2];             /* GRU / LSTM_SEQ: h' also at out[d] + m * ldout */
+  int32_t ldout, ndir;
+  void* s_hi[2];             /* fused hi/lo outputs (fp16 tiles [KB][rows_pad][64]) at columns s_k0[slot] + n, or NULL: */
+  void* s_lo[2];             /*   SKINNY slot 0 = y (PLAIN) / xres (LSTM), slot 1 = h (LSTM); GRU slot 0 = direction 0's h' */
+  int32_t s_k0[2];
+  void* nxt_hi[2];           /* GRU / LSTM_SEQ: the next step's operand tiles of h' (direction d), or NULL */
+  void* nxt_lo[2];
+  int32_t act;               /* BIG: 0 none, 1 ReLU */
+  const float* bn_scale;     /* BIG: y = act(.) * bn_scale + bn_shift, or NULL */
+  const float* bn_shift;
+  const float* res;          /* BIG: residual [M][ldres] or NULL */
+  int32_t ldres;
+  int32_t compact;           /* SKINNY: compact 8-stage ring for <= 64 rows: 0 / 1, -1 = MB_TACO_RING8 */
+  int32_t cluster;           /* SKINNY: activation multicast cluster 1 / 2 / 4 / 8, 0 = MB_TACO_MC */
+  int32_t pdl;               /* 0 / 1, -1 = MB_TACO_PDL */
+  void* a_tiles;             /* optional out: the activation operand tiles, hi plane then lo plane (direction 0) */
+  void* w_tiles;             /* optional out: the packed weight image (direction 0) */
+} mb_taco_tc_debug_spec;
+/* device workspace the spec needs */
+size_t mb_taco_tc_debug_workspace_bytes(const mb_taco_tc_debug_spec* spec);
+/* synchronises `stream` (the pack scale is read back); writes one line into `report`:
+ * "kernel=K grid=X,Y cluster=C compact=0|1 rows_pad=R mma_groups=G,G_last inv_scale=S a_bytes=A w_bytes=W" */
+int mb_taco_tc_debug(const mb_taco_tc_debug_spec* spec, void* workspace, size_t workspace_bytes, void* stream, char* report,
+                     size_t report_len);
+
 /* ---------------------------------------------------------------------------------------------
  * Speaker encoder (cfg 5 front half)
  *   replaces  models/encoder/model.py:41-61 (SpeakerEncoder.forward: 3 x LSTM(40 -> 256), last hidden of

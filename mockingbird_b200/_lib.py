@@ -65,6 +65,29 @@ class GanDebugSpec(C.Structure):
     ]
 
 
+MB_TACO_TC_SKINNY_PLAIN = 0
+MB_TACO_TC_SKINNY_LSTM = 1
+MB_TACO_TC_GRU = 2
+MB_TACO_TC_LSTM_SEQ = 3
+MB_TACO_TC_BIG = 4
+
+
+class TacoTcDebugSpec(C.Structure):
+    _fields_ = [
+        ("kind", C.c_int32), ("M", C.c_int32), ("N", C.c_int32), ("H", C.c_int32), ("K0", C.c_int32), ("K1", C.c_int32),
+        ("w", C.c_void_p * 2), ("b", C.c_void_p * 2), ("ldw", C.c_int32), ("nseg", C.c_int32), ("T", C.c_int32),
+        ("x", C.c_void_p * 5), ("ldx", C.c_int32 * 5), ("shift", C.c_int32 * 5), ("w_off", C.c_int32 * 5),
+        ("w_stride", C.c_int32 * 5), ("kb0", C.c_int32), ("kb_count", C.c_int32), ("pre", C.c_void_p), ("ldpre", C.c_int32),
+        ("step_ptr", C.c_void_p), ("step_j", C.c_int32), ("y_step", C.c_int64), ("y", C.c_void_p), ("ldy", C.c_int32),
+        ("c", C.c_void_p), ("h", C.c_void_p), ("xres", C.c_void_p), ("gi", C.c_void_p * 2), ("ldgi", C.c_int32),
+        ("hst", C.c_void_p * 2), ("out", C.c_void_p * 2), ("ldout", C.c_int32), ("ndir", C.c_int32),
+        ("s_hi", C.c_void_p * 2), ("s_lo", C.c_void_p * 2), ("s_k0", C.c_int32 * 2), ("nxt_hi", C.c_void_p * 2),
+        ("nxt_lo", C.c_void_p * 2), ("act", C.c_int32), ("bn_scale", C.c_void_p), ("bn_shift", C.c_void_p),
+        ("res", C.c_void_p), ("ldres", C.c_int32), ("compact", C.c_int32), ("cluster", C.c_int32), ("pdl", C.c_int32),
+        ("a_tiles", C.c_void_p), ("w_tiles", C.c_void_p),
+    ]
+
+
 class WaveRNNConfig(C.Structure):
     _fields_ = [
         ("rnn_dims", C.c_int32),
@@ -182,6 +205,8 @@ SIGNATURES = {
     "mb_tacotron_generate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                        C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mb_taco_tc_debug_workspace_bytes": (C.c_size_t, [C.POINTER(TacoTcDebugSpec)]),
+    "mb_taco_tc_debug": (C.c_int, [C.POINTER(TacoTcDebugSpec), C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]),
     "mb_encoder_create": (C.c_int, [C.POINTER(EncoderConfig), C.POINTER(C.c_void_p)]),
     "mb_encoder_destroy": (None, [C.c_void_p]),
     "mb_encoder_arena_bytes": (C.c_size_t, [C.c_void_p]),

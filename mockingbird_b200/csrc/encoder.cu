@@ -249,7 +249,7 @@ int mb_encoder_finalize(mb_encoder* h, void* stream) {
     MB_LAUNCH_CHECK("add_vec_kernel");
   }
   if (enc_use_tc(h->cfg)) {
-    // tensor-core images of every W_hh (power-of-two scale from max |w|, see tacotron.cu tc_prepare)
+    // tensor-core images of every W_hh (power-of-two scale from max |w|, tc_weight_scale)
     const int H = h->cfg.hidden_size;
     unsigned int* dmax = reinterpret_cast<unsigned int*>(P(h, "scratch.absmax.bias_sum"));
     MB_CUDA_CHECK(cudaMemsetAsync(dmax, 0, 8 * sizeof(unsigned int), st));
@@ -259,11 +259,7 @@ int mb_encoder_finalize(mb_encoder* h, void* stream) {
     MB_CUDA_CHECK(cudaMemcpyAsync(hmax, dmax, sizeof(hmax), cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
     for (int l = 0; l < h->cfg.num_layers; ++l) {
-      float mx;
-      memcpy(&mx, &hmax[l], sizeof(float));
-      int e = 0;
-      if (mx > 0.f && mx < 3.0e38f) frexpf(mx, &e);
-      const float scale = ldexpf(1.f, 12 - e);
+      const float scale = tc_weight_scale(hmax[l]);
       h->tc_inv_scale[l] = 1.f / scale;
       const std::string s = std::to_string(l);
       TK(tc_skinny_pack(P(h, "lstm.weight_hh_l" + s), H, nullptr, 0, nullptr, nullptr, 4 * H, H, scale,
@@ -309,10 +305,6 @@ int mb_encoder_embed_frames(mb_encoder* h, const float* frames, int32_t rows, in
         unsigned int hmax = 0;
         MB_CUDA_CHECK(cudaMemcpyAsync(&hmax, dmax, sizeof(hmax), cudaMemcpyDeviceToHost, st));
         MB_CUDA_CHECK(cudaStreamSynchronize(st));
-        float mx;
-        memcpy(&mx, &hmax, sizeof(float));
-        int e = 0;
-        if (mx > 0.f && mx < 3.0e38f) frexpf(mx, &e);
         TcBigPack q;
         memset(&q, 0, sizeof(q));
         q.W = P(h, "lstm.weight_ih_l" + s);
@@ -323,7 +315,7 @@ int mb_encoder_embed_frames(mb_encoder* h, const float* frames, int32_t rows, in
         q.KBs = KBs;
         q.w_off[0] = 0;
         q.w_stride[0] = 1;
-        q.scale = ldexpf(1.f, 12 - e);
+        q.scale = tc_weight_scale(hmax);
         h->big_inv_scale[l] = 1.f / q.scale;
         TK(launch_pack_big_w(q, wimg, st));
         h->big_packed[l] = true;

@@ -625,10 +625,6 @@ int cbhg_gemm(mb_tacotron* h, const std::string& key, const GemmArgs& a, cudaStr
     unsigned int hmax = 0;
     MB_CUDA_CHECK(cudaMemcpyAsync(&hmax, dmax, sizeof(hmax), cudaMemcpyDeviceToHost, st));
     MB_CUDA_CHECK(cudaStreamSynchronize(st));
-    float mx;
-    memcpy(&mx, &hmax, sizeof(float));
-    int e = 0;
-    if (mx > 0.f && mx < 3.0e38f) frexpf(mx, &e);
     TcBigPack q;
     memset(&q, 0, sizeof(q));
     q.W = a.W;
@@ -641,7 +637,7 @@ int cbhg_gemm(mb_tacotron* h, const std::string& key, const GemmArgs& a, cudaStr
       q.w_off[s] = a.seg[s].w_off;
       q.w_stride[s] = a.seg[s].w_stride;
     }
-    q.scale = ldexpf(1.f, 12 - e);
+    q.scale = tc_weight_scale(hmax);
     h->tc_inv_scale[key + ".bigw"] = 1.f / q.scale;
     TK(launch_pack_big_w(q, wimg, st));
     h->big_packed.insert(key);
@@ -838,8 +834,7 @@ int run_cbhg(mb_tacotron* h, const std::string& p, int K, int cin, int ch, int p
   return MB_OK;
 }
 
-// absmax -> power-of-two scale (max |w| lands in [2^11, 2^12): the lo parts of the fp16 split stay clear of the
-// subnormal range) -> hi/lo tile images "<name>.tcw" + tile-order bias "<name>.tcb".  Synchronises the stream.
+// absmax -> power-of-two scale (tc_weight_scale) -> hi/lo tile images "<name>.tcw" + tile-order bias "<name>.tcb".  Synchronises the stream.
 int tc_prepare(mb_tacotron* h, const std::string& name, const float* w0, int K0, const float* w1, int K1, const float* b0,
                const float* b1, int N, int lstm_H, cudaStream_t st) {
   unsigned int* dmax = reinterpret_cast<unsigned int*>(P(h, "scratch.absmax.tcb"));
@@ -849,11 +844,7 @@ int tc_prepare(mb_tacotron* h, const std::string& name, const float* w0, int K0,
   unsigned int hmax = 0;
   MB_CUDA_CHECK(cudaMemcpyAsync(&hmax, dmax, sizeof(hmax), cudaMemcpyDeviceToHost, st));
   MB_CUDA_CHECK(cudaStreamSynchronize(st));
-  float mx;
-  memcpy(&mx, &hmax, sizeof(float));
-  int e = 0;
-  if (mx > 0.f && mx < 3.0e38f) frexpf(mx, &e);  // mx = f * 2^e, f in [0.5, 1)
-  const float scale = ldexpf(1.f, 12 - e);
+  const float scale = tc_weight_scale(hmax);
   h->tc_inv_scale[name] = 1.f / scale;
   TK(tc_skinny_pack(w0, K0, w1, K1, b0, b1, N, lstm_H, scale, reinterpret_cast<__half*>(P(h, name + ".tcw")),
                     P(h, name + ".tcb"), st));

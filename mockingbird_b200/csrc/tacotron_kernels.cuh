@@ -207,9 +207,14 @@ struct TcBigArgs {
 };
 size_t tc_big_weight_bytes(int N, int nseg, int K);
 size_t tc_big_act_bytes(int M, int nseg, int K);
+// what a tensor-core launch ran with (filled by the launchers when asked; mb_taco_tc_debug reports it)
+struct TcLaunchInfo {
+  int grid_x, grid_y, cluster, compact, rows_pad, mma_groups, mma_groups_last;  // mma_groups(_last): first / last row block
+};
+// pdl: -1 = MB_TACO_PDL (read once per process), 0 = plain launch, 1 = programmatic dependent launch
 cudaError_t launch_im2col_split(const TcIm2col& q, __half* a_hi, __half* a_lo, cudaStream_t st);
 cudaError_t launch_pack_big_w(const TcBigPack& q, __half* dst, cudaStream_t st);
-cudaError_t launch_tc_big(const TcBigArgs& a, cudaStream_t st);
+cudaError_t launch_tc_big(const TcBigArgs& a, cudaStream_t st, int pdl = -1, TcLaunchInfo* info = nullptr);
 
 // one time step of an LSTM layer over M rows (any M; operand tiles hold rows_total = ceil128(M) rows per k-block)
 struct TcLstmSeqArgs {
@@ -224,18 +229,27 @@ struct TcLstmSeqArgs {
   float inv_scale;
   int ldgi, ldout, KB, M, H, rows_total;
 };
-cudaError_t launch_tc_lstm_seq(const TcLstmSeqArgs& a, cudaStream_t st);
+cudaError_t launch_tc_lstm_seq(const TcLstmSeqArgs& a, cudaStream_t st, int pdl = -1, TcLaunchInfo* info = nullptr);
 size_t tc_gated_weight_bytes(int H, int K);
 size_t tc_skinny_weight_bytes(int N, int K);
 size_t tc_skinny_act_bytes(int M, int K);
 // max |w| into *dev_out (uint bit pattern of a non-negative float; caller zeroes it first)
 cudaError_t tc_skinny_absmax(const float* w, size_t n, unsigned int* dev_out, cudaStream_t st);
+// power-of-two pack scale of a weight whose max |w| is `absmax_bits` (the bit pattern tc_skinny_absmax leaves): max |w| * scale
+// lands in [2^11, 2^12), so the lo parts of the fp16 split stay clear of the subnormal range; a zero, inf or NaN max gives 2^12.
+// Every weight image of the tensor-core GEMMs is packed with this scale and read back with 1 / scale.
+float tc_weight_scale(unsigned int absmax_bits);
 // weights [N][K0 | K1] (two row-major sources) * scale -> hi/lo tiles; lstm_H > 0: gate-interleaved rows
 cudaError_t tc_skinny_pack(const float* w0, int K0, const float* w1, int K1, const float* b0, const float* b1, int N,
                            int lstm_H, float scale, __half* w_dst, float* bias_dst, cudaStream_t st);
 cudaError_t launch_act_split(const float* s0, int K0, int ld0, const float* s1, int K1, int ld1, int M, __half* a_hi,
                              __half* a_lo, cudaStream_t st);
+// Launch variants are arguments: ring8 (compact 8-stage ring for <= 64 rows) 0 / 1, mc = cluster size of the activation multicast
+// 1 / 2 / 4 / 8 (used only where it divides the tile count), pdl as above.  The two-argument form takes all three from the
+// environment (MB_TACO_RING8, MB_TACO_MC, MB_TACO_PDL), as the forward does.
+cudaError_t launch_tc_skinny(const TcSkinnyArgs& a, cudaStream_t st, int ring8, int mc, int pdl, TcLaunchInfo* info = nullptr);
 cudaError_t launch_tc_skinny(const TcSkinnyArgs& a, cudaStream_t st);
+cudaError_t launch_tc_gru(const TcGruArgs& a, cudaStream_t st, int pdl, TcLaunchInfo* info = nullptr);
 
 }  // namespace taco
 }  // namespace mb

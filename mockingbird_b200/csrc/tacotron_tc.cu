@@ -5,8 +5,13 @@
 // kernels are compute-bound there at ~7 TFLOP/s; the tensor cores need fp16 operands, which alone would
 // break the 1e-3 parity bar after 200 recurrent steps.  So every product is computed as a 3-term split
 //     a*w ~= hi(a)*hi(w) + lo(a)*hi(w) + hi(a)*lo(w),   hi(v) = fp16(v), lo(v) = fp16(v - hi(v))
-// with FP32 accumulation in registers: ~2^-21 relative per product, i.e. FP32-equivalent (weights are
-// pre-scaled by a power of two so that their lo parts stay out of the fp16 subnormal range).
+// with FP32 accumulation in registers.  Weights are pre-scaled by a power of two (tc_weight_scale) so that their lo parts stay out
+// of the fp16 subnormal range; activations are not scaled.  Precision contract per product, for |a| < 65520 (fp16(a) = inf
+// beyond):  |a w - split(a, w)| <= 2^-20 |a||w| + 2^-24 |w|  (+ 2^-24 |a| / scale, negligible).  The relative term is
+// FP32-equivalent; the absolute floor comes from lo(a) being an fp16 subnormal for |a| < 2^-3.  The FP32 accumulation adds at most
+// 2^-22 of the running-sum magnitudes per wgmma step.  oracle/tc_split_oracle.py derives both; tests/test_taco_tc_gemm.py holds every
+// kernel to them.  No shipped path feeds |a| >= 65520: the decoder and CBHG inputs are tanh / sigmoid / ReLU-BN outputs, embeddings
+// and mel frames of unit scale, and the encoder's mel power is bounded far below it (DESIGN.md section 4c).
 //
 //   grid      : one CTA per 32 output columns (LSTM: the 4 gates of 8 hidden units, interleaved at pack
 //               time, so the cell update c' = f*c + i*g, h' = o*tanh(c') runs in the epilogue)
@@ -370,7 +375,8 @@ __global__ void __launch_bounds__(kThreads, 1) tc_big_kernel(const __grid_consta
 }
 
 // im2col of a channels-last fp32 tensor into hi / lo operand tiles [nseg * KBs][rows_total][64]: segment s holds
-// x[row + shift_s][0 .. K) (zero outside the row's own length-T sequence, zero for k >= K and rows >= M)
+// x[row + shift_s][0 .. K) (zero outside the row's own length-T sequence, zero for k >= K and rows >= M; source rows >= M are
+// outside every sequence)
 __global__ void im2col_split_kernel(const TcIm2col q, __half* __restrict__ a_hi, __half* __restrict__ a_lo) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // one thread per 16-byte chunk
   const size_t total = (size_t)q.nseg * q.KBs * q.rows_total * 8;
@@ -384,8 +390,8 @@ __global__ void im2col_split_kernel(const TcIm2col q, __half* __restrict__ a_hi,
   int row = m;
   if (ok && q.shift[sg] != 0) {
     const int t = m % q.T + q.shift[sg];
-    ok = (t >= 0 && t < q.T);
     row = m + q.shift[sg];
+    ok = (t >= 0 && t < q.T && row < q.M);  // a last, partial sequence (M not a multiple of T) ends at row M
   }
   const float* src = q.x[sg] + (size_t)row * q.ld[sg];
 #pragma unroll
@@ -514,10 +520,11 @@ __global__ void absmax_kernel(const float* __restrict__ w, size_t n, unsigned in
 
 }  // namespace
 
-// launch with the programmatic-stream-serialization attribute (MB_TACO_PDL=0: plain launches)
+// launch with the programmatic-stream-serialization attribute (pdl = -1: MB_TACO_PDL, whose 0 means plain launches)
 template <typename Args>
-cudaError_t launch_pdl(void (*kern)(const Args), dim3 grid, size_t smem, cudaStream_t st, const Args& args, int cluster_x = 1) {
-  static const bool pdl = [] {
+cudaError_t launch_pdl(void (*kern)(const Args), dim3 grid, size_t smem, cudaStream_t st, const Args& args, int cluster_x = 1,
+                       int pdl = -1) {
+  static const bool pdl_env = [] {
     const char* e = getenv("MB_TACO_PDL");
     return e ? atoi(e) != 0 : true;
   }();
@@ -529,7 +536,7 @@ cudaError_t launch_pdl(void (*kern)(const Args), dim3 grid, size_t smem, cudaStr
   cfg.stream = st;
   cudaLaunchAttribute attr[2];
   int na = 0;
-  if (pdl) {
+  if (pdl < 0 ? pdl_env : pdl != 0) {
     attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[na].val.programmaticStreamSerializationAllowed = 1;
     ++na;
@@ -544,6 +551,27 @@ cudaError_t launch_pdl(void (*kern)(const Args), dim3 grid, size_t smem, cudaStr
   cfg.attrs = attr;
   cfg.numAttrs = na;
   return cudaLaunchKernelEx(&cfg, kern, args);
+}
+
+namespace {
+void fill_info(TcLaunchInfo* info, dim3 grid, int cluster, int compact, int rows_pad, int rows_first, int rows_last) {
+  if (!info) return;
+  info->grid_x = (int)grid.x;
+  info->grid_y = (int)grid.y;
+  info->cluster = cluster;
+  info->compact = compact;
+  info->rows_pad = rows_pad;
+  info->mma_groups = rows_first > 64 ? 2 : 1;  // skinny_body_t: the second MMA warpgroup only for more than 64 rows
+  info->mma_groups_last = rows_last > 64 ? 2 : 1;
+}
+}  // namespace
+
+float tc_weight_scale(unsigned int absmax_bits) {
+  float mx;
+  memcpy(&mx, &absmax_bits, sizeof(float));
+  int e = 0;
+  if (mx > 0.f && mx < 3.0e38f) frexpf(mx, &e);  // mx = f * 2^e, f in [0.5, 1)
+  return ldexpf(1.f, 12 - e);
 }
 
 size_t tc_skinny_weight_bytes(int N, int K) {
@@ -605,7 +633,7 @@ cudaError_t launch_pack_big_w(const TcBigPack& q, __half* dst, cudaStream_t st) 
   return cudaGetLastError();
 }
 
-cudaError_t launch_tc_big(const TcBigArgs& a, cudaStream_t st) {
+cudaError_t launch_tc_big(const TcBigArgs& a, cudaStream_t st, int pdl, TcLaunchInfo* info) {
   if (a.M <= 0 || a.N <= 0 || a.N % 4 || a.KB <= 0 || a.rows_total % 128 || a.rows_total < a.M) return cudaErrorInvalidValue;
   constexpr size_t smem = kBigStages * stage_bytes<128>() + 1024 + 1024 + kEpiStageBytes;
   static bool attr = false;
@@ -614,10 +642,12 @@ cudaError_t launch_tc_big(const TcBigArgs& a, cudaStream_t st) {
     if (e != cudaSuccess) return e;
     attr = true;
   }
-  return launch_pdl(tc_big_kernel, dim3((a.N + 127) / 128, (a.M + 127) / 128), smem, st, a);
+  const dim3 grid((a.N + 127) / 128, (a.M + 127) / 128);
+  fill_info(info, grid, 1, 0, 128, a.M < 128 ? a.M : 128, a.M - (int)(grid.y - 1) * 128);
+  return launch_pdl(tc_big_kernel, grid, smem, st, a, 1, pdl);
 }
 
-cudaError_t launch_tc_lstm_seq(const TcLstmSeqArgs& a, cudaStream_t st) {
+cudaError_t launch_tc_lstm_seq(const TcLstmSeqArgs& a, cudaStream_t st, int pdl, TcLaunchInfo* info) {
   if (a.M <= 0 || a.H <= 0 || a.H % 8 || a.KB <= 0 || a.rows_total % 128 || a.rows_total < a.M) return cudaErrorInvalidValue;
   constexpr size_t smem = kStages * kStageBytes + 1024 + 1024 + kEpiStageBytes;
   static bool attr = false;
@@ -626,10 +656,12 @@ cudaError_t launch_tc_lstm_seq(const TcLstmSeqArgs& a, cudaStream_t st) {
     if (e != cudaSuccess) return e;
     attr = true;
   }
-  return launch_pdl(tc_lstm_seq_kernel, dim3(a.H / 8, (a.M + 127) / 128), smem, st, a);
+  const dim3 grid(a.H / 8, (a.M + 127) / 128);
+  fill_info(info, grid, 1, 0, 128, a.M < 128 ? a.M : 128, a.M - (int)(grid.y - 1) * 128);
+  return launch_pdl(tc_lstm_seq_kernel, grid, smem, st, a, 1, pdl);
 }
 
-cudaError_t launch_tc_gru(const TcGruArgs& a, cudaStream_t st) {
+cudaError_t launch_tc_gru(const TcGruArgs& a, cudaStream_t st, int pdl, TcLaunchInfo* info) {
   if (a.M <= 0 || a.M > 128 || a.H <= 0 || a.H % 8 || a.KB <= 0 || a.ndir < 1 || a.ndir > 2) return cudaErrorInvalidValue;
   TcGruArgs p = a;
   p.rows_pad = a.M <= 64 ? 64 : 128;
@@ -640,17 +672,17 @@ cudaError_t launch_tc_gru(const TcGruArgs& a, cudaStream_t st) {
     if (e != cudaSuccess) return e;
     attr = true;
   }
-  return launch_pdl(tc_gru_kernel, dim3(a.H / 8, a.ndir), smem, st, p);
+  const dim3 grid(a.H / 8, a.ndir);
+  fill_info(info, grid, 1, 0, p.rows_pad, a.M, a.M);
+  return launch_pdl(tc_gru_kernel, grid, smem, st, p, 1, pdl);
 }
 
-cudaError_t launch_tc_skinny(const TcSkinnyArgs& a, cudaStream_t st) {
+cudaError_t launch_tc_gru(const TcGruArgs& a, cudaStream_t st) { return launch_tc_gru(a, st, -1); }
+
+cudaError_t launch_tc_skinny(const TcSkinnyArgs& a, cudaStream_t st, int ring8, int mc, int pdl, TcLaunchInfo* info) {
   if (a.M <= 0 || a.M > 128 || a.N <= 0 || a.KB <= 0) return cudaErrorInvalidValue;
   TcSkinnyArgs p = a;
   p.rows_pad = a.M <= 64 ? 64 : 128;
-  static const bool ring8 = [] {
-    const char* e = getenv("MB_TACO_RING8");  // A/B switch: 0 = 4 stages of 40 KB for every batch size (round 2)
-    return e ? atoi(e) != 0 : true;
-  }();
   p.compact = (ring8 && p.rows_pad == 64) ? 1 : 0;
   constexpr size_t smem = (kStages * kStageBytes > 2 * kStages * (kATile + 2 * kWTile) ? kStages * kStageBytes : 2 * kStages * (kATile + 2 * kWTile)) + 1024 + 1024 + kEpiStageBytes;
   static bool attr = false;
@@ -659,6 +691,17 @@ cudaError_t launch_tc_skinny(const TcSkinnyArgs& a, cudaStream_t st) {
     if (e != cudaSuccess) return e;
     attr = true;
   }
+  const int tiles = (a.N + 31) / 32;
+  const int cl = (mc > 1 && tiles % mc == 0 && (p.rows_pad * 128) % (16 * mc) == 0) ? mc : 1;
+  fill_info(info, dim3(tiles), cl, p.compact, p.rows_pad, a.M, a.M);
+  return launch_pdl(tc_skinny_kernel, dim3(tiles), smem, st, p, cl, pdl);
+}
+
+cudaError_t launch_tc_skinny(const TcSkinnyArgs& a, cudaStream_t st) {
+  static const bool ring8 = [] {
+    const char* e = getenv("MB_TACO_RING8");  // A/B switch: 0 = 4 stages of 40 KB for every batch size (round 2)
+    return e ? atoi(e) != 0 : true;
+  }();
   // MB_TACO_MC = 2 / 4 / 8: cluster size of the activation-tile multicast (launches whose tile count it divides).  Default 1 (no
   // clusters): MEASURED SLOWER - cfg 4 takes 42.1 ms with clusters of 8 and 36.3 ms with 4 against 35.6 ms without (same box, ABAB).
   // The launches are not bound by L2 traffic; co-scheduling 8 SMs of a GPC per cluster and refilling a stage only when the slowest
@@ -668,9 +711,7 @@ cudaError_t launch_tc_skinny(const TcSkinnyArgs& a, cudaStream_t st) {
     const int v = e ? atoi(e) : 1;
     return (v == 2 || v == 4 || v == 8) ? v : 1;
   }();
-  const int tiles = (a.N + 31) / 32;
-  const int cl = (mc_env > 1 && tiles % mc_env == 0 && (p.rows_pad * 128) % (16 * mc_env) == 0) ? mc_env : 1;
-  return launch_pdl(tc_skinny_kernel, dim3(tiles), smem, st, p, cl);
+  return launch_tc_skinny(a, st, ring8 ? 1 : 0, mc_env, -1);
 }
 
 }  // namespace taco
