@@ -542,6 +542,57 @@ int mb_ppg2mel_inference(mb_ppg2mel* h, const float* ppg, const float* lf0_uv, c
                          float* mel, float* mel_post, float* align, float* stop, int32_t* steps_host, void* workspace,
                          size_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Voice-conversion PPG extractor (Conformer ASR encoder)
+ *   replaces  models/ppg_extractor/__init__.py:25-39 (PPGModel.forward: DefaultFrontend STFT + log-mel, UtteranceMVN,
+ *             ConformerEncoder with a Conv2d input layer, relative or absolute positional attention, macaron FFN and
+ *             convolution module)
+ * Every config value comes from the caller (the reference's args.frontend_conf / normalize_conf / encoder_conf); options
+ * the kernels do not implement are rejected by create with MB_ERR_INVALID and a message.
+ * ------------------------------------------------------------------------------------------- */
+#define MB_PPGX_INPUT_CONV2D 0        /* input_layer: "conv2d" (only this); 1 "linear", 2 "vgg2l", 3 "embed" */
+#define MB_PPGX_POS_ABS 0             /* pos_enc_layer_type "abs_pos" */
+#define MB_PPGX_POS_SCALED_ABS 1      /*   "scaled_abs_pos" (rejected) */
+#define MB_PPGX_POS_REL 2             /*   "rel_pos" */
+#define MB_PPGX_ATTN_SELF 0           /* selfattention_layer_type "selfattn" */
+#define MB_PPGX_ATTN_REL 1            /*   "rel_selfattn" */
+#define MB_PPGX_FF_LINEAR 0           /* positionwise_layer_type "linear"; 1 "conv1d", 2 "conv1d-linear" (rejected) */
+#define MB_PPGX_ACT_SWISH 0           /* activation_type "swish" */
+#define MB_PPGX_ACT_RELU 1            /*   "relu" */
+typedef struct mb_ppgx_config {
+  int32_t n_fft, win_length, hop_length, n_mels;  /* frontend_conf (n_fft <= 1024, win_length <= n_fft) */
+  int32_t kaldi_padding_mode, downsample_rate;    /* frontend_conf: 0 and 1 only */
+  int32_t norm_means, norm_vars;                  /* normalize_conf */
+  int32_t attention_dim, attention_heads, linear_units, num_blocks;
+  int32_t input_layer, no_subsample, subsample_by_2;
+  int32_t normalize_before, concat_after, positionwise_layer_type;
+  int32_t macaron_style, pos_enc_layer_type, selfattention_layer_type, activation_type;
+  int32_t use_cnn_module, cnn_module_kernel;
+} mb_ppgx_config;
+
+typedef struct mb_ppgx mb_ppgx;
+
+int mb_ppgx_create(const mb_ppgx_config* cfg, mb_ppgx** out);
+void mb_ppgx_destroy(mb_ppgx* h);
+size_t mb_ppgx_arena_bytes(const mb_ppgx* h);
+int mb_ppgx_set_arena(mb_ppgx* h, void* arena, size_t bytes);
+/* tensors of PPGModel.state_dict() under their reference names (frontend.logmel.melmat [n_fft / 2 + 1][n_mels] is an input
+ * weight; inv_melmat and num_batches_tracked are accepted and ignored); finalize packs the tensor-core weight images */
+int mb_ppgx_set_weight(mb_ppgx* h, const char* name, const float* w, const int64_t* dims, int32_t ndim, void* stream);
+int mb_ppgx_finalize(mb_ppgx* h, void* stream);
+/* PPG frames of an n-sample utterance: 1 + n / hop_length, halved by each stride-2 conv of the input layer */
+int32_t mb_ppgx_num_frames(const mb_ppgx* h, int32_t n_samples);
+size_t mb_ppgx_workspace_bytes(const mb_ppgx* h, int32_t batch, int32_t n_samples_max);
+/* PPGModel.forward for a padded batch of 1..128 rows, each row computed as its own B = 1 call (bitwise):
+ *   wav fp32 [B][n_max] (device); n_samples int32 [B] (host): n_fft / 2 < n_samples[b] <= n_max
+ *   pe_len: rows of the positional table the module instance holds (max(5000, longest T it has seen)); pos_table fp32
+ *     [T_max][attention_dim] (device): rows [0, T_max) of that table as the reference builds it (rel_pos: row k encodes
+ *     position pe_len - 1 - k; abs_pos: position k), T_max = mb_ppgx_num_frames(h, n_max)
+ *   out fp32 [B][T_max][attention_dim] (device), zero past each row's frames;
+ *   taps fp32 [num_blocks + 1][B][T_max][attention_dim] or NULL: the embed output and each block's output */
+int mb_ppgx_forward(mb_ppgx* h, const float* wav, const int32_t* n_samples, int32_t batch, int32_t n_max, int32_t pe_len,
+                    const float* pos_table, float* out, float* taps, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

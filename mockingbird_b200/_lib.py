@@ -121,6 +121,14 @@ class Ppg2MelConfig(C.Structure):
                 ("num_mels", C.c_int32)]
 
 
+class PpgxConfig(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in (
+        "n_fft", "win_length", "hop_length", "n_mels", "kaldi_padding_mode", "downsample_rate", "norm_means", "norm_vars",
+        "attention_dim", "attention_heads", "linear_units", "num_blocks", "input_layer", "no_subsample", "subsample_by_2",
+        "normalize_before", "concat_after", "positionwise_layer_type", "macaron_style", "pos_enc_layer_type",
+        "selfattention_layer_type", "activation_type", "use_cnn_module", "cnn_module_kernel")]
+
+
 class MelSpecConfig(C.Structure):
     _fields_ = [("sample_rate", C.c_int32), ("n_fft", C.c_int32), ("hop_length", C.c_int32), ("win_length", C.c_int32),
                 ("n_mels", C.c_int32), ("fmin", C.c_float), ("fmax", C.c_float), ("pad_mode", C.c_int32),
@@ -234,6 +242,16 @@ SIGNATURES = {
     "mb_ppg2mel_inference": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32,
                                        C.c_int32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mb_ppgx_create": (C.c_int, [C.POINTER(PpgxConfig), C.POINTER(C.c_void_p)]),
+    "mb_ppgx_destroy": (None, [C.c_void_p]),
+    "mb_ppgx_arena_bytes": (C.c_size_t, [C.c_void_p]),
+    "mb_ppgx_set_arena": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "mb_ppgx_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int32, C.c_void_p]),
+    "mb_ppgx_finalize": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "mb_ppgx_num_frames": (C.c_int32, [C.c_void_p, C.c_int32]),
+    "mb_ppgx_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.c_int32]),
+    "mb_ppgx_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 _lib: Optional[C.CDLL] = None

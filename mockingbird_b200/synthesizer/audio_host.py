@@ -125,6 +125,26 @@ def mel_basis(sr: int, n_fft: int, n_mels: int, fmin: float, fmax: float) -> np.
     return (w * (2.0 / (mel_f[2:n_mels + 2] - mel_f[:n_mels]))[:, None]).astype(np.float32)
 
 
+def ppg_melmat(sr: int, n_fft: int, n_mels: int, fmin: float, fmax: float, norm=1) -> np.ndarray:
+    """``librosa.filters.mel(sr, n_fft, n_mels, fmin, fmax, norm=norm).T`` restated: [1 + n_fft // 2, n_mels], the
+    ``frontend.logmel.melmat`` buffer of the PPG extractor (models/ppg_extractor/log_mel.py:47-49).  The reference pins no
+    librosa version and ``norm=1`` changed meaning in librosa 0.8: before it, area ("slaney") normalisation; since, each
+    filter divided by its L1 norm.  ``norm=1`` here is the current meaning, ``norm="slaney"`` the old one."""
+    fftfreqs = np.linspace(0, sr / 2.0, 1 + n_fft // 2)
+    mel_f = _mel_to_hz(np.linspace(_hz_to_mel(fmin), _hz_to_mel(fmax), n_mels + 2))
+    fdiff = np.diff(mel_f)
+    ramps = mel_f[:, None] - fftfreqs[None, :]
+    w = np.maximum(0, np.minimum(-ramps[:-2] / fdiff[:-1, None], ramps[2:] / fdiff[1:, None])).astype(np.float32)
+    if norm == "slaney":
+        w = w * (2.0 / (mel_f[2:n_mels + 2] - mel_f[:n_mels]))[:, None].astype(np.float32)
+    elif norm == 1:
+        s = np.abs(w).astype(np.float64).sum(axis=1, keepdims=True)
+        w = np.where(s > np.finfo(np.float32).tiny, w / np.maximum(s, np.finfo(np.float32).tiny), w)
+    elif norm is not None:
+        raise ValueError(f"unsupported mel norm {norm!r}")
+    return np.ascontiguousarray(w.astype(np.float32).T)
+
+
 _inv_basis = {}
 
 

@@ -488,3 +488,128 @@ def ppg2mel_state_dict(seed: int = 0, randomize_bn: bool = True) -> Dict[str, to
                 elif k.endswith(".bias"):
                     sd[k] = torch.randn(sd[k].shape, generator=g2) * 0.2
     return sd
+
+
+# ---- PPG extractor (models/ppg_extractor/__init__.py:66-72: UtteranceMVN, DefaultFrontend, ConformerEncoder) ----------
+# The released extractor's yaml is not in the reference tree: a stand-in in the reference's `args` layout.  D = 144 is
+# ppg2mel's bottle_neck_feature_dim; 100 Hz frames without subsampling pair one to one with pyworld's 10 ms lf0_uv.
+PPGX_CONFIG = dict(
+    frontend_conf=dict(fs=16000, n_fft=400, win_length=400, hop_length=160, fmin=0, fmax=8000, n_mels=80),
+    normalize_conf=dict(norm_means=True, norm_vars=True),
+    encoder_conf=dict(attention_dim=144, attention_heads=4, linear_units=576, num_blocks=16, input_layer="conv2d",
+                      no_subsample=True, macaron_style=True, pos_enc_layer_type="rel_pos",
+                      selfattention_layer_type="rel_selfattn", activation_type="swish", use_cnn_module=True,
+                      cnn_module_kernel=15))
+
+
+def _ppgx_variant(base: dict, frontend=None, normalize=None, **enc) -> dict:
+    return dict(frontend_conf=dict(base["frontend_conf"], **(frontend or {})),
+                normalize_conf=dict(base["normalize_conf"], **(normalize or {})),
+                encoder_conf=dict(base["encoder_conf"], **enc))
+
+
+# test-only small config and variants reaching every supported option
+PPGX_CONFIG_SMALL = _ppgx_variant(PPGX_CONFIG, attention_dim=32, attention_heads=2, linear_units=64, num_blocks=2,
+                                  cnn_module_kernel=7)
+PPGX_SMALL_VARIANTS = {
+    "sub4": _ppgx_variant(PPGX_CONFIG_SMALL, no_subsample=False),
+    "sub2": _ppgx_variant(PPGX_CONFIG_SMALL, no_subsample=False, subsample_by_2=True),
+    "abs_pos": _ppgx_variant(PPGX_CONFIG_SMALL, pos_enc_layer_type="abs_pos", selfattention_layer_type="selfattn"),
+    "plain": _ppgx_variant(PPGX_CONFIG_SMALL, macaron_style=False, use_cnn_module=False, activation_type="relu"),
+    "no_vars": _ppgx_variant(PPGX_CONFIG_SMALL, normalize=dict(norm_vars=False)),
+    "fft512": _ppgx_variant(PPGX_CONFIG_SMALL, frontend=dict(n_fft=512, win_length=400)),
+    "vars_only": _ppgx_variant(PPGX_CONFIG_SMALL, normalize=dict(norm_means=False, norm_vars=True)),
+    # frontend_conf without the STFT keys: DefaultFrontend's defaults n_fft 1024, win_length 800, hop_length 160
+    "fe_defaults": dict(frontend_conf=dict(fs=16000, fmin=0, fmax=8000, n_mels=80),
+                        normalize_conf=dict(PPGX_CONFIG_SMALL["normalize_conf"]),
+                        encoder_conf=dict(PPGX_CONFIG_SMALL["encoder_conf"])),
+}
+
+
+def ppgx_frames(cfg: dict, n_samples: int) -> int:
+    """PPG frames of an n-sample utterance: 1 + n // hop STFT frames (center=True; DefaultFrontend's default hop is
+    160), halved by each stride-2 conv"""
+    t = 1 + n_samples // cfg["frontend_conf"].get("hop_length", 160)
+    enc = cfg["encoder_conf"]
+    if not enc.get("no_subsample", False):
+        t //= 2
+        if not enc.get("subsample_by_2", False):
+            t //= 2
+    return t
+
+
+def ppg_extractor_state_dict(cfg: dict, seed: int = 0, randomize_bn: bool = True) -> Dict[str, torch.Tensor]:
+    """``torch.manual_seed(seed); build_model(argparse.Namespace(**cfg)).state_dict()`` rebuilt from stock torch layers in
+    the constructor's order (encoder/conformer_encoder.py:80-200, subsampling.py, attention.py, convolution.py).  The
+    melmat buffer is the current librosa meaning of ``norm=1`` (mockingbird_b200.synthesizer.audio_host.ppg_melmat).
+    ``randomize_bn`` replaces the conv-module BatchNorm statistics and affines (identity in a fresh module) by seeded draws."""
+    import numpy as np
+
+    from mockingbird_b200.synthesizer.audio_host import ppg_melmat
+
+    nn = torch.nn
+    fe, enc = cfg["frontend_conf"], cfg["encoder_conf"]
+    D, H, U = enc["attention_dim"], enc["attention_heads"], enc["linear_units"]
+    n_mels = fe.get("n_mels", 80)
+    fs = fe["fs"]  # DefaultFrontend has no default for it
+    torch.manual_seed(seed)
+    sd: Dict[str, torch.Tensor] = {}
+
+    def put(name, m):
+        for n, p in m.state_dict().items():
+            sd[f"{name}.{n}"] = p.detach().clone()
+
+    mel = ppg_melmat(fs, fe.get("n_fft", 1024), n_mels, fe.get("fmin") or 0.0,
+                     fe["fmax"] if fe.get("fmax") is not None else fs / 2, norm=fe.get("norm", 1))
+    sd["frontend.logmel.melmat"] = torch.from_numpy(mel).float()
+    sd["frontend.logmel.inv_melmat"] = torch.from_numpy(np.linalg.pinv(mel.T).T).float()
+    if enc.get("no_subsample", False):
+        convs, f_out = [(1, 5, 1, 2), (D, 5, 1, 2)], n_mels
+    elif enc.get("subsample_by_2", False):
+        convs, f_out = [(1, 5, 1, 2), (D, 4, 2, 1)], n_mels // 2
+    else:
+        convs, f_out = [(1, 4, 2, 1), (D, 4, 2, 1)], n_mels // 4
+    for i, (cin, k, s, p) in zip((0, 2), convs):
+        put(f"encoder.embed.conv.{i}", nn.Conv2d(cin, D, k, s, p))
+    put("encoder.embed.out.0", nn.Linear(D * f_out, D))
+    rel = enc.get("selfattention_layer_type", "selfattn") == "rel_selfattn"
+    for b in range(enc["num_blocks"]):
+        pre = f"encoder.encoders.{b}"
+        att = {n: nn.Linear(D, D) for n in ("linear_q", "linear_k", "linear_v", "linear_out")}
+        if rel:
+            att["linear_pos"] = nn.Linear(D, D, bias=False)
+            u, v = torch.empty(H, D // H), torch.empty(H, D // H)
+            nn.init.xavier_uniform_(u)
+            nn.init.xavier_uniform_(v)
+            sd[f"{pre}.self_attn.pos_bias_u"], sd[f"{pre}.self_attn.pos_bias_v"] = u, v
+        for n, m in att.items():
+            put(f"{pre}.self_attn.{n}", m)
+        ffs = ["feed_forward"] + (["feed_forward_macaron"] if enc.get("macaron_style", False) else [])
+        for n in ffs:
+            put(f"{pre}.{n}.w_1", nn.Linear(D, U))
+            put(f"{pre}.{n}.w_2", nn.Linear(U, D))
+        cnn = enc.get("use_cnn_module", False)
+        if cnn:
+            K = enc.get("cnn_module_kernel", 31)
+            put(f"{pre}.conv_module.pointwise_conv1", nn.Conv1d(D, 2 * D, 1))
+            put(f"{pre}.conv_module.depthwise_conv", nn.Conv1d(D, D, K, padding=(K - 1) // 2, groups=D))
+            put(f"{pre}.conv_module.norm", nn.BatchNorm1d(D))
+            put(f"{pre}.conv_module.pointwise_conv2", nn.Conv1d(D, D, 1))
+        norms = ["norm_ff", "norm_mha"] + (["norm_ff_macaron"] if len(ffs) == 2 else []) + \
+            (["norm_conv", "norm_final"] if cnn else [])
+        for n in norms:
+            put(f"{pre}.{n}", nn.LayerNorm(D, eps=1e-12))
+    put("encoder.after_norm", nn.LayerNorm(D, eps=1e-12))
+    if randomize_bn:
+        g2 = torch.Generator().manual_seed(40_000 + seed)
+        for k in sorted(sd):
+            if ".conv_module.norm." in k:
+                if k.endswith(".running_var"):
+                    sd[k] = torch.rand(sd[k].shape, generator=g2) * 1.5 + 0.25
+                elif k.endswith(".running_mean"):
+                    sd[k] = torch.randn(sd[k].shape, generator=g2) * 0.3
+                elif k.endswith(".weight"):
+                    sd[k] = torch.rand(sd[k].shape, generator=g2) + 0.5
+                elif k.endswith(".bias"):
+                    sd[k] = torch.randn(sd[k].shape, generator=g2) * 0.2
+    return sd
