@@ -17,6 +17,12 @@
  *     stacks and the encoder's input projections - at the first use of a layer after any set_arena / set_weight (no
  *     cudaMalloc: the packers' scratch is a slot of the arena).  Exceptions (no device memory): mb_tacotron owns two
  *     streams and ten events (created at its first generate call), mb_mtstream its pinned host ring, a side stream and events.
+ *   - weights: mb_*_set_arena, then mb_*_set_weight once per checkpoint tensor, then mb_*_finalize.  A tensor is fp32,
+ *     contiguous, device-resident and has exactly its reference shape (a transposed or flattened tensor is refused).
+ *     Derived tensors (packed images, folded BatchNorm, scratch) are not settable.  set_arena forgets every tensor set
+ *     before it: finalize and the compute calls return MB_ERR_STATE until all are set again and finalized.  set_weight
+ *     reports argument errors (NULL pointers, unknown name, wrong shape: MB_ERR_INVALID) before call-order errors (no
+ *     arena: MB_ERR_STATE).
  *   - every launch goes to the cudaStream_t passed as `stream` (void* here so that the header
  *     needs no CUDA include); functions are asynchronous with respect to the host unless stated.
  *   - multi-GPU: the library links no communication library and has no global state.  The packed arena of every model
@@ -99,8 +105,7 @@ int mb_gan_set_arena(mb_gan* h, void* arena, size_t bytes);
 /* Feed one tensor of ckpt['generator'] (hifigan/inference.py:51) AFTER weight-norm folding
  * (w = g*v/||v||, models.py:152-162 - the host layer folds): name as in state_dict
  * ("conv_pre.weight", "ups.0.bias", "resblocks.3.convs1.0.weight", "cond_up.1.weight",
- * "res_output.0.1.weight" ...), fp32, contiguous, reference shape.  Packs into the arena on
- * `stream`.  */
+ * "res_output.0.1.weight" ...).  Packs into the arena on `stream`.  */
 int mb_gan_set_weight(mb_gan* h, const char* name, const float* w, const int64_t* dims, int32_t ndim,
                       void* stream);
 /* verifies that every tensor the config needs has been set */
@@ -197,8 +202,7 @@ int mb_wavernn_create(const mb_wavernn_config* cfg, mb_wavernn** out);
 void mb_wavernn_destroy(mb_wavernn* h);
 size_t mb_wavernn_arena_bytes(const mb_wavernn* h);
 int mb_wavernn_set_arena(mb_wavernn* h, void* arena, size_t bytes);
-/* tensors of ckpt['model_state'] (wavernn/inference.py:36-37), reference names and shapes
- * (SURVEY.md appendix B), fp32 */
+/* tensors of ckpt['model_state'] (wavernn/inference.py:36-37) under their reference names (SURVEY.md appendix B) */
 int mb_wavernn_set_weight(mb_wavernn* h, const char* name, const float* w, const int64_t* dims,
                           int32_t ndim, void* stream);
 int mb_wavernn_finalize(mb_wavernn* h, void* stream);
@@ -335,7 +339,7 @@ int mb_tacotron_create(const mb_tacotron_config* cfg, mb_tacotron** out);
 void mb_tacotron_destroy(mb_tacotron* h);
 size_t mb_tacotron_arena_bytes(const mb_tacotron* h);
 int mb_tacotron_set_arena(mb_tacotron* h, void* arena, size_t bytes);
-/* tensors of ckpt['model_state'] under their reference names (SURVEY.md appendix B), fp32, plus one
+/* tensors of ckpt['model_state'] under their reference names (SURVEY.md appendix B), plus one
  * derived tensor "gst.const_enc" [gst_E/2]: the GST ReferenceEncoder applied to the all-zero input of
  * tacotron.py:251 - input independent, folded at load time by the host layer */
 int mb_tacotron_set_weight(mb_tacotron* h, const char* name, const float* w, const int64_t* dims, int32_t ndim,

@@ -293,3 +293,30 @@ def require_cuda():
     if not torch.cuda.is_available():
         raise MbError("mockingbird_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
     return torch.device("cuda", torch.cuda.current_device())
+
+
+def upload_weights(model: str, handle, weights, device, align: int = 256):
+    """The weight protocol of a model handle: a zeroed arena of mb_<model>_arena_bytes aligned to `align`, set_arena,
+    set_weight for every tensor of `weights` (name -> tensor, already filtered to what the model takes), finalize, then a
+    synchronise.  Returns the arena as one uint8 device tensor (what multi-GPU start-up broadcasts)."""
+    import torch
+
+    L = lib()
+    nbytes = int(getattr(L, f"mb_{model}_arena_bytes")(handle))
+    with torch.cuda.device(device):
+        arena = torch.zeros(nbytes + align, dtype=torch.uint8, device=device)
+        base = (arena.data_ptr() + align - 1) // align * align
+        check(getattr(L, f"mb_{model}_set_arena")(handle, C.c_void_p(base), nbytes))
+        stream = torch.cuda.current_stream(device)
+        sp = C.c_void_p(stream.cuda_stream)
+        keep = []  # the copies are asynchronous: the converted tensors live until the synchronise
+        for name, t in weights.items():
+            d = t.to(device=device, dtype=torch.float32).contiguous()
+            keep.append(d)
+            dims = (C.c_int64 * max(1, d.dim()))(*d.shape)
+            check(getattr(L, f"mb_{model}_set_weight")(handle, name.encode(), C.c_void_p(d.data_ptr()), dims, d.dim(), sp))
+        finalize = getattr(L, f"mb_{model}_finalize")
+        # mb_gan_finalize only checks that every tensor was set (the GAN packs in set_weight): it takes no stream
+        check(finalize(handle) if len(finalize.argtypes) == 1 else finalize(handle, sp))
+        stream.synchronize()
+    return arena

@@ -312,36 +312,18 @@ __global__ void k_deepmind_pack(const float* __restrict__ R, const float* __rest
   }
 }
 
-struct Slot {
-  const char* name;
-  size_t n;
-  size_t off;
-  bool set;
-};
-
 }  // namespace
 }  // namespace mb
 
 using namespace mb;
 
 struct mb_deepmind {
-  std::vector<Slot> slots;
-  size_t raw_floats = 0;
+  WeightTable w;
   float* arena = nullptr;
   bool finalized = false;
 };
 
 namespace {
-const Slot kSlots[] = {{"R.weight", (size_t)3 * H * H, 0, false},      {"O1.weight", (size_t)S * S, 0, false}, {"O1.bias", S, 0, false},
-                       {"O2.weight", (size_t)Q * S, 0, false},          {"O2.bias", Q, 0, false},               {"O3.weight", (size_t)S * S, 0, false},
-                       {"O3.bias", S, 0, false},                        {"O4.weight", (size_t)Q * S, 0, false}, {"O4.bias", Q, 0, false},
-                       {"I_coarse.weight", (size_t)3 * S * 2, 0, false}, {"I_fine.weight", (size_t)3 * S * 3, 0, false},
-                       {"bias_u", H, 0, false},                         {"bias_r", H, 0, false},                {"bias_e", H, 0, false}};
-float* slot_ptr(mb_deepmind* h, const char* name) {
-  for (auto& s : h->slots)
-    if (!strcmp(s.name, name)) return h->arena + s.off;
-  return nullptr;
-}
 // workspace (floats): hidden [2][896] | x1 [448] | logits [512] | prev [2 ints] | barrier
 constexpr size_t WS_HIDDEN = 0, WS_X1 = 2 * H, WS_LOGITS = WS_X1 + S, WS_PREV = WS_LOGITS + 2 * Q, WS_BAR = WS_PREV + 64, WS_TOTAL = WS_BAR + 64;
 }  // namespace
@@ -353,55 +335,45 @@ int mb_deepmind_create(int32_t hidden_size, int32_t quantisation, mb_deepmind** 
   if (hidden_size != H || quantisation != Q)
     return fail(MB_ERR_INVALID, "mb_deepmind_create: only hidden_size=%d, quantisation=%d (the reference defaults) are built", H, Q);
   mb_deepmind* h = new mb_deepmind();
-  size_t off = 0;
-  for (const Slot& s : kSlots) {
-    Slot t = s;
-    t.off = off;
-    off += align_up(t.n, 64);
-    h->slots.push_back(t);
+  WeightTable& w = h->w;
+  w.add("R.weight", {3 * H, H});
+  for (const auto& o : {std::make_pair("O1", S), std::make_pair("O2", Q), std::make_pair("O3", S), std::make_pair("O4", Q)}) {
+    w.add(std::string(o.first) + ".weight", {o.second, S});
+    w.add(std::string(o.first) + ".bias", {o.second});
   }
-  h->raw_floats = off;
+  w.add("I_coarse.weight", {3 * S, 2});
+  w.add("I_fine.weight", {3 * S, 3});
+  for (const char* b : {"bias_u", "bias_r", "bias_e"}) w.add(b, {H});
   *out = h;
   return MB_OK;
 }
 
 void mb_deepmind_destroy(mb_deepmind* h) { delete h; }
 
-size_t mb_deepmind_arena_bytes(const mb_deepmind* h) { return h ? (h->raw_floats + (size_t)NCTA * WPACK) * sizeof(float) : 0; }
+size_t mb_deepmind_arena_bytes(const mb_deepmind* h) { return h ? (h->w.floats() + (size_t)NCTA * WPACK) * sizeof(float) : 0; }
 
 int mb_deepmind_set_arena(mb_deepmind* h, void* arena, size_t bytes) {
-  if (!h || !arena) return fail(MB_ERR_INVALID, "mb_deepmind_set_arena: null argument");
-  if (bytes < mb_deepmind_arena_bytes(h)) return fail(MB_ERR_WORKSPACE, "mb_deepmind_set_arena: arena too small");
-  if (((uintptr_t)arena & 255) != 0) return fail(MB_ERR_INVALID, "mb_deepmind_set_arena: arena must be 256-byte aligned");
+  if (int rc = check_arena("mb_deepmind_set_arena", h, arena, bytes, mb_deepmind_arena_bytes(h), 256)) return rc;
+  h->w.attach((float*)arena);
   h->arena = (float*)arena;
   h->finalized = false;
   return MB_OK;
 }
 
 int mb_deepmind_set_weight(mb_deepmind* h, const char* name, const float* w, const int64_t* dims, int32_t ndim, void* stream) {
-  if (!h || !name || !w || !dims) return fail(MB_ERR_INVALID, "mb_deepmind_set_weight: null argument");
-  if (!h->arena) return fail(MB_ERR_STATE, "mb_deepmind_set_weight: call mb_deepmind_set_arena first");
-  size_t n = 1;
-  for (int i = 0; i < ndim; ++i) n *= (size_t)dims[i];
-  for (auto& s : h->slots) {
-    if (strcmp(s.name, name)) continue;
-    if (n != s.n) return fail(MB_ERR_INVALID, "mb_deepmind_set_weight: %s has %zu elements, expected %zu", name, n, s.n);
-    MB_CUDA_CHECK(cudaMemcpyAsync(h->arena + s.off, w, n * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-    s.set = true;
-    h->finalized = false;
-    return MB_OK;
-  }
-  return fail(MB_ERR_INVALID, "mb_deepmind_set_weight: unknown tensor '%s'", name);
+  if (!h) return fail(MB_ERR_INVALID, "mb_deepmind_set_weight: null argument");
+  if (int rc = h->w.set("mb_deepmind_set_weight", name, w, dims, ndim, stream)) return rc;
+  h->finalized = false;
+  return MB_OK;
 }
 
 int mb_deepmind_finalize(mb_deepmind* h, void* stream) {
   if (!h || !h->arena) return fail(MB_ERR_STATE, "mb_deepmind_finalize: no arena");
-  for (auto& s : h->slots)
-    if (!s.set) return fail(MB_ERR_STATE, "mb_deepmind_finalize: tensor %s was never set", s.name);
+  if (int rc = h->w.check_all_set("mb_deepmind_finalize")) return rc;
   k_deepmind_pack<<<NCTA, 256, 0, (cudaStream_t)stream>>>(
-      slot_ptr(h, "R.weight"), slot_ptr(h, "O1.weight"), slot_ptr(h, "O1.bias"), slot_ptr(h, "O2.weight"), slot_ptr(h, "O2.bias"),
-      slot_ptr(h, "O3.weight"), slot_ptr(h, "O3.bias"), slot_ptr(h, "O4.weight"), slot_ptr(h, "O4.bias"), slot_ptr(h, "I_coarse.weight"),
-      slot_ptr(h, "I_fine.weight"), slot_ptr(h, "bias_u"), slot_ptr(h, "bias_r"), slot_ptr(h, "bias_e"), h->arena + h->raw_floats);
+      h->w.ptr("R.weight"), h->w.ptr("O1.weight"), h->w.ptr("O1.bias"), h->w.ptr("O2.weight"), h->w.ptr("O2.bias"),
+      h->w.ptr("O3.weight"), h->w.ptr("O3.bias"), h->w.ptr("O4.weight"), h->w.ptr("O4.bias"), h->w.ptr("I_coarse.weight"),
+      h->w.ptr("I_fine.weight"), h->w.ptr("bias_u"), h->w.ptr("bias_r"), h->w.ptr("bias_e"), h->arena + h->w.floats());
   MB_LAUNCH_CHECK("k_deepmind_pack");
   h->finalized = true;
   return MB_OK;
@@ -424,7 +396,7 @@ int mb_deepmind_generate(mb_deepmind* h, int32_t steps, int32_t step0, int32_t n
   MB_CUDA_CHECK(cudaMemsetAsync(ws + WS_BAR, 0, 256, st));
   DmParams p;
   memset(&p, 0, sizeof(p));
-  p.wpack = h->arena + h->raw_floats;
+  p.wpack = h->arena + h->w.floats();
   p.hidden = ws + WS_HIDDEN;
   p.x1 = ws + WS_X1;
   p.logits = ws + WS_LOGITS;

@@ -13,7 +13,6 @@
 // in the epilogue; h_t written as the next step's operand tiles); MB_ENC_TC=0 keeps the FFMA path.
 #include <cstdlib>
 #include <cstring>
-#include <map>
 #include <string>
 
 #include "../../include/mockingbird_b200.h"
@@ -25,13 +24,7 @@ using namespace mb::taco;
 
 struct mb_encoder {
   mb_encoder_config cfg{};
-  struct Slot {
-    size_t off, n;
-    bool set;
-  };
-  std::map<std::string, Slot> slots;
-  size_t total = 0;
-  float* arena = nullptr;
+  WeightTable w;
   bool finalized = false;
   float tc_inv_scale[8] = {1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f};
   float big_inv_scale[8] = {1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f};  // input-projection images (packed on first use)
@@ -40,15 +33,7 @@ struct mb_encoder {
 
 namespace {
 
-void slot(mb_encoder* h, const std::string& name, size_t n) {
-  h->slots[name] = {h->total, n, false};
-  h->total += align_up(n, 64);
-}
-
-float* P(const mb_encoder* h, const std::string& name) {
-  auto it = h->slots.find(name);
-  return it == h->slots.end() ? nullptr : h->arena + it->second.off;
-}
+float* P(const mb_encoder* h, const std::string& name) { return h->w.ptr(name); }
 
 #define TK(expr)                                                                                          \
   do {                                                                                                    \
@@ -181,54 +166,43 @@ int mb_encoder_create(const mb_encoder_config* cfg, mb_encoder** out) {
     return fail(MB_ERR_INVALID, "mb_encoder_create: unsupported hyper-parameters");
   mb_encoder* h = new mb_encoder();
   h->cfg = c;
-  const size_t H = c.hidden_size;
-  slot(h, "scratch.absmax.bias_sum", 64);  // device scratch of the weight-image packers (derived: no cudaMalloc after create)
+  const int H = c.hidden_size;
+  WeightTable& w = h->w;
+  w.add_derived("scratch.absmax.bias_sum", 64);  // device scratch of the weight-image packers (no cudaMalloc after create)
   for (int l = 0; l < c.num_layers; ++l) {
-    const size_t in = l == 0 ? c.mel_n_channels : H;
+    const int in = l == 0 ? c.mel_n_channels : H;
     const std::string s = std::to_string(l);
-    slot(h, "lstm.weight_ih_l" + s, 4 * H * in);
-    slot(h, "lstm.weight_hh_l" + s, 4 * H * H);
-    slot(h, "lstm.bias_ih_l" + s, 4 * H);
-    slot(h, "lstm.bias_hh_l" + s, 4 * H);
-    slot(h, "lstm.bias_sum_l" + s, 4 * H);  // derived: b_ih + b_hh
-    slot(h, "lstm.hh_tcw_l" + s, tc_gated_weight_bytes((int)H, (int)H) / 4);  // derived: tensor-core images of W_hh
-    slot(h, "lstm.hh_tcb_l" + s, 4 * H);                                      // (unused zero bias of the images)
-    slot(h, "lstm.ih_bigw_l" + s, tc_big_weight_bytes((int)(4 * H), 1, (int)in) / 4);  // derived: images of W_ih
+    w.add("lstm.weight_ih_l" + s, {4 * H, in});
+    w.add("lstm.weight_hh_l" + s, {4 * H, H});
+    w.add("lstm.bias_ih_l" + s, {4 * H});
+    w.add("lstm.bias_hh_l" + s, {4 * H});
+    w.add_derived("lstm.bias_sum_l" + s, 4 * H);                          // b_ih + b_hh
+    w.add_derived("lstm.hh_tcw_l" + s, tc_gated_weight_bytes(H, H) / 4);  // tensor-core images of W_hh
+    w.add_derived("lstm.hh_tcb_l" + s, 4 * H);                            // (unused zero bias of the images)
+    w.add_derived("lstm.ih_bigw_l" + s, tc_big_weight_bytes(4 * H, 1, in) / 4);  // images of W_ih
   }
-  slot(h, "linear.weight", (size_t)c.embedding_size * H);
-  slot(h, "linear.bias", c.embedding_size);
+  w.add("linear.weight", {c.embedding_size, H});
+  w.add("linear.bias", {c.embedding_size});
   *out = h;
   return MB_OK;
 }
 
 void mb_encoder_destroy(mb_encoder* h) { delete h; }
 
-size_t mb_encoder_arena_bytes(const mb_encoder* h) { return h ? h->total * sizeof(float) : 0; }
+size_t mb_encoder_arena_bytes(const mb_encoder* h) { return h ? h->w.floats() * sizeof(float) : 0; }
 
 int mb_encoder_set_arena(mb_encoder* h, void* arena, size_t bytes) {
-  if (!h || !arena) return fail(MB_ERR_INVALID, "mb_encoder_set_arena: null argument");
-  if (bytes < mb_encoder_arena_bytes(h)) return fail(MB_ERR_WORKSPACE, "mb_encoder_set_arena: arena too small");
-  if (((uintptr_t)arena & 255) != 0) return fail(MB_ERR_INVALID, "mb_encoder_set_arena: arena must be 256-byte aligned");
-  h->arena = (float*)arena;
-  for (bool& b : h->big_packed) b = false;  // a new arena holds none of the lazily packed images
+  if (int rc = check_arena("mb_encoder_set_arena", h, arena, bytes, mb_encoder_arena_bytes(h), 256)) return rc;
+  h->w.attach((float*)arena);
   h->finalized = false;
+  for (bool& b : h->big_packed) b = false;  // a new arena holds none of the lazily packed images
   return MB_OK;
 }
 
 int mb_encoder_set_weight(mb_encoder* h, const char* name, const float* w, const int64_t* dims, int32_t ndim,
                           void* stream) {
-  if (!h || !name || !w) return fail(MB_ERR_INVALID, "mb_encoder_set_weight: null argument");
-  if (!h->arena) return fail(MB_ERR_STATE, "mb_encoder_set_weight: call mb_encoder_set_arena first");
-  auto it = h->slots.find(name);
-  if (it == h->slots.end() || std::string(name).find("bias_sum") != std::string::npos ||
-      std::string(name).find("hh_tc") != std::string::npos || std::string(name).find("ih_bigw") != std::string::npos)
-    return fail(MB_ERR_INVALID, "mb_encoder_set_weight: unknown tensor '%s'", name);
-  size_t n = 1;
-  for (int i = 0; i < ndim; ++i) n *= (size_t)dims[i];
-  if (n != it->second.n)
-    return fail(MB_ERR_INVALID, "mb_encoder_set_weight: %s has %zu elements, expected %zu", name, n, it->second.n);
-  MB_CUDA_CHECK(cudaMemcpyAsync(h->arena + it->second.off, w, n * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  it->second.set = true;
+  if (!h) return fail(MB_ERR_INVALID, "mb_encoder_set_weight: null argument");
+  if (int rc = h->w.set("mb_encoder_set_weight", name, w, dims, ndim, stream)) return rc;
   h->finalized = false;
   for (bool& b : h->big_packed) b = false;  // images packed from the previous weights are stale
   return MB_OK;
@@ -237,10 +211,7 @@ int mb_encoder_set_weight(mb_encoder* h, const char* name, const float* w, const
 int mb_encoder_finalize(mb_encoder* h, void* stream) {
   if (!h) return fail(MB_ERR_INVALID, "mb_encoder_finalize: null handle");
   cudaStream_t st = (cudaStream_t)stream;
-  for (auto& kv : h->slots)
-    if (!kv.second.set && kv.first.find("bias_sum") == std::string::npos && kv.first.find("hh_tc") == std::string::npos &&
-        kv.first.find("ih_bigw") == std::string::npos)
-      return fail(MB_ERR_STATE, "mb_encoder_finalize: tensor %s was never set", kv.first.c_str());
+  if (int rc = h->w.check_all_set("mb_encoder_finalize")) return rc;
   const int n = 4 * h->cfg.hidden_size;
   for (int l = 0; l < h->cfg.num_layers; ++l) {
     const std::string s = std::to_string(l);

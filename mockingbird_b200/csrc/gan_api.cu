@@ -538,18 +538,16 @@ size_t mb_gan_arena_bytes(const mb_gan* h) {
 }
 
 int mb_gan_set_arena(mb_gan* h, void* arena, size_t bytes) {
-  if (!h || !arena) return fail(MB_ERR_INVALID, "mb_gan_set_arena: null argument");
-  if (bytes < mb_gan_arena_bytes(h)) return fail(MB_ERR_WORKSPACE, "mb_gan_set_arena: need %zu bytes, got %zu",
-                                                 mb_gan_arena_bytes(h), bytes);
-  if (((uintptr_t)arena & 255) != 0) return fail(MB_ERR_INVALID, "mb_gan_set_arena: arena must be 256-byte aligned");
+  if (int rc = check_arena("mb_gan_set_arena", h, arena, bytes, mb_gan_arena_bytes(h), 256)) return rc;
   h->arena = (float*)arena;
   h->arena_bytes = bytes;
+  h->finalized = false;
+  for (Layer& L : h->layers) L.w_set = L.b_set = false;  // a new arena holds none of the packed layers
   return MB_OK;
 }
 
 int mb_gan_set_weight(mb_gan* h, const char* name, const float* w, const int64_t* dims, int32_t ndim, void* stream) {
   if (!h || !name || !w || !dims) return fail(MB_ERR_INVALID, "mb_gan_set_weight: null argument");
-  if (!h->arena) return fail(MB_ERR_STATE, "mb_gan_set_weight: call mb_gan_set_arena first");
   cudaStream_t st = (cudaStream_t)stream;
   const std::string n(name);
   const size_t dot = n.rfind('.');
@@ -560,6 +558,7 @@ int mb_gan_set_weight(mb_gan* h, const char* name, const float* w, const int64_t
     if (leaf == "bias") {
       if (ndim != 1 || dims[0] != L.cout_w)
         return fail(MB_ERR_INVALID, "mb_gan_set_weight: %s expects [%d]", name, L.cout_w);
+      if (!h->arena) return fail(MB_ERR_STATE, "mb_gan_set_weight: call mb_gan_set_arena first");
       if (L.cout != L.cout_w) MB_CUDA_CHECK(cudaMemsetAsync(h->arena + L.b_off, 0, sizeof(float) * L.cout, st));
       MB_CUDA_CHECK(cudaMemcpyAsync(h->arena + L.b_off, w, sizeof(float) * L.cout_w, cudaMemcpyDeviceToDevice, st));
       L.b_set = true;
@@ -570,6 +569,7 @@ int mb_gan_set_weight(mb_gan* h, const char* name, const float* w, const int64_t
       if (ndim != 3 || dims[0] != d0 || dims[1] != d1 || dims[2] != L.k)
         return fail(MB_ERR_INVALID, "mb_gan_set_weight: %s expects [%lld,%lld,%d]", name, (long long)d0,
                     (long long)d1, L.k);
+      if (!h->arena) return fail(MB_ERR_STATE, "mb_gan_set_weight: call mb_gan_set_arena first");
       cudaError_t e = L.nearest > 1
                           ? launch_fold_slabs_f32(w, h->arena + L.w_off, L.cout_w, L.cin_w, L.k, L.fold, L.cout, L.cin, st)
                           : launch_pack_slabs_f32(w, h->arena + L.w_off, L.cout_w, L.cin_w, L.k, L.transposed, st, L.cout, L.cin);

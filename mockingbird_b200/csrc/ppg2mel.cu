@@ -22,7 +22,9 @@
 #include "../../include/mb_wavernn_math.h"
 #include "mb_common.h"
 
+using mb::check_arena;
 using mb::fail;
+using mb::WeightTable;
 
 namespace {
 
@@ -522,87 +524,62 @@ __global__ void add_kernel(const float* a, const float* b, float* dst, int n) {
   if (i < n) dst[i] = a[i] + b[i];
 }
 
-// ---------------------------------------------------------------------------------------------- weights
-struct WeightSpec {
-  std::string name;
-  std::vector<int64_t> dims;
-  size_t off = 0;  // floats into the arena
-  bool set = false;
-};
-
 }  // namespace
 
 struct mb_ppg2mel {
   mb_ppg2mel_config cfg{};
-  std::vector<WeightSpec> w;
-  size_t derived_off = 0, total_floats = 0;
+  WeightTable w;
+  size_t total_floats = 0;
   size_t d_w1t = 0, d_w2t = 0, d_att_b = 0, d_dec_b = 0;
   float* arena = nullptr;
   bool finalized = false;
   cudaStream_t st = nullptr;
   cudaEvent_t ev_in = nullptr, ev_out = nullptr;
 
-  const float* p(const char* name) const {
-    for (const auto& s : w)
-      if (s.name == name) return arena + s.off;
-    return nullptr;
-  }
+  const float* p(const std::string& name) const { return w.ptr(name); }
 };
 
 namespace {
-
-void add_spec(mb_ppg2mel* h, const std::string& name, std::vector<int64_t> dims) {
-  WeightSpec s;
-  s.name = name;
-  s.dims = std::move(dims);
-  h->w.push_back(s);
-}
 
 void build_specs(mb_ppg2mel* h) {
   const int D = h->cfg.bottle_neck_feature_dim, Ds = h->cfg.spk_embed_dim;
   for (const char* br : {"bnf_prenet", "pitch_convs"}) {
     const std::string b = br;
-    add_spec(h, b + ".0.weight", {kE, b == "bnf_prenet" ? D : 2, 1});
+    h->w.add(b + ".0.weight", {kE, b == "bnf_prenet" ? D : 2, 1});
     for (const char* i : {".3", ".6"}) {
-      add_spec(h, b + i + ".weight", {kE, kE, 4});
-      add_spec(h, b + i + ".bias", {kE});
+      h->w.add(b + i + ".weight", {kE, kE, 4});
+      h->w.add(b + i + ".bias", {kE});
     }
   }
-  add_spec(h, "reduce_proj.weight", {kE, kE + Ds});
-  add_spec(h, "reduce_proj.bias", {kE});
-  add_spec(h, "decoder.prenet.layers.0.linear_layer.weight", {kP1, kNM});
-  add_spec(h, "decoder.prenet.layers.1.linear_layer.weight", {kP2, kP1});
+  h->w.add("reduce_proj.weight", {kE, kE + Ds});
+  h->w.add("reduce_proj.bias", {kE});
+  h->w.add("decoder.prenet.layers.0.linear_layer.weight", {kP1, kNM});
+  h->w.add("decoder.prenet.layers.1.linear_layer.weight", {kP2, kP1});
   for (const auto& pr : {std::make_pair("decoder.attention_rnn", kP2 + kE),
                          std::make_pair("decoder.decoder_rnn_layers.0", kH + kE)}) {
     const std::string b = pr.first;
-    add_spec(h, b + ".weight_ih", {4 * kH, pr.second});
-    add_spec(h, b + ".weight_hh", {4 * kH, kH});
-    add_spec(h, b + ".bias_ih", {4 * kH});
-    add_spec(h, b + ".bias_hh", {4 * kH});
+    h->w.add(b + ".weight_ih", {4 * kH, pr.second});
+    h->w.add(b + ".weight_hh", {4 * kH, kH});
+    h->w.add(b + ".bias_ih", {4 * kH});
+    h->w.add(b + ".bias_hh", {4 * kH});
   }
-  add_spec(h, "decoder.attention_layer.query_layer.0.weight", {kQ, kH});
-  add_spec(h, "decoder.attention_layer.query_layer.0.bias", {kQ});
-  add_spec(h, "decoder.attention_layer.query_layer.2.weight", {3 * kM, kQ});
-  add_spec(h, "decoder.attention_layer.query_layer.2.bias", {3 * kM});
-  add_spec(h, "decoder.linear_projection.linear_layer.weight", {kNM * kR, kH + kE});
-  add_spec(h, "decoder.linear_projection.linear_layer.bias", {kNM * kR});
-  add_spec(h, "decoder.stop_layer.linear_layer.weight", {1, kH + kE});
-  add_spec(h, "decoder.stop_layer.linear_layer.bias", {1});
+  h->w.add("decoder.attention_layer.query_layer.0.weight", {kQ, kH});
+  h->w.add("decoder.attention_layer.query_layer.0.bias", {kQ});
+  h->w.add("decoder.attention_layer.query_layer.2.weight", {3 * kM, kQ});
+  h->w.add("decoder.attention_layer.query_layer.2.bias", {3 * kM});
+  h->w.add("decoder.linear_projection.linear_layer.weight", {kNM * kR, kH + kE});
+  h->w.add("decoder.linear_projection.linear_layer.bias", {kNM * kR});
+  h->w.add("decoder.stop_layer.linear_layer.weight", {1, kH + kE});
+  h->w.add("decoder.stop_layer.linear_layer.bias", {1});
   const int ch[6] = {kNM, 512, 512, 512, 512, kNM};
   for (int i = 0; i < 5; ++i) {
     const std::string b = "postnet.convolutions." + std::to_string(i);
-    add_spec(h, b + ".0.conv.weight", {ch[i + 1], ch[i], 5});
-    add_spec(h, b + ".0.conv.bias", {ch[i + 1]});
-    for (const char* leaf : {".1.weight", ".1.bias", ".1.running_mean", ".1.running_var"}) add_spec(h, b + leaf, {ch[i + 1]});
+    h->w.add(b + ".0.conv.weight", {ch[i + 1], ch[i], 5});
+    h->w.add(b + ".0.conv.bias", {ch[i + 1]});
+    for (const char* leaf : {".1.weight", ".1.bias", ".1.running_mean", ".1.running_var"}) h->w.add(b + leaf, {ch[i + 1]});
   }
-  size_t off = 0;
-  for (auto& s : h->w) {
-    s.off = off;
-    size_t n = 1;
-    for (auto d : s.dims) n *= (size_t)d;
-    off += mb::align_up(n, 64);
-  }
-  h->derived_off = off;
+  // the model's own derived region follows the table
+  size_t off = h->w.floats();
   h->d_w1t = off;
   off += mb::align_up((size_t)kNM * kP1, 64);
   h->d_w2t = off;
@@ -712,6 +689,9 @@ int mb_ppg2mel_create(const mb_ppg2mel_config* cfg, mb_ppg2mel** out) {
   auto* h = new mb_ppg2mel();
   h->cfg = c;
   build_specs(h);
+  h->w.ignored = [](const std::string& n) {  // in the checkpoint, never read by inference
+    return n.rfind("decoder.prenet_pitch.", 0) == 0 || n.find("num_batches_tracked") != std::string::npos;
+  };
   *out = h;
   return MB_OK;
 }
@@ -727,43 +707,24 @@ void mb_ppg2mel_destroy(mb_ppg2mel* h) {
 size_t mb_ppg2mel_arena_bytes(const mb_ppg2mel* h) { return h ? h->total_floats * sizeof(float) : 0; }
 
 int mb_ppg2mel_set_arena(mb_ppg2mel* h, void* arena, size_t bytes) {
-  if (!h || !arena) return fail(MB_ERR_INVALID, "mb_ppg2mel_set_arena: null argument");
-  if (bytes < mb_ppg2mel_arena_bytes(h)) return fail(MB_ERR_WORKSPACE, "mb_ppg2mel_set_arena: arena too small");
-  if (reinterpret_cast<uintptr_t>(arena) % 256) return fail(MB_ERR_INVALID, "mb_ppg2mel_set_arena: arena not 256-aligned");
+  if (int rc = check_arena("mb_ppg2mel_set_arena", h, arena, bytes, mb_ppg2mel_arena_bytes(h), 256)) return rc;
+  h->w.attach(static_cast<float*>(arena));
   h->arena = static_cast<float*>(arena);
   h->finalized = false;
-  for (auto& s : h->w) s.set = false;
   return MB_OK;
 }
 
 int mb_ppg2mel_set_weight(mb_ppg2mel* h, const char* name, const float* w, const int64_t* dims, int32_t ndim,
                           void* stream) {
-  if (!h || !name || !w || (!dims && ndim > 0)) return fail(MB_ERR_INVALID, "mb_ppg2mel_set_weight: null argument");
-  if (!h->arena) return fail(MB_ERR_STATE, "mb_ppg2mel_set_weight: set_arena first");
-  const std::string n = name;
-  if (n.rfind("decoder.prenet_pitch.", 0) == 0 || n.find("num_batches_tracked") != std::string::npos)
-    return MB_OK;  // in the checkpoint, never read by inference
-  for (auto& s : h->w) {
-    if (s.name != n) continue;
-    bool ok = (int)s.dims.size() == ndim;
-    for (int i = 0; ok && i < ndim; ++i) ok = s.dims[i] == dims[i];
-    if (!ok) return fail(MB_ERR_INVALID, "mb_ppg2mel_set_weight: %s has the wrong shape", name);
-    size_t cnt = 1;
-    for (auto d : s.dims) cnt *= (size_t)d;
-    MB_CUDA_CHECK(cudaMemcpyAsync(h->arena + s.off, w, cnt * sizeof(float), cudaMemcpyDeviceToDevice,
-                                  static_cast<cudaStream_t>(stream)));
-    s.set = true;
-    h->finalized = false;
-    return MB_OK;
-  }
-  return fail(MB_ERR_INVALID, "mb_ppg2mel_set_weight: unknown weight %s", name);
+  if (!h) return fail(MB_ERR_INVALID, "mb_ppg2mel_set_weight: null argument");
+  if (int rc = h->w.set("mb_ppg2mel_set_weight", name, w, dims, ndim, stream)) return rc;
+  h->finalized = false;
+  return MB_OK;
 }
 
 int mb_ppg2mel_finalize(mb_ppg2mel* h, void* stream) {
   if (!h) return fail(MB_ERR_INVALID, "mb_ppg2mel_finalize: null handle");
-  if (!h->arena) return fail(MB_ERR_STATE, "mb_ppg2mel_finalize: set_arena first");
-  for (const auto& s : h->w)
-    if (!s.set) return fail(MB_ERR_STATE, "mb_ppg2mel_finalize: weight %s was never set", s.name.c_str());
+  if (int rc = h->w.check_all_set("mb_ppg2mel_finalize")) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   float* A = h->arena;
   transpose_kernel<<<(kP1 * kNM + 255) / 256, 256, 0, st>>>(h->p("decoder.prenet.layers.0.linear_layer.weight"),

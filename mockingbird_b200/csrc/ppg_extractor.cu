@@ -395,13 +395,6 @@ __global__ void __launch_bounds__(128) attn_kernel(const float* __restrict__ qkv
 }
 
 // ---------------------------------------------------------------------------------------------- weights
-struct WeightSpec {
-  std::string name;
-  std::vector<int64_t> dims;
-  size_t off = 0;  // floats into the arena
-  bool set = false;
-};
-
 // one tensor-core GEMM: packed weight image + the fp32 sources it is packed from
 struct Gemm {
   std::vector<std::string> w;  // row blocks concatenated along N (QKV, linear_pos of all blocks)
@@ -428,7 +421,7 @@ struct mb_ppgx {
   int D = 0, H = 0, dk = 0, U = 0, nb = 0, F = 0, n_freq = 0;
   int k0 = 5, s0 = 1, p0 = 2, k2 = 5, s2 = 1, p2 = 2, F1 = 0, F2 = 0;
   bool rel = false;
-  std::vector<WeightSpec> w;
+  WeightTable w;
   std::vector<Gemm> g;     // [0] embed.out, [1] linear_pos (rel), then per block: qkv, out, (mac w1, mac w2), w1, w2, (pw1, pw2)
   int g_pos = -1;
   std::vector<int> g_block;  // first GEMM of each block
@@ -441,11 +434,7 @@ struct mb_ppgx {
   const float *melmat = nullptr, *conv0_w = nullptr, *conv0_b = nullptr, *conv2_b = nullptr, *after_w = nullptr,
               *after_b = nullptr;
 
-  const float* p(const std::string& name) const {
-    for (const auto& s : w)
-      if (s.name == name) return reinterpret_cast<const float*>(arena) + s.off;
-    return nullptr;
-  }
+  const float* p(const std::string& name) const { return w.ptr(name); }
   float* fl(size_t off) const { return reinterpret_cast<float*>(arena) + off; }
   int frames_stft(int n) const { return 1 + n / cfg.hop_length; }
   // torch's conv output length floor((L + 2p - k) / s) + 1, with a floor (not truncating) division
@@ -459,25 +448,18 @@ struct mb_ppgx {
 
 namespace {
 
-void add_spec(mb_ppgx* h, const std::string& name, std::vector<int64_t> dims) {
-  WeightSpec s;
-  s.name = name;
-  s.dims = std::move(dims);
-  h->w.push_back(s);
-}
-
 int kb_of(int K) { return (K + 63) / 64; }
 size_t ceil128(size_t m) { return (m + 127) / 128 * 128; }
 
 void build_specs(mb_ppgx* h) {
   const int D = h->D, U = h->U;
-  add_spec(h, "frontend.logmel.melmat", {h->n_freq, h->F});
-  add_spec(h, "encoder.embed.conv.0.weight", {D, 1, h->k0, h->k0});
-  add_spec(h, "encoder.embed.conv.0.bias", {D});
-  add_spec(h, "encoder.embed.conv.2.weight", {D, D, h->k2, h->k2});
-  add_spec(h, "encoder.embed.conv.2.bias", {D});
-  add_spec(h, "encoder.embed.out.0.weight", {D, (int64_t)D * h->F2});
-  add_spec(h, "encoder.embed.out.0.bias", {D});
+  h->w.add("frontend.logmel.melmat", {h->n_freq, h->F});
+  h->w.add("encoder.embed.conv.0.weight", {D, 1, h->k0, h->k0});
+  h->w.add("encoder.embed.conv.0.bias", {D});
+  h->w.add("encoder.embed.conv.2.weight", {D, D, h->k2, h->k2});
+  h->w.add("encoder.embed.conv.2.bias", {D});
+  h->w.add("encoder.embed.out.0.weight", {D, (int64_t)D * h->F2});
+  h->w.add("encoder.embed.out.0.bias", {D});
   Gemm ge;
   ge.w = {"encoder.embed.out.0.weight"};
   ge.b = {"encoder.embed.out.0.bias"};
@@ -494,31 +476,31 @@ void build_specs(mb_ppgx* h) {
   for (int i = 0; i < h->nb; ++i) {
     const std::string b = "encoder.encoders." + std::to_string(i) + ".";
     for (const char* n : {"linear_q", "linear_k", "linear_v", "linear_out"}) {
-      add_spec(h, b + "self_attn." + n + ".weight", {D, D});
-      add_spec(h, b + "self_attn." + n + ".bias", {D});
+      h->w.add(b + "self_attn." + n + ".weight", {D, D});
+      h->w.add(b + "self_attn." + n + ".bias", {D});
     }
     if (h->rel) {
-      add_spec(h, b + "self_attn.linear_pos.weight", {D, D});
-      add_spec(h, b + "self_attn.pos_bias_u", {h->H, h->dk});
-      add_spec(h, b + "self_attn.pos_bias_v", {h->H, h->dk});
+      h->w.add(b + "self_attn.linear_pos.weight", {D, D});
+      h->w.add(b + "self_attn.pos_bias_u", {h->H, h->dk});
+      h->w.add(b + "self_attn.pos_bias_v", {h->H, h->dk});
     }
     std::vector<std::string> ffs = {"feed_forward"};
     if (mac) ffs.push_back("feed_forward_macaron");
     for (const auto& f : ffs) {
-      add_spec(h, b + f + ".w_1.weight", {U, D});
-      add_spec(h, b + f + ".w_1.bias", {U});
-      add_spec(h, b + f + ".w_2.weight", {D, U});
-      add_spec(h, b + f + ".w_2.bias", {D});
+      h->w.add(b + f + ".w_1.weight", {U, D});
+      h->w.add(b + f + ".w_1.bias", {U});
+      h->w.add(b + f + ".w_2.weight", {D, U});
+      h->w.add(b + f + ".w_2.bias", {D});
     }
     if (cnn) {
       const std::string c = b + "conv_module.";
-      add_spec(h, c + "pointwise_conv1.weight", {2 * D, D, 1});
-      add_spec(h, c + "pointwise_conv1.bias", {2 * D});
-      add_spec(h, c + "depthwise_conv.weight", {D, 1, h->cfg.cnn_module_kernel});
-      add_spec(h, c + "depthwise_conv.bias", {D});
-      for (const char* n : {"weight", "bias", "running_mean", "running_var"}) add_spec(h, c + "norm." + n, {D});
-      add_spec(h, c + "pointwise_conv2.weight", {D, D, 1});
-      add_spec(h, c + "pointwise_conv2.bias", {D});
+      h->w.add(c + "pointwise_conv1.weight", {2 * D, D, 1});
+      h->w.add(c + "pointwise_conv1.bias", {2 * D});
+      h->w.add(c + "depthwise_conv.weight", {D, 1, h->cfg.cnn_module_kernel});
+      h->w.add(c + "depthwise_conv.bias", {D});
+      for (const char* n : {"weight", "bias", "running_mean", "running_var"}) h->w.add(c + "norm." + n, {D});
+      h->w.add(c + "pointwise_conv2.weight", {D, D, 1});
+      h->w.add(c + "pointwise_conv2.bias", {D});
     }
     std::vector<std::string> norms = {"norm_ff", "norm_mha"};
     if (mac) norms.push_back("norm_ff_macaron");
@@ -527,8 +509,8 @@ void build_specs(mb_ppgx* h) {
       norms.push_back("norm_final");
     }
     for (const auto& n : norms) {
-      add_spec(h, b + n + ".weight", {D});
-      add_spec(h, b + n + ".bias", {D});
+      h->w.add(b + n + ".weight", {D});
+      h->w.add(b + n + ".bias", {D});
     }
     h->g_block.push_back((int)h->g.size());
     Gemm q;
@@ -565,15 +547,9 @@ void build_specs(mb_ppgx* h) {
       h->g.push_back(c2);
     }
   }
-  add_spec(h, "encoder.after_norm.weight", {D});
-  add_spec(h, "encoder.after_norm.bias", {D});
-  size_t off = 0;
-  for (auto& s : h->w) {
-    s.off = off;
-    size_t n = 1;
-    for (auto d : s.dims) n *= (size_t)d;
-    off += mb::align_up(n, 64);
-  }
+  h->w.add("encoder.after_norm.weight", {D});
+  h->w.add("encoder.after_norm.bias", {D});
+  size_t off = h->w.floats();  // the model's own derived regions follow the table
   for (auto& gm : h->g) {
     if (gm.w.size() > 1) {
       gm.w_cat = off;
@@ -768,6 +744,9 @@ int mb_ppgx_create(const mb_ppgx_config* cfg, mb_ppgx** out) {
   h->F1 = (h->F + 2 * h->p0 - h->k0) / h->s0 + 1;
   h->F2 = (h->F1 + 2 * h->p2 - h->k2) / h->s2 + 1;
   build_specs(h);
+  h->w.ignored = [](const std::string& n) {  // in the checkpoint, never read by inference
+    return n == "frontend.logmel.inv_melmat" || n.find("num_batches_tracked") != std::string::npos;
+  };
   *out = h;
   return MB_OK;
 }
@@ -777,41 +756,23 @@ void mb_ppgx_destroy(mb_ppgx* h) { delete h; }
 size_t mb_ppgx_arena_bytes(const mb_ppgx* h) { return h ? h->total_bytes : 0; }
 
 int mb_ppgx_set_arena(mb_ppgx* h, void* arena, size_t bytes) {
-  if (!h || !arena) return fail(MB_ERR_INVALID, "mb_ppgx_set_arena: null argument");
-  if (bytes < h->total_bytes) return fail(MB_ERR_WORKSPACE, "mb_ppgx_set_arena: arena too small");
-  if (reinterpret_cast<uintptr_t>(arena) % 1024) return fail(MB_ERR_INVALID, "mb_ppgx_set_arena: arena not 1024-aligned");
+  if (int rc = check_arena("mb_ppgx_set_arena", h, arena, bytes, mb_ppgx_arena_bytes(h), 1024)) return rc;
+  h->w.attach(static_cast<float*>(arena));
   h->arena = static_cast<char*>(arena);
   h->finalized = false;
-  for (auto& s : h->w) s.set = false;
   return MB_OK;
 }
 
 int mb_ppgx_set_weight(mb_ppgx* h, const char* name, const float* w, const int64_t* dims, int32_t ndim, void* stream) {
-  if (!h || !name || !w || (!dims && ndim > 0)) return fail(MB_ERR_INVALID, "mb_ppgx_set_weight: null argument");
-  if (!h->arena) return fail(MB_ERR_STATE, "mb_ppgx_set_weight: set_arena first");
-  const std::string n = name;
-  if (n == "frontend.logmel.inv_melmat" || n.find("num_batches_tracked") != std::string::npos) return MB_OK;
-  for (auto& s : h->w) {
-    if (s.name != n) continue;
-    bool ok = (int)s.dims.size() == ndim;
-    for (int i = 0; ok && i < ndim; ++i) ok = s.dims[i] == dims[i];
-    if (!ok) return fail(MB_ERR_INVALID, "mb_ppgx_set_weight: %s has the wrong shape", name);
-    size_t cnt = 1;
-    for (auto d : s.dims) cnt *= (size_t)d;
-    MB_CUDA_CHECK(cudaMemcpyAsync(h->fl(s.off), w, cnt * sizeof(float), cudaMemcpyDeviceToDevice,
-                                  static_cast<cudaStream_t>(stream)));
-    s.set = true;
-    h->finalized = false;
-    return MB_OK;
-  }
-  return fail(MB_ERR_INVALID, "mb_ppgx_set_weight: unknown weight %s", name);
+  if (!h) return fail(MB_ERR_INVALID, "mb_ppgx_set_weight: null argument");
+  if (int rc = h->w.set("mb_ppgx_set_weight", name, w, dims, ndim, stream)) return rc;
+  h->finalized = false;
+  return MB_OK;
 }
 
 int mb_ppgx_finalize(mb_ppgx* h, void* stream) {
   if (!h) return fail(MB_ERR_INVALID, "mb_ppgx_finalize: null handle");
-  if (!h->arena) return fail(MB_ERR_STATE, "mb_ppgx_finalize: set_arena first");
-  for (const auto& s : h->w)
-    if (!s.set) return fail(MB_ERR_STATE, "mb_ppgx_finalize: weight %s was never set", s.name.c_str());
+  if (int rc = h->w.check_all_set("mb_ppgx_finalize")) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   // concatenations (QKV, linear_pos of all blocks) and their biases
   for (auto& gm : h->g) {

@@ -380,14 +380,7 @@ using namespace mb::taco;
 
 struct mb_tacotron {
   mb_tacotron_config cfg{};
-  struct Slot {
-    size_t off;
-    size_t n;
-    bool set;
-  };
-  std::map<std::string, Slot> slots;
-  size_t total = 0;
-  float* arena = nullptr;
+  WeightTable w;
   bool finalized = false;
   int packed_r = 0;
   std::map<std::string, float> tc_inv_scale;  // tensor-core weight images: 1 / pack scale per tensor
@@ -403,51 +396,44 @@ struct mb_tacotron {
 
 namespace {
 
-void slot(mb_tacotron* h, const std::string& name, size_t n) {
-  h->slots[name] = {h->total, n, false};
-  h->total += align_up(n, 64);
-}
+float* P(const mb_tacotron* h, const std::string& name) { return h->w.ptr(name); }
 
-float* P(const mb_tacotron* h, const std::string& name) {
-  auto it = h->slots.find(name);
-  return it == h->slots.end() ? nullptr : h->arena + it->second.off;
-}
-
-void cbhg_slots(mb_tacotron* h, const std::string& p, int K, int cin, int ch, int p0, int p1, int nh) {
+void cbhg_slots(WeightTable& w, const std::string& p, int K, int cin, int ch, int p0, int p1, int nh) {
   auto bnconv = [&](const std::string& n, int ci, int co, int k) {
-    slot(h, n + ".conv.weight", (size_t)co * ci * k);
-    for (const char* leaf : {".bnorm.weight", ".bnorm.bias", ".bnorm.running_mean", ".bnorm.running_var"}) slot(h, n + leaf, co);
-    slot(h, n + ".bn_scale", co);  // derived at finalize
-    slot(h, n + ".bn_shift", co);
+    w.add(n + ".conv.weight", {co, ci, k});
+    for (const char* leaf : {".bnorm.weight", ".bnorm.bias", ".bnorm.running_mean", ".bnorm.running_var"}) w.add(n + leaf, {co});
+    w.add_derived(n + ".bn_scale", co);  // at finalize
+    w.add_derived(n + ".bn_shift", co);
   };
   for (int i = 0; i < K; ++i) bnconv(p + ".conv1d_bank." + std::to_string(i), cin, ch, i + 1);
   bnconv(p + ".conv_project1", K * ch, p0, 3);
   bnconv(p + ".conv_project2", p0, p1, 3);
-  if (p1 != ch) slot(h, p + ".pre_highway.weight", (size_t)ch * p1);
+  if (p1 != ch) w.add(p + ".pre_highway.weight", {ch, p1});
   // derived: tensor-core images of the large-M GEMMs (cbhg_gemm), packed on first use
-  for (int i = 0; i < K; ++i) slot(h, p + ".conv1d_bank." + std::to_string(i) + ".bigw", tc_big_weight_bytes(ch, i + 1, cin) / 4);
-  slot(h, p + ".conv_project1.bigw", tc_big_weight_bytes(p0, 3, K * ch) / 4);
-  slot(h, p + ".conv_project2.bigw", tc_big_weight_bytes(p1, 3, p0) / 4);
-  if (p1 != ch) slot(h, p + ".pre_highway.bigw", tc_big_weight_bytes(ch, 1, p1) / 4);
-  for (int i = 0; i < nh; ++i) slot(h, p + ".highways." + std::to_string(i) + ".bigw", tc_big_weight_bytes(2 * ch, 1, ch) / 4);
-  for (const char* sfx : {"", "_reverse"}) slot(h, p + ".rnn.ih" + sfx + ".bigw", tc_big_weight_bytes(3 * (ch / 2), 1, ch) / 4);
+  for (int i = 0; i < K; ++i) w.add_derived(p + ".conv1d_bank." + std::to_string(i) + ".bigw", tc_big_weight_bytes(ch, i + 1, cin) / 4);
+  w.add_derived(p + ".conv_project1.bigw", tc_big_weight_bytes(p0, 3, K * ch) / 4);
+  w.add_derived(p + ".conv_project2.bigw", tc_big_weight_bytes(p1, 3, p0) / 4);
+  if (p1 != ch) w.add_derived(p + ".pre_highway.bigw", tc_big_weight_bytes(ch, 1, p1) / 4);
+  for (int i = 0; i < nh; ++i) w.add_derived(p + ".highways." + std::to_string(i) + ".bigw", tc_big_weight_bytes(2 * ch, 1, ch) / 4);
+  for (const char* sfx : {"", "_reverse"}) w.add_derived(p + ".rnn.ih" + sfx + ".bigw", tc_big_weight_bytes(3 * (ch / 2), 1, ch) / 4);
   for (int i = 0; i < nh; ++i) {
     const std::string q = p + ".highways." + std::to_string(i);
-    slot(h, q + ".W1.weight", (size_t)ch * ch);
-    slot(h, q + ".W1.bias", ch);
-    slot(h, q + ".W2.weight", (size_t)ch * ch);
-    slot(h, q + ".W2.bias", ch);
-    slot(h, q + ".W12", (size_t)2 * ch * ch);  // derived: [W1; W2] stacked
-    slot(h, q + ".b12", (size_t)2 * ch);
+    w.add(q + ".W1.weight", {ch, ch});
+    w.add(q + ".W1.bias", {ch});
+    w.add(q + ".W2.weight", {ch, ch});
+    w.add(q + ".W2.bias", {ch});
+    w.add_derived(q + ".W12", (size_t)2 * ch * ch);  // [W1; W2] stacked
+    w.add_derived(q + ".b12", (size_t)2 * ch);
   }
+  const int H = ch / 2;
   for (const char* sfx : {"", "_reverse"}) {
-    slot(h, p + ".rnn.weight_ih_l0" + sfx, (size_t)3 * (ch / 2) * ch);
-    slot(h, p + ".rnn.weight_hh_l0" + sfx, (size_t)3 * (ch / 2) * (ch / 2));
-    slot(h, p + ".rnn.bias_ih_l0" + sfx, (size_t)3 * (ch / 2));
-    slot(h, p + ".rnn.bias_hh_l0" + sfx, (size_t)3 * (ch / 2));
+    w.add(p + ".rnn.weight_ih_l0" + sfx, {3 * H, ch});
+    w.add(p + ".rnn.weight_hh_l0" + sfx, {3 * H, H});
+    w.add(p + ".rnn.bias_ih_l0" + sfx, {3 * H});
+    w.add(p + ".rnn.bias_hh_l0" + sfx, {3 * H});
     // derived: tensor-core images of W_hh (gates r|z|n interleaved per 8 units) + tile-order b_hh
-    slot(h, p + ".rnn.hh" + sfx + ".tcw", tc_gated_weight_bytes(ch / 2, ch / 2) / 4);
-    slot(h, p + ".rnn.hh" + sfx + ".tcb", (size_t)4 * (ch / 2));
+    w.add_derived(p + ".rnn.hh" + sfx + ".tcw", tc_gated_weight_bytes(H, H) / 4);
+    w.add_derived(p + ".rnn.hh" + sfx + ".tcb", (size_t)4 * H);
   }
 }
 
@@ -607,11 +593,11 @@ int cbhg_gemm(mb_tacotron* h, const std::string& key, const GemmArgs& a, cudaStr
     return e ? atoi(e) != 0 : true;
   }();
   bool ok = env && bw.hi && a.M >= 512 && a.N % 4 == 0 && a.nseg >= 1 && a.nseg <= kMaxSeg && !a.mask && !a.step_mode &&
-            a.act != ACT_SIGMOID && a.act != ACT_TANH && h->slots.count(key + ".bigw") && (a.ldy % 4) == 0 &&
+            a.act != ACT_SIGMOID && a.act != ACT_TANH && h->w.has(key + ".bigw") && (a.ldy % 4) == 0 &&
             (!a.res || (a.ldres % 4) == 0);
   const int K = a.seg[0].K;
   for (int s = 1; ok && s < a.nseg; ++s) ok = a.seg[s].K == K;
-  if (ok) ok = tc_big_act_bytes(a.M, a.nseg, K) <= bw.bytes && tc_big_weight_bytes(a.N, a.nseg, K) / 4 <= h->slots[key + ".bigw"].n;
+  if (ok) ok = tc_big_act_bytes(a.M, a.nseg, K) <= bw.bytes && tc_big_weight_bytes(a.N, a.nseg, K) / 4 <= h->w.size(key + ".bigw");
   if (!ok) {
     TK(launch_gemm(a, st));
     return MB_OK;
@@ -864,62 +850,64 @@ int mb_tacotron_create(const mb_tacotron_config* cfg, mb_tacotron** out) {
   mb_tacotron* h = new mb_tacotron();
   h->cfg = c;
   const int E = c.encoder_dims, D = c.decoder_dims, proj_dims = E + c.speaker_embedding_size + c.gst_E;
-  slot(h, "scratch.absmax.tcb", 64);  // device scratch of the weight-image packers (derived slot: no cudaMalloc after create)
-  slot(h, "encoder.embedding.weight", (size_t)c.num_chars * c.embed_dims);
-  slot(h, "encoder.pre_net.fc1.weight", (size_t)E * c.embed_dims);
-  slot(h, "encoder.pre_net.fc1.bias", E);
-  slot(h, "encoder.pre_net.fc2.weight", (size_t)E * E);
-  slot(h, "encoder.pre_net.fc2.bias", E);
-  cbhg_slots(h, "encoder.cbhg", c.encoder_K, E, E, E, E, c.num_highways);
-  slot(h, "encoder_proj.weight", (size_t)D * proj_dims);
-  slot(h, "gst.const_enc", c.gst_E / 2);  // ReferenceEncoder(zeros): input independent, folded by the host
-  slot(h, "gst.stl.embed", (size_t)c.gst_tokens * (c.gst_E / c.gst_heads));
-  slot(h, "gst.stl.attention.W_query.weight", (size_t)c.gst_E * (c.gst_E / 2 + c.speaker_embedding_size));
-  slot(h, "gst.stl.attention.W_key.weight", (size_t)c.gst_E * (c.gst_E / c.gst_heads));
-  slot(h, "gst.stl.attention.W_value.weight", (size_t)c.gst_E * (c.gst_E / c.gst_heads));
-  slot(h, "gst.tanh_embed", (size_t)c.gst_tokens * (c.gst_E / c.gst_heads));  // derived
-  slot(h, "gst.keys", (size_t)c.gst_tokens * c.gst_E);
-  slot(h, "gst.values", (size_t)c.gst_tokens * c.gst_E);
-  slot(h, "decoder.prenet.fc1.weight", (size_t)2 * D * c.n_mels);
-  slot(h, "decoder.prenet.fc1.bias", 2 * D);
-  slot(h, "decoder.prenet.fc2.weight", (size_t)2 * D * 2 * D);
-  slot(h, "decoder.prenet.fc2.bias", 2 * D);
-  slot(h, "decoder.attn_net.conv.weight", ATT_F * ATT_K);
-  slot(h, "decoder.attn_net.conv.bias", ATT_F);
-  slot(h, "decoder.attn_net.L.weight", ATT_D * ATT_F);
-  slot(h, "decoder.attn_net.W.weight", ATT_D * ATT_D);
-  slot(h, "decoder.attn_net.W.bias", ATT_D);
-  slot(h, "decoder.attn_net.v.weight", ATT_D);
-  slot(h, "decoder.attn_rnn.weight_ih", (size_t)3 * D * (proj_dims + 2 * D));
-  slot(h, "decoder.attn_rnn.weight_hh", (size_t)3 * D * D);
-  slot(h, "decoder.attn_rnn.bias_ih", 3 * D);
-  slot(h, "decoder.attn_rnn.bias_hh", 3 * D);
-  slot(h, "decoder.attn_rnn.ih.tcw", tc_skinny_weight_bytes(3 * D, proj_dims + 2 * D) / 4);  // derived tensor-core images
-  slot(h, "decoder.attn_rnn.ih.tcb", 3 * D);
-  slot(h, "decoder.attn_rnn.hh.tcw", tc_gated_weight_bytes(D, D) / 4);
-  slot(h, "decoder.attn_rnn.hh.tcb", 4 * D);
-  slot(h, "decoder.rnn_input.weight", (size_t)c.lstm_dims * (proj_dims + D));
-  slot(h, "decoder.rnn_input.bias", c.lstm_dims);
+  const int dk = c.gst_E / c.gst_heads, L = c.lstm_dims;
+  WeightTable& w = h->w;
+  w.add_derived("scratch.absmax.tcb", 64);  // device scratch of the weight-image packers (no cudaMalloc after create)
+  w.add("encoder.embedding.weight", {c.num_chars, c.embed_dims});
+  w.add("encoder.pre_net.fc1.weight", {E, c.embed_dims});
+  w.add("encoder.pre_net.fc1.bias", {E});
+  w.add("encoder.pre_net.fc2.weight", {E, E});
+  w.add("encoder.pre_net.fc2.bias", {E});
+  cbhg_slots(w, "encoder.cbhg", c.encoder_K, E, E, E, E, c.num_highways);
+  w.add("encoder_proj.weight", {D, proj_dims});
+  w.add("gst.const_enc", {c.gst_E / 2});  // ReferenceEncoder(zeros): input independent, folded by the host
+  w.add("gst.stl.embed", {c.gst_tokens, dk});
+  w.add("gst.stl.attention.W_query.weight", {c.gst_E, c.gst_E / 2 + c.speaker_embedding_size});
+  w.add("gst.stl.attention.W_key.weight", {c.gst_E, dk});
+  w.add("gst.stl.attention.W_value.weight", {c.gst_E, dk});
+  w.add_derived("gst.tanh_embed", (size_t)c.gst_tokens * dk);
+  w.add_derived("gst.keys", (size_t)c.gst_tokens * c.gst_E);
+  w.add_derived("gst.values", (size_t)c.gst_tokens * c.gst_E);
+  w.add("decoder.prenet.fc1.weight", {2 * D, c.n_mels});
+  w.add("decoder.prenet.fc1.bias", {2 * D});
+  w.add("decoder.prenet.fc2.weight", {2 * D, 2 * D});
+  w.add("decoder.prenet.fc2.bias", {2 * D});
+  w.add("decoder.attn_net.conv.weight", {ATT_F, 1, ATT_K});
+  w.add("decoder.attn_net.conv.bias", {ATT_F});
+  w.add("decoder.attn_net.L.weight", {ATT_D, ATT_F});
+  w.add("decoder.attn_net.W.weight", {ATT_D, ATT_D});
+  w.add("decoder.attn_net.W.bias", {ATT_D});
+  w.add("decoder.attn_net.v.weight", {1, ATT_D});
+  w.add("decoder.attn_rnn.weight_ih", {3 * D, proj_dims + 2 * D});
+  w.add("decoder.attn_rnn.weight_hh", {3 * D, D});
+  w.add("decoder.attn_rnn.bias_ih", {3 * D});
+  w.add("decoder.attn_rnn.bias_hh", {3 * D});
+  w.add_derived("decoder.attn_rnn.ih.tcw", tc_skinny_weight_bytes(3 * D, proj_dims + 2 * D) / 4);  // tensor-core images
+  w.add_derived("decoder.attn_rnn.ih.tcb", 3 * D);
+  w.add_derived("decoder.attn_rnn.hh.tcw", tc_gated_weight_bytes(D, D) / 4);
+  w.add_derived("decoder.attn_rnn.hh.tcb", 4 * D);
+  w.add("decoder.rnn_input.weight", {L, proj_dims + D});
+  w.add("decoder.rnn_input.bias", {L});
   for (const char* n : {"decoder.res_rnn1", "decoder.res_rnn2"}) {
-    slot(h, std::string(n) + ".weight_ih", (size_t)4 * c.lstm_dims * c.lstm_dims);
-    slot(h, std::string(n) + ".weight_hh", (size_t)4 * c.lstm_dims * c.lstm_dims);
-    slot(h, std::string(n) + ".bias_ih", 4 * c.lstm_dims);
-    slot(h, std::string(n) + ".bias_hh", 4 * c.lstm_dims);
-    slot(h, std::string(n) + ".bias_sum", 4 * c.lstm_dims);  // derived: b_hh + b_ih
-    slot(h, std::string(n) + ".tcw", tc_skinny_weight_bytes(4 * c.lstm_dims, 2 * c.lstm_dims) / 4);  // derived: hi/lo tiles
-    slot(h, std::string(n) + ".tcb", 4 * c.lstm_dims);                                                // derived: tile-order bias
+    w.add(std::string(n) + ".weight_ih", {4 * L, L});
+    w.add(std::string(n) + ".weight_hh", {4 * L, L});
+    w.add(std::string(n) + ".bias_ih", {4 * L});
+    w.add(std::string(n) + ".bias_hh", {4 * L});
+    w.add_derived(std::string(n) + ".bias_sum", 4 * L);                                   // b_hh + b_ih
+    w.add_derived(std::string(n) + ".tcw", tc_skinny_weight_bytes(4 * L, 2 * L) / 4);  // hi/lo tiles
+    w.add_derived(std::string(n) + ".tcb", 4 * L);                                        // tile-order bias
   }
-  slot(h, "decoder.mel_proj.weight", (size_t)c.n_mels * c.max_r * c.lstm_dims);
-  slot(h, "decoder.mel_proj.packed", (size_t)c.n_mels * c.max_r * c.lstm_dims);  // derived for the current r
-  slot(h, "decoder.mel_proj.tcw", tc_skinny_weight_bytes(c.n_mels * c.max_r, c.lstm_dims) / 4);  // derived (current r)
-  slot(h, "decoder.mel_proj.tcb", (size_t)c.n_mels * c.max_r + 32);
-  slot(h, "decoder.rnn_input.tcw", tc_skinny_weight_bytes(c.lstm_dims, proj_dims + D) / 4);     // derived
-  slot(h, "decoder.rnn_input.tcb", c.lstm_dims);
-  slot(h, "decoder.stop_proj.weight", (size_t)(proj_dims + c.lstm_dims));
-  slot(h, "decoder.stop_proj.bias", 1);
-  cbhg_slots(h, "postnet", c.postnet_K, c.n_mels, c.postnet_dims, c.postnet_dims, c.n_mels, c.num_highways);
-  slot(h, "post_proj.weight", (size_t)c.n_mels * c.postnet_dims);
-  slot(h, "post_proj.bigw", tc_big_weight_bytes(c.n_mels, 1, c.postnet_dims) / 4);
+  w.add("decoder.mel_proj.weight", {c.n_mels * c.max_r, L});
+  w.add_derived("decoder.mel_proj.packed", (size_t)c.n_mels * c.max_r * L);                     // for the current r
+  w.add_derived("decoder.mel_proj.tcw", tc_skinny_weight_bytes(c.n_mels * c.max_r, L) / 4);  // (current r)
+  w.add_derived("decoder.mel_proj.tcb", (size_t)c.n_mels * c.max_r + 32);
+  w.add_derived("decoder.rnn_input.tcw", tc_skinny_weight_bytes(L, proj_dims + D) / 4);
+  w.add_derived("decoder.rnn_input.tcb", L);
+  w.add("decoder.stop_proj.weight", {1, proj_dims + L});
+  w.add("decoder.stop_proj.bias", {1});
+  cbhg_slots(w, "postnet", c.postnet_K, c.n_mels, c.postnet_dims, c.postnet_dims, c.n_mels, c.num_highways);
+  w.add("post_proj.weight", {c.n_mels, c.postnet_dims});
+  w.add_derived("post_proj.bigw", tc_big_weight_bytes(c.n_mels, 1, c.postnet_dims) / 4);
   *out = h;
   return MB_OK;
 }
@@ -935,33 +923,23 @@ void mb_tacotron_destroy(mb_tacotron* h) {
   delete h;
 }
 
-size_t mb_tacotron_arena_bytes(const mb_tacotron* h) { return h ? h->total * sizeof(float) : 0; }
+size_t mb_tacotron_arena_bytes(const mb_tacotron* h) { return h ? h->w.floats() * sizeof(float) : 0; }
 
 int mb_tacotron_set_arena(mb_tacotron* h, void* arena, size_t bytes) {
-  if (!h || !arena) return fail(MB_ERR_INVALID, "mb_tacotron_set_arena: null argument");
-  if (bytes < mb_tacotron_arena_bytes(h)) return fail(MB_ERR_WORKSPACE, "mb_tacotron_set_arena: arena too small");
-  if (((uintptr_t)arena & 255) != 0) return fail(MB_ERR_INVALID, "mb_tacotron_set_arena: arena must be 256-byte aligned");
-  h->arena = (float*)arena;
+  if (int rc = check_arena("mb_tacotron_set_arena", h, arena, bytes, mb_tacotron_arena_bytes(h), 256)) return rc;
+  h->w.attach((float*)arena);
+  h->finalized = false;
   // a new arena holds none of the derived images: forget every lazily packed tensor-core image and its scale
   h->big_packed.clear();
   h->tc_inv_scale.clear();
   h->packed_r = 0;
-  h->finalized = false;
   return MB_OK;
 }
 
 int mb_tacotron_set_weight(mb_tacotron* h, const char* name, const float* w, const int64_t* dims, int32_t ndim,
                            void* stream) {
-  if (!h || !name || !w) return fail(MB_ERR_INVALID, "mb_tacotron_set_weight: null argument");
-  if (!h->arena) return fail(MB_ERR_STATE, "mb_tacotron_set_weight: call mb_tacotron_set_arena first");
-  auto it = h->slots.find(name);
-  if (it == h->slots.end()) return fail(MB_ERR_INVALID, "mb_tacotron_set_weight: unknown tensor '%s'", name);
-  size_t n = 1;
-  for (int i = 0; i < ndim; ++i) n *= (size_t)dims[i];
-  if (n != it->second.n)
-    return fail(MB_ERR_INVALID, "mb_tacotron_set_weight: %s has %zu elements, expected %zu", name, n, it->second.n);
-  MB_CUDA_CHECK(cudaMemcpyAsync(h->arena + it->second.off, w, n * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  it->second.set = true;
+  if (!h) return fail(MB_ERR_INVALID, "mb_tacotron_set_weight: null argument");
+  if (int rc = h->w.set("mb_tacotron_set_weight", name, w, dims, ndim, stream)) return rc;
   h->finalized = false;
   h->big_packed.clear();  // images packed from the previous weights are stale
   h->packed_r = 0;
@@ -973,36 +951,26 @@ int mb_tacotron_finalize(mb_tacotron* h, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   h->big_packed.clear();  // re-packed from the current weights at first use
   const mb_tacotron_config& c = h->cfg;
-  auto derived = [](const std::string& n) {
-    return n.find(".bn_scale") != std::string::npos || n.find(".bn_shift") != std::string::npos ||
-           n.find(".W12") != std::string::npos || n.find(".b12") != std::string::npos || n == "gst.tanh_embed" ||
-           n == "gst.keys" || n == "gst.values" || n.find(".bias_sum") != std::string::npos || n.find(".tcw") != std::string::npos ||
-           n.find(".tcb") != std::string::npos || n.find(".tcw") != std::string::npos || n.find(".bigw") != std::string::npos ||
-           n == "decoder.mel_proj.packed";
-  };
-  for (auto& kv : h->slots)
-    if (!kv.second.set && !derived(kv.first))
-      return fail(MB_ERR_STATE, "mb_tacotron_finalize: tensor %s was never set", kv.first.c_str());
+  if (int rc = h->w.check_all_set("mb_tacotron_finalize")) return rc;
+  // the BatchNorm'd convolutions and the highways of both CBHG stacks
+  std::vector<std::string> bnconvs, highways;
+  for (const auto& cb : {std::make_pair(std::string("encoder.cbhg"), c.encoder_K), std::make_pair(std::string("postnet"), c.postnet_K)}) {
+    for (int i = 0; i < cb.second; ++i) bnconvs.push_back(cb.first + ".conv1d_bank." + std::to_string(i));
+    bnconvs.push_back(cb.first + ".conv_project1");
+    bnconvs.push_back(cb.first + ".conv_project2");
+    for (int i = 0; i < c.num_highways; ++i) highways.push_back(cb.first + ".highways." + std::to_string(i));
+  }
   // fold eval BatchNorm into scale/shift
-  for (auto& kv : h->slots) {
-    const std::string& n = kv.first;
-    const size_t pos = n.find(".bnorm.weight");
-    if (pos == std::string::npos) continue;
-    const std::string base = n.substr(0, pos);
-    const int co = (int)kv.second.n;
+  for (const std::string& base : bnconvs) {
+    const int co = (int)h->w.size(base + ".bnorm.weight");
     bn_fold_kernel<<<(co + 255) / 256, 256, 0, st>>>(P(h, base + ".bnorm.weight"), P(h, base + ".bnorm.bias"),
                                                      P(h, base + ".bnorm.running_mean"), P(h, base + ".bnorm.running_var"),
                                                      P(h, base + ".bn_scale"), P(h, base + ".bn_shift"), co);
     MB_LAUNCH_CHECK("bn_fold_kernel");
   }
   // stacked highway weights [W1; W2]
-  for (auto& kv : h->slots) {
-    const std::string& n = kv.first;
-    const size_t pos = n.find(".W1.weight");
-    if (pos == std::string::npos) continue;
-    const std::string base = n.substr(0, pos);
-    const size_t nn = kv.second.n;
-    const size_t ch = h->slots[base + ".W1.bias"].n;
+  for (const std::string& base : highways) {
+    const size_t nn = h->w.size(base + ".W1.weight"), ch = h->w.size(base + ".W1.bias");
     MB_CUDA_CHECK(cudaMemcpyAsync(P(h, base + ".W12"), P(h, base + ".W1.weight"), nn * 4, cudaMemcpyDeviceToDevice, st));
     MB_CUDA_CHECK(cudaMemcpyAsync(P(h, base + ".W12") + nn, P(h, base + ".W2.weight"), nn * 4, cudaMemcpyDeviceToDevice, st));
     MB_CUDA_CHECK(cudaMemcpyAsync(P(h, base + ".b12"), P(h, base + ".W1.bias"), ch * 4, cudaMemcpyDeviceToDevice, st));

@@ -623,19 +623,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
 // =================================================================================================
 using namespace mb;
 
-namespace {
-struct WSlot {
-  std::string name;
-  std::vector<int64_t> dims;
-  size_t off = 0;  // float offset in the arena
-  bool set = false;
-};
-}  // namespace
-
 struct mb_wavernn {
   mb_wavernn_config cfg{};
-  std::vector<WSlot> slots;
-  size_t raw_floats = 0;   // raw weights as given
+  WeightTable w;           // raw weights as given
   size_t pack_off = 0;     // per-CTA packs
   size_t total_floats = 0;
   float* arena = nullptr;
@@ -647,22 +637,7 @@ struct mb_wavernn {
 
 namespace {
 
-const float* W(const mb_wavernn* h, const std::string& name) {
-  for (const WSlot& s : h->slots)
-    if (s.name == name) return h->arena + s.off;
-  return nullptr;
-}
-
-void add_slot(mb_wavernn* h, const std::string& name, std::vector<int64_t> dims) {
-  WSlot s;
-  s.name = name;
-  s.dims = dims;
-  size_t n = 1;
-  for (int64_t d : dims) n *= (size_t)d;
-  s.off = h->raw_floats;
-  h->raw_floats += align_up(n, 64);
-  h->slots.push_back(s);
-}
+const float* W(const mb_wavernn* h, const std::string& name) { return h->w.ptr(name); }
 
 struct WsLayout {
   size_t aux, melup, aux2P, aux3P, aux4P, tmpA, tmpB, tmpR, padP, lad5, lad25, lad200, starts, condI, h1, h2, f1, f2, logits, xprev,
@@ -721,39 +696,39 @@ int mb_wavernn_create(const mb_wavernn_config* cfg, mb_wavernn** out) {
                 "upsample (5,5,8), 80 mels, compute/res_out 128)");
   mb_wavernn* h = new mb_wavernn();
   h->cfg = *cfg;
-  add_slot(h, "upsample.resnet.conv_in.weight", {CDIM, FEAT, 5});
+  h->w.add("upsample.resnet.conv_in.weight", {CDIM, FEAT, 5});
   auto bn = [&](const std::string& p) {
-    for (const char* leaf : {".weight", ".bias", ".running_mean", ".running_var"}) add_slot(h, p + leaf, {CDIM});
+    for (const char* leaf : {".weight", ".bias", ".running_mean", ".running_var"}) h->w.add(p + leaf, {CDIM});
   };
   bn("upsample.resnet.batch_norm");
   for (int i = 0; i < cfg->res_blocks; ++i) {
     const std::string b = "upsample.resnet.layers." + std::to_string(i);
-    add_slot(h, b + ".conv1.weight", {CDIM, CDIM, 1});
-    add_slot(h, b + ".conv2.weight", {CDIM, CDIM, 1});
+    h->w.add(b + ".conv1.weight", {CDIM, CDIM, 1});
+    h->w.add(b + ".conv2.weight", {CDIM, CDIM, 1});
     bn(b + ".batch_norm1");
     bn(b + ".batch_norm2");
   }
-  add_slot(h, "upsample.resnet.conv_out.weight", {CDIM, CDIM, 1});
-  add_slot(h, "upsample.resnet.conv_out.bias", {CDIM});
+  h->w.add("upsample.resnet.conv_out.weight", {CDIM, CDIM, 1});
+  h->w.add("upsample.resnet.conv_out.bias", {CDIM});
   for (int j = 0; j < 3; ++j)
-    add_slot(h, "upsample.up_layers." + std::to_string(2 * j + 1) + ".weight", {1, 1, 1, 2 * cfg->upsample_factors[j] + 1});
-  add_slot(h, "I.weight", {RNN, FEAT + AUXD + 1});
-  add_slot(h, "I.bias", {RNN});
-  add_slot(h, "rnn1.weight_ih_l0", {3 * RNN, RNN});
-  add_slot(h, "rnn1.weight_hh_l0", {3 * RNN, RNN});
-  add_slot(h, "rnn1.bias_ih_l0", {3 * RNN});
-  add_slot(h, "rnn1.bias_hh_l0", {3 * RNN});
-  add_slot(h, "rnn2.weight_ih_l0", {3 * RNN, RNN + AUXD});
-  add_slot(h, "rnn2.weight_hh_l0", {3 * RNN, RNN});
-  add_slot(h, "rnn2.bias_ih_l0", {3 * RNN});
-  add_slot(h, "rnn2.bias_hh_l0", {3 * RNN});
-  add_slot(h, "fc1.weight", {RNN, RNN + AUXD});
-  add_slot(h, "fc1.bias", {RNN});
-  add_slot(h, "fc2.weight", {RNN, RNN + AUXD});
-  add_slot(h, "fc2.bias", {RNN});
-  add_slot(h, "fc3.weight", {NCLS, RNN});
-  add_slot(h, "fc3.bias", {NCLS});
-  h->pack_off = h->raw_floats;
+    h->w.add("upsample.up_layers." + std::to_string(2 * j + 1) + ".weight", {1, 1, 1, 2 * cfg->upsample_factors[j] + 1});
+  h->w.add("I.weight", {RNN, FEAT + AUXD + 1});
+  h->w.add("I.bias", {RNN});
+  h->w.add("rnn1.weight_ih_l0", {3 * RNN, RNN});
+  h->w.add("rnn1.weight_hh_l0", {3 * RNN, RNN});
+  h->w.add("rnn1.bias_ih_l0", {3 * RNN});
+  h->w.add("rnn1.bias_hh_l0", {3 * RNN});
+  h->w.add("rnn2.weight_ih_l0", {3 * RNN, RNN + AUXD});
+  h->w.add("rnn2.weight_hh_l0", {3 * RNN, RNN});
+  h->w.add("rnn2.bias_ih_l0", {3 * RNN});
+  h->w.add("rnn2.bias_hh_l0", {3 * RNN});
+  h->w.add("fc1.weight", {RNN, RNN + AUXD});
+  h->w.add("fc1.bias", {RNN});
+  h->w.add("fc2.weight", {RNN, RNN + AUXD});
+  h->w.add("fc2.bias", {RNN});
+  h->w.add("fc3.weight", {NCLS, RNN});
+  h->w.add("fc3.bias", {NCLS});
+  h->pack_off = h->w.floats();
   h->total_floats = h->pack_off + (size_t)NCTA * WPACK_FLOATS + RNN;
   *out = h;
   return MB_OK;
@@ -764,35 +739,24 @@ void mb_wavernn_destroy(mb_wavernn* h) { delete h; }
 size_t mb_wavernn_arena_bytes(const mb_wavernn* h) { return h ? h->total_floats * sizeof(float) : 0; }
 
 int mb_wavernn_set_arena(mb_wavernn* h, void* arena, size_t bytes) {
-  if (!h || !arena) return fail(MB_ERR_INVALID, "mb_wavernn_set_arena: null argument");
-  if (bytes < mb_wavernn_arena_bytes(h)) return fail(MB_ERR_WORKSPACE, "mb_wavernn_set_arena: arena too small");
-  if (((uintptr_t)arena & 255) != 0) return fail(MB_ERR_INVALID, "mb_wavernn_set_arena: arena must be 256-byte aligned");
+  if (int rc = check_arena("mb_wavernn_set_arena", h, arena, bytes, mb_wavernn_arena_bytes(h), 256)) return rc;
+  h->w.attach((float*)arena);
   h->arena = (float*)arena;
+  h->finalized = false;
   return MB_OK;
 }
 
 int mb_wavernn_set_weight(mb_wavernn* h, const char* name, const float* w, const int64_t* dims, int32_t ndim,
                           void* stream) {
-  if (!h || !name || !w || !dims) return fail(MB_ERR_INVALID, "mb_wavernn_set_weight: null argument");
-  if (!h->arena) return fail(MB_ERR_STATE, "mb_wavernn_set_weight: call mb_wavernn_set_arena first");
-  for (WSlot& s : h->slots) {
-    if (s.name != name) continue;
-    size_t n = 1, given = 1;
-    for (int64_t d : s.dims) n *= (size_t)d;
-    for (int i = 0; i < ndim; ++i) given *= (size_t)dims[i];
-    if (given != n) return fail(MB_ERR_INVALID, "mb_wavernn_set_weight: %s has %zu elements, expected %zu", name, given, n);
-    MB_CUDA_CHECK(cudaMemcpyAsync(h->arena + s.off, w, n * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-    s.set = true;
-    h->finalized = false;
-    return MB_OK;
-  }
-  return fail(MB_ERR_INVALID, "mb_wavernn_set_weight: unknown tensor '%s'", name);
+  if (!h) return fail(MB_ERR_INVALID, "mb_wavernn_set_weight: null argument");
+  if (int rc = h->w.set("mb_wavernn_set_weight", name, w, dims, ndim, stream)) return rc;
+  h->finalized = false;
+  return MB_OK;
 }
 
 int mb_wavernn_finalize(mb_wavernn* h, void* stream) {
   if (!h) return fail(MB_ERR_INVALID, "mb_wavernn_finalize: null handle");
-  for (const WSlot& s : h->slots)
-    if (!s.set) return fail(MB_ERR_STATE, "mb_wavernn_finalize: tensor %s was never set", s.name.c_str());
+  if (int rc = h->w.check_all_set("mb_wavernn_finalize")) return rc;
   PackSrc ps;
   ps.r1_wih = W(h, "rnn1.weight_ih_l0");
   ps.r1_whh = W(h, "rnn1.weight_hh_l0");

@@ -56,27 +56,13 @@ class SpeakerEncoder:
     def _upload(self):
         if self._state is None:
             raise _lib.MbError("SpeakerEncoder has no weights: call load_state_dict first")
-        dev = self._device or _lib.require_cuda()
-        self._device = dev
-        L = _lib.lib()
-        nbytes = int(L.mb_encoder_arena_bytes(self._handle))
-        with torch.cuda.device(dev):
-            self._arena = torch.zeros(nbytes + 256, dtype=torch.uint8, device=dev)
-            base = (self._arena.data_ptr() + 255) // 256 * 256
-            _lib.check(L.mb_encoder_set_arena(self._handle, C.c_void_p(base), nbytes))
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            keep = []
-            for name, t in self._state.items():
-                if not (name.startswith("lstm.") or name.startswith("linear.")):
-                    continue  # similarity_weight / similarity_bias: loss only (model.py:27-28)
-                d = t.to(device=dev, dtype=torch.float32).contiguous()
-                keep.append(d)
-                dims = (C.c_int64 * max(1, d.dim()))(*d.shape)
-                _lib.check(L.mb_encoder_set_weight(self._handle, name.encode(), C.c_void_p(d.data_ptr()), dims, d.dim(),
-                                                   C.c_void_p(stream)))
-            _lib.check(L.mb_encoder_finalize(self._handle, C.c_void_p(stream)))
-            torch.cuda.current_stream(dev).synchronize()
+        self._device = self._device or _lib.require_cuda()
+        self._arena = _lib.upload_weights("encoder", self._handle, self.weights_for_upload(), self._device)
         self._ready = True
+
+    def weights_for_upload(self) -> Dict[str, torch.Tensor]:
+        """the LSTM and the Linear; similarity_weight / similarity_bias are loss only (model.py:27-28)"""
+        return {k: v for k, v in self._state.items() if k.startswith("lstm.") or k.startswith("linear.")}
 
     def packed_arena(self) -> torch.Tensor:
         if not self._ready:

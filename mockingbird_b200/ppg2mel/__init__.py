@@ -90,27 +90,13 @@ class MelDecoderMOLv2:
     def _upload(self):
         if self._state is None:
             raise _lib.MbError("MelDecoderMOLv2 has no weights: call load_state_dict first")
-        dev = self._device or _lib.require_cuda()
-        self._device = dev
-        L = _lib.lib()
-        nbytes = int(L.mb_ppg2mel_arena_bytes(self._handle))
-        with torch.cuda.device(dev):
-            self._arena = torch.zeros(nbytes + 256, dtype=torch.uint8, device=dev)
-            base = (self._arena.data_ptr() + 255) // 256 * 256
-            _lib.check(L.mb_ppg2mel_set_arena(self._handle, C.c_void_p(base), nbytes))
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            keep = []
-            for name, t in self._state.items():
-                if not t.dtype.is_floating_point:
-                    continue
-                d = t.to(device=dev, dtype=torch.float32).contiguous()
-                keep.append(d)
-                dims = (C.c_int64 * max(1, d.dim()))(*d.shape)
-                _lib.check(L.mb_ppg2mel_set_weight(self._handle, name.encode(), C.c_void_p(d.data_ptr()), dims, d.dim(),
-                                                   C.c_void_p(stream)))
-            _lib.check(L.mb_ppg2mel_finalize(self._handle, C.c_void_p(stream)))
-            torch.cuda.current_stream(dev).synchronize()
+        self._device = self._device or _lib.require_cuda()
+        self._arena = _lib.upload_weights("ppg2mel", self._handle, self.weights_for_upload(), self._device)
         self._ready = True
+
+    def weights_for_upload(self) -> Dict[str, torch.Tensor]:
+        """the float tensors of the checkpoint (the library drops the ones inference never reads)"""
+        return {k: v for k, v in self._state.items() if v.dtype.is_floating_point}
 
     # -- inference -----------------------------------------------------------------------------------------------------
     def _run(self, ppg: torch.Tensor, lf0_uv: torch.Tensor, spk: torch.Tensor, lengths: List[int], masks=None,

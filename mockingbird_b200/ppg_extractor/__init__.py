@@ -206,29 +206,15 @@ class PPGModel:
     def _upload(self):
         if self._state is None:
             raise _lib.MbError("PPGModel has no weights: call load_state_dict first")
-        dev = self._device or _lib.require_cuda()
-        self._device = dev
-        L = _lib.lib()
-        nbytes = int(L.mb_ppgx_arena_bytes(self._handle))
-        state = dict(self._state)
-        state.setdefault("frontend.logmel.melmat", self._default_melmat)
-        with torch.cuda.device(dev):
-            self._arena = torch.zeros(nbytes + 1024, dtype=torch.uint8, device=dev)
-            base = (self._arena.data_ptr() + 1023) // 1024 * 1024
-            _lib.check(L.mb_ppgx_set_arena(self._handle, C.c_void_p(base), nbytes))
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            keep = []
-            for name, t in state.items():
-                if not t.dtype.is_floating_point:
-                    continue
-                d = t.to(device=dev, dtype=torch.float32).contiguous()
-                keep.append(d)
-                dims = (C.c_int64 * max(1, d.dim()))(*d.shape)
-                _lib.check(L.mb_ppgx_set_weight(self._handle, name.encode(), C.c_void_p(d.data_ptr()), dims, d.dim(),
-                                                C.c_void_p(stream)))
-            _lib.check(L.mb_ppgx_finalize(self._handle, C.c_void_p(stream)))
-            torch.cuda.current_stream(dev).synchronize()
+        self._device = self._device or _lib.require_cuda()
+        self._arena = _lib.upload_weights("ppgx", self._handle, self.weights_for_upload(), self._device, align=1024)
         self._ready = True
+
+    def weights_for_upload(self) -> Dict[str, torch.Tensor]:
+        """the float tensors of the checkpoint, with the default mel basis where the checkpoint has none"""
+        state = {k: v for k, v in self._state.items() if v.dtype.is_floating_point}
+        state.setdefault("frontend.logmel.melmat", self._default_melmat)
+        return state
 
     def _prepare(self):
         self.eval()

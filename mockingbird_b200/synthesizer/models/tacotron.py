@@ -125,29 +125,16 @@ class Tacotron:
     def _upload(self):
         if self._state is None:
             raise _lib.MbError("Tacotron has no weights: call load_state_dict / load first")
-        dev = self._device or _lib.require_cuda()
-        self._device = dev
-        L = _lib.lib()
-        nbytes = int(L.mb_tacotron_arena_bytes(self._handle))
-        skip_prefix = ("gst.encoder.",)
-        with torch.cuda.device(dev):
-            self._arena = torch.zeros(nbytes + 256, dtype=torch.uint8, device=dev)
-            base = (self._arena.data_ptr() + 255) // 256 * 256
-            _lib.check(L.mb_tacotron_set_arena(self._handle, C.c_void_p(base), nbytes))
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            keep = []
-            tensors = {k: v for k, v in self._state.items()
-                       if v.dtype.is_floating_point and not k.startswith(skip_prefix) and k not in ("stop_threshold",)}
-            tensors["gst.const_enc"] = self._gst_const_enc()
-            for name, t in tensors.items():
-                d = t.to(device=dev, dtype=torch.float32).contiguous()
-                keep.append(d)
-                dims = (C.c_int64 * max(1, d.dim()))(*d.shape)
-                _lib.check(L.mb_tacotron_set_weight(self._handle, name.encode(), C.c_void_p(d.data_ptr()), dims, d.dim(),
-                                                    C.c_void_p(stream)))
-            _lib.check(L.mb_tacotron_finalize(self._handle, C.c_void_p(stream)))
-            torch.cuda.current_stream(dev).synchronize()
+        self._device = self._device or _lib.require_cuda()
+        self._arena = _lib.upload_weights("tacotron", self._handle, self.weights_for_upload(), self._device)
         self._ready = True
+
+    def weights_for_upload(self) -> Dict[str, torch.Tensor]:
+        """the float tensors of the checkpoint without the GST reference encoder, which is folded into gst.const_enc"""
+        tensors = {k: v for k, v in self._state.items()
+                   if v.dtype.is_floating_point and not k.startswith("gst.encoder.") and k != "stop_threshold"}
+        tensors["gst.const_enc"] = self._gst_const_enc()
+        return tensors
 
     def packed_arena(self) -> torch.Tensor:
         if not self._ready:

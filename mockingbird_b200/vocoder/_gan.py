@@ -174,27 +174,13 @@ class GanGenerator:
         else:
             self._upload_weights()
 
+    def weights_for_upload(self) -> Dict[str, torch.Tensor]:
+        """the weight-norm-folded convolution weights and biases, as mb_gan_set_weight takes them"""
+        return {k: v for k, v in fold_weight_norm(self._state).items() if k.endswith(".weight") or k.endswith(".bias")}
+
     def _upload_weights(self):
-        dev = self._device or _lib.require_cuda()
-        self._device = dev
-        L = _lib.lib()
-        nbytes = int(L.mb_gan_arena_bytes(self._handle))
-        with torch.cuda.device(dev):
-            self._arena = torch.zeros(nbytes + 256, dtype=torch.uint8, device=dev)
-            base = (self._arena.data_ptr() + 255) // 256 * 256
-            _lib.check(L.mb_gan_set_arena(self._handle, C.c_void_p(base), nbytes))
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            keep = []
-            for name, t in fold_weight_norm(self._state).items():
-                if not (name.endswith(".weight") or name.endswith(".bias")):
-                    continue
-                d = t.to(device=dev, dtype=torch.float32).contiguous()
-                keep.append(d)
-                dims = (C.c_int64 * d.dim())(*d.shape)
-                _lib.check(L.mb_gan_set_weight(self._handle, name.encode(), C.c_void_p(d.data_ptr()), dims,
-                                               d.dim(), C.c_void_p(stream)))
-            torch.cuda.current_stream(dev).synchronize()
-            _lib.check(L.mb_gan_finalize(self._handle))
+        self._device = self._device or _lib.require_cuda()
+        self._arena = _lib.upload_weights("gan", self._handle, self.weights_for_upload(), self._device)
         self._ready = True
 
     def packed_arena(self) -> torch.Tensor:

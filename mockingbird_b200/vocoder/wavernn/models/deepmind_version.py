@@ -69,25 +69,14 @@ class WaveRNN:
     def _upload(self):
         if self._state is None:
             raise _lib.MbError("WaveRNN has no weights: call load_state_dict first")
-        dev = self._device or _lib.require_cuda()
-        self._device = dev
-        L = _lib.lib()
-        nbytes = int(L.mb_deepmind_arena_bytes(self._handle))
-        with torch.cuda.device(dev):
-            self._arena = torch.zeros(nbytes + 256, dtype=torch.uint8, device=dev)
-            base = (self._arena.data_ptr() + 255) // 256 * 256
-            _lib.check(L.mb_deepmind_set_arena(self._handle, C.c_void_p(base), nbytes))
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            keep = []
-            for name, t in self._state.items():
-                d = t.to(device=dev, dtype=torch.float32).contiguous()
-                keep.append(d)
-                dims = (C.c_int64 * max(1, d.dim()))(*d.shape)
-                _lib.check(L.mb_deepmind_set_weight(self._handle, name.encode(), C.c_void_p(d.data_ptr()), dims, d.dim(), C.c_void_p(stream)))
-            _lib.check(L.mb_deepmind_finalize(self._handle, C.c_void_p(stream)))
-            torch.cuda.current_stream(dev).synchronize()
-            self._ws = torch.empty(int(L.mb_deepmind_workspace_bytes(self._handle)) + 256, dtype=torch.uint8, device=dev)
+        dev = self._device = self._device or _lib.require_cuda()
+        self._arena = _lib.upload_weights("deepmind", self._handle, self.weights_for_upload(), dev)
+        self._ws = torch.empty(int(_lib.lib().mb_deepmind_workspace_bytes(self._handle)) + 256, dtype=torch.uint8, device=dev)
         self._ready = True
+
+    def weights_for_upload(self) -> Dict[str, torch.Tensor]:
+        """every tensor of the checkpoint"""
+        return dict(self._state)
 
     def generate(self, seq_len: int, noise: Optional[torch.Tensor] = None):
         """-> (output int64 [seq_len], coarse int64 [seq_len], fine int64 [seq_len]) numpy, like the reference (:75-162).
