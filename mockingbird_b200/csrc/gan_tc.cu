@@ -210,6 +210,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(const __grid_con
     float acc[MT][N / 2];
     const int C4 = p.Cout >> 2;
     const int ocw = f16_cw(p.Cout);  // output plane: channels per row chunk
+    constexpr int kUnits = MT * (N / 32);  // epilogue units (64 rows x 32 columns) per work item and warpgroup
     for (int work = blockIdx.x; work < p.n_work; work += gridDim.x) {
       const WorkItem wi = decode_work(p, work);
       const int delta = (kPadRows + wi.m0 + p.omin) & 7;  // rows the window start was rounded down by
@@ -324,44 +325,63 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(const __grid_con
       // 16 consecutive columns (the fp16 plane stores 8 channels and the F32B plane 4 channels per 16-byte access)
       const int valid_out = p.lengths ? min(p.Lout, p.lengths[wi.b] * p.len_mul_out) : p.Lout;
       const int row_in_tile = tid & 63;
+      // global reads of unit k: residual (rv / rh) and running sum (ov).  Where the accumulators leave room for a second register
+      // set (MT x N / 2 <= 64 of them; 128 spill), they are issued one unit ahead, before the previous unit goes through shared
+      // memory.
+      constexpr bool kLoadAhead = MT * N / 2 <= 64;
+      constexpr int kSets = kLoadAhead ? 2 : 1;
+      float4 rv[kSets][UC / 4], ov[kSets][UC / 4];
+      uint4 rh[kSets][UC / 8];
+      auto load_unit = [&](int k, float4 (&rv)[UC / 4], float4 (&ov)[UC / 4], uint4 (&rh)[UC / 8]) {
+        const int mt = k / (N / 32);
+        const int col0 = (k % (N / 32)) * 32 + (tid >> 6) * UC;
+        const int q = wi.m0 + (g * MT + mt) * 64 + row_in_tile;
+        const int lo = q * p.stride + wi.r;
+        const bool inb = q < p.Lin && (g * MT + mt) * 64 + row_in_tile < p.rows_item;
+        const size_t i32 = ((size_t)wi.b * C4 + (col0 >> 2)) * p.Lout + lo;  // + g * Lout per 4 channels
+        if (inb && p.res32) {
 #pragma unroll
-      for (int mt = 0; mt < MT; ++mt) {
+          for (int j = 0; j < UC / 4; ++j) rv[j] = reinterpret_cast<const float4*>(p.res32)[i32 + (size_t)j * p.Lout];
+        }
+        if (inb && p.res16) {  // (the lo halves of a hi/lo residual share rv's registers: res32 and res16 are exclusive)
+          const int rr = kPadRows + lo;
+          if (!p.res_hilo) {
+            const size_t rbase = (((size_t)wi.b * (p.Cout / ocw) + col0 / ocw) * p.res_Lp + rr) * (size_t)(ocw >> 3);
+            const int c0 = (col0 & (ocw - 1)) >> 3, sw = f16_swz(ocw, rr);
 #pragma unroll
-        for (int u = 0; u < N / 32; ++u) {
+            for (int j = 0; j < UC / 8; ++j) rh[j] = reinterpret_cast<const uint4*>(p.res16)[rbase + (size_t)((c0 + j) ^ sw)];
+          } else {
+            // hi/lo plane: rows of 64 channels; hi block = channels [0, Cout), lo block = [Cout, 2 Cout)
+            const int nch = (2 * p.Cout) >> 6, sw = f16_swz(64, rr);
+#pragma unroll
+            for (int j = 0; j < UC / 8; ++j) {
+              const int ch = col0 + 8 * j, cl = ch + p.Cout;
+              rh[j] = reinterpret_cast<const uint4*>(p.res16)[(((size_t)wi.b * nch + (ch >> 6)) * p.res_Lp + rr) * 8 + (size_t)(((ch & 63) >> 3) ^ sw)];
+              rv[j] = reinterpret_cast<const float4*>(p.res16)[(((size_t)wi.b * nch + (cl >> 6)) * p.res_Lp + rr) * 8 + (size_t)(((cl & 63) >> 3) ^ sw)];
+            }
+          }
+        }
+        if (inb && p.mode != EPI_STORE && !p.red_add) {
+#pragma unroll
+          for (int j = 0; j < UC / 4; ++j) ov[j] = reinterpret_cast<const float4*>(p.y32)[i32 + (size_t)j * p.Lout];
+        }
+      };
+      if constexpr (kLoadAhead) load_unit(0, rv[0], ov[0], rh[0]);
+#pragma unroll
+      for (int k = 0; k < kUnits; ++k) {
+        {
+          const int mt = k / (N / 32), u = k % (N / 32);
           const int col0 = u * 32 + (tid >> 6) * UC;
           const int q = wi.m0 + (g * MT + mt) * 64 + row_in_tile;
           const int lo = q * p.stride + wi.r;
           const bool inb = q < p.Lin && (g * MT + mt) * 64 + row_in_tile < p.rows_item;
           const bool live = inb && lo < valid_out;
           const size_t i32 = ((size_t)wi.b * C4 + (col0 >> 2)) * p.Lout + lo;  // + g * Lout per 4 channels
-          float4 rv[UC / 4], ov[UC / 4];
-          uint4 rh[UC / 8];
-          if (inb && p.res32) {
-#pragma unroll
-            for (int j = 0; j < UC / 4; ++j) rv[j] = reinterpret_cast<const float4*>(p.res32)[i32 + (size_t)j * p.Lout];
-          }
-          if (inb && p.res16) {  // (the lo halves of a hi/lo residual share rv's registers: res32 and res16 are exclusive)
-            const int rr = kPadRows + lo;
-            if (!p.res_hilo) {
-              const size_t rbase = (((size_t)wi.b * (p.Cout / ocw) + col0 / ocw) * p.res_Lp + rr) * (size_t)(ocw >> 3);
-              const int c0 = (col0 & (ocw - 1)) >> 3, sw = f16_swz(ocw, rr);
-#pragma unroll
-              for (int j = 0; j < UC / 8; ++j) rh[j] = reinterpret_cast<const uint4*>(p.res16)[rbase + (size_t)((c0 + j) ^ sw)];
-            } else {
-              // hi/lo plane: rows of 64 channels; hi block = channels [0, Cout), lo block = [Cout, 2 Cout)
-              const int nch = (2 * p.Cout) >> 6, sw = f16_swz(64, rr);
-#pragma unroll
-              for (int j = 0; j < UC / 8; ++j) {
-                const int ch = col0 + 8 * j, cl = ch + p.Cout;
-                rh[j] = reinterpret_cast<const uint4*>(p.res16)[(((size_t)wi.b * nch + (ch >> 6)) * p.res_Lp + rr) * 8 + (size_t)(((ch & 63) >> 3) ^ sw)];
-                rv[j] = reinterpret_cast<const float4*>(p.res16)[(((size_t)wi.b * nch + (cl >> 6)) * p.res_Lp + rr) * 8 + (size_t)(((cl & 63) >> 3) ^ sw)];
-              }
-            }
-          }
-          if (inb && p.mode != EPI_STORE && !p.red_add) {
-#pragma unroll
-            for (int j = 0; j < UC / 4; ++j) ov[j] = reinterpret_cast<const float4*>(p.y32)[i32 + (size_t)j * p.Lout];
-          }
+          if (!kLoadAhead) load_unit(k, rv[0], ov[0], rh[0]);
+          else if (k + 1 < kUnits) load_unit(k + 1, rv[(k + 1) % kSets], ov[(k + 1) % kSets], rh[(k + 1) % kSets]);
+          const float4(&rvk)[UC / 4] = rv[k % kSets];
+          const float4(&ovk)[UC / 4] = ov[k % kSets];
+          const uint4(&rhk)[UC / 8] = rh[k % kSets];
           group_sync(1 + g, 128);  // the previous unit's rows have been read
           stage_acc32(stage, &acc[mt][u * 16], tid);
           group_sync(1 + g, 128);
@@ -373,20 +393,20 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(const __grid_con
           if (p.res32) {
 #pragma unroll
             for (int j = 0; j < UC / 4; ++j) {
-              v[4 * j + 0] += rv[j].x; v[4 * j + 1] += rv[j].y; v[4 * j + 2] += rv[j].z; v[4 * j + 3] += rv[j].w;
+              v[4 * j + 0] += rvk[j].x; v[4 * j + 1] += rvk[j].y; v[4 * j + 2] += rvk[j].z; v[4 * j + 3] += rvk[j].w;
             }
           }
           if (p.res16) {
 #pragma unroll
             for (int j = 0; j < UC / 8; ++j) {
-              if (p.res_hilo) add_res16_hilo(&v[8 * j], rh[j], *reinterpret_cast<const uint4*>(&rv[j]), p.res_inv);
-              else add_res16(&v[8 * j], rh[j], p.res_inv);
+              if (p.res_hilo) add_res16_hilo(&v[8 * j], rhk[j], *reinterpret_cast<const uint4*>(&rvk[j]), p.res_inv);
+              else add_res16(&v[8 * j], rhk[j], p.res_inv);
             }
           }
           if (p.mode != EPI_STORE && !p.red_add) {
 #pragma unroll
             for (int j = 0; j < UC / 4; ++j) {
-              v[4 * j + 0] += ov[j].x; v[4 * j + 1] += ov[j].y; v[4 * j + 2] += ov[j].z; v[4 * j + 3] += ov[j].w;
+              v[4 * j + 0] += ovk[j].x; v[4 * j + 1] += ovk[j].y; v[4 * j + 2] += ovk[j].z; v[4 * j + 3] += ovk[j].w;
             }
             if (p.mode == EPI_ADD_DIV) {
 #pragma unroll
