@@ -597,6 +597,55 @@ size_t mb_ppgx_workspace_bytes(const mb_ppgx* h, int32_t batch, int32_t n_sample
 int mb_ppgx_forward(mb_ppgx* h, const float* wav, const int32_t* n_samples, int32_t batch, int32_t n_max, int32_t pe_len,
                     const float* pos_table, float* out, float* taps, void* workspace, size_t workspace_bytes, void* stream);
 
+/* test hook: ONE launch of a PPG-extractor kernel on caller-provided device tensors (no model handle), through the launch
+ * helpers the forward uses; CONV2D_TC also packs w as finalize does (absmax -> tc_weight_scale -> conv2d_tc_pack).  Row b of a
+ * padded batch has len[b] valid entries of T.  "Operand tiles" are fp16 hi / lo planes [ceil(cols / 64)][rows_total][64] with
+ * 16-byte chunk c of row m at c ^ (m & 7), the layout every tensor-core GEMM of the extractor reads. */
+#define MB_PPGX_DBG_FRONTEND 0  /* log-mel of wav x [B][n_max] (len: samples, len2: frames) -> y [B][T][F]; w = melmat        */
+#define MB_PPGX_DBG_MVN 1       /* y [B][T][F] in place over len frames; flags 1 norm_means | 2 norm_vars                      */
+#define MB_PPGX_DBG_CONV0 2     /* relu(conv k/stride/pad of x [B][T][F], len frames; w [N][1][k][k]) -> y_hi / y_lo planes    */
+                                /*   [B][T_out][F_out][N] channels-last                                                        */
+#define MB_PPGX_DBG_CONV2D_TC 3 /* relu(conv of the planes x_hi + x_lo [B][T][F][C], len frames; w [N][C][k][k]) -> operand     */
+                                /*   tiles of [B T_out][N F_out] (column n F_out + f), zeroed first                            */
+#define MB_PPGX_DBG_LN_TILES 4  /* LayerNorm (w, bias) of x [M][D] -> operand tiles of [rows_total][D]                         */
+#define MB_PPGX_DBG_ACT_TILES 5 /* act of x [M][ld] columns [0, D) -> operand tiles of [rows_total][D]                         */
+#define MB_PPGX_DBG_LN_ROWS 6   /* LayerNorm (w, bias) of x [B T][D] -> y (may be x); flags 4: zero_pad rows t >= len[b]       */
+#define MB_PPGX_DBG_DW 7        /* GLU of x [B T][2 D], depthwise conv w [D][k] + bias, BatchNorm bn[4], act -> operand tiles  */
+#define MB_PPGX_DBG_ATTN 8      /* attention of x = qkv [B T][3 D], heads H x dk, rel: P [T][ldp], pos biases pu / pv [H][dk] */
+                                /*   -> y = ctx [B T][D]                                                                       */
+typedef struct mb_ppgx_debug_spec {
+  int32_t kind;                  /* MB_PPGX_DBG_* */
+  int32_t B, T;                  /* rows; padded frames of each row (FRONTEND: STFT frames of n_max; CONV*: input frames) */
+  const int32_t* len;            /* device [B]: valid samples (FRONTEND) / frames of each row */
+  const int32_t* len2;           /* FRONTEND: device [B] STFT frames of each row */
+  int32_t n_max, n_fft, win_length, hop_length;  /* FRONTEND */
+  int32_t F;                     /* mel bins (FRONTEND, MVN, CONV0); input plane width (CONV2D_TC) */
+  int32_t C, N;                  /* CONV2D_TC input channels; CONV0 / CONV2D_TC output channels */
+  int32_t k, stride, pad;        /* CONV0 / CONV2D_TC: k x k kernel; DW: kernel size (odd) */
+  int32_t M, D, ld, rows_total;  /* LN_TILES / ACT_TILES rows; features; ACT_TILES row stride; operand tile rows (x 128) */
+  int32_t act;                   /* ACT_TILES / DW: 0 none, 1 ReLU, 2 swish */
+  int32_t flags;                 /* MVN: 1 norm_means | 2 norm_vars; LN_ROWS: 4 zero_pad */
+  int32_t H, dk, ldp, rel;       /* ATTN */
+  const float* x;
+  const void* x_hi;              /* CONV2D_TC input planes (fp16) */
+  const void* x_lo;
+  const float* w;
+  const float* bias;
+  const float* bn[4];            /* DW: weight, bias, running_mean, running_var */
+  const float* P;
+  const float* pu;
+  const float* pv;
+  float* y;
+  void* y_hi;                    /* CONV0 planes / operand tiles (fp16) */
+  void* y_lo;
+} mb_ppgx_debug_spec;
+/* device workspace the spec needs */
+size_t mb_ppgx_debug_workspace_bytes(const mb_ppgx_debug_spec* spec);
+/* synchronises `stream` (CONV2D_TC reads the pack scale back); writes one line into `report`:
+ * "kernel=K inst=I grid=X,Y,Z inv_scale=S" (inst: NT of conv2d_tc, DK of attn_kernel, 0 otherwise) */
+int mb_ppgx_debug(const mb_ppgx_debug_spec* spec, void* workspace, size_t workspace_bytes, void* stream, char* report,
+                  size_t report_len);
+
 #ifdef __cplusplus
 }
 #endif

@@ -88,6 +88,29 @@ class TacoTcDebugSpec(C.Structure):
     ]
 
 
+MB_PPGX_DBG_FRONTEND = 0
+MB_PPGX_DBG_MVN = 1
+MB_PPGX_DBG_CONV0 = 2
+MB_PPGX_DBG_CONV2D_TC = 3
+MB_PPGX_DBG_LN_TILES = 4
+MB_PPGX_DBG_ACT_TILES = 5
+MB_PPGX_DBG_LN_ROWS = 6
+MB_PPGX_DBG_DW = 7
+MB_PPGX_DBG_ATTN = 8
+
+
+class PpgxDebugSpec(C.Structure):
+    _fields_ = [
+        ("kind", C.c_int32), ("B", C.c_int32), ("T", C.c_int32), ("len", C.c_void_p), ("len2", C.c_void_p),
+        ("n_max", C.c_int32), ("n_fft", C.c_int32), ("win_length", C.c_int32), ("hop_length", C.c_int32), ("F", C.c_int32),
+        ("C", C.c_int32), ("N", C.c_int32), ("k", C.c_int32), ("stride", C.c_int32), ("pad", C.c_int32), ("M", C.c_int32),
+        ("D", C.c_int32), ("ld", C.c_int32), ("rows_total", C.c_int32), ("act", C.c_int32), ("flags", C.c_int32),
+        ("H", C.c_int32), ("dk", C.c_int32), ("ldp", C.c_int32), ("rel", C.c_int32), ("x", C.c_void_p), ("x_hi", C.c_void_p),
+        ("x_lo", C.c_void_p), ("w", C.c_void_p), ("bias", C.c_void_p), ("bn", C.c_void_p * 4), ("P", C.c_void_p),
+        ("pu", C.c_void_p), ("pv", C.c_void_p), ("y", C.c_void_p), ("y_hi", C.c_void_p), ("y_lo", C.c_void_p),
+    ]
+
+
 class WaveRNNConfig(C.Structure):
     _fields_ = [
         ("rnn_dims", C.c_int32),
@@ -252,6 +275,8 @@ SIGNATURES = {
     "mb_ppgx_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.c_int32]),
     "mb_ppgx_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mb_ppgx_debug_workspace_bytes": (C.c_size_t, [C.POINTER(PpgxDebugSpec)]),
+    "mb_ppgx_debug": (C.c_int, [C.POINTER(PpgxDebugSpec), C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]),
 }
 
 _lib: Optional[C.CDLL] = None

@@ -20,6 +20,8 @@
 
 #include <climits>
 #include <cmath>
+#include <cstdint>
+#include <cstdio>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -652,23 +654,74 @@ int to_tiles(const float* src, int ld, int M, int K, int KB, int rows_total, int
   return MB_OK;
 }
 
-int ln_tiles(const mb_ppgx* h, const float* x, int M, int RT, const float* const (&ln)[2], __half* hi, __half* lo, cudaStream_t st) {
-  ln_tiles_kernel<<<RT / 8, 256, 0, st>>>(x, M, h->D, kb_of(h->D), RT, ln[0], ln[1], hi, lo);
+int ln_tiles(int D, const float* x, int M, int RT, const float* g, const float* be, __half* hi, __half* lo, cudaStream_t st) {
+  ln_tiles_kernel<<<RT / 8, 256, 0, st>>>(x, M, D, kb_of(D), RT, g, be, hi, lo);
   MB_LAUNCH_CHECK("ln_tiles_kernel");
+  return MB_OK;
+}
+
+int ln_rows(const float* x, float* dst, int M, int D, const float* g, const float* be, const int* len, int T, int zero_pad,
+            cudaStream_t st) {
+  ln_rows_kernel<<<(M + 7) / 8, 256, 0, st>>>(x, dst, M, D, g, be, len, T, zero_pad);
+  MB_LAUNCH_CHECK("ln_rows_kernel");
+  return MB_OK;
+}
+
+int launch_frontend(const float* wav, int n_max, const int* nsamp, const int* tf_len, int B, int Tf, int n_fft, int win, int hop,
+                    const float* melmat, int n_mels, float* feat, cudaStream_t st) {
+  const size_t smem = sizeof(double) * (3 * n_fft + n_fft / 2 + 1);
+  frontend_kernel<<<dim3(Tf, B), 256, smem, st>>>(wav, n_max, nsamp, tf_len, Tf, n_fft, win, hop, melmat, n_mels, feat);
+  MB_LAUNCH_CHECK("frontend_kernel");
+  return MB_OK;
+}
+
+int launch_mvn(float* feat, const int* tf_len, int B, int Tf, int F, int norm_means, int norm_vars, cudaStream_t st) {
+  mvn_kernel<<<B, 128, 0, st>>>(feat, tf_len, Tf, F, norm_means, norm_vars);
+  MB_LAUNCH_CHECK("mvn_kernel");
+  return MB_OK;
+}
+
+int launch_conv0(const float* feat, const int* tf_len, int B, int Tf, int F, const float* w, const float* bias, int D, int k, int s,
+                 int p, int T1, int F1, __half* y_hi, __half* y_lo, cudaStream_t st) {
+  const size_t per = (size_t)T1 * F1 * D;
+  conv0_kernel<<<dim3((unsigned)((per + 255) / 256), B), 256, 0, st>>>(feat, tf_len, Tf, F, w, bias, D, k, s, p, T1, F1, y_hi,
+                                                                         y_lo);
+  MB_LAUNCH_CHECK("conv0_kernel");
+  return MB_OK;
+}
+
+// embed.conv.2 into embed.out.0's operand tiles [kb_of(N F_out)][rows_total][64], zeroed first: the rows past M and the
+// columns past N F_out are read by the GEMM
+int run_conv2d(const ppgx::Conv2dTcArgs& c, cudaStream_t st) {
+  const size_t bytes = sizeof(__half) * (size_t)kb_of(c.N * c.F_out) * c.rows_total * 64;
+  MB_CUDA_CHECK(cudaMemsetAsync(c.y_hi, 0, bytes, st));
+  MB_CUDA_CHECK(cudaMemsetAsync(c.y_lo, 0, bytes, st));
+  const cudaError_t e = ppgx::launch_conv2d_tc(c, st);
+  if (e != cudaSuccess) return fail(MB_ERR_CUDA, "conv2d_tc launch failed: %s", cudaGetErrorString(e));
+  count_launch();
+  return MB_OK;
+}
+
+int launch_dw(const float* pw, int D, int M, int T, const int* len, const float* w, const float* bias, int K, const float* bn_w,
+              const float* bn_b, const float* bn_m, const float* bn_v, int act, int RT, __half* hi, __half* lo, cudaStream_t st) {
+  const size_t n = (size_t)kb_of(D) * RT * 8;
+  dw_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pw, D, M, T, len, w, bias, K, bn_w, bn_b, bn_m, bn_v, act, kb_of(D), RT,
+                                                         hi, lo);
+  MB_LAUNCH_CHECK("dw_kernel");
   return MB_OK;
 }
 
 int attention_dk(int dk) { return dk <= 16 ? 16 : dk <= 32 ? 32 : dk <= 40 ? 40 : dk <= 64 ? 64 : 0; }
 
-int launch_attn(const mb_ppgx* h, const float* qkv, const float* P, const float* pu, const float* pv, const int* len, int B,
-                int T, float* ctx, cudaStream_t st) {
-  dim3 grid((T + kQ - 1) / kQ, h->H, B);
-  const size_t smem = sizeof(float) * 6 * kKT * h->dk;
-  const int ldp = h->nb * h->D;
-  switch (attention_dk(h->dk)) {
+// attention of B rows of T padded frames: qkv [B T][3 D], heads of dk at column h dk, P rows at stride ldp (rel only)
+int launch_attn(const float* qkv, const float* P, int ldp, const float* pu, const float* pv, const int* len, int B, int T, int H,
+                int dk, int D, int rel, float* ctx, cudaStream_t st) {
+  dim3 grid((T + kQ - 1) / kQ, H, B);
+  const size_t smem = sizeof(float) * 6 * kKT * dk;
+  switch (attention_dk(dk)) {
 #define MB_ATTN(DK)                                                                                                       \
   case DK:                                                                                                                \
-    attn_kernel<DK><<<grid, 128, smem, st>>>(qkv, P, ldp, pu, pv, len, T, h->D, h->dk, h->rel ? 1 : 0, ctx);            \
+    attn_kernel<DK><<<grid, 128, smem, st>>>(qkv, P, ldp, pu, pv, len, T, D, dk, rel, ctx);                              \
     break;
     MB_ATTN(16)
     MB_ATTN(32)
@@ -676,7 +729,7 @@ int launch_attn(const mb_ppgx* h, const float* qkv, const float* P, const float*
     MB_ATTN(64)
 #undef MB_ATTN
     default:
-      return fail(MB_ERR_INVALID, "attention head dim %d > 64", h->dk);
+      return fail(MB_ERR_INVALID, "attention head dim %d > 64", dk);
   }
   MB_LAUNCH_CHECK("attn_kernel");
   return MB_OK;
@@ -912,21 +965,13 @@ int mb_ppgx_forward(mb_ppgx* h, const float* wav, const int32_t* n_samples, int3
   float* ctx = reinterpret_cast<float*>(ws + L.ctx);
 
   // frontend + MVN
-  {
-    const size_t smem = sizeof(double) * (3 * h->cfg.n_fft + h->n_freq);
-    frontend_kernel<<<dim3(L.Tf, B), 256, smem, st>>>(wav, n_max, d_n, d_tf, L.Tf, h->cfg.n_fft, h->cfg.win_length,
-                                                       h->cfg.hop_length, h->melmat, h->F, feat);
-    MB_LAUNCH_CHECK("frontend_kernel");
-    mvn_kernel<<<B, 128, 0, st>>>(feat, d_tf, L.Tf, h->F, h->cfg.norm_means, h->cfg.norm_vars);
-    MB_LAUNCH_CHECK("mvn_kernel");
-  }
+  MB_TRY(launch_frontend(wav, n_max, d_n, d_tf, B, L.Tf, h->cfg.n_fft, h->cfg.win_length, h->cfg.hop_length, h->melmat, h->F,
+                         feat, st));
+  MB_TRY(launch_mvn(feat, d_tf, B, L.Tf, h->F, h->cfg.norm_means, h->cfg.norm_vars, st));
   // input layer
   {
-    const size_t per = (size_t)L.T1 * h->F1 * D;
-    conv0_kernel<<<dim3((unsigned)((per + 255) / 256), B), 256, 0, st>>>(
-        feat, d_tf, L.Tf, h->F, h->conv0_w, h->conv0_b, D, h->k0, h->s0, h->p0,
-        L.T1, h->F1, hp(L.pl_hi), hp(L.pl_lo));
-    MB_LAUNCH_CHECK("conv0_kernel");
+    MB_TRY(launch_conv0(feat, d_tf, B, L.Tf, h->F, h->conv0_w, h->conv0_b, D, h->k0, h->s0, h->p0, L.T1, h->F1, hp(L.pl_hi),
+                        hp(L.pl_lo), st));
     ppgx::Conv2dTcArgs c{};
     c.x_hi = hp(L.pl_hi);
     c.x_lo = hp(L.pl_lo);
@@ -940,12 +985,7 @@ int mb_ppgx_forward(mb_ppgx* h, const float* wav, const int32_t* n_samples, int3
     c.y_hi = hp(L.e_hi);
     c.y_lo = hp(L.e_lo);
     c.rows_total = RT;
-    // rows past M of the operand tiles are read by the GEMM: keep them zero
-    MB_CUDA_CHECK(cudaMemsetAsync(ws + L.e_hi, 0, sizeof(__half) * (size_t)L.KBe * RT * 64, st));
-    MB_CUDA_CHECK(cudaMemsetAsync(ws + L.e_lo, 0, sizeof(__half) * (size_t)L.KBe * RT * 64, st));
-    const cudaError_t e = ppgx::launch_conv2d_tc(c, st);
-    if (e != cudaSuccess) return fail(MB_ERR_CUDA, "conv2d_tc launch failed: %s", cudaGetErrorString(e));
-    count_launch();
+    MB_TRY(run_conv2d(c, st));
     MB_TRY(run_gemm(h, h->g[0], hp(L.e_hi), hp(L.e_lo), M, RT, nullptr, y, D, st));
     const size_t n = (size_t)M * D;
     embed_finish_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(y, x, M, D, T, sqrtf((float)D), h->rel ? nullptr : pos_table);
@@ -974,39 +1014,159 @@ int mb_ppgx_forward(mb_ppgx* h, const float* wav, const int32_t* n_samples, int3
     auto ffn = [&](const float* const (&norm)[2]) -> int {
       const Gemm &w1 = h->g[gi], &w2 = h->g[gi + 1];
       gi += 2;
-      MB_TRY(ln_tiles(h, x, M, RT, norm, th, tl, st));
+      MB_TRY(ln_tiles(D, x, M, RT, norm[0], norm[1], th, tl, st));
       MB_TRY(run_gemm(h, w1, th, tl, M, RT, nullptr, y, h->U, st));
       MB_TRY(to_tiles(y, h->U, M, h->U, kb_of(h->U), RT, act, th, tl, st));
       return run_gemm(h, w2, th, tl, M, RT, x, x, D, st);  // x += ff_scale * w_2(.)
     };
     if (h->cfg.macaron_style) MB_TRY(ffn(w.ln_mac));
-    MB_TRY(ln_tiles(h, x, M, RT, w.ln_mha, th, tl, st));
+    MB_TRY(ln_tiles(D, x, M, RT, w.ln_mha[0], w.ln_mha[1], th, tl, st));
     MB_TRY(run_gemm(h, g_qkv, th, tl, M, RT, nullptr, y, 3 * D, st));
-    MB_TRY(launch_attn(h, y, h->rel ? P + (size_t)i * D : nullptr, w.pu, w.pv, d_t, B, T, ctx, st));
+    MB_TRY(launch_attn(y, h->rel ? P + (size_t)i * D : nullptr, h->nb * D, w.pu, w.pv, d_t, B, T, h->H, h->dk, D, h->rel ? 1 : 0,
+                       ctx, st));
     MB_TRY(to_tiles(ctx, D, M, D, kb_of(D), RT, 0, th, tl, st));
     MB_TRY(run_gemm(h, g_out, th, tl, M, RT, x, x, D, st));
     if (h->cfg.use_cnn_module) {
       // the block's GEMM order is qkv, out, (macaron), ffn, conv: the conv module's pair sits after the FFN pair(s)
       const int gc = gi + 2;
-      MB_TRY(ln_tiles(h, x, M, RT, w.ln_conv, th, tl, st));
+      MB_TRY(ln_tiles(D, x, M, RT, w.ln_conv[0], w.ln_conv[1], th, tl, st));
       MB_TRY(run_gemm(h, h->g[gc], th, tl, M, RT, nullptr, y, 2 * D, st));
-      const size_t n = (size_t)kb_of(D) * RT * 8;
-      dw_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
-          y, D, M, T, d_t, w.dw_w, w.dw_b, h->cfg.cnn_module_kernel, w.bn_w, w.bn_b, w.bn_m, w.bn_v, act, kb_of(D), RT, th,
-          tl);
-      MB_LAUNCH_CHECK("dw_kernel");
+      MB_TRY(launch_dw(y, D, M, T, d_t, w.dw_w, w.dw_b, h->cfg.cnn_module_kernel, w.bn_w, w.bn_b, w.bn_m, w.bn_v, act, RT, th, tl,
+                       st));
       MB_TRY(run_gemm(h, h->g[gc + 1], th, tl, M, RT, x, x, D, st));
     }
     MB_TRY(ffn(w.ln_ff));
-    if (h->cfg.use_cnn_module) {
-      ln_rows_kernel<<<(M + 7) / 8, 256, 0, st>>>(x, x, M, D, w.ln_final[0], w.ln_final[1], d_t, T, 0);
-      MB_LAUNCH_CHECK("ln_rows_kernel");
-    }
+    if (h->cfg.use_cnn_module) MB_TRY(ln_rows(x, x, M, D, w.ln_final[0], w.ln_final[1], d_t, T, 0, st));
     MB_TRY(tap(i + 1));
   }
-  ln_rows_kernel<<<(M + 7) / 8, 256, 0, st>>>(x, out, M, D, h->after_w, h->after_b,
-                                              d_t, T, 1);
-  MB_LAUNCH_CHECK("ln_rows_kernel");
+  return ln_rows(x, out, M, D, h->after_w, h->after_b, d_t, T, 1, st);
+}
+
+// ---------------------------------------------------------------------------------------------- one-launch test hook
+size_t mb_ppgx_debug_workspace_bytes(const mb_ppgx_debug_spec* s) {
+  if (!s) return 0;
+  if (s->kind != MB_PPGX_DBG_CONV2D_TC) return 256;
+  return 2048 + mb::align_up(ppgx::conv2d_tc_weight_bytes(s->N, s->C, s->k, s->k), 1024);  // absmax slot, then the image
+}
+
+int mb_ppgx_debug(const mb_ppgx_debug_spec* spec, void* workspace, size_t workspace_bytes, void* stream, char* report,
+                  size_t report_len) {
+  const char* me = "mb_ppgx_debug";
+  if (!spec || !workspace) return fail(MB_ERR_INVALID, "%s: null argument", me);
+  const mb_ppgx_debug_spec& s = *spec;
+  const size_t need = mb_ppgx_debug_workspace_bytes(spec);
+  if (workspace_bytes < need) return fail(MB_ERR_WORKSPACE, "%s: workspace %zu < %zu bytes", me, workspace_bytes, need);
+  const bool rows = s.kind != MB_PPGX_DBG_LN_TILES && s.kind != MB_PPGX_DBG_ACT_TILES;  // kinds over a padded batch
+  if (rows && (s.B < 1 || s.T < 1 || !s.len)) return fail(MB_ERR_INVALID, "%s: B %d / T %d / len", me, s.B, s.T);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  auto hp = [](void* p) { return static_cast<__half*>(p); };
+  const char* kname = "";
+  int inst = 0;
+  dim3 grid(0, 0, 0);
+  float inv_scale = 1.f;
+  switch (s.kind) {
+    case MB_PPGX_DBG_FRONTEND:
+      if (s.n_fft < 2 || s.n_fft > kMaxFft || s.win_length < 1 || s.win_length > s.n_fft || s.hop_length < 1 || !s.len2)
+        return fail(MB_ERR_INVALID, "%s: n_fft %d / win_length %d / hop_length %d", me, s.n_fft, s.win_length, s.hop_length);
+      MB_TRY(launch_frontend(s.x, s.n_max, s.len, s.len2, s.B, s.T, s.n_fft, s.win_length, s.hop_length, s.w, s.F, s.y, st));
+      kname = "frontend_kernel";
+      grid = dim3(s.T, s.B);
+      break;
+    case MB_PPGX_DBG_MVN:
+      MB_TRY(launch_mvn(s.y, s.len, s.B, s.T, s.F, s.flags & 1, (s.flags >> 1) & 1, st));
+      kname = "mvn_kernel";
+      grid = dim3(s.B);
+      break;
+    case MB_PPGX_DBG_CONV0: {
+      const int T1 = mb_ppgx::conv_len(s.T, s.k, s.stride, s.pad), F1 = mb_ppgx::conv_len(s.F, s.k, s.stride, s.pad);
+      if (T1 < 1 || F1 < 1) return fail(MB_ERR_INVALID, "%s: conv0 output %d x %d", me, T1, F1);
+      MB_TRY(launch_conv0(s.x, s.len, s.B, s.T, s.F, s.w, s.bias, s.N, s.k, s.stride, s.pad, T1, F1, hp(s.y_hi), hp(s.y_lo), st));
+      kname = "conv0_kernel";
+      grid = dim3((unsigned)(((size_t)T1 * F1 * s.N + 255) / 256), s.B);
+      break;
+    }
+    case MB_PPGX_DBG_CONV2D_TC: {
+      const int NT = ppgx::conv2d_tc_ntile(s.N);
+      ppgx::Conv2dTcArgs c{};
+      c.x_hi = static_cast<const __half*>(s.x_hi);
+      c.x_lo = static_cast<const __half*>(s.x_lo);
+      c.len_in = s.len;
+      c.B = s.B, c.T_in = s.T, c.F_in = s.F, c.C = s.C;
+      c.T_out = mb_ppgx::conv_len(s.T, s.k, s.stride, s.pad), c.F_out = mb_ppgx::conv_len(s.F, s.k, s.stride, s.pad);
+      c.kh = c.kw = s.k, c.stride = s.stride, c.pad = s.pad;
+      c.N = s.N, c.K = s.k * s.k * s.C, c.KB = kb_of(c.K);
+      c.bias = s.bias;
+      c.y_hi = hp(s.y_hi);
+      c.y_lo = hp(s.y_lo);
+      c.rows_total = s.rows_total;
+      if (NT == 0 || s.C % 8 || c.T_out < 1 || c.F_out < 1 || s.rows_total % 128 || s.rows_total < s.B * c.T_out)
+        return fail(MB_ERR_INVALID, "%s: conv2d N %d / C %d / output %d x %d / rows_total %d", me, s.N, s.C, c.T_out, c.F_out,
+                    s.rows_total);
+      // as finalize: max |w| -> power-of-two scale (one host read-back) -> packed image
+      char* ws = reinterpret_cast<char*>(((uintptr_t)workspace + 1023) & ~(uintptr_t)1023);
+      unsigned int* d_abs = reinterpret_cast<unsigned int*>(ws);
+      __half* img = reinterpret_cast<__half*>(ws + 1024);
+      if (reinterpret_cast<char*>(img) + ppgx::conv2d_tc_weight_bytes(s.N, s.C, s.k, s.k) >
+          static_cast<char*>(workspace) + workspace_bytes)
+        return fail(MB_ERR_WORKSPACE, "%s: workspace too small for the weight image", me);
+      MB_CUDA_CHECK(cudaMemsetAsync(d_abs, 0, sizeof(unsigned int), st));
+      cudaError_t e = taco::tc_skinny_absmax(s.w, (size_t)s.N * s.C * s.k * s.k, d_abs, st);
+      if (e != cudaSuccess) return fail(MB_ERR_CUDA, "absmax: %s", cudaGetErrorString(e));
+      unsigned int bits = 0;
+      MB_CUDA_CHECK(cudaMemcpyAsync(&bits, d_abs, sizeof(bits), cudaMemcpyDeviceToHost, st));
+      MB_CUDA_CHECK(cudaStreamSynchronize(st));
+      const float scale = taco::tc_weight_scale(bits);
+      inv_scale = 1.f / scale;
+      c.inv_scale = inv_scale;
+      c.w = img;
+      e = ppgx::conv2d_tc_pack(s.w, s.N, s.C, s.k, s.k, scale, img, st);
+      if (e != cudaSuccess) return fail(MB_ERR_CUDA, "conv2d pack: %s", cudaGetErrorString(e));
+      count_launch();
+      MB_TRY(run_conv2d(c, st));
+      kname = "conv2d_tc";
+      inst = NT;
+      grid = dim3((unsigned)((s.B * c.T_out * c.F_out + 127) / 128), (unsigned)(s.N / NT));
+      break;
+    }
+    case MB_PPGX_DBG_LN_TILES:
+      if (s.rows_total % 128 || s.M > s.rows_total) return fail(MB_ERR_INVALID, "%s: rows_total %d", me, s.rows_total);
+      MB_TRY(ln_tiles(s.D, s.x, s.M, s.rows_total, s.w, s.bias, hp(s.y_hi), hp(s.y_lo), st));
+      kname = "ln_tiles_kernel";
+      grid = dim3(s.rows_total / 8);
+      break;
+    case MB_PPGX_DBG_ACT_TILES:
+      if (s.rows_total % 128 || s.M > s.rows_total) return fail(MB_ERR_INVALID, "%s: rows_total %d", me, s.rows_total);
+      MB_TRY(to_tiles(s.x, s.ld, s.M, s.D, kb_of(s.D), s.rows_total, s.act, hp(s.y_hi), hp(s.y_lo), st));
+      kname = "act_tiles_kernel";
+      grid = dim3((unsigned)(((size_t)kb_of(s.D) * s.rows_total * 8 + 255) / 256));
+      break;
+    case MB_PPGX_DBG_LN_ROWS:
+      MB_TRY(ln_rows(s.x, s.y, s.B * s.T, s.D, s.w, s.bias, s.len, s.T, (s.flags >> 2) & 1, st));
+      kname = "ln_rows_kernel";
+      grid = dim3((s.B * s.T + 7) / 8);
+      break;
+    case MB_PPGX_DBG_DW:
+      if (s.k < 1 || s.k % 2 == 0 || s.rows_total % 128 || s.B * s.T > s.rows_total)
+        return fail(MB_ERR_INVALID, "%s: dw kernel %d / rows_total %d", me, s.k, s.rows_total);
+      MB_TRY(launch_dw(s.x, s.D, s.B * s.T, s.T, s.len, s.w, s.bias, s.k, s.bn[0], s.bn[1], s.bn[2], s.bn[3], s.act, s.rows_total,
+                       hp(s.y_hi), hp(s.y_lo), st));
+      kname = "dw_kernel";
+      grid = dim3((unsigned)(((size_t)kb_of(s.D) * s.rows_total * 8 + 255) / 256));
+      break;
+    case MB_PPGX_DBG_ATTN:
+      if (s.H < 1 || s.dk < 1 || s.H * s.dk > s.D) return fail(MB_ERR_INVALID, "%s: H %d x dk %d > D %d", me, s.H, s.dk, s.D);
+      MB_TRY(launch_attn(s.x, s.P, s.ldp, s.pu, s.pv, s.len, s.B, s.T, s.H, s.dk, s.D, s.rel, s.y, st));
+      kname = "attn_kernel";
+      inst = attention_dk(s.dk);
+      grid = dim3((s.T + kQ - 1) / kQ, s.H, s.B);
+      break;
+    default:
+      return fail(MB_ERR_INVALID, "%s: bad kind %d", me, s.kind);
+  }
+  MB_CUDA_CHECK(cudaStreamSynchronize(st));
+  if (report && report_len)
+    snprintf(report, report_len, "kernel=%s inst=%d grid=%u,%u,%u inv_scale=%.9e\n", kname, inst, grid.x, grid.y, grid.z,
+             (double)inv_scale);
   return MB_OK;
 }
 

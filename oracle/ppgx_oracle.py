@@ -107,6 +107,19 @@ def rel_shift_closed_form(bd: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def attention(q, kk, v, pp=None, pos_u=None, pos_v=None):
+    """softmax(scores) . V of one utterance: q [1, T, H, dk], kk / v / pp [1, H, T, dk] (pp = linear_pos(pos_emb), rel_pos
+    only), pos_u / pos_v [H, dk] -> [1, T, H dk].  rel_pos (pp given): ((q + u) k^T + rel_shift((q + v) p^T)) / sqrt(dk)"""
+    dk = q.shape[-1]
+    if pp is not None:
+        qu = (q + pos_u).transpose(1, 2)
+        qv = (q + pos_v).transpose(1, 2)
+        scores = (torch.matmul(qu, kk.transpose(-2, -1)) + rel_shift(torch.matmul(qv, pp.transpose(-2, -1)))) / math.sqrt(dk)
+    else:
+        scores = torch.matmul(q.transpose(1, 2), kk.transpose(-2, -1)) / math.sqrt(dk)
+    return torch.matmul(torch.softmax(scores, dim=-1), v).transpose(1, 2).contiguous().view(1, q.shape[1], -1)
+
+
 def _ln(x, sd, name):
     return F.layer_norm(x, (x.shape[-1],), sd[name + ".weight"], sd[name + ".bias"], 1e-12)
 
@@ -155,14 +168,10 @@ def forward(sd: Dict[str, torch.Tensor], cfg: dict, wav: torch.Tensor, pe_len: O
         q = _lin(h, sd, pre + ".self_attn.linear_q").view(1, T, H, dk)
         kk = _lin(h, sd, pre + ".self_attn.linear_k").view(1, T, H, dk).transpose(1, 2)
         v = _lin(h, sd, pre + ".self_attn.linear_v").view(1, T, H, dk).transpose(1, 2)
+        pp = None
         if rel:
             pp = F.linear(pos_emb, sd[pre + ".self_attn.linear_pos.weight"]).view(1, -1, H, dk).transpose(1, 2)
-            qu = (q + sd[pre + ".self_attn.pos_bias_u"]).transpose(1, 2)
-            qv = (q + sd[pre + ".self_attn.pos_bias_v"]).transpose(1, 2)
-            scores = (torch.matmul(qu, kk.transpose(-2, -1)) + rel_shift(torch.matmul(qv, pp.transpose(-2, -1)))) / math.sqrt(dk)
-        else:
-            scores = torch.matmul(q.transpose(1, 2), kk.transpose(-2, -1)) / math.sqrt(dk)
-        a = torch.matmul(torch.softmax(scores, dim=-1), v).transpose(1, 2).contiguous().view(1, -1, D)
+        a = attention(q, kk, v, pp, sd.get(pre + ".self_attn.pos_bias_u"), sd.get(pre + ".self_attn.pos_bias_v"))
         x = x + _lin(a, sd, pre + ".self_attn.linear_out")
         if f"{pre}.conv_module.pointwise_conv1.weight" in sd:
             cm = pre + ".conv_module"
