@@ -528,6 +528,8 @@ int mb_ppg2mel_set_arena(mb_ppg2mel* h, void* arena, size_t bytes);
 int mb_ppg2mel_set_weight(mb_ppg2mel* h, const char* name, const float* w, const int64_t* dims, int32_t ndim,
                           void* stream);
 int mb_ppg2mel_finalize(mb_ppg2mel* h, void* stream);
+/* 0 when frames < 4, when the device query fails, or when T_enc = frames / 4 needs more shared memory than the MoL
+ * attention kernel can have (the message names the limit: 29 039 on an H100 80GB HBM3) */
 size_t mb_ppg2mel_workspace_bytes(const mb_ppg2mel* h, int32_t batch, int32_t frames);
 
 /* MelDecoderMOLv2.inference for a padded batch of 1..128 rows, each row computed as its own B = 1 call:
@@ -538,6 +540,8 @@ size_t mb_ppg2mel_workspace_bytes(const mb_ppg2mel* h, int32_t batch, int32_t fr
  *   outputs (device, zero-filled past each row's end): mel / mel_post fp32 [B][2 S][80], align fp32 [B][S][frames / 4],
  *     stop fp32 [B][S] (stop logits, may be NULL); steps_host int32 [B] (host): decoder steps n of each row (2 n mel
  *     frames, n alignment rows).
+ * frames / 4 above the attention's shared-memory limit (see mb_ppg2mel_workspace_bytes) is MB_ERR_INVALID, before anything is
+ * queued.
  * Row b stops after step n when sigmoid(stop) > 0.5 and n >= 2 T_enc[b] - 5, or when n = 2 T_enc[b]; a finished row
  * is frozen while the others run on.  The decoder steps are replayed from a CUDA graph of 16 steps on an internal
  * stream ordered after `stream` (events); the host polls the finished rows once per graph replay. */

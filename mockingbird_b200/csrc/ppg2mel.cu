@@ -14,6 +14,7 @@
 // division.  See DESIGN.md section 4g for the kernel map and the precision study of the MoL attention.
 #include <cuda_runtime.h>
 
+#include <atomic>
 #include <climits>
 #include <cstring>
 #include <string>
@@ -650,6 +651,39 @@ int launch_in(float* x, int T, const int* len, const float* add, int B, cudaStre
   return MB_OK;
 }
 
+// dynamic shared memory of mol_attention_kernel: phi [Te_buf + 1] and alpha [Te_buf]
+size_t att_smem_bytes(int Te_buf) { return sizeof(float) * (2 * (size_t)Te_buf + 1); }
+
+// largest Te_buf whose attention shared memory fits one block: the device's opt-in limit less the kernel's static
+// arrays, queried once per device; 0 (with a message) when the device cannot be queried
+int max_att_tenc() {
+  constexpr int kMaxDevices = 64;
+  static std::atomic<int> cached[kMaxDevices];
+  int dev = 0, optin = 0;
+  cudaFuncAttributes fa{};
+  if (cudaGetDevice(&dev) != cudaSuccess) {
+    const cudaError_t e = cudaGetLastError();
+    fail(MB_ERR_CUDA, "ppg2mel: no current device for the attention's shared-memory limit: %s", cudaGetErrorString(e));
+    return 0;
+  }
+  if (dev < kMaxDevices) {
+    const int te = cached[dev].load(std::memory_order_relaxed);
+    if (te > 0) return te;
+  }
+  if (cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
+      cudaFuncGetAttributes(&fa, mol_attention_kernel) != cudaSuccess) {
+    const cudaError_t e = cudaGetLastError();
+    fail(MB_ERR_CUDA, "ppg2mel: cannot query the attention kernel's shared-memory limit: %s", cudaGetErrorString(e));
+    return 0;
+  }
+  const size_t room = (size_t)optin - fa.sharedSizeBytes;
+  int te = (int)((room / sizeof(float) - 1) / 2);
+  while (te > 0 && att_smem_bytes(te) > room) --te;
+  while (att_smem_bytes(te + 1) <= room) ++te;
+  if (dev < kMaxDevices) cached[dev].store(te, std::memory_order_relaxed);
+  return te;
+}
+
 #define MB_TRY(x)               \
   do {                          \
     const int _rc = (x);        \
@@ -745,6 +779,18 @@ int mb_ppg2mel_finalize(mb_ppg2mel* h, void* stream) {
 
 size_t mb_ppg2mel_workspace_bytes(const mb_ppg2mel* h, int32_t batch, int32_t frames) {
   if (!h || batch < 1 || frames < 4) return 0;
+  int dev = 0;
+  if (cudaGetDevice(&dev) == cudaSuccess) {  // without a device nothing can run: the size alone is still answered
+    const int te_max = max_att_tenc();
+    if (te_max == 0) return 0;  // the query failed: mb_last_error says why
+    if (frames / 4 > te_max) {
+      fail(MB_ERR_INVALID, "mb_ppg2mel_workspace_bytes: frames %d gives T_enc %d > %d, the most the MoL attention's shared "
+           "memory holds (frames <= %d)", frames, frames / 4, te_max, 4 * te_max + 3);
+      return 0;
+    }
+  } else {
+    cudaGetLastError();
+  }
   return ws_layout(batch, frames).total;
 }
 
@@ -756,6 +802,11 @@ int mb_ppg2mel_inference(mb_ppg2mel* h, const float* ppg, const float* lf0_uv, c
   if (!h->finalized) return fail(MB_ERR_STATE, "mb_ppg2mel_inference: weights not finalized");
   if (batch < 1 || batch > kMaxRows) return fail(MB_ERR_INVALID, "mb_ppg2mel_inference: batch %d outside 1..%d", batch, kMaxRows);
   if (frames < 4) return fail(MB_ERR_INVALID, "mb_ppg2mel_inference: frames %d < 4", frames);
+  const int te_max = max_att_tenc();
+  if (te_max == 0) return MB_ERR_CUDA;
+  if (frames / 4 > te_max)
+    return fail(MB_ERR_INVALID, "mb_ppg2mel_inference: frames %d gives T_enc %d > %d, the most the MoL attention's shared "
+                "memory holds (frames <= %d)", frames, frames / 4, te_max, 4 * te_max + 3);
   if (!ppg || !lf0_uv || !spk || !lengths || !mel || !mel_post || !align || !steps_host || !workspace)
     return fail(MB_ERR_INVALID, "mb_ppg2mel_inference: null argument");
   if ((mask1 == nullptr) != (mask2 == nullptr))
@@ -840,7 +891,7 @@ int mb_ppg2mel_inference(mb_ppg2mel* h, const float* ppg, const float* lf0_uv, c
   float* ah[2] = {F(L.ah), F(L.ah) + (size_t)B * kH};
   float* dh[2] = {F(L.dh), F(L.dh) + (size_t)B * kH};
   const dim3 rows_grid_h(kH / 8, (B + kRowsPerWarp - 1) / kRowsPerWarp);
-  const size_t att_smem = sizeof(float) * (2 * T2 + 1);
+  const size_t att_smem = att_smem_bytes(T2);
   if (att_smem > 48 * 1024)
     MB_CUDA_CHECK(cudaFuncSetAttribute(mol_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
   const float* A = h->arena;

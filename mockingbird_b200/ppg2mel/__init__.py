@@ -108,6 +108,9 @@ class MelDecoderMOLv2:
         Te = T // 4
         S = 2 * Te
         with torch.cuda.device(dev):
+            need = int(L.mb_ppg2mel_workspace_bytes(self._handle, B, T))
+            if need == 0:
+                raise ValueError(L.mb_last_error().decode())
             mel = torch.empty(B, 2 * S, self.num_mels, device=dev)
             post = torch.empty_like(mel)
             align = torch.empty(B, S, Te, device=dev)
@@ -118,7 +121,6 @@ class MelDecoderMOLv2:
                 m2 = masks[1].to(device=dev, dtype=torch.uint8).contiguous()
                 if tuple(m1.shape) != (S, B, 256) or tuple(m2.shape) != (S, B, 128):
                     raise ValueError(f"dropout masks must be [{S},{B},256] and [{S},{B},128]")
-            need = int(L.mb_ppg2mel_workspace_bytes(self._handle, B, T))
             if self._ws is None or self._ws.numel() < need:
                 self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
             lens = (C.c_int32 * B)(*lengths)

@@ -430,9 +430,10 @@ PPG2MEL_CONFIG = dict(num_speakers=1, spk_embed_dim=256, bottle_neck_feature_dim
                       mask_padding=True)
 
 
-def ppg2mel_state_dict(seed: int = 0, randomize_bn: bool = True) -> Dict[str, torch.Tensor]:
+def ppg2mel_state_dict(seed: int = 0, randomize_bn: bool = True, bnf_dim: int = 144,
+                       spk_dim: int = 256) -> Dict[str, torch.Tensor]:
     """``torch.manual_seed(seed); MelDecoderMOLv2(**PPG2MEL_CONFIG)`` state_dict rebuilt from stock torch layers in the
-    constructor's order.  The reference's ``Linear`` / ``Conv1d`` wrappers (utils/basic_layers.py:27-56) build the
+    constructor's order (``bnf_dim`` / ``spk_dim``: the config's bottle_neck_feature_dim / spk_embed_dim).  The reference's ``Linear`` / ``Conv1d`` wrappers (utils/basic_layers.py:27-56) build the
     torch layer (default init) and then redraw the weight with xavier_uniform_; MOLAttention.initialize_bias
     (utils/mol_attention.py:41-54) overwrites the sigma / Delta biases with constants (r = 2/4 < 1: Delta = -0.432).
     ``randomize_bn`` replaces the postnet BatchNorm statistics and affines (identity in a fresh module) by seeded draws."""
@@ -445,11 +446,11 @@ def ppg2mel_state_dict(seed: int = 0, randomize_bn: bool = True) -> Dict[str, to
         for n, p in m.state_dict().items():
             sd[f"{name}.{n}"] = p.detach().clone()
 
-    for branch, cin in (("bnf_prenet", 144), ("pitch_convs", 2)):
+    for branch, cin in (("bnf_prenet", bnf_dim), ("pitch_convs", 2)):
         put(f"{branch}.0", nn.Conv1d(cin, 256, 1, bias=False))
         put(f"{branch}.3", nn.Conv1d(256, 256, 4, 2, 1))
         put(f"{branch}.6", nn.Conv1d(256, 256, 4, 2, 1))
-    put("reduce_proj", nn.Linear(512, 256))
+    put("reduce_proj", nn.Linear(256 + spk_dim, 256))
 
     def xlinear(name, i, o, bias=True, g="linear"):
         m = nn.Linear(i, o, bias=bias)

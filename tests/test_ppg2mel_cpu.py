@@ -88,6 +88,13 @@ def test_state_dict_bit_identical_to_reference_constructor():
         assert ref[k].shape == sd[k].shape and torch.equal(ref[k], sd[k]), k
     n = sum(v.numel() for k, v in ref.items() if v.dtype.is_floating_point and "running" not in k)
     assert n == 10_396_576
+    # the feature widths are the only free config values: one non-default pair draws the same way
+    torch.manual_seed(0)
+    ref = MelDecoderMOLv2(**dict(ri.PPG2MEL_CONFIG, bottle_neck_feature_dim=37, spk_embed_dim=1024)).state_dict()
+    sd = ri.ppg2mel_state_dict(0, randomize_bn=False, bnf_dim=37, spk_dim=1024)
+    assert list(ref) == list(sd)
+    for k in ref:
+        assert ref[k].shape == sd[k].shape and torch.equal(ref[k], sd[k]), k
 
 
 def _cfg(**over):

@@ -7,6 +7,7 @@ import torch
 
 import golden_io
 import ppg2mel_oracle as po
+from ppg2mel_kernel_oracle import philox_keep as _philox_keep
 import ref_init as ri
 
 pytestmark = pytest.mark.gpu
@@ -163,22 +164,6 @@ def test_padding_frames_do_not_leak(model_c):
     for r in range(2):
         for a, b in zip(out[r], clean[r]):
             assert torch.equal(a, b), r
-
-
-def _philox_keep(seed, step, row, units, layer):
-    """Python restatement of the library's device-drawn keep flags (Philox-4x32-10, mb_wavernn_math.h)"""
-    M = 0xFFFFFFFF
-    out = []
-    for u in units:
-        c = [u >> 2, row, step, (0x70326D00 + layer) & M]
-        k0, k1 = seed & M, (seed >> 32) & M
-        for _ in range(10):
-            p0 = 0xD2511F53 * c[0]
-            p1 = 0xCD9E8D57 * c[2]
-            c = [((p1 >> 32) ^ c[1] ^ k0) & M, p1 & M, ((p0 >> 32) ^ c[3] ^ k1) & M, p0 & M]
-            k0, k1 = (k0 + 0x9E3779B9) & M, (k1 + 0xBB67AE85) & M
-        out.append((c[u & 3] >> 16) & 1)
-    return torch.tensor(out, dtype=torch.bool)
 
 
 def test_device_dropout_seeded(model_c):
