@@ -255,6 +255,37 @@ int mb_wavernn_generate_rows_mol(mb_wavernn* h, const int32_t* fold_starts_host,
                                  int32_t step0, int32_t nsteps, const float* uniforms, int32_t noise_folds, int32_t row0,
                                  uint64_t seed, float* out_x, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Several utterances of different lengths in one sample loop (the loop costs about the same per step for 1 row as for 64:
+ * DESIGN.md section 4.7).  Utterance u's samples are those of mb_wavernn_condition + mb_wavernn_generate_rows[_mol] on it alone.
+ *
+ * mb_wavernn_condition_multi: mels [80, frames[u]] fp32 back to back in `mel_concat`; the conditioning tables of all
+ * utterances are kept concatenated in the workspace (one launch per layer whatever n_utts is).
+ *
+ * mb_wavernn_generate_multi[_mol]: `rows` rows, row r = (row_utt[r], row_start[r] offset in upsampled time, row_steps[r],
+ * row_fold[r] = index of the row among the folds of its utterance), all host arrays.  The folds 0 .. n-1 of an utterance are
+ * adjacent rows of one length and the rows are ordered longest first, so that the rows alive at any step are a prefix:
+ *   max_steps   : steps of row 0; out_idx / out_x is [rows, max_steps], row r written at [r, 0 .. row_steps[r])
+ *   step0/nsteps: as in mb_wavernn_generate; step0 == 0 resets the state and uploads the row table
+ *   n_live      : number of rows with row_steps > step0; only the 64-row blocks that hold one of them run
+ *   noise       : RAW: Exp(1) fp32 [nsteps][n_live][512].  MOL: uniforms fp32 [nsteps][11 * n_live], per step and per live
+ *                 utterance of n folds its n x 10 mixture uniforms and then its n logistic uniforms (each utterance's draws
+ *                 of a step are contiguous, as one generator per utterance produces them).  NULL: the built-in generator
+ *                 keyed by (utt_seeds[row_utt[r]], step, row_fold[r], slot) - what the single call draws for that utterance
+ *                 under that seed.
+ *   utt_seeds   : one per conditioned utterance; may be NULL when noise is given */
+size_t mb_wavernn_workspace_bytes_multi(const mb_wavernn* h, int32_t n_utts, const int32_t* frames, int32_t rows,
+                                        int32_t max_steps);
+int mb_wavernn_condition_multi(mb_wavernn* h, const float* mel_concat, const int32_t* frames, int32_t n_utts, void* workspace,
+                               size_t workspace_bytes, void* stream);
+int mb_wavernn_generate_multi(mb_wavernn* h, const int32_t* row_utt, const int32_t* row_start, const int32_t* row_steps,
+                              const int32_t* row_fold, int32_t rows, const uint64_t* utt_seeds, int32_t max_steps,
+                              int32_t step0, int32_t nsteps, int32_t n_live, const float* noise, int16_t* out_idx,
+                              void* workspace, size_t workspace_bytes, void* stream);
+int mb_wavernn_generate_multi_mol(mb_wavernn* h, const int32_t* row_utt, const int32_t* row_start, const int32_t* row_steps,
+                                  const int32_t* row_fold, int32_t rows, const uint64_t* utt_seeds, int32_t max_steps,
+                                  int32_t step0, int32_t nsteps, int32_t n_live, const float* uniforms, float* out_x,
+                                  void* workspace, size_t workspace_bytes, void* stream);
+
 /* The float64 tail of WaveRNN.generate on the device (fatchord_version.py:236-253, :340-402; wavernn/audio.py:92-107):
  * class indices int16 [folds, steps] (device) -> sample = 2*idx/(n_classes-1) - 1 -> equal-power cross-fade + unfold
  * (batched) -> mu-law decode -> de-emphasis y[n] = x[n] + preemphasis*y[n-1] (0 = off) -> out[:wave_len] ->
@@ -327,6 +358,12 @@ int mb_mtstream_consumed(mb_mtstream* ms, void* main_stream);
 int mb_mtstream_finish(mb_mtstream* ms, uint32_t* state624_out, int32_t* left_out, int32_t* next_out);
 /* host-only: n raw draws continuing from (state, left, next), which are advanced in place */
 int mb_mt19937_fill(uint32_t* state624, int32_t* left, int32_t* next, uint32_t* out, uint64_t n);
+/* host-only: one chunk of noise from several independent streams (one generator position per utterance of a multi-utterance
+ * sample loop).  Source s continues from (states[s][624], left[s], next[s]) - advanced in place - and writes, for each of the
+ * first steps[s] steps j of the chunk, words_per_step[s] finished draws at out[j * stride + col[s]]; a source whose utterance
+ * ends inside the chunk has fewer steps than the others.  n_threads host threads share the sources. */
+int mb_mt19937_fill_sources(int32_t n_src, uint32_t* states, int32_t* left, int32_t* next, const uint64_t* words_per_step,
+                            const uint64_t* col, const int32_t* steps, uint32_t* out, uint64_t stride, int32_t n_threads);
 /* device conversion alone: raw draws [n_elems][2] (device) -> Exp(1) fp32 [n_elems] */
 int mb_mt_to_exp(const void* dev_raw, float* dev_noise, uint64_t n_elems, void* stream);
 /* The uniforms of the MOL sampler: ATen's CPU float `uniform_(1e-5, 1 - 1e-5)` takes ONE 32-bit draw per element,

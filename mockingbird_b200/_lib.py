@@ -208,6 +208,16 @@ SIGNATURES = {
     "mb_wavernn_generate_rows_mol": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32,
                                                C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_uint64, C.c_void_p,
                                                C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mb_wavernn_workspace_bytes_multi": (C.c_size_t, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_int32]),
+    "mb_wavernn_condition_multi": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_size_t,
+                                             C.c_void_p]),
+    "mb_wavernn_generate_multi": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                            C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_uint64), C.c_int32, C.c_int32,
+                                            C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mb_wavernn_generate_multi_mol": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                                C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_uint64), C.c_int32, C.c_int32,
+                                                C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                C.c_void_p]),
     "mb_wavernn_postprocess_f32": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double,
                                              C.c_int64, C.c_int32, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p, C.c_size_t,
                                              C.c_void_p]),
@@ -233,6 +243,8 @@ SIGNATURES = {
     "mb_mtstream_consumed": (C.c_int, [C.c_void_p, C.c_void_p]),
     "mb_mtstream_finish": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "mb_mt19937_fill": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p, C.c_uint64]),
+    "mb_mt19937_fill_sources": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_uint64, C.c_int32]),
     "mb_mt_to_exp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     "mb_mtstream_next_uniform": (C.c_int, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "mb_mt_to_uniform": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),

@@ -297,6 +297,43 @@ int mb_mt19937_fill(uint32_t* state624, int32_t* left, int32_t* next, uint32_t* 
   return MB_OK;
 }
 
+// Several independent streams into one chunk of noise (the multi-utterance sample loop: one generator position per
+// utterance).  Source s continues from (states[s], left[s], next[s]) and writes, for each of the first steps[s] steps j of the
+// chunk, its words_per_step[s] draws at out[j * stride + col[s]]; the positions are advanced in place.  The sources are
+// independent, so n_threads host threads take them one at a time from a shared counter.
+int mb_mt19937_fill_sources(int32_t n_src, uint32_t* states, int32_t* left, int32_t* next, const uint64_t* words_per_step,
+                            const uint64_t* col, const int32_t* steps, uint32_t* out, uint64_t stride, int32_t n_threads) {
+  if (n_src <= 0 || !states || !left || !next || !words_per_step || !col || !steps || !out || n_threads <= 0)
+    return mb::fail(MB_ERR_INVALID, "mb_mt19937_fill_sources: bad argument");
+  for (int s = 0; s < n_src; ++s) {
+    if (steps[s] < 0 || col[s] + words_per_step[s] > stride)
+      return mb::fail(MB_ERR_INVALID, "mb_mt19937_fill_sources: source %d (columns [%llu, %llu)) outside the step of %llu words", s,
+                      (unsigned long long)col[s], (unsigned long long)(col[s] + words_per_step[s]), (unsigned long long)stride);
+    if (left[s] < 1 || left[s] > kN || next[s] < 0 || next[s] > kN || (left[s] > 1 && next[s] + (left[s] - 1) != kN))
+      return mb::fail(MB_ERR_INVALID, "mb_mt19937_fill_sources: inconsistent generator position of source %d (left=%d next=%d)", s,
+                      left[s], next[s]);
+  }
+  std::atomic<int> cursor{0};
+  auto run = [&] {
+    for (int s = cursor.fetch_add(1); s < n_src; s = cursor.fetch_add(1)) {
+      MtPos g;
+      memcpy(g.s, states + (size_t)s * kN, sizeof(uint32_t) * kN);
+      g.avail = left[s] - 1;
+      g.idx = next[s];
+      for (int j = 0; j < steps[s]; ++j) mt_fill(g, out + (size_t)j * stride + col[s], (size_t)words_per_step[s]);
+      memcpy(states + (size_t)s * kN, g.s, sizeof(uint32_t) * kN);
+      left[s] = g.avail + 1;
+      next[s] = g.idx;
+    }
+  };
+  const int nt = n_threads < n_src ? n_threads : n_src;
+  std::vector<std::thread> pool;
+  for (int t = 1; t < nt; ++t) pool.emplace_back(run);
+  run();
+  for (auto& t : pool) t.join();
+  return MB_OK;
+}
+
 // device conversion alone (test hook / callers that bring their own raw draws)
 int mb_mt_to_exp(const void* dev_raw, float* dev_noise, uint64_t n_elems, void* stream) {
   if (!dev_raw || !dev_noise) return mb::fail(MB_ERR_INVALID, "mb_mt_to_exp: null argument");

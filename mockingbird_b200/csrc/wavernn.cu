@@ -131,6 +131,86 @@ __global__ void k_aux_table(const float* __restrict__ W, int ld, int K0, const f
   out[i] = acc + bias[g];
 }
 
+// ------------------------------------------------------------------------------------------------
+// conditioning of a set of utterances (mb_wavernn_condition_multi).  The frames of all utterances are concatenated:
+// utterance u owns frames [segF[u], segF[u] + segT[u]) of the [C][Ttot] activations, of aux [Ttot][128] and (x200) of melup,
+// padded frames [segF[u] + 4u, + segT[u] + 4) of the ladder buffers and rows [segF[u] + u, + segT[u] + 1) of the aux tables
+// (the last one is its "past the end" row).  k_bn / k_conv1x1 are frame-wise and run unchanged over Ttot frames; the kernels
+// below are the ones that must not look across an utterance boundary.  fseg / pseg: utterance of a frame / padded frame.
+// Per output the fmaf chain is that of the single-utterance kernel, so utterance u's tables equal mb_wavernn_condition's.
+// ------------------------------------------------------------------------------------------------
+__global__ void k_conv_in_multi(const float* __restrict__ w, const float* __restrict__ mel, int Ttot,
+                                const int* __restrict__ fseg, const int* __restrict__ segF, const int* __restrict__ segT,
+                                float* __restrict__ y) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= CDIM * Ttot) return;
+  const int o = i / Ttot, tg = i - o * Ttot;
+  const int u = fseg[tg], F = segF[u], T = segT[u], t = tg - F;
+  const float* m = mel + (size_t)FEAT * F;  // mels [80, T_u] back to back
+  float acc = 0.0f;
+  for (int ci = 0; ci < FEAT; ++ci)
+    for (int k = 0; k < 5; ++k) {
+      const int s = t + k - 2;
+      const float v = (s >= 0 && s < T) ? m[ci * T + s] : 0.0f;
+      acc = fmaf(w[(o * FEAT + ci) * 5 + k], v, acc);
+    }
+  y[i] = acc;
+}
+
+__global__ void k_pad_mel_multi(const float* __restrict__ mel, int Tptot, const int* __restrict__ pseg,
+                                const int* __restrict__ segF, const int* __restrict__ segT, float* __restrict__ P) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= FEAT * Tptot) return;
+  const int c = i / Tptot, pg = i - c * Tptot;
+  const int u = pseg[pg], F = segF[u], T = segT[u], t = pg - (F + 4 * u);
+  P[i] = (t >= 2 && t < T + 2) ? mel[(size_t)FEAT * F + c * T + t - 2] : 0.0f;
+}
+
+// one ladder stage over all utterances; `per` = input positions per padded frame (1, 5, 25)
+__global__ void k_ladder_multi(const float* __restrict__ w, const float* __restrict__ x, int len, int s, int per,
+                               const int* __restrict__ pseg, const int* __restrict__ segF, const int* __restrict__ segT,
+                               float* __restrict__ y) {
+  const size_t nl = (size_t)len * s;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= FEAT * nl) return;
+  const int c = (int)(i / nl), pg = (int)(i - c * nl);
+  const int u = pseg[pg / (per * s)];
+  const int seg0 = (segF[u] + 4 * u) * per * s, seglen = (segT[u] + 4) * per * s;
+  const int p = pg - seg0;
+  float acc = 0.0f;
+  for (int j = 0; j <= 2 * s; ++j) {
+    const int src = p + j - s;
+    const float v = (src >= 0 && src < seglen) ? x[(size_t)c * len + (seg0 + src) / s] : 0.0f;
+    acc = fmaf(w[j], v, acc);
+  }
+  y[i] = acc;
+}
+
+__global__ void k_crop_melup_multi(const float* __restrict__ y3, int len, int Ttot, const int* __restrict__ fseg,
+                                   float* __restrict__ melup) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)HOP * Ttot * FEAT) return;
+  const int tg = (int)(i / FEAT), c = (int)(i - (size_t)tg * FEAT);
+  const int u = fseg[tg / HOP];
+  melup[i] = y3[(size_t)c * len + tg + HOP * (4 * u) + 2 * HOP];
+}
+
+// tsrc[f]: frame of aux behind table row f, or -1 for an utterance's "past the end" row
+__global__ void k_aux_table_multi(const float* __restrict__ W, int ld, int K0, const float* __restrict__ bias,
+                                  const float* __restrict__ aux, int a0, const int* __restrict__ tsrc, int R, int G,
+                                  float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= R * G) return;
+  const int f = i / G, g = i - f * G;
+  const int src = tsrc[f];
+  float acc = 0.0f;
+  for (int j = 0; j < AUXD; ++j) {
+    const float a = (src >= 0) ? aux[(size_t)src * CDIM + a0 + j] : 0.0f;
+    acc = fmaf(W[(size_t)g * ld + K0 + j], a, acc);
+  }
+  out[i] = acc + bias[g];
+}
+
 // per-chunk conditioning of the I layer in the exchange layout:
 //   condI[i][u][r] = dot_seq(I_w[u][1:113], [melup[t]; aux[t/200][0:32]]) + I_b[u],  t = start[r] + step0 + i
 __global__ void __launch_bounds__(256) k_condI(const float* __restrict__ I_w, const float* __restrict__ I_b,
@@ -154,6 +234,33 @@ __global__ void __launch_bounds__(256) k_condI(const float* __restrict__ I_w, co
     const float* wr = I_w + (size_t)u * 113 + 1;
     for (int j = 0; j < FEAT + AUXD; ++j) acc = fmaf(wr[j], c[j], acc);
     out[((size_t)i * RNN + u) * Bpad + r] = (r < B) ? acc + I_b[u] : 0.0f;
+  }
+}
+
+// the same for the multi-utterance loop: row r is described by rowc[r] = {start, T_u, table base, frame base}; only the
+// W = 64 * (live row blocks) leading rows are computed
+__global__ void __launch_bounds__(256) k_condI_multi(const float* __restrict__ I_w, const float* __restrict__ I_b,
+                                                     const float* __restrict__ melup, const float* __restrict__ aux,
+                                                     const int4* __restrict__ rowc, int W, int Bpad, int step0, int nsteps,
+                                                     float* __restrict__ out) {
+  __shared__ float c[FEAT + AUXD];
+  const int r = blockIdx.x % W;
+  const int i = blockIdx.x / W;
+  if (i >= nsteps) return;
+  const int4 d = rowc[r];  // rows past the table: T_u == 0, never live
+  const int t = d.x + step0 + i;
+  const bool live = t < HOP * d.y;
+  for (int j = threadIdx.x; j < FEAT + AUXD; j += blockDim.x) {
+    float v = 0.0f;
+    if (live) v = (j < FEAT) ? melup[((size_t)HOP * d.w + t) * FEAT + j] : aux[(size_t)(d.w + t / HOP) * CDIM + (j - FEAT)];
+    c[j] = v;
+  }
+  __syncthreads();
+  for (int u = threadIdx.x; u < RNN; u += blockDim.x) {
+    float acc = 0.0f;
+    const float* wr = I_w + (size_t)u * 113 + 1;
+    for (int j = 0; j < FEAT + AUXD; ++j) acc = fmaf(wr[j], c[j], acc);
+    out[((size_t)i * RNN + u) * Bpad + r] = acc + I_b[u];
   }
 }
 
@@ -186,6 +293,11 @@ struct LoopParams {
   float* out_x;             // MOL: float samples [B][steps_total]
   unsigned int* barrier;    // grid barrier counter / per-CTA epoch flags [NCTA] (zeroed by the host before launch)
   int flagbar;              // 1: flag barrier, 0: single atomic counter
+  // multi-utterance loop (k_sample_loop<MOL, true>): per-row descriptors [Bpad] replace starts / T / row0 / seed; B is the
+  // number of live rows (a prefix: rows are ordered longest first), noise_B == B, steps_total the longest row's steps
+  const int4* rowc;         // {start, T_u, first table row of its utterance, first frame of its utterance}
+  const int4* rown;         // {steps, fold index in its utterance, first row of its utterance, folds of its utterance}
+  const uint64_t* rowseed;  // seed of its utterance (built-in generator: keyed by (seed, step, fold index, slot))
 };
 
 // per-CTA weight pack (floats):
@@ -316,7 +428,9 @@ __device__ __forceinline__ void tile_gemv(const float* __restrict__ wsm /*[512][
 __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 
 // MOL: fc3 has 30 outputs (units of CTAs 0..7; the other CTAs skip phase E) and phase F is the mixture-of-logistics draw
-template <bool MOL>
+// MULTI: rows of several utterances with their own lengths (LoopParams::rowc / rown / rowseed); only the row blocks that
+// hold a live row run, and a row stores nothing past its own last step
+template <bool MOL, bool MULTI>
 __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p) {
   extern __shared__ __align__(16) float sm[];
   float* wsm = sm;
@@ -330,7 +444,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
   const int kh = lane >> 4;   // k half within the warp's slice
   const int cta = blockIdx.x;
   const int Bpad = p.Bpad;
-  const int nrb = Bpad / RB;
+  const int nrb = MULTI ? (p.B + RB - 1) / RB : Bpad / RB;
 
   {  // one-time: weights -> shared memory
     const float4* src = reinterpret_cast<const float4*>(p.wpack + (size_t)cta * WPACK_FLOATS);
@@ -364,11 +478,20 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
     float mol_pre = 0.0f;
     if (MOL && p.noise && cta < p.B && warp == 0 && lane < MB_MOL_UNIFORMS) {
       const size_t base = (size_t)i * MB_MOL_UNIFORMS * p.noise_B;
-      mol_pre = p.noise[base + (lane < MB_MOL_NMIX ? (size_t)(p.row0 + cta) * MB_MOL_NMIX + lane
-                                                   : (size_t)MB_MOL_NMIX * p.noise_B + (p.row0 + cta))];
+      if constexpr (MULTI) {  // per utterance block of nf rows starting at row r0: [nf x 10 mixture | nf logistic]
+        const int4 d = p.rown[cta];
+        mol_pre = p.noise[base + (size_t)MB_MOL_UNIFORMS * d.z +
+                          (lane < MB_MOL_NMIX ? d.y * MB_MOL_NMIX + lane : MB_MOL_NMIX * d.w + d.y)];
+      } else {
+        mol_pre = p.noise[base + (lane < MB_MOL_NMIX ? (size_t)(p.row0 + cta) * MB_MOL_NMIX + lane
+                                                     : (size_t)MB_MOL_NMIX * p.noise_B + (p.row0 + cta))];
+      }
     }
     // built-in generator: the same 512 values, one per thread, computed here instead of inside the sampling phase
-    if (!MOL && !p.noise && cta < p.B && tid < NCLS) qsm[tid] = mb_exp1_noise(p.seed, (uint32_t)gstep, (uint32_t)(p.row0 + cta), (uint32_t)tid);
+    if (!MOL && !p.noise && cta < p.B && tid < NCLS) {
+      if constexpr (MULTI) qsm[tid] = mb_exp1_noise(p.rowseed[cta], (uint32_t)gstep, (uint32_t)p.rown[cta].y, (uint32_t)tid);
+      else qsm[tid] = mb_exp1_noise(p.seed, (uint32_t)gstep, (uint32_t)(p.row0 + cta), (uint32_t)tid);
+    }
 
     // ================= phase A: rnn1 =================
     for (int rb = 0; rb < nrb; ++rb) {
@@ -469,7 +592,11 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
         const int row = rb * RB + r;
         const int unit = cta * UPC + j;
         int frame = p.T;  // "past the end" row of the tables
-        if (row < p.B) {
+        if constexpr (MULTI) {
+          const int4 d = p.rowc[row];
+          const int t = d.x + gstep;
+          frame = d.z + (t < HOP * d.y ? t / HOP : d.y);
+        } else if (row < p.B) {
           const int t = p.starts[row] + gstep;
           if (t < HOP * p.T) frame = t / HOP;
         }
@@ -545,7 +672,11 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
           float v = s[0];
           if (layer < 2) {
             int frame = p.T;
-            if (row < p.B) {
+            if constexpr (MULTI) {
+              const int4 d = p.rowc[row];
+              const int t = d.x + gstep;
+              frame = d.z + (t < HOP * d.y ? t / HOP : d.y);
+            } else if (row < p.B) {
               const int t = p.starts[row] + gstep;
               if (t < HOP * p.T) frame = t / HOP;
             }
@@ -568,12 +699,19 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
       if (warp == 0) {
         const size_t base = (size_t)i * MB_MOL_UNIFORMS * p.noise_B;
         for (int row = cta; row < p.B; row += gridDim.x) {
-          const uint32_t grow = (uint32_t)(p.row0 + row);
+          int4 dn = make_int4(0, 0, 0, 0);
+          if constexpr (MULTI) dn = p.rown[row];
+          const uint32_t grow = MULTI ? (uint32_t)dn.y : (uint32_t)(p.row0 + row);  // noise row key
+          const uint64_t seed = MULTI ? p.rowseed[row] : p.seed;
+          // element offsets of the row's mixture uniforms and of its logistic uniform within the step
+          const size_t mix0 = MULTI ? (size_t)MB_MOL_UNIFORMS * dn.z + (size_t)dn.y * MB_MOL_NMIX : (size_t)grow * MB_MOL_NMIX;
+          const size_t log0 = MULTI ? (size_t)MB_MOL_UNIFORMS * dn.z + (size_t)MB_MOL_NMIX * dn.w + dn.y
+                                    : (size_t)MB_MOL_NMIX * p.noise_B + grow;
           float sc = -3.0e38f;
           if (lane < MB_MOL_NMIX) {
             const float t = (row == cta && p.noise) ? mol_pre
-                            : (p.noise ? p.noise[base + (size_t)grow * MB_MOL_NMIX + lane]
-                                       : mb_mol_uniform(p.seed, (uint32_t)gstep, grow, (uint32_t)lane));
+                            : (p.noise ? p.noise[base + mix0 + lane]
+                                       : mb_mol_uniform(seed, (uint32_t)gstep, grow, (uint32_t)lane));
             sc = mb_mol_score(p.logits[(size_t)lane * Bpad + row], t);
           }
           int best = lane;
@@ -589,11 +727,11 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
           const float u_pre = __shfl_sync(0xffffffffu, mol_pre, MB_MOL_NMIX);
           if (lane == 0) {
             const float u = (row == cta && p.noise) ? u_pre
-                            : (p.noise ? p.noise[base + (size_t)MB_MOL_NMIX * p.noise_B + grow]
-                                       : mb_mol_uniform(p.seed, (uint32_t)gstep, grow, MB_MOL_NMIX));
+                            : (p.noise ? p.noise[base + log0]
+                                       : mb_mol_uniform(seed, (uint32_t)gstep, grow, MB_MOL_NMIX));
             const float x = mb_mol_sample(p.logits[(size_t)(MB_MOL_NMIX + best) * Bpad + row],
                                           p.logits[(size_t)(2 * MB_MOL_NMIX + best) * Bpad + row], u);
-            p.out_x[(size_t)row * p.steps_total + gstep] = x;
+            if (!MULTI || gstep < dn.x) p.out_x[(size_t)row * p.steps_total + gstep] = x;
             p.xprev[row] = x;
           }
         }
@@ -639,6 +777,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
           const int cls = lane + 32 * jj;
           const float q = (row == cta) ? qsm[cls]
                           : (p.noise ? p.noise[((size_t)i * p.noise_B + (size_t)(p.row0 + row)) * NCLS + cls]
+                             : MULTI ? mb_exp1_noise(p.rowseed[row], (uint32_t)gstep, (uint32_t)p.rown[row].y, (uint32_t)cls)
                                      : mb_exp1_noise(p.seed, (uint32_t)gstep, (uint32_t)(p.row0 + row), (uint32_t)cls));
           const float v = (e[jj] / S2) / q;
           if (v > bestv) {  // ascending class order within the lane: first maximum wins
@@ -656,7 +795,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
           }
         }
         if (lane == 0) {
-          p.out_idx[(size_t)row * p.steps_total + gstep] = (int16_t)best;
+          if (!MULTI || gstep < p.rown[row].x) p.out_idx[(size_t)row * p.steps_total + gstep] = (int16_t)best;
           p.xprev[row] = (2.0f * (float)best) / 511.0f - 1.0f;
         }
       }
@@ -685,6 +824,8 @@ struct mb_wavernn {
   // conditioning of the current utterance (workspace-resident)
   int cond_T = 0;
   void* cond_ws = nullptr;
+  // ... or of the current set of utterances (mb_wavernn_condition_multi): frames per utterance; empty otherwise
+  std::vector<int32_t> cond_frames;
 };
 
 namespace {
@@ -692,11 +833,13 @@ namespace {
 const float* W(const mb_wavernn* h, const std::string& name) { return h->w.ptr(name); }
 
 struct WsLayout {
-  size_t aux, melup, aux2P, aux3P, aux4P, tmpA, tmpB, tmpR, padP, lad5, lad25, lad200, starts, condI, h1, h2, f1, f2, logits, xprev,
-      barrier, total;
+  size_t aux, melup, aux2P, aux3P, aux4P, tmpA, tmpB, tmpR, padP, lad5, lad25, lad200, segs, starts, condI, h1, h2, f1, f2, logits,
+      xprev, barrier, rowdesc, total;
 };
 
-WsLayout ws_layout(int T, int Bpad, int chunk_steps) {
+// T frames of U utterances in all (each utterance has its own "past the end" table row and its own 4 frames of ladder padding);
+// multi: the segment tables of the conditioning kernels and the row descriptors of the multi-utterance loop are laid out too
+WsLayout ws_layout(int T, int Bpad, int chunk_steps, int U = 1, bool multi = false) {
   WsLayout L{};
   size_t o = 0;
   auto take = [&](size_t floats) {
@@ -706,16 +849,17 @@ WsLayout ws_layout(int T, int Bpad, int chunk_steps) {
   };
   L.aux = take((size_t)T * CDIM);
   L.melup = take((size_t)HOP * T * FEAT);
-  L.aux2P = take((size_t)(T + 1) * 3 * RNN);
-  L.aux3P = take((size_t)(T + 1) * RNN);
-  L.aux4P = take((size_t)(T + 1) * RNN);
+  L.aux2P = take((size_t)(T + U) * 3 * RNN);
+  L.aux3P = take((size_t)(T + U) * RNN);
+  L.aux4P = take((size_t)(T + U) * RNN);
   L.tmpA = take((size_t)CDIM * T);
   L.tmpB = take((size_t)CDIM * T);
   L.tmpR = take((size_t)CDIM * T);
-  L.padP = take((size_t)FEAT * (T + 4));
-  L.lad5 = take((size_t)FEAT * (T + 4) * 5);
-  L.lad25 = take((size_t)FEAT * (T + 4) * 25);
-  L.lad200 = take((size_t)FEAT * (T + 4) * HOP);
+  L.padP = take((size_t)FEAT * (T + 4 * U));
+  L.lad5 = take((size_t)FEAT * (T + 4 * U) * 5);
+  L.lad25 = take((size_t)FEAT * (T + 4 * U) * 25);
+  L.lad200 = take((size_t)FEAT * (T + 4 * U) * HOP);
+  if (multi) L.segs = take((size_t)3 * T + 7 * U);  // int32: fseg[T] pseg[T+4U] tsrc[T+U] segF[U] segT[U]
   L.starts = take((size_t)Bpad);
   L.condI = take((size_t)chunk_steps * RNN * Bpad);
   L.h1 = take((size_t)2 * RNN * Bpad);
@@ -725,6 +869,7 @@ WsLayout ws_layout(int T, int Bpad, int chunk_steps) {
   L.logits = take((size_t)RNN * Bpad);
   L.xprev = take((size_t)Bpad);
   L.barrier = take(256);  // 1 KB: counter, or one epoch word per CTA
+  if (multi) L.rowdesc = take((size_t)10 * Bpad);  // int4 rowc[Bpad] | int4 rown[Bpad] | uint64 rowseed[Bpad]
   L.total = o;
   return L;
 }
@@ -911,6 +1056,7 @@ int mb_wavernn_condition(mb_wavernn* h, const float* mel, int32_t T, void* works
   MB_LAUNCH_CHECK("k_aux_table");
   h->cond_T = T;
   h->cond_ws = workspace;
+  h->cond_frames.clear();
   return MB_OK;
 }
 
@@ -925,11 +1071,12 @@ int mb_wavernn_generate(mb_wavernn* h, const int32_t* fold_starts_host, int32_t 
 
 namespace {
 
+int launch_sample_loop(mb_wavernn* h, LoopParams& p, const WsLayout& L, float* ws, bool multi, cudaStream_t st);
+
 // one chunk of the sample loop; exactly one of out_idx (RAW handle) / out_x (MOL handle) is given
 int generate_rows_impl(mb_wavernn* h, const int32_t* fold_starts_host, int32_t B, int32_t steps, int32_t step0,
                        int32_t nsteps, const float* noise, int32_t noise_folds, int32_t row0, uint64_t seed,
                        int16_t* out_idx, float* out_x, void* workspace, size_t workspace_bytes, void* stream) {
-  const bool mol = h->mode == MB_WAVERNN_MOL;
   if (row0 < 0 || (noise && row0 + B > noise_folds))
     return fail(MB_ERR_INVALID, "mb_wavernn_generate_rows: rows [%d, %d) outside the %d noise rows", row0, row0 + B, noise_folds);
   if (!h->finalized) return fail(MB_ERR_STATE, "mb_wavernn_generate: weights not finalized");
@@ -955,15 +1102,8 @@ int generate_rows_impl(mb_wavernn* h, const int32_t* fold_starts_host, int32_t B
   k_condI<<<nsteps * Bpad, 256, 0, st>>>(W(h, "I.weight"), W(h, "I.bias"), ws + L.melup, ws + L.aux, T, starts, B, Bpad,
                                          step0, nsteps, ws + L.condI);
   MB_LAUNCH_CHECK("k_condI");
-  MB_CUDA_CHECK(cudaMemsetAsync(ws + L.barrier, 0, 1024, st));
   LoopParams p;
   memset(&p, 0, sizeof(p));
-  p.wpack = h->arena + h->pack_off;
-  p.I0 = h->arena + h->pack_off + (size_t)NCTA * WPACK_FLOATS;
-  p.aux2P = ws + L.aux2P;
-  p.aux3P = ws + L.aux3P;
-  p.aux4P = ws + L.aux4P;
-  p.condI = ws + L.condI;
   p.starts = starts;
   p.T = T;
   p.B = B;
@@ -971,18 +1111,31 @@ int generate_rows_impl(mb_wavernn* h, const int32_t* fold_starts_host, int32_t B
   p.step0 = step0;
   p.nsteps = nsteps;
   p.steps_total = steps;
-  p.h1 = ws + L.h1;
-  p.h2 = ws + L.h2;
-  p.f1 = ws + L.f1;
-  p.f2 = ws + L.f2;
-  p.logits = ws + L.logits;
-  p.xprev = ws + L.xprev;
   p.noise = noise;
   p.noise_B = noise_folds;
   p.row0 = row0;
   p.seed = seed;
   p.out_idx = out_idx;
   p.out_x = out_x;
+  return launch_sample_loop(h, p, L, ws, false, st);
+}
+
+// fills the workspace pointers of `p` and launches the loop instance of the handle's sampler
+int launch_sample_loop(mb_wavernn* h, LoopParams& p, const WsLayout& L, float* ws, bool multi, cudaStream_t st) {
+  const bool mol = h->mode == MB_WAVERNN_MOL;
+  MB_CUDA_CHECK(cudaMemsetAsync(ws + L.barrier, 0, 1024, st));
+  p.wpack = h->arena + h->pack_off;
+  p.I0 = h->arena + h->pack_off + (size_t)NCTA * WPACK_FLOATS;
+  p.aux2P = ws + L.aux2P;
+  p.aux3P = ws + L.aux3P;
+  p.aux4P = ws + L.aux4P;
+  p.condI = ws + L.condI;
+  p.h1 = ws + L.h1;
+  p.h2 = ws + L.h2;
+  p.f1 = ws + L.f1;
+  p.f2 = ws + L.f2;
+  p.logits = ws + L.logits;
+  p.xprev = ws + L.xprev;
   p.barrier = reinterpret_cast<unsigned int*>(ws + L.barrier);
   static const int flagbar = [] {
     // A/B switch.  Measured: the flag barrier is much SLOWER (604 vs 428 ms per cfg-3 call: 128 x 128 polling threads swamp the
@@ -992,11 +1145,14 @@ int generate_rows_impl(mb_wavernn* h, const int32_t* fold_starts_host, int32_t B
   }();
   p.flagbar = flagbar;
   const size_t smem = sizeof(float) * SMEM_FLOATS;
-  static bool attr[2] = {false, false};
-  const void* kern = mol ? (const void*)k_sample_loop<true> : (const void*)k_sample_loop<false>;
-  if (!attr[mol]) {
+  static bool attr[4] = {false, false, false, false};
+  const void* kerns[4] = {(const void*)k_sample_loop<false, false>, (const void*)k_sample_loop<true, false>,
+                          (const void*)k_sample_loop<false, true>, (const void*)k_sample_loop<true, true>};
+  const int which = (multi ? 2 : 0) + (mol ? 1 : 0);
+  const void* kern = kerns[which];
+  if (!attr[which]) {
     MB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr[mol] = true;
+    attr[which] = true;
   }
   void* args[] = {(void*)&p};
   MB_CUDA_CHECK(cudaLaunchCooperativeKernel(kern, dim3(NCTA), dim3(kThreads), args, smem, st));
@@ -1040,6 +1196,240 @@ int mb_wavernn_last_logits(mb_wavernn* h, float* logits, int32_t B, void* worksp
     MB_CUDA_CHECK(cudaMemcpy2DAsync(logits + (size_t)r * ncls, sizeof(float), ws + L.logits + r, sizeof(float) * Bpad,
                                     sizeof(float), ncls, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return MB_OK;
+}
+
+}  // extern "C"
+
+// =================================================================================================
+// several utterances in one sample loop
+// =================================================================================================
+namespace {
+
+// total frames of a set of utterances, or -1 when the list is not usable
+int64_t total_frames(const int32_t* frames, int32_t n_utts) {
+  if (!frames || n_utts <= 0) return -1;
+  int64_t tot = 0;
+  for (int u = 0; u < n_utts; ++u) {
+    if (frames[u] <= 0) return -1;
+    tot += frames[u];
+  }
+  // the kernels index the x200 upsampled, 80-channel ladder with 32-bit ints
+  return ((tot + 4 * (int64_t)n_utts) * HOP * FEAT < (int64_t)1 << 31) ? tot : -1;
+}
+
+int generate_multi_impl(const char* fn, mb_wavernn* h, const int32_t* row_utt, const int32_t* row_start,
+                        const int32_t* row_steps, const int32_t* row_fold, int32_t rows, const uint64_t* utt_seeds,
+                        int32_t max_steps, int32_t step0, int32_t nsteps, int32_t n_live, const float* noise, int16_t* out_idx,
+                        float* out_x, void* workspace, size_t workspace_bytes, void* stream) {
+  if (rows <= 0 || max_steps <= 0 || nsteps <= 0 || nsteps > kChunkMax || step0 < 0 || step0 + nsteps > max_steps)
+    return fail(MB_ERR_INVALID, "%s: bad row count or step range (at most %d steps per call)", fn, kChunkMax);
+  // the row table: whole utterances side by side (folds 0 .. n-1 of one utterance, all of one length), longest rows first
+  int alive = 0;
+  for (int r = 0; r < rows; ++r) {
+    if (row_utt[r] < 0 || row_start[r] < 0 || row_steps[r] <= 0 || row_steps[r] > max_steps || row_fold[r] < 0)
+      return fail(MB_ERR_INVALID, "%s: row %d (utterance %d, start %d, steps %d, fold %d) outside the table", fn, r, row_utt[r],
+                  row_start[r], row_steps[r], row_fold[r]);
+    if (r > 0 && row_steps[r] > row_steps[r - 1]) return fail(MB_ERR_INVALID, "%s: rows must be ordered longest first (row %d)", fn, r);
+    const bool cont = r > 0 && row_utt[r] == row_utt[r - 1];
+    if (cont ? (row_fold[r] != row_fold[r - 1] + 1 || row_steps[r] != row_steps[r - 1]) : row_fold[r] != 0)
+      return fail(MB_ERR_INVALID, "%s: the folds of an utterance must be adjacent rows 0, 1, .. of one length (row %d)", fn, r);
+    alive += row_steps[r] > step0;
+  }
+  if (n_live != alive)
+    return fail(MB_ERR_INVALID, "%s: %d rows are alive at step %d, the call says %d", fn, alive, step0, n_live);
+  if (n_live < rows && row_utt[n_live] == row_utt[n_live - 1])
+    return fail(MB_ERR_INVALID, "%s: the live rows end inside utterance %d", fn, row_utt[n_live]);
+  if (!h->finalized) return fail(MB_ERR_STATE, "%s: weights not finalized", fn);
+  if (h->cond_frames.empty() || h->cond_ws != workspace)
+    return fail(MB_ERR_STATE, "%s: call mb_wavernn_condition_multi on this workspace first", fn);
+  const int U = (int)h->cond_frames.size();
+  int Ttot = 0;
+  for (int t : h->cond_frames) Ttot += t;
+  for (int r = 0; r < rows; ++r)
+    if (row_utt[r] >= U) return fail(MB_ERR_INVALID, "%s: row %d names utterance %d of %d", fn, r, row_utt[r], U);
+  const int Bpad = bpad_of(rows);
+  const WsLayout L = ws_layout(Ttot, Bpad, kChunkMax, U, true);
+  if (workspace_bytes < L.total * sizeof(float) + 256) return fail(MB_ERR_WORKSPACE, "%s: workspace too small", fn);
+  float* ws = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  cudaStream_t st = (cudaStream_t)stream;
+  int4* rowc = reinterpret_cast<int4*>(ws + L.rowdesc);
+  int4* rown = rowc + Bpad;
+  uint64_t* rowseed = reinterpret_cast<uint64_t*>(rown + Bpad);
+  if (step0 == 0) {
+    // zero initial state and upload the row descriptors (rows past the table: T_u == 0, never live)
+    MB_CUDA_CHECK(cudaMemsetAsync(ws + L.h1, 0, sizeof(float) * (L.xprev + align_up((size_t)Bpad, 64) - L.h1), st));
+    std::vector<int32_t> fbase(U);
+    for (int u = 0, f = 0; u < U; f += h->cond_frames[u], ++u) fbase[u] = f;
+    std::vector<int32_t> tmp((size_t)10 * Bpad, 0);
+    int32_t* c = tmp.data();
+    int32_t* n = c + 4 * Bpad;
+    uint64_t* sd = reinterpret_cast<uint64_t*>(n + 4 * Bpad);
+    for (int r = 0, first = 0; r < rows; ++r) {
+      const int u = row_utt[r];
+      if (row_fold[r] == 0) first = r;
+      c[4 * r + 0] = row_start[r];
+      c[4 * r + 1] = h->cond_frames[u];
+      c[4 * r + 2] = fbase[u] + u;
+      c[4 * r + 3] = fbase[u];
+      n[4 * r + 0] = row_steps[r];
+      n[4 * r + 1] = row_fold[r];
+      n[4 * r + 2] = first;
+      sd[r] = utt_seeds ? utt_seeds[u] : 0;
+    }
+    for (int r = rows - 1, nf = 0; r >= 0; --r) {  // folds of the row's utterance
+      if (r == rows - 1 || row_fold[r + 1] == 0) nf = row_fold[r] + 1;
+      n[4 * r + 3] = nf;
+    }
+    MB_CUDA_CHECK(cudaMemcpyAsync(rowc, tmp.data(), sizeof(int32_t) * tmp.size(), cudaMemcpyHostToDevice, st));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));  // tmp goes out of scope
+  }
+  const int Wl = bpad_of(n_live);  // rows of the live row blocks
+  k_condI_multi<<<nsteps * Wl, 256, 0, st>>>(W(h, "I.weight"), W(h, "I.bias"), ws + L.melup, ws + L.aux, rowc, Wl, Bpad, step0,
+                                             nsteps, ws + L.condI);
+  MB_LAUNCH_CHECK("k_condI_multi");
+  LoopParams p;
+  memset(&p, 0, sizeof(p));
+  p.B = n_live;
+  p.Bpad = Bpad;
+  p.step0 = step0;
+  p.nsteps = nsteps;
+  p.steps_total = max_steps;
+  p.noise = noise;
+  p.noise_B = n_live;
+  p.out_idx = out_idx;
+  p.out_x = out_x;
+  p.rowc = rowc;
+  p.rown = rown;
+  p.rowseed = rowseed;
+  return launch_sample_loop(h, p, L, ws, true, st);
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t mb_wavernn_workspace_bytes_multi(const mb_wavernn* h, int32_t n_utts, const int32_t* frames, int32_t rows,
+                                        int32_t max_steps) {
+  const int64_t Ttot = total_frames(frames, n_utts);
+  if (!h || Ttot < 0 || rows <= 0) return 0;
+  (void)max_steps;
+  return ws_layout((int)Ttot, bpad_of(rows), kChunkMax, n_utts, true).total * sizeof(float) + 256;
+}
+
+int mb_wavernn_condition_multi(mb_wavernn* h, const float* mel_concat, const int32_t* frames, int32_t n_utts, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+  if (!h || !mel_concat || !frames || !workspace) return fail(MB_ERR_INVALID, "mb_wavernn_condition_multi: null argument");
+  const int64_t tot = total_frames(frames, n_utts);
+  if (tot < 0) return fail(MB_ERR_INVALID, "mb_wavernn_condition_multi: bad utterance lengths (each > 0, %d frames in all at most)",
+                           (int)(((int64_t)1 << 31) / (HOP * FEAT)));
+  const int U = n_utts, Ttot = (int)tot, Tptot = Ttot + 4 * U, R = Ttot + U;
+  // the conditioning part of the layout does not depend on the row count
+  const WsLayout L = ws_layout(Ttot, RB, kChunkMax, U, true);
+  if (workspace_bytes < (L.starts) * sizeof(float) + 256)
+    return fail(MB_ERR_WORKSPACE, "mb_wavernn_condition_multi: workspace too small");
+  if (!h->finalized) return fail(MB_ERR_STATE, "mb_wavernn_condition_multi: weights not finalized");
+  float* ws = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  cudaStream_t st = (cudaStream_t)stream;
+  // segment tables
+  std::vector<int32_t> seg((size_t)3 * Ttot + 7 * U);
+  int32_t* fseg_h = seg.data();
+  int32_t* pseg_h = fseg_h + Ttot;
+  int32_t* tsrc_h = pseg_h + Tptot;
+  int32_t* segF_h = tsrc_h + R;
+  int32_t* segT_h = segF_h + U;
+  for (int u = 0, F = 0; u < U; F += frames[u], ++u) {
+    const int T = frames[u];
+    segF_h[u] = F;
+    segT_h[u] = T;
+    for (int t = 0; t < T; ++t) fseg_h[F + t] = u;
+    for (int t = 0; t < T + 4; ++t) pseg_h[F + 4 * u + t] = u;
+    for (int t = 0; t <= T; ++t) tsrc_h[F + u + t] = t < T ? F + t : -1;
+  }
+  int* fseg = reinterpret_cast<int*>(ws + L.segs);
+  const int *pseg = fseg + Ttot, *tsrc = pseg + Tptot, *segF = tsrc + R, *segT = segF + U;
+  MB_CUDA_CHECK(cudaMemcpyAsync(fseg, seg.data(), sizeof(int32_t) * seg.size(), cudaMemcpyHostToDevice, st));
+  MB_CUDA_CHECK(cudaStreamSynchronize(st));  // seg goes out of scope
+  const int n = CDIM * Ttot, nb = (n + 255) / 256;
+  float *x = ws + L.tmpA, *y = ws + L.tmpB, *r = ws + L.tmpR;
+  k_conv_in_multi<<<nb, 256, 0, st>>>(W(h, "upsample.resnet.conv_in.weight"), mel_concat, Ttot, fseg, segF, segT, x);
+  MB_LAUNCH_CHECK("k_conv_in_multi");
+  auto bnrun = [&](const std::string& p, float* buf, int relu, const float* res) -> int {
+    k_bn<<<nb, 256, 0, st>>>(W(h, p + ".weight"), W(h, p + ".bias"), W(h, p + ".running_mean"), W(h, p + ".running_var"),
+                             buf, Ttot, relu, res);
+    MB_LAUNCH_CHECK("k_bn");
+    return MB_OK;
+  };
+  int rc = bnrun("upsample.resnet.batch_norm", x, 1, nullptr);
+  if (rc) return rc;
+  for (int i = 0; i < h->cfg.res_blocks; ++i) {
+    const std::string b = "upsample.resnet.layers." + std::to_string(i);
+    MB_CUDA_CHECK(cudaMemcpyAsync(r, x, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
+    k_conv1x1<<<nb, 256, 0, st>>>(W(h, b + ".conv1.weight"), x, Ttot, y, nullptr, 0);
+    MB_LAUNCH_CHECK("k_conv1x1");
+    if ((rc = bnrun(b + ".batch_norm1", y, 1, nullptr))) return rc;
+    k_conv1x1<<<nb, 256, 0, st>>>(W(h, b + ".conv2.weight"), y, Ttot, x, nullptr, 0);
+    MB_LAUNCH_CHECK("k_conv1x1");
+    if ((rc = bnrun(b + ".batch_norm2", x, 0, r))) return rc;
+  }
+  k_conv1x1<<<nb, 256, 0, st>>>(W(h, "upsample.resnet.conv_out.weight"), x, Ttot, ws + L.aux,
+                                W(h, "upsample.resnet.conv_out.bias"), 1);
+  MB_LAUNCH_CHECK("k_conv1x1");
+  float* P = ws + L.padP;
+  float* l5 = ws + L.lad5;
+  float* l25 = ws + L.lad25;
+  float* l1 = ws + L.lad200;
+  k_pad_mel_multi<<<(FEAT * Tptot + 255) / 256, 256, 0, st>>>(mel_concat, Tptot, pseg, segF, segT, P);
+  MB_LAUNCH_CHECK("k_pad_mel_multi");
+  const int s0 = h->cfg.upsample_factors[0], s1 = h->cfg.upsample_factors[1], s2 = h->cfg.upsample_factors[2];
+  auto blocks = [](size_t n_out) { return (unsigned)((n_out + 255) / 256); };
+  k_ladder_multi<<<blocks((size_t)FEAT * Tptot * s0), 256, 0, st>>>(W(h, "upsample.up_layers.1.weight"), P, Tptot, s0, 1, pseg, segF,
+                                                                   segT, l5);
+  MB_LAUNCH_CHECK("k_ladder_multi");
+  k_ladder_multi<<<blocks((size_t)FEAT * Tptot * s0 * s1), 256, 0, st>>>(W(h, "upsample.up_layers.3.weight"), l5, Tptot * s0, s1, s0,
+                                                                        pseg, segF, segT, l25);
+  MB_LAUNCH_CHECK("k_ladder_multi");
+  k_ladder_multi<<<blocks((size_t)FEAT * Tptot * HOP), 256, 0, st>>>(W(h, "upsample.up_layers.5.weight"), l25, Tptot * s0 * s1, s2,
+                                                                    s0 * s1, pseg, segF, segT, l1);
+  MB_LAUNCH_CHECK("k_ladder_multi");
+  k_crop_melup_multi<<<blocks((size_t)HOP * Ttot * FEAT), 256, 0, st>>>(l1, Tptot * HOP, Ttot, fseg, ws + L.melup);
+  MB_LAUNCH_CHECK("k_crop_melup_multi");
+  k_aux_table_multi<<<(R * 3 * RNN + 255) / 256, 256, 0, st>>>(W(h, "rnn2.weight_ih_l0"), RNN + AUXD, RNN, W(h, "rnn2.bias_ih_l0"),
+                                                               ws + L.aux, AUXD, tsrc, R, 3 * RNN, ws + L.aux2P);
+  MB_LAUNCH_CHECK("k_aux_table_multi");
+  k_aux_table_multi<<<(R * RNN + 255) / 256, 256, 0, st>>>(W(h, "fc1.weight"), RNN + AUXD, RNN, W(h, "fc1.bias"), ws + L.aux,
+                                                           2 * AUXD, tsrc, R, RNN, ws + L.aux3P);
+  MB_LAUNCH_CHECK("k_aux_table_multi");
+  k_aux_table_multi<<<(R * RNN + 255) / 256, 256, 0, st>>>(W(h, "fc2.weight"), RNN + AUXD, RNN, W(h, "fc2.bias"), ws + L.aux,
+                                                           3 * AUXD, tsrc, R, RNN, ws + L.aux4P);
+  MB_LAUNCH_CHECK("k_aux_table_multi");
+  h->cond_T = 0;
+  h->cond_ws = workspace;
+  h->cond_frames.assign(frames, frames + U);
+  return MB_OK;
+}
+
+int mb_wavernn_generate_multi(mb_wavernn* h, const int32_t* row_utt, const int32_t* row_start, const int32_t* row_steps,
+                              const int32_t* row_fold, int32_t rows, const uint64_t* utt_seeds, int32_t max_steps,
+                              int32_t step0, int32_t nsteps, int32_t n_live, const float* noise, int16_t* out_idx,
+                              void* workspace, size_t workspace_bytes, void* stream) {
+  if (!h || !row_utt || !row_start || !row_steps || !row_fold || !out_idx || !workspace || (!noise && !utt_seeds))
+    return fail(MB_ERR_INVALID, "mb_wavernn_generate_multi: null argument");
+  if (h->mode != MB_WAVERNN_RAW)
+    return fail(MB_ERR_INVALID, "mb_wavernn_generate_multi: a MOL handle samples floats (mb_wavernn_generate_multi_mol)");
+  return generate_multi_impl("mb_wavernn_generate_multi", h, row_utt, row_start, row_steps, row_fold, rows, utt_seeds, max_steps,
+                             step0, nsteps, n_live, noise, out_idx, nullptr, workspace, workspace_bytes, stream);
+}
+
+int mb_wavernn_generate_multi_mol(mb_wavernn* h, const int32_t* row_utt, const int32_t* row_start, const int32_t* row_steps,
+                                  const int32_t* row_fold, int32_t rows, const uint64_t* utt_seeds, int32_t max_steps,
+                                  int32_t step0, int32_t nsteps, int32_t n_live, const float* uniforms, float* out_x,
+                                  void* workspace, size_t workspace_bytes, void* stream) {
+  if (!h || !row_utt || !row_start || !row_steps || !row_fold || !out_x || !workspace || (!uniforms && !utt_seeds))
+    return fail(MB_ERR_INVALID, "mb_wavernn_generate_multi_mol: null argument");
+  if (h->mode != MB_WAVERNN_MOL)
+    return fail(MB_ERR_INVALID, "mb_wavernn_generate_multi_mol: the handle was not created in MOL mode");
+  return generate_multi_impl("mb_wavernn_generate_multi_mol", h, row_utt, row_start, row_steps, row_fold, rows, utt_seeds,
+                             max_steps, step0, nsteps, n_live, uniforms, nullptr, out_x, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

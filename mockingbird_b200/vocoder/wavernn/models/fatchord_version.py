@@ -25,7 +25,8 @@ from __future__ import annotations
 
 import ctypes as C
 import time
-from typing import Dict, Optional, Tuple
+import os
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -48,6 +49,54 @@ def fold_geometry(total_len: int, target: int, overlap: int):
     if remaining != 0:
         num_folds += 1
     return num_folds, np.arange(num_folds, dtype=np.int32) * (target + overlap)
+
+
+class RowPlan:
+    """Row table of one multi-utterance sample loop (``WaveRNN.generate_many``).  Every utterance contributes its folds
+    (``batched``) or one row of ``hop * frames`` steps as adjacent rows; utterances are ordered longest rows first (ties:
+    input order), so the rows alive at any step are a prefix of the table and a 64-row block of the kernel empties as
+    soon as its last row ends.
+
+    ``order``: input index of the k-th utterance in row order; ``row_utt`` (k, not the input index), ``row_start``,
+    ``row_steps``, ``row_fold``: one entry per row; ``utt_row0[k]``, ``utt_rows[k]``, ``utt_steps[k]``: the k-th
+    utterance's block."""
+
+    def __init__(self, frames: Sequence[int], batched: bool, target: int, overlap: int, total_scale: int = 200):
+        geo = []
+        for T in frames:
+            total = int(T) * total_scale
+            if batched:
+                B, starts = fold_geometry(total, target, overlap)
+                steps = target + 2 * overlap
+            else:
+                B, starts, steps = 1, np.zeros(1, dtype=np.int32), total
+            if T <= 0 or B <= 0 or steps <= 0:
+                raise ValueError(f"an utterance of {T} frames has no row to generate")
+            geo.append((B, starts, steps))
+        self.order = sorted(range(len(geo)), key=lambda u: (-geo[u][2], u))
+        self.frames = [int(frames[u]) for u in self.order]
+        self.utt_rows = [geo[u][0] for u in self.order]
+        self.utt_steps = [geo[u][2] for u in self.order]
+        self.utt_row0 = [int(v) for v in np.concatenate([[0], np.cumsum(self.utt_rows)[:-1]])]
+        self.rows = int(sum(self.utt_rows))
+        self.max_steps = self.utt_steps[0]
+        self.row_utt = np.repeat(np.arange(len(geo), dtype=np.int32), self.utt_rows)
+        self.row_start = np.concatenate([geo[u][1] for u in self.order]).astype(np.int32)
+        self.row_steps = np.repeat(np.asarray(self.utt_steps, np.int32), self.utt_rows)
+        self.row_fold = np.concatenate([np.arange(b, dtype=np.int32) for b in self.utt_rows])
+
+    def live(self, step0: int) -> Tuple[int, int]:
+        """(utterances, rows) still running at step ``step0``"""
+        k = int(np.searchsorted(-np.asarray(self.utt_steps), -step0, side="left"))  # utt_steps > step0
+        return k, (self.utt_row0[k] if k < len(self.utt_rows) else self.rows)
+
+    def chunks(self, chunk: int):
+        """(step0, nsteps, live utterances, live rows) of every kernel call"""
+        out = []
+        for step0 in range(0, self.max_steps, chunk):
+            k, r = self.live(step0)
+            out.append((step0, min(chunk, self.max_steps - step0), k, r))
+        return out
 
 
 def torch_cpu_generator_position():
@@ -333,11 +382,16 @@ class WaveRNN:
                     set_torch_cpu_generator_position(g_state, left_c.value, next_c.value)
         return out
 
-    def _skip_noise(self, B_all: int, steps: int) -> None:
-        """advance the global generator as a full generate() would (a rank that owns no fold of the utterance)"""
+    def _skip_noise(self, B_all: int, steps: int, advance: bool = True):
+        """advance the global generator as a full generate() would (a rank that owns no fold of the utterance); returns
+        the position (state, left, next) at which that generate() starts to draw its noise.  ``advance=False`` stops
+        there (after the two GRUCell constructions)."""
         nn.GRUCell(self.rnn_dims, self.rnn_dims)
         nn.GRUCell(self.rnn_dims + self.aux_dims, self.rnn_dims)
         state, left, nxt = torch_cpu_generator_position()
+        begin = (state.copy(), left, nxt)
+        if not advance:
+            return begin
         per_step, wpe = self._noise_layout(B_all)
         n = steps * per_step * wpe
         scratch = np.empty(1 << 20, np.uint32)
@@ -347,6 +401,168 @@ class WaveRNN:
             _lib.check(_lib.lib().mb_mt19937_fill(state.ctypes.data, C.byref(l), C.byref(x), scratch.ctypes.data, m))
             n -= m
         set_torch_cpu_generator_position(state, l.value, x.value)
+        return begin
+
+    def noise_starts(self, blocks: Sequence[Tuple[int, int]], seeds: Optional[Sequence[int]]):
+        """Generator position at which each utterance's noise begins; ``blocks[u] = (rows, steps)`` in input order.
+        ``seeds=None``: where ``[generate(m) for m in mels]`` would begin utterance u under the global generator's current
+        state - the stream is walked once on the host, and the generator is left where that loop leaves it.  ``seeds``:
+        the position after ``torch.manual_seed(seeds[u])`` and the two GRUCell constructions; the global generator is
+        put back as it was."""
+        if seeds is None:
+            return [self._skip_noise(B, steps) for B, steps in blocks]
+        if len(seeds) != len(blocks):
+            raise ValueError(f"{len(seeds)} seeds for {len(blocks)} utterances")
+        saved = torch.get_rng_state()
+        try:
+            pos = []
+            for (B, steps), s in zip(blocks, seeds):
+                torch.default_generator.manual_seed(int(s))  # the CPU generator only: the noise is drawn from it
+                pos.append(self._skip_noise(B, steps, advance=False))
+        finally:
+            torch.set_rng_state(saved)
+        return pos
+
+    def generate_many_device(self, mels: Sequence[torch.Tensor], batched: bool, target: int, overlap: int,
+                             seeds: Optional[Sequence[int]] = None, progress_callback=None,
+                             noise: Optional[Sequence[torch.Tensor]] = None, prefill=None) -> List[torch.Tensor]:
+        """The device part of generate_many(): for utterance u (input order) the int16 class indices (RAW) or float32
+        samples (MOL) ``[folds_u, steps_u]`` that generate_indices_device / generate_samples_device return for it alone,
+        all utterances sharing one sequence of sample-loop launches.  ``mels[u]``: ``[1, 80, T_u]`` or ``[80, T_u]``.
+        ``noise[u]``: injected noise in the single call's layout (``[steps_u, folds_u, 512]`` / ``[steps_u, 11 * folds_u]``).
+        ``seeds``: with ``rng="torch"`` see noise_starts(); with ``rng="device"`` the built-in generator's seed per
+        utterance (default: ``self.seed`` for all).  ``prefill``: value the output buffer holds before the loop (tests:
+        a row writes nothing past its own last step); the results are views of that ``[rows, max_steps]`` buffer."""
+        mol = self.mode == 'MOL'
+        if not self._ready:
+            self._upload()
+        if len(mels) == 0:
+            return []
+        if self.rng not in ("torch", "device"):
+            raise ValueError(f"generate_many draws its noise with rng 'torch' or 'device', not {self.rng!r} "
+                             "('torch_host' is the single-utterance replay)")
+        L = _lib.lib()
+        dev = self._device
+        mel2d = [m.reshape(-1, m.shape[-1]).to(dtype=torch.float32) for m in mels]
+        plan = RowPlan([int(m.shape[1]) for m in mel2d], batched, target, overlap, self._total_scale)
+        U, rows, max_steps = len(mel2d), plan.rows, plan.max_steps
+        if seeds is not None and len(seeds) != U:
+            raise ValueError(f"{len(seeds)} seeds for {U} utterances")
+        per_row, wpe = self._noise_layout(1)  # noise elements per row and step, MT19937 words per element
+        use_mt = noise is None and self.rng == "torch"
+        if use_mt:
+            blocks = [None] * U
+            for k, u in enumerate(plan.order):
+                blocks[u] = (plan.utt_rows[k], plan.utt_steps[k])
+            starts = self.noise_starts(blocks, seeds)
+            mt_state = np.stack([starts[u][0] for u in plan.order]).astype(np.uint32)
+            mt_left = np.array([starts[u][1] for u in plan.order], np.int32)
+            mt_next = np.array([starts[u][2] for u in plan.order], np.int32)
+            wps = np.array([b * per_row * wpe for b in plan.utt_rows], np.uint64)
+            col = np.concatenate([[0], np.cumsum(wps)[:-1]]).astype(np.uint64)
+            threads = max(1, min(8, os.cpu_count() or 1))
+        useed = [int(s) for s in seeds] if seeds is not None else [int(self.seed)] * U
+        seeds_c = (C.c_uint64 * U)(*[useed[u] for u in plan.order])
+        start_t = time.time()
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev)
+            frames_c = (C.c_int32 * U)(*plan.frames)
+            need = int(L.mb_wavernn_workspace_bytes_multi(self._handle, U, frames_c, rows, max_steps)) + 256
+            if need <= 256:
+                raise _lib.MbError("generate_many: the utterances do not fit one loop (too many frames in all)")
+            if self._ws is None or self._ws.numel() < need:
+                self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            ws = self._ws
+            mel_cat = torch.cat([mel2d[u].reshape(-1) for u in plan.order]).to(dev).contiguous()
+            _lib.check(L.mb_wavernn_condition_multi(self._handle, C.c_void_p(mel_cat.data_ptr()), frames_c, U,
+                                                    C.c_void_p(ws.data_ptr()), ws.numel(), C.c_void_p(stream.cuda_stream)))
+            out_dtype = torch.float32 if mol else torch.int16
+            out = torch.empty(rows, max_steps, dtype=out_dtype, device=dev)
+            if prefill is not None:
+                out.fill_(prefill)
+            as_i32 = lambda a: np.ascontiguousarray(a, np.int32).ctypes.data_as(C.POINTER(C.c_int32))
+            row_utt, row_start, row_steps, row_fold = plan.row_utt, plan.row_start, plan.row_steps, plan.row_fold
+            per_step = rows * per_row
+            host_noise = noise is not None or use_mt
+            dbufs = [torch.empty(CHUNK * per_step, dtype=torch.float32, device=dev) for _ in range(2)] if host_noise else None
+            if use_mt:
+                # chunk k+1 is drawn on the host and copied / converted on a side stream while the loop runs chunk k
+                side = torch.cuda.Stream(dev)
+                pinned = [torch.empty(CHUNK * per_step * wpe, dtype=torch.int32).pin_memory() for _ in range(2)]
+                raw = [torch.empty(CHUNK * per_step * wpe, dtype=torch.int32, device=dev) for _ in range(2)]
+                copied = [torch.cuda.Event() for _ in range(2)]
+                consumed = [torch.cuda.Event() for _ in range(2)]
+                convert = L.mb_mt_to_uniform if mol else L.mb_mt_to_exp
+            gen = L.mb_wavernn_generate_multi_mol if mol else L.mb_wavernn_generate_multi
+            for ci, (step0, n, k_live, n_live) in enumerate(plan.chunks(CHUNK)):
+                nptr = None
+                slot = ci & 1
+                stride = n_live * per_row
+                if noise is not None:
+                    view = dbufs[slot][:n * stride].view(n, stride)
+                    for k in range(k_live):
+                        nk = min(n, plan.utt_steps[k] - step0)
+                        c0, c1 = plan.utt_row0[k] * per_row, (plan.utt_row0[k] + plan.utt_rows[k]) * per_row
+                        src = noise[plan.order[k]][step0:step0 + nk].to(torch.float32).reshape(nk, c1 - c0)
+                        view[:nk, c0:c1].copy_(src, non_blocking=True)
+                    nptr = C.c_void_p(dbufs[slot].data_ptr())
+                elif use_mt:
+                    if ci >= 2:
+                        copied[slot].synchronize()  # the H2D that last read this pinned buffer is done
+                    nst = np.minimum(n, np.asarray(plan.utt_steps[:k_live]) - step0).astype(np.int32)
+                    _lib.check(L.mb_mt19937_fill_sources(k_live, mt_state.ctypes.data, mt_left.ctypes.data, mt_next.ctypes.data,
+                                                         wps.ctypes.data, col.ctypes.data, nst.ctypes.data,
+                                                         C.c_void_p(pinned[slot].data_ptr()), stride * wpe, threads))
+                    with torch.cuda.stream(side):
+                        if ci >= 2:
+                            side.wait_event(consumed[slot])
+                        raw[slot][:n * stride * wpe].copy_(pinned[slot][:n * stride * wpe], non_blocking=True)
+                        copied[slot].record(side)
+                        _lib.check(convert(C.c_void_p(raw[slot].data_ptr()), C.c_void_p(dbufs[slot].data_ptr()), n * stride,
+                                           C.c_void_p(side.cuda_stream)))
+                    stream.wait_stream(side)
+                    nptr = C.c_void_p(dbufs[slot].data_ptr())
+                _lib.check(gen(self._handle, as_i32(row_utt), as_i32(row_start), as_i32(row_steps), as_i32(row_fold), rows,
+                               seeds_c, max_steps, step0, n, n_live, nptr, C.c_void_p(out.data_ptr()),
+                               C.c_void_p(ws.data_ptr()), ws.numel(), C.c_void_p(stream.cuda_stream)))
+                if use_mt:
+                    consumed[slot].record(stream)
+                if progress_callback is not None:
+                    gen_rate = (step0 + 1) / max(time.time() - start_t, 1e-9) * n_live / 1000
+                    progress_callback(step0, max_steps, n_live, gen_rate)
+            if use_mt:
+                stream.synchronize()  # the pinned and raw buffers die with this frame
+        res = [None] * U
+        for k, u in enumerate(plan.order):
+            r0 = plan.utt_row0[k]
+            res[u] = out[r0:r0 + plan.utt_rows[k], :plan.utt_steps[k]]
+        return res
+
+    def generate_many(self, mels: Sequence[torch.Tensor], batched, target, overlap, mu_law, seeds=None,
+                      progress_callback=None) -> List[np.ndarray]:
+        """generate() for a list of utterances ``[1, 80, T_u]`` in one sample loop: the float64 waveforms in input order,
+        each what ``generate(mels[u], ...)`` returns for it alone.  ``seeds=None``: as the Python loop of generate() calls
+        under the global generator's state (which is left where that loop leaves it); ``seeds=[s_u]``: utterance u as
+        under ``torch.manual_seed(s_u)``, the global generator untouched."""
+        mu_law = mu_law if self.mode == 'RAW' else False
+        fade = 20 * self.hop_length
+        for m in mels:  # the single call fails on these in its fade-out, after generating
+            T = int(m.shape[-1])
+            total = T * self._total_scale
+            span = fold_geometry(total, target, overlap)[0] * (target + overlap) + overlap if batched else total
+            if min(span, (T - 1) * self.hop_length) < fade:
+                raise ValueError(f"an utterance of {T} frames is shorter than the {fade}-sample fade-out")
+        self.eval()
+        idx = self.generate_many_device(mels, batched, target, overlap, seeds, progress_callback or self.gen_display)
+        wavs = []
+        for m, rows in zip(mels, idx):
+            T = int(m.shape[-1])
+            if self.post == "device":
+                wavs.append(self.postprocess_device(rows, T, batched, target, overlap, mu_law))
+            else:
+                wavs.append(self.postprocess(rows.cpu().numpy(), T, batched, target, overlap, mu_law))
+        self.train()  # side effect of generate() kept
+        return wavs
 
     def postprocess(self, idx: np.ndarray, frames: int, batched: bool, target: int, overlap: int, mu_law: bool) -> np.ndarray:
         """class indices [folds, steps] (RAW) or float samples (MOL) -> waveform, the host float64 tail of generate()
