@@ -558,6 +558,57 @@ int32_t mb_melspec_num_frames(const mb_melspec* h, int32_t n_samples);   /* 1 + 
 int mb_melspec_forward(mb_melspec* h, const float* wav, int32_t n_samples, float* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Griffin-Lim inversion of normalised dB mel spectrograms (DESIGN.md section 4i; csrc/griffinlim.cu)
+ *   replaces  models/synthesizer/audio.py:84-99 (inv_mel_spectrogram), :105-124 (_griffin_lim with librosa.stft / istft),
+ *             :162-166 (_mel_to_linear), :177-206 (_db_to_amp, _denormalize), :25-28 (inv_preemphasis)
+ * librosa's contract: centred frames (n_fft / 2 padding), periodic Hann window of win_length centred in n_fft, ISTFT by
+ * overlap-add divided by the window sum-square where it exceeds FLT_MIN and trimmed to hop (T - 1) samples, angle(0) = 0,
+ * the imaginary parts of the DC and Nyquist bins ignored by the inverse transform.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct mb_griffinlim_config {
+  int32_t n_fft;                /* 256, 512, 1024 or 2048 */
+  int32_t hop_length;           /* 1 .. win_length */
+  int32_t win_length;           /* 1 .. n_fft */
+  int32_t n_mels;               /* 1 .. 1024 */
+  int32_t pad_mode;             /* centred frames of the STFT: 0 = reflect, 1 = constant (zeros) */
+  float power;                  /* S = max(1e-10, inv_mel_basis @ amp) ** power (hparams.power, 1.5) */
+  double preemphasis;           /* 0: off; else out = lfilter([1], [1, -k], y), 0 < k with k^W < 2^-30 for W <= 4096 */
+  int32_t signal_normalization; /* 1: _denormalize the input first */
+  int32_t allow_clipping;       /* allow_clipping_in_normalization: clip to [-A, A] (symmetric) or [0, A] first */
+  int32_t symmetric;            /* symmetric_mels */
+  float max_abs_value;          /* A */
+  float min_level_db, ref_level_db;
+} mb_griffinlim_config;
+
+typedef struct mb_griffinlim mb_griffinlim;
+
+/* MB_ERR_INVALID, with a message, for a non-power-of-two or out-of-range n_fft, win_length > n_fft, hop_length >
+ * win_length, and a pre-emphasis whose inverse filter needs a warm-up of more than 4096 samples */
+int mb_griffinlim_create(const mb_griffinlim_config* cfg, mb_griffinlim** out);
+void mb_griffinlim_destroy(mb_griffinlim* h);
+size_t mb_griffinlim_arena_bytes(const mb_griffinlim* h);
+int mb_griffinlim_set_arena(mb_griffinlim* h, void* arena, size_t bytes);
+/* one tensor, "inv_mel_basis" [n_fft / 2 + 1][n_mels] (the caller's pseudo-inverse of the mel basis); finalize writes the
+ * window and the FFT twiddles (computed on the host in float64 at create) into the arena and synchronises `stream` */
+int mb_griffinlim_set_weight(mb_griffinlim* h, const char* name, const float* w, const int64_t* dims, int32_t ndim,
+                             void* stream);
+int mb_griffinlim_finalize(mb_griffinlim* h, void* stream);
+/* frames_host int32 [batch] (host); 0 when batch < 1 or a length is < 1 */
+size_t mb_griffinlim_workspace_bytes(const mb_griffinlim* h, int32_t batch, const int32_t* frames_host);
+/* inv_mel_spectrogram for `batch` utterances of frames_host[b] frames in one sequence of 2 n_iters + 4 launches:
+ *   mels fp32: one [n_mels][T_b] row-major block per utterance, back to back (device)
+ *   uniforms float64: one [n_fft / 2 + 1][T_b] block per utterance, back to back (device), the initial phases exp(2 pi i u);
+ *     or NULL and seeds_host uint64 [batch] (host): u drawn on the device from Philox keyed by (seed_b, bin, frame).
+ *     Exactly one of the two is given.
+ *   out fp32 [sum_b hop (T_b - 1)] (device)
+ * Each utterance's output is bitwise what a batch of that utterance alone gives.  MB_ERR_INVALID before anything is queued
+ * for n_iters < 0 and for an utterance too short for the pad mode (reflect: hop (T - 1) > n_fft / 2; constant: T >= 2);
+ * the message names the utterance.  The row tables are copied from pageable host memory into the workspace. */
+int mb_griffinlim_forward(mb_griffinlim* h, const float* mels, const int32_t* frames_host, int32_t batch,
+                          const double* uniforms, const uint64_t* seeds_host, int32_t n_iters, float* out, void* workspace,
+                          size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Voice-conversion mel decoder (ppg2mel)
  *   replaces  models/ppg2mel/__init__.py:166-192 (MelDecoderMOLv2.inference: PPG / pitch encoder, reduce_proj with the
  *             normalised speaker embedding), models/ppg2mel/rnn_decoder_mol.py:267-315 (Decoder.inference: PreNet with

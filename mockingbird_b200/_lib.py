@@ -162,6 +162,13 @@ class MelSpecConfig(C.Structure):
                 ("symmetric", C.c_int32), ("transpose_out", C.c_int32)]
 
 
+class GriffinLimConfig(C.Structure):
+    _fields_ = [("n_fft", C.c_int32), ("hop_length", C.c_int32), ("win_length", C.c_int32), ("n_mels", C.c_int32),
+                ("pad_mode", C.c_int32), ("power", C.c_float), ("preemphasis", C.c_double),
+                ("signal_normalization", C.c_int32), ("allow_clipping", C.c_int32), ("symmetric", C.c_int32),
+                ("max_abs_value", C.c_float), ("min_level_db", C.c_float), ("ref_level_db", C.c_float)]
+
+
 # name -> (restype, argtypes); every symbol include/mockingbird_b200.h declares
 SIGNATURES = {
     "mb_last_error": (C.c_char_p, []),
@@ -278,6 +285,15 @@ SIGNATURES = {
     "mb_melspec_set_arena": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_melspec_num_frames": (C.c_int32, [C.c_void_p, C.c_int32]),
     "mb_melspec_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "mb_griffinlim_create": (C.c_int, [C.POINTER(GriffinLimConfig), C.POINTER(C.c_void_p)]),
+    "mb_griffinlim_destroy": (None, [C.c_void_p]),
+    "mb_griffinlim_arena_bytes": (C.c_size_t, [C.c_void_p]),
+    "mb_griffinlim_set_arena": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "mb_griffinlim_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int32, C.c_void_p]),
+    "mb_griffinlim_finalize": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "mb_griffinlim_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]),
+    "mb_griffinlim_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p,
+                                        C.POINTER(C.c_uint64), C.c_int32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_ppg2mel_create": (C.c_int, [C.POINTER(Ppg2MelConfig), C.POINTER(C.c_void_p)]),
     "mb_ppg2mel_destroy": (None, [C.c_void_p]),
     "mb_ppg2mel_arena_bytes": (C.c_size_t, [C.c_void_p]),

@@ -116,6 +116,15 @@ class Synthesizer:
 
         return audio_host.inv_mel_spectrogram(mel, hparams)
 
+    @staticmethod
+    def griffin_lim_many(mels, seeds=None):
+        """Griffin-Lim of a list of mel spectrograms [80, T_b] in one sequence of launches on the H100 -> list of float64
+        waveforms (synthesizer/audio.py inv_mel_spectrograms: seeds=None draws the phases from numpy's global state as the
+        same sequence of griffin_lim calls would)"""
+        from . import audio
+
+        return audio.inv_mel_spectrograms(mels, hparams, seeds)
+
     def synthesize_from_sequences(self, inputs, embeddings, return_alignments=False, style_idx=0, min_stop_token=5,
                                   steps=2000, dropout_masks=None):
         """the part of synthesize_spectrograms after the text front-end (inference.py:104-142)"""
