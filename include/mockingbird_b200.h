@@ -609,6 +609,56 @@ int mb_griffinlim_forward(mb_griffinlim* h, const float* mels, const int32_t* fr
                           size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Log-MMSE speech enhancement (DESIGN.md section 4j; csrc/logmmse.cu)
+ *   replaces  utils/logmmse.py:36-69 (profile_noise), :72-133 (denoise), as models/synthesizer/inference.py:145-159
+ *             (load_preprocess_wav) calls them
+ * The reference's contract: samples + DBL_EPSILON times the caller's window, zero-padded n_fft-point FFTs; the profile averages
+ * |X| over the non-overlapping frames of the noise and squares it; the denoiser runs nframes = L // len2 - W // len2 frames
+ * at hop len2 with the gain recursion of utils/logmmse.py, overlap-adds the first W samples of each Re(IFFT(hw X)) and
+ * leaves the samples past nframes * len2 at zero.  All float64; the output is rounded once to fp32.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct mb_logmmse_config {
+  int32_t window_size; /* W: even, 2 .. n_fft (NoiseProfile.window_size, 320 at 16 kHz) */
+  int32_t len1, len2;  /* both W / 2 */
+  int32_t n_fft;       /* 2^a or 5 * 2^a in [64, 2048] (2 W in the reference) */
+} mb_logmmse_config;
+
+typedef struct mb_logmmse mb_logmmse;
+
+/* MB_ERR_INVALID, with a message naming the field, for any other n_fft, W or len1 / len2 */
+int mb_logmmse_create(const mb_logmmse_config* cfg, mb_logmmse** out);
+void mb_logmmse_destroy(mb_logmmse* h);
+/* the handle holds no checkpoint tensor: its arena is the FFT twiddles (float64, computed on the host at create), which
+ * finalize writes and then synchronises `stream` */
+size_t mb_logmmse_arena_bytes(const mb_logmmse* h);
+int mb_logmmse_set_arena(mb_logmmse* h, void* arena, size_t bytes);
+int mb_logmmse_finalize(mb_logmmse* h, void* stream);
+/* lengths_host int32 [batch] (host); 0 when batch < 1 or a length is < 2 len2.  Also enough for mb_logmmse_profile with
+ * the same lengths. */
+size_t mb_logmmse_workspace_bytes(const mb_logmmse* h, int32_t batch, const int32_t* lengths_host);
+/* profile_noise for `batch` noise signals in one launch:
+ *   noise fp32: the signals back to back (device), lengths_host[b] >= W samples each (host)
+ *   window float64 [W] (device): NoiseProfile.win
+ *   noise_mu2 float64 [batch][n_fft] (device, out)
+ * MB_ERR_INVALID before anything is queued for a signal shorter than W; the message names it. */
+int mb_logmmse_profile(mb_logmmse* h, const float* noise, const int32_t* lengths_host, int32_t batch, const double* window,
+                       double* noise_mu2, void* workspace, size_t workspace_bytes, void* stream);
+/* denoise for `batch` utterances in one sequence of 4 launches:
+ *   x fp32: the utterances back to back (device), lengths_host[b] >= 2 len2 samples each (host)
+ *   window float64 [W], noise_mu2 float64 [batch][n_fft] (device): each utterance's NoiseProfile (bins 0 .. n_fft / 2 read)
+ *   eta: the VAD threshold below which noise_mu2 is updated (0 disables the update)
+ *   out fp32 [sum_b L_b] (device)
+ *   vad_out float64 [sum_b nframes_b] (device) or NULL: each frame's VAD statistic
+ * Each utterance's output is bitwise what a batch of that utterance alone gives.  MB_ERR_INVALID before anything is queued
+ * for an utterance shorter than 2 len2 (the reference fails on it); the message names the utterance.  The row tables are
+ * copied from pageable host memory into the workspace. */
+int mb_logmmse_denoise(mb_logmmse* h, const float* x, const int32_t* lengths_host, int32_t batch, const double* window,
+                       const double* noise_mu2, double eta, float* out, double* vad_out, void* workspace,
+                       size_t workspace_bytes, void* stream);
+/* E1(x) = expint(1, x) for x > 0, the device function the gains use: x, y float64 [n] (device) */
+int mb_logmmse_exp1(const double* x, double* y, int64_t n, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Voice-conversion mel decoder (ppg2mel)
  *   replaces  models/ppg2mel/__init__.py:166-192 (MelDecoderMOLv2.inference: PPG / pitch encoder, reduce_proj with the
  *             normalised speaker embedding), models/ppg2mel/rnn_decoder_mol.py:267-315 (Decoder.inference: PreNet with

@@ -169,6 +169,10 @@ class GriffinLimConfig(C.Structure):
                 ("max_abs_value", C.c_float), ("min_level_db", C.c_float), ("ref_level_db", C.c_float)]
 
 
+class LogMmseConfig(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("window_size", "len1", "len2", "n_fft")]
+
+
 # name -> (restype, argtypes); every symbol include/mockingbird_b200.h declares
 SIGNATURES = {
     "mb_last_error": (C.c_char_p, []),
@@ -294,6 +298,17 @@ SIGNATURES = {
     "mb_griffinlim_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]),
     "mb_griffinlim_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p,
                                         C.POINTER(C.c_uint64), C.c_int32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mb_logmmse_create": (C.c_int, [C.POINTER(LogMmseConfig), C.POINTER(C.c_void_p)]),
+    "mb_logmmse_destroy": (None, [C.c_void_p]),
+    "mb_logmmse_arena_bytes": (C.c_size_t, [C.c_void_p]),
+    "mb_logmmse_set_arena": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "mb_logmmse_finalize": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "mb_logmmse_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]),
+    "mb_logmmse_profile": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mb_logmmse_denoise": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p,
+                                     C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mb_logmmse_exp1": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "mb_ppg2mel_create": (C.c_int, [C.POINTER(Ppg2MelConfig), C.POINTER(C.c_void_p)]),
     "mb_ppg2mel_destroy": (None, [C.c_void_p]),
     "mb_ppg2mel_arena_bytes": (C.c_size_t, [C.c_void_p]),

@@ -15,8 +15,8 @@
 //
 // One CTA per pair of consecutive frames of ONE utterance (local frames 2p, 2p + 1; an odd last frame is paired with
 // zeros): the two real frames are the real and imaginary parts of one complex transform.  The pairing depends on the
-// utterance alone, so each utterance's output is bitwise what a B = 1 call gives.  The FFT is a shared-memory Stockham
-// radix-4 (radix-2 last stage for odd log2 n_fft) over twiddles computed on the host in float64.
+// utterance alone, so each utterance's output is bitwise what a B = 1 call gives.  The FFT is the shared-memory Stockham of
+// mb_fft.cuh (radix 4, radix-2 last stage for odd log2 n_fft) over twiddles computed on the host in float64.
 #include <cfloat>
 #include <cmath>
 #include <cstring>
@@ -24,6 +24,7 @@
 
 #include "../../include/mb_wavernn_math.h"
 #include "mb_common.h"
+#include "mb_fft.cuh"
 
 using namespace mb;
 
@@ -55,49 +56,6 @@ struct GlParams {
   float* y;             // [sum hop (T - 1)]
   float* out;
 };
-
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) {
-  return make_float2(fmaf(a.x, b.x, -(a.y * b.y)), fmaf(a.x, b.y, a.y * b.x));
-}
-__device__ __forceinline__ float2 cadd(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
-__device__ __forceinline__ float2 csub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
-
-// Stockham autosort FFT of N = 2^m complex points in shared memory (a -> b -> a ...); returns the buffer holding the
-// result.  INV: exp(+2 pi i) twiddles, unscaled.
-template <bool INV>
-__device__ float2* stockham(float2* a, float2* b, const float2* __restrict__ tw, int N) {
-  for (int Ns = 1; Ns < N;) {
-    const int R = ((N / Ns) & 3) == 0 ? 4 : 2;
-    const int nr = N / R, step = N / (Ns * R);
-    for (int j = threadIdx.x; j < nr; j += blockDim.x) {
-      const int k = j & (Ns - 1);
-      const int d = (j - k) * R + k;
-      if (R == 4) {
-        float2 t1 = __ldg(tw + k * step), t2 = __ldg(tw + 2 * k * step), t3 = __ldg(tw + 3 * k * step);
-        if (INV) t1.y = -t1.y, t2.y = -t2.y, t3.y = -t3.y;
-        const float2 v0 = a[j], v1 = cmul(a[j + nr], t1), v2 = cmul(a[j + 2 * nr], t2), v3 = cmul(a[j + 3 * nr], t3);
-        const float2 b0 = cadd(v0, v2), b1 = csub(v0, v2), b2 = cadd(v1, v3), e = csub(v1, v3);
-        const float2 b3 = INV ? make_float2(-e.y, e.x) : make_float2(e.y, -e.x);  // (v1 - v3) * (+-i)
-        b[d] = cadd(b0, b2);
-        b[d + Ns] = cadd(b1, b3);
-        b[d + 2 * Ns] = csub(b0, b2);
-        b[d + 3 * Ns] = csub(b1, b3);
-      } else {
-        float2 t1 = __ldg(tw + k * step);
-        if (INV) t1.y = -t1.y;
-        const float2 v0 = a[j], v1 = cmul(a[j + nr], t1);
-        b[d] = cadd(v0, v1);
-        b[d + Ns] = csub(v0, v1);
-      }
-    }
-    __syncthreads();
-    float2* t = a;
-    a = b;
-    b = t;
-    Ns *= R;
-  }
-  return a;
-}
 
 // sample i of the centred signal (i in padded coordinates minus n_fft / 2): reflect (numpy "reflect") or zero outside [0, L)
 __device__ __forceinline__ float sample_at(const float* __restrict__ y, int L, int i, int pad_mode) {

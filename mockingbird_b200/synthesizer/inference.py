@@ -101,6 +101,30 @@ class Synthesizer:
         return wav
 
     @staticmethod
+    def load_preprocess_wavs(fpaths_or_wavs):
+        """the reference's load_preprocess_wav (inference.py:145-159) for a list of clips, denoised on the device: each
+        path is loaded at the synthesizer rate (an array is taken as already at that rate) and rescaled; every clip longer
+        than 0.4 s is then denoised with the noise profile of its first and last 0.15 s, all profiles in one launch and all
+        clips in one logmmse.denoise_many.  -> list of float32 waveforms"""
+        from .. import logmmse
+        from . import audio_host
+
+        sr = hparams.sample_rate
+        wavs = []
+        for x in fpaths_or_wavs:
+            wav = audio_host.load_wav(x, sr)[0] if isinstance(x, (str, Path)) else np.asarray(x)
+            if hparams.rescale:
+                wav = wav / np.abs(wav).max() * hparams.rescaling_max
+            wavs.append(wav)
+        noisy = [i for i, w in enumerate(wavs) if len(w) > sr * (0.3 + 0.1)]
+        if noisy:
+            edge = int(sr * 0.15)
+            profiles = logmmse.profile_noise_many([np.concatenate([wavs[i][:edge], wavs[i][-edge:]]) for i in noisy], sr)
+            for i, w in zip(noisy, logmmse.denoise_many([wavs[i] for i in noisy], profiles)):
+                wavs[i] = w
+        return wavs
+
+    @staticmethod
     def make_spectrogram(fpath_or_wav):
         """inference.py:160-172: mel spectrogram [80, M] as fed to the synthesizer in training (GPU front-end,
         synthesizer/audio.py)"""
