@@ -408,7 +408,11 @@ int mb_tacotron_set_arena(mb_tacotron* h, void* arena, size_t bytes);
 int mb_tacotron_set_weight(mb_tacotron* h, const char* name, const float* w, const int64_t* dims, int32_t ndim,
                            void* stream);
 int mb_tacotron_finalize(mb_tacotron* h, void* stream);
+/* 0 for a shape generate would refuse, including more characters than mb_tacotron_max_chars() (when a device can be asked) */
 size_t mb_tacotron_workspace_bytes(const mb_tacotron* h, int32_t batch, int32_t chars, int32_t steps, int32_t r);
+/* the longest input (characters per utterance) generate accepts on the current device: the attention step keeps
+ * 4 * (5438 + 38 * chars) bytes in shared memory, within the per-block opt-in limit (1386 on an H100); 0 without a device */
+int32_t mb_tacotron_max_chars(void);
 
 /* Tacotron.generate (tacotron.py:295-298) for one padded batch:
  *   chars  int32 [B][Tc] (pad id 0), spk fp32 [B][speaker_embedding_size]
@@ -487,6 +491,67 @@ size_t mb_taco_tc_debug_workspace_bytes(const mb_taco_tc_debug_spec* spec);
  * "kernel=K grid=X,Y cluster=C compact=0|1 rows_pad=R mma_groups=G,G_last inv_scale=S a_bytes=A w_bytes=W" */
 int mb_taco_tc_debug(const mb_taco_tc_debug_spec* spec, void* workspace, size_t workspace_bytes, void* stream, char* report,
                      size_t report_len);
+
+/* test hook: ONE launch of an FP32 kernel of the Tacotron path (csrc/tacotron_kernels.cu, csrc/tacotron.cu) on caller-provided
+ * device tensors (no model handle), through the launcher the forward uses.  GEMM and STOP_STEP read the GemmArgs fields; the
+ * other kinds read in[] / out[] / n[] as listed (n[] entries are sizes, strides and flags in the order given).  Every kind
+ * honours step_ptr / step_j where its kernel takes them. */
+#define MB_TACO_DBG_GEMM 0             /* launch_gemm: the GemmArgs fields below                                              */
+#define MB_TACO_DBG_PRENET 1           /* in: x, x_first, W1, b1, W2, b2, m1, m2  out: y, s_hi, s_lo
+                                          n: B, K, H, ldy, x_ld, x_step, mask_step, s_k0, s_rows_pad                         */
+#define MB_TACO_DBG_GRU_CELL 2         /* in: gi, gh  out: h, out2  n: M, H, ldgi, ldh, ldout2                                 */
+#define MB_TACO_DBG_LSTM_CELL 3        /* in: g  out: c, h, x (x += h, or NULL)  n: M, H                                        */
+#define MB_TACO_DBG_HIGHWAY 4          /* in: x12  out: y  n: M, C                                                              */
+#define MB_TACO_DBG_MAXPOOL2 5         /* in: x  out: y  n: B, T, C                                                             */
+#define MB_TACO_DBG_EMBEDDING 6        /* in: ids (int32), table  out: y  n: M, D                                               */
+#define MB_TACO_DBG_COPY_COLS 7        /* in: src  out: dst  n: M, n, ldsrc, rows_per_src, lddst, off                           */
+#define MB_TACO_DBG_LSA_STEP 8         /* in: pq, proj, seq, chars, conv_w, conv_b, L, v, q_in, Wq, bq  out: cum, scores, ctx
+                                          n: B, Tc, seq_dim, scores_ld, threads (256 | 512); q_in NULL: pq is read          */
+#define MB_TACO_DBG_LSA_CTX 9          /* in: scores, seq  out: ctx, sa_hi, sa_lo, sb_hi, sb_lo
+                                          n: B, Tc, seq_dim (a multiple of 256), scores_ld, s_rows_pad                       */
+#define MB_TACO_DBG_GST_ATTENTION 10   /* in: q, keys, values  out: y  n: B, ntok (<= 16), E, heads (<= 8)                      */
+#define MB_TACO_DBG_STOP_STEP 11       /* GemmArgs (x, W, bias, y, ldy; N = 1) and out: flags, ticket  n: B, r  fval: min_stop */
+#define MB_TACO_DBG_STOP_FLAG 12       /* in: stopv  out: flags  n: B, r  fval: min_stop_token                                  */
+#define MB_TACO_DBG_FILL_MASKS 13      /* out: m  n: count, stream_id  seed (step_ptr: stream_id += *step_ptr)                  */
+#define MB_TACO_DBG_FILL_MASKS_STEPS 14 /* out: m  n: per_step, steps  seed                                                     */
+#define MB_TACO_DBG_PACK_MELPROJ 15    /* in: W  out: dst  n: n_mels, max_r, r, K                                               */
+#define MB_TACO_DBG_TO_NCL 16          /* in: x  out: y  n: steps, B, C, frames                                                 */
+#define MB_TACO_DBG_BN_FOLD 17         /* in: gamma, beta, mean, var  out: scale, shift  n: count                               */
+typedef struct mb_taco_debug_spec {
+  int32_t kind;                /* MB_TACO_DBG_* */
+  /* GemmArgs (csrc/tacotron_kernels.cuh) */
+  int32_t nseg;
+  const float* x[5];
+  int32_t K[5], ld[5], shift[5], w_off[5], w_stride[5];
+  const float* W;
+  int32_t ldw;
+  const float* bias;
+  int32_t M, N, T, act;
+  const float* bn_scale;
+  const float* bn_shift;
+  const uint8_t* mask;
+  const float* res;
+  int32_t ldres;
+  float* y;
+  int32_t ldy;
+  int32_t step_mode;
+  const int32_t* step_ptr;     /* every kind: step = (*step_ptr or 0) + step_j */
+  int32_t step_j;
+  int64_t x_step;
+  const float* x_first;
+  int64_t mask_step;
+  /* the other kinds */
+  const void* in[12];
+  void* out[6];
+  int64_t n[10];
+  float fval;
+  uint64_t seed;
+} mb_taco_debug_spec;
+/* device workspace the spec needs (no kind needs scratch: a nominal 256 bytes), 0 for a spec mb_taco_debug refuses */
+size_t mb_taco_debug_workspace_bytes(const mb_taco_debug_spec* spec);
+/* enqueues the launch on `stream` (no synchronisation); writes one line into `report`: "kernel=K grid=X,Y block=T smem=S" */
+int mb_taco_debug(const mb_taco_debug_spec* spec, void* workspace, size_t workspace_bytes, void* stream, char* report,
+                  size_t report_len);
 
 /* ---------------------------------------------------------------------------------------------
  * Speaker encoder (cfg 5 front half)

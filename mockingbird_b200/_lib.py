@@ -90,6 +90,23 @@ class TacoTcDebugSpec(C.Structure):
     ]
 
 
+MB_TACO_DBG = {k: i for i, k in enumerate((
+    "gemm", "prenet", "gru_cell", "lstm_cell", "highway", "maxpool2", "embedding", "copy_cols", "lsa_step", "lsa_ctx",
+    "gst_attention", "stop_step", "stop_flag", "fill_masks", "fill_masks_steps", "pack_melproj", "to_ncl", "bn_fold"))}
+
+
+class TacoDebugSpec(C.Structure):
+    _fields_ = [
+        ("kind", C.c_int32), ("nseg", C.c_int32), ("x", C.c_void_p * 5), ("K", C.c_int32 * 5), ("ld", C.c_int32 * 5),
+        ("shift", C.c_int32 * 5), ("w_off", C.c_int32 * 5), ("w_stride", C.c_int32 * 5), ("W", C.c_void_p), ("ldw", C.c_int32),
+        ("bias", C.c_void_p), ("M", C.c_int32), ("N", C.c_int32), ("T", C.c_int32), ("act", C.c_int32),
+        ("bn_scale", C.c_void_p), ("bn_shift", C.c_void_p), ("mask", C.c_void_p), ("res", C.c_void_p), ("ldres", C.c_int32),
+        ("y", C.c_void_p), ("ldy", C.c_int32), ("step_mode", C.c_int32), ("step_ptr", C.c_void_p), ("step_j", C.c_int32),
+        ("x_step", C.c_int64), ("x_first", C.c_void_p), ("mask_step", C.c_int64), ("in_", C.c_void_p * 12),
+        ("out", C.c_void_p * 6), ("n", C.c_int64 * 10), ("fval", C.c_float), ("seed", C.c_uint64),
+    ]
+
+
 MB_PPGX_DBG_FRONTEND = 0
 MB_PPGX_DBG_MVN = 1
 MB_PPGX_DBG_CONV0 = 2
@@ -272,6 +289,9 @@ SIGNATURES = {
                                        C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_taco_tc_debug_workspace_bytes": (C.c_size_t, [C.POINTER(TacoTcDebugSpec)]),
     "mb_taco_tc_debug": (C.c_int, [C.POINTER(TacoTcDebugSpec), C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]),
+    "mb_tacotron_max_chars": (C.c_int32, []),
+    "mb_taco_debug_workspace_bytes": (C.c_size_t, [C.POINTER(TacoDebugSpec)]),
+    "mb_taco_debug": (C.c_int, [C.POINTER(TacoDebugSpec), C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]),
     "mb_encoder_create": (C.c_int, [C.POINTER(EncoderConfig), C.POINTER(C.c_void_p)]),
     "mb_encoder_destroy": (None, [C.c_void_p]),
     "mb_encoder_arena_bytes": (C.c_size_t, [C.c_void_p]),

@@ -189,6 +189,29 @@ __global__ void __launch_bounds__(512) lsa_step_kernel(const float* __restrict__
   }
 }
 
+// dynamic shared memory of lsa_step_kernel (the layout at its top): 4 * (5438 + 38 Tc) bytes
+size_t lsa_step_smem_bytes(int Tc) {
+  return sizeof(float) * (ATT_F * ATT_K + ATT_D * ATT_F + 2 * ATT_D + ATT_F + (Tc + 30) + Tc + 32 + (size_t)Tc * ATT_F + (size_t)Tc * 4);
+}
+
+// the longest input (characters per utterance) lsa_step_kernel can take on the current device: its shared memory must fit the
+// per-block opt-in limit (1386 at the H100's 227 KB); 0 when there is no device to ask
+int lsa_max_chars() {
+  int dev = 0, optin = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess) {
+    cudaGetLastError();
+    return 0;
+  }
+  const size_t fixed = lsa_step_smem_bytes(0), per_char = lsa_step_smem_bytes(1) - fixed;
+  return (size_t)optin > fixed ? (int)(((size_t)optin - fixed) / per_char) : 0;
+}
+
+// raises the kernel's dynamic shared memory limit where the input needs more than the default 48 KB
+cudaError_t lsa_step_prepare(int Tc) {
+  const size_t smem = lsa_step_smem_bytes(Tc);
+  return smem > 48 * 1024 ? cudaFuncSetAttribute(lsa_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) : cudaSuccess;
+}
+
 // context = scores @ encoder_seq (tacotron.py:104 via lsa.py:40): ctx[b][f] = sum_t scores[b][t] seq[b][t][f].
 // grid (seq_dim / 256, B): 64 float4 feature lanes x 4 interleaved t-groups per CTA, partials reduced in smem.
 // The whole encoder sequence (B x Tc x 1024 fp32) is re-read every decoder step from L2: the kernel needs many
@@ -1026,6 +1049,8 @@ int mb_tacotron_finalize(mb_tacotron* h, void* stream) {
 
 size_t mb_tacotron_workspace_bytes(const mb_tacotron* h, int32_t B, int32_t Tc, int32_t steps, int32_t r) {
   if (!h || B <= 0 || Tc <= 0 || steps <= 0 || r <= 0) return 0;
+  const int max_chars = lsa_max_chars();  // 0: no device to ask; mb_tacotron_generate still refuses
+  if (max_chars > 0 && Tc > max_chars) return 0;
   const int nst = (steps + r - 1) / r;
   return ws_layout(h->cfg, B, Tc, nst * r, r).total * sizeof(float) + 256;
 }
@@ -1039,6 +1064,10 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
   if (!h->finalized) return fail(MB_ERR_STATE, "mb_tacotron_generate: weights not finalized");
   const mb_tacotron_config& c = h->cfg;
   if (B <= 0 || Tc <= 0 || steps <= 0 || r <= 0 || r > c.max_r) return fail(MB_ERR_INVALID, "mb_tacotron_generate: bad shape");
+  const int max_chars = lsa_max_chars();
+  if (Tc > max_chars)
+    return fail(MB_ERR_INVALID, "mb_tacotron_generate: %d characters exceed the limit of %d (the attention step's shared memory)",
+                Tc, max_chars);
   const int nst = (steps + r - 1) / r;
   const int steps_alloc = nst * r;  // the reference emits r frames per decoder step (tacotron.py:264-272)
   const Ws L = ws_layout(c, B, Tc, steps_alloc, r);
@@ -1144,8 +1173,8 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
   MB_CUDA_CHECK(cudaMemsetAsync(flags, 0, sizeof(int) * nst, st));
   uint8_t* dm = reinterpret_cast<uint8_t*>(ws + L.dmask);
   const size_t dmask_n = (size_t)B * 2 * D;
-  const size_t lsa_smem = sizeof(float) * (ATT_F * ATT_K + ATT_D * ATT_F + 2 * ATT_D + ATT_F + (Tc + 30) + Tc + 32 + (size_t)Tc * ATT_F + (size_t)Tc * 4);
-  if (lsa_smem > 48 * 1024) MB_CUDA_CHECK(cudaFuncSetAttribute(lsa_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsa_smem));
+  const size_t lsa_smem = lsa_step_smem_bytes(Tc);
+  MB_CUDA_CHECK(lsa_step_prepare(Tc));
   if (!dec_masks) {
     const size_t total = 2 * dmask_n * (size_t)nst;
     fill_masks_steps_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(dm, 2 * dmask_n, nst, seed);
@@ -1710,6 +1739,219 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
   }
   MB_CUDA_CHECK(cudaEventRecord(h->ev_out, st));
   MB_CUDA_CHECK(cudaStreamWaitEvent(caller, h->ev_out, 0));
+  return MB_OK;
+}
+
+int32_t mb_tacotron_max_chars(void) { return lsa_max_chars(); }
+
+}  // extern "C"
+
+// ---- mb_taco_debug: one FP32 kernel of this path per call, launched as the forward launches it ----------------------------
+namespace {
+
+GemmArgs debug_gemm_args(const mb_taco_debug_spec& s) {
+  GemmArgs a;
+  memset(&a, 0, sizeof(a));
+  a.nseg = s.nseg;
+  for (int j = 0; j < s.nseg && j < kMaxSeg; ++j) a.seg[j] = {s.x[j], s.K[j], s.ld[j], s.shift[j], s.w_off[j], s.w_stride[j]};
+  a.W = s.W;
+  a.ldw = s.ldw;
+  a.bias = s.bias;
+  a.M = s.M;
+  a.N = s.N;
+  a.T = s.T;
+  a.act = s.act;
+  a.bn_scale = s.bn_scale;
+  a.bn_shift = s.bn_shift;
+  a.mask = s.mask;
+  a.res = s.res;
+  a.ldres = s.ldres;
+  a.Y = s.y;
+  a.ldy = s.ldy;
+  a.step_mode = s.step_mode;
+  a.step_ptr = s.step_ptr;
+  a.step_j = s.step_j;
+  a.x_step = s.x_step;
+  a.x_first = s.x_first;
+  a.mask_step = s.mask_step;
+  return a;
+}
+
+int debug_check(const mb_taco_debug_spec& s) {
+  const char* me = "mb_taco_debug";
+  if (s.kind < MB_TACO_DBG_GEMM || s.kind > MB_TACO_DBG_BN_FOLD) return fail(MB_ERR_INVALID, "%s: bad kind %d", me, s.kind);
+  if (s.kind == MB_TACO_DBG_GEMM || s.kind == MB_TACO_DBG_STOP_STEP) {
+    if (s.nseg < 1 || s.nseg > kMaxSeg || !s.W || !s.y || s.M <= 0 || s.N <= 0)
+      return fail(MB_ERR_INVALID, "%s: GEMM nseg %d, M %d, N %d or a null operand", me, s.nseg, s.M, s.N);
+    for (int j = 0; j < s.nseg; ++j)
+      if (!s.x[j] || s.K[j] <= 0) return fail(MB_ERR_INVALID, "%s: segment %d empty", me, j);
+    if (s.kind == MB_TACO_DBG_STOP_STEP && (s.N != 1 || !s.out[0] || !s.out[1] || s.n[0] != s.M))
+      return fail(MB_ERR_INVALID, "%s: STOP_STEP needs N = 1, flags, ticket and B = M", me);
+    return MB_OK;
+  }
+  for (int i = 0; i < 10; ++i)
+    if (s.n[i] < 0) return fail(MB_ERR_INVALID, "%s: n[%d] = %lld", me, i, (long long)s.n[i]);
+  if (s.kind == MB_TACO_DBG_LSA_STEP) {
+    if (s.n[4] != 256 && s.n[4] != 512) return fail(MB_ERR_INVALID, "%s: LSA_STEP threads %lld", me, (long long)s.n[4]);
+    if (s.n[1] < 1 || s.n[1] > lsa_max_chars()) return fail(MB_ERR_INVALID, "%s: Tc = %lld outside [1, %d]", me, (long long)s.n[1], lsa_max_chars());
+  }
+  if (s.kind == MB_TACO_DBG_LSA_CTX && (s.n[2] <= 0 || s.n[2] % 256 || s.n[1] < 1))
+    return fail(MB_ERR_INVALID, "%s: LSA_CTX seq_dim %lld must be a positive multiple of 256", me, (long long)s.n[2]);
+  if (s.kind == MB_TACO_DBG_GST_ATTENTION && (s.n[1] < 1 || s.n[1] > 16 || s.n[3] < 1 || s.n[3] > 8 || s.n[2] % s.n[3]))
+    return fail(MB_ERR_INVALID, "%s: GST ntok %lld (<= 16), heads %lld (<= 8, dividing E)", me, (long long)s.n[1], (long long)s.n[3]);
+  return MB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t mb_taco_debug_workspace_bytes(const mb_taco_debug_spec* spec) {
+  return spec && debug_check(*spec) == MB_OK ? 256 : 0;
+}
+
+int mb_taco_debug(const mb_taco_debug_spec* spec, void* workspace, size_t workspace_bytes, void* stream, char* report,
+                  size_t report_len) {
+  if (!spec) return fail(MB_ERR_INVALID, "mb_taco_debug: null spec");
+  const mb_taco_debug_spec& s = *spec;
+  int rc = debug_check(s);
+  if (rc != MB_OK) return rc;
+  if (!workspace || workspace_bytes < 256) return fail(MB_ERR_WORKSPACE, "mb_taco_debug: workspace %zu < 256 bytes", workspace_bytes);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t* n = s.n;
+  auto fin = [&](int i) { return reinterpret_cast<const float*>(s.in[i]); };
+  auto fout = [&](int i) { return reinterpret_cast<float*>(s.out[i]); };
+  auto hout = [&](int i) { return reinterpret_cast<__half*>(s.out[i]); };
+  auto blocks = [](int64_t count) { return (unsigned)((count + 255) / 256); };
+  GemmLaunchInfo info{"", 0, 1, 256, 0};
+  switch (s.kind) {
+    case MB_TACO_DBG_GEMM:
+      TK(launch_gemm(debug_gemm_args(s), st, &info));
+      break;
+    case MB_TACO_DBG_PRENET: {
+      PrenetArgs pa;
+      memset(&pa, 0, sizeof(pa));
+      pa.x = fin(0);
+      pa.x_first = fin(1);
+      pa.W1 = fin(2);
+      pa.b1 = fin(3);
+      pa.W2 = fin(4);
+      pa.b2 = fin(5);
+      pa.m1 = reinterpret_cast<const uint8_t*>(s.in[6]);
+      pa.m2 = reinterpret_cast<const uint8_t*>(s.in[7]);
+      pa.y = fout(0);
+      pa.s_hi = hout(1);
+      pa.s_lo = hout(2);
+      pa.B = (int)n[0];
+      pa.K = (int)n[1];
+      pa.H = (int)n[2];
+      pa.ldy = (int)n[3];
+      pa.x_ld = n[4];
+      pa.x_step = n[5];
+      pa.mask_step = n[6];
+      pa.s_k0 = (int)n[7];
+      pa.s_rows_pad = (int)n[8];
+      pa.step_ptr = s.step_ptr;
+      pa.step_j = s.step_j;
+      TK(launch_prenet_fused(pa, st));
+      info = {"prenet_fused", (pa.B + 3) / 4, 1, 512, 0};
+      break;
+    }
+    case MB_TACO_DBG_GRU_CELL:
+      TK(launch_gru_cell(fin(0), (int)n[2], fin(1), fout(0), (int)n[3], fout(1), (int)n[4], (int)n[0], (int)n[1], st));
+      info = {"gru_cell", (int)blocks(n[0] * n[1]), 1, 256, 0};
+      break;
+    case MB_TACO_DBG_LSTM_CELL:
+      TK(launch_lstm_cell(fin(0), fout(0), fout(1), fout(2), (int)n[0], (int)n[1], st));
+      info = {"lstm_cell", (int)blocks(n[0] * n[1]), 1, 256, 0};
+      break;
+    case MB_TACO_DBG_HIGHWAY:
+      TK(launch_highway(fin(0), fout(0), (int)n[0], (int)n[1], st));
+      info = {"highway", (int)blocks(n[0] * n[1]), 1, 256, 0};
+      break;
+    case MB_TACO_DBG_MAXPOOL2:
+      TK(launch_maxpool2(fin(0), fout(0), (int)n[0], (int)n[1], (int)n[2], st));
+      info = {"maxpool2", (int)blocks(n[0] * n[1] * n[2]), 1, 256, 0};
+      break;
+    case MB_TACO_DBG_EMBEDDING:
+      TK(launch_embedding(reinterpret_cast<const int32_t*>(s.in[0]), fin(1), fout(0), (int)n[0], (int)n[1], st));
+      info = {"embedding", (int)blocks(n[0] * n[1]), 1, 256, 0};
+      break;
+    case MB_TACO_DBG_COPY_COLS:
+      TK(launch_copy_cols(fin(0), (int)n[2], (int)n[3], fout(0), (int)n[4], (int)n[5], (int)n[0], (int)n[1], st));
+      info = {"copy_cols", (int)blocks(n[0] * n[1]), 1, 256, 0};
+      break;
+    case MB_TACO_DBG_LSA_STEP: {
+      const int B = (int)n[0], Tc = (int)n[1], threads = (int)n[4];
+      const size_t smem = lsa_step_smem_bytes(Tc);
+      MB_CUDA_CHECK(lsa_step_prepare(Tc));
+      MB_CUDA_CHECK(launch_pdl2(lsa_step_kernel, dim3(B), dim3(threads), smem, st, fin(0), fin(1), fin(2), (int)n[2],
+                                reinterpret_cast<const int32_t*>(s.in[3]), fout(0), fin(4), fin(5), fin(6), fin(7), fout(1),
+                                (int)n[3], fout(2), Tc, s.step_ptr, s.step_j, fin(8), fin(9), fin(10)));
+      MB_LAUNCH_CHECK("lsa_step_kernel");
+      info = {"lsa_step", B, 1, threads, smem};
+      break;
+    }
+    case MB_TACO_DBG_LSA_CTX: {
+      const int B = (int)n[0], Tc = (int)n[1], seq_dim = (int)n[2];
+      const size_t smem = sizeof(float) * Tc;
+      MB_CUDA_CHECK(launch_pdl2(lsa_ctx_kernel, dim3(seq_dim / 256, B), dim3(256), smem, st, fin(0), (int)n[3], fin(1), seq_dim, Tc,
+                                fout(0), s.step_ptr, s.step_j, hout(1), hout(2), hout(3), hout(4), (int)n[4]));
+      MB_LAUNCH_CHECK("lsa_ctx_kernel");
+      info = {"lsa_ctx", seq_dim / 256, B, 256, smem};
+      break;
+    }
+    case MB_TACO_DBG_GST_ATTENTION: {
+      const int B = (int)n[0], E = (int)n[2], heads = (int)n[3];
+      gst_attention_kernel<<<B, 256, 0, st>>>(fin(0), fin(1), fin(2), (int)n[1], fout(0), E, heads, 1.0f / sqrtf((float)(E / heads)));
+      MB_LAUNCH_CHECK("gst_attention_kernel");
+      info = {"gst_attention", B, 1, 256, 0};
+      break;
+    }
+    case MB_TACO_DBG_STOP_STEP: {
+      const int B = (int)n[0];
+      stop_step_kernel<<<B, 256, 0, st>>>(debug_gemm_args(s), B, s.fval, (int)n[1], reinterpret_cast<int*>(s.out[0]), s.step_ptr,
+                                          s.step_j, reinterpret_cast<unsigned int*>(s.out[1]));
+      MB_LAUNCH_CHECK("stop_step_kernel");
+      info = {"stop_step", B, 1, 256, 0};
+      break;
+    }
+    case MB_TACO_DBG_STOP_FLAG:
+      stop_flag_kernel<<<1, 32, 0, st>>>(fin(0), (int)n[0], s.fval, (int)n[1], reinterpret_cast<int*>(s.out[0]), s.step_ptr, s.step_j);
+      MB_LAUNCH_CHECK("stop_flag_kernel");
+      info = {"stop_flag", 1, 1, 32, 0};
+      break;
+    case MB_TACO_DBG_FILL_MASKS:
+      fill_masks_kernel<<<blocks(n[0]), 256, 0, st>>>(reinterpret_cast<uint8_t*>(s.out[0]), (size_t)n[0], s.seed, (uint32_t)n[1],
+                                                       s.step_ptr);
+      MB_LAUNCH_CHECK("fill_masks_kernel");
+      info = {"fill_masks", (int)blocks(n[0]), 1, 256, 0};
+      break;
+    case MB_TACO_DBG_FILL_MASKS_STEPS:
+      fill_masks_steps_kernel<<<blocks(n[0] * n[1]), 256, 0, st>>>(reinterpret_cast<uint8_t*>(s.out[0]), (size_t)n[0], (int)n[1],
+                                                                    s.seed);
+      MB_LAUNCH_CHECK("fill_masks_steps_kernel");
+      info = {"fill_masks_steps", (int)blocks(n[0] * n[1]), 1, 256, 0};
+      break;
+    case MB_TACO_DBG_PACK_MELPROJ:
+      pack_melproj_kernel<<<blocks(n[2] * n[0] * n[3]), 256, 0, st>>>(fin(0), fout(0), (int)n[0], (int)n[1], (int)n[2], (int)n[3]);
+      MB_LAUNCH_CHECK("pack_melproj_kernel");
+      info = {"pack_melproj", (int)blocks(n[2] * n[0] * n[3]), 1, 256, 0};
+      break;
+    case MB_TACO_DBG_TO_NCL:
+      to_ncl_kernel<<<blocks(n[1] * n[2] * n[3]), 256, 0, st>>>(fin(0), (int)n[0], fout(0), (int)n[1], (int)n[2], (int)n[3]);
+      MB_LAUNCH_CHECK("to_ncl_kernel");
+      info = {"to_ncl", (int)blocks(n[1] * n[2] * n[3]), 1, 256, 0};
+      break;
+    case MB_TACO_DBG_BN_FOLD:
+      bn_fold_kernel<<<blocks(n[0]), 256, 0, st>>>(fin(0), fin(1), fin(2), fin(3), fout(0), fout(1), (int)n[0]);
+      MB_LAUNCH_CHECK("bn_fold_kernel");
+      info = {"bn_fold", (int)blocks(n[0]), 1, 256, 0};
+      break;
+  }
+  if (report && report_len)
+    snprintf(report, report_len, "kernel=%s grid=%d,%d block=%d smem=%zu\n", info.kernel, info.grid_x, info.grid_y, info.block,
+             info.smem);
   return MB_OK;
 }
 

@@ -338,7 +338,8 @@ __global__ void __launch_bounds__(256) rowdot_kernel(const GemmArgs a) {
   const int m = blockIdx.x, tid = threadIdx.x;
   float s = 0.f;
   for (int sgi = 0; sgi < a.nseg; ++sgi) {
-    const Seg sg = a.seg[sgi];
+    Seg sg = a.seg[sgi];
+    if (sgi == 0) step_seg0(a, sg);
     for (int k = tid; k < sg.K; k += 256) s = fmaf(sg.x[(size_t)m * sg.ld + k], a.W[sg.w_off + (size_t)k * sg.w_stride], s);
   }
   for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
@@ -517,11 +518,15 @@ cudaError_t launch_prenet_fused(const PrenetArgs& a, cudaStream_t st) {
   return cudaGetLastError();
 }
 
-cudaError_t launch_gemm(const GemmArgs& a, cudaStream_t st) {
+cudaError_t launch_gemm(const GemmArgs& a, cudaStream_t st, GemmLaunchInfo* info) {
   if (a.M <= 0 || a.N <= 0) return cudaSuccess;
   bool shifted = false;
   for (int s = 0; s < a.nseg; ++s) shifted = shifted || a.seg[s].shift != 0;
+  auto note = [&](const char* k, dim3 grid, size_t smem) {
+    if (info) *info = GemmLaunchInfo{k, (int)grid.x, (int)grid.y, 256, smem};
+  };
   if (a.N == 1 && !shifted && !a.mask && !a.res && !a.bn_scale) {
+    note("rowdot", dim3(a.M), 0);
     rowdot_kernel<<<a.M, 256, 0, st>>>(a);
     return cudaGetLastError();
   }
@@ -533,24 +538,29 @@ cudaError_t launch_gemm(const GemmArgs& a, cudaStream_t st) {
         cudaFuncSetAttribute(gemm_skinny_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         attr = true;
       }
+      note("gemm_skinny4", dim3((a.N + 31) / 32), smem);
       gemm_skinny_kernel<4><<<(a.N + 31) / 32, 256, smem, st>>>(a);
     } else {
       constexpr size_t smem = sizeof(float) * (8 * SKK * 68 + 8 * SKK * 8);
+      note("gemm_skinny1", dim3((a.N + 7) / 8), smem);
       gemm_skinny_kernel<1><<<(a.N + 7) / 8, 256, smem, st>>>(a);
     }
     return cudaGetLastError();
   }
   if (a.M >= 1024 && a.N >= 128) {
     dim3 grid((a.N + LBN - 1) / LBN, (a.M + LBM - 1) / LBM);
+    note("gemm_big", grid, 0);
     gemm_big_kernel<<<grid, 256, 0, st>>>(a);
     return cudaGetLastError();
   }
   // small-M (decoder step) problems: narrower N tiles -> more CTAs
   if (a.M <= 128 && a.N >= 512) {
     dim3 grid((a.N + 31) / 32, (a.M + BM - 1) / BM);
+    note("gemm32", grid, 0);
     gemm_kernel<32><<<grid, 256, 0, st>>>(a);
   } else {
     dim3 grid((a.N + 63) / 64, (a.M + BM - 1) / BM);
+    note("gemm64", grid, 0);
     gemm_kernel<64><<<grid, 256, 0, st>>>(a);
   }
   return cudaGetLastError();

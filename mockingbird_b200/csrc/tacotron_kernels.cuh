@@ -84,7 +84,13 @@ struct GemmArgs {
 
 __device__ __forceinline__ int step_index(const int* step_ptr, int step_j) { return (step_ptr ? *step_ptr : 0) + step_j; }
 
-cudaError_t launch_gemm(const GemmArgs& a, cudaStream_t st);
+// which kernel launch_gemm chose and its launch shape (filled when asked; mb_taco_debug reports it)
+struct GemmLaunchInfo {
+  const char* kernel;
+  int grid_x, grid_y, block;
+  size_t smem;
+};
+cudaError_t launch_gemm(const GemmArgs& a, cudaStream_t st, GemmLaunchInfo* info = nullptr);
 
 // Decoder PreNet (sublayer/pre_net.py:11-27) as ONE launch: y = drop2(relu(W2 drop1(relu(W1 x + b1)) + b2)), dropout p = 0.5 with
 // injected / device-drawn keep masks (x2).  The intermediate never leaves shared memory; replaces two skinny GEMM launches

@@ -151,6 +151,11 @@ class Tacotron:
         chars = x.to(device=dev, dtype=torch.int32).contiguous()
         spk = speaker_embedding.to(device=dev, dtype=torch.float32).contiguous()
         B, Tc = chars.shape
+        with torch.cuda.device(dev):
+            max_chars = int(L.mb_tacotron_max_chars())
+        if Tc > max_chars:
+            raise ValueError(f"{Tc} characters exceed the limit of {max_chars} per utterance on this GPU "
+                             "(the attention step keeps 4 * (5438 + 38 * chars) bytes in shared memory)")
         r = self._r
         nst = (steps + r - 1) // r
         M = nst * r
