@@ -435,6 +435,26 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
                          const uint8_t* dec_masks, uint64_t seed, float* mel, float* linear, float* attn,
                          int32_t* frames_out_host, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Many utterances as independent rows (Tacotron.generate_many): row b is computed as that utterance's own B = 1 generate.
+ *   chars int32 [B][Tc] (row b's first row_chars[b] entries are its text; the rest is never read as input), spk [B][256],
+ *   B <= 128.  Row b stops at its own stop rule (stop * 10 > min_stop_token and frame t > 10) or at its cap of
+ *   ceil(row_steps[b] / r) decoder steps; a finished row keeps computing until every row is done, and nothing it computes
+ *   after its stop reaches its outputs or another row.  Its frames, (done step + 1) * r, go to row_frames_host[b].
+ *   Outputs: mel, linear [B][80][F] and attn [B][F / r][Tc] with F = *frames_out_host = the largest row_frames_host[b];
+ *   row b's part is [:, :row_frames_host[b]] (attn [:row_frames_host[b] / r, :row_chars[b]]).  Buffers are sized for
+ *   F = ceil(max row_steps / r) * r.
+ *   Dropout: enc_masks [2][B][Tc][256] and dec_masks [ceil(max row_steps / r)][2][B][256] as for mb_tacotron_generate,
+ *   or, when null, drawn on the device with Philox keyed by row_seeds[b] and counted by (unit, character or step, layer):
+ *   an utterance draws the same masks whatever its row or its neighbours.
+ *   Every layer takes a route chosen from something other than the row count (DESIGN.md section 4b), so a row's outputs are
+ *   bitwise the same in any batch.  The call blocks the host like mb_tacotron_generate. */
+size_t mb_tacotron_ragged_workspace_bytes(const mb_tacotron* h, int32_t batch, int32_t n_chars, int32_t max_steps, int32_t r);
+int mb_tacotron_generate_ragged(mb_tacotron* h, const int32_t* chars, const float* spk, int32_t batch, int32_t n_chars,
+                                const int32_t* row_chars, const int32_t* row_steps, const uint64_t* row_seeds, int32_t r,
+                                int32_t style_idx, float min_stop_token, const uint8_t* enc_masks, const uint8_t* dec_masks,
+                                float* mel, float* linear, float* attn, int32_t* frames_out_host, int32_t* row_frames_host,
+                                void* workspace, size_t workspace_bytes, void* stream);
+
 /* test hook: ONE launch of a 3-term-split tensor-core GEMM of the Tacotron / speaker-encoder family on caller-provided fp32
  * device tensors (no model handle), through the functions the forward uses, in its order: tc_skinny_absmax -> tc_weight_scale ->
  * tc_skinny_pack / pack_big_w -> act_split / im2col_split -> launch_tc_{skinny,gru,lstm_seq,big}.  Tensors are row-major. */

@@ -290,6 +290,11 @@ SIGNATURES = {
     "mb_taco_tc_debug_workspace_bytes": (C.c_size_t, [C.POINTER(TacoTcDebugSpec)]),
     "mb_taco_tc_debug": (C.c_int, [C.POINTER(TacoTcDebugSpec), C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]),
     "mb_tacotron_max_chars": (C.c_int32, []),
+    "mb_tacotron_ragged_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "mb_tacotron_generate_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_void_p,
+                                              C.c_size_t, C.c_void_p]),
     "mb_taco_debug_workspace_bytes": (C.c_size_t, [C.POINTER(TacoDebugSpec)]),
     "mb_taco_debug": (C.c_int, [C.POINTER(TacoDebugSpec), C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]),
     "mb_encoder_create": (C.c_int, [C.POINTER(EncoderConfig), C.POINTER(C.c_void_p)]),

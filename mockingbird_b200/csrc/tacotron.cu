@@ -28,6 +28,10 @@ namespace {
 //   loc[f]  = conv1d(cumulative, k=31)[t]   (32 filters)
 //   u[t]    = v . tanh(pq + proj[b,t] + L loc) * (chars[b,t] != 0)
 //   scores  = softmax_t(u); cumulative += scores; ctx = scores @ seq[b]
+// Ragged rows (lens != nullptr): row b has lens[b] characters.  Positions >= lens[b] get the energy -inf, so their exp is
+// exactly 0: every max, sum and score of the row is bitwise what it would be with the loops cut at lens[b], i.e. what the row
+// computes alone, and their cumulative attention stays at its initial 0, which is what the location conv reads past the row's
+// end.  (Cutting the loops instead keeps the length live in a register and makes ptxas spill.)
 constexpr int ATT_D = 128, ATT_F = 32, ATT_K = 31;
 
 // launch with the programmatic-stream-serialization attribute (MB_TACO_PDL2=0: plain launch): the kernel may start while the
@@ -59,7 +63,8 @@ __global__ void __launch_bounds__(512) lsa_step_kernel(const float* __restrict__
                                                        const float* __restrict__ Lw, const float* __restrict__ vw,
                                                        float* __restrict__ scores_out, int scores_ld, float* ctx, int Tc,
                                                        const int* step_ptr, int step_j, const float* __restrict__ q_in,
-                                                       const float* __restrict__ Wq, const float* __restrict__ bq) {
+                                                       const float* __restrict__ Wq, const float* __restrict__ bq,
+                                                       const int* __restrict__ lens) {
   extern __shared__ float sm[];
   scores_out += (size_t)step_index(step_ptr, step_j) * Tc;  // this decoder step's row of the alignment matrix
   float* s_cw = sm;                         // [32][31]
@@ -148,9 +153,11 @@ __global__ void __launch_bounds__(512) lsa_step_kernel(const float* __restrict__
     }
   }
   __syncthreads();
+  const int len = lens ? lens[b] : Tc;
   for (int t = tid; t < Tc; t += blockDim.x) {
     const float u = (s_part[t * 4 + 0] + s_part[t * 4 + 1]) + (s_part[t * 4 + 2] + s_part[t * 4 + 3]);
-    s_u[t] = chars[(size_t)b * Tc + t] != 0 ? u : 0.f;  // u * (chars != 0): padded positions score exp(0)
+    // u * (chars != 0): padded positions of the row score exp(0); positions past a ragged row's end are out of it
+    s_u[t] = t >= len ? -INFINITY : chars[(size_t)b * Tc + t] != 0 ? u : 0.f;
   }
   __syncthreads();
   // softmax over t
@@ -215,24 +222,25 @@ cudaError_t lsa_step_prepare(int Tc) {
 // context = scores @ encoder_seq (tacotron.py:104 via lsa.py:40): ctx[b][f] = sum_t scores[b][t] seq[b][t][f].
 // grid (seq_dim / 256, B): 64 float4 feature lanes x 4 interleaved t-groups per CTA, partials reduced in smem.
 // The whole encoder sequence (B x Tc x 1024 fp32) is re-read every decoder step from L2: the kernel needs many
-// 16-byte loads in flight, which one CTA per batch row cannot provide.
+// 16-byte loads in flight, which one CTA per batch row cannot provide.  Ragged rows (lens): only t < lens[b] is read.
 __global__ void __launch_bounds__(256) lsa_ctx_kernel(const float* __restrict__ scores, int scores_ld, const float* __restrict__ seq,
                                                       int seq_dim, int Tc, float* __restrict__ ctx, const int* step_ptr,
                                                       int step_j, __half* sa_hi, __half* sa_lo, __half* sb_hi, __half* sb_lo,
-                                                      int s_rows_pad) {
+                                                      int s_rows_pad, const int* __restrict__ lens) {
   __shared__ float4 part[4][64];
   extern __shared__ float s_sc[];
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   const int b = blockIdx.y, f4 = blockIdx.x * 64 + (threadIdx.x & 63), tg = threadIdx.x >> 6;
   const float* sc = scores + (size_t)step_index(step_ptr, step_j) * Tc + (size_t)b * scores_ld;
-  for (int t = threadIdx.x; t < Tc; t += 256) s_sc[t] = sc[t];
+  const int Tb = lens ? lens[b] : Tc;
+  for (int t = threadIdx.x; t < Tb; t += 256) s_sc[t] = sc[t];
   __syncthreads();
   float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
   const float4* sp = reinterpret_cast<const float4*>(seq + (size_t)b * Tc * seq_dim) + f4;
   const int q4 = seq_dim >> 2;
 #pragma unroll 6
-  for (int t = tg; t < Tc; t += 4) {
+  for (int t = tg; t < Tb; t += 4) {
     const float4 v = sp[(size_t)t * q4];
     const float w = s_sc[t];
     a.x = fmaf(w, v.x, a.x);
@@ -334,21 +342,62 @@ __global__ void fill_masks_steps_kernel(uint8_t* m, size_t n_per_step, int n_ste
   m[g] = (uint8_t)((o[i & 3] >> 16) & 1u);
 }
 
+// PreNet dropout keep flags of ragged rows, keyed by each utterance's own seed: the Philox counter is (unit / 4, position, layer),
+// position = character (encoder) or decoder step, so an utterance draws the same flags whatever its row, batch or neighbours.
+//   encoder (dec == 0): m [2 layers][B][npos][units];  decoder (dec == 1): m [npos steps][2 layers][B][units]
+__global__ void fill_masks_seeded_kernel(uint8_t* m, int B, int npos, int units, const uint64_t* __restrict__ seeds, int dec) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)2 * B * npos * units) return;
+  const int u = (int)(i % units);
+  size_t q = i / units;
+  int b, l, pos;
+  if (dec) {
+    b = (int)(q % B);
+    q /= B;
+    l = (int)(q & 1);
+    pos = (int)(q >> 1);
+  } else {
+    pos = (int)(q % npos);
+    q /= npos;
+    b = (int)(q % B);
+    l = (int)(q / B);
+  }
+  const uint64_t seed = seeds[b];
+  uint32_t o[4];
+  mb_philox4x32((uint32_t)u >> 2, (uint32_t)pos, (uint32_t)(2 * dec + l), 0x72616767u, (uint32_t)seed, (uint32_t)(seed >> 32), o);
+  m[i] = (uint8_t)((o[u & 3] >> 16) & 1u);
+}
+
+// stop rule of tacotron.py:275 at decoder step si (frame t = si * r) over the B stop values stopv[b * ld].  Padded batch
+// (row_done == nullptr): flags[si] = every row passes and t > 10.  Ragged rows: row b ends at the first step where it passes with
+// t > 10 or reaches its cap of row_caps[b] steps (row_done[b] = that step, -1 before); flags[si] = every row has ended.
+__device__ void apply_stop_rule(const float* stopv, int ld, int B, float min_stop_token, int r, int si, int* flags, int* row_done,
+                                const int* row_caps) {
+  bool all = true;
+  for (int b = 0; b < B; ++b) {
+    const bool pass = __ldcg(stopv + (size_t)b * ld) * 10.f > min_stop_token;
+    if (row_done) {
+      if (row_done[b] < 0 && ((pass && si * r > 10) || si + 1 >= row_caps[b])) row_done[b] = si;
+      all = all && row_done[b] >= 0;
+    } else {
+      all = all && pass;
+    }
+  }
+  flags[si] = row_done ? (all ? 1 : 0) : ((all && si * r > 10) ? 1 : 0);
+}
+
 // decoder step si = (step_ptr ? *step_ptr : 0) + step_j; frame t = si * r; flags[si] = stop rule of tacotron.py:275
 __global__ void stop_flag_kernel(const float* stopv, int B, float min_stop_token, int r, int* flags, const int* step_ptr,
-                                 int step_j) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) {
-    const int si = step_index(step_ptr, step_j);
-    bool all = true;
-    for (int b = 0; b < B; ++b) all = all && (stopv[b] * 10.f > min_stop_token);
-    flags[si] = (all && si * r > 10) ? 1 : 0;
-  }
+                                 int step_j, int* row_done = nullptr, const int* row_caps = nullptr) {
+  if (threadIdx.x == 0 && blockIdx.x == 0)
+    apply_stop_rule(stopv, 1, B, min_stop_token, r, step_index(step_ptr, step_j), flags, row_done, row_caps);
 }
 
 // stop projection (sigmoid(w . [x | ctx] + b), tacotron.py:131-133) of one batch row per CTA, then - in the CTA that takes the
 // last ticket - the stop rule over all rows.  Same summation order as rowdot_kernel.
 __global__ void __launch_bounds__(256) stop_step_kernel(const GemmArgs a, int B, float min_stop_token, int r, int* flags,
-                                                        const int* step_ptr, int step_j, unsigned int* ticket) {
+                                                        const int* step_ptr, int step_j, unsigned int* ticket,
+                                                        int* row_done = nullptr, const int* row_caps = nullptr) {
   __shared__ float red[8];
   __shared__ bool last;
   const int m = blockIdx.x, tid = threadIdx.x;
@@ -372,10 +421,7 @@ __global__ void __launch_bounds__(256) stop_step_kernel(const GemmArgs a, int B,
   if (last && tid == 0) {
     *ticket = 0u;
     __threadfence();
-    const int si = step_index(step_ptr, step_j);
-    bool all = true;
-    for (int b = 0; b < B; ++b) all = all && (__ldcg(a.Y + (size_t)b * a.ldy) * 10.f > min_stop_token);
-    flags[si] = (all && si * r > 10) ? 1 : 0;
+    apply_stop_rule(a.Y, a.ldy, B, min_stop_token, r, step_index(step_ptr, step_j), flags, row_done, row_caps);
   }
 }
 
@@ -609,18 +655,20 @@ struct BigWs {
 };
 
 // A large-M GEMM / conv of the CBHG stacks: tensor cores (tc_big_kernel, 3-term fp16 split) when the layer qualifies,
-// else the FP32 FFMA kernels.  MB_TACO_CONV_TC=0 disables the tensor-core route.
-int cbhg_gemm(mb_tacotron* h, const std::string& key, const GemmArgs& a, cudaStream_t st, const BigWs& bw) {
+// else the FP32 FFMA kernels.  MB_TACO_CONV_TC=0 disables the tensor-core route.  Ragged batches (lens = valid length of each
+// length-T sequence) always take the tensor-core route, whatever M, so a row's arithmetic does not depend on the batch.
+int cbhg_gemm(mb_tacotron* h, const std::string& key, const GemmArgs& a, cudaStream_t st, const BigWs& bw, const int* lens = nullptr) {
   static const bool env = [] {
     const char* e = getenv("MB_TACO_CONV_TC");
     return e ? atoi(e) != 0 : true;
   }();
-  bool ok = env && bw.hi && a.M >= 512 && a.N % 4 == 0 && a.nseg >= 1 && a.nseg <= kMaxSeg && !a.mask && !a.step_mode &&
+  bool ok = (env || lens) && bw.hi && (a.M >= 512 || lens) && a.N % 4 == 0 && a.nseg >= 1 && a.nseg <= kMaxSeg && !a.mask && !a.step_mode &&
             a.act != ACT_SIGMOID && a.act != ACT_TANH && h->w.has(key + ".bigw") && (a.ldy % 4) == 0 &&
             (!a.res || (a.ldres % 4) == 0);
   const int K = a.seg[0].K;
   for (int s = 1; ok && s < a.nseg; ++s) ok = a.seg[s].K == K;
   if (ok) ok = tc_big_act_bytes(a.M, a.nseg, K) <= bw.bytes && tc_big_weight_bytes(a.N, a.nseg, K) / 4 <= h->w.size(key + ".bigw");
+  if (!ok && lens) return fail(MB_ERR_STATE, "%s: no tensor-core route for this layer of a ragged batch", key.c_str());
   if (!ok) {
     TK(launch_gemm(a, st));
     return MB_OK;
@@ -664,6 +712,7 @@ int cbhg_gemm(mb_tacotron* h, const std::string& key, const GemmArgs& a, cudaStr
   q.M = a.M;
   q.T = a.T > 0 ? a.T : 1;
   q.rows_total = (a.M + 127) / 128 * 128;
+  q.len = lens;
   TK(launch_im2col_split(q, reinterpret_cast<__half*>(bw.hi), reinterpret_cast<__half*>(bw.lo), st));
   TcBigArgs t;
   memset(&t, 0, sizeof(t));
@@ -687,16 +736,18 @@ int cbhg_gemm(mb_tacotron* h, const std::string& key, const GemmArgs& a, cudaStr
   return MB_OK;
 }
 
-// CBHG (sublayer/cbhg.py:42-79) on x [B*T][cin] channels-last -> out [B*T][ch] written at out (ld ldout)
+// CBHG (sublayer/cbhg.py:42-79) on x [B*T][cin] channels-last -> out [B*T][ch] written at out (ld ldout).  Ragged batches
+// (lens: sequence b is its first lens[b] of T rows) run every layer on the tensor cores; the convolutions read zeros past a
+// sequence's end and the backward GRU starts at its last row from h = 0, so rows past the end never reach rows before it.
 int run_cbhg(mb_tacotron* h, const std::string& p, int K, int cin, int ch, int p0, int p1, int nh, const float* x, int B,
              int T, float* bank, float* pool, float* pj1, float* y, float* hw12, float* gi_f, float* gi_b, float* gh,
              float* hst, float* out, int ldout, cudaStream_t st, float* tc_hi = nullptr, float* tc_lo = nullptr,
-             size_t tc_bytes = 0, const BigWs& bw = BigWs()) {
+             size_t tc_bytes = 0, const BigWs& bw = BigWs(), const int* lens = nullptr) {
   const int M = B * T;
-#define CG(key, args)                                 \
-  do {                                                \
-    int _rc = cbhg_gemm(h, (key), (args), st, bw);    \
-    if (_rc != MB_OK) return _rc;                     \
+#define CG(key, args)                                    \
+  do {                                                   \
+    int _rc = cbhg_gemm(h, (key), (args), st, bw, lens); \
+    if (_rc != MB_OK) return _rc;                        \
   } while (0)
   // convolution bank: k = 1..K, "same" padding k//2 cropped to T, ReLU then BatchNorm
   for (int i = 0; i < K; ++i) {
@@ -798,6 +849,7 @@ int run_cbhg(mb_tacotron* h, const std::string& p, int K, int cin, int ch, int p
     g.M = B;
     g.H = H;
     g.ndir = 2;
+    g.len1 = lens;
     const char* sfx[2] = {"", "_reverse"};
     for (int d = 0; d < 2; ++d) {
       g.w[d] = reinterpret_cast<const __half*>(P(h, p + ".rnn.hh" + sfx[d] + ".tcw"));
@@ -817,10 +869,12 @@ int run_cbhg(mb_tacotron* h, const std::string& p, int K, int cin, int ch, int p
       g.gi[1] = gi_b + (size_t)t_b * 3 * H;
       g.out[0] = out + (size_t)s * ldout;
       g.out[1] = out + (size_t)t_b * ldout + H;
+      g.t1 = t_b;
       TK(launch_tc_gru(g, st));
     }
     return MB_OK;
   }
+  if (lens) return fail(MB_ERR_STATE, "%s: no tensor-core GRU route for a ragged batch", p.c_str());
   MB_CUDA_CHECK(cudaMemsetAsync(hst, 0, sizeof(float) * 2 * B * H, st));
   float* hf = hst;
   float* hb = hst + (size_t)B * H;
@@ -1055,10 +1109,26 @@ size_t mb_tacotron_workspace_bytes(const mb_tacotron* h, int32_t B, int32_t Tc, 
   return ws_layout(h->cfg, B, Tc, nst * r, r).total * sizeof(float) + 256;
 }
 
-int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk, int32_t B, int32_t Tc, int32_t steps,
-                         int32_t r, int32_t style_idx, float min_stop_token, const uint8_t* enc_masks,
-                         const uint8_t* dec_masks, uint64_t seed, float* mel_out, float* linear_out, float* attn_out,
-                         int32_t* frames_out_host, void* workspace, size_t workspace_bytes, void* stream) {
+}  // extern "C"
+
+namespace {
+
+// per-row description of a ragged batch (mb_tacotron_generate_ragged), host arrays of B entries
+struct RaggedRows {
+  const int32_t* chars;   // characters of each row (<= Tc)
+  const int32_t* steps;   // frame cap of each row: ceil(steps / r) decoder steps
+  const uint64_t* seeds;  // dropout seed of each utterance
+  int32_t* frames;        // out: frames of each row
+};
+
+// device int32 entries behind the ws_layout of a ragged batch: chars, caps (decoder steps), done step, frames [B] each, seeds [B] u64
+size_t ragged_ws_floats(int B) { return align_up((size_t)6 * B, 64); }
+
+// Tacotron.generate of one padded batch (rg == nullptr) or of B ragged rows, each computed as that utterance alone (rg)
+int generate_impl(mb_tacotron* h, const int32_t* chars, const float* spk, int32_t B, int32_t Tc, int32_t steps,
+                  int32_t r, int32_t style_idx, float min_stop_token, const uint8_t* enc_masks,
+                  const uint8_t* dec_masks, uint64_t seed, float* mel_out, float* linear_out, float* attn_out,
+                  int32_t* frames_out_host, void* workspace, size_t workspace_bytes, void* stream, const RaggedRows* rg) {
   if (!h || !chars || !spk || !mel_out || !linear_out || !frames_out_host || !workspace)
     return fail(MB_ERR_INVALID, "mb_tacotron_generate: null argument");
   if (!h->finalized) return fail(MB_ERR_STATE, "mb_tacotron_generate: weights not finalized");
@@ -1071,7 +1141,8 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
   const int nst = (steps + r - 1) / r;
   const int steps_alloc = nst * r;  // the reference emits r frames per decoder step (tacotron.py:264-272)
   const Ws L = ws_layout(c, B, Tc, steps_alloc, r);
-  if (workspace_bytes < L.total * sizeof(float) + 256) return fail(MB_ERR_WORKSPACE, "mb_tacotron_generate: workspace too small");
+  const size_t need = (L.total + (rg ? ragged_ws_floats(B) : 0)) * sizeof(float) + 256;
+  if (workspace_bytes < need) return fail(MB_ERR_WORKSPACE, "mb_tacotron_generate: workspace too small");
   float* ws = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
   cudaStream_t caller = (cudaStream_t)stream;
   if (!h->own_stream) {
@@ -1090,13 +1161,36 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
     const char* e = getenv("MB_TACO_TC");
     return e ? atoi(e) != 0 : true;
   }();
-  const bool use_tc = tc_env && B <= 128 && LD % 64 == 0;
+  // a ragged batch always takes the tensor-core routes: their arithmetic per row does not depend on the row count
+  const bool use_tc = (tc_env || rg) && B <= 128 && LD % 64 == 0;
+  if (rg && !use_tc) return fail(MB_ERR_INVALID, "mb_tacotron_generate_ragged: more than 128 rows or lstm_dims %% 64 != 0");
   BigWs bw;
   bw.hi = ws + L.big_hi;
   bw.lo = ws + L.big_lo;
   bw.bytes = L.big_bytes;
   const int SE = c.speaker_embedding_size, proj_dims = E + SE + c.gst_E;
   const int Me = B * Tc;
+  int* d_lens = nullptr;   // ragged rows: characters, caps, done steps, frames, seeds (device copies)
+  int* d_caps = nullptr;
+  int* d_done = nullptr;
+  int* d_flen = nullptr;
+  const uint64_t* d_seeds = nullptr;
+  if (rg) {
+    int32_t* base = reinterpret_cast<int32_t*>(ws + L.total);
+    std::vector<int32_t> hv((size_t)6 * B, 0);
+    for (int b = 0; b < B; ++b) {
+      hv[b] = rg->chars[b];
+      hv[B + b] = (rg->steps[b] + r - 1) / r;
+      hv[2 * B + b] = -1;
+    }
+    memcpy(hv.data() + 4 * B, rg->seeds, sizeof(uint64_t) * B);
+    MB_CUDA_CHECK(cudaMemcpyAsync(base, hv.data(), sizeof(int32_t) * hv.size(), cudaMemcpyHostToDevice, st));
+    d_lens = base;
+    d_caps = base + B;
+    d_done = base + 2 * B;
+    d_flen = base + 3 * B;
+    d_seeds = reinterpret_cast<const uint64_t*>(base + 4 * B);
+  }
 
   if (h->packed_r != r) {
     const size_t n = (size_t)r * NM * LD;
@@ -1114,6 +1208,9 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
   const size_t enc_mask_n = (size_t)Me * E;
   if (enc_masks) {
     MB_CUDA_CHECK(cudaMemcpyAsync(em, enc_masks, 2 * enc_mask_n, cudaMemcpyDeviceToDevice, st));
+  } else if (rg) {
+    fill_masks_seeded_kernel<<<(unsigned)((2 * enc_mask_n + 255) / 256), 256, 0, st>>>(em, B, Tc, E, d_seeds, 0);
+    MB_LAUNCH_CHECK("fill_masks_seeded_kernel");
   } else {
     fill_masks_kernel<<<(unsigned)((2 * enc_mask_n + 255) / 256), 256, 0, st>>>(em, 2 * enc_mask_n, seed, 0xffffffffu);
     MB_LAUNCH_CHECK("fill_masks_kernel");
@@ -1122,16 +1219,19 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
     GemmArgs a = gemm1(ws + L.emb, c.embed_dims, c.embed_dims, P(h, "encoder.pre_net.fc1.weight"), c.embed_dims,
                        P(h, "encoder.pre_net.fc1.bias"), Me, E, ws + L.p1, E, ACT_RELU);
     a.mask = em;
+    a.fma_chain = rg != nullptr;
     TK(launch_gemm(a, st));
     GemmArgs b = gemm1(ws + L.p1, E, E, P(h, "encoder.pre_net.fc2.weight"), E, P(h, "encoder.pre_net.fc2.bias"), Me, E,
                        ws + L.x0, E, ACT_RELU);
     b.mask = em + enc_mask_n;
+    b.fma_chain = rg != nullptr;
     TK(launch_gemm(b, st));
   }
   float* seq = ws + L.seq;
   int rc = run_cbhg(h, "encoder.cbhg", c.encoder_K, E, E, E, E, c.num_highways, ws + L.x0, B, Tc, ws + L.bank, ws + L.pool,
                     ws + L.pj1, ws + L.y, ws + L.hw12, ws + L.gi_f, ws + L.gi_b, ws + L.gh, ws + L.hst, seq, proj_dims, st,
-                    use_tc ? ws + L.a_hi : nullptr, use_tc ? ws + L.a_lo : nullptr, tc_skinny_act_bytes(B > 128 ? 128 : B, 2 * LD), bw);
+                    use_tc ? ws + L.a_hi : nullptr, use_tc ? ws + L.a_lo : nullptr, tc_skinny_act_bytes(B > 128 ? 128 : B, 2 * LD), bw,
+                    d_lens);
   if (rc != MB_OK) return rc;
   // speaker embedding per char (tacotron.py:236), style embedding (tacotron.py:238-253)
   TK(launch_copy_cols(spk, SE, Tc, seq, proj_dims, E, Me, SE, st));
@@ -1151,6 +1251,7 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
     a.T = 1;
     a.Y = ws + L.style_q;
     a.ldy = c.gst_E;
+    a.fma_chain = rg != nullptr;
     TK(launch_gemm(a, st));
     const int dk = c.gst_E / c.gst_heads;
     gst_attention_kernel<<<B, 256, 0, st>>>(ws + L.style_q, P(h, "gst.keys"), P(h, "gst.values"), c.gst_tokens,
@@ -1160,6 +1261,7 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
   }
   {
     GemmArgs a = gemm1(seq, proj_dims, proj_dims, P(h, "encoder_proj.weight"), proj_dims, nullptr, Me, D, ws + L.proj, D);
+    a.fma_chain = rg != nullptr;
     TK(launch_gemm(a, st));
   }
 
@@ -1175,7 +1277,10 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
   const size_t dmask_n = (size_t)B * 2 * D;
   const size_t lsa_smem = lsa_step_smem_bytes(Tc);
   MB_CUDA_CHECK(lsa_step_prepare(Tc));
-  if (!dec_masks) {
+  if (!dec_masks && rg) {
+    fill_masks_seeded_kernel<<<(unsigned)((2 * dmask_n * (size_t)nst + 255) / 256), 256, 0, st>>>(dm, B, nst, 2 * D, d_seeds, 1);
+    MB_LAUNCH_CHECK("fill_masks_seeded_kernel");
+  } else if (!dec_masks) {
     const size_t total = 2 * dmask_n * (size_t)nst;
     fill_masks_steps_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(dm, 2 * dmask_n, nst, seed);
     MB_LAUNCH_CHECK("fill_masks_steps_kernel");
@@ -1400,7 +1505,7 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
                                 P(h, "decoder.attn_net.conv.bias"), P(h, "decoder.attn_net.L.weight"),
                                 P(h, "decoder.attn_net.v.weight"), ws + L.scores_all, nst * Tc,
                                 (proj_dims % 256 == 0) ? nullptr : ws + L.ctx, Tc, sp, sj, qf ? ws + L.attn_h : nullptr,
-                                P(h, "decoder.attn_net.W.weight"), P(h, "decoder.attn_net.W.bias")));
+                                P(h, "decoder.attn_net.W.weight"), P(h, "decoder.attn_net.W.bias"), d_lens));
       MB_LAUNCH_CHECK("lsa_step_kernel");
       if (proj_dims % 256 == 0) {
         if (have_stop) {  // the previous step's stop projection (side stream) still reads ctx and x, which are rewritten from here on
@@ -1410,7 +1515,7 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
         MB_CUDA_CHECK(launch_pdl2(lsa_ctx_kernel, dim3(proj_dims / 256, B), dim3(256), sizeof(float) * Tc, st, ws + L.scores_all,
                                   nst * Tc, seq, proj_dims, Tc, ws + L.ctx, sp, sj, fsplit ? fhi(fs.p1) : nullptr,
                                   fsplit ? fhi(fs.p1 + fs.b1) : nullptr, fsplit ? fhi(fs.p2) : nullptr,
-                                  fsplit ? fhi(fs.p2 + fs.b2) : nullptr, f_rows_pad));
+                                  fsplit ? fhi(fs.p2 + fs.b2) : nullptr, f_rows_pad, d_lens));
         MB_LAUNCH_CHECK("lsa_ctx_kernel");
       }
       if (dag) {  // side stream: context half of the NEXT step's attention-GRU input projection
@@ -1620,7 +1725,7 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
         // the CTA that finishes last applies the stop rule (ticket counter behind the step counter, reset by that CTA).
         // With the step DAG it runs on the side stream (after the second LSTM's fork): the next step does not need it.
         stop_step_kernel<<<B, 256, 0, dag ? sd : st>>>(s, B, min_stop_token, r, flags, sp, sj,
-                                                       reinterpret_cast<unsigned int*>(ws + L.step) + 16);
+                                                       reinterpret_cast<unsigned int*>(ws + L.step) + 16, d_done, d_caps);
         MB_LAUNCH_CHECK("stop_step_kernel");
         if (dag) {
           MB_CUDA_CHECK(cudaEventRecord(h->ev_side[6], sd));
@@ -1628,7 +1733,7 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
         }
       } else {
         TK(launch_gemm(s, st));
-        stop_flag_kernel<<<1, 32, 0, st>>>(ws + L.stopv, B, min_stop_token, r, flags, sp, sj);
+        stop_flag_kernel<<<1, 32, 0, st>>>(ws + L.stopv, B, min_stop_token, r, flags, sp, sj, d_done, d_caps);
         MB_LAUNCH_CHECK("stop_flag_kernel");
       }
     }
@@ -1699,9 +1804,21 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
       if (rc2 != MB_OK) return rc2;
     }
   }
-  const int nsteps_done = (done_step >= 0 ? done_step : nst - 1) + 1;
-  int frames = nsteps_done * r;
-  if (frames > steps_alloc) frames = steps_alloc;
+  int frames = 0;
+  if (rg) {  // a ragged row ends at its own done step; the postnet runs over the longest row, each row over its own frames
+    std::vector<int32_t> hdone(B), hflen(B);
+    MB_CUDA_CHECK(cudaMemcpyAsync(hdone.data(), d_done, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int b = 0; b < B; ++b) {
+      hflen[b] = ((hdone[b] >= 0 ? hdone[b] : nst - 1) + 1) * r;
+      rg->frames[b] = hflen[b];
+      if (hflen[b] > frames) frames = hflen[b];
+    }
+    MB_CUDA_CHECK(cudaMemcpyAsync(d_flen, hflen.data(), sizeof(int32_t) * B, cudaMemcpyHostToDevice, st));
+  } else {
+    frames = ((done_step >= 0 ? done_step : nst - 1) + 1) * r;
+  }
+  const int nsteps_done = frames / r;
   *frames_out_host = frames;
 
   // ------------------------------------------------------------------ postnet (tacotron.py:281-283)
@@ -1718,11 +1835,12 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
   }
   rc = run_cbhg(h, "postnet", c.postnet_K, NM, PD, PD, NM, c.num_highways, melc, B, frames, ws + L.pbank, ws + L.ppool,
                 ws + L.ppj1, ws + L.py, ws + L.phw12, ws + L.pgi_f, ws + L.pgi_b, ws + L.pgh, ws + L.phst, ws + L.pout, PD, st,
-                use_tc ? ws + L.a_hi : nullptr, use_tc ? ws + L.a_lo : nullptr, tc_skinny_act_bytes(B > 128 ? 128 : B, 2 * LD), bw);
+                use_tc ? ws + L.a_hi : nullptr, use_tc ? ws + L.a_lo : nullptr, tc_skinny_act_bytes(B > 128 ? 128 : B, 2 * LD), bw,
+                d_flen);
   if (rc != MB_OK) return rc;
   {
     GemmArgs a = gemm1(ws + L.pout, PD, PD, P(h, "post_proj.weight"), PD, nullptr, B * frames, NM, ws + L.lin, NM);
-    int rc2 = cbhg_gemm(h, "post_proj", a, st, bw);
+    int rc2 = cbhg_gemm(h, "post_proj", a, st, bw, d_flen);
     if (rc2 != MB_OK) return rc2;
   }
   // outputs in the reference's layouts: mel [B][80][frames], linear [B][80][frames], attn [B][nsteps][Tc]
@@ -1740,6 +1858,44 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
   MB_CUDA_CHECK(cudaEventRecord(h->ev_out, st));
   MB_CUDA_CHECK(cudaStreamWaitEvent(caller, h->ev_out, 0));
   return MB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk, int32_t B, int32_t Tc, int32_t steps,
+                         int32_t r, int32_t style_idx, float min_stop_token, const uint8_t* enc_masks,
+                         const uint8_t* dec_masks, uint64_t seed, float* mel_out, float* linear_out, float* attn_out,
+                         int32_t* frames_out_host, void* workspace, size_t workspace_bytes, void* stream) {
+  return generate_impl(h, chars, spk, B, Tc, steps, r, style_idx, min_stop_token, enc_masks, dec_masks, seed, mel_out, linear_out,
+                       attn_out, frames_out_host, workspace, workspace_bytes, stream, nullptr);
+}
+
+size_t mb_tacotron_ragged_workspace_bytes(const mb_tacotron* h, int32_t B, int32_t Tc, int32_t steps, int32_t r) {
+  if (B > 128) return 0;
+  const size_t base = mb_tacotron_workspace_bytes(h, B, Tc, steps, r);
+  return base ? base + ragged_ws_floats(B) * sizeof(float) : 0;
+}
+
+int mb_tacotron_generate_ragged(mb_tacotron* h, const int32_t* chars, const float* spk, int32_t B, int32_t Tc,
+                                const int32_t* row_chars, const int32_t* row_steps, const uint64_t* row_seeds, int32_t r,
+                                int32_t style_idx, float min_stop_token, const uint8_t* enc_masks, const uint8_t* dec_masks,
+                                float* mel_out, float* linear_out, float* attn_out, int32_t* frames_out_host,
+                                int32_t* row_frames_host, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* me = "mb_tacotron_generate_ragged";
+  if (!h || !row_chars || !row_steps || !row_seeds || !row_frames_host) return fail(MB_ERR_INVALID, "%s: null argument", me);
+  if (B <= 0 || B > 128 || Tc <= 0) return fail(MB_ERR_INVALID, "%s: %d rows of %d characters (1 to 128 rows)", me, B, Tc);
+  int steps = 0;
+  for (int b = 0; b < B; ++b) {
+    if (row_chars[b] < 1 || row_chars[b] > Tc)
+      return fail(MB_ERR_INVALID, "%s: row %d has %d characters, outside [1, %d]", me, b, row_chars[b], Tc);
+    if (row_steps[b] < 1) return fail(MB_ERR_INVALID, "%s: row %d has a frame cap of %d", me, b, row_steps[b]);
+    if (row_steps[b] > steps) steps = row_steps[b];
+  }
+  RaggedRows rg{row_chars, row_steps, row_seeds, row_frames_host};
+  return generate_impl(h, chars, spk, B, Tc, steps, r, style_idx, min_stop_token, enc_masks, dec_masks, 0, mel_out, linear_out,
+                       attn_out, frames_out_host, workspace, workspace_bytes, stream, &rg);
 }
 
 int32_t mb_tacotron_max_chars(void) { return lsa_max_chars(); }
@@ -1887,7 +2043,7 @@ int mb_taco_debug(const mb_taco_debug_spec* spec, void* workspace, size_t worksp
       MB_CUDA_CHECK(lsa_step_prepare(Tc));
       MB_CUDA_CHECK(launch_pdl2(lsa_step_kernel, dim3(B), dim3(threads), smem, st, fin(0), fin(1), fin(2), (int)n[2],
                                 reinterpret_cast<const int32_t*>(s.in[3]), fout(0), fin(4), fin(5), fin(6), fin(7), fout(1),
-                                (int)n[3], fout(2), Tc, s.step_ptr, s.step_j, fin(8), fin(9), fin(10)));
+                                (int)n[3], fout(2), Tc, s.step_ptr, s.step_j, fin(8), fin(9), fin(10), nullptr));
       MB_LAUNCH_CHECK("lsa_step_kernel");
       info = {"lsa_step", B, 1, threads, smem};
       break;
@@ -1896,7 +2052,7 @@ int mb_taco_debug(const mb_taco_debug_spec* spec, void* workspace, size_t worksp
       const int B = (int)n[0], Tc = (int)n[1], seq_dim = (int)n[2];
       const size_t smem = sizeof(float) * Tc;
       MB_CUDA_CHECK(launch_pdl2(lsa_ctx_kernel, dim3(seq_dim / 256, B), dim3(256), smem, st, fin(0), (int)n[3], fin(1), seq_dim, Tc,
-                                fout(0), s.step_ptr, s.step_j, hout(1), hout(2), hout(3), hout(4), (int)n[4]));
+                                fout(0), s.step_ptr, s.step_j, hout(1), hout(2), hout(3), hout(4), (int)n[4], nullptr));
       MB_LAUNCH_CHECK("lsa_ctx_kernel");
       info = {"lsa_ctx", seq_dim / 256, B, 256, smem};
       break;

@@ -525,12 +525,12 @@ cudaError_t launch_gemm(const GemmArgs& a, cudaStream_t st, GemmLaunchInfo* info
   auto note = [&](const char* k, dim3 grid, size_t smem) {
     if (info) *info = GemmLaunchInfo{k, (int)grid.x, (int)grid.y, 256, smem};
   };
-  if (a.N == 1 && !shifted && !a.mask && !a.res && !a.bn_scale) {
+  if (a.N == 1 && !shifted && !a.mask && !a.res && !a.bn_scale && !a.fma_chain) {
     note("rowdot", dim3(a.M), 0);
     rowdot_kernel<<<a.M, 256, 0, st>>>(a);
     return cudaGetLastError();
   }
-  if (a.M <= 64 && !shifted) {
+  if (a.M <= 64 && !shifted && !a.fma_chain) {
     if (a.N >= 2048) {
       constexpr size_t smem = sizeof(float) * (8 * SKK * 68 + 8 * SKK * 32);
       static bool attr = false;

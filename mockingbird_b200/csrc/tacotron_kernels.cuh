@@ -80,6 +80,9 @@ struct GemmArgs {
   long long x_step;
   const float* x_first;
   long long mask_step;
+  // nonzero: only the tiled kernels (gemm32 / gemm64 / gemm_big), in which every output is one fmaf chain over k in segment
+  // order from 0 - the same bits whichever of them M selects, so a row's result does not depend on how many rows share the launch
+  int fma_chain;
 };
 
 __device__ __forceinline__ int step_index(const int* step_ptr, int step_j) { return (step_ptr ? *step_ptr : 0) + step_j; }
@@ -180,6 +183,8 @@ struct TcGruArgs {
   __half* s_hi;           // optional (direction 0): h_t also into columns [s_k0, s_k0 + H) of another GEMM's operand tiles
   __half* s_lo;
   int s_k0;
+  const int* len1;        // optional: valid length of row m's sequence; direction 1 (at time t1) keeps h = 0 while t1 >= len1[m],
+  int t1;                 //   so a ragged row's backward recurrence starts at its own last step from h = 0
 };
 cudaError_t launch_tc_gru(const TcGruArgs& a, cudaStream_t st);
 // ---- large-M tensor-core GEMM / conv over time (CBHG stacks), 128 x 128 output tiles ---------------------------
@@ -189,6 +194,7 @@ struct TcIm2col {       // im2col of the layer input into hi/lo operand tiles (o
   int shift[kMaxSeg];
   int nseg, K, KBs;     // K features per segment, KBs = ceil(K / 64) k-blocks per segment
   int M, T, rows_total;
+  const int* len;       // optional: valid length of each length-T sequence; a tap reads zeros at and past it (ragged batches)
 };
 struct TcBigPack {      // weights as GemmArgs describes them: W[n * ldw + w_off_s + k * w_stride_s]
   const float* W;

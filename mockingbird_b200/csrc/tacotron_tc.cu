@@ -286,13 +286,14 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gru_kernel(const __grid_consta
               [&](int m, float* v) {
                 const float* gi = p.gi[dir] + (size_t)m * p.ldgi + (size_t)tile * 8;
                 float* hp = p.h[dir] + (size_t)m * H + (size_t)tile * 8;
+                const bool before_start = dir == 1 && p.len1 && p.t1 >= p.len1[m];  // past a ragged row's end: h stays 0
                 float hn[8];
 #pragma unroll
                 for (int e = 0; e < 8; ++e) {
                   const float r = sigm(v[e] + gi[e]);
                   const float z = sigm(v[8 + e] + gi[H + e]);
                   const float n = tanhf(gi[2 * H + e] + v[16 + e] * r);
-                  hn[e] = (hp[e] - n) * z + n;
+                  hn[e] = before_start ? 0.f : (hp[e] - n) * z + n;
                 }
                 *reinterpret_cast<float4*>(hp) = make_float4(hn[0], hn[1], hn[2], hn[3]);
                 *reinterpret_cast<float4*>(hp + 4) = make_float4(hn[4], hn[5], hn[6], hn[7]);
@@ -375,8 +376,8 @@ __global__ void __launch_bounds__(kThreads, 1) tc_big_kernel(const __grid_consta
 }
 
 // im2col of a channels-last fp32 tensor into hi / lo operand tiles [nseg * KBs][rows_total][64]: segment s holds
-// x[row + shift_s][0 .. K) (zero outside the row's own length-T sequence, zero for k >= K and rows >= M; source rows >= M are
-// outside every sequence)
+// x[row + shift_s][0 .. K) (zero outside the row's own length-T sequence - or its first len[seq] rows - zero for k >= K and
+// rows >= M; source rows >= M are outside every sequence)
 __global__ void im2col_split_kernel(const TcIm2col q, __half* __restrict__ a_hi, __half* __restrict__ a_lo) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // one thread per 16-byte chunk
   const size_t total = (size_t)q.nseg * q.KBs * q.rows_total * 8;
@@ -391,7 +392,8 @@ __global__ void im2col_split_kernel(const TcIm2col q, __half* __restrict__ a_hi,
   if (ok && q.shift[sg] != 0) {
     const int t = m % q.T + q.shift[sg];
     row = m + q.shift[sg];
-    ok = (t >= 0 && t < q.T && row < q.M);  // a last, partial sequence (M not a multiple of T) ends at row M
+    const int len = q.len ? q.len[m / q.T] : q.T;
+    ok = (t >= 0 && t < len && row < q.M);  // a last, partial sequence (M not a multiple of T) ends at row M
   }
   const float* src = q.x[sg] + (size_t)row * q.ld[sg];
 #pragma unroll

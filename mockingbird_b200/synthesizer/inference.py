@@ -80,6 +80,31 @@ class Synthesizer:
         inputs = [text_to_sequence(text, hparams.tts_cleaner_names) for text in texts]
         return self.synthesize_from_sequences(inputs, embeddings, return_alignments, style_idx, min_stop_token, steps)
 
+    def synthesize_spectrograms_many(self, texts: List[str], embeddings: Union[np.ndarray, List[np.ndarray]],
+                                     return_alignments=False, style_idx=0, min_stop_token=5, steps=2000, seeds=None):
+        """synthesize_spectrograms with every text computed as its own batch of one (Tacotron.generate_many): a text's
+        spectrogram does not depend on the texts around it.  Same text front-end, postnet output and trailing trim;
+        -> list of [80, f_i] host arrays in input order (plus a list of per-text alignments when return_alignments)"""
+        if not self.is_loaded():
+            self.load()
+        if lazy_pinyin is not None:
+            texts = [" ".join(lazy_pinyin(v, style=Style.TONE3, neutral_tone_with_five=True)) for v in texts]
+        inputs = [text_to_sequence(text, hparams.tts_cleaner_names) for text in texts]
+        emb = np.stack([np.asarray(e, dtype=np.float32) for e in embeddings]) if len(embeddings) else np.zeros((0, 256), np.float32)
+        if emb.shape[0] != len(inputs):
+            raise ValueError(f"{emb.shape[0]} speaker embeddings for {len(inputs)} texts")
+        outs = self._model.generate_many(inputs, torch.from_numpy(emb), steps=steps, style_idx=style_idx,
+                                         min_stop_token=min_stop_token, seeds=seeds)
+        specs, alignments = [], []
+        for _, lin, attn in outs:
+            m = lin.cpu().numpy()
+            # Trim silence from end of each spectrogram (inference.py:135-138)
+            while m.shape[1] > 0 and np.max(m[:, -1]) < hparams.tts_stop_threshold:
+                m = m[:, :-1]
+            specs.append(m)
+            alignments.append(attn.cpu().numpy())
+        return (specs, alignments) if return_alignments else specs
+
     @staticmethod
     def load_preprocess_wav(fpath):
         """inference.py:143-158 (host utility): load at the synthesizer rate and rescale.  The reference additionally

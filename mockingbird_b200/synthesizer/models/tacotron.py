@@ -13,11 +13,24 @@ from __future__ import annotations
 import ctypes as C
 from typing import Dict, Optional
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
 from ... import _lib
 from ..hparams import gst_hparams
+
+# rows per ragged batch of generate_many (at most 128, the tensor-core decoder's limit); see DESIGN.md section 4b
+MANY_CHUNK_ROWS = 128
+
+
+def many_plan(lengths, chunk_rows):
+    """generate_many's batches: utterance indices sorted longest first (ties in input order), cut into chunks of at most
+    ``chunk_rows`` (1..128)"""
+    if not 1 <= int(chunk_rows) <= 128:
+        raise ValueError(f"chunk_rows must be in [1, 128], got {chunk_rows}")
+    order = sorted(range(len(lengths)), key=lambda i: (-int(lengths[i]), i))
+    return [order[k:k + int(chunk_rows)] for k in range(0, len(order), int(chunk_rows))]
 
 
 class Tacotron:
@@ -184,6 +197,105 @@ class Tacotron:
         lin = lin[: B * self.n_mels * f].view(B, self.n_mels, f)
         attn = attn[: B * (f // r) * Tc].view(B, f // r, Tc)
         return mel, lin, attn
+
+    def generate_many(self, seqs, speaker_embeddings, steps=2000, style_idx=0, min_stop_token=5, seeds=None,
+                      dropout_masks=None, chunk_rows=None):
+        """Many texts, each computed as its own B = 1 ``generate`` -> list of N ``(mel [80, f_i], linear [80, f_i],
+        attn [f_i / r, Tc_i])`` device tensors in input order.
+
+        ``seqs``: N unpadded int sequences; ``speaker_embeddings`` [N, 256]; ``steps``: one frame cap or N of them.  Each
+        utterance stops at its own stop rule or cap.  Utterances are sorted longest first and run in ragged batches of at
+        most ``chunk_rows`` (default ``MANY_CHUNK_ROWS``) rows; a result is bitwise the same whatever the list around it.
+        Dropout is drawn from ``seeds[i]`` (default ``self.seed + i``) or injected per utterance as
+        ``dropout_masks = (enc, dec)`` with enc[i] [2, Tc_i, 256] and dec[i] [>= ceil(steps_i / r), 2, 256]."""
+        self.eval()
+        N = len(seqs)
+        rows = [torch.as_tensor(s).reshape(-1).to(torch.int32) for s in seqs]
+        if N == 0:
+            return []
+        L = _lib.lib()
+        with torch.cuda.device(self._device or _lib.require_cuda()):
+            max_chars = int(L.mb_tacotron_max_chars())
+        for i, s in enumerate(rows):
+            if s.numel() == 0:
+                raise ValueError(f"text {i} is empty")
+            if s.numel() > max_chars:
+                raise ValueError(f"text {i} has {s.numel()} characters, over the limit of {max_chars} per utterance on this GPU")
+        spk_all = torch.as_tensor(speaker_embeddings).to(dtype=torch.float32)
+        if spk_all.dim() != 2 or spk_all.shape[0] != N or spk_all.shape[1] != self.speaker_embedding_size:
+            raise ValueError(f"speaker_embeddings has shape {tuple(spk_all.shape)}, expected ({N}, {self.speaker_embedding_size})")
+        caps = [int(steps)] * N if isinstance(steps, (int, np.integer)) else [int(v) for v in steps]
+        if len(caps) != N:
+            raise ValueError(f"{len(caps)} frame caps for {N} texts")
+        if min(caps) < 1:
+            raise ValueError("every frame cap must be at least 1")
+        seeds = [self.seed + i for i in range(N)] if seeds is None else [int(v) for v in seeds]
+        if len(seeds) != N:
+            raise ValueError(f"{len(seeds)} seeds for {N} texts")
+        r = self._r
+        E, D2 = self.encoder_dims, 2 * self.decoder_dims
+        if dropout_masks is not None:
+            enc_l, dec_l = dropout_masks
+            if len(enc_l) != N or len(dec_l) != N:
+                raise ValueError(f"dropout_masks need {N} encoder and {N} decoder masks")
+            for i in range(N):
+                if tuple(enc_l[i].shape) != (2, rows[i].numel(), E):
+                    raise ValueError(f"encoder mask {i} has shape {tuple(enc_l[i].shape)}, expected (2, {rows[i].numel()}, {E})")
+                nst_i = -(-caps[i] // r)
+                if enc_l[i].dim() != 3 or dec_l[i].dim() != 3 or dec_l[i].shape[0] < nst_i or tuple(dec_l[i].shape[1:]) != (2, D2):
+                    raise ValueError(f"decoder mask {i} has shape {tuple(dec_l[i].shape)}, expected ({nst_i}, 2, {D2})")
+        if not self._ready:
+            self._upload()
+        dev = self._device
+        out = [None] * N
+        for chunk in many_plan([s.numel() for s in rows], chunk_rows or MANY_CHUNK_ROWS):
+            B = len(chunk)
+            Tc = max(rows[i].numel() for i in chunk)
+            lens = [rows[i].numel() for i in chunk]
+            ccaps = [caps[i] for i in chunk]
+            nst = -(-max(ccaps) // r)
+            M = nst * r
+            chars = torch.zeros(B, Tc, dtype=torch.int32)
+            for b, i in enumerate(chunk):
+                chars[b, : lens[b]] = rows[i]
+            chars = chars.to(dev)
+            spk = spk_all[chunk].to(dev).contiguous()
+            enc_p = dec_p = None
+            if dropout_masks is not None:
+                enc_m = torch.zeros(2, B, Tc, E, dtype=torch.uint8)
+                dec_m = torch.zeros(nst, 2, B, D2, dtype=torch.uint8)
+                for b, i in enumerate(chunk):
+                    enc_m[:, b, : lens[b]] = enc_l[i].to(torch.uint8)
+                    n_i = -(-caps[i] // r)
+                    dec_m[:n_i, :, b] = dec_l[i][:n_i].to(torch.uint8)
+                enc_m, dec_m = enc_m.to(dev), dec_m.to(dev)
+                enc_p, dec_p = C.c_void_p(enc_m.data_ptr()), C.c_void_p(dec_m.data_ptr())
+            mel = torch.empty(B * self.n_mels * M, dtype=torch.float32, device=dev)
+            lin = torch.empty(B * self.n_mels * M, dtype=torch.float32, device=dev)
+            attn = torch.empty(B * nst * Tc, dtype=torch.float32, device=dev)
+            row_chars = (C.c_int32 * B)(*lens)
+            row_steps = (C.c_int32 * B)(*ccaps)
+            row_seeds = (C.c_uint64 * B)(*[seeds[i] & 0xFFFFFFFFFFFFFFFF for i in chunk])
+            row_frames = (C.c_int32 * B)()
+            frames = C.c_int32(0)
+            with torch.cuda.device(dev):
+                need = int(L.mb_tacotron_ragged_workspace_bytes(self._handle, B, Tc, max(ccaps), r)) + 256
+                if self._ws is None or self._ws.numel() < need:
+                    self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+                stream = torch.cuda.current_stream(dev).cuda_stream
+                _lib.check(L.mb_tacotron_generate_ragged(
+                    self._handle, C.c_void_p(chars.data_ptr()), C.c_void_p(spk.data_ptr()), B, Tc, row_chars, row_steps,
+                    row_seeds, r, int(style_idx), C.c_float(float(min_stop_token)), enc_p, dec_p, C.c_void_p(mel.data_ptr()),
+                    C.c_void_p(lin.data_ptr()), C.c_void_p(attn.data_ptr()), C.byref(frames), row_frames,
+                    C.c_void_p(self._ws.data_ptr()), self._ws.numel(), C.c_void_p(stream)))
+            F_ = frames.value
+            mel = mel[: B * self.n_mels * F_].view(B, self.n_mels, F_)
+            lin = lin[: B * self.n_mels * F_].view(B, self.n_mels, F_)
+            attn = attn[: B * (F_ // r) * Tc].view(B, F_ // r, Tc)
+            for b, i in enumerate(chunk):
+                f = row_frames[b]
+                out[i] = (mel[b, :, :f].clone(), lin[b, :, :f].clone(), attn[b, : f // r, : lens[b]].clone())
+        return out
 
     def __del__(self):
         try:
