@@ -606,6 +606,21 @@ int mb_encoder_embed_frames(mb_encoder* h, const float* frames, int32_t rows, in
  * [offsets[u], offsets[u+1]) (int32 device array [n_utterances+1]); out = L2(mean of those rows) */
 int mb_encoder_reduce_partials(mb_encoder* h, const float* partial_embeds, const int32_t* offsets,
                                int32_t n_utterances, float* utterance_embeds, void* stream);
+/* device workspace of mb_encoder_embed_rows for `rows` rows of at most max_len frames; 0 for a non-positive argument */
+size_t mb_encoder_rows_workspace_bytes(const mb_encoder* h, int32_t rows, int32_t max_len);
+/* SpeakerEncoder.forward on rows cut straight out of a ragged frame buffer (many utterances in one call):
+ *   frames fp32 [n_frames][mel_n_channels] (device): e.g. the utterances' mels of mb_melspec_forward_ragged back to back
+ *   row_start_host, row_len_host int32 [rows] (host): row r is frames [row_start[r], row_start[r] + row_len[r])
+ *   embeds fp32 [rows][embedding_size] (device, out)
+ * The LSTM runs to max_len = max row_len over inputs that are zero past each row's end; row r's embedding comes from the top
+ * layer's hidden state at its own step row_len[r] - 1, which the LSTM being causal makes exactly the row alone.  Every launch
+ * takes a route chosen without looking at the row count (tensor-core input projections at any rows * frames and tc_lstm_seq
+ * steps; with MB_ENC_TC=0 the FP32 GEMMs of one fmaf chain per output; the final Linear always the latter), so a row's result
+ * is bitwise the same whatever rows share the call.  MB_ERR_INVALID before anything is queued for an empty row or a row
+ * outside [0, n_frames); the message names the row.  The row table is copied from pageable host memory into the workspace. */
+int mb_encoder_embed_rows(mb_encoder* h, const float* frames, int64_t n_frames, const int32_t* row_start_host,
+                          const int32_t* row_len_host, int32_t rows, float* embeds, void* workspace, size_t workspace_bytes,
+                          void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Mel-spectrogram front-ends (SURVEY.md 8f rows N1 / N2)
@@ -641,6 +656,21 @@ int mb_melspec_set_arena(mb_melspec* h, void* arena, size_t bytes, void* stream)
 int32_t mb_melspec_num_frames(const mb_melspec* h, int32_t n_samples);   /* 1 + n_samples / hop_length */
 /* wav fp32 [n_samples] (device) -> out fp32 [frames][n_mels] or [n_mels][frames] (device) */
 int mb_melspec_forward(mb_melspec* h, const float* wav, int32_t n_samples, float* out, void* stream);
+/* device workspace of mb_melspec_forward_ragged for `batch` utterances (its utterance table); 0 when batch < 1 */
+size_t mb_melspec_ragged_workspace_bytes(const mb_melspec* h, int32_t batch);
+/* the mels of many utterances in one launch:
+ *   wavs fp32: the utterances back to back (device), lengths_host[b] > 0 samples each (host)
+ *   signal_lengths_host int32 [batch] (host) or NULL: utterance b is framed as a signal of signal_lengths_host[b] >=
+ *     lengths_host[b] samples whose tail past lengths_host[b] is zero, bitwise as if the zeros were stored (np.pad); NULL:
+ *     the stored lengths.  Reflect padding needs more than n_fft/2 signal samples.
+ *   out fp32 (device): utterance b has F_b = 1 + signal_b / hop_length frames, stored from out + n_mels * (F_0 + .. + F_{b-1})
+ *     as [F_b][n_mels] or [n_mels][F_b] (transpose_out)
+ * Padding, pre-emphasis and the output layout use each utterance's own indices, so utterance b's frames are bitwise
+ * mb_melspec_forward of it alone.  MB_ERR_INVALID before anything is queued for an empty or too short utterance; the message
+ * names it.  The utterance table is copied from pageable host memory into the workspace. */
+int mb_melspec_forward_ragged(mb_melspec* h, const float* wavs, const int32_t* lengths_host,
+                              const int32_t* signal_lengths_host, int32_t batch, float* out, void* workspace,
+                              size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Griffin-Lim inversion of normalised dB mel spectrograms (DESIGN.md section 4i; csrc/griffinlim.cu)

@@ -308,12 +308,18 @@ SIGNATURES = {
     "mb_encoder_embed_frames": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                           C.c_size_t, C.c_void_p]),
     "mb_encoder_reduce_partials": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "mb_encoder_rows_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.c_int32]),
+    "mb_encoder_embed_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                        C.c_int32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_melspec_create": (C.c_int, [C.POINTER(MelSpecConfig), C.POINTER(C.c_void_p)]),
     "mb_melspec_destroy": (None, [C.c_void_p]),
     "mb_melspec_arena_bytes": (C.c_size_t, [C.c_void_p]),
     "mb_melspec_set_arena": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_melspec_num_frames": (C.c_int32, [C.c_void_p, C.c_int32]),
     "mb_melspec_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "mb_melspec_ragged_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32]),
+    "mb_melspec_forward_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32,
+                                            C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_griffinlim_create": (C.c_int, [C.POINTER(GriffinLimConfig), C.POINTER(C.c_void_p)]),
     "mb_griffinlim_destroy": (None, [C.c_void_p]),
     "mb_griffinlim_arena_bytes": (C.c_size_t, [C.c_void_p]),

@@ -11,9 +11,13 @@
 // GEMM operand, and the next layer's input).  When hidden_size % 64 == 0 the recurrent step is ONE launch of
 // the tensor-core kernel tc_lstm_seq_kernel (tacotron_tc.cu: 3-term fp16 split, FP32-equivalent; cell update
 // in the epilogue; h_t written as the next step's operand tiles); MB_ENC_TC=0 keeps the FFMA path.
+// mb_encoder_embed_rows (many utterances, DESIGN.md section 4c): rows gathered on the device from a ragged frame buffer through
+// a row table, each row's embedding taken at its own last step, and routes that never depend on the row count.
+#include <climits>
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <vector>
 
 #include "../../include/mockingbird_b200.h"
 #include "mb_common.h"
@@ -99,6 +103,26 @@ __global__ void enc_reduce_kernel(const float* __restrict__ partial, const int32
   for (int j = lane; j < E; j += 32) out[(size_t)u * E + j] *= inv;
 }
 
+// mb_encoder_embed_rows: tab = row_start [R] | row_len [R].  x[r][t] = frames[row_start[r] + t] for t < row_len[r], else 0
+__global__ void enc_gather_rows_kernel(const float* __restrict__ frames, const int32_t* __restrict__ tab, float* __restrict__ x,
+                                       int R, int T, int C) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (size_t)R * T * C) return;
+  const int r = (int)(idx / ((size_t)T * C));
+  const int rem = (int)(idx - (size_t)r * T * C), t = rem / C, k = rem - t * C;
+  x[idx] = t < tab[R + r] ? frames[((size_t)tab[r] + t) * C + k] : 0.f;
+}
+
+// last[r] = seq[r][row_len[r] - 1]: each row's top-layer hidden state at its own last step (the LSTM is causal, so the steps
+// past a row's end do not reach it)
+__global__ void enc_gather_last_kernel(const float* __restrict__ seq, const int32_t* __restrict__ tab, float* __restrict__ last,
+                                       int R, int T, int H) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= R * H) return;
+  const int r = idx / H, j = idx - r * H;
+  last[idx] = seq[((size_t)r * T + tab[R + r] - 1) * H + j];
+}
+
 GemmArgs gemm1(const float* x, int K, int ld, const float* W, int ldw, const float* bias, int M, int N, float* Y,
                int ldy, int act = ACT_NONE) {
   GemmArgs a;
@@ -119,6 +143,7 @@ GemmArgs gemm1(const float* x, int K, int ld, const float* W, int ldw, const flo
 
 struct Ws {
   size_t xproj, seq0, seq1, gates, c, raw, t_hi, t_lo, big_hi, big_lo, total;
+  size_t in, last, tab;  // mb_encoder_embed_rows only: gathered input [R][T][C], last hidden rows [R][H], row table [2][R]
 };
 
 bool enc_use_tc(const mb_encoder_config& c) {
@@ -129,8 +154,9 @@ bool enc_use_tc(const mb_encoder_config& c) {
   return env && c.hidden_size % 64 == 0;
 }
 
-Ws ws_layout(const mb_encoder_config& c, size_t R, size_t T) {
+Ws ws_layout(const mb_encoder_config& c, size_t R, size_t T, bool rows = false) {
   Ws L;
+  L.in = L.last = L.tab = 0;
   size_t o = 0;
   auto take = [&](size_t n) {
     const size_t r = o;
@@ -151,8 +177,147 @@ Ws ws_layout(const mb_encoder_config& c, size_t R, size_t T) {
   const int kmax = c.hidden_size > c.mel_n_channels ? c.hidden_size : c.mel_n_channels;
   L.big_hi = take(tc_big_act_bytes((int)(R * T), 1, kmax) / 4);  // operand tiles of the whole-sequence input projection
   L.big_lo = take(tc_big_act_bytes((int)(R * T), 1, kmax) / 4);
+  if (rows) {
+    L.in = take(R * T * (size_t)c.mel_n_channels);
+    L.last = take(R * H);
+    L.tab = take(2 * R);
+  }
   L.total = o;
   return L;
+}
+
+// The LSTM stack over frames [R][T][C]; *top = the last layer's output sequence [R][T][H].  fixed_route: every launch takes a
+// route chosen without looking at R or T (tc_big input projections and tc_lstm_seq steps, or with MB_ENC_TC=0 fma_chain
+// GEMMs), so a row's bits do not depend on how many rows share the call; otherwise the input projection takes tc_big only
+// from 512 rows*frames and launch_gemm picks its kernel by M.
+int run_layers(mb_encoder* h, const float* frames, int R, int T, const Ws& L, float* ws, bool fixed_route, const float** top,
+               cudaStream_t st) {
+  const mb_encoder_config& c = h->cfg;
+  const int H = c.hidden_size, C = c.mel_n_channels;
+  const float* in = frames;
+  int in_dim = C;
+  float* seq[2] = {ws + L.seq0, ws + L.seq1};
+  for (int l = 0; l < c.num_layers; ++l) {
+    const std::string s = std::to_string(l);
+    float* outseq = seq[l & 1];
+    // input projection of the whole sequence: xproj[r*T + t] = W_ih x_t + (b_ih + b_hh)
+    if (enc_use_tc(c) && (fixed_route || (size_t)R * T >= 512)) {
+      // whole-sequence input projection on the 128x128-tile tensor-core GEMM (3-term split; images packed on first use)
+      __half* wimg = reinterpret_cast<__half*>(P(h, "lstm.ih_bigw_l" + s));
+      const int KBs = (in_dim + 63) / 64;
+      if (!h->big_packed[l]) {
+        unsigned int* dmax = reinterpret_cast<unsigned int*>(P(h, "scratch.absmax.bias_sum"));
+        MB_CUDA_CHECK(cudaMemsetAsync(dmax, 0, sizeof(unsigned int), st));
+        TK(tc_skinny_absmax(P(h, "lstm.weight_ih_l" + s), (size_t)4 * H * in_dim, dmax, st));
+        unsigned int hmax = 0;
+        MB_CUDA_CHECK(cudaMemcpyAsync(&hmax, dmax, sizeof(hmax), cudaMemcpyDeviceToHost, st));
+        MB_CUDA_CHECK(cudaStreamSynchronize(st));
+        TcBigPack q;
+        memset(&q, 0, sizeof(q));
+        q.W = P(h, "lstm.weight_ih_l" + s);
+        q.ldw = in_dim;
+        q.N = 4 * H;
+        q.nseg = 1;
+        q.K = in_dim;
+        q.KBs = KBs;
+        q.w_off[0] = 0;
+        q.w_stride[0] = 1;
+        q.scale = tc_weight_scale(hmax);
+        h->big_inv_scale[l] = 1.f / q.scale;
+        TK(launch_pack_big_w(q, wimg, st));
+        h->big_packed[l] = true;
+      }
+      TcIm2col q;
+      memset(&q, 0, sizeof(q));
+      q.x[0] = in;
+      q.ld[0] = in_dim;
+      q.nseg = 1;
+      q.K = in_dim;
+      q.KBs = KBs;
+      q.M = R * T;
+      q.T = 1;
+      q.rows_total = (R * T + 127) / 128 * 128;
+      TK(launch_im2col_split(q, reinterpret_cast<__half*>(ws + L.big_hi), reinterpret_cast<__half*>(ws + L.big_lo), st));
+      TcBigArgs t;
+      memset(&t, 0, sizeof(t));
+      t.a_hi = reinterpret_cast<const __half*>(ws + L.big_hi);
+      t.a_lo = reinterpret_cast<const __half*>(ws + L.big_lo);
+      t.w = wimg;
+      t.bias = P(h, "lstm.bias_sum_l" + s);
+      t.KB = KBs;
+      t.M = R * T;
+      t.N = 4 * H;
+      t.rows_total = q.rows_total;
+      t.act = ACT_NONE;
+      t.inv_scale = h->big_inv_scale[l];
+      t.y = ws + L.xproj;
+      t.ldy = 4 * H;
+      TK(launch_tc_big(t, st));
+    } else {
+      GemmArgs a = gemm1(in, in_dim, in_dim, P(h, "lstm.weight_ih_l" + s), in_dim, P(h, "lstm.bias_sum_l" + s), R * T, 4 * H,
+                         ws + L.xproj, 4 * H);
+      a.fma_chain = fixed_route;
+      TK(launch_gemm(a, st));
+    }
+    const float* whh = P(h, "lstm.weight_hh_l" + s);
+    if (enc_use_tc(c)) {
+      const size_t rows_total = ((size_t)R + 127) / 128 * 128;
+      const size_t tile_bytes = (size_t)(H / 64) * rows_total * 128;
+      MB_CUDA_CHECK(cudaMemsetAsync(ws + L.t_hi, 0, 2 * tile_bytes, st));  // h_{-1} = 0 (and the rows past R)
+      MB_CUDA_CHECK(cudaMemsetAsync(ws + L.t_lo, 0, 2 * tile_bytes, st));
+      MB_CUDA_CHECK(cudaMemsetAsync(ws + L.c, 0, sizeof(float) * (size_t)R * H, st));
+      TcLstmSeqArgs ta;
+      memset(&ta, 0, sizeof(ta));
+      ta.w = reinterpret_cast<const __half*>(P(h, "lstm.hh_tcw_l" + s));
+      ta.c = ws + L.c;
+      ta.inv_scale = h->tc_inv_scale[l];
+      ta.ldgi = T * 4 * H;
+      ta.ldout = T * H;
+      ta.KB = H / 64;
+      ta.M = R;
+      ta.H = H;
+      ta.rows_total = (int)rows_total;
+      for (int t = 0; t < T; ++t) {
+        const int par = t & 1;
+        ta.a_hi = reinterpret_cast<const __half*>(reinterpret_cast<const char*>(ws + L.t_hi) + par * tile_bytes);
+        ta.a_lo = reinterpret_cast<const __half*>(reinterpret_cast<const char*>(ws + L.t_lo) + par * tile_bytes);
+        ta.nxt_hi = reinterpret_cast<__half*>(reinterpret_cast<char*>(ws + L.t_hi) + (par ^ 1) * tile_bytes);
+        ta.nxt_lo = reinterpret_cast<__half*>(reinterpret_cast<char*>(ws + L.t_lo) + (par ^ 1) * tile_bytes);
+        ta.gi = ws + L.xproj + (size_t)t * 4 * H;
+        ta.out = outseq + (size_t)t * H;
+        TK(launch_tc_lstm_seq(ta, st));
+      }
+      in = outseq;
+      in_dim = H;
+      continue;
+    }
+    for (int t = 0; t < T; ++t) {
+      const float* g = ws + L.xproj + (size_t)t * 4 * H;  // row r of step t at + r*T*4H
+      size_t ldg = (size_t)T * 4 * H;
+      if (t > 0) {
+        GemmArgs b = gemm1(outseq + (size_t)(t - 1) * H, H, T * H, whh, H, nullptr, R, 4 * H, ws + L.gates, 4 * H);
+        b.res = g;
+        b.ldres = (int)ldg;
+        b.fma_chain = fixed_route;
+        TK(launch_gemm(b, st));
+        g = ws + L.gates;
+        ldg = 4 * H;
+      }
+      if (ldg == (size_t)4 * H) {
+        enc_lstm_cell_kernel<<<(R * H + 255) / 256, 256, 0, st>>>(g, ws + L.c, outseq + (size_t)t * H, (size_t)T * H, R, H, 0);
+      } else {
+        // t == 0: h_{-1} = 0, the gates are the projected input alone; copy rows into the dense gate buffer
+        MB_CUDA_CHECK(cudaMemcpy2DAsync(ws + L.gates, (size_t)4 * H * 4, g, ldg * 4, (size_t)4 * H * 4, R,
+                                        cudaMemcpyDeviceToDevice, st));
+        enc_lstm_cell_kernel<<<(R * H + 255) / 256, 256, 0, st>>>(ws + L.gates, ws + L.c, outseq, (size_t)T * H, R, H, 1);
+      }
+      MB_LAUNCH_CHECK("enc_lstm_cell_kernel");
+    }
+    in = outseq;
+    in_dim = H;
+  }
+  *top = in;
+  return MB_OK;
 }
 
 }  // namespace
@@ -257,130 +422,59 @@ int mb_encoder_embed_frames(mb_encoder* h, const float* frames, int32_t rows, in
     return fail(MB_ERR_WORKSPACE, "mb_encoder_embed_frames: workspace too small");
   float* ws = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
   cudaStream_t st = (cudaStream_t)stream;
-  const int R = rows, T = n_frames, H = c.hidden_size, C = c.mel_n_channels, E = c.embedding_size;
-  const float* in = frames;
-  int in_dim = C;
-  float* seq[2] = {ws + L.seq0, ws + L.seq1};
-  for (int l = 0; l < c.num_layers; ++l) {
-    const std::string s = std::to_string(l);
-    float* outseq = seq[l & 1];
-    // input projection of the whole sequence: xproj[r*T + t] = W_ih x_t + (b_ih + b_hh)
-    if (enc_use_tc(c) && (size_t)R * T >= 512) {
-      // whole-sequence input projection on the 128x128-tile tensor-core GEMM (3-term split; images packed on first use)
-      __half* wimg = reinterpret_cast<__half*>(P(h, "lstm.ih_bigw_l" + s));
-      const int KBs = (in_dim + 63) / 64;
-      if (!h->big_packed[l]) {
-        unsigned int* dmax = reinterpret_cast<unsigned int*>(P(h, "scratch.absmax.bias_sum"));
-        MB_CUDA_CHECK(cudaMemsetAsync(dmax, 0, sizeof(unsigned int), st));
-        TK(tc_skinny_absmax(P(h, "lstm.weight_ih_l" + s), (size_t)4 * H * in_dim, dmax, st));
-        unsigned int hmax = 0;
-        MB_CUDA_CHECK(cudaMemcpyAsync(&hmax, dmax, sizeof(hmax), cudaMemcpyDeviceToHost, st));
-        MB_CUDA_CHECK(cudaStreamSynchronize(st));
-        TcBigPack q;
-        memset(&q, 0, sizeof(q));
-        q.W = P(h, "lstm.weight_ih_l" + s);
-        q.ldw = in_dim;
-        q.N = 4 * H;
-        q.nseg = 1;
-        q.K = in_dim;
-        q.KBs = KBs;
-        q.w_off[0] = 0;
-        q.w_stride[0] = 1;
-        q.scale = tc_weight_scale(hmax);
-        h->big_inv_scale[l] = 1.f / q.scale;
-        TK(launch_pack_big_w(q, wimg, st));
-        h->big_packed[l] = true;
-      }
-      TcIm2col q;
-      memset(&q, 0, sizeof(q));
-      q.x[0] = in;
-      q.ld[0] = in_dim;
-      q.nseg = 1;
-      q.K = in_dim;
-      q.KBs = KBs;
-      q.M = R * T;
-      q.T = 1;
-      q.rows_total = (R * T + 127) / 128 * 128;
-      TK(launch_im2col_split(q, reinterpret_cast<__half*>(ws + L.big_hi), reinterpret_cast<__half*>(ws + L.big_lo), st));
-      TcBigArgs t;
-      memset(&t, 0, sizeof(t));
-      t.a_hi = reinterpret_cast<const __half*>(ws + L.big_hi);
-      t.a_lo = reinterpret_cast<const __half*>(ws + L.big_lo);
-      t.w = wimg;
-      t.bias = P(h, "lstm.bias_sum_l" + s);
-      t.KB = KBs;
-      t.M = R * T;
-      t.N = 4 * H;
-      t.rows_total = q.rows_total;
-      t.act = ACT_NONE;
-      t.inv_scale = h->big_inv_scale[l];
-      t.y = ws + L.xproj;
-      t.ldy = 4 * H;
-      TK(launch_tc_big(t, st));
-    } else {
-      GemmArgs a = gemm1(in, in_dim, in_dim, P(h, "lstm.weight_ih_l" + s), in_dim, P(h, "lstm.bias_sum_l" + s), R * T, 4 * H,
-                         ws + L.xproj, 4 * H);
-      TK(launch_gemm(a, st));
-    }
-    const float* whh = P(h, "lstm.weight_hh_l" + s);
-    if (enc_use_tc(c)) {
-      const size_t rows_total = ((size_t)R + 127) / 128 * 128;
-      const size_t tile_bytes = (size_t)(H / 64) * rows_total * 128;
-      MB_CUDA_CHECK(cudaMemsetAsync(ws + L.t_hi, 0, 2 * tile_bytes, st));  // h_{-1} = 0 (and the rows past R)
-      MB_CUDA_CHECK(cudaMemsetAsync(ws + L.t_lo, 0, 2 * tile_bytes, st));
-      MB_CUDA_CHECK(cudaMemsetAsync(ws + L.c, 0, sizeof(float) * (size_t)R * H, st));
-      TcLstmSeqArgs ta;
-      memset(&ta, 0, sizeof(ta));
-      ta.w = reinterpret_cast<const __half*>(P(h, "lstm.hh_tcw_l" + s));
-      ta.c = ws + L.c;
-      ta.inv_scale = h->tc_inv_scale[l];
-      ta.ldgi = T * 4 * H;
-      ta.ldout = T * H;
-      ta.KB = H / 64;
-      ta.M = R;
-      ta.H = H;
-      ta.rows_total = (int)rows_total;
-      for (int t = 0; t < T; ++t) {
-        const int par = t & 1;
-        ta.a_hi = reinterpret_cast<const __half*>(reinterpret_cast<const char*>(ws + L.t_hi) + par * tile_bytes);
-        ta.a_lo = reinterpret_cast<const __half*>(reinterpret_cast<const char*>(ws + L.t_lo) + par * tile_bytes);
-        ta.nxt_hi = reinterpret_cast<__half*>(reinterpret_cast<char*>(ws + L.t_hi) + (par ^ 1) * tile_bytes);
-        ta.nxt_lo = reinterpret_cast<__half*>(reinterpret_cast<char*>(ws + L.t_lo) + (par ^ 1) * tile_bytes);
-        ta.gi = ws + L.xproj + (size_t)t * 4 * H;
-        ta.out = outseq + (size_t)t * H;
-        TK(launch_tc_lstm_seq(ta, st));
-      }
-      in = outseq;
-      in_dim = H;
-      continue;
-    }
-    for (int t = 0; t < T; ++t) {
-      const float* g = ws + L.xproj + (size_t)t * 4 * H;  // row r of step t at + r*T*4H
-      size_t ldg = (size_t)T * 4 * H;
-      if (t > 0) {
-        GemmArgs b = gemm1(outseq + (size_t)(t - 1) * H, H, T * H, whh, H, nullptr, R, 4 * H, ws + L.gates, 4 * H);
-        b.res = g;
-        b.ldres = (int)ldg;
-        TK(launch_gemm(b, st));
-        g = ws + L.gates;
-        ldg = 4 * H;
-      }
-      if (ldg == (size_t)4 * H) {
-        enc_lstm_cell_kernel<<<(R * H + 255) / 256, 256, 0, st>>>(g, ws + L.c, outseq + (size_t)t * H, (size_t)T * H, R, H, 0);
-      } else {
-        // t == 0: h_{-1} = 0, the gates are the projected input alone; copy rows into the dense gate buffer
-        MB_CUDA_CHECK(cudaMemcpy2DAsync(ws + L.gates, (size_t)4 * H * 4, g, ldg * 4, (size_t)4 * H * 4, R,
-                                        cudaMemcpyDeviceToDevice, st));
-        enc_lstm_cell_kernel<<<(R * H + 255) / 256, 256, 0, st>>>(ws + L.gates, ws + L.c, outseq, (size_t)T * H, R, H, 1);
-      }
-      MB_LAUNCH_CHECK("enc_lstm_cell_kernel");
-    }
-    in = outseq;
-    in_dim = H;
-  }
+  const int R = rows, T = n_frames, H = c.hidden_size, E = c.embedding_size;
+  const float* top = nullptr;
+  if (int rc = run_layers(h, frames, R, T, L, ws, false, &top, st)) return rc;
   // hidden[-1] = last layer's h at t = T-1 -> relu(linear) -> L2 normalise
-  GemmArgs e = gemm1(in + (size_t)(T - 1) * H, H, T * H, P(h, "linear.weight"), H, P(h, "linear.bias"), R, E, ws + L.raw, E,
+  GemmArgs e = gemm1(top + (size_t)(T - 1) * H, H, T * H, P(h, "linear.weight"), H, P(h, "linear.bias"), R, E, ws + L.raw, E,
                      ACT_RELU);
+  TK(launch_gemm(e, st));
+  enc_l2norm_kernel<<<(R + 7) / 8, 256, 0, st>>>(ws + L.raw, embeds, R, E);
+  MB_LAUNCH_CHECK("enc_l2norm_kernel");
+  return MB_OK;
+}
+
+size_t mb_encoder_rows_workspace_bytes(const mb_encoder* h, int32_t rows, int32_t max_len) {
+  if (!h || rows <= 0 || max_len <= 0) return 0;
+  return ws_layout(h->cfg, rows, max_len, true).total * sizeof(float) + 256;
+}
+
+int mb_encoder_embed_rows(mb_encoder* h, const float* frames, int64_t n_frames, const int32_t* row_start_host,
+                          const int32_t* row_len_host, int32_t rows, float* embeds, void* workspace, size_t workspace_bytes,
+                          void* stream) {
+  const char* fn = "mb_encoder_embed_rows";
+  if (!h || !frames || !row_start_host || !row_len_host || !embeds || !workspace) return fail(MB_ERR_INVALID, "%s: null argument", fn);
+  if (!h->finalized) return fail(MB_ERR_STATE, "%s: weights not finalized", fn);
+  if (rows <= 0) return fail(MB_ERR_INVALID, "%s: rows = %d", fn, (int)rows);
+  const mb_encoder_config& c = h->cfg;
+  const int R = rows, H = c.hidden_size, C = c.mel_n_channels, E = c.embedding_size;
+  int T = 0;
+  std::vector<int32_t> tab(2 * (size_t)R);
+  for (int r = 0; r < R; ++r) {
+    const int32_t s0 = row_start_host[r], n = row_len_host[r];
+    if (n <= 0 || s0 < 0 || (int64_t)s0 + n > n_frames)
+      return fail(MB_ERR_INVALID, "%s: row %d = frames [%d, %d + %d) is empty or outside the %lld frames", fn, r, (int)s0,
+                  (int)s0, (int)n, (long long)n_frames);
+    tab[r] = s0;
+    tab[R + r] = n;
+    T = n > T ? n : T;
+  }
+  if ((int64_t)R * T * 4 * H > INT32_MAX) return fail(MB_ERR_INVALID, "%s: %d rows of up to %d frames are too many for one call", fn, R, T);
+  const Ws L = ws_layout(c, R, T, true);
+  if (workspace_bytes < L.total * sizeof(float) + 256) return fail(MB_ERR_WORKSPACE, "%s: workspace too small", fn);
+  float* ws = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  cudaStream_t st = (cudaStream_t)stream;
+  int32_t* dtab = reinterpret_cast<int32_t*>(ws + L.tab);
+  MB_CUDA_CHECK(cudaMemcpyAsync(dtab, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  const size_t n_in = (size_t)R * T * C;
+  enc_gather_rows_kernel<<<(unsigned)((n_in + 255) / 256), 256, 0, st>>>(frames, dtab, ws + L.in, R, T, C);
+  MB_LAUNCH_CHECK("enc_gather_rows_kernel");
+  const float* top = nullptr;
+  if (int rc = run_layers(h, ws + L.in, R, T, L, ws, true, &top, st)) return rc;
+  enc_gather_last_kernel<<<(R * H + 255) / 256, 256, 0, st>>>(top, dtab, ws + L.last, R, T, H);
+  MB_LAUNCH_CHECK("enc_gather_last_kernel");
+  GemmArgs e = gemm1(ws + L.last, H, H, P(h, "linear.weight"), H, P(h, "linear.bias"), R, E, ws + L.raw, E, ACT_RELU);
+  e.fma_chain = 1;
   TK(launch_gemm(e, st));
   enc_l2norm_kernel<<<(R + 7) / 8, 256, 0, st>>>(ws + L.raw, embeds, R, E);
   MB_LAUNCH_CHECK("enc_l2norm_kernel");

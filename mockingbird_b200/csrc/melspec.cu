@@ -12,6 +12,9 @@
 //
 // One CTA per frame: windowed frame -> shared memory, direct DFT (n_fft <= 2048: O(N^2) is ~0.5 MFLOP per frame),
 // magnitude / power -> shared memory, mel projection (one warp per mel band, shuffle reduction), dB / normalise.
+// A launch covers one utterance (mb_melspec_forward) or many (mb_melspec_forward_ragged: a CTA finds its utterance in a table
+// by binary search; padding, pre-emphasis and output layout use utterance-local indices, so each is bitwise its single call).
+#include <climits>
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -38,9 +41,19 @@ double mel_to_hz(double m) {
   return m >= min_log_mel ? min_log_hz * std::exp(logstep * (m - min_log_mel)) : f_sp * m;
 }
 
+// One utterance of a ragged call: its samples wav[wav_off .. wav_off + n_stored), read as a signal of n_signal >= n_stored
+// samples whose tail past n_stored is zero (embed_utterance's np.pad without a host copy); its frames are
+// [frame_off, frame_off + n_frames) of the call, stored at out + frame_off * n_mels in the utterance's own layout.
+struct MelUtt {
+  long long wav_off;
+  int n_stored, n_signal, frame_off, n_frames;
+};
+
 struct MelParams {
   const float* wav;
-  int n_samples, n_frames;
+  const MelUtt* utt;  // [n_utt] (device); nullptr: the single utterance `one`
+  MelUtt one;
+  int n_utt;
   int n_fft, hop, n_bins, n_mels, pad_mode, power, to_db, normalize, symmetric, transpose_out;
   float preemphasis, min_level, ref_level_db, min_level_db, max_abs_value;
   const float* window;
@@ -50,19 +63,22 @@ struct MelParams {
   float* out;
 };
 
-__device__ __forceinline__ float sample_at(const MelParams& p, int i) {
+// sample i of the utterance's signal (utterance-local; zero in the virtual tail)
+__device__ __forceinline__ float stored_at(const float* w, const MelUtt& u, int i) { return i < u.n_stored ? w[i] : 0.f; }
+
+__device__ __forceinline__ float sample_at(const MelParams& p, const MelUtt& u, const float* w, int i) {
   // centered framing: index i of the padded signal refers to sample i - n_fft/2; reflect (or zero) outside
   int j = i;
   if (j < 0) {
     if (p.pad_mode != 0) return 0.f;
     j = -j;
-  } else if (j >= p.n_samples) {
+  } else if (j >= u.n_signal) {
     if (p.pad_mode != 0) return 0.f;
-    j = 2 * (p.n_samples - 1) - j;
+    j = 2 * (u.n_signal - 1) - j;
   }
-  if (j < 0 || j >= p.n_samples) return 0.f;
-  float v = p.wav[j];
-  if (p.preemphasis != 0.f && j > 0) v -= p.preemphasis * p.wav[j - 1];  // lfilter([1, -k], [1], wav)
+  if (j < 0 || j >= u.n_signal) return 0.f;
+  float v = stored_at(w, u, j);
+  if (p.preemphasis != 0.f && j > 0) v -= p.preemphasis * stored_at(w, u, j - 1);  // lfilter([1, -k], [1], wav)
   return v;
 }
 
@@ -72,10 +88,23 @@ __global__ void __launch_bounds__(256) melspec_kernel(const MelParams p) {
   float* tc = fr + p.n_fft;        // [n_fft] cos
   float* ts = tc + p.n_fft;        // [n_fft] sin
   float* mag = ts + p.n_fft;       // [n_bins]
-  const int f = blockIdx.x, tid = threadIdx.x;
+  const int tid = threadIdx.x;
+  MelUtt u = p.one;
+  if (p.utt) {  // the utterance owning this CTA's frame: last u with frame_off <= blockIdx.x
+    int lo = 0, hi = p.n_utt - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (p.utt[mid].frame_off <= (int)blockIdx.x) lo = mid;
+      else hi = mid - 1;
+    }
+    u = p.utt[lo];
+  }
+  const int f = (int)blockIdx.x - u.frame_off;
+  const float* w = p.wav + u.wav_off;
+  float* out = p.out + (size_t)u.frame_off * p.n_mels;
   const int start = f * p.hop - p.n_fft / 2;
   for (int j = tid; j < p.n_fft; j += blockDim.x) {
-    fr[j] = sample_at(p, start + j) * p.window[j];
+    fr[j] = sample_at(p, u, w, start + j) * p.window[j];
     tc[j] = p.cs[j];
     ts[j] = p.sn[j];
   }
@@ -103,12 +132,12 @@ __global__ void __launch_bounds__(256) melspec_kernel(const MelParams p) {
       float v = a;
       if (p.to_db) v = 20.f * log10f(fmaxf(p.min_level, v)) - p.ref_level_db;
       if (p.normalize) {
-        const float u = (v - p.min_level_db) / (-p.min_level_db);
-        v = p.symmetric ? fminf(fmaxf(2.f * p.max_abs_value * u - p.max_abs_value, -p.max_abs_value), p.max_abs_value)
-                        : fminf(fmaxf(p.max_abs_value * u, 0.f), p.max_abs_value);
+        const float s = (v - p.min_level_db) / (-p.min_level_db);
+        v = p.symmetric ? fminf(fmaxf(2.f * p.max_abs_value * s - p.max_abs_value, -p.max_abs_value), p.max_abs_value)
+                        : fminf(fmaxf(p.max_abs_value * s, 0.f), p.max_abs_value);
       }
-      if (p.transpose_out) p.out[(size_t)f * p.n_mels + m] = v;
-      else p.out[(size_t)m * p.n_frames + f] = v;
+      if (p.transpose_out) out[(size_t)f * p.n_mels + m] = v;
+      else out[(size_t)m * u.n_frames + f] = v;
     }
   }
 }
@@ -177,18 +206,15 @@ int32_t mb_melspec_num_frames(const mb_melspec* h, int32_t n_samples) {
   return 1 + n_samples / h->cfg.hop_length;  // librosa center=True
 }
 
-int mb_melspec_forward(mb_melspec* h, const float* wav, int32_t n_samples, float* out, void* stream) {
-  if (!h || !wav || !out) return fail(MB_ERR_INVALID, "mb_melspec_forward: null argument");
-  if (!h->arena) return fail(MB_ERR_STATE, "mb_melspec_forward: call mb_melspec_set_arena first");
+}  // extern "C"
+
+namespace {
+
+// the kernel's parameters from the handle; the caller sets wav, utt / one, n_utt and out
+MelParams base_params(const mb_melspec* h) {
   const mb_melspec_config& c = h->cfg;
-  if (n_samples <= 0) return fail(MB_ERR_INVALID, "mb_melspec_forward: empty signal");
-  if (c.pad_mode == 0 && n_samples <= c.n_fft / 2)
-    return fail(MB_ERR_INVALID, "mb_melspec_forward: reflect padding needs more than n_fft/2 = %d samples", c.n_fft / 2);
   MelParams p;
   memset(&p, 0, sizeof(p));
-  p.wav = wav;
-  p.n_samples = n_samples;
-  p.n_frames = mb_melspec_num_frames(h, n_samples);
   p.n_fft = c.n_fft;
   p.hop = c.hop_length;
   p.n_bins = h->n_bins;
@@ -208,11 +234,81 @@ int mb_melspec_forward(mb_melspec* h, const float* wav, int32_t n_samples, float
   p.cs = h->arena + c.n_fft;
   p.sn = h->arena + 2 * c.n_fft;
   p.basis = h->arena + 3 * c.n_fft;
-  p.out = out;
-  const size_t smem = sizeof(float) * ((size_t)3 * c.n_fft + h->n_bins);
-  melspec_kernel<<<p.n_frames, 256, smem, (cudaStream_t)stream>>>(p);
+  return p;
+}
+
+int launch_melspec(const mb_melspec* h, const MelParams& p, int total_frames, cudaStream_t st) {
+  const size_t smem = sizeof(float) * ((size_t)3 * h->cfg.n_fft + h->n_bins);
+  melspec_kernel<<<total_frames, 256, smem, st>>>(p);
   MB_LAUNCH_CHECK("melspec_kernel");
   return MB_OK;
+}
+
+// utterance b of a call: stored and signal lengths valid for the handle's padding
+int check_utterance(const mb_melspec* h, const char* fn, int b, int32_t n_stored, int32_t n_signal) {
+  const mb_melspec_config& c = h->cfg;
+  if (n_stored <= 0) return fail(MB_ERR_INVALID, "%s: utterance %d is empty", fn, b);
+  if (n_signal < n_stored)
+    return fail(MB_ERR_INVALID, "%s: utterance %d: signal length %d is shorter than its %d samples", fn, b, (int)n_signal,
+                (int)n_stored);
+  if (c.pad_mode == 0 && n_signal <= c.n_fft / 2)
+    return fail(MB_ERR_INVALID, "%s: utterance %d has %d samples; reflect padding needs more than n_fft/2 = %d", fn, b,
+                (int)n_signal, c.n_fft / 2);
+  return MB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mb_melspec_forward(mb_melspec* h, const float* wav, int32_t n_samples, float* out, void* stream) {
+  if (!h || !wav || !out) return fail(MB_ERR_INVALID, "mb_melspec_forward: null argument");
+  if (!h->arena) return fail(MB_ERR_STATE, "mb_melspec_forward: call mb_melspec_set_arena first");
+  const mb_melspec_config& c = h->cfg;
+  if (n_samples <= 0) return fail(MB_ERR_INVALID, "mb_melspec_forward: empty signal");
+  if (c.pad_mode == 0 && n_samples <= c.n_fft / 2)
+    return fail(MB_ERR_INVALID, "mb_melspec_forward: reflect padding needs more than n_fft/2 = %d samples", c.n_fft / 2);
+  MelParams p = base_params(h);
+  p.wav = wav;
+  p.one = MelUtt{0, n_samples, n_samples, 0, mb_melspec_num_frames(h, n_samples)};
+  p.n_utt = 1;
+  p.out = out;
+  return launch_melspec(h, p, p.one.n_frames, (cudaStream_t)stream);
+}
+
+size_t mb_melspec_ragged_workspace_bytes(const mb_melspec* h, int32_t batch) {
+  if (!h || batch <= 0) return 0;
+  return align_up(sizeof(MelUtt) * (size_t)batch, 256) + 256;
+}
+
+int mb_melspec_forward_ragged(mb_melspec* h, const float* wavs, const int32_t* lengths_host,
+                              const int32_t* signal_lengths_host, int32_t batch, float* out, void* workspace,
+                              size_t workspace_bytes, void* stream) {
+  const char* fn = "mb_melspec_forward_ragged";
+  if (!h || !wavs || !lengths_host || !out || !workspace) return fail(MB_ERR_INVALID, "%s: null argument", fn);
+  if (!h->arena) return fail(MB_ERR_STATE, "%s: call mb_melspec_set_arena first", fn);
+  if (batch <= 0) return fail(MB_ERR_INVALID, "%s: batch = %d", fn, (int)batch);
+  if (workspace_bytes < mb_melspec_ragged_workspace_bytes(h, batch)) return fail(MB_ERR_WORKSPACE, "%s: workspace too small", fn);
+  std::vector<MelUtt> utt(batch);
+  long long o = 0, f0 = 0;
+  for (int b = 0; b < batch; ++b) {
+    const int32_t n = lengths_host[b], ns = signal_lengths_host ? signal_lengths_host[b] : n;
+    if (int rc = check_utterance(h, fn, b, n, ns)) return rc;
+    const int nf = mb_melspec_num_frames(h, ns);
+    if (f0 + nf > INT32_MAX) return fail(MB_ERR_INVALID, "%s: more than 2^31 - 1 frames in one call", fn);
+    utt[b] = MelUtt{o, n, ns, (int)f0, nf};
+    o += n;
+    f0 += nf;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  MelUtt* dutt = (MelUtt*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  MB_CUDA_CHECK(cudaMemcpyAsync(dutt, utt.data(), sizeof(MelUtt) * utt.size(), cudaMemcpyHostToDevice, st));
+  MelParams p = base_params(h);
+  p.wav = wavs;
+  p.utt = dutt;
+  p.n_utt = batch;
+  p.out = out;
+  return launch_melspec(h, p, (int)f0, st);
 }
 
 }  // extern "C"

@@ -1,7 +1,9 @@
 """Drop-in for ``models/encoder/inference.py`` (reference :15-172): module-global model,
 ``load_model`` / ``set_model`` / ``is_loaded`` / ``embed_frames_batch`` / ``compute_partial_slices`` /
 ``embed_utterance``.  The network runs on the H100 (mb_encoder_*); outputs are host numpy like the
-reference.  Extension: ``embed_utterances_frames`` embeds many utterances' partial stacks in one batch.
+reference.  Extensions: ``embed_utterances_frames`` embeds many utterances' partial stacks in one batch, and
+``embed_utterances`` is ``embed_utterance`` for a list of waveforms, mels and rows on the device, each result independent
+of the list around it.
 """
 from __future__ import annotations
 
@@ -14,7 +16,7 @@ import torch
 from .. import _lib
 from .model import SpeakerEncoder
 from .params_data import *  # noqa: F401,F403  (the reference re-exports these, inference.py:1)
-from .params_data import mel_window_step, partials_n_frames, sampling_rate
+from .params_data import mel_n_channels, mel_window_step, partials_n_frames, sampling_rate
 from ..synthesizer import audio_host as _audio_host
 
 _model = None  # type: SpeakerEncoder
@@ -137,3 +139,86 @@ def embed_utterance(wav, using_partials=True, return_partials=False, **kwargs):
     raw_embed = np.mean(partial_embeds, axis=0)
     embed = raw_embed / np.linalg.norm(raw_embed, 2)
     return (embed, partial_embeds, wave_slices) if return_partials else embed
+
+
+# rows per mb_encoder_embed_rows call, and rows x longest row per call: a full call's workspace is ~1.2 GB
+# (mb_encoder_rows_workspace_bytes(1024, 160), which the model keeps for its lifetime); see DESIGN.md section 4c
+MANY_ROWS = 1024
+MANY_FRAMES = MANY_ROWS * partials_n_frames
+
+
+def utterance_rows(n_samples, using_partials=True, **kwargs):
+    """How embed_utterance cuts an utterance of n_samples samples: (signal length, wave_slices, row starts, row lengths).
+    With partials the rows are the mel_slices of compute_partial_slices over the waveform zero-padded to
+    wave_slices[-1].stop (the signal length when that is longer); without, one row of all 1 + n // hop frames."""
+    samples_per_frame = int(sampling_rate * mel_window_step / 1000)
+    if not using_partials:
+        return n_samples, None, [0], [1 + n_samples // samples_per_frame]
+    wave_slices, mel_slices = compute_partial_slices(n_samples, **kwargs)
+    return (max(n_samples, wave_slices[-1].stop), wave_slices, [s.start for s in mel_slices],
+            [s.stop - s.start for s in mel_slices])
+
+
+def many_plan(row_lens, max_rows=MANY_ROWS, max_frames=MANY_FRAMES):
+    """embed_utterances' library calls.  row_lens[u]: utterance u's row lengths.  Utterances are taken longest row first
+    (then most rows, then input order) and their rows packed into calls of at most max_rows rows and max_frames rows x
+    longest row; an utterance may span calls.  Returns a list of calls, each a list of (u, first row, end row)."""
+    if max_rows < 1 or max_frames < 1:
+        raise ValueError(f"max_rows = {max_rows} and max_frames = {max_frames} must be positive")
+    order = sorted(range(len(row_lens)), key=lambda u: (-max(row_lens[u]), -len(row_lens[u]), u))
+    calls, cur, rows, T = [], [], 0, 0
+    for u in order:
+        for r, n in enumerate(row_lens[u]):
+            if rows and (rows + 1 > max_rows or (rows + 1) * max(T, n) > max_frames):
+                calls.append(cur)
+                cur, rows, T = [], 0, 0
+            if cur and cur[-1][0] == u and cur[-1][2] == r:
+                cur[-1] = (u, cur[-1][1], r + 1)
+            else:
+                cur.append((u, r, r + 1))
+            rows, T = rows + 1, max(T, n)
+    if cur:
+        calls.append(cur)
+    return calls
+
+
+def embed_utterances(wavs, using_partials=True, return_partials=False, **kwargs):
+    """embed_utterance (inference.py:128-172) for a list of waveforms: [U, 256] float32, or with return_partials a list of
+    (embed, partial_embeds, wave_slices) per utterance.  The slices come from compute_partial_slices with the same kwargs for
+    every utterance.  Utterances are sorted by length and their mels and rows computed in a few library calls
+    (``many_plan``): one mel launch and one mb_encoder_embed_rows per call, the frames never leaving the device.  A result
+    is bitwise the same whatever the list around it (order, neighbours, chunking), and within FP32 rounding of
+    embed_utterance on the same waveform."""
+    if _model is None:
+        raise Exception("Model was not loaded. Call load_model() before inference.")
+    from . import audio
+    from ..melspec import as_wavs
+
+    wavs = as_wavs(wavs)
+    plans = [utterance_rows(len(w), using_partials, **kwargs) for w in wavs]
+    audio.check(wavs, [p[0] for p in plans])
+    E = _model._cfg.embedding_size
+    if not wavs:
+        return [] if return_partials else np.zeros((0, E), np.float32)
+    offsets = np.concatenate([[0], np.cumsum([len(p[2]) for p in plans])]).astype(np.int64)
+    dev = _model.resolved_device()
+    part = torch.empty(int(offsets[-1]), E, dtype=torch.float32, device=dev)
+    front = audio.mel_front(dev)  # the frames are computed where the encoder reads them
+    for call in many_plan([p[3] for p in plans]):
+        utts = list(dict.fromkeys(u for u, _, _ in call))
+        flat, counts = front.many_flat([wavs[u] for u in utts], [plans[u][0] for u in utts])
+        first = dict(zip(utts, np.concatenate([[0], np.cumsum(counts)[:-1]]).tolist()))
+        starts, lens, dst = [], [], []
+        for u, r0, r1 in call:
+            starts += [first[u] + s for s in plans[u][2][r0:r1]]
+            lens += plans[u][3][r0:r1]
+            dst += range(int(offsets[u]) + r0, int(offsets[u]) + r1)
+        rows = _model.embed_rows(flat.view(-1, mel_n_channels), starts, lens)
+        part.index_copy_(0, torch.tensor(dst, dtype=torch.long, device=dev), rows)
+    embeds = (_model.reduce_partials(part, offsets.astype(np.int32)) if using_partials else part).cpu().numpy()
+    if not return_partials:
+        return embeds
+    if not using_partials:
+        return [(embeds[u], None, None) for u in range(len(wavs))]
+    pe = part.cpu().numpy()
+    return [(embeds[u], pe[offsets[u]:offsets[u + 1]], plans[u][1]) for u in range(len(wavs))]

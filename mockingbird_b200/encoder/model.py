@@ -94,6 +94,37 @@ class SpeakerEncoder:
 
     __call__ = forward
 
+    def resolved_device(self) -> torch.device:
+        """the device the weights live on, with its index (uploads them first if needed)"""
+        if not self._ready:
+            self._upload()
+        d = self._device
+        return d if d.index is not None else torch.device("cuda", torch.cuda.current_device())
+
+    def embed_rows(self, frames: torch.Tensor, row_starts, row_lens) -> torch.Tensor:
+        """forward() on rows cut out of a ragged frame buffer (mb_encoder_embed_rows): frames [n_frames, 40] on the device,
+        row r = frames[row_starts[r] : row_starts[r] + row_lens[r]]; returns [R, 256] on the device.  Each row's result is
+        bitwise the same whatever rows share the call."""
+        dev = self.resolved_device()
+        if frames.device != dev or frames.dtype != torch.float32 or not frames.is_contiguous() or frames.dim() != 2 \
+                or frames.shape[1] != self._cfg.mel_n_channels:
+            raise _lib.MbError(f"embed_rows: frames must be a contiguous float32 [n, {self._cfg.mel_n_channels}] tensor on "
+                               f"{dev}, got {frames.dtype} {tuple(frames.shape)} on {frames.device}")
+        L = _lib.lib()
+        R = len(row_starts)
+        starts = (C.c_int32 * R)(*[int(v) for v in row_starts])
+        lens = (C.c_int32 * R)(*[int(v) for v in row_lens])
+        out = torch.empty(R, self._cfg.embedding_size, dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            need = int(L.mb_encoder_rows_workspace_bytes(self._handle, R, max(int(v) for v in row_lens))) + 256
+            if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
+                self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            _lib.check(L.mb_encoder_embed_rows(self._handle, C.c_void_p(frames.data_ptr()), frames.shape[0], starts, lens, R,
+                                               C.c_void_p(out.data_ptr()), C.c_void_p(self._ws.data_ptr()), self._ws.numel(),
+                                               C.c_void_p(stream)))
+        return out
+
     def reduce_partials(self, partial_embeds: torch.Tensor, offsets) -> torch.Tensor:
         """L2(mean of the partial embeddings) per utterance (inference.py:164-166); offsets = CSR [U+1]"""
         dev = self._device

@@ -25,7 +25,7 @@ def get_hop_size(hparams):
     return hop_size
 
 
-def melspectrogram(wav, hparams):
+def _mel_front(hparams):
     if getattr(hparams, "use_lws", False):
         raise NotImplementedError("use_lws=True (lws STFT) is not built")
     if not getattr(hparams, "allow_clipping_in_normalization", True):
@@ -40,7 +40,25 @@ def melspectrogram(wav, hparams):
                                      min_level_db=hparams.min_level_db, ref_level_db=hparams.ref_level_db,
                                      normalize=bool(hparams.signal_normalization), max_abs_value=hparams.max_abs_value,
                                      symmetric=bool(hparams.symmetric_mels), transpose_out=False)
-    return _front[key](np.asarray(wav, dtype=np.float32)).cpu().numpy()
+    return _front[key]
+
+
+def melspectrogram(wav, hparams):
+    return _mel_front(hparams)(np.asarray(wav, dtype=np.float32)).cpu().numpy()
+
+
+def melspectrograms(wavs, hparams):
+    """melspectrogram of many waveforms in one launch: a list of float32 [num_mels, n_i], entry i bitwise
+    melspectrogram(wavs[i], hparams).  Pre-emphasis starts afresh at each waveform's first sample.  Every waveform is
+    checked (1-D, not empty, more than n_fft / 2 samples with reflect padding) before anything is queued; the ValueError
+    names the first bad one."""
+    from ..melspec import as_wavs, check_wavs, min_signal_length
+
+    wavs = as_wavs(wavs)
+    check_wavs(wavs, min_signal_length(hparams.n_fft, pad_mode))
+    if not wavs:
+        return []
+    return _mel_front(hparams).many(wavs)
 
 
 _inverse = {}
