@@ -504,6 +504,10 @@ typedef struct mb_taco_tc_debug_spec {
   int32_t pdl;               /* 0 / 1, -1 = MB_TACO_PDL */
   void* a_tiles;             /* optional out: the activation operand tiles, hi plane then lo plane (direction 0) */
   void* w_tiles;             /* optional out: the packed weight image (direction 0) */
+  const int32_t* len;        /* ragged rows, or NULL (the padded path).  BIG: device [ceil(M / T)] valid length of each length-T
+                                sequence: a shifted tap reads zeros at and past it (TcIm2col::len).  GRU: device [M] valid
+                                length of each row: direction 1 keeps h = 0 (state, out[1], nxt tiles) while t1 >= len[m] */
+  int32_t t1;                /* GRU with len: the time index direction 1 is at in this step (TcGruArgs::t1) */
 } mb_taco_tc_debug_spec;
 /* device workspace the spec needs */
 size_t mb_taco_tc_debug_workspace_bytes(const mb_taco_tc_debug_spec* spec);
@@ -526,17 +530,22 @@ int mb_taco_tc_debug(const mb_taco_tc_debug_spec* spec, void* workspace, size_t 
 #define MB_TACO_DBG_EMBEDDING 6        /* in: ids (int32), table  out: y  n: M, D                                               */
 #define MB_TACO_DBG_COPY_COLS 7        /* in: src  out: dst  n: M, n, ldsrc, rows_per_src, lddst, off                           */
 #define MB_TACO_DBG_LSA_STEP 8         /* in: pq, proj, seq, chars, conv_w, conv_b, L, v, q_in, Wq, bq  out: cum, scores, ctx
-                                          n: B, Tc, seq_dim, scores_ld, threads (256 | 512); q_in NULL: pq is read          */
+                                          n: B, Tc, seq_dim, scores_ld, threads (256 | 512); q_in NULL: pq is read
+                                          row_len: the kernel's lens (row b ends at row_len[b] <= Tc), or NULL              */
 #define MB_TACO_DBG_LSA_CTX 9          /* in: scores, seq  out: ctx, sa_hi, sa_lo, sb_hi, sb_lo
-                                          n: B, Tc, seq_dim (a multiple of 256), scores_ld, s_rows_pad                       */
+                                          n: B, Tc, seq_dim (a multiple of 256), scores_ld, s_rows_pad
+                                          row_len: the kernel's lens (only t < row_len[b] is read), or NULL                 */
 #define MB_TACO_DBG_GST_ATTENTION 10   /* in: q, keys, values  out: y  n: B, ntok (<= 16), E, heads (<= 8)                      */
-#define MB_TACO_DBG_STOP_STEP 11       /* GemmArgs (x, W, bias, y, ldy; N = 1) and out: flags, ticket  n: B, r  fval: min_stop */
-#define MB_TACO_DBG_STOP_FLAG 12       /* in: stopv  out: flags  n: B, r  fval: min_stop_token                                  */
+#define MB_TACO_DBG_STOP_STEP 11       /* GemmArgs (x, W, bias, y, ldy; N = 1) and out: flags, ticket  n: B, r  fval: min_stop
+                                          row_done / row_caps: the per-row rule of ragged batches, or NULL (both or neither) */
+#define MB_TACO_DBG_STOP_FLAG 12       /* in: stopv  out: flags  n: B, r  fval: min_stop_token  row_done / row_caps as above   */
 #define MB_TACO_DBG_FILL_MASKS 13      /* out: m  n: count, stream_id  seed (step_ptr: stream_id += *step_ptr)                  */
 #define MB_TACO_DBG_FILL_MASKS_STEPS 14 /* out: m  n: per_step, steps  seed                                                     */
 #define MB_TACO_DBG_PACK_MELPROJ 15    /* in: W  out: dst  n: n_mels, max_r, r, K                                               */
 #define MB_TACO_DBG_TO_NCL 16          /* in: x  out: y  n: steps, B, C, frames                                                 */
 #define MB_TACO_DBG_BN_FOLD 17         /* in: gamma, beta, mean, var  out: scale, shift  n: count                               */
+#define MB_TACO_DBG_FILL_MASKS_SEEDED 18 /* out: m  n: B, npos, units, dec (0: m [2][B][npos][units], 1: m [npos][2][B][units])
+                                            row_seeds: device [B] Philox key of each row                                     */
 typedef struct mb_taco_debug_spec {
   int32_t kind;                /* MB_TACO_DBG_* */
   /* GemmArgs (csrc/tacotron_kernels.cuh) */
@@ -566,6 +575,12 @@ typedef struct mb_taco_debug_spec {
   int64_t n[10];
   float fval;
   uint64_t seed;
+  /* ragged rows (all NULL / 0: the padded path) */
+  const int32_t* row_len;      /* LSA_STEP / LSA_CTX: device [B] characters of each row */
+  int32_t* row_done;           /* STOP_STEP / STOP_FLAG: device [B] done step of each row (-1 while running), in/out */
+  const int32_t* row_caps;     /* STOP_STEP / STOP_FLAG: device [B] decoder-step cap of each row */
+  const uint64_t* row_seeds;   /* FILL_MASKS_SEEDED: device [B] */
+  int32_t fma_chain;           /* GEMM / STOP_STEP: into GemmArgs::fma_chain (launch_gemm keeps to gemm32 / gemm64 / gemm_big) */
 } mb_taco_debug_spec;
 /* device workspace the spec needs (no kind needs scratch: a nominal 256 bytes), 0 for a spec mb_taco_debug refuses */
 size_t mb_taco_debug_workspace_bytes(const mb_taco_debug_spec* spec);

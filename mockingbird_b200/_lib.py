@@ -86,13 +86,14 @@ class TacoTcDebugSpec(C.Structure):
         ("s_hi", C.c_void_p * 2), ("s_lo", C.c_void_p * 2), ("s_k0", C.c_int32 * 2), ("nxt_hi", C.c_void_p * 2),
         ("nxt_lo", C.c_void_p * 2), ("act", C.c_int32), ("bn_scale", C.c_void_p), ("bn_shift", C.c_void_p),
         ("res", C.c_void_p), ("ldres", C.c_int32), ("compact", C.c_int32), ("cluster", C.c_int32), ("pdl", C.c_int32),
-        ("a_tiles", C.c_void_p), ("w_tiles", C.c_void_p),
+        ("a_tiles", C.c_void_p), ("w_tiles", C.c_void_p), ("len", C.c_void_p), ("t1", C.c_int32),
     ]
 
 
 MB_TACO_DBG = {k: i for i, k in enumerate((
     "gemm", "prenet", "gru_cell", "lstm_cell", "highway", "maxpool2", "embedding", "copy_cols", "lsa_step", "lsa_ctx",
-    "gst_attention", "stop_step", "stop_flag", "fill_masks", "fill_masks_steps", "pack_melproj", "to_ncl", "bn_fold"))}
+    "gst_attention", "stop_step", "stop_flag", "fill_masks", "fill_masks_steps", "pack_melproj", "to_ncl", "bn_fold",
+    "fill_masks_seeded"))}
 
 
 class TacoDebugSpec(C.Structure):
@@ -103,7 +104,8 @@ class TacoDebugSpec(C.Structure):
         ("bn_scale", C.c_void_p), ("bn_shift", C.c_void_p), ("mask", C.c_void_p), ("res", C.c_void_p), ("ldres", C.c_int32),
         ("y", C.c_void_p), ("ldy", C.c_int32), ("step_mode", C.c_int32), ("step_ptr", C.c_void_p), ("step_j", C.c_int32),
         ("x_step", C.c_int64), ("x_first", C.c_void_p), ("mask_step", C.c_int64), ("in_", C.c_void_p * 12),
-        ("out", C.c_void_p * 6), ("n", C.c_int64 * 10), ("fval", C.c_float), ("seed", C.c_uint64),
+        ("out", C.c_void_p * 6), ("n", C.c_int64 * 10), ("fval", C.c_float), ("seed", C.c_uint64), ("row_len", C.c_void_p),
+        ("row_done", C.c_void_p), ("row_caps", C.c_void_p), ("row_seeds", C.c_void_p), ("fma_chain", C.c_int32),
     ]
 
 

@@ -184,6 +184,7 @@ int mb_taco_tc_debug(const mb_taco_tc_debug_spec* spec, void* workspace, size_t 
     c.M = s.M;
     c.T = s.T;
     c.rows_total = (s.M + 127) / 128 * 128;
+    c.len = s.len;
     TK(launch_im2col_split(c, half_at(L.a_hi[0]), half_at(L.a_lo[0]), st));
     TcBigArgs t;
     memset(&t, 0, sizeof(t));
@@ -266,6 +267,8 @@ int mb_taco_tc_debug(const mb_taco_tc_debug_spec* spec, void* workspace, size_t 
     g.s_hi = (__half*)s.s_hi[0];
     g.s_lo = (__half*)s.s_lo[0];
     g.s_k0 = s.s_k0[0];
+    g.len1 = s.len;
+    g.t1 = s.t1;
     TK(launch_tc_gru(g, st, pdl, &info));
     kname = "tc_gru";
   } else {

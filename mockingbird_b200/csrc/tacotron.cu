@@ -188,10 +188,11 @@ __global__ void __launch_bounds__(512) lsa_step_kernel(const float* __restrict__
   }
   if (ctx == nullptr) return;  // context vector computed by lsa_ctx_kernel (more CTAs, vector loads)
   __syncthreads();
+  // t < len: a ragged row never reads the encoder sequence past its end (0 * seq[t] would be NaN there were seq[t] not finite)
   for (int f = tid; f < seq_dim; f += blockDim.x) {
     float a = 0.f;
     const float* sp = seq + (size_t)b * Tc * seq_dim + f;
-    for (int t = 0; t < Tc; ++t) a = fmaf(s_u[t], sp[(size_t)t * seq_dim], a);
+    for (int t = 0; t < len; ++t) a = fmaf(s_u[t], sp[(size_t)t * seq_dim], a);
     ctx[(size_t)b * seq_dim + f] = a;
   }
 }
@@ -1930,12 +1931,14 @@ GemmArgs debug_gemm_args(const mb_taco_debug_spec& s) {
   a.x_step = s.x_step;
   a.x_first = s.x_first;
   a.mask_step = s.mask_step;
+  a.fma_chain = s.fma_chain;
   return a;
 }
 
 int debug_check(const mb_taco_debug_spec& s) {
   const char* me = "mb_taco_debug";
-  if (s.kind < MB_TACO_DBG_GEMM || s.kind > MB_TACO_DBG_BN_FOLD) return fail(MB_ERR_INVALID, "%s: bad kind %d", me, s.kind);
+  if (s.kind < MB_TACO_DBG_GEMM || s.kind > MB_TACO_DBG_FILL_MASKS_SEEDED) return fail(MB_ERR_INVALID, "%s: bad kind %d", me, s.kind);
+  if ((s.row_done == nullptr) != (s.row_caps == nullptr)) return fail(MB_ERR_INVALID, "%s: row_done and row_caps go together", me);
   if (s.kind == MB_TACO_DBG_GEMM || s.kind == MB_TACO_DBG_STOP_STEP) {
     if (s.nseg < 1 || s.nseg > kMaxSeg || !s.W || !s.y || s.M <= 0 || s.N <= 0)
       return fail(MB_ERR_INVALID, "%s: GEMM nseg %d, M %d, N %d or a null operand", me, s.nseg, s.M, s.N);
@@ -1953,6 +1956,8 @@ int debug_check(const mb_taco_debug_spec& s) {
   }
   if (s.kind == MB_TACO_DBG_LSA_CTX && (s.n[2] <= 0 || s.n[2] % 256 || s.n[1] < 1))
     return fail(MB_ERR_INVALID, "%s: LSA_CTX seq_dim %lld must be a positive multiple of 256", me, (long long)s.n[2]);
+  if (s.kind == MB_TACO_DBG_FILL_MASKS_SEEDED && (!s.row_seeds || !s.out[0] || s.n[3] > 1))
+    return fail(MB_ERR_INVALID, "%s: FILL_MASKS_SEEDED needs row_seeds, m and dec 0 or 1", me);
   if (s.kind == MB_TACO_DBG_GST_ATTENTION && (s.n[1] < 1 || s.n[1] > 16 || s.n[3] < 1 || s.n[3] > 8 || s.n[2] % s.n[3]))
     return fail(MB_ERR_INVALID, "%s: GST ntok %lld (<= 16), heads %lld (<= 8, dividing E)", me, (long long)s.n[1], (long long)s.n[3]);
   return MB_OK;
@@ -2043,7 +2048,7 @@ int mb_taco_debug(const mb_taco_debug_spec* spec, void* workspace, size_t worksp
       MB_CUDA_CHECK(lsa_step_prepare(Tc));
       MB_CUDA_CHECK(launch_pdl2(lsa_step_kernel, dim3(B), dim3(threads), smem, st, fin(0), fin(1), fin(2), (int)n[2],
                                 reinterpret_cast<const int32_t*>(s.in[3]), fout(0), fin(4), fin(5), fin(6), fin(7), fout(1),
-                                (int)n[3], fout(2), Tc, s.step_ptr, s.step_j, fin(8), fin(9), fin(10), nullptr));
+                                (int)n[3], fout(2), Tc, s.step_ptr, s.step_j, fin(8), fin(9), fin(10), s.row_len));
       MB_LAUNCH_CHECK("lsa_step_kernel");
       info = {"lsa_step", B, 1, threads, smem};
       break;
@@ -2052,7 +2057,7 @@ int mb_taco_debug(const mb_taco_debug_spec* spec, void* workspace, size_t worksp
       const int B = (int)n[0], Tc = (int)n[1], seq_dim = (int)n[2];
       const size_t smem = sizeof(float) * Tc;
       MB_CUDA_CHECK(launch_pdl2(lsa_ctx_kernel, dim3(seq_dim / 256, B), dim3(256), smem, st, fin(0), (int)n[3], fin(1), seq_dim, Tc,
-                                fout(0), s.step_ptr, s.step_j, hout(1), hout(2), hout(3), hout(4), (int)n[4], nullptr));
+                                fout(0), s.step_ptr, s.step_j, hout(1), hout(2), hout(3), hout(4), (int)n[4], s.row_len));
       MB_LAUNCH_CHECK("lsa_ctx_kernel");
       info = {"lsa_ctx", seq_dim / 256, B, 256, smem};
       break;
@@ -2067,13 +2072,14 @@ int mb_taco_debug(const mb_taco_debug_spec* spec, void* workspace, size_t worksp
     case MB_TACO_DBG_STOP_STEP: {
       const int B = (int)n[0];
       stop_step_kernel<<<B, 256, 0, st>>>(debug_gemm_args(s), B, s.fval, (int)n[1], reinterpret_cast<int*>(s.out[0]), s.step_ptr,
-                                          s.step_j, reinterpret_cast<unsigned int*>(s.out[1]));
+                                          s.step_j, reinterpret_cast<unsigned int*>(s.out[1]), s.row_done, s.row_caps);
       MB_LAUNCH_CHECK("stop_step_kernel");
       info = {"stop_step", B, 1, 256, 0};
       break;
     }
     case MB_TACO_DBG_STOP_FLAG:
-      stop_flag_kernel<<<1, 32, 0, st>>>(fin(0), (int)n[0], s.fval, (int)n[1], reinterpret_cast<int*>(s.out[0]), s.step_ptr, s.step_j);
+      stop_flag_kernel<<<1, 32, 0, st>>>(fin(0), (int)n[0], s.fval, (int)n[1], reinterpret_cast<int*>(s.out[0]), s.step_ptr, s.step_j,
+                                         s.row_done, s.row_caps);
       MB_LAUNCH_CHECK("stop_flag_kernel");
       info = {"stop_flag", 1, 1, 32, 0};
       break;
@@ -2104,6 +2110,14 @@ int mb_taco_debug(const mb_taco_debug_spec* spec, void* workspace, size_t worksp
       MB_LAUNCH_CHECK("bn_fold_kernel");
       info = {"bn_fold", (int)blocks(n[0]), 1, 256, 0};
       break;
+    case MB_TACO_DBG_FILL_MASKS_SEEDED: {
+      const int64_t count = 2 * n[0] * n[1] * n[2];
+      fill_masks_seeded_kernel<<<blocks(count), 256, 0, st>>>(reinterpret_cast<uint8_t*>(s.out[0]), (int)n[0], (int)n[1], (int)n[2],
+                                                              s.row_seeds, (int)n[3]);
+      MB_LAUNCH_CHECK("fill_masks_seeded_kernel");
+      info = {"fill_masks_seeded", (int)blocks(count), 1, 256, 0};
+      break;
+    }
   }
   if (report && report_len)
     snprintf(report, report_len, "kernel=%s grid=%d,%d block=%d smem=%zu\n", info.kernel, info.grid_x, info.grid_y, info.block,

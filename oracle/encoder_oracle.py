@@ -49,3 +49,31 @@ def embed_utterance_partials(sd: Dict[str, torch.Tensor], partial_frames: torch.
     pe = embed_frames(sd, partial_frames).numpy()
     raw = np.mean(pe, axis=0)
     return raw / np.linalg.norm(raw, 2)
+
+
+def reduce_partials(partial, offsets):
+    """inference.py:164-166 per utterance u (partials offsets[u] .. offsets[u + 1]): e = mean of its partial embeddings, e / |e|,
+    in float64, with the bound of an fp32 evaluation in any summation order (n partials, E features, u = 2^-24):
+    mean: gamma(n + 2) sum |p| / n (n - 1 additions, the rounded 1 / n and the product); |e|^2: gamma(E + 6) |e|^2 plus the
+    propagated 2 sum |e_j| d_j; 1 / sqrt: half the relative error of |e|^2 and 3 u (sqrt, reciprocal); the product one u."""
+    p = np.asarray(partial, np.float64)
+    off = np.asarray(offsets)
+    U, E = len(off) - 1, p.shape[1]
+    u24 = 2.0 ** -24
+
+    def gamma(n):
+        return n * u24 / (1 - n * u24)
+
+    out, bound = np.zeros((U, E)), np.zeros((U, E))
+    for i in range(U):
+        blk = p[off[i]:off[i + 1]]
+        n = blk.shape[0]
+        mean = blk.mean(0)
+        dm = gamma(n + 2) * np.abs(blk).sum(0) / n
+        ss = float(mean @ mean)
+        dss = gamma(E + 6) * ss + 2 * float(np.abs(mean) @ dm) + float(dm @ dm)
+        inv = 1.0 / np.sqrt(ss)
+        dinv = inv * (dss / ss / 2 * 1.01 + 3 * u24)
+        out[i] = mean * inv
+        bound[i] = dm * inv + np.abs(mean) * dinv + u24 * np.abs(out[i])
+    return out, bound

@@ -222,6 +222,40 @@ def context(s, seq, ds=None):
     return c, d
 
 
+def lsa_step_rows(row_len, proj, seq, chars, cum, pq=None, q_in=None, ctx=True, **kw):
+    """LSA step of a ragged batch in the reference's per-utterance semantics: row b is the B = 1 utterance of its first
+    row_len[b] characters, unpadded (lsa_step on the row cut to its length, whose location conv pads with zeros past the end).
+    Positions t >= row_len[b] are not part of the utterance: their score is exactly 0 (bound 0) and their cumulative
+    attention is the input's (bound 0).  Same arguments and result as lsa_step."""
+    B, Tc = np.asarray(chars).shape
+    S = np.asarray(seq).shape[2]
+    out = {"scores": (np.zeros((B, Tc)), np.zeros((B, Tc))), "cum": (_f64(cum).copy(), np.zeros((B, Tc)))}
+    if ctx:
+        out["ctx"] = (np.zeros((B, S)), np.zeros((B, S)))
+    for b in range(B):
+        n = int(row_len[b])
+        one = lsa_step(pq=None if pq is None else pq[b:b + 1], proj=proj[b:b + 1, :n], seq=seq[b:b + 1, :n],
+                       chars=np.asarray(chars)[b:b + 1, :n], cum=np.asarray(cum)[b:b + 1, :n],
+                       q_in=None if q_in is None else q_in[b:b + 1], ctx=ctx, **kw)
+        for k, (v, d) in one.items():
+            if k == "ctx":
+                out[k][0][b], out[k][1][b] = v[0], d[0]
+            else:
+                out[k][0][b, :n], out[k][1][b, :n] = v[0], d[0]
+    return out
+
+
+def context_rows(s, seq, row_len, ds=None):
+    """context of a ragged batch: row b is context() of its first row_len[b] scores and encoder rows"""
+    s = _f64(s)
+    c, d = np.zeros((s.shape[0], np.asarray(seq).shape[2])), np.zeros((s.shape[0], np.asarray(seq).shape[2]))
+    for b in range(s.shape[0]):
+        n = int(row_len[b])
+        cb, db = context(s[b:b + 1, :n], np.asarray(seq)[b:b + 1, :n], None if ds is None else ds[b:b + 1, :n])
+        c[b], d[b] = cb[0], db[0]
+    return c, d
+
+
 # ---- global style token attention (gst_attention_kernel) -----------------------------------------------------------------
 def gst_attention(q, keys, values, heads):
     """multi-head attention of global_style_token.py:110-145 for one query per row: scores = q_h k_h / sqrt(E / heads),
@@ -256,6 +290,24 @@ def stop_value(xs, w, bias):
 def stop_flag(stopv, min_stop_token, step, r):
     """tacotron.py:275: stop when every row's stop * 10 > min_stop_token and the frame index step * r > 10"""
     return int(bool(np.all(np.asarray(stopv, np.float32) * np.float32(10) > np.float32(min_stop_token))) and step * r > 10)
+
+
+def stop_rows(stopv, min_stop_token, r, caps):
+    """per-row stop rule of a ragged batch, as the B = 1 decoder loop of tacotron.py:268-276 would break for each utterance:
+    stopv [n_steps][B] stop values of decoder steps 0 ..; row b's loop runs si = 0 .. caps[b] - 1 (frame t = si * r, caps[b] =
+    ceil(steps_b / r)) and breaks at the first si with stop * 10 > min_stop_token and t > 10.  Returns (done [B], flags
+    [n_steps]): done[b] = the step the row's loop ends at (its last step, caps[b] - 1, without a break; -1 when it has not ended
+    within n_steps), flags[si] = 1 when every row has ended by step si"""
+    v = np.asarray(stopv, np.float32)
+    n_steps, B = v.shape
+    done = np.full(B, -1)
+    for b in range(B):
+        for si in range(min(int(caps[b]), n_steps)):
+            if (v[si, b] * np.float32(10) > np.float32(min_stop_token) and si * r > 10) or si == int(caps[b]) - 1:
+                done[b] = si
+                break
+    flags = np.array([int(np.all((done >= 0) & (done <= si))) for si in range(n_steps)])
+    return done, flags
 
 
 # ---- BN fold, layout kernels ---------------------------------------------------------------------------------------------
@@ -312,3 +364,22 @@ def fill_masks(n, seed, stream_id, first=0):
 def fill_masks_steps(n_per_step, n_steps, seed):
     """fill_masks_steps_kernel: step s of all decoder steps uses stream_id = s"""
     return np.concatenate([fill_masks(n_per_step, seed, s) for s in range(n_steps)])
+
+
+SEEDED_TAG = 0x72616767  # counter word 3 of the per-utterance dropout streams of ragged batches ("ragg")
+
+
+def seeded_masks(seed, npos, units, dec):
+    """one utterance's PreNet keep flags [2 layers][npos][units] drawn with its own seed (fill_masks_seeded_kernel): bit 16 of
+    word (u & 3) of Philox((u >> 2, position, 2 dec + layer, "ragg"), (seed lo, seed hi)); position = character (dec 0, the
+    encoder PreNet) or decoder step (dec 1).  Nothing depends on the row or the batch."""
+    l, pos, u = np.meshgrid(np.arange(2), np.arange(npos), np.arange(units), indexing="ij")
+    o = philox4x32(u >> 2, pos, 2 * dec + l, SEEDED_TAG, seed & 0xFFFFFFFF, seed >> 32)
+    words = np.choose(u & 3, o)
+    return ((words >> np.uint32(16)) & np.uint32(1)).astype(np.uint8)
+
+
+def fill_masks_seeded(seeds, npos, units, dec):
+    """the kernel's layouts of the per-utterance flags: dec 0 [2][B][npos][units], dec 1 [npos][2][B][units]"""
+    m = np.stack([seeded_masks(int(s), npos, units, dec) for s in seeds], 1)  # [2][B][npos][units]
+    return m if dec == 0 else np.ascontiguousarray(m.transpose(2, 0, 1, 3))

@@ -225,6 +225,35 @@ def im2col(xs, shifts, K, M, T):
     return out
 
 
+def im2col_rows(xs, shifts, K, M, T, lens):
+    """im2col of a ragged batch in per-utterance semantics: sequence j (rows j T ..) is an utterance of its first lens[j] rows
+    (clipped at row M), and its rows are im2col of that utterance alone, unpadded (T = its length: taps read zeros past its end).
+    Rows past an utterance's end belong to no utterance and are NaN."""
+    out = np.full((M, len(xs) * K), np.nan, np.float32)
+    for j in range((M + T - 1) // T):
+        r0 = j * T
+        n = min(int(lens[j]), M - r0)
+        if n > 0:
+            out[r0:r0 + n] = im2col([np.asarray(x, np.float32)[r0:r0 + n] for x in xs], shifts, K, n, n)
+    return out
+
+
+def gru_reverse_rows(gi, W, b, lens):
+    """backward direction of a GRU over a ragged batch, float64: row m is the reverse recurrence of its own first lens[m]
+    steps, started from h = 0 at its last step t = lens[m] - 1 (gh = W h + b, gi [M][T][3H] = W_ih x_t + b_ih).  Steps at and past
+    the row's end are not part of it: h = 0 there.  -> [M][T][H]"""
+    gi = _f64(gi)
+    M, T, H3 = gi.shape
+    H = H3 // 3
+    out = np.zeros((M, T, H))
+    for m in range(M):
+        h = np.zeros((1, H))
+        for t in range(int(lens[m]) - 1, -1, -1):
+            h = gru_cell(_f64(h) @ _f64(W).T + _f64(b), gi[m:m + 1, t], h, H)
+            out[m, t] = h[0]
+    return out
+
+
 def unpack_act_tiles(tiles, rows_pad, KB):
     """fp16 [KB][rows_pad][64] with 16-byte chunks at c8 ^ (m & 7) -> [rows_pad][KB * 64]"""
     t = np.asarray(tiles).reshape(KB, rows_pad, 8, 8)

@@ -277,3 +277,139 @@ def test_fill_masks_known_bits():
     hi = ko.fill_masks(8, 7, 0, first=1 << 34)
     o = ko.philox4x32(np.arange(2), 1, 0, ko.MASK_TAG, 7, 0)
     assert [int((o[i & 3][i >> 2] >> 16) & 1) for i in range(8)] == hi.tolist()
+
+
+# ---- ragged batches: each row is the B = 1 utterance of its own length -----------------------------------------------------
+def test_lsa_step_rows_is_each_row_alone():
+    """the ragged LSA step of a row is torch's LSA step on that row alone, cut to its length; past the end the score is 0 and
+    the cumulative attention untouched.  The padded-batch row (positions past the end scored as chars == 0) is rejected."""
+    a = _lsa_inputs(11, B=3, Tc=40)
+    lens = np.array([40, 23, 1])
+    a["chars"] = np.where(np.arange(40)[None, :] < lens[:, None], 9, 0)
+    a["chars"][0, 5] = 0  # a zero character inside the row: scored as exp(0), as in the reference
+    a["cum"][np.arange(40)[None, :] >= lens[:, None]] = 0
+    ref = ko.lsa_step_rows(lens, **a)
+    for b, n in enumerate(lens):
+        one = {k: (v[b:b + 1, :n] if k in ("proj", "seq", "chars", "cum") else v[b:b + 1] if k == "pq" else v) for k, v in a.items()}
+        s, cum, ctx = _lsa_torch(one)
+        _accept("lsa rows scores", s, ref["scores"][0][b:b + 1, :n], ref["scores"][1][b:b + 1, :n])
+        _accept("lsa rows cum", cum, ref["cum"][0][b:b + 1, :n], ref["cum"][1][b:b + 1, :n])
+        _accept("lsa rows ctx", ctx, ref["ctx"][0][b:b + 1], ref["ctx"][1][b:b + 1])
+        assert not ref["scores"][0][b, n:].any() and not ref["scores"][1][b, n:].any()
+        assert np.array_equal(ref["cum"][0][b, n:], a["cum"][b, n:]) and not ref["cum"][1][b, n:].any()
+    padded = ko.lsa_step(**a)
+    _reject("padded-batch row scores", padded["scores"][0][1:2], ref["scores"][0][1:2], ref["scores"][1][1:2])
+    cs, cd = ko.context_rows(ref["scores"][0], a["seq"], lens, ref["scores"][1])
+    assert np.array_equal(cs, ref["ctx"][0]) and np.array_equal(cd, ref["ctx"][1])
+
+
+def test_stop_rows():
+    """the per-row stop rule as the B = 1 loop breaks: at the first step with stop * 10 > min_stop and t = si r > 10, else at the
+    cap; a row that passed at t <= 10 and fails later does not end; flags once every row has ended"""
+    r, mst = 2, 5.0
+    v = np.full((10, 5), 0.4, np.float32)
+    v[:, 1] = 0.9  # passes from the start: ends at si = 6 (t = 12), not 5 (t = 10)
+    v[:6, 2] = 0.9  # passes while t <= 10, fails after: runs to its cap
+    v[8:, 3] = 0.9
+    caps = np.array([1, 20, 9, 20, 20])
+    done, flags = ko.stop_rows(v, mst, r, caps)
+    assert done.tolist() == [0, 6, 8, 8, -1]
+    assert flags.tolist() == [0] * 10
+    done, flags = ko.stop_rows(v[:, :4], mst, r, caps[:4])
+    assert flags.tolist() == [0] * 8 + [1, 1]
+    # B = 1 rows agree with the padded rule's flag at the step they end (stop_flag), and a batch of one row is its own loop
+    for b in range(4):
+        d, f = ko.stop_rows(v[:, b:b + 1], mst, r, caps[b:b + 1])
+        assert d[0] == done[b] and f[d[0]] == 1 and not f[:d[0]].any()
+        if d[0] < caps[b] - 1:
+            assert ko.stop_flag(v[d[0], b:b + 1], mst, d[0], r) == 1
+
+
+def test_seeded_masks_bits_and_independence():
+    """fill_masks_seeded: bit 16 of word (u & 3) of Philox((u >> 2, position, 2 dec + layer, "ragg"), seed); an utterance's flags
+    do not depend on its row, the batch or npos, and differ from the padded path's "taco" streams and from a swapped counter"""
+    seed = 0x123456789ABCDEF0
+    m = ko.seeded_masks(seed, 7, 12, 1)
+    o = ko.philox4x32(5 >> 2, 3, 2 * 1 + 1, ko.SEEDED_TAG, seed & 0xFFFFFFFF, seed >> 32)
+    assert m[1, 3, 5] == (int(o[5 & 3]) >> 16) & 1
+    seeds = [7, seed, 0]
+    for dec in (0, 1):
+        lay = ko.fill_masks_seeded(seeds, 9, 16, dec)
+        wide = ko.fill_masks_seeded([3] + seeds, 11, 16, dec)
+        for b, s in enumerate(seeds):
+            own = ko.seeded_masks(s, 9, 16, dec)
+            got = lay[:, b] if dec == 0 else lay[:, :, b].transpose(1, 0, 2)
+            got_w = wide[:, b + 1, :9] if dec == 0 else wide[:9, :, b + 1].transpose(1, 0, 2)
+            assert np.array_equal(got, own) and np.array_equal(got_w, own)
+    l, pos, u = np.meshgrid(np.arange(2), np.arange(9), np.arange(16), indexing="ij")
+    sw = ko.philox4x32(pos >> 2, u, l, ko.SEEDED_TAG, 7, 0)
+    swapped = ((np.choose(u & 3, sw) >> np.uint32(16)) & np.uint32(1)).astype(np.uint8)
+    assert not np.array_equal(swapped, ko.seeded_masks(7, 9, 16, 0))
+    assert 0.4 < ko.seeded_masks(7, 64, 256, 0).mean() < 0.6
+
+
+def test_im2col_rows_is_each_utterance_alone():
+    """im2col with per-sequence lengths @ the tap weights = torch's zero-padded Conv1d of each utterance alone; the padded
+    batch's im2col (taps reading the rows past the end) is rejected"""
+    import tc_split_oracle as so
+
+    g = _g(12)
+    T, Ci, Co, k = 9, 6, 5, 4
+    lens = [9, 1, 5, 2]
+    M = T * 3 + 2  # a last, partial sequence of 2 rows
+    x = _f32(g.standard_normal((M, Ci)))
+    W = _f32(g.standard_normal((Co, Ci, k)))
+    shifts = [j - k // 2 for j in range(k)]
+    A = so.im2col_rows([x] * k, shifts, Ci, M, T, lens)
+    Wc = np.concatenate([W[:, :, j] for j in range(k)], 1)
+    got = np.asarray(A, np.float64) @ np.asarray(Wc, np.float64).T
+    for j, n in enumerate(lens):
+        r0 = j * T
+        xc = _t(x[r0:r0 + n]).T[None]
+        ref = F.conv1d(F.pad(xc, (k // 2, k - 1 - k // 2)), _t(W))[0].T.numpy()
+        bound = np.abs(np.asarray(A[r0:r0 + n], np.float64)) @ np.abs(np.asarray(Wc, np.float64)).T * ko.gamma(Ci * k)
+        _accept("im2col rows", ref, got[r0:r0 + n], bound + 1e-300)
+        assert np.isnan(A[r0 + n:(j + 1) * T]).all()
+    padded = np.asarray(so.im2col([x] * k, shifts, Ci, M, T), np.float64) @ np.asarray(Wc, np.float64).T
+    _reject("padded im2col", padded[T:T + 1], got[T:T + 1], np.abs(got[T:T + 1]) * 1e-6)
+
+
+def test_gru_reverse_rows_is_each_row_alone():
+    """the backward GRU of a ragged batch = torch's GRU run over each row's own steps reversed, from h = 0"""
+    import tc_split_oracle as so
+
+    g = _g(13)
+    M, T, H, Ki = 4, 7, 8, 5
+    lens = [7, 1, 2, 4]
+    x = _f32(g.standard_normal((M, T, Ki)))
+    gru = torch.nn.GRU(Ki, H, batch_first=True)
+    with torch.no_grad():
+        for p in gru.parameters():
+            p.copy_(_t(_f32(g.standard_normal(tuple(p.shape)) * 0.5)))
+    gi = F.linear(_t(x), gru.weight_ih_l0, gru.bias_ih_l0).detach().numpy()
+    ref = so.gru_reverse_rows(gi, gru.weight_hh_l0.detach().numpy(), gru.bias_hh_l0.detach().numpy(), lens)
+    for m, n in enumerate(lens):
+        with torch.no_grad():
+            y, _ = gru(_t(x[m:m + 1, :n]).flip(1))
+        _accept("gru reverse rows", y.flip(1)[0].numpy(), ref[m, :n], 1e-5 * (1 + np.abs(ref[m, :n])))
+        assert not ref[m, n:].any()
+    padded, _ = gru(_t(x[1:2]).flip(1))
+    _reject("backward GRU from the padded end", padded.flip(1)[0, :1].detach().numpy(), ref[1, :1], 1e-5 * np.ones((1, H)))
+
+
+def test_reduce_partials():
+    """L2(mean of the partials) per utterance: the bound accepts a float32 numpy evaluation and rejects the unnormalised mean"""
+    import encoder_oracle as eo
+
+    g = _g(14)
+    E = 100
+    counts = [1, 2, 600, 3]
+    off = np.concatenate([[0], np.cumsum(counts)])
+    p = _f32(np.abs(g.standard_normal((off[-1], E))))
+    p /= np.linalg.norm(p, axis=1, keepdims=True)
+    ref, bound = eo.reduce_partials(p, off)
+    for u in range(len(counts)):
+        raw = np.mean(p[off[u]:off[u + 1]], axis=0, dtype=np.float32)
+        _accept("reduce partials", raw / np.linalg.norm(raw, 2), ref[u:u + 1], bound[u:u + 1])
+    raw = np.mean(p[off[2]:off[3]], axis=0)
+    _reject("mean without the norm", raw[None], ref[2:3], bound[2:3])
