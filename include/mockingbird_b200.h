@@ -172,11 +172,32 @@ typedef struct mb_gan_debug_spec {
   float* y;            /* running sum in (modes 1, 2), result out; may be NULL in mode 0 */
   float* y16;          /* out16: the plane read back, C16 = Cout (plain) or the hi/lo plane's
                           channels (2 Cout, at least 64): hi channels first, then lo */
+  /* mb_gan_debug_f32 only (zero / NULL: NCL everywhere, no second destination).  The layouts say how
+   * the kernel sees its tensors; the caller's tensors are fp32 NCL either way and are converted. */
+  int32_t x_layout;    /* 0 / 1 NCL fp32, 2 channel-quad blocked fp32, 3 fp16 plane (activated
+                          with the layer's input slope when converted, as the forward writes it) */
+  int32_t y_layout;    /* residual / y / y2 as the kernel sees them: 0 / 1 NCL fp32, 2 blocked fp32 */
+  float* y2;           /* second destination [B, Cout, L*stride]: running sum in, y2 + v out (NULL: none) */
+  int32_t y2_out16;    /* fp16 plane of the second destination: 0 none, 1 plain, 2 hi/lo */
+  float y2_slope;      /* leaky-relu slope of that plane */
+  float* y2_16;        /* y2_out16: the plane read back (mb_gan_debug_f32 sizes both y16 and y2_16 as the
+                          forward sizes the planes of its FP32 layers: Cout plain, 2 Cout hi/lo) */
 } mb_gan_debug_spec;
 /* writes one line per kernel launch into `report`:
  * "kernel=N,MT,CW,PAIR rows_item= resident= wstages= n_work= grid= red_add=" */
 int mb_gan_debug_launch(mb_gan* h, const mb_gan_debug_spec* spec, void* workspace, size_t workspace_bytes,
                         void* stream, char* report, size_t report_len);
+
+/* test hook: op `layer_index` of any handle (fp32, f16tc, f16x3) run once on the FP32 kernels, with the
+ * caller's epilogue inputs and outputs (pair, red_add and res_kind 2 / 3 are refused).  An add op
+ * (mb_gan_layer_info "add ...") computes y += x and refreshes the fp16 plane out16 = lrelu(y, out_slope).
+ * post_variant picks the Cout = 1 kernel: MB_GAN_POST_DEFAULT (the MB_POST_* switches), 1 / 2 / 4
+ * output rows per thread, or MB_GAN_POST_TILE; other ops take MB_GAN_POST_DEFAULT.  Writes
+ * "kernel=NAME" into `report`: tapconv_f32, cout1<R>, post_tile<7,CQ>, add or add_dst16. */
+#define MB_GAN_POST_DEFAULT 0
+#define MB_GAN_POST_TILE (-1)
+int mb_gan_debug_f32(mb_gan* h, const mb_gan_debug_spec* spec, int32_t post_variant, void* workspace,
+                     size_t workspace_bytes, void* stream, char* report, size_t report_len);
 
 /* ---------------------------------------------------------------------------------------------
  * fatchord WaveRNN

@@ -64,6 +64,12 @@ class GanDebugSpec(C.Structure):
         ("lengths", C.c_void_p),
         ("y", C.c_void_p),
         ("y16", C.c_void_p),
+        ("x_layout", C.c_int32),
+        ("y_layout", C.c_int32),
+        ("y2", C.c_void_p),
+        ("y2_out16", C.c_int32),
+        ("y2_slope", C.c_float),
+        ("y2_16", C.c_void_p),
     ]
 
 
@@ -219,6 +225,8 @@ SIGNATURES = {
     "mb_gan_tc_plan_info": (C.c_int, [C.c_void_p, C.c_int32, C.c_char_p, C.c_size_t]),
     "mb_gan_debug_launch": (C.c_int, [C.c_void_p, C.POINTER(GanDebugSpec), C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p,
                                       C.c_size_t]),
+    "mb_gan_debug_f32": (C.c_int, [C.c_void_p, C.POINTER(GanDebugSpec), C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p,
+                                   C.c_char_p, C.c_size_t]),
     "mb_wavernn_create": (C.c_int, [C.POINTER(WaveRNNConfig), C.POINTER(C.c_void_p)]),
     "mb_wavernn_create_mode": (C.c_int, [C.POINTER(WaveRNNConfig), C.c_int32, C.POINTER(C.c_void_p)]),
     "mb_wavernn_destroy": (None, [C.c_void_p]),

@@ -5,6 +5,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "gan_kernels.h"
@@ -822,6 +823,118 @@ int mb_gan_debug_launch(mb_gan* h, const mb_gan_debug_spec* s, void* workspace, 
       used += (size_t)w;
     }
   }
+  return MB_OK;
+}
+
+int mb_gan_debug_f32(mb_gan* h, const mb_gan_debug_spec* s, int32_t post_variant, void* workspace, size_t workspace_bytes,
+                     void* stream, char* report, size_t report_len) {
+  if (!h || !s || !workspace || !s->x) return fail(MB_ERR_INVALID, "mb_gan_debug_f32: null argument");
+  const int32_t i = s->layer_index;
+  if (i < 0 || i >= (int32_t)h->layers.size()) return fail(MB_ERR_INVALID, "mb_gan_debug_f32: bad layer %d", i);
+  const Layer& L = h->layers[i];
+  if (s->pair || s->red_add) return fail(MB_ERR_INVALID, "mb_gan_debug_f32: pairs and red.global.add are tensor-core launches");
+  if (s->mode < EPI_STORE || s->mode > EPI_ADD_DIV) return fail(MB_ERR_INVALID, "mb_gan_debug_f32: bad mode %d", s->mode);
+  if (s->res_kind != 0 && s->res_kind != 1)
+    return fail(MB_ERR_INVALID, "mb_gan_debug_f32: the FP32 kernels take an fp32 residual only (res_kind %d)", s->res_kind);
+  if (s->res_kind == 1 && !s->residual) return fail(MB_ERR_INVALID, "mb_gan_debug_f32: res_kind 1 without residual");
+  if (s->out16 < 0 || s->out16 > 2 || s->y2_out16 < 0 || s->y2_out16 > 2 || (s->out16 && !s->y16) ||
+      (s->y2_out16 && (!s->y2_16 || !s->y2)))
+    return fail(MB_ERR_INVALID, "mb_gan_debug_f32: bad fp16 output planes");
+  if (s->mode != EPI_STORE && !s->y) return fail(MB_ERR_INVALID, "mb_gan_debug_f32: accumulate mode without y");
+  if (s->batch <= 0 || s->frames_in <= 0) return fail(MB_ERR_INVALID, "mb_gan_debug_f32: empty batch");
+  if (L.kind == OP_CONV && (!L.w_set || !L.b_set))
+    return fail(MB_ERR_STATE, "mb_gan_debug_f32: weights of %s not set", L.name.c_str());
+  const bool cout1 = L.kind == OP_CONV && L.cout == 1 && L.taps.stride == 1;
+  if (post_variant != MB_GAN_POST_DEFAULT && !cout1)
+    return fail(MB_ERR_INVALID, "mb_gan_debug_f32: post_variant applies to Cout = 1 layers only");
+  const int B = s->batch, Lin = s->frames_in, mult = L.rate_out / L.rate_in, Lout = Lin * mult;
+  const int Cin = L.kind == OP_CONV ? L.cin : L.cout, Cout = L.cout;
+  const int xl = s->x_layout ? s->x_layout : LAYOUT_NCL, yl = s->y_layout ? s->y_layout : LAYOUT_NCL;
+  auto bad_f16 = [](int C) { return C % 8 != 0 || C % f16_cw(C) != 0; };
+  if (xl < LAYOUT_NCL || xl > LAYOUT_F16B || (xl == LAYOUT_F32B && Cin % 4) || (xl == LAYOUT_F16B && bad_f16(Cin)) ||
+      (yl != LAYOUT_NCL && yl != LAYOUT_F32B) || (yl == LAYOUT_F32B && Cout % 4))
+    return fail(MB_ERR_INVALID, "mb_gan_debug_f32: layouts x=%d y=%d do not fit %s (%d -> %d channels)", xl, yl, L.name.c_str(), Cin,
+                Cout);
+  // a hi/lo plane has 2 Cout channels, as tc_forward sizes the planes the FP32 kernels write (lo of channel c at c + Cout)
+  const int c16 = s->out16 == 2 ? 2 * Cout : Cout, c2_16 = s->y2_out16 == 2 ? 2 * Cout : Cout;
+  if ((s->out16 && bad_f16(c16)) || (s->y2_out16 && bad_f16(c2_16)))
+    return fail(MB_ERR_INVALID, "mb_gan_debug_f32: no fp16 plane of %d channels", Cout);
+  if (L.kind != OP_CONV && (xl != yl || !s->y || s->residual || s->y2 || s->mode != EPI_STORE))
+    return fail(MB_ERR_INVALID, "mb_gan_debug_f32: an add op takes x and y in one layout, mode 0, no residual or y2");
+  // workspace: converted planes of x, residual, y, y2 and the fp16 outputs (zeroed: fp16 pad rows read as 0)
+  auto f16b = [&](int C, int Lr) { return align_up((size_t)B * C * f16_lp(Lr) * 2, 1024); };
+  auto f32b = [&](int C, int Lr) { return align_up((size_t)B * C * Lr * 4, 1024); };
+  const size_t b_x = xl == LAYOUT_F16B ? f16b(Cin, Lin) : (xl == LAYOUT_F32B ? f32b(Cin, Lin) : 0);
+  const size_t b_y = yl == LAYOUT_F32B ? f32b(Cout, Lout) : 0;
+  const size_t b_16 = s->out16 ? f16b(c16, Lout) : 0, b_2_16 = s->y2_out16 ? f16b(c2_16, Lout) : 0;
+  const size_t need = b_x + 3 * b_y + b_16 + b_2_16;
+  if (workspace_bytes < need + 1024)
+    return fail(MB_ERR_WORKSPACE, "mb_gan_debug_f32: workspace %zu < %zu bytes", workspace_bytes, need + 1024);
+  cudaStream_t st = (cudaStream_t)stream;
+  char* ws = (char*)(((uintptr_t)workspace + 1023) & ~(uintptr_t)1023);
+  if (need) MB_CUDA_CHECK(cudaMemsetAsync(ws, 0, need, st));
+  auto ref = [](const void* p, int layout, int C, int Lr) {
+    TRef t = ncl(p, C, Lr);
+    if (p) t.layout = layout;
+    return t;
+  };
+  const TRef x_ncl = ncl(s->x, Cin, Lin), res_ncl = ncl(s->res_kind ? s->residual : nullptr, Cout, Lout),
+             y_ncl = ncl(s->y, Cout, Lout), y2_ncl = ncl(s->y2, Cout, Lout);
+  char* p = ws;
+  const TRef x = xl == LAYOUT_NCL ? x_ncl : ref(p, xl, Cin, Lin);
+  p += b_x;
+  const TRef res = yl == LAYOUT_NCL ? res_ncl : ref(res_ncl.p ? p : nullptr, yl, Cout, Lout);
+  const TRef y32 = yl == LAYOUT_NCL ? y_ncl : ref(y_ncl.p ? p + b_y : nullptr, yl, Cout, Lout);
+  const TRef y2 = yl == LAYOUT_NCL ? y2_ncl : ref(y2_ncl.p ? p + 2 * b_y : nullptr, yl, Cout, Lout);
+  p += 3 * b_y;
+  TRef y16 = ref(s->out16 ? p : nullptr, LAYOUT_F16B, c16, Lout);
+  y16.hilo = s->out16 == 2;
+  p += b_16;
+  TRef y2_16 = ref(s->y2_out16 ? p : nullptr, LAYOUT_F16B, c2_16, Lout);
+  y2_16.hilo = s->y2_out16 == 2;
+  const float x_slope = (L.kind == OP_CONV && xl == LAYOUT_F16B) ? L.taps.in_slope : 1.f;
+  std::vector<std::pair<TRef, TRef>> in = {{x_ncl, x}, {res_ncl, res}, {y_ncl, y32}, {y2_ncl, y2}};
+  for (const auto& c : in) {
+    if (!c.first.p || c.first.p == c.second.p) continue;
+    cudaError_t e = launch_convert_layout(c.first, c.second, B, &c == &in[0] ? x_slope : 1.f, st);
+    if (e != cudaSuccess) return fail(MB_ERR_CUDA, "mb_gan_debug_f32: convert: %s", cudaGetErrorString(e));
+  }
+  const char* kernel = "tapconv_f32";
+  cudaError_t e;
+  if (L.kind != OP_CONV) {
+    kernel = y16.p ? "add_dst16" : "add";
+    e = launch_add_inplace_f32(y32, x, y16, s->out_slope, B, st);
+  } else {
+    TapConv tp = L.taps;
+    tp.B = B;
+    tp.Lin = Lin;
+    tp.Lout = Lout;
+    tp.lengths = s->lengths;
+    tp.len_mul_in = 1;
+    tp.len_mul_out = mult;
+    tp.mode = s->mode;
+    tp.div = s->div;
+    TapConvIO io;
+    io.x = x;
+    io.res = res;
+    io.y32 = y32;
+    io.y16 = y16;
+    io.out16_slope = s->out_slope;
+    io.y2_32 = y2;
+    io.y2_16 = y2_16;
+    io.y2_16_slope = s->y2_slope;
+    e = cout1 ? launch_tapconv_cout1_f32(tp, io, h->arena + L.w_off, h->arena + L.b_off, st, post_variant, &kernel)
+              : launch_tapconv_f32(tp, io, h->arena + L.w_off, h->arena + L.b_off, st);
+  }
+  if (e != cudaSuccess) return fail(MB_ERR_CUDA, "mb_gan_debug_f32 (%s): %s", L.name.c_str(), cudaGetErrorString(e));
+  count_launch();
+  std::vector<std::pair<TRef, TRef>> out = {{y32, y_ncl}, {y2, y2_ncl}, {y16, ncl(s->y16, c16, Lout)}, {y2_16, ncl(s->y2_16, c2_16, Lout)}};
+  for (const auto& c : out) {
+    if (!c.first.p || c.first.p == c.second.p) continue;
+    e = launch_convert_layout(c.first, c.second, B, 1.f, st);
+    if (e != cudaSuccess) return fail(MB_ERR_CUDA, "mb_gan_debug_f32: convert: %s", cudaGetErrorString(e));
+  }
+  if (report && report_len) snprintf(report, report_len, "kernel=%s\n", kernel);
   return MB_OK;
 }
 

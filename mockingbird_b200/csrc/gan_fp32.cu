@@ -363,9 +363,13 @@ cudaError_t launch_tapconv_f32(const TapConv& p, const TapConvIO& io, const floa
 }
 
 cudaError_t launch_tapconv_cout1_f32(const TapConv& p, const TapConvIO& io, const float* w, const float* bias,
-                                     cudaStream_t stream) {
+                                     cudaStream_t stream, int variant, const char** kernel) {
   if (p.Cout != 1 || p.stride != 1) return cudaErrorInvalidValue;
-  {
+  const int nt = p.ntaps[0];
+  bool contiguous = true;
+  for (int t = 1; t < nt; ++t) contiguous = contiguous && (p.off[0][t] == p.off[0][0] + t);
+  const bool tile_fits = nt == 7 && contiguous && io.x.layout == LAYOUT_F32B && (p.Cin == 32 || p.Cin == 16);
+  if (variant == kCout1Default) {
     // MB_POST_TILE=1: shared-memory tile kernel for the F32B plane with 7 contiguous taps (conv_post of both generators).  Default 0:
     // bit-identical output but MEASURED SLOWER than the R-rows-per-thread kernel (0.123 vs 0.099 ms; 0.191 ms before the staging loads
     // were batched eight per thread): three 67 KB blocks per SM alternate between a load phase and a compute phase and keep fewer bytes in
@@ -374,35 +378,37 @@ cudaError_t launch_tapconv_cout1_f32(const TapConv& p, const TapConvIO& io, cons
       const char* e = getenv("MB_POST_TILE");
       return e ? atoi(e) != 0 : false;
     }();
-    const int nt = p.ntaps[0];
-    bool contiguous = true;
-    for (int t = 1; t < nt; ++t) contiguous = contiguous && (p.off[0][t] == p.off[0][0] + t);
-    if (tile_on && nt == 7 && contiguous && io.x.layout == LAYOUT_F32B && (p.Cin == 32 || p.Cin == 16)) {
-      const size_t smem = sizeof(float) * (((size_t)nt * p.Cin + 3) & ~(size_t)3) +
-                          sizeof(float4) * (size_t)(p.Cin >> 2) * 4 * (kPostTile / 4 + 2);
-      static bool attr = false;
-      if (!attr) {
-        cudaError_t e = cudaFuncSetAttribute(convpost_tile_kernel<7, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(convpost_tile_kernel<7, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-        if (e != cudaSuccess) return e;
-        attr = true;
-      }
-      dim3 grid((p.Lin + kPostTile - 1) / kPostTile, p.B);
-      if (p.Cin == 32) convpost_tile_kernel<7, 8><<<grid, 128, smem, stream>>>(p, io, w, bias);
-      else convpost_tile_kernel<7, 4><<<grid, 128, smem, stream>>>(p, io, w, bias);
-      return cudaGetLastError();
-    }
+    static const int rows = [] {
+      const char* e = getenv("MB_POST_ROWS");  // A/B switch: 1, 2 (default: measured fastest, 0.099 vs 0.127 / 0.122 ms) or 4 output rows per thread
+      const int r = e ? atoi(e) : 2;
+      return (r == 2 || r == 4) ? r : 1;
+    }();
+    variant = (tile_on && tile_fits) ? kCout1Tile : rows;
   }
-  static const int rows = [] {
-    const char* e = getenv("MB_POST_ROWS");  // A/B switch: 1, 2 (default: measured fastest, 0.099 vs 0.127 / 0.122 ms) or 4 output rows per thread
-    const int r = e ? atoi(e) : 2;
-    return (r == 2 || r == 4) ? r : 1;
-  }();
-  dim3 grid((p.Lin + 256 * rows - 1) / (256 * rows), p.B);
+  if (variant == kCout1Tile) {
+    if (!tile_fits) return cudaErrorInvalidValue;
+    const size_t smem = sizeof(float) * (((size_t)nt * p.Cin + 3) & ~(size_t)3) +
+                        sizeof(float4) * (size_t)(p.Cin >> 2) * 4 * (kPostTile / 4 + 2);
+    static bool attr = false;
+    if (!attr) {
+      cudaError_t e = cudaFuncSetAttribute(convpost_tile_kernel<7, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(convpost_tile_kernel<7, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
+      if (e != cudaSuccess) return e;
+      attr = true;
+    }
+    dim3 grid((p.Lin + kPostTile - 1) / kPostTile, p.B);
+    if (p.Cin == 32) convpost_tile_kernel<7, 8><<<grid, 128, smem, stream>>>(p, io, w, bias);
+    else convpost_tile_kernel<7, 4><<<grid, 128, smem, stream>>>(p, io, w, bias);
+    if (kernel) *kernel = p.Cin == 32 ? "post_tile<7,8>" : "post_tile<7,4>";
+    return cudaGetLastError();
+  }
+  if (variant != 1 && variant != 2 && variant != 4) return cudaErrorInvalidValue;
+  dim3 grid((p.Lin + 256 * variant - 1) / (256 * variant), p.B);
   const size_t smem = sizeof(float) * p.ntaps[0] * p.Cin;
-  if (rows == 4) tapconv_cout1_kernel<4><<<grid, 256, smem, stream>>>(p, io, w, bias);
-  else if (rows == 2) tapconv_cout1_kernel<2><<<grid, 256, smem, stream>>>(p, io, w, bias);
+  if (variant == 4) tapconv_cout1_kernel<4><<<grid, 256, smem, stream>>>(p, io, w, bias);
+  else if (variant == 2) tapconv_cout1_kernel<2><<<grid, 256, smem, stream>>>(p, io, w, bias);
   else tapconv_cout1_kernel<1><<<grid, 256, smem, stream>>>(p, io, w, bias);
+  if (kernel) *kernel = variant == 4 ? "cout1<4>" : (variant == 2 ? "cout1<2>" : "cout1<1>");
   return cudaGetLastError();
 }
 

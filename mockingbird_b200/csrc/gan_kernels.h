@@ -93,9 +93,13 @@ struct TapConvIO {
 cudaError_t launch_tapconv_f32(const TapConv& p, const TapConvIO& io, const float* w, const float* bias,
                                cudaStream_t stream);
 
-// Cout == 1 special case (conv_post, models.py:146-148): one thread per output sample
+// Cout == 1 special case (conv_post, models.py:146-148).  variant: kCout1Default (the MB_POST_TILE / MB_POST_ROWS switches),
+// 1 / 2 / 4 output rows per thread, or kCout1Tile (the shared-memory tile kernel; cudaErrorInvalidValue where it does not apply).
+// All variants accumulate in the same order and give bit-identical results.  *kernel (if given) names the instance launched.
+constexpr int kCout1Default = 0;
+constexpr int kCout1Tile = -1;
 cudaError_t launch_tapconv_cout1_f32(const TapConv& p, const TapConvIO& io, const float* w, const float* bias,
-                                     cudaStream_t stream);
+                                     cudaStream_t stream, int variant = kCout1Default, const char** kernel = nullptr);
 
 // dst32 += src32 (same layout), optionally refresh dst16 = lrelu(dst32, slope)
 cudaError_t launch_add_inplace_f32(const TRef& dst32, const TRef& src32, const TRef& dst16, float slope, int B,

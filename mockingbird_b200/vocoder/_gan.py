@@ -333,6 +333,69 @@ class GanGenerator:
             lo = y16[:, c16 // 2:c16 // 2 + cout] if out16 == "hilo" else None
         return y, hi, lo, launches
 
+    LAYOUTS = {"ncl": 1, "f32b": 2, "f16b": 3}
+    POST_VARIANTS = {None: 0, 1: 1, 2: 2, 4: 4, "tile": -1}
+
+    def debug_launch_f32(self, i: int, x: torch.Tensor, *, mode: str = "store", div: float = 1.0,
+                         y_init: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None,
+                         out16: Optional[str] = None, out_slope: float = 1.0, lengths: Optional[torch.Tensor] = None,
+                         x_layout: str = "ncl", y_layout: str = "ncl", want_y: bool = True, y2_init: Optional[torch.Tensor] = None,
+                         y2_out16: Optional[str] = None, y2_slope: float = 1.0, post=None):
+        """op i of this handle (any precision) run once on the FP32 kernels, through mb_gan_debug_f32.  x [B, Cin, L] (not
+        activated; for an add op the addend [B, C, L]), residual [B, Cout, L*stride] (fp32), y_init the running sum of the
+        accumulate modes (the add op's destination), y2_init the second destination's running sum (None: no second destination),
+        lengths int32 [B] in input rows.  x_layout / y_layout: how the kernel sees its input / its fp32 tensors ("ncl", "f32b",
+        "f16b" for x).  want_y=False: no fp32 output plane (store mode).  post: the Cout = 1 kernel (None: the MB_POST_* switches,
+        1 / 2 / 4 rows per thread, "tile").  Returns (y, y16_hi, y16_lo, y2, y2_hi, y2_lo, kernel) as fp32 NCL tensors (None where
+        not requested) and the name of the kernel instance that ran."""
+        if not self._ready:
+            self._upload()
+        x = x.contiguous().float()
+        B, _, L = x.shape
+        info = self.layer_info(i)
+        cout = int(info.split("cout=")[1].split()[0])
+        stride = int(info.split("stride=")[1].split()[0]) if info.startswith("conv") else 1
+        Lout = L * stride
+        dev = x.device
+
+        def fresh(init):
+            return init.contiguous().float().clone() if init is not None else torch.zeros(B, cout, Lout, dtype=torch.float32, device=dev)
+
+        def plane(kind):
+            c16 = 2 * cout if kind == "hilo" else cout  # the hi/lo plane geometry of the forward's FP32 layers
+            return torch.zeros(B, c16, Lout, dtype=torch.float32, device=dev) if kind else None
+
+        y = fresh(y_init) if want_y else None
+        y2 = fresh(y2_init) if y2_init is not None else None
+        y16, y2_16 = plane(out16), plane(y2_out16)
+        res = residual.contiguous().float() if residual is not None else None
+        lens = lengths.to(device=dev, dtype=torch.int32).contiguous() if lengths is not None else None
+        spec = _lib.GanDebugSpec()
+        spec.layer_index, spec.mode, spec.div = i, self.EPI_MODES[mode], div
+        spec.res_kind = 1 if res is not None else 0
+        spec.out16, spec.out_slope = self.OUT16_KINDS[out16], out_slope
+        spec.y2_out16, spec.y2_slope = self.OUT16_KINDS[y2_out16], y2_slope
+        spec.x_layout, spec.y_layout = self.LAYOUTS[x_layout], self.LAYOUTS[y_layout]
+        spec.batch, spec.frames_in = B, L
+        for field, t in (("x", x), ("residual", res), ("lengths", lens), ("y", y), ("y16", y16), ("y2", y2), ("y2_16", y2_16)):
+            setattr(spec, field, t.data_ptr() if t is not None else None)
+        cmax = max(x.shape[1], cout, 32)
+        ws = torch.empty(B * 8 * cmax * (max(L, Lout) + 88) * 4 + (1 << 20), dtype=torch.uint8, device=dev)
+        report = C.create_string_buffer(256)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        _lib.check(_lib.lib().mb_gan_debug_f32(self._handle, C.byref(spec), self.POST_VARIANTS[post], C.c_void_p(ws.data_ptr()),
+                                               ws.numel(), C.c_void_p(stream), report, 256))
+        kernel = report.value.decode().strip().split("kernel=")[1]
+
+        def split(t, kind):
+            if t is None:
+                return None, None
+            return t[:, :cout], (t[:, t.shape[1] // 2:t.shape[1] // 2 + cout] if kind == "hilo" else None)
+
+        hi, lo = split(y16, out16)
+        hi2, lo2 = split(y2_16, y2_out16)
+        return y, hi, lo, y2, hi2, lo2, kernel
+
     def __del__(self):
         try:
             if getattr(self, "_handle", None) is not None and self._handle.value:
