@@ -810,6 +810,66 @@ int mb_logmmse_denoise(mb_logmmse* h, const float* x, const int32_t* lengths_hos
 int mb_logmmse_exp1(const double* x, double* y, int64_t n, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Polyphase resampling and per-clip levelling (DESIGN.md section 4k; csrc/resample.cu)
+ *   replaces  scipy.signal.resample_poly(x, up, down) as synthesizer/audio_host.py load_wav and preprocess_wav call it
+ *             (librosa.load's resampling in the reference), normalize_volume (models/encoder/audio.py:108-117) and the
+ *             rescale of load_preprocess_wav (models/synthesizer/inference.py:145-150)
+ * scipy's float32 contract, bitwise: the filter is firwin(20 max(up, down) + 1, 1 / max(up, down), ('kaiser', 5.0)) cast
+ * to float32 and multiplied by up in float32 (designed by the caller, one per reduced ratio); output sample j is the sum,
+ * over input samples in ascending order, of one rounded float32 multiply tap * x and one rounded float32 add, from zero;
+ * ceil(n up / down) samples.  up == down == 1 is a copy.
+ * ------------------------------------------------------------------------------------------- */
+#define MB_RESAMPLE_F32 0 /* float32 samples */
+#define MB_RESAMPLE_I16 1 /* int16 PCM, converted on the device as x / 32768.0f (exact, what load_wav does) */
+
+typedef struct mb_resample mb_resample;
+
+/* filter_smem_bytes: the largest polyphase table [up][ceil(taps / up)] (fp32) staged in shared memory per work item; larger
+ * tables are read through L2.  < 0: the default (64 KB); at most 128 KB. */
+int mb_resample_create(int32_t filter_smem_bytes, mb_resample** out);
+void mb_resample_destroy(mb_resample* h);
+/* register the filter of a reduced ratio (gcd(up, down) == 1, not 1 / 1): taps_host fp32 [20 max(up, down) + 1] (host),
+ * already multiplied by up.  Returns its index (the same index for a ratio added before).  A new filter forgets the arena:
+ * set_arena and finalize again.  MB_ERR_INVALID for a ratio whose tile would read more input than shared memory holds. */
+int mb_resample_add_filter(mb_resample* h, int32_t up, int32_t down, const float* taps_host, int32_t n_taps, int32_t* index_out);
+/* the polyphase tables of every filter added so far; 16-byte aligned */
+size_t mb_resample_arena_bytes(const mb_resample* h);
+int mb_resample_set_arena(mb_resample* h, void* arena, size_t bytes);
+/* writes the tables into the arena and synchronises `stream` */
+int mb_resample_finalize(mb_resample* h, void* stream);
+/* 1: filter `index` is staged in shared memory, 0: read through L2, -1: no such filter (host only) */
+int mb_resample_filter_in_smem(const mb_resample* h, int32_t index);
+/* ceil(n up / down); -1 for a bad argument (host only) */
+int64_t mb_resample_output_length(int32_t up, int32_t down, int64_t n);
+/* the work items of a mb_resample_forward call with these clips (host only): tile0_host int32 [batch + 1] gets the first work
+ * item of every clip and the number of work items, out_offsets_host int64 [batch + 1] the first output sample of every clip
+ * and the output length.  MB_ERR_INVALID, naming the clip, for what forward refuses. */
+int mb_resample_work_items(const mb_resample* h, const int32_t* lengths_host, const int32_t* filters_host, int32_t batch,
+                           int32_t* tile0_host, int64_t* out_offsets_host);
+/* device workspace of mb_resample_forward (its clip table); 0 when batch < 1 */
+size_t mb_resample_workspace_bytes(const mb_resample* h, int32_t batch);
+/* resample_poly of `batch` clips in one launch, one work item per (clip, tile of 512 output samples):
+ *   x: the clips back to back (device, 16-byte aligned), dtype MB_RESAMPLE_F32 or MB_RESAMPLE_I16, lengths_host[b] >= 1
+ *   filters_host int32 [batch] (host): the add_filter index of clip b's ratio, or -1 for a copy
+ *   out fp32 (device): clip b's ceil(n_b up_b / down_b) samples after those of clips 0 .. b-1
+ * Each clip's output is bitwise what a batch of that clip alone gives.  MB_ERR_INVALID before anything is queued for an
+ * empty clip or an unknown filter; the message names the clip.  The clip table is copied from pageable host memory. */
+int mb_resample_forward(mb_resample* h, const void* x, int32_t dtype, const int32_t* lengths_host, const int32_t* filters_host,
+                        int32_t batch, float* out, void* workspace, size_t workspace_bytes, void* stream);
+/* device workspace of the three levelling calls below (their clip table); 0 when batch < 1 */
+size_t mb_resample_level_workspace_bytes(int32_t batch);
+/* x fp32: `batch` clips back to back (device), lengths_host[b] >= 1 (host).  sumsq fp32 [batch] (device): the float32 sum of
+ * x * x in numpy's pairwise order, bitwise np.add.reduce(x ** 2) (np.mean(x ** 2) is that sum / n, rounded once) */
+int mb_resample_sumsq(const float* x, const int32_t* lengths_host, int32_t batch, float* sumsq, void* workspace,
+                      size_t workspace_bytes, void* stream);
+/* y = x * gains[b] (one rounded fp32 multiply; gains fp32 [batch], device); y may be x */
+int mb_resample_scale(const float* x, const int32_t* lengths_host, int32_t batch, const float* gains, float* y, void* workspace,
+                      size_t workspace_bytes, void* stream);
+/* y = (x / max |x|) * peak per clip (two rounded fp32 operations); y may be x */
+int mb_resample_rescale(const float* x, const int32_t* lengths_host, int32_t batch, float peak, float* y, void* workspace,
+                        size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Voice-conversion mel decoder (ppg2mel)
  *   replaces  models/ppg2mel/__init__.py:166-192 (MelDecoderMOLv2.inference: PPG / pitch encoder, reduce_proj with the
  *             normalised speaker embedding), models/ppg2mel/rnn_decoder_mol.py:267-315 (Decoder.inference: PreNet with

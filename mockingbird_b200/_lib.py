@@ -350,6 +350,26 @@ SIGNATURES = {
     "mb_logmmse_denoise": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p,
                                      C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_logmmse_exp1": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "mb_resample_create": (C.c_int, [C.c_int32, C.POINTER(C.c_void_p)]),
+    "mb_resample_destroy": (None, [C.c_void_p]),
+    "mb_resample_add_filter": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]),
+    "mb_resample_arena_bytes": (C.c_size_t, [C.c_void_p]),
+    "mb_resample_set_arena": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "mb_resample_finalize": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "mb_resample_filter_in_smem": (C.c_int, [C.c_void_p, C.c_int32]),
+    "mb_resample_output_length": (C.c_int64, [C.c_int32, C.c_int32, C.c_int64]),
+    "mb_resample_work_items": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32,
+                                         C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
+    "mb_resample_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32]),
+    "mb_resample_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32,
+                                      C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mb_resample_level_workspace_bytes": (C.c_size_t, [C.c_int32]),
+    "mb_resample_sumsq": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p, C.c_size_t,
+                                    C.c_void_p]),
+    "mb_resample_scale": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_size_t, C.c_void_p]),
+    "mb_resample_rescale": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_float, C.c_void_p, C.c_void_p,
+                                      C.c_size_t, C.c_void_p]),
     "mb_ppg2mel_create": (C.c_int, [C.POINTER(Ppg2MelConfig), C.POINTER(C.c_void_p)]),
     "mb_ppg2mel_destroy": (None, [C.c_void_p]),
     "mb_ppg2mel_arena_bytes": (C.c_size_t, [C.c_void_p]),

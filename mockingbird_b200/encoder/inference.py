@@ -31,6 +31,34 @@ def preprocess_wav(fpath_or_wav, source_sr=None, normalize=True, trim_silence=Tr
     return _audio_host.preprocess_wav(fpath_or_wav, source_sr, normalize, trim_silence, sampling_rate, audio_norm_target_dBFS)
 
 
+def _have_webrtcvad():
+    try:
+        import webrtcvad  # noqa: F401
+    except Exception:
+        return False
+    return True
+
+
+def preprocess_wavs(fpaths_or_wavs, source_srs=None, normalize=True, trim_silence=True, device=None):
+    """preprocess_wav for a list of paths and float32 arrays, resampled to 16 kHz and volume-normalised on the device
+    (mockingbird_b200.resample): a path is read at its own rate (16-bit mono PCM uploaded as int16), an array is at
+    source_srs (one int, or one per clip; None: already 16 kHz).  -> a resample.DeviceClips whose clip i is bitwise
+    preprocess_wav(fpaths_or_wavs[i], source_srs[i]) (``.numpy()`` for host arrays; ``embed_utterances`` takes it as it
+    is).  Silence trimming runs on the host, clip by clip, and only where webrtcvad is installed, as in preprocess_wav."""
+    from .. import resample
+    from .params_data import audio_norm_target_dBFS
+
+    clips, rates = resample.load_clips(fpaths_or_wavs, source_srs, sampling_rate)
+    out = resample.resample_device(clips, rates, sampling_rate, device)
+    if normalize:
+        out = resample.normalize_volume_device(out, audio_norm_target_dBFS, increase_only=True)
+    if trim_silence and len(out) and _have_webrtcvad():
+        trimmed = [_audio_host.trim_long_silences(w, sampling_rate) for w in out.numpy()]
+        out = resample.DeviceClips(torch.from_numpy(np.concatenate(trimmed)).to(out.device), [len(w) for w in trimmed],
+                                   sampling_rate)
+    return out
+
+
 def load_model(weights_fpath: Path, device=None):
     """inference.py:15-37: checkpoint['model_state'] -> module-global model; returns the model"""
     global _model, _device
@@ -188,13 +216,17 @@ def embed_utterances(wavs, using_partials=True, return_partials=False, **kwargs)
     every utterance.  Utterances are sorted by length and their mels and rows computed in a few library calls
     (``many_plan``): one mel launch and one mb_encoder_embed_rows per call, the frames never leaving the device.  A result
     is bitwise the same whatever the list around it (order, neighbours, chunking), and within FP32 rounding of
-    embed_utterance on the same waveform."""
+    embed_utterance on the same waveform.  `wavs` may be a resample.DeviceClips (what preprocess_wavs returns): its
+    samples go to the mel front-end without leaving the device, with the same results as the same samples from the host."""
     if _model is None:
         raise Exception("Model was not loaded. Call load_model() before inference.")
     from . import audio
     from ..melspec import as_wavs
+    from ..resample import DeviceClips
 
-    wavs = as_wavs(wavs)
+    resident = isinstance(wavs, DeviceClips)
+    if not resident:
+        wavs = as_wavs(wavs)
     plans = [utterance_rows(len(w), using_partials, **kwargs) for w in wavs]
     audio.check(wavs, [p[0] for p in plans])
     E = _model._cfg.embedding_size
@@ -206,7 +238,11 @@ def embed_utterances(wavs, using_partials=True, return_partials=False, **kwargs)
     front = audio.mel_front(dev)  # the frames are computed where the encoder reads them
     for call in many_plan([p[3] for p in plans]):
         utts = list(dict.fromkeys(u for u, _, _ in call))
-        flat, counts = front.many_flat([wavs[u] for u in utts], [plans[u][0] for u in utts])
+        if resident:
+            sel = wavs.select(utts)
+            flat, counts = front.many_flat_device(sel.data, sel.lengths, [plans[u][0] for u in utts])
+        else:
+            flat, counts = front.many_flat([wavs[u] for u in utts], [plans[u][0] for u in utts])
         first = dict(zip(utts, np.concatenate([[0], np.cumsum(counts)[:-1]]).tolist()))
         starts, lens, dst = [], [], []
         for u, r0, r1 in call:

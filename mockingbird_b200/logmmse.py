@@ -86,21 +86,35 @@ def _handle(W, len1, len2, n_fft) -> _Handle:
 
 
 def _flat(clips, dev):
+    if _resident(clips):
+        return clips.data.to(dev)
     return torch.from_numpy(np.concatenate(clips) if len(clips) > 1 else clips[0]).to(dev)
 
 
+def _resident(clips):
+    from .resample import DeviceClips
+
+    return isinstance(clips, DeviceClips)
+
+
+def _lengths(clips):
+    return list(clips.lengths) if _resident(clips) else [len(c) for c in clips]
+
+
 def profile_noise_many(noises, sampling_rate, window_size=0):
-    """profile_noise for every signal of `noises` in one launch -> list of NoiseProfile"""
-    noises = [_check_float32(n, f"noise {i}") for i, n in enumerate(noises)]
+    """profile_noise for every signal of `noises` in one launch -> list of NoiseProfile.  `noises` may be a
+    resample.DeviceClips, read where it lies."""
+    if not _resident(noises):
+        noises = [_check_float32(n, f"noise {i}") for i, n in enumerate(noises)]
     W, len1, len2, win, n_fft = _params(sampling_rate, window_size)
-    for i, n in enumerate(noises):
-        if len(n) < W:
-            raise ValueError(f"noise {i} has {len(n)} samples, fewer than one window of {W}")
-    if not noises:
+    for i, n in enumerate(_lengths(noises)):
+        if n < W:
+            raise ValueError(f"noise {i} has {n} samples, fewer than one window of {W}")
+    if not len(noises):
         return []
     h = _handle(W, len1, len2, n_fft)
     dev = h.device
-    lengths = [len(n) for n in noises]
+    lengths = _lengths(noises)
     with torch.cuda.device(dev):
         T, ws = h.workspace(lengths)
         x = _flat(noises, dev)
@@ -121,11 +135,13 @@ def profile_noise(noise, sampling_rate, window_size=0) -> NoiseProfile:
 
 def denoise_many(wavs, noise_profiles, eta=0.15, vad_out=None):
     """denoise(wavs[i], noise_profiles[i], eta) for every i in one sequence of launches -> list of float32 arrays.  The
-    profiles must share one window.  vad_out: a list that receives each clip's per-frame VAD statistics (float64)."""
-    wavs = [_check_float32(w, f"wav {i}") for i, w in enumerate(wavs)]
+    profiles must share one window.  vad_out: a list that receives each clip's per-frame VAD statistics (float64).  `wavs`
+    may be a resample.DeviceClips, read where it lies."""
+    if not _resident(wavs):
+        wavs = [_check_float32(w, f"wav {i}") for i, w in enumerate(wavs)]
     if len(noise_profiles) != len(wavs):
         raise ValueError(f"{len(noise_profiles)} noise profiles for {len(wavs)} waveforms")
-    if not wavs:
+    if not len(wavs):
         return []
     p0 = noise_profiles[0]
     for i, p in enumerate(noise_profiles):
@@ -134,12 +150,12 @@ def denoise_many(wavs, noise_profiles, eta=0.15, vad_out=None):
             raise ValueError(f"noise profile {i} has another window than profile 0: one call takes one window")
         if np.shape(p.noise_mu2) != (p0.n_fft,):
             raise ValueError(f"noise profile {i}: noise_mu2 must have n_fft = {p0.n_fft} entries, got {np.shape(p.noise_mu2)}")
-    for i, w in enumerate(wavs):
-        if len(w) < 2 * p0.len2:
-            raise ValueError(f"wav {i} has {len(w)} samples; utils/logmmse.denoise needs at least 2 * len2 = {2 * p0.len2}")
+    for i, n in enumerate(_lengths(wavs)):
+        if n < 2 * p0.len2:
+            raise ValueError(f"wav {i} has {n} samples; utils/logmmse.denoise needs at least 2 * len2 = {2 * p0.len2}")
     h = _handle(p0.window_size, p0.len1, p0.len2, p0.n_fft)
     dev = h.device
-    lengths = [len(w) for w in wavs]
+    lengths = _lengths(wavs)
     with torch.cuda.device(dev):
         T, ws = h.workspace(lengths)
         x = _flat(wavs, dev)

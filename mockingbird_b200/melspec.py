@@ -87,14 +87,23 @@ class MelSpectrogram:
         signal_lengths[i] >= len(wavs[i]) frames utterance i as if zeros were appended to that length.
         Returns (device tensor holding utterance i's frames after those of 0 .. i-1, in the handle's layout, list of frame
         counts)."""
-        sig = [len(w) for w in wavs] if signal_lengths is None else [int(n) for n in signal_lengths]
-        L = _lib.lib()
-        counts = [self.num_frames(n) for n in sig]
-        B = len(wavs)
-        lens = (C.c_int32 * B)(*[len(w) for w in wavs])
-        sigs = (C.c_int32 * B)(*sig)
         with torch.cuda.device(self._device):
             x = torch.from_numpy(np.concatenate(wavs)).to(self._device)
+        return self.many_flat_device(x, [len(w) for w in wavs], signal_lengths)
+
+    def many_flat_device(self, x, lengths, signal_lengths=None):
+        """``many_flat`` of utterances already on the device: x holds utterance i's lengths[i] float32 samples after those
+        of 0 .. i-1 (a ``resample.DeviceClips``' data, for instance); moved to the handle's device if elsewhere"""
+        sig = [int(n) for n in lengths] if signal_lengths is None else [int(n) for n in signal_lengths]
+        L = _lib.lib()
+        counts = [self.num_frames(n) for n in sig]
+        B = len(lengths)
+        if x.dtype != torch.float32 or x.dim() != 1 or x.numel() != sum(int(n) for n in lengths):
+            raise ValueError(f"x must be 1-D float32 holding the {B} utterances back to back")
+        lens = (C.c_int32 * B)(*[int(n) for n in lengths])
+        sigs = (C.c_int32 * B)(*sig)
+        with torch.cuda.device(self._device):
+            x = x.to(self._device).contiguous()
             out = torch.empty(sum(counts) * self.n_mels, dtype=torch.float32, device=self._device)
             need = int(L.mb_melspec_ragged_workspace_bytes(self._handle, B))
             ws = torch.empty(need, dtype=torch.uint8, device=self._device)

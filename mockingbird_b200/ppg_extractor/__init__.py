@@ -288,7 +288,8 @@ class PPGModel:
         rows and <= MAX_BATCH_FRAMES padded frames, longest first; each result equals its own B = 1 call made in that
         order.  The order matters only past 5000 frames (50 s at a 10 ms hop): the positional table's high-water mark
         rises to the longest utterance before any shorter one runs, whereas B = 1 calls in the caller's order would
-        see the mark each utterance's predecessors left."""
+        see the mark each utterance's predecessors left.  `wavs` may be a resample.DeviceClips (clips resampled to the
+        extractor's rate on the device), whose clips are read where they lie."""
         self._prepare()
         ws = [torch.as_tensor(np.asarray(w, dtype=np.float32) if not torch.is_tensor(w) else w).reshape(-1) for w in wavs]
         order = sorted(range(len(ws)), key=lambda i: -ws[i].numel())

@@ -126,28 +126,34 @@ class Synthesizer:
         return wav
 
     @staticmethod
-    def load_preprocess_wavs(fpaths_or_wavs):
-        """the reference's load_preprocess_wav (inference.py:145-159) for a list of clips, denoised on the device: each
-        path is loaded at the synthesizer rate (an array is taken as already at that rate) and rescaled; every clip longer
-        than 0.4 s is then denoised with the noise profile of its first and last 0.15 s, all profiles in one launch and all
-        clips in one logmmse.denoise_many.  -> list of float32 waveforms"""
-        from .. import logmmse
-        from . import audio_host
+    def load_preprocess_wavs(fpaths_or_wavs, source_srs=None):
+        """the reference's load_preprocess_wav (inference.py:145-159) for a list of clips, on the device from the file's
+        samples to the denoised clip: each path is read at its own rate (16-bit mono PCM uploaded as int16), an array is at
+        source_srs (one int, or one per clip; None: already at the synthesizer rate) and must hold float32 samples; every
+        clip is resampled to the synthesizer rate (mockingbird_b200.resample, bitwise load_wav's resample_poly) and
+        rescaled; every clip longer than 0.4 s is then denoised with the noise profile of its first and last 0.15 s, all
+        profiles in one launch and all clips in one logmmse.denoise_many.  -> list of float32 waveforms, each bitwise the
+        host route (load_wav, rescale, the same denoiser)"""
+        from .. import logmmse, resample
 
         sr = hparams.sample_rate
-        wavs = []
-        for x in fpaths_or_wavs:
-            wav = audio_host.load_wav(x, sr)[0] if isinstance(x, (str, Path)) else np.asarray(x)
-            if hparams.rescale:
-                wav = wav / np.abs(wav).max() * hparams.rescaling_max
-            wavs.append(wav)
-        noisy = [i for i, w in enumerate(wavs) if len(w) > sr * (0.3 + 0.1)]
+        clips, rates = resample.load_clips(fpaths_or_wavs, source_srs, sr)
+        if not clips:
+            return []
+        wavs = resample.resample_device(clips, rates, sr)
+        if hparams.rescale:
+            wavs = resample.rescale_device(wavs, hparams.rescaling_max)
+        noisy = [i for i, n in enumerate(wavs.lengths) if n > sr * (0.3 + 0.1)]
+        out = wavs.numpy() if len(noisy) < len(wavs) else [None] * len(wavs)
         if noisy:
             edge = int(sr * 0.15)
-            profiles = logmmse.profile_noise_many([np.concatenate([wavs[i][:edge], wavs[i][-edge:]]) for i in noisy], sr)
-            for i, w in zip(noisy, logmmse.denoise_many([wavs[i] for i in noisy], profiles)):
-                wavs[i] = w
-        return wavs
+            loud = wavs.select(noisy)
+            edges = resample.DeviceClips(torch.cat([t for w in loud for t in (w[:edge], w[-edge:])]), [2 * edge] * len(noisy),
+                                         sr)
+            profiles = logmmse.profile_noise_many(edges, sr)
+            for i, w in zip(noisy, logmmse.denoise_many(loud, profiles)):
+                out[i] = w
+        return out
 
     @staticmethod
     def make_spectrogram(fpath_or_wav):
