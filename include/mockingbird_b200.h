@@ -666,7 +666,8 @@ int mb_encoder_embed_rows(mb_encoder* h, const float* frames, int64_t n_frames, 
  * ------------------------------------------------------------------------------------------- */
 typedef struct mb_melspec_config {
   int32_t sample_rate;
-  int32_t n_fft;          /* <= 2048 */
+  int32_t n_fft;          /* even, 16 .. 2048 (bin k at k sr / n_fft; odd n_fft is refused: librosa's grid for it
+                             depends on the librosa version) */
   int32_t hop_length;
   int32_t win_length;     /* periodic Hann, zero padded (centered) to n_fft */
   int32_t n_mels;
@@ -808,6 +809,12 @@ int mb_logmmse_denoise(mb_logmmse* h, const float* x, const int32_t* lengths_hos
                        size_t workspace_bytes, void* stream);
 /* E1(x) = expint(1, x) for x > 0, the device function the gains use: x, y float64 [n] (device) */
 int mb_logmmse_exp1(const double* x, double* y, int64_t n, void* stream);
+
+/* The shared Stockham FFT of Griffin-Lim and log-MMSE (csrc/mb_fft.cuh) on its own, for tests: y[r] = sum_j x[r][j]
+ * exp(-+2 pi i j k / n) for each of `rows` rows of n complex points, unscaled in both directions, over the handles' twiddle
+ * table.  x, y [rows][n] (device) of float2 (dtype 0) or double2 (dtype 1); inverse != 0 takes the + sign.  n is 2^a or 5 * 2^a
+ * in [64, 2048]; MB_ERR_INVALID before anything is queued otherwise.  Synchronises the stream. */
+int mb_fft_debug(const void* x, void* y, int32_t n, int32_t rows, int32_t dtype, int32_t inverse, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Polyphase resampling and per-clip levelling (DESIGN.md section 4k; csrc/resample.cu)

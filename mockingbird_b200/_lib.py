@@ -350,6 +350,7 @@ SIGNATURES = {
     "mb_logmmse_denoise": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p,
                                      C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_logmmse_exp1": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "mb_fft_debug": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "mb_resample_create": (C.c_int, [C.c_int32, C.POINTER(C.c_void_p)]),
     "mb_resample_destroy": (None, [C.c_void_p]),
     "mb_resample_add_filter": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]),

@@ -307,10 +307,7 @@ int mb_griffinlim_create(const mb_griffinlim_config* cfg, mb_griffinlim** out) {
   const double PI = 3.14159265358979323846;
   const int lpad = (N - c.win_length) / 2;  // periodic Hann of win_length, centred in n_fft (librosa.util.pad_center)
   for (int i = 0; i < c.win_length; ++i) h->tables[lpad + i] = (float)(0.5 - 0.5 * std::cos(2.0 * PI * i / c.win_length));
-  for (int k = 0; k < N; ++k) {
-    h->tables[N + 2 * k] = (float)std::cos(2.0 * PI * k / N);
-    h->tables[N + 2 * k + 1] = (float)(-std::sin(2.0 * PI * k / N));
-  }
+  fft_twiddles(N, h->tables.data() + N);
   *out = h;
   return MB_OK;
 }

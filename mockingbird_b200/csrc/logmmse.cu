@@ -299,12 +299,6 @@ __global__ void lm_exp1_kernel(const double* __restrict__ x, double* __restrict_
   if (i < n) y[i] = lm_exp1(x[i]);
 }
 
-bool supported_n_fft(int n) {
-  if (n < 64 || n > 2048) return false;
-  if (n % 5 == 0) n /= 5;
-  return (n & (n - 1)) == 0;
-}
-
 struct Layout {
   size_t pairs, utt, sg, frames, total;
   int64_t n_pairs, F;
@@ -347,7 +341,7 @@ int mb_logmmse_create(const mb_logmmse_config* cfg, mb_logmmse** out) {
   if (!cfg || !out) return fail(MB_ERR_INVALID, "mb_logmmse_create: null argument");
   const mb_logmmse_config& c = *cfg;
   const int N = c.n_fft;
-  if (!supported_n_fft(N))
+  if (!fft_supported(N))
     return fail(MB_ERR_INVALID, "mb_logmmse_create: n_fft = %d is not 2^a or 5 * 2^a in [64, 2048]", N);
   if (c.window_size <= 0 || c.window_size % 2 != 0 || c.window_size > N)
     return fail(MB_ERR_INVALID, "mb_logmmse_create: window_size = %d must be even and in [2, n_fft = %d]", c.window_size, N);
@@ -360,11 +354,7 @@ int mb_logmmse_create(const mb_logmmse_config* cfg, mb_logmmse** out) {
   h->stride = (h->nb + 1) & ~1;  // rows of a multiple of 16 bytes
   h->w.add_derived("twiddles", 4 * (size_t)N);
   h->tw.resize(2 * (size_t)N);
-  const double PI = 3.14159265358979323846;
-  for (int k = 0; k < N; ++k) {
-    h->tw[2 * k] = std::cos(2.0 * PI * k / N);
-    h->tw[2 * k + 1] = -std::sin(2.0 * PI * k / N);
-  }
+  fft_twiddles(N, h->tw.data());
   *out = h;
   return MB_OK;
 }

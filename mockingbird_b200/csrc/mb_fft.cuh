@@ -8,7 +8,27 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <cmath>
+
 namespace mb {
+
+// the twiddle table of an N-point transform, tw[2 m] + i tw[2 m + 1] = exp(-2 pi i m / N), computed in float64 and rounded
+// once to R (float for the float2 instance); every user of stockham() builds its table here
+template <class R>
+inline void fft_twiddles(int N, R* tw) {
+  const double PI = 3.14159265358979323846;
+  for (int k = 0; k < N; ++k) {
+    tw[2 * k] = (R)std::cos(2.0 * PI * k / N);
+    tw[2 * k + 1] = (R)(-std::sin(2.0 * PI * k / N));
+  }
+}
+
+// 2^a or 5 * 2^a in [64, 2048]: the sizes stockham() is built and tested for
+inline bool fft_supported(int n) {
+  if (n < 64 || n > 2048) return false;
+  if (n % 5 == 0) n /= 5;
+  return (n & (n - 1)) == 0;
+}
 
 __device__ __forceinline__ float2 cmul(float2 a, float2 b) {
   return make_float2(fmaf(a.x, b.x, -(a.y * b.y)), fmaf(a.x, b.y, a.y * b.x));

@@ -152,6 +152,13 @@ int mb_melspec_create(const mb_melspec_config* cfg, mb_melspec** out) {
   if (c.n_fft < 16 || c.n_fft > 2048 || c.hop_length <= 0 || c.win_length <= 0 || c.win_length > c.n_fft || c.n_mels <= 0 ||
       c.sample_rate <= 0 || (c.power != 1 && c.power != 2) || c.fmax <= c.fmin || c.fmax > c.sample_rate * 0.5f + 1e-3f)
     return fail(MB_ERR_INVALID, "mb_melspec_create: unsupported parameters");
+  // bin k lies at k sr / n_fft below; for odd n_fft librosa's own grid depends on its version (linspace(0, sr / 2, 1 +
+  // n_fft // 2) before 0.10's rfftfreq), so the filterbank would have no one reference to agree with
+  if (c.n_fft % 2 != 0)
+    return fail(MB_ERR_INVALID,
+                "mb_melspec_create: n_fft = %d is odd; its FFT-bin frequencies differ between librosa versions, so only even "
+                "n_fft is supported",
+                c.n_fft);
   mb_melspec* h = new mb_melspec();
   h->cfg = c;
   const int N = c.n_fft, nb = N / 2 + 1;

@@ -11,7 +11,10 @@ librosa's published algorithm as the reference calls it:
 librosa.stft: center=True (pad n_fft//2; pad_mode "reflect" up to librosa 0.9, "constant" from 0.10 - a parameter
 here), periodic Hann window of win_length centered in n_fft, rfft per frame; n_frames = 1 + len(y) // hop.
 librosa.filters.mel: Slaney scale (htk=False), norm="slaney".  The STFT part is cross-checked against torch.stft in
-tests/test_oracle_pinned.py.
+tests/test_oracle_pinned.py, odd n_fft and odd window lengths included.
+FFT-bin frequencies: librosa's fft_frequencies was np.linspace(0, sr / 2, 1 + n_fft // 2) before 0.10 and rfftfreq from it.
+The two agree for even n_fft only, so, like pad_mode, the answer for odd n_fft depends on the librosa version.  No shipped
+config uses an odd n_fft; mel_basis refuses one, as mb_melspec_create does.
 """
 from __future__ import annotations
 
@@ -38,7 +41,9 @@ def mel_to_hz(m):
 
 
 def mel_basis(sr: int, n_fft: int, n_mels: int, fmin: float, fmax: float) -> np.ndarray:
-    """librosa.filters.mel(sr, n_fft, n_mels, fmin, fmax) -> [n_mels, 1 + n_fft // 2] float32"""
+    """librosa.filters.mel(sr, n_fft, n_mels, fmin, fmax) -> [n_mels, 1 + n_fft // 2] float32; n_fft even (module header)"""
+    if n_fft % 2:
+        raise ValueError(f"n_fft = {n_fft} is odd: librosa's FFT-bin frequencies for it depend on the librosa version")
     fftfreqs = np.linspace(0, sr / 2.0, 1 + n_fft // 2)
     mel_f = mel_to_hz(np.linspace(hz_to_mel(fmin), hz_to_mel(fmax), n_mels + 2))
     fdiff = np.diff(mel_f)
@@ -73,14 +78,21 @@ def encoder_mel(wav: np.ndarray, pad_mode: str = "reflect") -> np.ndarray:
 
 
 def synthesizer_mel(wav: np.ndarray, hp: dict, pad_mode: str = "reflect") -> np.ndarray:
-    """models/synthesizer/audio.py:59-65 -> float32 [num_mels, n_frames]"""
+    """models/synthesizer/audio.py:59-65 -> float32 [num_mels, n_frames].  Optional keys beyond the reference's hparams
+    cover every mb_melspec_config: power (1: |D|, 2: |D|^2; default 1), to_db (default True), signal_normalization
+    (default True, applied to the dB or linear values alike)."""
     from scipy.signal import lfilter
 
     y = lfilter([1, -hp["preemphasis"]], [1], np.asarray(wav, dtype=np.float64)) if hp.get("preemphasize", True) else wav
     D = stft(y, hp["n_fft"], hp["hop_size"], hp["win_size"], pad_mode)
-    M = mel_basis(hp["sample_rate"], hp["n_fft"], hp["num_mels"], hp["fmin"], hp["fmax"]).astype(np.float64) @ np.abs(D)
-    min_level = np.exp(hp["min_level_db"] / 20 * np.log(10))
-    S = 20 * np.log10(np.maximum(min_level, M)) - hp["ref_level_db"]
+    M = mel_basis(hp["sample_rate"], hp["n_fft"], hp["num_mels"], hp["fmin"], hp["fmax"]).astype(np.float64) @ \
+        np.abs(D) ** hp.get("power", 1)
+    S = M
+    if hp.get("to_db", True):
+        min_level = np.exp(hp["min_level_db"] / 20 * np.log(10))
+        S = 20 * np.log10(np.maximum(min_level, M)) - hp["ref_level_db"]
+    if not hp.get("signal_normalization", True):
+        return S.astype(np.float32)
     A = hp["max_abs_value"]
     if hp.get("symmetric_mels", True):
         S = np.clip((2 * A) * ((S - hp["min_level_db"]) / (-hp["min_level_db"])) - A, -A, A)

@@ -180,13 +180,21 @@ def test_melspec_oracle_stft_matches_torch_and_mel_basis_matches_transformers():
 
     rng = np.random.default_rng(0)
     y = (rng.standard_normal(5000) * 0.1).astype(np.float32)
-    for n_fft, hop, mode in ((400, 160, "reflect"), (1024, 256, "constant"), (1024, 256, "reflect")):
-        D = mo.stft(y, n_fft, hop, n_fft, mode)
-        T = torch.stft(torch.from_numpy(y).double(), n_fft, hop, n_fft,
-                       window=torch.hann_window(n_fft, periodic=True, dtype=torch.float64), center=True, pad_mode=mode,
+    # odd n_fft, odd windows (the window's left pad rounds down) and windows shorter than n_fft by an odd count included
+    for n_fft, hop, win, mode in ((400, 160, 400, "reflect"), (1024, 256, 1024, "constant"), (1024, 256, 1024, "reflect"),
+                                  (1024, 256, 1023, "reflect"), (1024, 200, 801, "constant"), (400, 160, 301, "reflect"),
+                                  (401, 160, 401, "reflect"), (17, 5, 16, "constant"), (16, 20, 11, "reflect")):
+        D = mo.stft(y, n_fft, hop, win, mode)
+        T = torch.stft(torch.from_numpy(y).double(), n_fft, hop, win,
+                       window=torch.hann_window(win, periodic=True, dtype=torch.float64), center=True, pad_mode=mode,
                        return_complex=True).numpy()
-        assert D.shape == T.shape == (1 + n_fft // 2, 1 + len(y) // hop)
-        assert np.abs(D - T).max() < 1e-10
+        # 1 + len // hop frames for even n_fft; an odd one pads 2 (n_fft // 2) = n_fft - 1 samples, one frame fewer when hop
+        # divides len
+        assert D.shape == T.shape == (1 + n_fft // 2, 1 + (len(y) + 2 * (n_fft // 2) - n_fft) // hop), (n_fft, win)
+        assert np.abs(D - T).max() < 1e-10, (n_fft, win)
+    # odd n_fft has no single librosa filterbank (the module header): refused, like mb_melspec_create does
+    with pytest.raises(ValueError, match="odd"):
+        mo.mel_basis(16000, 401, 40, 0.0, 8000.0)
     # transformers.audio_utils.mel_filter_bank is an independent implementation of librosa.filters.mel; it runs in a
     # fresh interpreter because the reference-import stubs of this test module shadow optional audio packages
     import subprocess
