@@ -23,6 +23,11 @@
  *     before it: finalize and the compute calls return MB_ERR_STATE until all are set again and finalized.  set_weight
  *     reports argument errors (NULL pointers, unknown name, wrong shape: MB_ERR_INVALID) before call-order errors (no
  *     arena: MB_ERR_STATE).
+ *   - workspaces: a compute call takes any alignment of `workspace` and needs at least the bytes its mb_*_workspace_bytes
+ *     reports, a figure that includes the slack for aligning the pointer inside the library.  A NULL workspace is
+ *     MB_ERR_INVALID and a shorter one MB_ERR_WORKSPACE, both reported before anything is queued.  Its contents do not
+ *     persist from one call to the next, except where an entry point says so: the sample-loop state of
+ *     mb_wavernn_generate* and mb_deepmind_generate, and what mb_wavernn_last_logits reads.
  *   - every launch goes to the cudaStream_t passed as `stream` (void* here so that the header
  *     needs no CUDA include); functions are asynchronous with respect to the host unless stated.
  *   - multi-GPU: the library links no communication library and has no global state.  The packed arena of every model
@@ -785,7 +790,7 @@ void mb_logmmse_destroy(mb_logmmse* h);
 size_t mb_logmmse_arena_bytes(const mb_logmmse* h);
 int mb_logmmse_set_arena(mb_logmmse* h, void* arena, size_t bytes);
 int mb_logmmse_finalize(mb_logmmse* h, void* stream);
-/* lengths_host int32 [batch] (host); 0 when batch < 1 or a length is < 2 len2.  Also enough for mb_logmmse_profile with
+/* lengths_host int32 [batch] (host); 0 when batch < 1 or a length is < 2 len2.  Also what mb_logmmse_profile needs for
  * the same lengths. */
 size_t mb_logmmse_workspace_bytes(const mb_logmmse* h, int32_t batch, const int32_t* lengths_host);
 /* profile_noise for `batch` noise signals in one launch:

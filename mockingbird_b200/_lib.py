@@ -436,6 +436,26 @@ def require_cuda():
     return torch.device("cuda", torch.cuda.current_device())
 
 
+def workspace(need: int, device, owner=None, attr: str = "_ws"):
+    """The device workspace of a compute call (see the header's Conventions), a uint8 tensor of at least max(need, 1)
+    bytes on `device`.  With an `owner`, it is cached as owner.<attr> and grows only: the cached tensor is returned
+    while it is large enough and on `device`, and is released before a new one is allocated."""
+    import torch
+
+    device = torch.device(device)
+    if device.type == "cuda" and device.index is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    ws = getattr(owner, attr) if owner is not None else None
+    if ws is None or ws.numel() < need or ws.device != device:
+        if owner is not None:
+            setattr(owner, attr, None)
+        ws = None  # the old block is free before the new one is allocated
+        ws = torch.empty(max(need, 1), dtype=torch.uint8, device=device)
+        if owner is not None:
+            setattr(owner, attr, ws)
+    return ws
+
+
 def upload_weights(model: str, handle, weights, device, align: int = 256):
     """The weight protocol of a model handle: a zeroed arena of mb_<model>_arena_bytes aligned to `align`, set_arena,
     set_weight for every tensor of `weights` (name -> tensor, already filtered to what the model takes), finalize, then a

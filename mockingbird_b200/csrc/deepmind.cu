@@ -326,6 +326,11 @@ struct mb_deepmind {
 namespace {
 // workspace (floats): hidden [2][896] | x1 [448] | logits [512] | prev [2 ints] | barrier
 constexpr size_t WS_HIDDEN = 0, WS_X1 = 2 * H, WS_LOGITS = WS_X1 + S, WS_PREV = WS_LOGITS + 2 * Q, WS_BAR = WS_PREV + 64, WS_TOTAL = WS_BAR + 64;
+WsLayout ws_layout() {
+  WsLayout L;
+  L.take<float>(WS_TOTAL);
+  return L;
+}
 }  // namespace
 
 extern "C" {
@@ -379,18 +384,18 @@ int mb_deepmind_finalize(mb_deepmind* h, void* stream) {
   return MB_OK;
 }
 
-size_t mb_deepmind_workspace_bytes(const mb_deepmind* h) { return h ? WS_TOTAL * sizeof(float) + 256 : 0; }
+size_t mb_deepmind_workspace_bytes(const mb_deepmind* h) { return h ? ws_layout().total() : 0; }
 
 /* samples [step0, step0+nsteps) of one generate(seq_len = steps) call; step0 == 0 resets hidden / previous outputs to zero
  * (deepmind_version.py:86-91).  noise: Exp(1) draws fp32 [nsteps][2][256] (coarse draw then fine draw per sample, the order
  * Categorical.sample() consumes the torch generator) or NULL for the built-in generator.  coarse / fine: int16 [steps]. */
 int mb_deepmind_generate(mb_deepmind* h, int32_t steps, int32_t step0, int32_t nsteps, const float* noise, uint64_t seed,
                          int16_t* coarse, int16_t* fine, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h || !coarse || !fine || !workspace) return fail(MB_ERR_INVALID, "mb_deepmind_generate: null argument");
+  if (!h || !coarse || !fine) return fail(MB_ERR_INVALID, "mb_deepmind_generate: null argument");
   if (!h->finalized) return fail(MB_ERR_STATE, "mb_deepmind_generate: weights not finalized");
   if (nsteps <= 0 || step0 < 0 || step0 + nsteps > steps) return fail(MB_ERR_INVALID, "mb_deepmind_generate: bad step range");
-  if (workspace_bytes < mb_deepmind_workspace_bytes(h)) return fail(MB_ERR_WORKSPACE, "mb_deepmind_generate: workspace too small");
-  float* ws = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  float* ws;
+  if (int rc = bind("mb_deepmind_generate", workspace, workspace_bytes, ws_layout().total(), &ws)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   if (step0 == 0) MB_CUDA_CHECK(cudaMemsetAsync(ws, 0, WS_TOTAL * sizeof(float), st));
   MB_CUDA_CHECK(cudaMemsetAsync(ws + WS_BAR, 0, 256, st));

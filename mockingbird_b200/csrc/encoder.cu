@@ -142,7 +142,8 @@ GemmArgs gemm1(const float* x, int K, int ld, const float* W, int ldw, const flo
 }
 
 struct Ws {
-  size_t xproj, seq0, seq1, gates, c, raw, t_hi, t_lo, big_hi, big_lo, total;
+  size_t xproj, seq0, seq1, gates, c, raw, t_hi, t_lo, big_hi, big_lo;  // float offsets
+  size_t total;                                                         // bytes
   size_t in, last, tab;  // mb_encoder_embed_rows only: gathered input [R][T][C], last hidden rows [R][H], row table [2][R]
 };
 
@@ -157,32 +158,28 @@ bool enc_use_tc(const mb_encoder_config& c) {
 Ws ws_layout(const mb_encoder_config& c, size_t R, size_t T, bool rows = false) {
   Ws L;
   L.in = L.last = L.tab = 0;
-  size_t o = 0;
-  auto take = [&](size_t n) {
-    const size_t r = o;
-    o += align_up(n, 64);
-    return r;
-  };
+  WsLayout W;
   const size_t H = c.hidden_size;
-  L.xproj = take(R * T * 4 * H);
-  L.seq0 = take(R * T * H);
-  L.seq1 = take(R * T * H);
-  L.gates = take(R * 4 * H);
-  L.c = take(R * H);
-  L.raw = take(R * (size_t)c.embedding_size);
+  L.xproj = W.take<float>(R * T * 4 * H);
+  L.seq0 = W.take<float>(R * T * H);
+  L.seq1 = W.take<float>(R * T * H);
+  L.gates = W.take<float>(R * 4 * H);
+  L.c = W.take<float>(R * H);
+  L.raw = W.take<float>(R * (size_t)c.embedding_size);
   const size_t rows_total = (R + 127) / 128 * 128;
   const size_t tile_floats = (H / 64) * rows_total * 128 / 4;  // one operand plane (hi or lo) of h, in floats
-  L.t_hi = take(2 * tile_floats);                               // two parities
-  L.t_lo = take(2 * tile_floats);
+  L.t_hi = W.take<float>(2 * tile_floats);  // two parities
+  L.t_lo = W.take<float>(2 * tile_floats);
   const int kmax = c.hidden_size > c.mel_n_channels ? c.hidden_size : c.mel_n_channels;
-  L.big_hi = take(tc_big_act_bytes((int)(R * T), 1, kmax) / 4);  // operand tiles of the whole-sequence input projection
-  L.big_lo = take(tc_big_act_bytes((int)(R * T), 1, kmax) / 4);
+  // operand tiles of the whole-sequence input projection
+  L.big_hi = W.take<float>(tc_big_act_bytes((int)(R * T), 1, kmax) / 4);
+  L.big_lo = W.take<float>(tc_big_act_bytes((int)(R * T), 1, kmax) / 4);
   if (rows) {
-    L.in = take(R * T * (size_t)c.mel_n_channels);
-    L.last = take(R * H);
-    L.tab = take(2 * R);
+    L.in = W.take<float>(R * T * (size_t)c.mel_n_channels);
+    L.last = W.take<float>(R * H);
+    L.tab = W.take<float>(2 * R);
   }
-  L.total = o;
+  L.total = W.total();
   return L;
 }
 
@@ -408,19 +405,18 @@ int mb_encoder_finalize(mb_encoder* h, void* stream) {
 
 size_t mb_encoder_workspace_bytes(const mb_encoder* h, int32_t rows, int32_t n_frames) {
   if (!h || rows <= 0 || n_frames <= 0) return 0;
-  return ws_layout(h->cfg, rows, n_frames).total * sizeof(float) + 256;
+  return ws_layout(h->cfg, rows, n_frames).total;
 }
 
 int mb_encoder_embed_frames(mb_encoder* h, const float* frames, int32_t rows, int32_t n_frames, float* embeds,
                             void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h || !frames || !embeds || !workspace) return fail(MB_ERR_INVALID, "mb_encoder_embed_frames: null argument");
+  if (!h || !frames || !embeds) return fail(MB_ERR_INVALID, "mb_encoder_embed_frames: null argument");
   if (!h->finalized) return fail(MB_ERR_STATE, "mb_encoder_embed_frames: weights not finalized");
   if (rows <= 0 || n_frames <= 0) return fail(MB_ERR_INVALID, "mb_encoder_embed_frames: bad shape");
   const mb_encoder_config& c = h->cfg;
   const Ws L = ws_layout(c, rows, n_frames);
-  if (workspace_bytes < L.total * sizeof(float) + 256)
-    return fail(MB_ERR_WORKSPACE, "mb_encoder_embed_frames: workspace too small");
-  float* ws = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  float* ws;
+  if (int rc = bind("mb_encoder_embed_frames", workspace, workspace_bytes, L.total, &ws)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const int R = rows, T = n_frames, H = c.hidden_size, E = c.embedding_size;
   const float* top = nullptr;
@@ -436,14 +432,14 @@ int mb_encoder_embed_frames(mb_encoder* h, const float* frames, int32_t rows, in
 
 size_t mb_encoder_rows_workspace_bytes(const mb_encoder* h, int32_t rows, int32_t max_len) {
   if (!h || rows <= 0 || max_len <= 0) return 0;
-  return ws_layout(h->cfg, rows, max_len, true).total * sizeof(float) + 256;
+  return ws_layout(h->cfg, rows, max_len, true).total;
 }
 
 int mb_encoder_embed_rows(mb_encoder* h, const float* frames, int64_t n_frames, const int32_t* row_start_host,
                           const int32_t* row_len_host, int32_t rows, float* embeds, void* workspace, size_t workspace_bytes,
                           void* stream) {
   const char* fn = "mb_encoder_embed_rows";
-  if (!h || !frames || !row_start_host || !row_len_host || !embeds || !workspace) return fail(MB_ERR_INVALID, "%s: null argument", fn);
+  if (!h || !frames || !row_start_host || !row_len_host || !embeds) return fail(MB_ERR_INVALID, "%s: null argument", fn);
   if (!h->finalized) return fail(MB_ERR_STATE, "%s: weights not finalized", fn);
   if (rows <= 0) return fail(MB_ERR_INVALID, "%s: rows = %d", fn, (int)rows);
   const mb_encoder_config& c = h->cfg;
@@ -461,8 +457,8 @@ int mb_encoder_embed_rows(mb_encoder* h, const float* frames, int64_t n_frames, 
   }
   if ((int64_t)R * T * 4 * H > INT32_MAX) return fail(MB_ERR_INVALID, "%s: %d rows of up to %d frames are too many for one call", fn, R, T);
   const Ws L = ws_layout(c, R, T, true);
-  if (workspace_bytes < L.total * sizeof(float) + 256) return fail(MB_ERR_WORKSPACE, "%s: workspace too small", fn);
-  float* ws = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  float* ws;
+  if (int rc = bind(fn, workspace, workspace_bytes, L.total, &ws)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   int32_t* dtab = reinterpret_cast<int32_t*>(ws + L.tab);
   MB_CUDA_CHECK(cudaMemcpyAsync(dtab, tab.data(), tab.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));

@@ -413,14 +413,12 @@ float* buf_ptr(const mb_gan* h, int buf, const float* in, float* out, float* ws,
   return ws + offs[buf];
 }
 
+// float offsets of the FP32 path's buffers in the workspace; *total = its bytes
 std::vector<size_t> buf_offsets(const mb_gan* h, size_t B, size_t T, size_t* total) {
   std::vector<size_t> offs(h->buf_cr.size());
-  size_t o = 0;
-  for (size_t i = 0; i < h->buf_cr.size(); ++i) {
-    offs[i] = o;
-    o += align_up(B * T * h->buf_cr[i], 64);
-  }
-  *total = o;
+  WsLayout L;
+  for (size_t i = 0; i < offs.size(); ++i) offs[i] = L.take<float>(B * T * h->buf_cr[i]);
+  *total = L.total();
   return offs;
 }
 
@@ -612,34 +610,34 @@ size_t mb_gan_workspace_bytes(const mb_gan* h, int32_t batch, int32_t frames) {
   }
   size_t total = 0;
   buf_offsets(h, (size_t)batch, (size_t)frames, &total);
-  return total * sizeof(float) + 256;
+  return total;
 }
 
 static int gan_forward_impl(mb_gan* h, const float* mel, const int32_t* lengths, int32_t batch, int32_t frames,
                             float* wav, void* workspace, size_t workspace_bytes, void* stream, cudaEvent_t* events) {
-  if (!h || !mel || !wav || !workspace) return fail(MB_ERR_INVALID, "mb_gan_forward: null argument");
+  if (!h || !mel || !wav) return fail(MB_ERR_INVALID, "mb_gan_forward: null argument");
   if (!h->finalized) return fail(MB_ERR_STATE, "mb_gan_forward: weights not finalized");
   if (batch <= 0 || frames <= 0) return fail(MB_ERR_INVALID, "mb_gan_forward: empty batch");
-  const size_t need = mb_gan_workspace_bytes(h, batch, frames);
-  if (workspace_bytes < need)
-    return fail(MB_ERR_WORKSPACE, "mb_gan_forward: workspace %zu < %zu bytes", workspace_bytes, need);
+  const bool tc = h->cfg.precision != MB_PREC_FP32;
+  char* ws;
+  if (int rc = bind("mb_gan_forward", workspace, workspace_bytes, mb_gan_workspace_bytes(h, batch, frames), &ws, tc ? 1024 : 256))
+    return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  if (h->cfg.precision != MB_PREC_FP32) {
+  if (tc) {
     const std::vector<TcOp> ops = tc_ops(h);
     std::vector<TcBufReq> req;
     for (size_t i = 0; i < h->buf_cr.size(); ++i) req.push_back({h->buf_cr[i]});
     char* tcbase = (char*)h->arena + align_up(h->f32_floats * sizeof(float), 256);
-    return tc_forward(ops, req, tcbase, mel, lengths, batch, frames, h->cfg.num_mels, h->hop, wav, workspace, st,
-                      events);
+    return tc_forward(ops, req, tcbase, mel, lengths, batch, frames, h->cfg.num_mels, h->hop, wav, ws, st, events);
   }
   size_t total = 0;
   const std::vector<size_t> offs = buf_offsets(h, (size_t)batch, (size_t)frames, &total);
-  float* ws = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  float* fws = (float*)ws;
   for (const Layer& L : h->layers) {
-    const float* src = buf_ptr(h, L.src, mel, wav, ws, batch, frames, offs);
-    const float* res = buf_ptr(h, L.res, mel, wav, ws, batch, frames, offs);
-    float* dst = buf_ptr(h, L.dst, mel, wav, ws, batch, frames, offs);
-    float* dst2 = buf_ptr(h, L.dst2, mel, wav, ws, batch, frames, offs);
+    const float* src = buf_ptr(h, L.src, mel, wav, fws, batch, frames, offs);
+    const float* res = buf_ptr(h, L.res, mel, wav, fws, batch, frames, offs);
+    float* dst = buf_ptr(h, L.dst, mel, wav, fws, batch, frames, offs);
+    float* dst2 = buf_ptr(h, L.dst2, mel, wav, fws, batch, frames, offs);
     if (events) MB_CUDA_CHECK(cudaEventRecord(events[&L - &h->layers[0]], st));
     int rc = run_layer_f32(h, L, src, res, dst, dst2, lengths, batch, frames, st);
     if (rc != MB_OK) return rc;
@@ -707,6 +705,8 @@ int mb_gan_debug_layer(mb_gan* h, int32_t i, const float* x, const float* residu
                        int32_t frames_in, float* y, void* workspace, size_t workspace_bytes, void* stream) {
   if (!h || !x || !y || i < 0 || i >= (int32_t)h->layers.size())
     return fail(MB_ERR_INVALID, "mb_gan_debug_layer: bad argument");
+  // the size the tensor-core path needs is checked where its planes are laid out
+  if (int rc = bind("mb_gan_debug_layer", workspace, workspace_bytes, 0)) return rc;
   const Layer& L0 = h->layers[i];
   if (L0.kind != OP_CONV) return fail(MB_ERR_INVALID, "mb_gan_debug_layer: layer %d is not a conv", i);
   if (!L0.w_set || !L0.b_set) return fail(MB_ERR_STATE, "mb_gan_debug_layer: weights of %s not set", L0.name.c_str());
@@ -758,7 +758,7 @@ int mb_gan_tc_plan_info(const mb_gan* h, int32_t i, char* buf, size_t buflen) {
 
 int mb_gan_debug_launch(mb_gan* h, const mb_gan_debug_spec* s, void* workspace, size_t workspace_bytes, void* stream,
                         char* report, size_t report_len) {
-  if (!h || !s || !workspace || !s->x) return fail(MB_ERR_INVALID, "mb_gan_debug_launch: null argument");
+  if (!h || !s || !s->x) return fail(MB_ERR_INVALID, "mb_gan_debug_launch: null argument");
   const int32_t i = s->layer_index;
   const int32_t n = (int32_t)h->layers.size();
   if (h->cfg.precision == MB_PREC_FP32) return fail(MB_ERR_INVALID, "mb_gan_debug_launch: fp32 handle has no tensor-core layers");
@@ -828,7 +828,7 @@ int mb_gan_debug_launch(mb_gan* h, const mb_gan_debug_spec* s, void* workspace, 
 
 int mb_gan_debug_f32(mb_gan* h, const mb_gan_debug_spec* s, int32_t post_variant, void* workspace, size_t workspace_bytes,
                      void* stream, char* report, size_t report_len) {
-  if (!h || !s || !workspace || !s->x) return fail(MB_ERR_INVALID, "mb_gan_debug_f32: null argument");
+  if (!h || !s || !s->x) return fail(MB_ERR_INVALID, "mb_gan_debug_f32: null argument");
   const int32_t i = s->layer_index;
   if (i < 0 || i >= (int32_t)h->layers.size()) return fail(MB_ERR_INVALID, "mb_gan_debug_f32: bad layer %d", i);
   const Layer& L = h->layers[i];
@@ -868,10 +868,9 @@ int mb_gan_debug_f32(mb_gan* h, const mb_gan_debug_spec* s, int32_t post_variant
   const size_t b_y = yl == LAYOUT_F32B ? f32b(Cout, Lout) : 0;
   const size_t b_16 = s->out16 ? f16b(c16, Lout) : 0, b_2_16 = s->y2_out16 ? f16b(c2_16, Lout) : 0;
   const size_t need = b_x + 3 * b_y + b_16 + b_2_16;
-  if (workspace_bytes < need + 1024)
-    return fail(MB_ERR_WORKSPACE, "mb_gan_debug_f32: workspace %zu < %zu bytes", workspace_bytes, need + 1024);
+  char* ws;
+  if (int rc = bind("mb_gan_debug_f32", workspace, workspace_bytes, need + 1024, &ws, 1024)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  char* ws = (char*)(((uintptr_t)workspace + 1023) & ~(uintptr_t)1023);
   if (need) MB_CUDA_CHECK(cudaMemsetAsync(ws, 0, need, st));
   auto ref = [](const void* p, int layout, int C, int Lr) {
     TRef t = ncl(p, C, Lr);

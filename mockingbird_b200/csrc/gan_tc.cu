@@ -1008,12 +1008,23 @@ int tc_pack_weights(const TcLayer& tc, const TapConv& taps, const float* w32_sla
   return MB_OK;
 }
 
+// the fp16 (hi/lo) and fp32 planes of every buffer, byte offsets into the workspace (optional outputs)
+static WsLayout tc_layout(const std::vector<TcBufReq>& bufs, int B, int T, std::vector<size_t>* o16 = nullptr,
+                          std::vector<size_t>* o32 = nullptr) {
+  WsLayout L{1024};
+  for (const TcBufReq& b : bufs) {
+    const size_t a = L.take(f16_plane_bytes(B, T, 2 * b.cr));  // 2x: hi/lo planes
+    const size_t c = L.take(f32_plane_bytes(B, T, b.cr));
+    if (o16) o16->push_back(a), o32->push_back(c);
+  }
+  L.take(1024);  // spare
+  return L;
+}
+
 size_t tc_workspace_bytes(const std::vector<TcBufReq>& bufs, int B, int T, int num_mels, int hop) {
   (void)num_mels;
   (void)hop;
-  size_t total = 2048;
-  for (const TcBufReq& b : bufs) total += f16_plane_bytes(B, T, 2 * b.cr) + f32_plane_bytes(B, T, b.cr);  // 2x: hi/lo planes
-  return total;
+  return tc_layout(bufs, B, T).total();
 }
 
 std::vector<char> tc_fusion_plan(const std::vector<TcOp>& ops, int nb) {
@@ -1109,13 +1120,9 @@ int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, 
   // carve planes
   std::vector<char*> p16(nb), p32(nb);
   std::vector<TRef> cur16(nb), cur32(nb);  // geometry each plane currently holds
-  char* ws = (char*)(((uintptr_t)workspace + 1023) & ~(uintptr_t)1023);
-  for (int i = 0; i < nb; ++i) {
-    p16[i] = ws;
-    ws += f16_plane_bytes(B, T, 2 * bufs[i].cr);
-    p32[i] = ws;
-    ws += f32_plane_bytes(B, T, bufs[i].cr);
-  }
+  std::vector<size_t> o16, o32;
+  tc_layout(bufs, B, T, &o16, &o32);
+  for (int i = 0; i < nb; ++i) p16[i] = (char*)workspace + o16[i], p32[i] = (char*)workspace + o32[i];
   // buffer -> fp16 / fp32 plane storage (identity: every layer writes its own buffer's planes)
   std::vector<int> map16(nb);
   for (int i = 0; i < nb; ++i) map16[i] = i;
@@ -1353,8 +1360,8 @@ int tc_debug_layer(const TcOp& op, const char* tc_arena, const float* x, const f
   const int xC = op.tc.x3 ? 64 * op.tc.x_pchunks : t.Cin;  // hi/lo plane: twice the channels
   const size_t b_x16 = align_up((size_t)B * xC * f16_lp(Lin) * 2 + kPlaneSlack, 1024);
   const size_t b_r32 = align_up((size_t)B * t.Cout * Lout * 4, 1024);
-  if (workspace_bytes < b_x16 + 2 * b_r32 + 2048) return fail(MB_ERR_WORKSPACE, "tc_debug_layer: workspace too small");
-  char* ws = (char*)(((uintptr_t)workspace + 1023) & ~(uintptr_t)1023);
+  char* ws;
+  if (int rc = bind("mb_gan_debug_layer", workspace, workspace_bytes, b_x16 + 2 * b_r32 + 2048, &ws, 1024)) return rc;
   TRef x16 = make_ref(ws, LAYOUT_F16B, xC, Lin);
   x16.hilo = op.tc.x3;
   TRef r32 = residual ? make_ref(ws + b_x16, LAYOUT_F32B, t.Cout, Lout) : TRef{};
@@ -1388,8 +1395,8 @@ int tc_debug_launch(const TcOp& op, const TcOp* c2, const TcDebugSpec& s, const 
   const size_t b_x16 = f16b(xC, Lin), b_mid = c2 ? f16b(Cout, Lin) : 0, b_res = f16b(hlC, Lout),
                b_r32 = align_up((size_t)B * Cout * Lout * 4, 1024), b_y16 = f16b(y16C, Lout);
   const size_t need = b_x16 + b_mid + b_res + 2 * b_r32 + b_y16 + 1024;
-  if (workspace_bytes < need) return fail(MB_ERR_WORKSPACE, "tc_debug_launch: workspace %zu < %zu bytes", workspace_bytes, need);
-  char* ws = (char*)(((uintptr_t)workspace + 1023) & ~(uintptr_t)1023);
+  char* ws;
+  if (int rc = bind("mb_gan_debug_launch", workspace, workspace_bytes, need, &ws, 1024)) return rc;
   MB_CUDA_CHECK(cudaMemsetAsync(ws, 0, need - 1024, st));  // zero pad rows of every fp16 plane
   char* p_mid = ws + b_x16;
   char* p_res = p_mid + b_mid;

@@ -60,6 +60,7 @@ struct TcOp {
   const float* b32;
 };
 
+// workspace: 1024-byte aligned, tc_workspace_bytes of it in use
 int tc_forward(const std::vector<TcOp>& ops, const std::vector<TcBufReq>& bufs, const char* tc_arena,
                const float* mel, const int32_t* lengths, int B, int T, int num_mels, int hop, float* wav,
                void* workspace, cudaStream_t stream, cudaEvent_t* events /* nullptr or [ops+1] */);

@@ -239,18 +239,13 @@ Layout layout(int n_fft, int n_bins, int hop, int32_t batch, const int32_t* fram
     l.F += T;
     l.samples += T > 0 ? (int64_t)hop * (T - 1) : 0;
   }
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    const size_t at = off;
-    off += align_up(bytes, 256);
-    return at;
-  };
-  l.pairs = take(sizeof(int2) * (size_t)l.n_pairs);
-  l.utt = take(sizeof(GlUtt) * (size_t)batch);
-  l.S = take(sizeof(float) * (size_t)l.F * n_bins);
-  l.frames = take(sizeof(float) * (size_t)l.F * n_fft);
-  l.y = take(sizeof(float) * (size_t)l.samples);
-  l.total = off + 256;  // the workspace pointer is aligned up to 256 bytes
+  WsLayout ws;  // byte offsets
+  l.pairs = ws.take(sizeof(int2) * (size_t)l.n_pairs);
+  l.utt = ws.take(sizeof(GlUtt) * (size_t)batch);
+  l.S = ws.take(sizeof(float) * (size_t)l.F * n_bins);
+  l.frames = ws.take(sizeof(float) * (size_t)l.F * n_fft);
+  l.y = ws.take(sizeof(float) * (size_t)l.samples);
+  l.total = ws.total();
   return l;
 }
 
@@ -354,7 +349,7 @@ size_t mb_griffinlim_workspace_bytes(const mb_griffinlim* h, int32_t batch, cons
 int mb_griffinlim_forward(mb_griffinlim* h, const float* mels, const int32_t* frames_host, int32_t batch,
                           const double* uniforms, const uint64_t* seeds_host, int32_t n_iters, float* out, void* workspace,
                           size_t workspace_bytes, void* stream) {
-  if (!h || !mels || !frames_host || !out || !workspace) return fail(MB_ERR_INVALID, "mb_griffinlim_forward: null argument");
+  if (!h || !mels || !frames_host || !out) return fail(MB_ERR_INVALID, "mb_griffinlim_forward: null argument");
   if (!h->finalized) return fail(MB_ERR_STATE, "mb_griffinlim_forward: weights not finalized");
   if (batch <= 0) return fail(MB_ERR_INVALID, "mb_griffinlim_forward: batch = %d", batch);
   if (n_iters < 0) return fail(MB_ERR_INVALID, "mb_griffinlim_forward: n_iters = %d is negative", n_iters);
@@ -376,8 +371,8 @@ int mb_griffinlim_forward(mb_griffinlim* h, const float* mels, const int32_t* fr
   if (F > ((int64_t)1 << 28))
     return fail(MB_ERR_INVALID, "mb_griffinlim_forward: %lld frames are too many for one call", (long long)F);
   const Layout l = layout(N, h->n_bins, H, batch, frames_host);
-  if (workspace_bytes < l.total) return fail(MB_ERR_WORKSPACE, "mb_griffinlim_forward: workspace too small");
-  char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  char* ws;
+  if (int rc = bind("mb_griffinlim_forward", workspace, workspace_bytes, l.total, &ws)) return rc;
   // host row tables: pair -> (utterance, first local frame); utterance -> offsets and seed
   std::vector<char> host(l.S - l.pairs);
   int2* pairs = (int2*)host.data();

@@ -311,17 +311,12 @@ Layout layout(const mb_logmmse_config& c, int stride, int32_t batch, const int32
     l.n_pairs += nf > 0 ? (nf + 1) / 2 : 1;
     l.F += nf > 0 ? nf : 0;
   }
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    const size_t at = off;
-    off += align_up(bytes, 256);
-    return at;
-  };
-  l.pairs = take(sizeof(int2) * (size_t)l.n_pairs);
-  l.utt = take(sizeof(LmUtt) * (size_t)batch);
-  l.sg = take(sizeof(double) * (size_t)l.F * stride);
-  l.frames = take(sizeof(double) * (size_t)l.F * c.window_size);
-  l.total = off + 256;  // the workspace pointer is aligned up to 256 bytes
+  WsLayout ws;  // byte offsets
+  l.pairs = ws.take(sizeof(int2) * (size_t)l.n_pairs);
+  l.utt = ws.take(sizeof(LmUtt) * (size_t)batch);
+  l.sg = ws.take(sizeof(double) * (size_t)l.F * stride);
+  l.frames = ws.take(sizeof(double) * (size_t)l.F * c.window_size);
+  l.total = ws.total();
   return l;
 }
 
@@ -408,8 +403,7 @@ static int fill_params(mb_logmmse* h, const char* fn, int32_t batch, const doubl
 
 int mb_logmmse_profile(mb_logmmse* h, const float* noise, const int32_t* lengths_host, int32_t batch, const double* window,
                        double* noise_mu2, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h || !noise || !lengths_host || !window || !noise_mu2 || !workspace)
-    return fail(MB_ERR_INVALID, "mb_logmmse_profile: null argument");
+  if (!h || !noise || !lengths_host || !window || !noise_mu2) return fail(MB_ERR_INVALID, "mb_logmmse_profile: null argument");
   LmParams p;
   if (int rc = fill_params(h, "mb_logmmse_profile", batch, window, p)) return rc;
   const int W = h->cfg.window_size;
@@ -417,9 +411,10 @@ int mb_logmmse_profile(mb_logmmse* h, const float* noise, const int32_t* lengths
     if (lengths_host[b] < W)
       return fail(MB_ERR_INVALID, "mb_logmmse_profile: noise %d has %d samples, fewer than window_size = %d", b,
                   (int)lengths_host[b], W);
-  const size_t need = align_up(sizeof(LmUtt) * (size_t)batch, 256) + 256;
-  if (workspace_bytes < need) return fail(MB_ERR_WORKSPACE, "mb_logmmse_profile: workspace too small");
-  char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  // the utterance table at the start of the workspace mb_logmmse_workspace_bytes sizes for these lengths
+  char* ws;
+  if (int rc = bind("mb_logmmse_profile", workspace, workspace_bytes, mb_logmmse_workspace_bytes(h, batch, lengths_host), &ws))
+    return rc;
   std::vector<LmUtt> utt(batch);
   int64_t o = 0;
   for (int b = 0; b < batch; ++b) {
@@ -441,8 +436,7 @@ int mb_logmmse_profile(mb_logmmse* h, const float* noise, const int32_t* lengths
 int mb_logmmse_denoise(mb_logmmse* h, const float* x, const int32_t* lengths_host, int32_t batch, const double* window,
                        const double* noise_mu2, double eta, float* out, double* vad_out, void* workspace,
                        size_t workspace_bytes, void* stream) {
-  if (!h || !x || !lengths_host || !window || !noise_mu2 || !out || !workspace)
-    return fail(MB_ERR_INVALID, "mb_logmmse_denoise: null argument");
+  if (!h || !x || !lengths_host || !window || !noise_mu2 || !out) return fail(MB_ERR_INVALID, "mb_logmmse_denoise: null argument");
   LmParams p;
   if (int rc = fill_params(h, "mb_logmmse_denoise", batch, window, p)) return rc;
   const mb_logmmse_config& c = h->cfg;
@@ -456,8 +450,8 @@ int mb_logmmse_denoise(mb_logmmse* h, const float* x, const int32_t* lengths_hos
   if (F > ((int64_t)1 << 28))
     return fail(MB_ERR_INVALID, "mb_logmmse_denoise: %lld frames are too many for one call", (long long)F);
   const Layout l = layout(c, h->stride, batch, lengths_host);
-  if (workspace_bytes < l.total) return fail(MB_ERR_WORKSPACE, "mb_logmmse_denoise: workspace too small");
-  char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  char* ws;
+  if (int rc = bind("mb_logmmse_denoise", workspace, workspace_bytes, l.total, &ws)) return rc;
   // host tables: pair -> (utterance, first local frame), one placeholder pair for an utterance without frames;
   // utterance -> first frame, frame count, first sample, length
   std::vector<char> host(l.sg - l.pairs);

@@ -1,4 +1,4 @@
-// Shared host-side helpers for libmockingbird_b200 (error reporting, launch counting, the weight table).
+// Shared host-side helpers for libmockingbird_b200 (error reporting, launch counting, the weight table, workspaces).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdarg>
@@ -41,6 +41,38 @@ static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; 
 // The weight-upload protocol of every model handle (set_arena, set_weight per tensor, finalize): null, size and
 // alignment check of an arena.  `fn` names the entry point in the error message.
 int check_arena(const char* fn, const void* h, const void* arena, size_t bytes, size_t need, size_t align);
+
+// The regions of a compute call's workspace, handed out in declaration order, each rounded up to `align` bytes.  total()
+// adds `align` bytes of slack so that any workspace pointer can be aligned up in place.  A `*_workspace_bytes` query and
+// its compute call build the same layout.
+struct WsLayout {
+  size_t align = 256, bytes = 0;
+  // n elements of T; the offset comes back in elements of T
+  template <class T = char>
+  size_t take(size_t n) {
+    const size_t at = bytes;
+    bytes += align_up(n * sizeof(T), align);
+    return at / sizeof(T);
+  }
+  size_t total() const { return bytes + align; }
+};
+
+// `ws` aligned up to `align` bytes
+template <class T = char>
+T* aligned(void* ws, size_t align = 256) {
+  return (T*)(((uintptr_t)ws + align - 1) & ~(uintptr_t)(align - 1));
+}
+
+// The workspace of compute entry point `fn`: MB_ERR_INVALID if it is null, MB_ERR_WORKSPACE if it has fewer than `need`
+// bytes, otherwise *base (if given) is the workspace aligned up to `align` bytes.  Call it before any CUDA call of the entry
+// point.
+template <class T = char>
+int bind(const char* fn, void* ws, size_t bytes, size_t need, T** base = nullptr, size_t align = 256) {
+  if (!ws) return fail(MB_ERR_INVALID, "%s: null workspace", fn);
+  if (bytes < need) return fail(MB_ERR_WORKSPACE, "%s: workspace too small (%zu < %zu bytes)", fn, bytes, need);
+  if (base) *base = aligned<T>(ws, align);
+  return MB_OK;
+}
 
 // The tensors at the start of a model's arena, laid out in declaration order at align_up(n, 64) floats each.  A
 // checkpoint tensor has an exact shape, is settable and is required by finalize; a derived region of n floats is

@@ -292,10 +292,11 @@ int mb_melspec_forward_ragged(mb_melspec* h, const float* wavs, const int32_t* l
                               const int32_t* signal_lengths_host, int32_t batch, float* out, void* workspace,
                               size_t workspace_bytes, void* stream) {
   const char* fn = "mb_melspec_forward_ragged";
-  if (!h || !wavs || !lengths_host || !out || !workspace) return fail(MB_ERR_INVALID, "%s: null argument", fn);
+  if (!h || !wavs || !lengths_host || !out) return fail(MB_ERR_INVALID, "%s: null argument", fn);
   if (!h->arena) return fail(MB_ERR_STATE, "%s: call mb_melspec_set_arena first", fn);
   if (batch <= 0) return fail(MB_ERR_INVALID, "%s: batch = %d", fn, (int)batch);
-  if (workspace_bytes < mb_melspec_ragged_workspace_bytes(h, batch)) return fail(MB_ERR_WORKSPACE, "%s: workspace too small", fn);
+  MelUtt* dutt;
+  if (int rc = bind(fn, workspace, workspace_bytes, mb_melspec_ragged_workspace_bytes(h, batch), &dutt)) return rc;
   std::vector<MelUtt> utt(batch);
   long long o = 0, f0 = 0;
   for (int b = 0; b < batch; ++b) {
@@ -308,7 +309,6 @@ int mb_melspec_forward_ragged(mb_melspec* h, const float* wavs, const int32_t* l
     f0 += nf;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  MelUtt* dutt = (MelUtt*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
   MB_CUDA_CHECK(cudaMemcpyAsync(dutt, utt.data(), sizeof(MelUtt) * utt.size(), cudaMemcpyHostToDevice, st));
   MelParams p = base_params(h);
   p.wav = wavs;

@@ -26,6 +26,7 @@
 using mb::check_arena;
 using mb::fail;
 using mb::WeightTable;
+using mb::WsLayout;
 
 namespace {
 
@@ -592,39 +593,34 @@ void build_specs(mb_ppg2mel* h) {
   h->total_floats = off;
 }
 
-// per-call workspace layout (bytes, 256-aligned regions)
-struct WsLayout {
+// per-call workspace layout (byte offsets)
+struct Ws {
   size_t ints, rowbias, x0, x1, e1, e2, mem, ah, ac, dh, dc, ctx, mu, frame, pre, q, p0, p1, total;
 };
 
-WsLayout ws_layout(int B, int T) {
-  WsLayout L{};
+Ws ws_layout(int B, int T) {
+  Ws L{};
   const size_t T1 = T / 2, T2 = T1 / 2, S = 2 * T2;
-  size_t o = 0;
-  auto take = [&](size_t floats) {
-    const size_t r = o;
-    o += mb::align_up(floats * 4, 256);
-    return r;
-  };
-  L.ints = take(8 * kMaxRows + 8);
-  L.rowbias = take((size_t)B * kE);
-  L.x0 = take((size_t)B * T * kE);
-  L.x1 = take((size_t)B * T1 * kE);
-  L.e1 = take((size_t)B * T2 * kE);
-  L.e2 = take((size_t)B * T2 * kE);
-  L.mem = take((size_t)B * T2 * kE);
-  L.ah = take((size_t)2 * B * kH);
-  L.ac = take((size_t)B * kH);
-  L.dh = take((size_t)2 * B * kH);
-  L.dc = take((size_t)B * kH);
-  L.ctx = take((size_t)B * kE);
-  L.mu = take((size_t)B * 8);
-  L.frame = take((size_t)B * kNM);
-  L.pre = take((size_t)B * kP2);
-  L.q = take((size_t)B * kQ);
-  L.p0 = take((size_t)B * 2 * S * 512);
-  L.p1 = take((size_t)B * 2 * S * 512);
-  L.total = o;
+  WsLayout W;
+  L.ints = W.take(sizeof(float) * (8 * kMaxRows + 8));
+  L.rowbias = W.take(sizeof(float) * (size_t)B * kE);
+  L.x0 = W.take(sizeof(float) * (size_t)B * T * kE);
+  L.x1 = W.take(sizeof(float) * (size_t)B * T1 * kE);
+  L.e1 = W.take(sizeof(float) * (size_t)B * T2 * kE);
+  L.e2 = W.take(sizeof(float) * (size_t)B * T2 * kE);
+  L.mem = W.take(sizeof(float) * (size_t)B * T2 * kE);
+  L.ah = W.take(sizeof(float) * (size_t)2 * B * kH);
+  L.ac = W.take(sizeof(float) * (size_t)B * kH);
+  L.dh = W.take(sizeof(float) * (size_t)2 * B * kH);
+  L.dc = W.take(sizeof(float) * (size_t)B * kH);
+  L.ctx = W.take(sizeof(float) * (size_t)B * kE);
+  L.mu = W.take(sizeof(float) * (size_t)B * 8);
+  L.frame = W.take(sizeof(float) * (size_t)B * kNM);
+  L.pre = W.take(sizeof(float) * (size_t)B * kP2);
+  L.q = W.take(sizeof(float) * (size_t)B * kQ);
+  L.p0 = W.take(sizeof(float) * (size_t)B * 2 * S * 512);
+  L.p1 = W.take(sizeof(float) * (size_t)B * 2 * S * 512);
+  L.total = W.total();
   return L;
 }
 
@@ -807,7 +803,7 @@ int mb_ppg2mel_inference(mb_ppg2mel* h, const float* ppg, const float* lf0_uv, c
   if (frames / 4 > te_max)
     return fail(MB_ERR_INVALID, "mb_ppg2mel_inference: frames %d gives T_enc %d > %d, the most the MoL attention's shared "
                 "memory holds (frames <= %d)", frames, frames / 4, te_max, 4 * te_max + 3);
-  if (!ppg || !lf0_uv || !spk || !lengths || !mel || !mel_post || !align || !steps_host || !workspace)
+  if (!ppg || !lf0_uv || !spk || !lengths || !mel || !mel_post || !align || !steps_host)
     return fail(MB_ERR_INVALID, "mb_ppg2mel_inference: null argument");
   if ((mask1 == nullptr) != (mask2 == nullptr))
     return fail(MB_ERR_INVALID, "mb_ppg2mel_inference: pass both dropout masks or neither");
@@ -817,11 +813,11 @@ int mb_ppg2mel_inference(mb_ppg2mel* h, const float* ppg, const float* lf0_uv, c
       return fail(MB_ERR_INVALID, "mb_ppg2mel_inference: lengths[%d] = %d outside 4..%d", b, lengths[b], frames);
     lens.v[b] = lengths[b];
   }
-  const WsLayout L = ws_layout(batch, frames);
-  if (workspace_bytes < L.total) return fail(MB_ERR_WORKSPACE, "mb_ppg2mel_inference: workspace too small");
+  const Ws L = ws_layout(batch, frames);
+  char* ws;
+  if (int rc = mb::bind("mb_ppg2mel_inference", workspace, workspace_bytes, L.total, &ws)) return rc;
   const int B = batch, T = frames, T1 = T / 2, T2 = T1 / 2, S = 2 * T2;
   const int Dp = h->cfg.bottle_neck_feature_dim, Ds = h->cfg.spk_embed_dim;
-  char* ws = static_cast<char*>(workspace);
   auto F = [&](size_t off) { return reinterpret_cast<float*>(ws + off); };
   int* ints = reinterpret_cast<int*>(ws + L.ints);
   State s{ints, ints + kMaxRows, ints + 2 * kMaxRows, ints + 3 * kMaxRows, ints + 4 * kMaxRows, ints + 5 * kMaxRows,

@@ -575,13 +575,13 @@ void build_specs(mb_ppgx* h) {
   h->total_bytes = bytes;
 }
 
-struct WsLayout {
-  size_t ints, feat, pl_hi, pl_lo, e_hi, e_lo, x, y, ctx, t_hi, t_lo, pt_hi, pt_lo, P, total;
+struct Ws {
+  size_t ints, feat, pl_hi, pl_lo, e_hi, e_lo, x, y, ctx, t_hi, t_lo, pt_hi, pt_lo, P, total;  // bytes
   int Tf, T1, T, M, RT, RTp, KBe, KBt, KBd;
 };
 
-WsLayout ws_layout(const mb_ppgx* h, int B, int n_max) {
-  WsLayout L{};
+Ws ws_layout(const mb_ppgx* h, int B, int n_max) {
+  Ws L{};
   L.Tf = h->frames_stft(n_max);
   L.T1 = h->frames1(n_max);
   L.T = h->frames(n_max);
@@ -592,29 +592,24 @@ WsLayout ws_layout(const mb_ppgx* h, int B, int n_max) {
   L.KBd = kb_of(h->D);
   L.KBt = std::max(kb_of(h->D), kb_of(h->U));
   const int wide = std::max(std::max(3 * h->D, h->U), 2 * h->D);
-  size_t o = 0;
-  auto take = [&](size_t bytes) {
-    const size_t r = o;
-    o += mb::align_up(bytes, 256);
-    return r;
-  };
-  L.ints = take(sizeof(int) * 4 * kMaxRows);
-  L.feat = take(sizeof(float) * (size_t)B * L.Tf * h->F);
-  L.pl_hi = take(sizeof(__half) * (size_t)B * L.T1 * h->F1 * h->D);
-  L.pl_lo = take(sizeof(__half) * (size_t)B * L.T1 * h->F1 * h->D);
-  L.e_hi = take(sizeof(__half) * (size_t)L.KBe * L.RT * 64);
-  L.e_lo = take(sizeof(__half) * (size_t)L.KBe * L.RT * 64);
-  L.x = take(sizeof(float) * (size_t)L.M * h->D);
-  L.y = take(sizeof(float) * (size_t)L.M * wide);
-  L.ctx = take(sizeof(float) * (size_t)L.M * h->D);
-  L.t_hi = take(sizeof(__half) * (size_t)L.KBt * L.RT * 64);
-  L.t_lo = take(sizeof(__half) * (size_t)L.KBt * L.RT * 64);
+  WsLayout W;
+  L.ints = W.take(sizeof(int) * 4 * kMaxRows);
+  L.feat = W.take(sizeof(float) * (size_t)B * L.Tf * h->F);
+  L.pl_hi = W.take(sizeof(__half) * (size_t)B * L.T1 * h->F1 * h->D);
+  L.pl_lo = W.take(sizeof(__half) * (size_t)B * L.T1 * h->F1 * h->D);
+  L.e_hi = W.take(sizeof(__half) * (size_t)L.KBe * L.RT * 64);
+  L.e_lo = W.take(sizeof(__half) * (size_t)L.KBe * L.RT * 64);
+  L.x = W.take(sizeof(float) * (size_t)L.M * h->D);
+  L.y = W.take(sizeof(float) * (size_t)L.M * wide);
+  L.ctx = W.take(sizeof(float) * (size_t)L.M * h->D);
+  L.t_hi = W.take(sizeof(__half) * (size_t)L.KBt * L.RT * 64);
+  L.t_lo = W.take(sizeof(__half) * (size_t)L.KBt * L.RT * 64);
   if (h->rel) {
-    L.pt_hi = take(sizeof(__half) * (size_t)L.KBd * L.RTp * 64);
-    L.pt_lo = take(sizeof(__half) * (size_t)L.KBd * L.RTp * 64);
-    L.P = take(sizeof(float) * (size_t)L.T * h->nb * h->D);
+    L.pt_hi = W.take(sizeof(__half) * (size_t)L.KBd * L.RTp * 64);
+    L.pt_lo = W.take(sizeof(__half) * (size_t)L.KBd * L.RTp * 64);
+    L.P = W.take(sizeof(float) * (size_t)L.T * h->nb * h->D);
   }
-  L.total = o;
+  L.total = W.total();
   return L;
 }
 
@@ -935,11 +930,11 @@ int mb_ppgx_forward(mb_ppgx* h, const float* wav, const int32_t* n_samples, int3
   if (!h) return fail(MB_ERR_INVALID, "mb_ppgx_forward: null handle");
   if (!h->finalized) return fail(MB_ERR_STATE, "mb_ppgx_forward: weights not finalized");
   if (batch < 1 || batch > kMaxRows) return fail(MB_ERR_INVALID, "mb_ppgx_forward: batch %d outside 1..%d", batch, kMaxRows);
-  if (!wav || !n_samples || !pos_table || !out || !workspace) return fail(MB_ERR_INVALID, "mb_ppgx_forward: null argument");
-  const size_t need = mb_ppgx_workspace_bytes(h, batch, n_max);
-  if (need == 0) return fail(MB_ERR_INVALID, "mb_ppgx_forward: n_max %d gives no frames", n_max);
-  if (workspace_bytes < need) return fail(MB_ERR_WORKSPACE, "mb_ppgx_forward: workspace %zu < %zu bytes", workspace_bytes, need);
-  const WsLayout L = ws_layout(h, batch, n_max);
+  if (!wav || !n_samples || !pos_table || !out) return fail(MB_ERR_INVALID, "mb_ppgx_forward: null argument");
+  if (mb_ppgx_workspace_bytes(h, batch, n_max) == 0) return fail(MB_ERR_INVALID, "mb_ppgx_forward: n_max %d gives no frames", n_max);
+  const Ws L = ws_layout(h, batch, n_max);
+  char* ws;
+  if (int rc = bind("mb_ppgx_forward", workspace, workspace_bytes, L.total, &ws)) return rc;
   if (h->rel && pe_len < L.T) return fail(MB_ERR_INVALID, "mb_ppgx_forward: pe_len %d < %d frames", pe_len, L.T);
   h->host_ints.assign(4 * kMaxRows, 0);
   for (int b = 0; b < batch; ++b) {
@@ -953,7 +948,6 @@ int mb_ppgx_forward(mb_ppgx* h, const float* wav, const int32_t* n_samples, int3
     h->host_ints[3 * kMaxRows + b] = h->frames(n);
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  char* ws = static_cast<char*>(workspace);
   int* d_ints = reinterpret_cast<int*>(ws + L.ints);
   const int *d_n = d_ints, *d_tf = d_ints + kMaxRows, *d_t1 = d_ints + 2 * kMaxRows, *d_t = d_ints + 3 * kMaxRows;
   MB_CUDA_CHECK(cudaMemcpyAsync(d_ints, h->host_ints.data(), sizeof(int) * 4 * kMaxRows, cudaMemcpyHostToDevice, st));
@@ -1046,16 +1040,21 @@ int mb_ppgx_forward(mb_ppgx* h, const float* wav, const int32_t* n_samples, int3
 size_t mb_ppgx_debug_workspace_bytes(const mb_ppgx_debug_spec* s) {
   if (!s) return 0;
   if (s->kind != MB_PPGX_DBG_CONV2D_TC) return 256;
-  return 2048 + mb::align_up(ppgx::conv2d_tc_weight_bytes(s->N, s->C, s->k, s->k), 1024);  // absmax slot, then the image
+  WsLayout L{1024};
+  L.take<unsigned int>(1);  // absmax slot, then the image
+  L.take(ppgx::conv2d_tc_weight_bytes(s->N, s->C, s->k, s->k));
+  return L.total();
 }
 
 int mb_ppgx_debug(const mb_ppgx_debug_spec* spec, void* workspace, size_t workspace_bytes, void* stream, char* report,
                   size_t report_len) {
   const char* me = "mb_ppgx_debug";
-  if (!spec || !workspace) return fail(MB_ERR_INVALID, "%s: null argument", me);
+  if (!spec) return fail(MB_ERR_INVALID, "%s: null argument", me);
   const mb_ppgx_debug_spec& s = *spec;
-  const size_t need = mb_ppgx_debug_workspace_bytes(spec);
-  if (workspace_bytes < need) return fail(MB_ERR_WORKSPACE, "%s: workspace %zu < %zu bytes", me, workspace_bytes, need);
+  char* ws;
+  // only CONV2D_TC uses its workspace: the 1024-byte aligned absmax slot and weight image
+  const size_t align = s.kind == MB_PPGX_DBG_CONV2D_TC ? 1024 : 256;
+  if (int rc = bind(me, workspace, workspace_bytes, mb_ppgx_debug_workspace_bytes(spec), &ws, align)) return rc;
   const bool rows = s.kind != MB_PPGX_DBG_LN_TILES && s.kind != MB_PPGX_DBG_ACT_TILES;  // kinds over a padded batch
   if (rows && (s.B < 1 || s.T < 1 || !s.len)) return fail(MB_ERR_INVALID, "%s: B %d / T %d / len", me, s.B, s.T);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1103,12 +1102,8 @@ int mb_ppgx_debug(const mb_ppgx_debug_spec* spec, void* workspace, size_t worksp
         return fail(MB_ERR_INVALID, "%s: conv2d N %d / C %d / output %d x %d / rows_total %d", me, s.N, s.C, c.T_out, c.F_out,
                     s.rows_total);
       // as finalize: max |w| -> power-of-two scale (one host read-back) -> packed image
-      char* ws = reinterpret_cast<char*>(((uintptr_t)workspace + 1023) & ~(uintptr_t)1023);
       unsigned int* d_abs = reinterpret_cast<unsigned int*>(ws);
       __half* img = reinterpret_cast<__half*>(ws + 1024);
-      if (reinterpret_cast<char*>(img) + ppgx::conv2d_tc_weight_bytes(s.N, s.C, s.k, s.k) >
-          static_cast<char*>(workspace) + workspace_bytes)
-        return fail(MB_ERR_WORKSPACE, "%s: workspace too small for the weight image", me);
       MB_CUDA_CHECK(cudaMemsetAsync(d_abs, 0, sizeof(unsigned int), st));
       cudaError_t e = taco::tc_skinny_absmax(s.w, (size_t)s.N * s.C * s.k * s.k, d_abs, st);
       if (e != cudaSuccess) return fail(MB_ERR_CUDA, "absmax: %s", cudaGetErrorString(e));

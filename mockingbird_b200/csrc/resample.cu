@@ -239,8 +239,6 @@ struct Filter {
   int64_t off;               // floats from the arena start (a multiple of 4)
 };
 
-char* aligned_ws(void* ws) { return (char*)(((uintptr_t)ws + 255) & ~(uintptr_t)255); }
-
 }  // namespace
 
 struct mb_resample {
@@ -398,20 +396,18 @@ int mb_resample_work_items(const mb_resample* h, const int32_t* lengths_host, co
 
 int mb_resample_forward(mb_resample* h, const void* x, int32_t dtype, const int32_t* lengths_host, const int32_t* filters_host,
                         int32_t batch, float* out, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h || !x || !lengths_host || !filters_host || !out || !workspace)
-    return fail(MB_ERR_INVALID, "mb_resample_forward: null argument");
+  if (!h || !x || !lengths_host || !filters_host || !out) return fail(MB_ERR_INVALID, "mb_resample_forward: null argument");
   if (dtype != MB_RESAMPLE_F32 && dtype != MB_RESAMPLE_I16)
     return fail(MB_ERR_INVALID, "mb_resample_forward: dtype = %d", (int)dtype);
   if ((uintptr_t)x % 16) return fail(MB_ERR_INVALID, "mb_resample_forward: x must be 16-byte aligned");
-  if (workspace_bytes < mb_resample_workspace_bytes(h, batch))
-    return fail(MB_ERR_WORKSPACE, "mb_resample_forward: workspace too small");
+  char* ws;
+  if (int rc = bind("mb_resample_forward", workspace, workspace_bytes, mb_resample_workspace_bytes(h, batch), &ws)) return rc;
   std::vector<RsClip> clips;
   int64_t tiles = 0, win_max = 0, filt_max = 0;
   if (int rc = plan(h, "mb_resample_forward", dtype, lengths_host, filters_host, batch, clips, tiles, win_max, filt_max))
     return rc;
   for (int b = 0; b < batch && !h->finalized; ++b)
     if (filters_host[b] >= 0) return fail(MB_ERR_STATE, "mb_resample_forward: clip %d: filters not finalized", b);
-  char* ws = aligned_ws(workspace);
   cudaStream_t st = (cudaStream_t)stream;
   MB_CUDA_CHECK(cudaMemcpyAsync(ws, clips.data(), sizeof(RsClip) * clips.size(), cudaMemcpyHostToDevice, st));
   RsParams p{x, out, (const RsClip*)ws, h->arena, batch, (int32_t)align_up((size_t)win_max, 16)};
@@ -431,7 +427,8 @@ size_t mb_resample_level_workspace_bytes(int32_t batch) {
 static int level_table(const char* fn, const int32_t* lengths_host, int32_t batch, void* workspace, size_t workspace_bytes,
                        cudaStream_t st, const LvClip** table, int32_t* max_len) {
   if (batch < 1) return fail(MB_ERR_INVALID, "%s: batch = %d", fn, (int)batch);
-  if (workspace_bytes < mb_resample_level_workspace_bytes(batch)) return fail(MB_ERR_WORKSPACE, "%s: workspace too small", fn);
+  LvClip* ws;
+  if (int rc = bind(fn, workspace, workspace_bytes, mb_resample_level_workspace_bytes(batch), &ws)) return rc;
   std::vector<LvClip> clips(batch);
   int64_t off = 0;
   *max_len = 0;
@@ -441,15 +438,14 @@ static int level_table(const char* fn, const int32_t* lengths_host, int32_t batc
     off += lengths_host[b];
     *max_len = std::max(*max_len, lengths_host[b]);
   }
-  char* ws = aligned_ws(workspace);
   MB_CUDA_CHECK(cudaMemcpyAsync(ws, clips.data(), sizeof(LvClip) * clips.size(), cudaMemcpyHostToDevice, st));
-  *table = (const LvClip*)ws;
+  *table = ws;
   return MB_OK;
 }
 
 int mb_resample_sumsq(const float* x, const int32_t* lengths_host, int32_t batch, float* sumsq, void* workspace,
                       size_t workspace_bytes, void* stream) {
-  if (!x || !lengths_host || !sumsq || !workspace) return fail(MB_ERR_INVALID, "mb_resample_sumsq: null argument");
+  if (!x || !lengths_host || !sumsq) return fail(MB_ERR_INVALID, "mb_resample_sumsq: null argument");
   cudaStream_t st = (cudaStream_t)stream;
   const LvClip* t;
   int32_t n_max;
@@ -461,7 +457,7 @@ int mb_resample_sumsq(const float* x, const int32_t* lengths_host, int32_t batch
 
 int mb_resample_scale(const float* x, const int32_t* lengths_host, int32_t batch, const float* gains, float* y, void* workspace,
                       size_t workspace_bytes, void* stream) {
-  if (!x || !lengths_host || !gains || !y || !workspace) return fail(MB_ERR_INVALID, "mb_resample_scale: null argument");
+  if (!x || !lengths_host || !gains || !y) return fail(MB_ERR_INVALID, "mb_resample_scale: null argument");
   cudaStream_t st = (cudaStream_t)stream;
   const LvClip* t;
   int32_t n_max;
@@ -474,7 +470,7 @@ int mb_resample_scale(const float* x, const int32_t* lengths_host, int32_t batch
 
 int mb_resample_rescale(const float* x, const int32_t* lengths_host, int32_t batch, float peak, float* y, void* workspace,
                         size_t workspace_bytes, void* stream) {
-  if (!x || !lengths_host || !y || !workspace) return fail(MB_ERR_INVALID, "mb_resample_rescale: null argument");
+  if (!x || !lengths_host || !y) return fail(MB_ERR_INVALID, "mb_resample_rescale: null argument");
   cudaStream_t st = (cudaStream_t)stream;
   const LvClip* t;
   int32_t n_max;

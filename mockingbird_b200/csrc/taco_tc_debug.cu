@@ -3,6 +3,7 @@
 // the tests compare each kernel, at shapes and launch variants the models never reach, with a float64 reference of its operation.
 #include <cuda_fp16.h>
 
+#include <algorithm>
 #include <cstdio>
 #include <cstring>
 
@@ -20,7 +21,7 @@ namespace {
     count_launch();                                                                                                        \
   } while (0)
 
-struct DebugWs {      // byte offsets into the workspace (256-byte aligned)
+struct DebugWs {      // byte offsets into the workspace
   size_t absmax;      // 2 x uint
   size_t w[2], bias[2], a_hi[2], a_lo[2], nxt_hi[2], nxt_lo[2];
   size_t w_bytes, bias_bytes, a_bytes;  // per direction
@@ -56,22 +57,17 @@ DebugWs debug_layout(const mb_taco_tc_debug_spec& s) {
       L.a_bytes = tc_big_act_bytes(s.M, s.nseg, K);
       break;
   }
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    const size_t o = off;
-    off += align_up(bytes > 0 ? bytes : 1, 256);
-    return o;
-  };
-  L.absmax = take(2 * sizeof(unsigned int));
+  WsLayout W;
+  L.absmax = W.take<unsigned int>(2);
   for (int d = 0; d < ndir; ++d) {
-    L.w[d] = take(L.w_bytes);
-    L.bias[d] = take(L.bias_bytes);
-    L.a_hi[d] = take(L.a_bytes);
-    L.a_lo[d] = take(L.a_bytes);
-    L.nxt_hi[d] = take(L.a_bytes);
-    L.nxt_lo[d] = take(L.a_bytes);
+    L.w[d] = W.take(L.w_bytes);
+    L.bias[d] = W.take(std::max<size_t>(L.bias_bytes, 1));  // a region of its own even where the kind has no bias
+    L.a_hi[d] = W.take(L.a_bytes);
+    L.a_lo[d] = W.take(L.a_bytes);
+    L.nxt_hi[d] = W.take(L.a_bytes);
+    L.nxt_lo[d] = W.take(L.a_bytes);
   }
-  L.total = off + 256;
+  L.total = W.total();
   return L;
 }
 
@@ -116,13 +112,13 @@ size_t mb_taco_tc_debug_workspace_bytes(const mb_taco_tc_debug_spec* spec) {
 
 int mb_taco_tc_debug(const mb_taco_tc_debug_spec* spec, void* workspace, size_t workspace_bytes, void* stream, char* report,
                      size_t report_len) {
-  if (!spec || !workspace) return fail(MB_ERR_INVALID, "mb_taco_tc_debug: null argument");
+  if (!spec) return fail(MB_ERR_INVALID, "mb_taco_tc_debug: null argument");
   const mb_taco_tc_debug_spec& s = *spec;
   int rc = check_spec(s);
   if (rc != MB_OK) return rc;
   const DebugWs L = debug_layout(s);
-  if (workspace_bytes < L.total) return fail(MB_ERR_WORKSPACE, "mb_taco_tc_debug: workspace %zu < %zu bytes", workspace_bytes, L.total);
-  char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  char* ws;
+  if ((rc = bind("mb_taco_tc_debug", workspace, workspace_bytes, L.total, &ws))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   auto half_at = [&](size_t off) { return reinterpret_cast<__half*>(ws + off); };
   const int K = spec_K(s);

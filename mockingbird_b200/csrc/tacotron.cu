@@ -535,92 +535,90 @@ struct Ws {
   size_t big_hi, big_lo, big_bytes;
   // outputs / postnet
   size_t mel_all, scores_all, pbank, ppool, ppj1, ppj2, py, phw12, pgi_f, pgi_b, pgh, phst, pout, lin;
-  size_t total;
+  // ragged batches only: int32 characters, caps (decoder steps), done step, frames [B] each, seeds [B] u64
+  size_t rows;
+  size_t total;  // bytes; every other field is an offset in floats
 };
 
-Ws ws_layout(const mb_tacotron_config& c, int B, int Tc, int steps, int r) {
+Ws ws_layout(const mb_tacotron_config& c, int B, int Tc, int steps, int r, bool ragged = false) {
   Ws L{};
-  size_t o = 0;
-  auto take = [&](size_t n) {
-    size_t q = o;
-    o += align_up(n, 64);
-    return q;
-  };
+  WsLayout W;
   const size_t Me = (size_t)B * Tc, Mp = (size_t)B * steps;
   const int E = c.encoder_dims, PD = c.postnet_dims, proj_dims = E + c.speaker_embedding_size + c.gst_E;
-  L.ids = take(Me);
-  L.emb = take(Me * c.embed_dims);
-  L.m_enc = take((2 * Me * E + 3) / 4 + 64);  // uint8 masks
-  L.p1 = take(Me * E);
-  L.x0 = take(Me * E);
-  L.bank = take(Me * c.encoder_K * E);
-  L.pool = take(Me * c.encoder_K * E);
-  L.pj1 = take(Me * E);
-  L.y = take(Me * E);
-  L.hw12 = take(Me * 2 * E);
-  L.gi_f = take(Me * 3 * (E / 2));
-  L.gi_b = take(Me * 3 * (E / 2));
-  L.gh = take((size_t)2 * B * 3 * (PD / 2));
-  L.hst = take((size_t)2 * B * (PD / 2));
-  L.seq = take(Me * proj_dims);
-  L.proj = take(Me * c.decoder_dims);
-  L.style_q = take((size_t)B * c.gst_E);
-  L.style = take((size_t)B * c.gst_E);
-  L.attn_h = take((size_t)B * c.decoder_dims);
-  L.h1 = take((size_t)B * c.lstm_dims);
-  L.c1 = take((size_t)B * c.lstm_dims);
-  L.h2 = take((size_t)B * c.lstm_dims);
-  L.c2 = take((size_t)B * c.lstm_dims);
-  L.ctx = take((size_t)B * proj_dims);
-  L.cum = take(Me);
-  L.dp1 = take((size_t)B * 2 * c.decoder_dims);
-  L.dp2 = take((size_t)B * 2 * c.decoder_dims);
-  L.dgi = take((size_t)B * 3 * c.decoder_dims);
-  L.dgh = take((size_t)B * 3 * c.decoder_dims);
-  L.pq = take((size_t)B * c.decoder_dims);
-  L.x = take((size_t)B * c.lstm_dims);
-  L.gates = take((size_t)B * 4 * c.lstm_dims);
-  L.a_hi = take(tc_skinny_act_bytes(B > 128 ? 128 : B, 2 * c.lstm_dims) / 4);
-  L.a_lo = take(tc_skinny_act_bytes(B > 128 ? 128 : B, 2 * c.lstm_dims) / 4);
-  L.ah_hi = take(2 * tc_skinny_act_bytes(B > 128 ? 128 : B, c.decoder_dims) / 4);  // attention-GRU state tiles, 2 parities
-  L.ah_lo = take(2 * tc_skinny_act_bytes(B > 128 ? 128 : B, c.decoder_dims) / 4);
+  L.ids = W.take<float>(Me);
+  L.emb = W.take<float>(Me * c.embed_dims);
+  L.m_enc = W.take<float>((2 * Me * E + 3) / 4 + 64);  // uint8 masks
+  L.p1 = W.take<float>(Me * E);
+  L.x0 = W.take<float>(Me * E);
+  L.bank = W.take<float>(Me * c.encoder_K * E);
+  L.pool = W.take<float>(Me * c.encoder_K * E);
+  L.pj1 = W.take<float>(Me * E);
+  L.y = W.take<float>(Me * E);
+  L.hw12 = W.take<float>(Me * 2 * E);
+  L.gi_f = W.take<float>(Me * 3 * (E / 2));
+  L.gi_b = W.take<float>(Me * 3 * (E / 2));
+  L.gh = W.take<float>((size_t)2 * B * 3 * (PD / 2));
+  L.hst = W.take<float>((size_t)2 * B * (PD / 2));
+  L.seq = W.take<float>(Me * proj_dims);
+  L.proj = W.take<float>(Me * c.decoder_dims);
+  L.style_q = W.take<float>((size_t)B * c.gst_E);
+  L.style = W.take<float>((size_t)B * c.gst_E);
+  L.attn_h = W.take<float>((size_t)B * c.decoder_dims);
+  L.h1 = W.take<float>((size_t)B * c.lstm_dims);
+  L.c1 = W.take<float>((size_t)B * c.lstm_dims);
+  L.h2 = W.take<float>((size_t)B * c.lstm_dims);
+  L.c2 = W.take<float>((size_t)B * c.lstm_dims);
+  L.ctx = W.take<float>((size_t)B * proj_dims);
+  L.cum = W.take<float>(Me);
+  L.dp1 = W.take<float>((size_t)B * 2 * c.decoder_dims);
+  L.dp2 = W.take<float>((size_t)B * 2 * c.decoder_dims);
+  L.dgi = W.take<float>((size_t)B * 3 * c.decoder_dims);
+  L.dgh = W.take<float>((size_t)B * 3 * c.decoder_dims);
+  L.pq = W.take<float>((size_t)B * c.decoder_dims);
+  L.x = W.take<float>((size_t)B * c.lstm_dims);
+  L.gates = W.take<float>((size_t)B * 4 * c.lstm_dims);
+  L.a_hi = W.take<float>(tc_skinny_act_bytes(B > 128 ? 128 : B, 2 * c.lstm_dims) / 4);
+  L.a_lo = W.take<float>(tc_skinny_act_bytes(B > 128 ? 128 : B, 2 * c.lstm_dims) / 4);
+  L.ah_hi = W.take<float>(2 * tc_skinny_act_bytes(B > 128 ? 128 : B, c.decoder_dims) / 4);  // attention-GRU state tiles, 2 parities
+  L.ah_lo = W.take<float>(2 * tc_skinny_act_bytes(B > 128 ? 128 : B, c.decoder_dims) / 4);
   {
     // operand tiles written by the producing kernels (fused act_split): P1 [ctx | prenet], P2 [ctx | attn_h], P3 / P4 [x | h] of the
     // two LSTMs (two step parities each), P5 [x]; hi and lo of each; zeroed with the attention-GRU tiles at the start of generate()
     const int Bc = B > 128 ? 128 : B;
     const FusedSplit f = fused_split_layout(Bc, proj_dims, c.decoder_dims, c.lstm_dims);
-    L.fsp = take(f.total / 4);
+    L.fsp = W.take<float>(f.total / 4);
   }
   // partial GEMM results computed a step early on the side stream: W_hh h of the two LSTMs, W_ih[:, ctx] ctx of the attention GRU
-  L.pre1 = take((size_t)B * 4 * c.lstm_dims);
-  L.pre2 = take((size_t)B * 4 * c.lstm_dims);
-  L.gic = take((size_t)B * 3 * c.decoder_dims);
-  L.stopv = take(B);
-  L.step = take(64);
+  L.pre1 = W.take<float>((size_t)B * 4 * c.lstm_dims);
+  L.pre2 = W.take<float>((size_t)B * 4 * c.lstm_dims);
+  L.gic = W.take<float>((size_t)B * 3 * c.decoder_dims);
+  L.stopv = W.take<float>(B);
+  L.step = W.take<float>(64);
   const int nst = (steps + r - 1) / r;
-  L.flags = take(nst);
-  L.dmask = take(((size_t)nst * 2 * B * 2 * c.decoder_dims + 3) / 4 + 64);  // PreNet dropout masks of every decoder step
-  L.mel_all = take(Mp * c.n_mels + (size_t)r * c.n_mels);
-  L.scores_all = take((size_t)B * nst * Tc);
-  L.pbank = take(Mp * c.postnet_K * PD);
-  L.ppool = take(Mp * c.postnet_K * PD);
-  L.ppj1 = take(Mp * PD);
-  L.ppj2 = take(Mp * c.n_mels);
-  L.py = take(Mp * PD);
-  L.phw12 = take(Mp * 2 * PD);
-  L.pgi_f = take(Mp * 3 * (PD / 2));
-  L.pgi_b = take(Mp * 3 * (PD / 2));
-  L.pgh = take((size_t)2 * B * 3 * (PD / 2));
-  L.phst = take((size_t)2 * B * (PD / 2));
-  L.pout = take(Mp * PD);
-  L.lin = take(Mp * c.n_mels);
+  L.flags = W.take<float>(nst);
+  L.dmask = W.take<float>(((size_t)nst * 2 * B * 2 * c.decoder_dims + 3) / 4 + 64);  // PreNet dropout masks of every decoder step
+  L.mel_all = W.take<float>(Mp * c.n_mels + (size_t)r * c.n_mels);
+  L.scores_all = W.take<float>((size_t)B * nst * Tc);
+  L.pbank = W.take<float>(Mp * c.postnet_K * PD);
+  L.ppool = W.take<float>(Mp * c.postnet_K * PD);
+  L.ppj1 = W.take<float>(Mp * PD);
+  L.ppj2 = W.take<float>(Mp * c.n_mels);
+  L.py = W.take<float>(Mp * PD);
+  L.phw12 = W.take<float>(Mp * 2 * PD);
+  L.pgi_f = W.take<float>(Mp * 3 * (PD / 2));
+  L.pgi_b = W.take<float>(Mp * 3 * (PD / 2));
+  L.pgh = W.take<float>((size_t)2 * B * 3 * (PD / 2));
+  L.phst = W.take<float>((size_t)2 * B * (PD / 2));
+  L.pout = W.take<float>(Mp * PD);
+  L.lin = W.take<float>(Mp * c.n_mels);
   {  // im2col operand planes of the large-M tensor-core GEMMs: the widest layer is conv_project1 (3 taps x K * ch)
     const size_t enc = tc_big_act_bytes((int)Me, 3, c.encoder_K * E), post = tc_big_act_bytes((int)Mp, 3, c.postnet_K * PD);
     L.big_bytes = enc > post ? enc : post;
-    L.big_hi = take(L.big_bytes / 4);
-    L.big_lo = take(L.big_bytes / 4);
+    L.big_hi = W.take<float>(L.big_bytes / 4);
+    L.big_lo = W.take<float>(L.big_bytes / 4);
   }
-  L.total = o;
+  if (ragged) L.rows = W.take<float>((size_t)6 * B);
+  L.total = W.total();
   return L;
 }
 
@@ -1107,7 +1105,7 @@ size_t mb_tacotron_workspace_bytes(const mb_tacotron* h, int32_t B, int32_t Tc, 
   const int max_chars = lsa_max_chars();  // 0: no device to ask; mb_tacotron_generate still refuses
   if (max_chars > 0 && Tc > max_chars) return 0;
   const int nst = (steps + r - 1) / r;
-  return ws_layout(h->cfg, B, Tc, nst * r, r).total * sizeof(float) + 256;
+  return ws_layout(h->cfg, B, Tc, nst * r, r).total;
 }
 
 }  // extern "C"
@@ -1122,15 +1120,12 @@ struct RaggedRows {
   int32_t* frames;        // out: frames of each row
 };
 
-// device int32 entries behind the ws_layout of a ragged batch: chars, caps (decoder steps), done step, frames [B] each, seeds [B] u64
-size_t ragged_ws_floats(int B) { return align_up((size_t)6 * B, 64); }
-
 // Tacotron.generate of one padded batch (rg == nullptr) or of B ragged rows, each computed as that utterance alone (rg)
 int generate_impl(mb_tacotron* h, const int32_t* chars, const float* spk, int32_t B, int32_t Tc, int32_t steps,
                   int32_t r, int32_t style_idx, float min_stop_token, const uint8_t* enc_masks,
                   const uint8_t* dec_masks, uint64_t seed, float* mel_out, float* linear_out, float* attn_out,
                   int32_t* frames_out_host, void* workspace, size_t workspace_bytes, void* stream, const RaggedRows* rg) {
-  if (!h || !chars || !spk || !mel_out || !linear_out || !frames_out_host || !workspace)
+  if (!h || !chars || !spk || !mel_out || !linear_out || !frames_out_host)
     return fail(MB_ERR_INVALID, "mb_tacotron_generate: null argument");
   if (!h->finalized) return fail(MB_ERR_STATE, "mb_tacotron_generate: weights not finalized");
   const mb_tacotron_config& c = h->cfg;
@@ -1141,10 +1136,9 @@ int generate_impl(mb_tacotron* h, const int32_t* chars, const float* spk, int32_
                 Tc, max_chars);
   const int nst = (steps + r - 1) / r;
   const int steps_alloc = nst * r;  // the reference emits r frames per decoder step (tacotron.py:264-272)
-  const Ws L = ws_layout(c, B, Tc, steps_alloc, r);
-  const size_t need = (L.total + (rg ? ragged_ws_floats(B) : 0)) * sizeof(float) + 256;
-  if (workspace_bytes < need) return fail(MB_ERR_WORKSPACE, "mb_tacotron_generate: workspace too small");
-  float* ws = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  const Ws L = ws_layout(c, B, Tc, steps_alloc, r, rg != nullptr);
+  float* ws;
+  if (int rc = bind("mb_tacotron_generate", workspace, workspace_bytes, L.total, &ws)) return rc;
   cudaStream_t caller = (cudaStream_t)stream;
   if (!h->own_stream) {
     MB_CUDA_CHECK(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
@@ -1177,7 +1171,7 @@ int generate_impl(mb_tacotron* h, const int32_t* chars, const float* spk, int32_
   int* d_flen = nullptr;
   const uint64_t* d_seeds = nullptr;
   if (rg) {
-    int32_t* base = reinterpret_cast<int32_t*>(ws + L.total);
+    int32_t* base = reinterpret_cast<int32_t*>(ws + L.rows);
     std::vector<int32_t> hv((size_t)6 * B, 0);
     for (int b = 0; b < B; ++b) {
       hv[b] = rg->chars[b];
@@ -1874,9 +1868,8 @@ int mb_tacotron_generate(mb_tacotron* h, const int32_t* chars, const float* spk,
 }
 
 size_t mb_tacotron_ragged_workspace_bytes(const mb_tacotron* h, int32_t B, int32_t Tc, int32_t steps, int32_t r) {
-  if (B > 128) return 0;
-  const size_t base = mb_tacotron_workspace_bytes(h, B, Tc, steps, r);
-  return base ? base + ragged_ws_floats(B) * sizeof(float) : 0;
+  if (B > 128 || !mb_tacotron_workspace_bytes(h, B, Tc, steps, r)) return 0;
+  return ws_layout(h->cfg, B, Tc, (steps + r - 1) / r * r, r, true).total;
 }
 
 int mb_tacotron_generate_ragged(mb_tacotron* h, const int32_t* chars, const float* spk, int32_t B, int32_t Tc,
@@ -1977,7 +1970,7 @@ int mb_taco_debug(const mb_taco_debug_spec* spec, void* workspace, size_t worksp
   const mb_taco_debug_spec& s = *spec;
   int rc = debug_check(s);
   if (rc != MB_OK) return rc;
-  if (!workspace || workspace_bytes < 256) return fail(MB_ERR_WORKSPACE, "mb_taco_debug: workspace %zu < 256 bytes", workspace_bytes);
+  if ((rc = bind("mb_taco_debug", workspace, workspace_bytes, mb_taco_debug_workspace_bytes(spec)))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t* n = s.n;
   auto fin = [&](int i) { return reinterpret_cast<const float*>(s.in[i]); };

@@ -832,45 +832,41 @@ namespace {
 
 const float* W(const mb_wavernn* h, const std::string& name) { return h->w.ptr(name); }
 
-struct WsLayout {
+struct Ws {
   size_t aux, melup, aux2P, aux3P, aux4P, tmpA, tmpB, tmpR, padP, lad5, lad25, lad200, segs, starts, condI, h1, h2, f1, f2, logits,
-      xprev, barrier, rowdesc, total;
+      xprev, barrier, rowdesc;  // floats
+  size_t total;                 // bytes
 };
 
 // T frames of U utterances in all (each utterance has its own "past the end" table row and its own 4 frames of ladder padding);
 // multi: the segment tables of the conditioning kernels and the row descriptors of the multi-utterance loop are laid out too
-WsLayout ws_layout(int T, int Bpad, int chunk_steps, int U = 1, bool multi = false) {
-  WsLayout L{};
-  size_t o = 0;
-  auto take = [&](size_t floats) {
-    size_t r = o;
-    o += align_up(floats, 64);
-    return r;
-  };
-  L.aux = take((size_t)T * CDIM);
-  L.melup = take((size_t)HOP * T * FEAT);
-  L.aux2P = take((size_t)(T + U) * 3 * RNN);
-  L.aux3P = take((size_t)(T + U) * RNN);
-  L.aux4P = take((size_t)(T + U) * RNN);
-  L.tmpA = take((size_t)CDIM * T);
-  L.tmpB = take((size_t)CDIM * T);
-  L.tmpR = take((size_t)CDIM * T);
-  L.padP = take((size_t)FEAT * (T + 4 * U));
-  L.lad5 = take((size_t)FEAT * (T + 4 * U) * 5);
-  L.lad25 = take((size_t)FEAT * (T + 4 * U) * 25);
-  L.lad200 = take((size_t)FEAT * (T + 4 * U) * HOP);
-  if (multi) L.segs = take((size_t)3 * T + 7 * U);  // int32: fseg[T] pseg[T+4U] tsrc[T+U] segF[U] segT[U]
-  L.starts = take((size_t)Bpad);
-  L.condI = take((size_t)chunk_steps * RNN * Bpad);
-  L.h1 = take((size_t)2 * RNN * Bpad);
-  L.h2 = take((size_t)2 * RNN * Bpad);
-  L.f1 = take((size_t)RNN * Bpad);
-  L.f2 = take((size_t)RNN * Bpad);
-  L.logits = take((size_t)RNN * Bpad);
-  L.xprev = take((size_t)Bpad);
-  L.barrier = take(256);  // 1 KB: counter, or one epoch word per CTA
-  if (multi) L.rowdesc = take((size_t)10 * Bpad);  // int4 rowc[Bpad] | int4 rown[Bpad] | uint64 rowseed[Bpad]
-  L.total = o;
+Ws ws_layout(int T, int Bpad, int chunk_steps, int U = 1, bool multi = false) {
+  Ws L{};
+  WsLayout W;
+  L.aux = W.take<float>((size_t)T * CDIM);
+  L.melup = W.take<float>((size_t)HOP * T * FEAT);
+  L.aux2P = W.take<float>((size_t)(T + U) * 3 * RNN);
+  L.aux3P = W.take<float>((size_t)(T + U) * RNN);
+  L.aux4P = W.take<float>((size_t)(T + U) * RNN);
+  L.tmpA = W.take<float>((size_t)CDIM * T);
+  L.tmpB = W.take<float>((size_t)CDIM * T);
+  L.tmpR = W.take<float>((size_t)CDIM * T);
+  L.padP = W.take<float>((size_t)FEAT * (T + 4 * U));
+  L.lad5 = W.take<float>((size_t)FEAT * (T + 4 * U) * 5);
+  L.lad25 = W.take<float>((size_t)FEAT * (T + 4 * U) * 25);
+  L.lad200 = W.take<float>((size_t)FEAT * (T + 4 * U) * HOP);
+  if (multi) L.segs = W.take<float>((size_t)3 * T + 7 * U);  // int32: fseg[T] pseg[T+4U] tsrc[T+U] segF[U] segT[U]
+  L.starts = W.take<float>((size_t)Bpad);
+  L.condI = W.take<float>((size_t)chunk_steps * RNN * Bpad);
+  L.h1 = W.take<float>((size_t)2 * RNN * Bpad);
+  L.h2 = W.take<float>((size_t)2 * RNN * Bpad);
+  L.f1 = W.take<float>((size_t)RNN * Bpad);
+  L.f2 = W.take<float>((size_t)RNN * Bpad);
+  L.logits = W.take<float>((size_t)RNN * Bpad);
+  L.xprev = W.take<float>((size_t)Bpad);
+  L.barrier = W.take<float>(256);  // 1 KB: counter, or one epoch word per CTA
+  if (multi) L.rowdesc = W.take<float>((size_t)10 * Bpad);  // int4 rowc[Bpad] | int4 rown[Bpad] | uint64 rowseed[Bpad]
+  L.total = W.total();
   return L;
 }
 
@@ -987,18 +983,17 @@ int mb_wavernn_finalize(mb_wavernn* h, void* stream) {
 size_t mb_wavernn_workspace_bytes(const mb_wavernn* h, int32_t frames, int32_t folds, int32_t steps) {
   if (!h || frames <= 0 || folds <= 0) return 0;
   (void)steps;
-  return ws_layout(frames, bpad_of(folds), kChunkMax).total * sizeof(float) + 256;
+  return ws_layout(frames, bpad_of(folds), kChunkMax).total;
 }
 
 int mb_wavernn_condition(mb_wavernn* h, const float* mel, int32_t T, void* workspace, size_t workspace_bytes,
                          void* stream) {
-  if (!h || !mel || !workspace || T <= 0) return fail(MB_ERR_INVALID, "mb_wavernn_condition: bad argument");
+  if (!h || !mel || T <= 0) return fail(MB_ERR_INVALID, "mb_wavernn_condition: bad argument");
   if (!h->finalized) return fail(MB_ERR_STATE, "mb_wavernn_condition: weights not finalized");
-  // the conditioning part of the layout does not depend on the fold count
-  const WsLayout L = ws_layout(T, RB, kChunkMax);
-  if (workspace_bytes < (L.starts) * sizeof(float) + 256)
-    return fail(MB_ERR_WORKSPACE, "mb_wavernn_condition: workspace too small");
-  float* ws = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  // the conditioning part of the layout does not depend on the fold count; the check asks for the smallest full workspace
+  const Ws L = ws_layout(T, RB, kChunkMax);
+  float* ws;
+  if (int rc = bind("mb_wavernn_condition", workspace, workspace_bytes, L.total, &ws)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const int n = CDIM * T, nb = (n + 255) / 256;
   float *x = ws + L.tmpA, *y = ws + L.tmpB, *r = ws + L.tmpR;
@@ -1071,7 +1066,7 @@ int mb_wavernn_generate(mb_wavernn* h, const int32_t* fold_starts_host, int32_t 
 
 namespace {
 
-int launch_sample_loop(mb_wavernn* h, LoopParams& p, const WsLayout& L, float* ws, bool multi, cudaStream_t st);
+int launch_sample_loop(mb_wavernn* h, LoopParams& p, const Ws& L, float* ws, bool multi, cudaStream_t st);
 
 // one chunk of the sample loop; exactly one of out_idx (RAW handle) / out_x (MOL handle) is given
 int generate_rows_impl(mb_wavernn* h, const int32_t* fold_starts_host, int32_t B, int32_t steps, int32_t step0,
@@ -1086,9 +1081,9 @@ int generate_rows_impl(mb_wavernn* h, const int32_t* fold_starts_host, int32_t B
     return fail(MB_ERR_INVALID, "mb_wavernn_generate: bad step range (at most %d steps per call)", kChunkMax);
   const int T = h->cond_T;
   const int Bpad = bpad_of(B);
-  const WsLayout L = ws_layout(T, Bpad, kChunkMax);
-  if (workspace_bytes < L.total * sizeof(float) + 256) return fail(MB_ERR_WORKSPACE, "mb_wavernn_generate: workspace too small");
-  float* ws = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  const Ws L = ws_layout(T, Bpad, kChunkMax);
+  float* ws;
+  if (int rc = bind("mb_wavernn_generate", workspace, workspace_bytes, L.total, &ws)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   if (step0 == 0) {
     // zero initial state (fatchord_version.py:178-185) and upload the fold starts
@@ -1121,7 +1116,7 @@ int generate_rows_impl(mb_wavernn* h, const int32_t* fold_starts_host, int32_t B
 }
 
 // fills the workspace pointers of `p` and launches the loop instance of the handle's sampler
-int launch_sample_loop(mb_wavernn* h, LoopParams& p, const WsLayout& L, float* ws, bool multi, cudaStream_t st) {
+int launch_sample_loop(mb_wavernn* h, LoopParams& p, const Ws& L, float* ws, bool multi, cudaStream_t st) {
   const bool mol = h->mode == MB_WAVERNN_MOL;
   MB_CUDA_CHECK(cudaMemsetAsync(ws + L.barrier, 0, 1024, st));
   p.wpack = h->arena + h->pack_off;
@@ -1185,8 +1180,8 @@ int mb_wavernn_generate_rows_mol(mb_wavernn* h, const int32_t* fold_starts_host,
 int mb_wavernn_last_logits(mb_wavernn* h, float* logits, int32_t B, void* workspace, void* stream) {
   if (!h || !logits || !workspace || h->cond_T <= 0) return fail(MB_ERR_INVALID, "mb_wavernn_last_logits: bad argument");
   const int Bpad = bpad_of(B);
-  const WsLayout L = ws_layout(h->cond_T, Bpad, kChunkMax);
-  float* ws = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  const Ws L = ws_layout(h->cond_T, Bpad, kChunkMax);
+  float* ws = aligned<float>(workspace);
   // logits are stored [class][Bpad]; return [B][ncls] (512 RAW, 30 MOL)
   const int ncls = h->ncls;
   MB_CUDA_CHECK(cudaMemcpy2DAsync(logits, sizeof(float) * ncls, ws + L.logits, sizeof(float), sizeof(float), 1,
@@ -1248,9 +1243,9 @@ int generate_multi_impl(const char* fn, mb_wavernn* h, const int32_t* row_utt, c
   for (int r = 0; r < rows; ++r)
     if (row_utt[r] >= U) return fail(MB_ERR_INVALID, "%s: row %d names utterance %d of %d", fn, r, row_utt[r], U);
   const int Bpad = bpad_of(rows);
-  const WsLayout L = ws_layout(Ttot, Bpad, kChunkMax, U, true);
-  if (workspace_bytes < L.total * sizeof(float) + 256) return fail(MB_ERR_WORKSPACE, "%s: workspace too small", fn);
-  float* ws = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  const Ws L = ws_layout(Ttot, Bpad, kChunkMax, U, true);
+  float* ws;
+  if (int rc = bind(fn, workspace, workspace_bytes, L.total, &ws)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   int4* rowc = reinterpret_cast<int4*>(ws + L.rowdesc);
   int4* rown = rowc + Bpad;
@@ -1313,22 +1308,21 @@ size_t mb_wavernn_workspace_bytes_multi(const mb_wavernn* h, int32_t n_utts, con
   const int64_t Ttot = total_frames(frames, n_utts);
   if (!h || Ttot < 0 || rows <= 0) return 0;
   (void)max_steps;
-  return ws_layout((int)Ttot, bpad_of(rows), kChunkMax, n_utts, true).total * sizeof(float) + 256;
+  return ws_layout((int)Ttot, bpad_of(rows), kChunkMax, n_utts, true).total;
 }
 
 int mb_wavernn_condition_multi(mb_wavernn* h, const float* mel_concat, const int32_t* frames, int32_t n_utts, void* workspace,
                                size_t workspace_bytes, void* stream) {
-  if (!h || !mel_concat || !frames || !workspace) return fail(MB_ERR_INVALID, "mb_wavernn_condition_multi: null argument");
+  if (!h || !mel_concat || !frames) return fail(MB_ERR_INVALID, "mb_wavernn_condition_multi: null argument");
   const int64_t tot = total_frames(frames, n_utts);
   if (tot < 0) return fail(MB_ERR_INVALID, "mb_wavernn_condition_multi: bad utterance lengths (each > 0, %d frames in all at most)",
                            (int)(((int64_t)1 << 31) / (HOP * FEAT)));
   const int U = n_utts, Ttot = (int)tot, Tptot = Ttot + 4 * U, R = Ttot + U;
-  // the conditioning part of the layout does not depend on the row count
-  const WsLayout L = ws_layout(Ttot, RB, kChunkMax, U, true);
-  if (workspace_bytes < (L.starts) * sizeof(float) + 256)
-    return fail(MB_ERR_WORKSPACE, "mb_wavernn_condition_multi: workspace too small");
+  // the conditioning part of the layout does not depend on the row count; the check asks for the smallest full workspace
+  const Ws L = ws_layout(Ttot, RB, kChunkMax, U, true);
+  float* ws;
+  if (int rc = bind("mb_wavernn_condition_multi", workspace, workspace_bytes, L.total, &ws)) return rc;
   if (!h->finalized) return fail(MB_ERR_STATE, "mb_wavernn_condition_multi: weights not finalized");
-  float* ws = (float*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
   cudaStream_t st = (cudaStream_t)stream;
   // segment tables
   std::vector<int32_t> seg((size_t)3 * Ttot + 7 * U);

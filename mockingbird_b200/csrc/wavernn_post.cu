@@ -122,7 +122,7 @@ template <typename In>
 int postprocess(const In* idx, int32_t folds, int32_t steps, int32_t batched, int32_t target, int32_t overlap,
                 int32_t n_classes, int32_t mu_law, double preemphasis, int64_t wave_len, int32_t fade_len,
                 double* out, int64_t* n_out, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!idx || !out || !n_out || !workspace) return mb::fail(MB_ERR_INVALID, "mb_wavernn_postprocess: null argument");
+  if (!idx || !out || !n_out) return mb::fail(MB_ERR_INVALID, "mb_wavernn_postprocess: null argument");
   if (folds <= 0 || steps <= 0 || n_classes < 2) return mb::fail(MB_ERR_INVALID, "mb_wavernn_postprocess: empty input");
   if (batched && (steps != target + 2 * overlap || overlap < 0 || target <= 0))
     return mb::fail(MB_ERR_INVALID, "mb_wavernn_postprocess: folds must be target + 2*overlap = %d steps long, got %d", target + 2 * overlap, steps);
@@ -143,9 +143,9 @@ int postprocess(const In* idx, int32_t folds, int32_t steps, int32_t batched, in
   p.fade_len = fade_len;
   if (p.n_out < fade_len) return mb::fail(MB_ERR_INVALID, "mb_wavernn_postprocess: output of %lld samples is shorter than the %d-sample fade "
                                           "(the reference raises here too)", p.n_out, fade_len);
-  if (workspace_bytes < workspace_bytes_of(folds, steps, batched, target, overlap))
-    return mb::fail(MB_ERR_WORKSPACE, "mb_wavernn_postprocess: workspace too small");
-  p.tmp = reinterpret_cast<double*>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  if (int rc = mb::bind("mb_wavernn_postprocess", workspace, workspace_bytes, workspace_bytes_of(folds, steps, batched, target, overlap),
+                        &p.tmp))
+    return rc;
   p.out = out;
   cudaStream_t st = (cudaStream_t)stream;
   k_unfold_decode<In><<<(unsigned)((p.total_len + 255) / 256), 256, 0, st>>>(p);

@@ -84,9 +84,8 @@ class SpeakerEncoder:
             stream = torch.cuda.current_stream(dev).cuda_stream
             for r0 in range(0, R, MAX_ROWS):
                 n = min(MAX_ROWS, R - r0)
-                need = int(L.mb_encoder_workspace_bytes(self._handle, n, T)) + 256
-                if self._ws is None or self._ws.numel() < need:
-                    self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+                need = int(L.mb_encoder_workspace_bytes(self._handle, n, T))
+                _lib.workspace(need, dev, self)
                 _lib.check(L.mb_encoder_embed_frames(self._handle, C.c_void_p(x[r0:r0 + n].data_ptr()), n, T,
                                                      C.c_void_p(out[r0:r0 + n].data_ptr()),
                                                      C.c_void_p(self._ws.data_ptr()), self._ws.numel(), C.c_void_p(stream)))
@@ -117,9 +116,8 @@ class SpeakerEncoder:
         out = torch.empty(R, self._cfg.embedding_size, dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev).cuda_stream
-            need = int(L.mb_encoder_rows_workspace_bytes(self._handle, R, max(int(v) for v in row_lens))) + 256
-            if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-                self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            need = int(L.mb_encoder_rows_workspace_bytes(self._handle, R, max(int(v) for v in row_lens)))
+            _lib.workspace(need, dev, self)
             _lib.check(L.mb_encoder_embed_rows(self._handle, C.c_void_p(frames.data_ptr()), frames.shape[0], starts, lens, R,
                                                C.c_void_p(out.data_ptr()), C.c_void_p(self._ws.data_ptr()), self._ws.numel(),
                                                C.c_void_p(stream)))

@@ -92,8 +92,7 @@ class GriffinLim:
         L = _lib.lib()
         need = int(L.mb_griffinlim_workspace_bytes(self._handle, B, T))
         with torch.cuda.device(dev):
-            if self._workspace is None or self._workspace.numel() < need:
-                self._workspace = torch.empty(max(need, 1), dtype=torch.uint8, device=dev)
+            _lib.workspace(need, dev, self, "_workspace")
             out = torch.empty(max(sum(lengths), 1), dtype=torch.float32, device=dev)
             stream = torch.cuda.current_stream(dev).cuda_stream
             _lib.check(L.mb_griffinlim_forward(self._handle, C.c_void_p(flat.data_ptr()), T, B,

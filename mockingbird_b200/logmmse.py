@@ -61,9 +61,7 @@ class _Handle:
         L = _lib.lib()
         T = (C.c_int32 * len(lengths))(*lengths)
         need = int(L.mb_logmmse_workspace_bytes(self._handle, len(lengths), T))
-        if self._workspace is None or self._workspace.numel() < need:
-            self._workspace = torch.empty(max(need, 1), dtype=torch.uint8, device=self.device)
-        return T, self._workspace
+        return T, _lib.workspace(need, self.device, self, "_workspace")
 
     def __del__(self):
         try:

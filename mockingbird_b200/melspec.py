@@ -106,10 +106,10 @@ class MelSpectrogram:
             x = x.to(self._device).contiguous()
             out = torch.empty(sum(counts) * self.n_mels, dtype=torch.float32, device=self._device)
             need = int(L.mb_melspec_ragged_workspace_bytes(self._handle, B))
-            ws = torch.empty(need, dtype=torch.uint8, device=self._device)
+            ws = _lib.workspace(need, self._device)
             stream = torch.cuda.current_stream(self._device).cuda_stream
             _lib.check(L.mb_melspec_forward_ragged(self._handle, C.c_void_p(x.data_ptr()), lens, sigs, B,
-                                                   C.c_void_p(out.data_ptr()), C.c_void_p(ws.data_ptr()), need,
+                                                   C.c_void_p(out.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(),
                                                    C.c_void_p(stream)))
         return out, counts
 

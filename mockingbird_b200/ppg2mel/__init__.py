@@ -121,8 +121,7 @@ class MelDecoderMOLv2:
                 m2 = masks[1].to(device=dev, dtype=torch.uint8).contiguous()
                 if tuple(m1.shape) != (S, B, 256) or tuple(m2.shape) != (S, B, 128):
                     raise ValueError(f"dropout masks must be [{S},{B},256] and [{S},{B},128]")
-            if self._ws is None or self._ws.numel() < need:
-                self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            _lib.workspace(need, dev, self)
             lens = (C.c_int32 * B)(*lengths)
             steps = (C.c_int32 * B)()
             stream = torch.cuda.current_stream(dev).cuda_stream

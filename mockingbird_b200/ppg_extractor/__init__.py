@@ -252,9 +252,7 @@ class PPGModel:
             need = int(Lb.mb_ppgx_workspace_bytes(self._handle, B, n_max))
             if need == 0:
                 raise ValueError(f"utterance of {n_max} samples is too short")
-            if self._ws is None or self._ws.numel() < need:
-                self._ws = None
-                self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            _lib.workspace(need, dev, self)
             ns = (C.c_int32 * B)(*lengths)
             stream = torch.cuda.current_stream(dev).cuda_stream
             _lib.check(Lb.mb_ppgx_forward(

@@ -148,10 +148,7 @@ class _Resampler:
         return _lib.lib().mb_resample_filter_in_smem(self._handle, self.filter_index(up, down)) == 1
 
     def workspace(self, need):
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = None
-            self._ws = torch.empty(max(need, 1), dtype=torch.uint8, device=self.device)
-        return self._ws
+        return _lib.workspace(need, self.device, self)
 
     def forward(self, clips, rates, target_sr) -> DeviceClips:
         L = _lib.lib()
@@ -224,7 +221,7 @@ def resample_many(wavs, source_srs, target_sr, device=None, filter_smem_bytes=-1
 def _level_ws(clips: DeviceClips):
     B = len(clips)
     need = int(_lib.lib().mb_resample_level_workspace_bytes(B))
-    return (C.c_int32 * B)(*clips.lengths), torch.empty(need, dtype=torch.uint8, device=clips.device)
+    return (C.c_int32 * B)(*clips.lengths), _lib.workspace(need, clips.device)
 
 
 def mean_squares(clips: DeviceClips) -> np.ndarray:

@@ -183,9 +183,8 @@ class Tacotron:
             enc_p, dec_p = C.c_void_p(enc_m.data_ptr()), C.c_void_p(dec_m.data_ptr())
         frames = C.c_int32(0)
         with torch.cuda.device(dev):
-            need = int(L.mb_tacotron_workspace_bytes(self._handle, B, Tc, steps, r)) + 256
-            if self._ws is None or self._ws.numel() < need:
-                self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            need = int(L.mb_tacotron_workspace_bytes(self._handle, B, Tc, steps, r))
+            _lib.workspace(need, dev, self)
             stream = torch.cuda.current_stream(dev).cuda_stream
             _lib.check(L.mb_tacotron_generate(self._handle, C.c_void_p(chars.data_ptr()), C.c_void_p(spk.data_ptr()), B, Tc,
                                               int(steps), r, int(style_idx), C.c_float(float(min_stop_token)), enc_p, dec_p,
@@ -279,9 +278,8 @@ class Tacotron:
             row_frames = (C.c_int32 * B)()
             frames = C.c_int32(0)
             with torch.cuda.device(dev):
-                need = int(L.mb_tacotron_ragged_workspace_bytes(self._handle, B, Tc, max(ccaps), r)) + 256
-                if self._ws is None or self._ws.numel() < need:
-                    self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+                need = int(L.mb_tacotron_ragged_workspace_bytes(self._handle, B, Tc, max(ccaps), r))
+                _lib.workspace(need, dev, self)
                 stream = torch.cuda.current_stream(dev).cuda_stream
                 _lib.check(L.mb_tacotron_generate_ragged(
                     self._handle, C.c_void_p(chars.data_ptr()), C.c_void_p(spk.data_ptr()), B, Tc, row_chars, row_steps,

@@ -191,10 +191,8 @@ class GanGenerator:
 
     # -- forward ---------------------------------------------------------------------------------
     def _ensure_workspace(self, B: int, T: int) -> torch.Tensor:
-        need = int(_lib.lib().mb_gan_workspace_bytes(self._handle, B, T)) + 256
-        if self._workspace is None or self._workspace.numel() < need:
-            self._workspace = torch.empty(need, dtype=torch.uint8, device=self._device)
-        return self._workspace
+        need = int(_lib.lib().mb_gan_workspace_bytes(self._handle, B, T))
+        return _lib.workspace(need, self._device, self, "_workspace")
 
     def forward(self, x: torch.Tensor, lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
         """mel [B, 80, T] (cuda fp32) -> wav [B, 1, T*hop].  ``lengths`` (int32 [B], optional, an

@@ -71,7 +71,6 @@ class WaveRNN:
             raise _lib.MbError("WaveRNN has no weights: call load_state_dict first")
         dev = self._device = self._device or _lib.require_cuda()
         self._arena = _lib.upload_weights("deepmind", self._handle, self.weights_for_upload(), dev)
-        self._ws = torch.empty(int(_lib.lib().mb_deepmind_workspace_bytes(self._handle)) + 256, dtype=torch.uint8, device=dev)
         self._ready = True
 
     def weights_for_upload(self) -> Dict[str, torch.Tensor]:
@@ -94,6 +93,7 @@ class WaveRNN:
         use_mt = noise is None and self.rng == "torch"
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev)
+            ws = _lib.workspace(int(L.mb_deepmind_workspace_bytes(self._handle)), dev, self)
             coarse = torch.empty(seq_len, dtype=torch.int16, device=dev)
             fine = torch.empty(seq_len, dtype=torch.int16, device=dev)
             dbufs = [torch.empty(CHUNK * per_step, dtype=torch.float32, device=dev) for _ in range(2)] if (use_mt or noise is not None) else None
@@ -119,7 +119,7 @@ class WaveRNN:
                         nptr = C.c_void_p(dbufs[slot].data_ptr())
                     _lib.check(L.mb_deepmind_generate(self._handle, seq_len, step0, n, nptr, C.c_uint64(self.seed),
                                                       C.c_void_p(coarse.data_ptr()), C.c_void_p(fine.data_ptr()),
-                                                      C.c_void_p(self._ws.data_ptr()), self._ws.numel(), C.c_void_p(stream.cuda_stream)))
+                                                      C.c_void_p(ws.data_ptr()), ws.numel(), C.c_void_p(stream.cuda_stream)))
                     if use_mt:
                         _lib.check(L.mb_mtstream_consumed(self._mt, C.c_void_p(stream.cuda_stream)))
                     step0 += n

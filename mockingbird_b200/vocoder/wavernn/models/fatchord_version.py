@@ -302,9 +302,8 @@ class WaveRNN:
         start_t = time.time()
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev)
-            need = int(L.mb_wavernn_workspace_bytes(self._handle, T, B, steps)) + 256
-            if self._ws is None or self._ws.numel() < need:
-                self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            need = int(L.mb_wavernn_workspace_bytes(self._handle, T, B, steps))
+            _lib.workspace(need, dev, self)
             ws = self._ws
             _lib.check(L.mb_wavernn_condition(self._handle, C.c_void_p(mel.data_ptr()), T, C.c_void_p(ws.data_ptr()),
                                               ws.numel(), C.c_void_p(stream.cuda_stream)))
@@ -467,11 +466,10 @@ class WaveRNN:
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev)
             frames_c = (C.c_int32 * U)(*plan.frames)
-            need = int(L.mb_wavernn_workspace_bytes_multi(self._handle, U, frames_c, rows, max_steps)) + 256
-            if need <= 256:
+            need = int(L.mb_wavernn_workspace_bytes_multi(self._handle, U, frames_c, rows, max_steps))
+            if need == 0:
                 raise _lib.MbError("generate_many: the utterances do not fit one loop (too many frames in all)")
-            if self._ws is None or self._ws.numel() < need:
-                self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            _lib.workspace(need, dev, self)
             ws = self._ws
             mel_cat = torch.cat([mel2d[u].reshape(-1) for u in plan.order]).to(dev).contiguous()
             _lib.check(L.mb_wavernn_condition_multi(self._handle, C.c_void_p(mel_cat.data_ptr()), frames_c, U,
@@ -599,7 +597,7 @@ class WaveRNN:
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev)
             need = int(L.mb_wavernn_postprocess_workspace_bytes(folds, steps, int(batched), target, overlap))
-            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            ws = _lib.workspace(need, dev)
             out = torch.empty(min(total, max(wave_len, 0)), dtype=torch.float64, device=dev)
             n_out = C.c_int64()
             preemph = float(hp.preemphasis) if hp.apply_preemphasis else 0.0
