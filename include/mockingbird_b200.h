@@ -73,6 +73,11 @@ uint64_t mb_launch_count(void);
  * InterpolationBlock(u) (nearest) + Conv1d(k, padding=(k-1)//2), checkpoint keys "ups.{i}.1.*"; k must be odd.  Lowered
  * to a polyphase tap conv with folded weights (DESIGN.md 3.6); same mb_gan_config fields as MB_GAN_HIFIGAN. */
 #define MB_GAN_HIFIGAN_INTERP 2
+/* The VITS decoder (models/synthesizer/models/vits.py:245-290, `Vits.dec`): HiFi-GAN's plan with num_mels input channels,
+ * ConvTranspose1d(k, u, padding=(k-u)//2) without output padding ((k-u) even), and conv_post without bias (its checkpoint
+ * has no "conv_post.bias"; the layer adds zero).  The per-utterance cond(g) of Generator.forward is not part of this kind:
+ * mb_vits feeds it as extra, time-constant input channels of conv_pre (see mb_vits_decode). */
+#define MB_GAN_VITS 3
 
 /* arithmetic of the channel-mixing convolutions */
 #define MB_PREC_FP32 0      /* FP32 FFMA everywhere (parity anchor, ~1e-6 of the reference)     */
@@ -1036,6 +1041,96 @@ size_t mb_ppgx_debug_workspace_bytes(const mb_ppgx_debug_spec* spec);
  * "kernel=K inst=I grid=X,Y,Z inv_scale=S" (inst: NT of conv2d_tc, DK of attn_kernel, 0 otherwise) */
 int mb_ppgx_debug(const mb_ppgx_debug_spec* spec, void* workspace, size_t workspace_bytes, void* stream, char* report,
                   size_t report_len);
+
+/* ---------------------------------------------------------------------------------------------
+ * VITS synthesizer: token ids -> waveform
+ *   replaces  models/synthesizer/models/vits.py:389-527  Vits.{__init__,infer} (enc_p, emb_g, dp, flow, dec)
+ *   driven by vits.ipynb: model.infer(x, x_lengths, sid=sid, noise_scale=.667, noise_scale_w=.8, length_scale=1, emo=emo)
+ * Two calls, because the frame count T_y is known only after the durations: mb_vits_durations (text encoder, speaker
+ * embedding, duration predictor, ceil(exp(logw) * mask * length_scale)), then - once the caller has read y_lengths back -
+ * mb_vits_decode (prior expansion along the monotonic path, prior noise, reverse coupling flow, decoder).  FP32 kernels
+ * everywhere but the decoder, which is an MB_GAN_VITS generator in `precision`.  Layout NCL; every T axis is padded to the
+ * call's T_x / T_y, rows past x_lengths / y_lengths are masked as the reference masks them.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct mb_vits_config {
+  int32_t n_vocab, inter_channels, hidden_channels, filter_channels, n_heads, n_layers, kernel_size;
+  int32_t resblock_type;         /* 1 = ResBlock1, 2 = ResBlock2 (vits_modules.py:180-249) */
+  int32_t num_kernels;           /* len(resblock_kernel_sizes) <= 4 */
+  int32_t resblock_kernel_sizes[4];
+  int32_t num_dilations;
+  int32_t resblock_dilation_sizes[4][4];
+  int32_t num_upsamples;         /* <= 8 */
+  int32_t upsample_rates[8];
+  int32_t upsample_kernel_sizes[8];
+  int32_t upsample_initial_channel;
+  int32_t n_speakers;            /* 0: no speaker embedding; > 1: emb_g [n_speakers, gin_channels]; 1 is refused */
+  int32_t gin_channels;          /* must be > 0 exactly when n_speakers > 1 */
+  int32_t use_sdp;               /* 1: StochasticDurationPredictor, 0: DurationPredictor */
+  int32_t precision;             /* MB_PREC_* of the decoder */
+} mb_vits_config;
+
+typedef struct mb_vits mb_vits;
+
+/* MB_ERR_INVALID, with a message naming the field, for a config the kernels do not cover (odd kernel_size, hidden %
+ * n_heads, inter_channels odd, head width > 256, the decoder constraints of MB_GAN_VITS) */
+int mb_vits_create(const mb_vits_config* cfg, mb_vits** out);
+void mb_vits_destroy(mb_vits* h);
+size_t mb_vits_arena_bytes(const mb_vits* h);
+int mb_vits_set_arena(mb_vits* h, void* arena, size_t bytes);
+/* One tensor of Vits.state_dict() after weight-norm folding ("...weight_g" / "...weight_v" -> "...weight").  enc_q.*, the
+ * discriminators, dp.post_* and dp.flows.1.* (the flow reverse inference drops) are accepted and ignored. */
+int mb_vits_set_weight(mb_vits* h, const char* name, const float* w, const int64_t* dims, int32_t ndim, void* stream);
+/* MB_ERR_STATE naming the first tensor never set; combines dec.conv_pre and dec.cond into the decoder's input layer */
+int mb_vits_finalize(mb_vits* h, void* stream);
+int32_t mb_vits_hop(const mb_vits* h);
+/* largest T_x the attention kernel takes (its scores row lives in shared memory) */
+int32_t mb_vits_max_tokens(void);
+
+size_t mb_vits_durations_workspace_bytes(const mb_vits* h, int32_t batch, int32_t t_x);
+/* x int32 [B, T_x] token ids, x_lengths int32 [B] in [1, T_x], sid int32 [B] (NULL without speakers), emo [B, 1024],
+ * noise [B, 2, T_x] (the SDP's torch.randn draw, unscaled; ignored and may be NULL when use_sdp == 0).  Writes m_p and
+ * logs_p [B, inter, T_x], w_ceil int32 [B, T_x] and y_lengths int32 [B] = max(1, sum w_ceil).  A token id or sid out of
+ * range reads as id 0 (the host layer checks them). */
+int mb_vits_durations(mb_vits* h, const int32_t* x, const int32_t* x_lengths, int32_t batch, int32_t t_x, const int32_t* sid,
+                      const float* emo, const float* noise, float noise_scale_w, float length_scale, float* m_p, float* logs_p,
+                      int32_t* w_ceil, int32_t* y_lengths, void* workspace, size_t workspace_bytes, void* stream);
+
+size_t mb_vits_decode_workspace_bytes(const mb_vits* h, int32_t batch, int32_t t_x, int32_t t_y, int32_t t_dec);
+/* m_p, logs_p, w_ceil, x_lengths and sid as mb_vits_durations took / wrote them; t_y >= max(y_lengths); eps [B, inter, T_y]
+ * the prior noise (torch.randn_like of the expanded m_p).  t_dec <= t_y frames are decoded (Vits.infer's max_len):
+ * wav [B, 1, t_dec * hop].  ragged == 0 decodes every row over all t_dec frames as the reference does (z * y_mask, no mask
+ * inside the decoder); ragged != 0 masks the decoder at min(y_length, t_dec), so that each row is bitwise the row decoded
+ * alone.  Optional outputs (NULL: not written): attn [B, 1, T_y, T_x], z_p / z / m_p_y / logs_p_y [B, inter, T_y]. */
+int mb_vits_decode(mb_vits* h, const float* m_p, const float* logs_p, const int32_t* w_ceil, const int32_t* x_lengths,
+                   const int32_t* sid, int32_t batch, int32_t t_x, int32_t t_y, const float* eps, float noise_scale, int32_t t_dec,
+                   int32_t ragged, float* wav, float* attn, float* z_p, float* z, float* m_p_y, float* logs_p_y, void* workspace,
+                   size_t workspace_bytes, void* stream);
+
+/* One kernel stage of a finalized handle on its own weights, for tests against float64 references.  lengths int32 [B] masks
+ * as the compute calls do.  Kinds:
+ *   SPLINE   ConvFlow `index` (3 / 5 / 7) reverse: x = the DDSConv output h [B, hidden, T], x2 = z [B, 2, T]; y = z with
+ *            channel c1 through the inverse spline that proj(h) parametrises, channel c0 kept, both masked
+ *   ATTN     encoder layer `index`: x, x2, x3 = q, k, v [B, hidden, T]; y = attention output [B, hidden, T]
+ *   WN       WN layer `sub` of coupling layer flow.flows.(2 * index): x = h [B, hidden, T], x2 = g [B, gin] or NULL;
+ *            y = h after the residual update, y2 = the skip stream [B, hidden, T] (read unless sub == 0, then written)
+ *   DDSCONV  DDSConv "dp.convs." (index 0) or "dp.flows.<index>.convs.": x [B, hidden, T] -> y
+ *   DECODER  dec(x, g) on z = x [B, inter, T] unmasked, x2 = sid int32 [B] (multi-speaker); y = wav [B, 1, T * hop] */
+#define MB_VITS_DBG_SPLINE 0
+#define MB_VITS_DBG_ATTN 1
+#define MB_VITS_DBG_WN 2
+#define MB_VITS_DBG_DDSCONV 3
+#define MB_VITS_DBG_DECODER 4
+typedef struct mb_vits_debug_spec {
+  int32_t kind, batch, frames, index, sub, c0, c1;
+  const int32_t* lengths;
+  const float* x;
+  const float* x2;
+  const float* x3;
+  float* y;
+  float* y2;
+} mb_vits_debug_spec;
+size_t mb_vits_debug_workspace_bytes(const mb_vits* h, const mb_vits_debug_spec* spec);
+int mb_vits_debug(mb_vits* h, const mb_vits_debug_spec* spec, void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

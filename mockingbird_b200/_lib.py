@@ -15,6 +15,7 @@ MB_OK = 0
 MB_GAN_HIFIGAN = 0
 MB_GAN_FREGAN = 1
 MB_GAN_HIFIGAN_INTERP = 2  # 24 kHz HiFi-GAN: nearest upsample + Conv1d per stage (hifigan/models.py:107-118)
+MB_GAN_VITS = 3  # the VITS decoder (synthesizer/models/vits.py:245-290)
 MB_WAVERNN_RAW = 0  # mb_wavernn_create_mode: softmax + Categorical over 2^bits classes
 MB_WAVERNN_MOL = 1  # mixture of logistics (voc_mode 'MOL'), fc3 [30, 512]
 MB_PREC_FP32 = 0
@@ -196,6 +197,22 @@ class GriffinLimConfig(C.Structure):
 
 class LogMmseConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("window_size", "len1", "len2", "n_fft")]
+
+
+class VitsConfig(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("n_vocab", "inter_channels", "hidden_channels", "filter_channels", "n_heads", "n_layers",
+                                         "kernel_size", "resblock_type", "num_kernels")] + [
+        ("resblock_kernel_sizes", C.c_int32 * 4), ("num_dilations", C.c_int32), ("resblock_dilation_sizes", (C.c_int32 * 4) * 4),
+        ("num_upsamples", C.c_int32), ("upsample_rates", C.c_int32 * 8), ("upsample_kernel_sizes", C.c_int32 * 8)] + [
+        (n, C.c_int32) for n in ("upsample_initial_channel", "n_speakers", "gin_channels", "use_sdp", "precision")]
+
+
+MB_VITS_DBG = {"spline": 0, "attn": 1, "wn": 2, "ddsconv": 3, "decoder": 4}
+
+
+class VitsDebugSpec(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("kind", "batch", "frames", "index", "sub", "c0", "c1")] + [
+        (n, C.c_void_p) for n in ("lengths", "x", "x2", "x3", "y", "y2")]
 
 
 # name -> (restype, argtypes); every symbol include/mockingbird_b200.h declares
@@ -393,6 +410,24 @@ SIGNATURES = {
                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_ppgx_debug_workspace_bytes": (C.c_size_t, [C.POINTER(PpgxDebugSpec)]),
     "mb_ppgx_debug": (C.c_int, [C.POINTER(PpgxDebugSpec), C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]),
+    "mb_vits_create": (C.c_int, [C.POINTER(VitsConfig), C.POINTER(C.c_void_p)]),
+    "mb_vits_destroy": (None, [C.c_void_p]),
+    "mb_vits_arena_bytes": (C.c_size_t, [C.c_void_p]),
+    "mb_vits_set_arena": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "mb_vits_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int32, C.c_void_p]),
+    "mb_vits_finalize": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "mb_vits_hop": (C.c_int32, [C.c_void_p]),
+    "mb_vits_max_tokens": (C.c_int32, []),
+    "mb_vits_durations_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.c_int32]),
+    "mb_vits_durations": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                    C.c_void_p]),
+    "mb_vits_decode_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "mb_vits_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                 C.c_int32, C.c_void_p, C.c_float, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mb_vits_debug_workspace_bytes": (C.c_size_t, [C.c_void_p, C.POINTER(VitsDebugSpec)]),
+    "mb_vits_debug": (C.c_int, [C.c_void_p, C.POINTER(VitsDebugSpec), C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 _lib: Optional[C.CDLL] = None

@@ -30,6 +30,8 @@ struct Layer {
   bool transposed = false;
   int nearest = 1;  // nearest-neighbour upsample factor in front of an odd-k conv (Fre-GAN res_output: k = 1; 24 kHz ups.*.1)
   float in_slope = 1.f;
+  int tpad = -1;         // MB_GAN_VITS: ConvTranspose1d padding (k-u)//2 without output padding (-1: HiFi-GAN's s/2 + s%2)
+  bool no_bias = false;  // MB_GAN_VITS conv_post (bias=False): the bias region stays zero and is not settable
   int src = BUF_NONE, dst = BUF_NONE, res = BUF_NONE, dst2 = BUF_NONE;
   int mode = EPI_STORE;
   float div = 1.f;
@@ -74,7 +76,7 @@ void build_taps(Layer& L) {
   if (L.transposed) {
     // ConvTranspose1d(k, stride=s, padding=p=s/2+s%2, output_padding=s%2) (models.py:120-123):
     //   out[i*s - p + kk] += x[i] * w[:, :, kk]   ->   phase r = o mod s gathers taps kk == r+p (mod s)
-    const int s = L.stride, p = s / 2 + s % 2;
+    const int s = L.stride, p = L.tpad >= 0 ? L.tpad : s / 2 + s % 2;
     t.stride = s;
     for (int r = 0; r < s; ++r) {
       int n = 0;
@@ -265,6 +267,7 @@ int build_plan(mb_gan* h) {
         return fail(MB_ERR_INVALID, "mb_gan_create: receptive field of resblock kernel %d dilation %d too wide",
                     c.resblock_kernel_sizes[j], c.resblock_dilation_sizes[j][m]);
   const bool interp = c.kind == MB_GAN_HIFIGAN_INTERP;
+  const bool vits = c.kind == MB_GAN_VITS;
   for (int i = 0; i < c.num_upsamples; ++i) {
     const int u = c.upsample_rates[i], k = c.upsample_kernel_sizes[i];
     if (u < 1 || u > kMaxPhases) return fail(MB_ERR_INVALID, "mb_gan_create: upsample rate %d unsupported", u);
@@ -286,6 +289,12 @@ int build_plan(mb_gan* h) {
       }
       continue;
     }
+    if (vits) {
+      // ConvTranspose1d(k, u, padding=(k-u)//2) (vits.py:255-257): (L-1)u - 2p + k = u*L exactly when k - u is even
+      if (k < u || (k - u) % 2 != 0)
+        return fail(MB_ERR_INVALID, "mb_gan_create: VITS upsample (k=%d,u=%d) does not produce u*L samples", k, u);
+      continue;
+    }
     // output length (L-1)u - 2p + k + op must equal u*L
     if (k - 2 * (u / 2 + u % 2) + (u % 2) != u)
       return fail(MB_ERR_INVALID, "mb_gan_create: upsample (k=%d,u=%d) does not produce u*L samples", k, u);
@@ -293,7 +302,7 @@ int build_plan(mb_gan* h) {
   const int T = new_buf(h), X = new_buf(h), R = new_buf(h), S = new_buf(h);
   const int C0 = c.upsample_initial_channel;
   int rate = 1;
-  if (c.kind == MB_GAN_HIFIGAN || interp) {
+  if (c.kind == MB_GAN_HIFIGAN || interp || vits) {
     add_conv(h, "conv_pre", c.num_mels, C0, 7, 1, 1, false, 1, 1.f, BUF_IN, T, BUF_NONE, 1);
     int cur = T;
     int ch = C0;
@@ -304,7 +313,8 @@ int build_plan(mb_gan* h) {
                  BUF_NONE, rate);
       else
         add_conv(h, "ups." + std::to_string(i), ch, ch / 2, c.upsample_kernel_sizes[i], 1, u, true, 1, 0.1f, cur, X,
-                 BUF_NONE, rate);
+                 BUF_NONE, rate)
+            .tpad = vits ? (c.upsample_kernel_sizes[i] - u) / 2 : -1;
       ch /= 2;
       rate *= u;
       add_mrf(h, i, ch, rate, X, R, T, S);
@@ -312,6 +322,7 @@ int build_plan(mb_gan* h) {
     }
     Layer& post = add_conv(h, "conv_post", ch, 1, 7, 1, 1, false, 1, 0.01f, S, BUF_OUT, BUF_NONE, rate);
     post.act_tanh = 1;
+    post.no_bias = vits;
   } else if (c.kind == MB_GAN_FREGAN) {
     const int cond_level = c.num_upsamples - c.fregan_top_k;
     if (cond_level < 1 || cond_level >= c.num_upsamples - 1)
@@ -507,7 +518,8 @@ int mb_gan_create(const mb_gan_config* cfg, mb_gan** out) {
       // (the 24 kHz HiFi-GAN's folded upsampling layers "ups.{i}.1" read the same leaky-relu plane as a transposed `ups` would)
       const bool res_output = L.name.rfind("res_output.", 0) == 0;
       const bool nearest_f32 = res_output && (L.name.rfind("res_output.0.", 0) == 0 || !env_flag("MB_GAN_NEAREST_TC", true));
-      d.force_f32 = (L.dst2 != BUF_NONE) || nearest_f32;
+      // MB_GAN_VITS conv_pre reads the caller's input with a channel count (inter + gin) the split-input path does not take
+      d.force_f32 = (L.dst2 != BUF_NONE) || nearest_f32 || (cfg->kind == MB_GAN_VITS && L.src == BUF_IN);
       // 3-term split (FP32-equivalent operands): every layer in MB_PREC_F16X3; in MB_PREC_F16TC the serial layers nothing
       // downstream averages out - the upsampling layers `ups.*` (transposed or folded interpolation) / `cond_up.*` (DESIGN.md 3.4;
       // MB_TC_UPS_X3=0 disables)
@@ -554,6 +566,8 @@ int mb_gan_set_weight(mb_gan* h, const char* name, const float* w, const int64_t
   const std::string base = n.substr(0, dot), leaf = n.substr(dot + 1);
   for (Layer& L : h->layers) {
     if (L.kind != OP_CONV || L.name != base) continue;
+    if (leaf == "bias" && L.no_bias)
+      return fail(MB_ERR_INVALID, "mb_gan_set_weight: %s has no bias in MB_GAN_VITS (Conv1d(bias=False))", base.c_str());
     if (leaf == "bias") {
       if (ndim != 1 || dims[0] != L.cout_w)
         return fail(MB_ERR_INVALID, "mb_gan_set_weight: %s expects [%d]", name, L.cout_w);
@@ -574,6 +588,10 @@ int mb_gan_set_weight(mb_gan* h, const char* name, const float* w, const int64_t
                           : launch_pack_slabs_f32(w, h->arena + L.w_off, L.cout_w, L.cin_w, L.k, L.transposed, st, L.cout, L.cin);
       if (e != cudaSuccess) return fail(MB_ERR_CUDA, "pack_slabs: %s", cudaGetErrorString(e));
       count_launch();
+      if (L.no_bias) {
+        MB_CUDA_CHECK(cudaMemsetAsync(h->arena + L.b_off, 0, sizeof(float) * L.cout, st));
+        L.b_set = true;
+      }
       if (h->cfg.precision != MB_PREC_FP32) {
         char* tcbase = (char*)h->arena + align_up(h->f32_floats * sizeof(float), 256);
         int rc = tc_pack_weights(L.tc, L.taps, h->arena + L.w_off, tcbase, st);

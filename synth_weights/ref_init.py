@@ -629,3 +629,120 @@ def ppg_extractor_state_dict(cfg: dict, seed: int = 0, randomize_bn: bool = True
                 elif k.endswith(".bias"):
                     sd[k] = torch.randn(sd[k].shape, generator=g2) * 0.2
     return sd
+
+
+# ---- VITS (models/synthesizer/models/vits.py:389-456), inference modules only ------------------------------------------
+# Two stand-in configurations: the reference tree ships no VITS config or checkpoint.  VITS_CONFIG is the usual VITS shape
+# (multi-speaker, gin_channels = 256); VITS_TOY a small one for fast tests.
+VITS_CONFIG = dict(n_vocab=80, spec_channels=513, segment_size=32, inter_channels=192, hidden_channels=192, filter_channels=768,
+                   n_heads=2, n_layers=6, kernel_size=3, p_dropout=0.1, resblock="1", resblock_kernel_sizes=[3, 7, 11],
+                   resblock_dilation_sizes=[[1, 3, 5], [1, 3, 5], [1, 3, 5]], upsample_rates=[8, 8, 2, 2],
+                   upsample_initial_channel=512, upsample_kernel_sizes=[16, 16, 4, 4], n_speakers=4, gin_channels=256, use_sdp=True)
+VITS_TOY = dict(n_vocab=20, spec_channels=33, segment_size=8, inter_channels=16, hidden_channels=16, filter_channels=32,
+                n_heads=2, n_layers=2, kernel_size=3, p_dropout=0.1, resblock="2", resblock_kernel_sizes=[3, 5],
+                resblock_dilation_sizes=[[1, 3], [1, 3]], upsample_rates=[4, 2], upsample_initial_channel=32,
+                upsample_kernel_sizes=[8, 4], n_speakers=3, gin_channels=8, use_sdp=True)
+
+# single speaker (no emb_g, no cond layers) with upsampling stages whose ConvTranspose1d padding (k-u)//2 differs from
+# HiFi-GAN's u//2 + u%2
+VITS_TOY_1SPK = dict(VITS_TOY, n_speakers=0, gin_channels=0, resblock="1", resblock_kernel_sizes=[3],
+                     resblock_dilation_sizes=[[1, 3, 5]], upsample_rates=[4, 2], upsample_kernel_sizes=[12, 6])
+
+
+def vits_state_dict(cfg: dict, seed: int = 0, gain: float = 1.0) -> Dict[str, torch.Tensor]:
+    """Seeded random weights for ``Vits(**cfg)``'s inference modules (enc_p, emb_g, dp, flow, dec), with the reference's
+    parameter names and shapes and folded ("weight") weight-norm tensors.  Every conv / linear weight is drawn with std
+    gain / sqrt(fan_in) and every bias from N(0, 0.05): the variance-preserving rescale the GAN goldens use, so that neither
+    the text encoder nor the decoder saturates.  ResidualCouplingLayer.post and ConvFlow.proj, zero at the reference's init,
+    are drawn with std 0.1 / sqrt(fan_in) so that every flow does work.  LayerNorm gains are 1 + N(0, 0.05), the SDP's
+    ElementwiseAffine N(0, 0.1)."""
+    import math
+
+    g = torch.Generator().manual_seed(seed)
+    sd: Dict[str, torch.Tensor] = {}
+
+    def rn(*shape, std=1.0):
+        return torch.randn(*shape, generator=g) * std
+
+    def conv(name, co, ci, k, bias=True, scale=1.0, fan=None):
+        sd[name + ".weight"] = rn(co, ci, k, std=scale * gain / math.sqrt(fan or ci * k))
+        if bias:
+            sd[name + ".bias"] = rn(co, std=0.05)
+
+    def ln(name, c):
+        sd[name + ".gamma"] = 1 + rn(c, std=0.05)
+        sd[name + ".beta"] = rn(c, std=0.05)
+
+    I, H, F, K = cfg["inter_channels"], cfg["hidden_channels"], cfg["filter_channels"], cfg["kernel_size"]
+    G, nh = cfg["gin_channels"], cfg["n_heads"]
+    sd["enc_p.emb.weight"] = rn(cfg["n_vocab"], H, std=H ** -0.5)
+    sd["enc_p.emo_proj.weight"] = rn(H, 1024, std=gain / math.sqrt(1024) * 0.5)
+    sd["enc_p.emo_proj.bias"] = rn(H, std=0.05)
+    for i in range(cfg["n_layers"]):
+        a = f"enc_p.encoder.attn_layers.{i}"
+        for c in ("conv_q", "conv_k", "conv_v", "conv_o"):
+            conv(f"{a}.{c}", H, H, 1)
+        sd[a + ".emb_rel_k"] = rn(1, 9, H // nh, std=(H // nh) ** -0.5)
+        sd[a + ".emb_rel_v"] = rn(1, 9, H // nh, std=(H // nh) ** -0.5)
+        ln(f"enc_p.encoder.norm_layers_1.{i}", H)
+        conv(f"enc_p.encoder.ffn_layers.{i}.conv_1", F, H, K)
+        conv(f"enc_p.encoder.ffn_layers.{i}.conv_2", H, F, K)
+        ln(f"enc_p.encoder.norm_layers_2.{i}", H)
+    conv("enc_p.proj", 2 * I, H, 1, scale=0.5)
+    if cfg["n_speakers"] > 1:
+        sd["emb_g.weight"] = rn(cfg["n_speakers"], G)
+
+    def dds(name, c):
+        for l in range(3):
+            conv(f"{name}.convs_sep.{l}", c, 1, 3)
+            conv(f"{name}.convs_1x1.{l}", c, c, 1)
+            ln(f"{name}.norms_1.{l}", c)
+            ln(f"{name}.norms_2.{l}", c)
+
+    if cfg["use_sdp"]:
+        conv("dp.pre", H, H, 1)
+        conv("dp.proj", H, H, 1)
+        dds("dp.convs", H)
+        if G:
+            conv("dp.cond", H, G, 1)
+        sd["dp.flows.0.m"] = rn(2, 1, std=0.1)
+        sd["dp.flows.0.logs"] = rn(2, 1, std=0.1)
+        for f in (1, 3, 5, 7):
+            conv(f"dp.flows.{f}.pre", H, 1, 1)
+            dds(f"dp.flows.{f}.convs", H)
+            conv(f"dp.flows.{f}.proj", 29, H, 1, scale=0.1)
+    else:
+        conv("dp.conv_1", 256, H, 3)
+        ln("dp.norm_1", 256)
+        conv("dp.conv_2", 256, 256, 3)
+        ln("dp.norm_2", 256)
+        conv("dp.proj", 1, 256, 1, scale=0.3)
+        sd["dp.proj.bias"] += 1.0  # logw around 1: durations of 2-4 frames, not all ceil'ed to 1
+        if G:
+            conv("dp.cond", H, G, 1)
+    for f in (0, 2, 4, 6):
+        n = f"flow.flows.{f}"
+        conv(n + ".pre", H, I // 2, 1)
+        for l in range(4):
+            conv(f"{n}.enc.in_layers.{l}", 2 * H, H, 5)
+            conv(f"{n}.enc.res_skip_layers.{l}", 2 * H if l < 3 else H, H, 1)
+        if G:
+            conv(n + ".enc.cond_layer", 2 * H * 4, G, 1)
+        conv(n + ".post", I // 2, H, 1, scale=0.1)
+    C0 = cfg["upsample_initial_channel"]
+    conv("dec.conv_pre", C0, I, 7)
+    if G:
+        conv("dec.cond", C0, G, 1)
+    ch = C0
+    for i, (u, k) in enumerate(zip(cfg["upsample_rates"], cfg["upsample_kernel_sizes"])):
+        sd[f"dec.ups.{i}.weight"] = rn(ch, ch // 2, k, std=gain / math.sqrt(ch * k / u))
+        sd[f"dec.ups.{i}.bias"] = rn(ch // 2, std=0.05)
+        ch //= 2
+        for j, (rk, ds) in enumerate(zip(cfg["resblock_kernel_sizes"], cfg["resblock_dilation_sizes"])):
+            base = f"dec.resblocks.{i * len(cfg['resblock_kernel_sizes']) + j}"
+            groups = ("convs1", "convs2") if str(cfg["resblock"]) == "1" else ("convs",)
+            for grp in groups:
+                for m in range(len(ds)):
+                    conv(f"{base}.{grp}.{m}", ch, ch, rk, scale=0.5)
+    conv("dec.conv_post", 1, ch, 7, bias=False)
+    return sd
