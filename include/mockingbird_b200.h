@@ -1132,6 +1132,82 @@ typedef struct mb_vits_debug_spec {
 size_t mb_vits_debug_workspace_bytes(const mb_vits* h, const mb_vits_debug_spec* spec);
 int mb_vits_debug(mb_vits* h, const mb_vits_debug_spec* spec, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- wav2vec2 emotion model (models/synthesizer/models/wav2emo.py EmotionExtractorModel, the model of extract_emo) ----------
+ * Wav2Vec2Config fields as the caller parsed them.  create refuses what the kernels do not implement: feat_extract_norm
+ * "group", do_stable_layer_norm False, activations other than "gelu", adapters, a head size other than 64, widths that are not
+ * multiples of 64, conv layers 1.. with more than 5 taps, and positional-conv groups that are not a multiple of 64 wide. */
+#define MB_EMO_NORM_LAYER 0           /* feat_extract_norm "layer"; MB_EMO_NORM_GROUP "group" (rejected) */
+#define MB_EMO_NORM_GROUP 1
+#define MB_EMO_ACT_GELU 0             /* feat_extract_activation / hidden_act "gelu"; MB_EMO_ACT_OTHER anything else (rejected) */
+#define MB_EMO_ACT_OTHER 1
+typedef struct mb_emo_config {
+  int32_t hidden_size, num_hidden_layers, num_attention_heads, intermediate_size;
+  int32_t num_conv_layers;                            /* len(conv_dim), 1..8 */
+  int32_t conv_dim[8], conv_kernel[8], conv_stride[8];
+  int32_t conv_bias;
+  int32_t num_conv_pos_embeddings, num_conv_pos_embedding_groups;
+  float layer_norm_eps;
+  int32_t feat_extract_norm, do_stable_layer_norm, feat_extract_activation, hidden_act, add_adapter;
+  int32_t num_labels;
+} mb_emo_config;
+
+typedef struct mb_emo mb_emo;
+
+int mb_emo_create(const mb_emo_config* cfg, mb_emo** out);
+void mb_emo_destroy(mb_emo* h);
+size_t mb_emo_arena_bytes(const mb_emo* h);
+int mb_emo_set_arena(mb_emo* h, void* arena, size_t bytes);
+/* tensors of EmotionExtractorModel.state_dict() under their reference names, except the positional conv: its weight norm is
+ * folded by the caller into "wav2vec2.encoder.pos_conv_embed.conv.weight" [hidden][hidden / groups][taps] (g v / ||v|| with
+ * one norm per tap).  wav2vec2.masked_spec_embed is accepted and ignored.  finalize packs the tensor-core weight images. */
+int mb_emo_set_weight(mb_emo* h, const char* name, const float* w, const int64_t* dims, int32_t ndim, void* stream);
+int mb_emo_finalize(mb_emo* h, void* stream);
+/* encoder frames of an n-sample clip: floor((n - k) / s) + 1 per conv layer; 0 when the clip is too short for one */
+int32_t mb_emo_num_frames(const mb_emo* h, int32_t n_samples);
+size_t mb_emo_workspace_bytes(const mb_emo* h, int32_t batch, int32_t n_samples_max);
+/* EmotionExtractorModel.forward of 1..128 clips, each computed as its own B = 1 call (bitwise):
+ *   wav fp32 (device): the clips' raw samples concatenated; n_samples int32 [B] (host), each with at least one frame
+ *   emb fp32 [B][hidden]: the mean of the last hidden state over the clip's frames; logits fp32 [B][num_labels]
+ *   normalize: 1 runs the feature extractor's zero-mean unit-variance normalisation (numpy's float32 order) on each clip
+ *     first; 0 takes wav as the model's input_values
+ *   normed fp32 like wav, or NULL (ignored unless normalize): the normalised input
+ *   hidden fp32 [B][T_max][hidden], or NULL: the last hidden state, zero past each clip's frames,
+ *     T_max = mb_emo_num_frames(h, max n_samples); the workspace is mb_emo_workspace_bytes(h, B, max n_samples) */
+int mb_emo_forward(mb_emo* h, const float* wav, const int32_t* n_samples, int32_t batch, int32_t normalize, float* emb,
+                   float* logits, float* normed, float* hidden, void* workspace, size_t workspace_bytes, void* stream);
+
+/* test hook: ONE launch of an emotion-model kernel on caller-provided device tensors (no model handle), through the launch
+ * helpers the forward uses.  lengths int32 [batch] (host): per clip, samples (NORM, CONV0) or valid frames of `frames`
+ * (every other kind); rows [B][frames] are padded per clip.  Kinds:
+ *   NORM     x: the clips' samples concatenated -> y like x, normalised
+ *   CONV0    x: normalised samples concatenated, w [dim][1][kernel], bias [dim] or NULL, stride -> y [B][frames][dim]
+ *   LN_ACT   x [B][frames][dim] -> y: LayerNorm (eps, gamma, beta) then act (0 none, 3 gelu); y may be x
+ *   POSCONV  x [B][frames][dim], w [dim][dim / groups][kernel] (folded), bias [dim] -> y = x + gelu(conv) (packs w as finalize)
+ *   ATTN     x = qkv [B][frames][3 dim], heads of 64 -> y = context [B][frames][dim]
+ *   MEAN     x [B][frames][dim] -> y [B][dim]
+ *   HEAD     x [B][dim], w [n_out][dim], bias [n_out], act (0 none, 1 tanh) -> y [B][n_out]
+ * Rows past each clip's frames are written as zeros where the forward writes them (CONV0, LN_ACT, POSCONV, ATTN). */
+#define MB_EMO_DBG_NORM 0
+#define MB_EMO_DBG_CONV0 1
+#define MB_EMO_DBG_LN_ACT 2
+#define MB_EMO_DBG_POSCONV 3
+#define MB_EMO_DBG_ATTN 4
+#define MB_EMO_DBG_MEAN 5
+#define MB_EMO_DBG_HEAD 6
+typedef struct mb_emo_debug_spec {
+  int32_t kind, batch, frames, dim, n_out, groups, kernel, stride, heads, act;
+  float eps;
+  const int32_t* lengths;
+  const float* x;
+  const float* w;
+  const float* bias;
+  const float* gamma;
+  const float* beta;
+  float* y;
+} mb_emo_debug_spec;
+size_t mb_emo_debug_workspace_bytes(const mb_emo_debug_spec* spec);
+int mb_emo_debug(const mb_emo_debug_spec* spec, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -180,6 +180,20 @@ class PpgxConfig(C.Structure):
         "selfattention_layer_type", "activation_type", "use_cnn_module", "cnn_module_kernel")]
 
 
+class EmoConfig(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("hidden_size", "num_hidden_layers", "num_attention_heads", "intermediate_size",
+                                         "num_conv_layers")] + [
+        ("conv_dim", C.c_int32 * 8), ("conv_kernel", C.c_int32 * 8), ("conv_stride", C.c_int32 * 8), ("conv_bias", C.c_int32),
+        ("num_conv_pos_embeddings", C.c_int32), ("num_conv_pos_embedding_groups", C.c_int32), ("layer_norm_eps", C.c_float)] + [
+        (n, C.c_int32) for n in ("feat_extract_norm", "do_stable_layer_norm", "feat_extract_activation", "hidden_act",
+                                 "add_adapter", "num_labels")]
+
+
+class EmoDebugSpec(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("kind", "batch", "frames", "dim", "n_out", "groups", "kernel", "stride", "heads", "act")] + [
+        ("eps", C.c_float), ("lengths", C.POINTER(C.c_int32))] + [(n, C.c_void_p) for n in ("x", "w", "bias", "gamma", "beta", "y")]
+
+
 class MelSpecConfig(C.Structure):
     _fields_ = [("sample_rate", C.c_int32), ("n_fft", C.c_int32), ("hop_length", C.c_int32), ("win_length", C.c_int32),
                 ("n_mels", C.c_int32), ("fmin", C.c_float), ("fmax", C.c_float), ("pad_mode", C.c_int32),
@@ -410,6 +424,18 @@ SIGNATURES = {
                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_ppgx_debug_workspace_bytes": (C.c_size_t, [C.POINTER(PpgxDebugSpec)]),
     "mb_ppgx_debug": (C.c_int, [C.POINTER(PpgxDebugSpec), C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]),
+    "mb_emo_create": (C.c_int, [C.POINTER(EmoConfig), C.POINTER(C.c_void_p)]),
+    "mb_emo_destroy": (None, [C.c_void_p]),
+    "mb_emo_arena_bytes": (C.c_size_t, [C.c_void_p]),
+    "mb_emo_set_arena": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "mb_emo_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int32, C.c_void_p]),
+    "mb_emo_finalize": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "mb_emo_num_frames": (C.c_int32, [C.c_void_p, C.c_int32]),
+    "mb_emo_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.c_int32]),
+    "mb_emo_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mb_emo_debug_workspace_bytes": (C.c_size_t, [C.POINTER(EmoDebugSpec)]),
+    "mb_emo_debug": (C.c_int, [C.POINTER(EmoDebugSpec), C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_vits_create": (C.c_int, [C.POINTER(VitsConfig), C.POINTER(C.c_void_p)]),
     "mb_vits_destroy": (None, [C.c_void_p]),
     "mb_vits_arena_bytes": (C.c_size_t, [C.c_void_p]),

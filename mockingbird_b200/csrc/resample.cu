@@ -25,6 +25,7 @@
 
 #include "gan_tc_dev.cuh"
 #include "mb_common.h"
+#include "mb_pairwise.cuh"
 
 using namespace mb;
 using namespace mb::tcdev;
@@ -138,55 +139,13 @@ struct LvClip {
   int32_t depth;  // the pairwise tree is split into 2^depth subtrees, one per thread; every node above them is internal
 };
 
-// numpy's pairwise_sum of float32 (numpy/_core/src/umath/loops_utils.h.src) over the squares of a[0 .. n)
-__device__ float pairwise_sq(const float* a, int64_t n) {
-  if (n < 8) {
-    float r = -0.0f;
-    for (int64_t i = 0; i < n; ++i) r = __fadd_rn(r, __fmul_rn(a[i], a[i]));
-    return r;
-  }
-  if (n <= 128) {
-    float r[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) r[k] = __fmul_rn(a[k], a[k]);
-    int64_t i = 8;
-    for (; i < n - (n % 8); i += 8)
-#pragma unroll
-      for (int k = 0; k < 8; ++k) r[k] = __fadd_rn(r[k], __fmul_rn(a[i + k], a[i + k]));
-    float res = __fadd_rn(__fadd_rn(__fadd_rn(r[0], r[1]), __fadd_rn(r[2], r[3])),
-                          __fadd_rn(__fadd_rn(r[4], r[5]), __fadd_rn(r[6], r[7])));
-    for (; i < n; ++i) res = __fadd_rn(res, __fmul_rn(a[i], a[i]));
-    return res;
-  }
-  int64_t n2 = n / 2;
-  n2 -= n2 % 8;
-  return __fadd_rn(pairwise_sq(a, n2), pairwise_sq(a + n2, n - n2));
-}
-
 __global__ void __launch_bounds__(kLevelThreads) rs_sumsq_kernel(const float* __restrict__ x, const LvClip* clips,
                                                                  float* __restrict__ sumsq) {
   __shared__ float part[kLevelThreads];
   const LvClip c = clips[blockIdx.x];
-  const int nsub = 1 << c.depth;
-  if ((int)threadIdx.x < nsub) {
-    int64_t off = 0, n = c.n;
-    for (int d = c.depth - 1; d >= 0; --d) {  // walk down: bit d of the thread index picks the right half
-      int64_t n2 = n / 2;
-      n2 -= n2 % 8;
-      if ((threadIdx.x >> d) & 1) off += n2, n -= n2;
-      else n = n2;
-    }
-    part[threadIdx.x] = pairwise_sq(x + c.off + off, n);
-  }
-  __syncthreads();
-  for (int w = nsub >> 1; w >= 1; w >>= 1) {  // the levels above the subtrees, bottom up: left + right
-    float v = 0.0f;
-    if ((int)threadIdx.x < w) v = __fadd_rn(part[2 * threadIdx.x], part[2 * threadIdx.x + 1]);
-    __syncthreads();
-    if ((int)threadIdx.x < w) part[threadIdx.x] = v;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) sumsq[blockIdx.x] = part[0];
+  const float* a = x + c.off;
+  const float s = pairwise_sum_block([a](int64_t i) { return __fmul_rn(a[i], a[i]); }, c.n, c.depth, part);
+  if (threadIdx.x == 0) sumsq[blockIdx.x] = s;
 }
 
 __global__ void __launch_bounds__(kLevelThreads) rs_scale_kernel(const float* __restrict__ x, const LvClip* clips,
@@ -212,26 +171,6 @@ __global__ void __launch_bounds__(kLevelThreads) rs_rescale_kernel(const float* 
   for (int64_t i = threadIdx.x; i < c.n; i += blockDim.x) y[c.off + i] = __fmul_rn(__fdiv_rn(xc[i], m), peak);
 }
 
-// the deepest level (<= 8) whose nodes all sit below internal nodes (more than 128 elements) of numpy's pairwise tree
-int pairwise_depth(int64_t n) {
-  std::vector<int64_t> sizes{n};
-  int d = 0;
-  while (d < 8) {
-    if (*std::min_element(sizes.begin(), sizes.end()) <= 128) break;
-    std::vector<int64_t> next;
-    for (int64_t s : sizes) {
-      int64_t n2 = s / 2;
-      n2 -= n2 % 8;
-      next.push_back(n2);
-      next.push_back(s - n2);
-    }
-    std::sort(next.begin(), next.end());
-    next.erase(std::unique(next.begin(), next.end()), next.end());
-    sizes.swap(next);
-    ++d;
-  }
-  return d;
-}
 
 struct Filter {
   int32_t up, down, half_len, taps;

@@ -22,16 +22,19 @@ def _cfg_get(h, key, default=None):
     return getattr(h, key, default)
 
 
-def fold_weight_norm(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+def fold_weight_norm(sd: Dict[str, torch.Tensor], dim: int = 0) -> Dict[str, torch.Tensor]:
     """``remove_weight_norm`` (hifigan/models.py:152-162): w = g * v / ||v|| with the norm over all
-    dims but 0 (weight_norm's default dim=0: C_out for Conv1d, C_in for ConvTranspose1d).
-    Load-time only, evaluated with torch ops on the tensors' own device."""
+    dims but `dim` (weight_norm's default dim=0: C_out for Conv1d, C_in for ConvTranspose1d; wav2vec2's
+    positional conv uses dim=2, one norm per tap).  Load-time only, evaluated with torch ops on the tensors' own device."""
     out: Dict[str, torch.Tensor] = {}
     for k, v in sd.items():
         if k.endswith(".weight_g"):
             base = k[: -len(".weight_g")]
             wv = sd[base + ".weight_v"].float()
-            norm = wv.reshape(wv.shape[0], -1).norm(dim=1).reshape(-1, *([1] * (wv.dim() - 1)))
+            wt = wv.transpose(0, dim)
+            shape = [1] * wv.dim()
+            shape[dim] = -1
+            norm = wt.reshape(wt.shape[0], -1).norm(dim=1).reshape(shape)
             out[base + ".weight"] = wv * (v.float() / norm)
         elif k.endswith(".weight_v"):
             continue

@@ -26,6 +26,7 @@ effective weights - they keep Conv1d's default kaiming-uniform init.
 """
 from __future__ import annotations
 
+import math
 from typing import Dict
 
 import torch
@@ -745,4 +746,87 @@ def vits_state_dict(cfg: dict, seed: int = 0, gain: float = 1.0) -> Dict[str, to
                 for m in range(len(ds)):
                     conv(f"{base}.{grp}.{m}", ch, ch, rk, scale=0.5)
     conv("dec.conv_post", 1, ch, 7, bias=False)
+    return sd
+
+
+# ---- wav2vec2 emotion model (models/synthesizer/models/wav2emo.py EmotionExtractorModel) -----------------------------------
+# The released checkpoint (audeering/wav2vec2-large-robust-12-ft-emotion-msp-dim) and its config.json are not in the
+# reference tree.  WAV2EMO_CONFIG is a stand-in with that model's published shape, taken from its public model card and
+# config: wav2vec2-large-robust pruned to 12 layers, hidden 1024, 16 heads, 4096 units, 128-tap positional conv in 16 groups,
+# conv_bias, layer_norm_eps 1e-5, and 3 regression labels (arousal, dominance, valence).
+WAV2EMO_CONFIG = dict(
+    hidden_size=1024, num_hidden_layers=12, num_attention_heads=16, intermediate_size=4096,
+    conv_dim=[512] * 7, conv_kernel=[10, 3, 3, 3, 3, 2, 2], conv_stride=[5, 2, 2, 2, 2, 2, 2], conv_bias=True,
+    num_conv_pos_embeddings=128, num_conv_pos_embedding_groups=16, layer_norm_eps=1e-5,
+    feat_extract_norm="layer", do_stable_layer_norm=True, feat_extract_activation="gelu", hidden_act="gelu",
+    add_adapter=False, num_labels=3, final_dropout=0.1, vocab_size=32,
+)
+WAV2EMO_CONFIG_SMALL = dict(WAV2EMO_CONFIG, hidden_size=128, num_hidden_layers=2, num_attention_heads=2, intermediate_size=256,
+                            conv_dim=[128] * 5, conv_kernel=[10, 3, 3, 2, 2], conv_stride=[5, 2, 2, 2, 2],
+                            num_conv_pos_embeddings=16, num_conv_pos_embedding_groups=2)
+WAV2EMO_SMALL_VARIANTS = {
+    "nobias": dict(conv_bias=False),
+    "oddpos": dict(num_conv_pos_embeddings=15),          # odd kernel: SamePad removes nothing
+    "groups1": dict(num_conv_pos_embedding_groups=1),    # one 128-channel group
+    "short": dict(conv_dim=[128] * 3, conv_kernel=[10, 3, 3], conv_stride=[5, 2, 2]),
+    "onelabel": dict(num_labels=1, layer_norm_eps=1e-6),
+}
+
+
+def wav2emo_variant(name: str) -> dict:
+    return dict(WAV2EMO_CONFIG_SMALL, **WAV2EMO_SMALL_VARIANTS[name])
+
+
+def wav2emo_state_dict(cfg: dict, seed: int = 0) -> Dict[str, torch.Tensor]:
+    """EmotionExtractorModel weights in transformers-5 key names (the positional conv's weight norm as
+    parametrizations.weight.original0 / original1).  Variance-preserving linear and conv weights, LayerNorm affines away from
+    (1, 0), small biases, and a classifier whose tanh input stays well inside (-1, 1), so every stage does work."""
+    g = torch.Generator().manual_seed(seed)
+
+    def normal(*shape, std=1.0):
+        return torch.randn(*shape, generator=g) * std
+
+    sd: Dict[str, torch.Tensor] = {}
+    D, U = cfg["hidden_size"], cfg["intermediate_size"]
+
+    def ln(name, n):
+        sd[name + ".weight"] = 1.0 + normal(n, std=0.1)
+        sd[name + ".bias"] = normal(n, std=0.1)
+
+    def linear(name, n_out, n_in, gain=1.0):
+        sd[name + ".weight"] = normal(n_out, n_in, std=gain / math.sqrt(n_in))
+        sd[name + ".bias"] = normal(n_out, std=0.05)
+
+    c_in = 1
+    for i, (c, k) in enumerate(zip(cfg["conv_dim"], cfg["conv_kernel"])):
+        b = f"wav2vec2.feature_extractor.conv_layers.{i}."
+        sd[b + "conv.weight"] = normal(c, c_in, k, std=1.0 / math.sqrt(c_in * k))
+        if cfg["conv_bias"]:
+            sd[b + "conv.bias"] = normal(c, std=0.05)
+        ln(b + "layer_norm", c)
+        c_in = c
+    ln("wav2vec2.feature_projection.layer_norm", c_in)
+    linear("wav2vec2.feature_projection.projection", D, c_in)
+    sd["wav2vec2.masked_spec_embed"] = torch.rand(D, generator=g)
+    k, G = cfg["num_conv_pos_embeddings"], cfg["num_conv_pos_embedding_groups"]
+    p = "wav2vec2.encoder.pos_conv_embed.conv."
+    sd[p + "bias"] = normal(D, std=0.05)
+    sd[p + "parametrizations.weight.original0"] = 0.5 + torch.rand(1, 1, k, generator=g) * math.sqrt(D / k)
+    sd[p + "parametrizations.weight.original1"] = normal(D, D // G, k)
+    ln("wav2vec2.encoder.layer_norm", D)
+    for i in range(cfg["num_hidden_layers"]):
+        b = f"wav2vec2.encoder.layers.{i}."
+        for n in ("q_proj", "k_proj", "v_proj", "out_proj"):
+            linear(b + "attention." + n, D, D)
+        ln(b + "layer_norm", D)
+        linear(b + "feed_forward.intermediate_dense", U, D)
+        linear(b + "feed_forward.output_dense", D, U)
+        ln(b + "final_layer_norm", D)
+    linear("classifier.dense", D, D, gain=2.0)
+    linear("classifier.out_proj", cfg["num_labels"], D)
+    # biases of magnitude 0.5..1 keep each logit away from zero, so its error is measured against a value the head produces
+    # rather than against the cancellation of out_proj's terms
+    n = cfg["num_labels"]
+    sign = torch.where(torch.rand(n, generator=g) < 0.5, -1.0, 1.0)
+    sd["classifier.out_proj.bias"] = sign * (0.5 + 0.5 * torch.rand(n, generator=g))
     return sd
