@@ -246,9 +246,11 @@ int mb_wavernn_finalize(mb_wavernn* h, void* stream);
 size_t mb_wavernn_workspace_bytes(const mb_wavernn* h, int32_t frames, int32_t folds, int32_t steps);
 
 /* UpsampleNetwork.forward on the padded mel (fatchord_version.py:168-170): mel [80, T] fp32
- * (already divided by mel_max_abs_value, inference.py:60-61) -> frame-rate conditioning kept in
- * the workspace (aux [T,128]; the mel FIR ladder is evaluated on the fly by the sample loop's
- * conditioning stage, the 200x upsampled tensors are never materialised in full). */
+ * (already divided by mel_max_abs_value, inference.py:60-61) -> the conditioning the sample loop reads, kept in
+ * the workspace: aux [T,128], the mel ladder's output melup [200T,80] and three frame-rate tables of the aux
+ * contributions (DESIGN.md section 4.1).  This is mb_wavernn_condition_multi with one utterance: T + 4 frames
+ * must stay below 2^31 / (200 * 80), i.e. T <= 134 213 (about 28 min at 16 kHz); a longer mel is refused with
+ * MB_ERR_INVALID and mb_wavernn_workspace_bytes returns 0 for it. */
 int mb_wavernn_condition(mb_wavernn* h, const float* mel, int32_t frames, void* workspace,
                          size_t workspace_bytes, void* stream);
 

@@ -42,23 +42,13 @@ constexpr int RB = 64;          // rows per row block
 constexpr int kThreads = 512;
 
 // ------------------------------------------------------------------------------------------------
-// conditioning kernels: one thread per output, sequential fmaf chains in the twin's order
+// conditioning kernels: one thread per output, sequential fmaf chains in the twin's order.  The frames of the call's
+// utterances are concatenated (one utterance is the case n_utts = 1): utterance u owns frames [segF[u], segF[u] + segT[u]) of
+// the [C][Ttot] activations, of aux [Ttot][128] and (x200) of melup, padded frames [segF[u] + 4u, + segT[u] + 4) of the ladder
+// buffers and rows [segF[u] + u, + segT[u] + 1) of the aux tables (the last one is its "past the end" row).  k_bn / k_conv1x1
+// are frame-wise and run over Ttot frames; the kernels after them must not look across an utterance boundary.
+// fseg / pseg: utterance of a frame / padded frame.
 // ------------------------------------------------------------------------------------------------
-__global__ void k_conv_in(const float* __restrict__ w, const float* __restrict__ mel, int T, float* __restrict__ y) {
-  // y[o][t] = sum_{ci,k} w[o][ci][k] * P[ci][t+k],  P = mel padded by 2 zero frames on both sides
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= CDIM * T) return;
-  const int o = i / T, t = i - o * T;
-  float acc = 0.0f;
-  for (int ci = 0; ci < FEAT; ++ci)
-    for (int k = 0; k < 5; ++k) {
-      const int s = t + k - 2;
-      const float v = (s >= 0 && s < T) ? mel[ci * T + s] : 0.0f;
-      acc = fmaf(w[(o * FEAT + ci) * 5 + k], v, acc);
-    }
-  y[i] = acc;
-}
-
 __global__ void k_bn(const float* __restrict__ g, const float* __restrict__ b, const float* __restrict__ mean,
                      const float* __restrict__ var, float* __restrict__ x, int T, int relu, const float* res) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -85,63 +75,9 @@ __global__ void k_conv1x1(const float* __restrict__ w, const float* __restrict__
   else y[i] = acc;
 }
 
-// one ladder stage: y[c][i] = sum_j w[j] * rep(x)[i + j - s]
-__global__ void k_ladder(const float* __restrict__ w, const float* __restrict__ x, int len, int s,
-                         float* __restrict__ y) {
-  const int nl = len * s;
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= FEAT * nl) return;
-  const int c = i / nl, p = i - c * nl;
-  float acc = 0.0f;
-  for (int j = 0; j <= 2 * s; ++j) {
-    const int src = p + j - s;
-    const float v = (src >= 0 && src < nl) ? x[c * len + src / s] : 0.0f;
-    acc = fmaf(w[j], v, acc);
-  }
-  y[i] = acc;
-}
-
-__global__ void k_pad_mel(const float* __restrict__ mel, int T, float* __restrict__ P) {
-  const int Tp = T + 4;
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= FEAT * Tp) return;
-  const int c = i / Tp, t = i - c * Tp;
-  P[i] = (t >= 2 && t < T + 2) ? mel[c * T + t - 2] : 0.0f;
-}
-
-__global__ void k_crop_melup(const float* __restrict__ y3, int len, int T, float* __restrict__ melup) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= HOP * T * FEAT) return;
-  const int t = i / FEAT, c = i - t * FEAT;
-  melup[i] = y3[c * len + t + 2 * HOP];
-}
-
-// frame-rate tables: out[f][g] = dot_seq(W[g][K0 : K0+32], aux[f][a0 : a0+32]) + bias[g]; row f == T is
-// the "past the end" row (zero conditioning)
-__global__ void k_aux_table(const float* __restrict__ W, int ld, int K0, const float* __restrict__ bias,
-                            const float* __restrict__ aux, int a0, int T, int G, float* __restrict__ out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (T + 1) * G) return;
-  const int f = i / G, g = i - f * G;
-  float acc = 0.0f;
-  for (int j = 0; j < AUXD; ++j) {
-    const float a = (f < T) ? aux[f * CDIM + a0 + j] : 0.0f;
-    acc = fmaf(W[(size_t)g * ld + K0 + j], a, acc);
-  }
-  out[i] = acc + bias[g];
-}
-
-// ------------------------------------------------------------------------------------------------
-// conditioning of a set of utterances (mb_wavernn_condition_multi).  The frames of all utterances are concatenated:
-// utterance u owns frames [segF[u], segF[u] + segT[u]) of the [C][Ttot] activations, of aux [Ttot][128] and (x200) of melup,
-// padded frames [segF[u] + 4u, + segT[u] + 4) of the ladder buffers and rows [segF[u] + u, + segT[u] + 1) of the aux tables
-// (the last one is its "past the end" row).  k_bn / k_conv1x1 are frame-wise and run unchanged over Ttot frames; the kernels
-// below are the ones that must not look across an utterance boundary.  fseg / pseg: utterance of a frame / padded frame.
-// Per output the fmaf chain is that of the single-utterance kernel, so utterance u's tables equal mb_wavernn_condition's.
-// ------------------------------------------------------------------------------------------------
-__global__ void k_conv_in_multi(const float* __restrict__ w, const float* __restrict__ mel, int Ttot,
-                                const int* __restrict__ fseg, const int* __restrict__ segF, const int* __restrict__ segT,
-                                float* __restrict__ y) {
+// y[o][t] = sum_{ci,k} w[o][ci][k] * P[ci][t+k],  P = the utterance's mel padded by 2 zero frames on both sides
+__global__ void k_conv_in(const float* __restrict__ w, const float* __restrict__ mel, int Ttot, const int* __restrict__ fseg,
+                          const int* __restrict__ segF, const int* __restrict__ segT, float* __restrict__ y) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= CDIM * Ttot) return;
   const int o = i / Ttot, tg = i - o * Ttot;
@@ -157,8 +93,8 @@ __global__ void k_conv_in_multi(const float* __restrict__ w, const float* __rest
   y[i] = acc;
 }
 
-__global__ void k_pad_mel_multi(const float* __restrict__ mel, int Tptot, const int* __restrict__ pseg,
-                                const int* __restrict__ segF, const int* __restrict__ segT, float* __restrict__ P) {
+__global__ void k_pad_mel(const float* __restrict__ mel, int Tptot, const int* __restrict__ pseg, const int* __restrict__ segF,
+                          const int* __restrict__ segT, float* __restrict__ P) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= FEAT * Tptot) return;
   const int c = i / Tptot, pg = i - c * Tptot;
@@ -166,10 +102,11 @@ __global__ void k_pad_mel_multi(const float* __restrict__ mel, int Tptot, const 
   P[i] = (t >= 2 && t < T + 2) ? mel[(size_t)FEAT * F + c * T + t - 2] : 0.0f;
 }
 
-// one ladder stage over all utterances; `per` = input positions per padded frame (1, 5, 25)
-__global__ void k_ladder_multi(const float* __restrict__ w, const float* __restrict__ x, int len, int s, int per,
-                               const int* __restrict__ pseg, const int* __restrict__ segF, const int* __restrict__ segT,
-                               float* __restrict__ y) {
+// one ladder stage, y[c][i] = sum_j w[j] * rep(x)[i + j - s] within each utterance; `per` = input positions per padded frame
+// (1, 5, 25)
+__global__ void k_ladder(const float* __restrict__ w, const float* __restrict__ x, int len, int s, int per,
+                         const int* __restrict__ pseg, const int* __restrict__ segF, const int* __restrict__ segT,
+                         float* __restrict__ y) {
   const size_t nl = (size_t)len * s;
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= FEAT * nl) return;
@@ -186,8 +123,8 @@ __global__ void k_ladder_multi(const float* __restrict__ w, const float* __restr
   y[i] = acc;
 }
 
-__global__ void k_crop_melup_multi(const float* __restrict__ y3, int len, int Ttot, const int* __restrict__ fseg,
-                                   float* __restrict__ melup) {
+__global__ void k_crop_melup(const float* __restrict__ y3, int len, int Ttot, const int* __restrict__ fseg,
+                             float* __restrict__ melup) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)HOP * Ttot * FEAT) return;
   const int tg = (int)(i / FEAT), c = (int)(i - (size_t)tg * FEAT);
@@ -195,10 +132,11 @@ __global__ void k_crop_melup_multi(const float* __restrict__ y3, int len, int Tt
   melup[i] = y3[(size_t)c * len + tg + HOP * (4 * u) + 2 * HOP];
 }
 
-// tsrc[f]: frame of aux behind table row f, or -1 for an utterance's "past the end" row
-__global__ void k_aux_table_multi(const float* __restrict__ W, int ld, int K0, const float* __restrict__ bias,
-                                  const float* __restrict__ aux, int a0, const int* __restrict__ tsrc, int R, int G,
-                                  float* __restrict__ out) {
+// frame-rate tables: out[f][g] = dot_seq(W[g][K0 : K0+32], aux[tsrc[f]][a0 : a0+32]) + bias[g]; tsrc[f] = -1 marks an
+// utterance's "past the end" row (zero conditioning)
+__global__ void k_aux_table(const float* __restrict__ W, int ld, int K0, const float* __restrict__ bias,
+                            const float* __restrict__ aux, int a0, const int* __restrict__ tsrc, int R, int G,
+                            float* __restrict__ out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= R * G) return;
   const int f = i / G, g = i - f * G;
@@ -821,11 +759,9 @@ struct mb_wavernn {
   size_t total_floats = 0;
   float* arena = nullptr;
   bool finalized = false;
-  // conditioning of the current utterance (workspace-resident)
-  int cond_T = 0;
-  void* cond_ws = nullptr;
-  // ... or of the current set of utterances (mb_wavernn_condition_multi): frames per utterance; empty otherwise
+  // conditioning held in the workspace cond_ws: frames per utterance of the last mb_wavernn_condition[_multi]; empty before
   std::vector<int32_t> cond_frames;
+  void* cond_ws = nullptr;
 };
 
 namespace {
@@ -839,8 +775,8 @@ struct Ws {
 };
 
 // T frames of U utterances in all (each utterance has its own "past the end" table row and its own 4 frames of ladder padding);
-// multi: the segment tables of the conditioning kernels and the row descriptors of the multi-utterance loop are laid out too
-Ws ws_layout(int T, int Bpad, int chunk_steps, int U = 1, bool multi = false) {
+// the segment tables of the conditioning kernels and the row descriptors of the multi-utterance loop are always laid out
+Ws ws_layout(int T, int Bpad, int chunk_steps, int U) {
   Ws L{};
   WsLayout W;
   L.aux = W.take<float>((size_t)T * CDIM);
@@ -855,7 +791,7 @@ Ws ws_layout(int T, int Bpad, int chunk_steps, int U = 1, bool multi = false) {
   L.lad5 = W.take<float>((size_t)FEAT * (T + 4 * U) * 5);
   L.lad25 = W.take<float>((size_t)FEAT * (T + 4 * U) * 25);
   L.lad200 = W.take<float>((size_t)FEAT * (T + 4 * U) * HOP);
-  if (multi) L.segs = W.take<float>((size_t)3 * T + 7 * U);  // int32: fseg[T] pseg[T+4U] tsrc[T+U] segF[U] segT[U]
+  L.segs = W.take<float>((size_t)3 * T + 7 * U);  // int32: fseg[T] pseg[T+4U] tsrc[T+U] segF[U] segT[U]
   L.starts = W.take<float>((size_t)Bpad);
   L.condI = W.take<float>((size_t)chunk_steps * RNN * Bpad);
   L.h1 = W.take<float>((size_t)2 * RNN * Bpad);
@@ -865,7 +801,7 @@ Ws ws_layout(int T, int Bpad, int chunk_steps, int U = 1, bool multi = false) {
   L.logits = W.take<float>((size_t)RNN * Bpad);
   L.xprev = W.take<float>((size_t)Bpad);
   L.barrier = W.take<float>(256);  // 1 KB: counter, or one epoch word per CTA
-  if (multi) L.rowdesc = W.take<float>((size_t)10 * Bpad);  // int4 rowc[Bpad] | int4 rown[Bpad] | uint64 rowseed[Bpad]
+  L.rowdesc = W.take<float>((size_t)10 * Bpad);  // int4 rowc[Bpad] | int4 rown[Bpad] | uint64 rowseed[Bpad]
   L.total = W.total();
   return L;
 }
@@ -873,6 +809,112 @@ Ws ws_layout(int T, int Bpad, int chunk_steps, int U = 1, bool multi = false) {
 constexpr int kChunkMax = 128;  // steps per mb_wavernn_generate call
 
 int bpad_of(int B) { return ((B + RB - 1) / RB) * RB; }
+
+// total frames of a set of utterances, or -1 when the list is not usable
+int64_t total_frames(const int32_t* frames, int32_t n_utts) {
+  if (!frames || n_utts <= 0) return -1;
+  int64_t tot = 0;
+  for (int u = 0; u < n_utts; ++u) {
+    if (frames[u] <= 0) return -1;
+    tot += frames[u];
+  }
+  // the kernels index the x200 upsampled, 80-channel ladder with 32-bit ints
+  return ((tot + 4 * (int64_t)n_utts) * HOP * FEAT < (int64_t)1 << 31) ? tot : -1;
+}
+
+// conditioning of n_utts utterances (mb_wavernn_condition is the case n_utts = 1): MelResNet, the x200 mel ladder and the three
+// frame-rate aux tables of every utterance, written into the workspace for the sample loop
+int condition_impl(const char* fn, mb_wavernn* h, const float* mel_concat, const int32_t* frames, int32_t n_utts,
+                   void* workspace, size_t workspace_bytes, void* stream) {
+  if (!h || !mel_concat || !frames) return fail(MB_ERR_INVALID, "%s: null argument", fn);
+  const int64_t tot = total_frames(frames, n_utts);
+  if (tot < 0) return fail(MB_ERR_INVALID, "%s: bad utterance lengths (each > 0, %d frames in all at most)", fn,
+                           (int)(((int64_t)1 << 31) / (HOP * FEAT)));
+  const int U = n_utts, Ttot = (int)tot, Tptot = Ttot + 4 * U, R = Ttot + U;
+  // the conditioning part of the layout does not depend on the row count; the check asks for the smallest full workspace
+  const Ws L = ws_layout(Ttot, RB, kChunkMax, U);
+  float* ws;
+  if (int rc = bind(fn, workspace, workspace_bytes, L.total, &ws)) return rc;
+  if (!h->finalized) return fail(MB_ERR_STATE, "%s: weights not finalized", fn);
+  cudaStream_t st = (cudaStream_t)stream;
+  // segment tables
+  std::vector<int32_t> seg((size_t)3 * Ttot + 7 * U);
+  int32_t* fseg_h = seg.data();
+  int32_t* pseg_h = fseg_h + Ttot;
+  int32_t* tsrc_h = pseg_h + Tptot;
+  int32_t* segF_h = tsrc_h + R;
+  int32_t* segT_h = segF_h + U;
+  for (int u = 0, F = 0; u < U; F += frames[u], ++u) {
+    const int T = frames[u];
+    segF_h[u] = F;
+    segT_h[u] = T;
+    for (int t = 0; t < T; ++t) fseg_h[F + t] = u;
+    for (int t = 0; t < T + 4; ++t) pseg_h[F + 4 * u + t] = u;
+    for (int t = 0; t <= T; ++t) tsrc_h[F + u + t] = t < T ? F + t : -1;
+  }
+  int* fseg = reinterpret_cast<int*>(ws + L.segs);
+  const int *pseg = fseg + Ttot, *tsrc = pseg + Tptot, *segF = tsrc + R, *segT = segF + U;
+  MB_CUDA_CHECK(cudaMemcpyAsync(fseg, seg.data(), sizeof(int32_t) * seg.size(), cudaMemcpyHostToDevice, st));
+  MB_CUDA_CHECK(cudaStreamSynchronize(st));  // seg goes out of scope
+  const int n = CDIM * Ttot, nb = (n + 255) / 256;
+  float *x = ws + L.tmpA, *y = ws + L.tmpB, *r = ws + L.tmpR;
+  k_conv_in<<<nb, 256, 0, st>>>(W(h, "upsample.resnet.conv_in.weight"), mel_concat, Ttot, fseg, segF, segT, x);
+  MB_LAUNCH_CHECK("k_conv_in");
+  auto bnrun = [&](const std::string& p, float* buf, int relu, const float* res) -> int {
+    k_bn<<<nb, 256, 0, st>>>(W(h, p + ".weight"), W(h, p + ".bias"), W(h, p + ".running_mean"), W(h, p + ".running_var"),
+                             buf, Ttot, relu, res);
+    MB_LAUNCH_CHECK("k_bn");
+    return MB_OK;
+  };
+  int rc = bnrun("upsample.resnet.batch_norm", x, 1, nullptr);
+  if (rc) return rc;
+  for (int i = 0; i < h->cfg.res_blocks; ++i) {
+    const std::string b = "upsample.resnet.layers." + std::to_string(i);
+    MB_CUDA_CHECK(cudaMemcpyAsync(r, x, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
+    k_conv1x1<<<nb, 256, 0, st>>>(W(h, b + ".conv1.weight"), x, Ttot, y, nullptr, 0);
+    MB_LAUNCH_CHECK("k_conv1x1");
+    if ((rc = bnrun(b + ".batch_norm1", y, 1, nullptr))) return rc;
+    k_conv1x1<<<nb, 256, 0, st>>>(W(h, b + ".conv2.weight"), y, Ttot, x, nullptr, 0);
+    MB_LAUNCH_CHECK("k_conv1x1");
+    if ((rc = bnrun(b + ".batch_norm2", x, 0, r))) return rc;
+  }
+  k_conv1x1<<<nb, 256, 0, st>>>(W(h, "upsample.resnet.conv_out.weight"), x, Ttot, ws + L.aux,
+                                W(h, "upsample.resnet.conv_out.bias"), 1);
+  MB_LAUNCH_CHECK("k_conv1x1");
+  // mel ladder: P (each utterance padded by 2 frames on both sides) -> x5 -> x25 -> x200, then crop
+  float* P = ws + L.padP;
+  float* l5 = ws + L.lad5;
+  float* l25 = ws + L.lad25;
+  float* l1 = ws + L.lad200;
+  k_pad_mel<<<(FEAT * Tptot + 255) / 256, 256, 0, st>>>(mel_concat, Tptot, pseg, segF, segT, P);
+  MB_LAUNCH_CHECK("k_pad_mel");
+  const int s0 = h->cfg.upsample_factors[0], s1 = h->cfg.upsample_factors[1], s2 = h->cfg.upsample_factors[2];
+  auto blocks = [](size_t n_out) { return (unsigned)((n_out + 255) / 256); };
+  k_ladder<<<blocks((size_t)FEAT * Tptot * s0), 256, 0, st>>>(W(h, "upsample.up_layers.1.weight"), P, Tptot, s0, 1, pseg, segF,
+                                                             segT, l5);
+  MB_LAUNCH_CHECK("k_ladder");
+  k_ladder<<<blocks((size_t)FEAT * Tptot * s0 * s1), 256, 0, st>>>(W(h, "upsample.up_layers.3.weight"), l5, Tptot * s0, s1, s0,
+                                                                  pseg, segF, segT, l25);
+  MB_LAUNCH_CHECK("k_ladder");
+  k_ladder<<<blocks((size_t)FEAT * Tptot * HOP), 256, 0, st>>>(W(h, "upsample.up_layers.5.weight"), l25, Tptot * s0 * s1, s2,
+                                                              s0 * s1, pseg, segF, segT, l1);
+  MB_LAUNCH_CHECK("k_ladder");
+  k_crop_melup<<<blocks((size_t)HOP * Ttot * FEAT), 256, 0, st>>>(l1, Tptot * HOP, Ttot, fseg, ws + L.melup);
+  MB_LAUNCH_CHECK("k_crop_melup");
+  // frame-rate tables of the aux contributions
+  k_aux_table<<<(R * 3 * RNN + 255) / 256, 256, 0, st>>>(W(h, "rnn2.weight_ih_l0"), RNN + AUXD, RNN, W(h, "rnn2.bias_ih_l0"),
+                                                         ws + L.aux, AUXD, tsrc, R, 3 * RNN, ws + L.aux2P);
+  MB_LAUNCH_CHECK("k_aux_table");
+  k_aux_table<<<(R * RNN + 255) / 256, 256, 0, st>>>(W(h, "fc1.weight"), RNN + AUXD, RNN, W(h, "fc1.bias"), ws + L.aux,
+                                                     2 * AUXD, tsrc, R, RNN, ws + L.aux3P);
+  MB_LAUNCH_CHECK("k_aux_table");
+  k_aux_table<<<(R * RNN + 255) / 256, 256, 0, st>>>(W(h, "fc2.weight"), RNN + AUXD, RNN, W(h, "fc2.bias"), ws + L.aux,
+                                                     3 * AUXD, tsrc, R, RNN, ws + L.aux4P);
+  MB_LAUNCH_CHECK("k_aux_table");
+  h->cond_ws = workspace;
+  h->cond_frames.assign(frames, frames + U);
+  return MB_OK;
+}
 
 }  // namespace
 
@@ -981,78 +1023,25 @@ int mb_wavernn_finalize(mb_wavernn* h, void* stream) {
 }
 
 size_t mb_wavernn_workspace_bytes(const mb_wavernn* h, int32_t frames, int32_t folds, int32_t steps) {
-  if (!h || frames <= 0 || folds <= 0) return 0;
-  (void)steps;
-  return ws_layout(frames, bpad_of(folds), kChunkMax).total;
+  return mb_wavernn_workspace_bytes_multi(h, 1, &frames, folds, steps);
+}
+
+size_t mb_wavernn_workspace_bytes_multi(const mb_wavernn* h, int32_t n_utts, const int32_t* frames, int32_t rows,
+                                        int32_t max_steps) {
+  const int64_t Ttot = total_frames(frames, n_utts);
+  if (!h || Ttot < 0 || rows <= 0) return 0;
+  (void)max_steps;
+  return ws_layout((int)Ttot, bpad_of(rows), kChunkMax, n_utts).total;
 }
 
 int mb_wavernn_condition(mb_wavernn* h, const float* mel, int32_t T, void* workspace, size_t workspace_bytes,
                          void* stream) {
-  if (!h || !mel || T <= 0) return fail(MB_ERR_INVALID, "mb_wavernn_condition: bad argument");
-  if (!h->finalized) return fail(MB_ERR_STATE, "mb_wavernn_condition: weights not finalized");
-  // the conditioning part of the layout does not depend on the fold count; the check asks for the smallest full workspace
-  const Ws L = ws_layout(T, RB, kChunkMax);
-  float* ws;
-  if (int rc = bind("mb_wavernn_condition", workspace, workspace_bytes, L.total, &ws)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int n = CDIM * T, nb = (n + 255) / 256;
-  float *x = ws + L.tmpA, *y = ws + L.tmpB, *r = ws + L.tmpR;
-  k_conv_in<<<nb, 256, 0, st>>>(W(h, "upsample.resnet.conv_in.weight"), mel, T, x);
-  MB_LAUNCH_CHECK("k_conv_in");
-  auto bnrun = [&](const std::string& p, float* buf, int relu, const float* res) -> int {
-    k_bn<<<nb, 256, 0, st>>>(W(h, p + ".weight"), W(h, p + ".bias"), W(h, p + ".running_mean"), W(h, p + ".running_var"),
-                             buf, T, relu, res);
-    MB_LAUNCH_CHECK("k_bn");
-    return MB_OK;
-  };
-  int rc = bnrun("upsample.resnet.batch_norm", x, 1, nullptr);
-  if (rc) return rc;
-  for (int i = 0; i < h->cfg.res_blocks; ++i) {
-    const std::string b = "upsample.resnet.layers." + std::to_string(i);
-    MB_CUDA_CHECK(cudaMemcpyAsync(r, x, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
-    k_conv1x1<<<nb, 256, 0, st>>>(W(h, b + ".conv1.weight"), x, T, y, nullptr, 0);
-    MB_LAUNCH_CHECK("k_conv1x1");
-    if ((rc = bnrun(b + ".batch_norm1", y, 1, nullptr))) return rc;
-    k_conv1x1<<<nb, 256, 0, st>>>(W(h, b + ".conv2.weight"), y, T, x, nullptr, 0);
-    MB_LAUNCH_CHECK("k_conv1x1");
-    if ((rc = bnrun(b + ".batch_norm2", x, 0, r))) return rc;
-  }
-  k_conv1x1<<<nb, 256, 0, st>>>(W(h, "upsample.resnet.conv_out.weight"), x, T, ws + L.aux,
-                                W(h, "upsample.resnet.conv_out.bias"), 1);
-  MB_LAUNCH_CHECK("k_conv1x1");
-  // mel ladder: P (Tp) -> x5 -> x25 -> x200, then crop
-  const int Tp = T + 4;
-  float* P = ws + L.padP;
-  float* l5 = ws + L.lad5;
-  float* l25 = ws + L.lad25;
-  float* l1 = ws + L.lad200;
-  k_pad_mel<<<(FEAT * Tp + 255) / 256, 256, 0, st>>>(mel, T, P);
-  MB_LAUNCH_CHECK("k_pad_mel");
-  const int s0 = h->cfg.upsample_factors[0], s1 = h->cfg.upsample_factors[1], s2 = h->cfg.upsample_factors[2];
-  k_ladder<<<(FEAT * Tp * s0 + 255) / 256, 256, 0, st>>>(W(h, "upsample.up_layers.1.weight"), P, Tp, s0, l5);
-  MB_LAUNCH_CHECK("k_ladder");
-  k_ladder<<<(FEAT * Tp * s0 * s1 + 255) / 256, 256, 0, st>>>(W(h, "upsample.up_layers.3.weight"), l5, Tp * s0, s1, l25);
-  MB_LAUNCH_CHECK("k_ladder");
-  k_ladder<<<(int)(((size_t)FEAT * Tp * HOP + 255) / 256), 256, 0, st>>>(W(h, "upsample.up_layers.5.weight"), l25,
-                                                                          Tp * s0 * s1, s2, l1);
-  MB_LAUNCH_CHECK("k_ladder");
-  k_crop_melup<<<(int)(((size_t)HOP * T * FEAT + 255) / 256), 256, 0, st>>>(l1, Tp * HOP, T, ws + L.melup);
-  MB_LAUNCH_CHECK("k_crop_melup");
-  // frame-rate tables of the aux contributions
-  k_aux_table<<<((T + 1) * 3 * RNN + 255) / 256, 256, 0, st>>>(W(h, "rnn2.weight_ih_l0"), RNN + AUXD, RNN,
-                                                               W(h, "rnn2.bias_ih_l0"), ws + L.aux, AUXD, T, 3 * RNN,
-                                                               ws + L.aux2P);
-  MB_LAUNCH_CHECK("k_aux_table");
-  k_aux_table<<<((T + 1) * RNN + 255) / 256, 256, 0, st>>>(W(h, "fc1.weight"), RNN + AUXD, RNN, W(h, "fc1.bias"),
-                                                           ws + L.aux, 2 * AUXD, T, RNN, ws + L.aux3P);
-  MB_LAUNCH_CHECK("k_aux_table");
-  k_aux_table<<<((T + 1) * RNN + 255) / 256, 256, 0, st>>>(W(h, "fc2.weight"), RNN + AUXD, RNN, W(h, "fc2.bias"),
-                                                           ws + L.aux, 3 * AUXD, T, RNN, ws + L.aux4P);
-  MB_LAUNCH_CHECK("k_aux_table");
-  h->cond_T = T;
-  h->cond_ws = workspace;
-  h->cond_frames.clear();
-  return MB_OK;
+  return condition_impl("mb_wavernn_condition", h, mel, &T, 1, workspace, workspace_bytes, stream);
+}
+
+int mb_wavernn_condition_multi(mb_wavernn* h, const float* mel_concat, const int32_t* frames, int32_t n_utts, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+  return condition_impl("mb_wavernn_condition_multi", h, mel_concat, frames, n_utts, workspace, workspace_bytes, stream);
 }
 
 int mb_wavernn_generate(mb_wavernn* h, const int32_t* fold_starts_host, int32_t B, int32_t steps, int32_t step0,
@@ -1075,13 +1064,13 @@ int generate_rows_impl(mb_wavernn* h, const int32_t* fold_starts_host, int32_t B
   if (row0 < 0 || (noise && row0 + B > noise_folds))
     return fail(MB_ERR_INVALID, "mb_wavernn_generate_rows: rows [%d, %d) outside the %d noise rows", row0, row0 + B, noise_folds);
   if (!h->finalized) return fail(MB_ERR_STATE, "mb_wavernn_generate: weights not finalized");
-  if (h->cond_T <= 0 || h->cond_ws != workspace)
+  if (h->cond_frames.size() != 1 || h->cond_ws != workspace)
     return fail(MB_ERR_STATE, "mb_wavernn_generate: call mb_wavernn_condition on this workspace first");
   if (B <= 0 || nsteps <= 0 || nsteps > kChunkMax || step0 < 0 || step0 + nsteps > steps)
     return fail(MB_ERR_INVALID, "mb_wavernn_generate: bad step range (at most %d steps per call)", kChunkMax);
-  const int T = h->cond_T;
+  const int T = h->cond_frames[0];
   const int Bpad = bpad_of(B);
-  const Ws L = ws_layout(T, Bpad, kChunkMax);
+  const Ws L = ws_layout(T, Bpad, kChunkMax, 1);
   float* ws;
   if (int rc = bind("mb_wavernn_generate", workspace, workspace_bytes, L.total, &ws)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
@@ -1178,9 +1167,10 @@ int mb_wavernn_generate_rows_mol(mb_wavernn* h, const int32_t* fold_starts_host,
 }
 
 int mb_wavernn_last_logits(mb_wavernn* h, float* logits, int32_t B, void* workspace, void* stream) {
-  if (!h || !logits || !workspace || h->cond_T <= 0) return fail(MB_ERR_INVALID, "mb_wavernn_last_logits: bad argument");
+  if (!h || !logits || !workspace || h->cond_frames.size() != 1)
+    return fail(MB_ERR_INVALID, "mb_wavernn_last_logits: bad argument");
   const int Bpad = bpad_of(B);
-  const Ws L = ws_layout(h->cond_T, Bpad, kChunkMax);
+  const Ws L = ws_layout(h->cond_frames[0], Bpad, kChunkMax, 1);
   float* ws = aligned<float>(workspace);
   // logits are stored [class][Bpad]; return [B][ncls] (512 RAW, 30 MOL)
   const int ncls = h->ncls;
@@ -1199,18 +1189,6 @@ int mb_wavernn_last_logits(mb_wavernn* h, float* logits, int32_t B, void* worksp
 // several utterances in one sample loop
 // =================================================================================================
 namespace {
-
-// total frames of a set of utterances, or -1 when the list is not usable
-int64_t total_frames(const int32_t* frames, int32_t n_utts) {
-  if (!frames || n_utts <= 0) return -1;
-  int64_t tot = 0;
-  for (int u = 0; u < n_utts; ++u) {
-    if (frames[u] <= 0) return -1;
-    tot += frames[u];
-  }
-  // the kernels index the x200 upsampled, 80-channel ladder with 32-bit ints
-  return ((tot + 4 * (int64_t)n_utts) * HOP * FEAT < (int64_t)1 << 31) ? tot : -1;
-}
 
 int generate_multi_impl(const char* fn, mb_wavernn* h, const int32_t* row_utt, const int32_t* row_start,
                         const int32_t* row_steps, const int32_t* row_fold, int32_t rows, const uint64_t* utt_seeds,
@@ -1243,7 +1221,7 @@ int generate_multi_impl(const char* fn, mb_wavernn* h, const int32_t* row_utt, c
   for (int r = 0; r < rows; ++r)
     if (row_utt[r] >= U) return fail(MB_ERR_INVALID, "%s: row %d names utterance %d of %d", fn, r, row_utt[r], U);
   const int Bpad = bpad_of(rows);
-  const Ws L = ws_layout(Ttot, Bpad, kChunkMax, U, true);
+  const Ws L = ws_layout(Ttot, Bpad, kChunkMax, U);
   float* ws;
   if (int rc = bind(fn, workspace, workspace_bytes, L.total, &ws)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
@@ -1302,105 +1280,6 @@ int generate_multi_impl(const char* fn, mb_wavernn* h, const int32_t* row_utt, c
 }  // namespace
 
 extern "C" {
-
-size_t mb_wavernn_workspace_bytes_multi(const mb_wavernn* h, int32_t n_utts, const int32_t* frames, int32_t rows,
-                                        int32_t max_steps) {
-  const int64_t Ttot = total_frames(frames, n_utts);
-  if (!h || Ttot < 0 || rows <= 0) return 0;
-  (void)max_steps;
-  return ws_layout((int)Ttot, bpad_of(rows), kChunkMax, n_utts, true).total;
-}
-
-int mb_wavernn_condition_multi(mb_wavernn* h, const float* mel_concat, const int32_t* frames, int32_t n_utts, void* workspace,
-                               size_t workspace_bytes, void* stream) {
-  if (!h || !mel_concat || !frames) return fail(MB_ERR_INVALID, "mb_wavernn_condition_multi: null argument");
-  const int64_t tot = total_frames(frames, n_utts);
-  if (tot < 0) return fail(MB_ERR_INVALID, "mb_wavernn_condition_multi: bad utterance lengths (each > 0, %d frames in all at most)",
-                           (int)(((int64_t)1 << 31) / (HOP * FEAT)));
-  const int U = n_utts, Ttot = (int)tot, Tptot = Ttot + 4 * U, R = Ttot + U;
-  // the conditioning part of the layout does not depend on the row count; the check asks for the smallest full workspace
-  const Ws L = ws_layout(Ttot, RB, kChunkMax, U, true);
-  float* ws;
-  if (int rc = bind("mb_wavernn_condition_multi", workspace, workspace_bytes, L.total, &ws)) return rc;
-  if (!h->finalized) return fail(MB_ERR_STATE, "mb_wavernn_condition_multi: weights not finalized");
-  cudaStream_t st = (cudaStream_t)stream;
-  // segment tables
-  std::vector<int32_t> seg((size_t)3 * Ttot + 7 * U);
-  int32_t* fseg_h = seg.data();
-  int32_t* pseg_h = fseg_h + Ttot;
-  int32_t* tsrc_h = pseg_h + Tptot;
-  int32_t* segF_h = tsrc_h + R;
-  int32_t* segT_h = segF_h + U;
-  for (int u = 0, F = 0; u < U; F += frames[u], ++u) {
-    const int T = frames[u];
-    segF_h[u] = F;
-    segT_h[u] = T;
-    for (int t = 0; t < T; ++t) fseg_h[F + t] = u;
-    for (int t = 0; t < T + 4; ++t) pseg_h[F + 4 * u + t] = u;
-    for (int t = 0; t <= T; ++t) tsrc_h[F + u + t] = t < T ? F + t : -1;
-  }
-  int* fseg = reinterpret_cast<int*>(ws + L.segs);
-  const int *pseg = fseg + Ttot, *tsrc = pseg + Tptot, *segF = tsrc + R, *segT = segF + U;
-  MB_CUDA_CHECK(cudaMemcpyAsync(fseg, seg.data(), sizeof(int32_t) * seg.size(), cudaMemcpyHostToDevice, st));
-  MB_CUDA_CHECK(cudaStreamSynchronize(st));  // seg goes out of scope
-  const int n = CDIM * Ttot, nb = (n + 255) / 256;
-  float *x = ws + L.tmpA, *y = ws + L.tmpB, *r = ws + L.tmpR;
-  k_conv_in_multi<<<nb, 256, 0, st>>>(W(h, "upsample.resnet.conv_in.weight"), mel_concat, Ttot, fseg, segF, segT, x);
-  MB_LAUNCH_CHECK("k_conv_in_multi");
-  auto bnrun = [&](const std::string& p, float* buf, int relu, const float* res) -> int {
-    k_bn<<<nb, 256, 0, st>>>(W(h, p + ".weight"), W(h, p + ".bias"), W(h, p + ".running_mean"), W(h, p + ".running_var"),
-                             buf, Ttot, relu, res);
-    MB_LAUNCH_CHECK("k_bn");
-    return MB_OK;
-  };
-  int rc = bnrun("upsample.resnet.batch_norm", x, 1, nullptr);
-  if (rc) return rc;
-  for (int i = 0; i < h->cfg.res_blocks; ++i) {
-    const std::string b = "upsample.resnet.layers." + std::to_string(i);
-    MB_CUDA_CHECK(cudaMemcpyAsync(r, x, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
-    k_conv1x1<<<nb, 256, 0, st>>>(W(h, b + ".conv1.weight"), x, Ttot, y, nullptr, 0);
-    MB_LAUNCH_CHECK("k_conv1x1");
-    if ((rc = bnrun(b + ".batch_norm1", y, 1, nullptr))) return rc;
-    k_conv1x1<<<nb, 256, 0, st>>>(W(h, b + ".conv2.weight"), y, Ttot, x, nullptr, 0);
-    MB_LAUNCH_CHECK("k_conv1x1");
-    if ((rc = bnrun(b + ".batch_norm2", x, 0, r))) return rc;
-  }
-  k_conv1x1<<<nb, 256, 0, st>>>(W(h, "upsample.resnet.conv_out.weight"), x, Ttot, ws + L.aux,
-                                W(h, "upsample.resnet.conv_out.bias"), 1);
-  MB_LAUNCH_CHECK("k_conv1x1");
-  float* P = ws + L.padP;
-  float* l5 = ws + L.lad5;
-  float* l25 = ws + L.lad25;
-  float* l1 = ws + L.lad200;
-  k_pad_mel_multi<<<(FEAT * Tptot + 255) / 256, 256, 0, st>>>(mel_concat, Tptot, pseg, segF, segT, P);
-  MB_LAUNCH_CHECK("k_pad_mel_multi");
-  const int s0 = h->cfg.upsample_factors[0], s1 = h->cfg.upsample_factors[1], s2 = h->cfg.upsample_factors[2];
-  auto blocks = [](size_t n_out) { return (unsigned)((n_out + 255) / 256); };
-  k_ladder_multi<<<blocks((size_t)FEAT * Tptot * s0), 256, 0, st>>>(W(h, "upsample.up_layers.1.weight"), P, Tptot, s0, 1, pseg, segF,
-                                                                   segT, l5);
-  MB_LAUNCH_CHECK("k_ladder_multi");
-  k_ladder_multi<<<blocks((size_t)FEAT * Tptot * s0 * s1), 256, 0, st>>>(W(h, "upsample.up_layers.3.weight"), l5, Tptot * s0, s1, s0,
-                                                                        pseg, segF, segT, l25);
-  MB_LAUNCH_CHECK("k_ladder_multi");
-  k_ladder_multi<<<blocks((size_t)FEAT * Tptot * HOP), 256, 0, st>>>(W(h, "upsample.up_layers.5.weight"), l25, Tptot * s0 * s1, s2,
-                                                                    s0 * s1, pseg, segF, segT, l1);
-  MB_LAUNCH_CHECK("k_ladder_multi");
-  k_crop_melup_multi<<<blocks((size_t)HOP * Ttot * FEAT), 256, 0, st>>>(l1, Tptot * HOP, Ttot, fseg, ws + L.melup);
-  MB_LAUNCH_CHECK("k_crop_melup_multi");
-  k_aux_table_multi<<<(R * 3 * RNN + 255) / 256, 256, 0, st>>>(W(h, "rnn2.weight_ih_l0"), RNN + AUXD, RNN, W(h, "rnn2.bias_ih_l0"),
-                                                               ws + L.aux, AUXD, tsrc, R, 3 * RNN, ws + L.aux2P);
-  MB_LAUNCH_CHECK("k_aux_table_multi");
-  k_aux_table_multi<<<(R * RNN + 255) / 256, 256, 0, st>>>(W(h, "fc1.weight"), RNN + AUXD, RNN, W(h, "fc1.bias"), ws + L.aux,
-                                                           2 * AUXD, tsrc, R, RNN, ws + L.aux3P);
-  MB_LAUNCH_CHECK("k_aux_table_multi");
-  k_aux_table_multi<<<(R * RNN + 255) / 256, 256, 0, st>>>(W(h, "fc2.weight"), RNN + AUXD, RNN, W(h, "fc2.bias"), ws + L.aux,
-                                                           3 * AUXD, tsrc, R, RNN, ws + L.aux4P);
-  MB_LAUNCH_CHECK("k_aux_table_multi");
-  h->cond_T = 0;
-  h->cond_ws = workspace;
-  h->cond_frames.assign(frames, frames + U);
-  return MB_OK;
-}
 
 int mb_wavernn_generate_multi(mb_wavernn* h, const int32_t* row_utt, const int32_t* row_start, const int32_t* row_steps,
                               const int32_t* row_fold, int32_t rows, const uint64_t* utt_seeds, int32_t max_steps,

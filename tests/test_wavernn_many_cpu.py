@@ -56,12 +56,15 @@ def test_workspace_grows_with_frames_and_row_blocks():
     L = _lib.lib()
     fr = lambda *a: (C.c_int32 * len(a))(*a)
     one = L.mb_wavernn_workspace_bytes_multi(h, 1, fr(30), 1, 6000)
-    assert one >= L.mb_wavernn_workspace_bytes(h, 30, 1, 6000) > 0
+    assert one == L.mb_wavernn_workspace_bytes(h, 30, 1, 6000) > 0
+    for T, folds in ((2400, 58), (80, 65)):  # the single call is the one-utterance case
+        assert L.mb_wavernn_workspace_bytes(h, T, folds, 8800) == L.mb_wavernn_workspace_bytes_multi(h, 1, fr(T), folds, 8800) > 0
     assert L.mb_wavernn_workspace_bytes_multi(h, 1, fr(30), 64, 6000) == one  # one row block
     assert L.mb_wavernn_workspace_bytes_multi(h, 1, fr(30), 65, 6000) > one
     assert L.mb_wavernn_workspace_bytes_multi(h, 2, fr(15, 15), 1, 3000) > one  # a second "past the end" row and padding
     assert L.mb_wavernn_workspace_bytes_multi(h, 2, fr(15, 0), 1, 3000) == 0
     assert L.mb_wavernn_workspace_bytes_multi(h, 1, fr(200000), 1, 100) == 0  # past the 32-bit indexing of the mel ladder
+    assert L.mb_wavernn_workspace_bytes(h, 200000, 1, 100) == 0
 
 
 def test_abi_argument_checks():
@@ -80,6 +83,8 @@ def test_abi_argument_checks():
     refused(L.mb_wavernn_condition_multi(raw._handle, p, i32(5, -1), 2, p, 1 << 30, None), "bad utterance lengths")
     refused(L.mb_wavernn_condition_multi(raw._handle, p, i32(5, 6), 2, p, 1024, None), "workspace too small")
     refused(L.mb_wavernn_condition_multi(raw._handle, p, i32(5, 6), 2, p, 1 << 30, None), "weights not finalized")
+    refused(L.mb_wavernn_condition(raw._handle, None, 5, p, 1 << 30, None), "null argument")
+    refused(L.mb_wavernn_condition(raw._handle, p, 200000, p, 1 << 30, None), "bad utterance lengths")
 
     def gen(fn, h, utt, start, steps, fold, max_steps, step0, n, n_live, noise=p, seeds=None):
         return fn(h, i32(*utt), i32(*start), i32(*steps), i32(*fold), len(utt), seeds, max_steps, step0, n, n_live, noise, p, p,

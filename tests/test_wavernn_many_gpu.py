@@ -1,6 +1,7 @@
 """GPU tests of the multi-utterance WaveRNN sample loop (WaveRNN.generate_many, mb_wavernn_condition_multi /
 mb_wavernn_generate_multi[_mol], k_sample_loop<MOL, true>): every utterance of a batch is bit for bit what the
 single-utterance call returns for it alone - conditioning tables, ragged lengths, per-utterance noise, RAW and MOL."""
+import ctypes as C
 import json
 
 import numpy as np
@@ -92,6 +93,23 @@ def test_unbatched_ragged_injected_noise(models, sds, mode):
     aux, melup = twin.condition(mels[0][0].numpy())
     ref = twin.generate(aux, melup, [0], 1400, noise[0].numpy())
     assert np.array_equal(many[0].cpu().numpy(), ref)
+
+
+def test_single_utterance_loop_refuses_many(models):
+    """a workspace conditioned with two utterances is refused by the single-utterance loop, before any device work"""
+    from mockingbird_b200 import _lib
+
+    model, L = models["RAW"], _lib.lib()
+    mel_cat = torch.cat([m.reshape(-1) for m in _mels([5, 9], seed=11)]).to(model._device)
+    frames = (C.c_int32 * 2)(5, 9)
+    stream = C.c_void_p(torch.cuda.current_stream(model._device).cuda_stream)
+    ws = _lib.workspace(L.mb_wavernn_workspace_bytes_multi(model._handle, 2, frames, 1, 1800), model._device, model)
+    _lib.check(L.mb_wavernn_condition_multi(model._handle, C.c_void_p(mel_cat.data_ptr()), frames, 2, C.c_void_p(ws.data_ptr()),
+                                            ws.numel(), stream))
+    out = torch.empty(1, 1000, dtype=torch.int16, device=model._device)
+    rc = L.mb_wavernn_generate_rows(model._handle, (C.c_int32 * 1)(0), 1, 1000, 0, 100, None, 1, 0, 0, C.c_void_p(out.data_ptr()),
+                                    C.c_void_p(ws.data_ptr()), ws.numel(), stream)
+    assert rc != 0 and "call mb_wavernn_condition on this workspace first" in L.mb_last_error().decode()
 
 
 @pytest.mark.parametrize("mode", MODES)
