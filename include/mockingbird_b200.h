@@ -488,6 +488,52 @@ int mb_tacotron_generate_ragged(mb_tacotron* h, const int32_t* chars, const floa
                                 float* mel, float* linear, float* attn, int32_t* frames_out_host, int32_t* row_frames_host,
                                 void* workspace, size_t workspace_bytes, void* stream);
 
+/* Streamed decoding (Tacotron.generate_stream): a decoder loop over `slots` (<= 128) rows that texts enter when a row is free
+ * and leave when their row stops.  Each text's mel, linear and attention are bitwise those mb_tacotron_generate_ragged gives it.
+ *   workspace_bytes / open: texts of at most n_chars characters and max_steps frames; 0 / MB_ERR_INVALID as generate would refuse.
+ *     The workspace holds the encoder's scratch, the decoder loop, the postnet's scratch, a staging pool of 2 x slots encoded
+ *     texts and a pool of 2 x slots finished rows; it must outlive the stream.  open captures the 8-step decoder graph once.
+ *   encode: n texts (chars int32 device [n][n_chars], zero past each text's row_chars[i]; spk device [n][256]; enc_masks device
+ *     [2][n][n_chars][256] or NULL: drawn from row_seeds) into staging-pool rows [pool_row, pool_row + n), inside one half of the
+ *     pool, on an internal encoder stream that runs while the decoder does; it waits for the admissions before it.  `stream`
+ *     does not wait for the encode (only the admissions that copy these rows do), so the inputs must stay allocated until
+ *     the stream is closed.
+ *   admit: texts from the staging pool into free slots, between graph replays (one launch: the slot's state reset to a fresh row's,
+ *     its encoder rows copied, its dropout masks copied from dec_masks[i] (device [>= ceil(row_steps / r)][2][256]) or drawn).
+ *   run: replays the decoder graph 16 steps at a time until at least one occupied row has stopped (at once when none is
+ *     occupied), copies each stopped row's frames and alignment to the finished-row pool and frees its slot; returns their text
+ *     ids and frames in the order found (steps_run: decoder steps run so far).  Blocks the host while it polls.
+ *   harvest: the postnet over the n oldest finished rows not harvested yet, on `stream`: mel, linear [n][80][frames] and attn
+ *     [n][frames / r][n_chars], frames = the longest of their frames; row i's part is its own frames.  Every harvest of a stream
+ *     must use the same `stream`.  run refuses when finished rows would overflow their pool: harvest at least every `slots` rows.
+ *   close: waits for the stream's work and frees it; the model handle stays usable. */
+typedef struct mb_taco_stream mb_taco_stream;
+/* test hook: the per-slot regions of an open stream (device addresses into its workspace).  Admission zeroes slot b's row of
+ * every region with reset = 1 and writes slot b's row of seq, proj, chars, lens, caps, done, start and dmask; pool_* are the
+ * staging pool the encoder writes.  Layouts by kind: */
+#define MB_TACO_REGION_F32 0  /* fp32 [rows][width] */
+#define MB_TACO_REGION_TILE 1 /* fp16 operand tile plane [ceil(width / 64)][rows][64], 16-byte chunks XOR (row & 7) */
+#define MB_TACO_REGION_U8 2   /* uint8 [depth][2][rows][width] (decoder dropout masks: ring steps, layers, slots, units) */
+#define MB_TACO_REGION_I32 3  /* int32 [rows][width] */
+typedef struct mb_taco_stream_region {
+  char name[24];
+  void* ptr;
+  int32_t kind, rows, width, depth, reset;
+} mb_taco_stream_region;
+/* fills up to `max` entries of out (may be NULL) and returns how many regions there are, or a negative error */
+int32_t mb_tacotron_stream_regions(const mb_taco_stream* s, mb_taco_stream_region* out, int32_t max);
+size_t mb_tacotron_stream_workspace_bytes(const mb_tacotron* h, int32_t slots, int32_t n_chars, int32_t max_steps, int32_t r);
+int mb_tacotron_stream_open(mb_tacotron* h, int32_t slots, int32_t n_chars, int32_t max_steps, int32_t r, int32_t style_idx,
+                            float min_stop_token, void* workspace, size_t workspace_bytes, void* stream, mb_taco_stream** out);
+int mb_tacotron_stream_encode(mb_taco_stream* s, int32_t pool_row, int32_t n, const int32_t* chars, const float* spk,
+                              const int32_t* row_chars, const uint64_t* row_seeds, const uint8_t* enc_masks, void* stream);
+int mb_tacotron_stream_admit(mb_taco_stream* s, int32_t n, const int32_t* slot, const int32_t* pool_row, const int64_t* text_id,
+                             const int32_t* row_chars, const int32_t* row_steps, const uint64_t* row_seeds,
+                             const uint8_t* const* dec_masks, void* stream);
+int mb_tacotron_stream_run(mb_taco_stream* s, int32_t* n_done, int64_t* done_ids, int32_t* done_frames, int64_t* steps_run);
+int mb_tacotron_stream_harvest(mb_taco_stream* s, int32_t n, int32_t frames, float* mel, float* linear, float* attn, void* stream);
+void mb_tacotron_stream_close(mb_taco_stream* s);
+
 /* test hook: ONE launch of a 3-term-split tensor-core GEMM of the Tacotron / speaker-encoder family on caller-provided fp32
  * device tensors (no model handle), through the functions the forward uses, in its order: tc_skinny_absmax -> tc_weight_scale ->
  * tc_skinny_pack / pack_big_w -> act_split / im2col_split -> launch_tc_{skinny,gru,lstm_seq,big}.  Tensors are row-major. */
@@ -541,6 +587,8 @@ typedef struct mb_taco_tc_debug_spec {
                                 sequence: a shifted tap reads zeros at and past it (TcIm2col::len).  GRU: device [M] valid
                                 length of each row: direction 1 keeps h = 0 (state, out[1], nxt tiles) while t1 >= len[m] */
   int32_t t1;                /* GRU with len: the time index direction 1 is at in this step (TcGruArgs::t1) */
+  const int32_t* row_start;  /* PLAIN: device [M] per-row step origin, or NULL: row m writes at y + ((step - row_start[m]) % ring) * y_step */
+  int32_t ring;
 } mb_taco_tc_debug_spec;
 /* device workspace the spec needs */
 size_t mb_taco_tc_debug_workspace_bytes(const mb_taco_tc_debug_spec* spec);
@@ -614,6 +662,12 @@ typedef struct mb_taco_debug_spec {
   const int32_t* row_caps;     /* STOP_STEP / STOP_FLAG: device [B] decoder-step cap of each row */
   const uint64_t* row_seeds;   /* FILL_MASKS_SEEDED: device [B] */
   int32_t fma_chain;           /* GEMM / STOP_STEP: into GemmArgs::fma_chain (launch_gemm keeps to gemm32 / gemm64 / gemm_big) */
+  /* per-row step origin of streamed decoding (NULL: every row's step is the global step) */
+  const int32_t* row_start;    /* PRENET / LSA_STEP / LSA_CTX / STOP_STEP / STOP_FLAG: device [B] global step row b started at; its
+                                  step is the global step minus it.  PRENET reads x and the masks, LSA_STEP writes and LSA_CTX reads
+                                  the scores at that step modulo `ring`; the stop kinds apply the rule at it, need row_done /
+                                  row_caps and take flags = NULL */
+  int32_t ring;                /* steps the per-step buffers hold (>= 1 with row_start) */
 } mb_taco_debug_spec;
 /* device workspace the spec needs (no kind needs scratch: a nominal 256 bytes), 0 for a spec mb_taco_debug refuses */
 size_t mb_taco_debug_workspace_bytes(const mb_taco_debug_spec* spec);

@@ -94,6 +94,7 @@ class TacoTcDebugSpec(C.Structure):
         ("nxt_lo", C.c_void_p * 2), ("act", C.c_int32), ("bn_scale", C.c_void_p), ("bn_shift", C.c_void_p),
         ("res", C.c_void_p), ("ldres", C.c_int32), ("compact", C.c_int32), ("cluster", C.c_int32), ("pdl", C.c_int32),
         ("a_tiles", C.c_void_p), ("w_tiles", C.c_void_p), ("len", C.c_void_p), ("t1", C.c_int32),
+        ("row_start", C.c_void_p), ("ring", C.c_int32),
     ]
 
 
@@ -113,7 +114,16 @@ class TacoDebugSpec(C.Structure):
         ("x_step", C.c_int64), ("x_first", C.c_void_p), ("mask_step", C.c_int64), ("in_", C.c_void_p * 12),
         ("out", C.c_void_p * 6), ("n", C.c_int64 * 10), ("fval", C.c_float), ("seed", C.c_uint64), ("row_len", C.c_void_p),
         ("row_done", C.c_void_p), ("row_caps", C.c_void_p), ("row_seeds", C.c_void_p), ("fma_chain", C.c_int32),
+        ("row_start", C.c_void_p), ("ring", C.c_int32),
     ]
+
+
+MB_TACO_REGION = {"f32": 0, "tile": 1, "u8": 2, "i32": 3}
+
+
+class TacoStreamRegion(C.Structure):
+    _fields_ = [("name", C.c_char * 24), ("ptr", C.c_void_p), ("kind", C.c_int32), ("rows", C.c_int32), ("width", C.c_int32),
+                ("depth", C.c_int32), ("reset", C.c_int32)]
 
 
 MB_PPGX_DBG_FRONTEND = 0
@@ -336,6 +346,17 @@ SIGNATURES = {
                                               C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
                                               C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_void_p,
                                               C.c_size_t, C.c_void_p]),
+    "mb_tacotron_stream_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "mb_tacotron_stream_open": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float,
+                                          C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "mb_tacotron_stream_encode": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p]),
+    "mb_tacotron_stream_admit": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mb_tacotron_stream_run": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
+    "mb_tacotron_stream_harvest": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mb_tacotron_stream_close": (None, [C.c_void_p]),
+    "mb_tacotron_stream_regions": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32]),
     "mb_taco_debug_workspace_bytes": (C.c_size_t, [C.POINTER(TacoDebugSpec)]),
     "mb_taco_debug": (C.c_int, [C.POINTER(TacoDebugSpec), C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]),
     "mb_encoder_create": (C.c_int, [C.POINTER(EncoderConfig), C.POINTER(C.c_void_p)]),

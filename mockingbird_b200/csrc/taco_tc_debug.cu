@@ -291,6 +291,8 @@ int mb_taco_tc_debug(const mb_taco_tc_debug_spec* spec, void* workspace, size_t 
     t.step_ptr = s.step_ptr;
     t.step_j = s.step_j;
     t.y_step = s.y_step;
+    t.row_start = s.row_start;
+    t.ring = s.ring;
     t.c = s.c;
     t.h = s.h;
     t.x = s.xres;

@@ -10,7 +10,9 @@
 
 #include <cstdlib>
 #include <cstring>
+#include <algorithm>
 #include <map>
+#include <memory>
 #include <set>
 #include <string>
 #include <vector>
@@ -64,9 +66,10 @@ __global__ void __launch_bounds__(512) lsa_step_kernel(const float* __restrict__
                                                        float* __restrict__ scores_out, int scores_ld, float* ctx, int Tc,
                                                        const int* step_ptr, int step_j, const float* __restrict__ q_in,
                                                        const float* __restrict__ Wq, const float* __restrict__ bq,
-                                                       const int* __restrict__ lens) {
+                                                       const int* __restrict__ lens, const int* __restrict__ row_start, int ring) {
   extern __shared__ float sm[];
-  scores_out += (size_t)step_index(step_ptr, step_j) * Tc;  // this decoder step's row of the alignment matrix
+  // this decoder step's row of the alignment matrix (the row's own step in a ring with a per-row step origin)
+  scores_out += (size_t)ring_slot(row_step(step_index(step_ptr, step_j), row_start, blockIdx.x), row_start, ring) * Tc;
   float* s_cw = sm;                         // [32][31]
   float* s_Lt = s_cw + ATT_F * ATT_K;       // [32][128]  (L transposed: conflict-free for d-major threads)
   float* s_v = s_Lt + ATT_D * ATT_F;        // [128]
@@ -227,13 +230,15 @@ cudaError_t lsa_step_prepare(int Tc) {
 __global__ void __launch_bounds__(256) lsa_ctx_kernel(const float* __restrict__ scores, int scores_ld, const float* __restrict__ seq,
                                                       int seq_dim, int Tc, float* __restrict__ ctx, const int* step_ptr,
                                                       int step_j, __half* sa_hi, __half* sa_lo, __half* sb_hi, __half* sb_lo,
-                                                      int s_rows_pad, const int* __restrict__ lens) {
+                                                      int s_rows_pad, const int* __restrict__ lens, const int* __restrict__ row_start,
+                                                      int ring) {
   __shared__ float4 part[4][64];
   extern __shared__ float s_sc[];
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   const int b = blockIdx.y, f4 = blockIdx.x * 64 + (threadIdx.x & 63), tg = threadIdx.x >> 6;
-  const float* sc = scores + (size_t)step_index(step_ptr, step_j) * Tc + (size_t)b * scores_ld;
+  const int sb = ring_slot(row_step(step_index(step_ptr, step_j), row_start, b), row_start, ring);
+  const float* sc = scores + (size_t)sb * Tc + (size_t)b * scores_ld;
   const int Tb = lens ? lens[b] : Tc;
   for (int t = threadIdx.x; t < Tb; t += 256) s_sc[t] = sc[t];
   __syncthreads();
@@ -371,34 +376,38 @@ __global__ void fill_masks_seeded_kernel(uint8_t* m, int B, int npos, int units,
 
 // stop rule of tacotron.py:275 at decoder step si (frame t = si * r) over the B stop values stopv[b * ld].  Padded batch
 // (row_done == nullptr): flags[si] = every row passes and t > 10.  Ragged rows: row b ends at the first step where it passes with
-// t > 10 or reaches its cap of row_caps[b] steps (row_done[b] = that step, -1 before); flags[si] = every row has ended.
+// t > 10 or reaches its cap of row_caps[b] steps (row_done[b] = that step, -1 before); flags[si] = every row has ended.  With a
+// per-row step origin (row_start) each row applies the rule at its own step and flags is null: the global step is unbounded, so
+// nothing is indexed by it, and the host polls row_done instead.
 __device__ void apply_stop_rule(const float* stopv, int ld, int B, float min_stop_token, int r, int si, int* flags, int* row_done,
-                                const int* row_caps) {
+                                const int* row_caps, const int* row_start) {
   bool all = true;
   for (int b = 0; b < B; ++b) {
     const bool pass = __ldcg(stopv + (size_t)b * ld) * 10.f > min_stop_token;
     if (row_done) {
-      if (row_done[b] < 0 && ((pass && si * r > 10) || si + 1 >= row_caps[b])) row_done[b] = si;
+      const int s = row_step(si, row_start, b);
+      if (row_done[b] < 0 && ((pass && s * r > 10) || s + 1 >= row_caps[b])) row_done[b] = s;
       all = all && row_done[b] >= 0;
     } else {
       all = all && pass;
     }
   }
-  flags[si] = row_done ? (all ? 1 : 0) : ((all && si * r > 10) ? 1 : 0);
+  if (flags) flags[si] = row_done ? (all ? 1 : 0) : ((all && si * r > 10) ? 1 : 0);
 }
 
 // decoder step si = (step_ptr ? *step_ptr : 0) + step_j; frame t = si * r; flags[si] = stop rule of tacotron.py:275
 __global__ void stop_flag_kernel(const float* stopv, int B, float min_stop_token, int r, int* flags, const int* step_ptr,
-                                 int step_j, int* row_done = nullptr, const int* row_caps = nullptr) {
+                                 int step_j, int* row_done = nullptr, const int* row_caps = nullptr, const int* row_start = nullptr) {
   if (threadIdx.x == 0 && blockIdx.x == 0)
-    apply_stop_rule(stopv, 1, B, min_stop_token, r, step_index(step_ptr, step_j), flags, row_done, row_caps);
+    apply_stop_rule(stopv, 1, B, min_stop_token, r, step_index(step_ptr, step_j), flags, row_done, row_caps, row_start);
 }
 
 // stop projection (sigmoid(w . [x | ctx] + b), tacotron.py:131-133) of one batch row per CTA, then - in the CTA that takes the
 // last ticket - the stop rule over all rows.  Same summation order as rowdot_kernel.
 __global__ void __launch_bounds__(256) stop_step_kernel(const GemmArgs a, int B, float min_stop_token, int r, int* flags,
                                                         const int* step_ptr, int step_j, unsigned int* ticket,
-                                                        int* row_done = nullptr, const int* row_caps = nullptr) {
+                                                        int* row_done = nullptr, const int* row_caps = nullptr,
+                                                        const int* row_start = nullptr) {
   __shared__ float red[8];
   __shared__ bool last;
   const int m = blockIdx.x, tid = threadIdx.x;
@@ -422,7 +431,7 @@ __global__ void __launch_bounds__(256) stop_step_kernel(const GemmArgs a, int B,
   if (last && tid == 0) {
     *ticket = 0u;
     __threadfence();
-    apply_stop_rule(a.Y, a.ldy, B, min_stop_token, r, step_index(step_ptr, step_j), flags, row_done, row_caps);
+    apply_stop_rule(a.Y, a.ldy, B, min_stop_token, r, step_index(step_ptr, step_j), flags, row_done, row_caps, row_start);
   }
 }
 
@@ -438,6 +447,89 @@ __global__ void to_ncl_kernel(const float* __restrict__ x, int steps, float* __r
   const int c = (int)((i / frames) % C);
   const int b = (int)(i / ((size_t)frames * C));
   y[i] = x[((size_t)b * steps + t) * C + c];
+}
+
+
+// a few host bytes carried into device memory as a kernel argument (upload() in the stream entry points)
+constexpr int kUploadBytes = 8192;
+struct UploadBlob {
+  unsigned char b[kUploadBytes];
+};
+__global__ void upload_kernel(const __grid_constant__ UploadBlob src, unsigned char* dst, int n) {
+  for (int i = threadIdx.x; i < n; i += blockDim.x) dst[i] = src.b[i];
+}
+
+// ---- streamed decoding (mb_tacotron_stream_*): row admission -----------------------------------------------------------------
+// One launch puts n texts into their slots between graph replays: every recurrent state, ctx, cum, the side stream's half-sums and
+// both parities of the fused-split operand tiles of the slot go to the zeros a fresh row starts from; the text's encoder rows
+// (seq, encoder_proj keys) and characters are copied from the staging pool; its decoder dropout masks are copied (injected) or drawn
+// (Philox keyed by its seed, as fill_masks_seeded_kernel) for its steps 0 .. cap - 1; its length, cap, done step (-1) and start
+// step are set.  blockIdx.y = admitted row.
+struct AdmitRow {
+  int slot, src, len, cap;  // slot, staging-pool row, characters, decoder-step cap
+  uint64_t seed;
+  const uint8_t* dmask;     // injected masks [>= cap][2][units], or null: drawn from seed
+};
+struct RowZero {            // row `slot` of a region: nchunks chunks of chunk_bytes at p + c * chunk_stride + slot * row_stride
+  char* p;
+  long long row_stride, chunk_stride;
+  int nchunks, chunk_bytes;
+};
+constexpr int kMaxZero = 32;
+struct AdmitArgs {
+  const AdmitRow* rows;
+  int start;                // global step the rows start at
+  RowZero zero[kMaxZero];
+  int nzero;
+  const float* src_seq;     // staging pool [2 * slots][Tc][seq_row / Tc]
+  float* seq;
+  long long seq_row;
+  const float* src_proj;
+  float* proj;
+  long long proj_row;
+  const int32_t* src_chars;
+  int32_t* chars;
+  int Tc;
+  int* lens;
+  int* caps;
+  int* done;
+  int* starts;
+  uint8_t* dmask;           // [ring][2][S][units]
+  int S, units;
+};
+
+__global__ void admit_rows_kernel(const __grid_constant__ AdmitArgs a) {
+  const AdmitRow row = a.rows[blockIdx.y];
+  const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x, nth = (long long)gridDim.x * blockDim.x;
+  for (int z = 0; z < a.nzero; ++z) {
+    const RowZero& r = a.zero[z];
+    const int words = r.chunk_bytes / 4;
+    for (long long i = tid; i < (long long)r.nchunks * words; i += nth) {
+      const long long c = i / words, w = i - c * words;
+      reinterpret_cast<uint32_t*>(r.p + c * r.chunk_stride + (long long)row.slot * r.row_stride)[w] = 0u;
+    }
+  }
+  for (long long i = tid; i < a.seq_row; i += nth) a.seq[row.slot * a.seq_row + i] = a.src_seq[row.src * a.seq_row + i];
+  for (long long i = tid; i < a.proj_row; i += nth) a.proj[row.slot * a.proj_row + i] = a.src_proj[row.src * a.proj_row + i];
+  for (long long i = tid; i < a.Tc; i += nth) a.chars[(long long)row.slot * a.Tc + i] = a.src_chars[(long long)row.src * a.Tc + i];
+  for (long long i = tid; i < (long long)row.cap * 2 * a.units; i += nth) {
+    const int u = (int)(i % a.units), l = (int)((i / a.units) & 1), pos = (int)(i / (2 * a.units));
+    uint8_t v;
+    if (row.dmask) {
+      v = row.dmask[i];
+    } else {
+      uint32_t o[4];
+      mb_philox4x32((uint32_t)u >> 2, (uint32_t)pos, (uint32_t)(2 + l), 0x72616767u, (uint32_t)row.seed, (uint32_t)(row.seed >> 32), o);
+      v = (uint8_t)((o[u & 3] >> 16) & 1u);
+    }
+    a.dmask[(((size_t)pos * 2 + l) * a.S + row.slot) * a.units + u] = v;
+  }
+  if (tid == 0) {
+    a.lens[row.slot] = row.len;
+    a.caps[row.slot] = row.cap;
+    a.done[row.slot] = -1;
+    a.starts[row.slot] = a.start;
+  }
 }
 
 }  // namespace
@@ -540,84 +632,90 @@ struct Ws {
   size_t total;  // bytes; every other field is an offset in floats
 };
 
-Ws ws_layout(const mb_tacotron_config& c, int B, int Tc, int steps, int r, bool ragged = false) {
+// What a workspace holds: the encoder's scratch, the decoder loop (its state, the encoder rows it reads, its per-step buffers), the
+// postnet's scratch.  generate uses all three in one workspace; a stream (mb_tacotron_stream_*) gives each its own, because the
+// encoder and the postnet run on their own streams while the decoder loop runs.  Fields of a part left out take no space.
+enum WsPart : int { WS_ENC = 1, WS_DEC = 2, WS_POST = 4, WS_ALL = 7 };
+
+Ws ws_layout(const mb_tacotron_config& c, int B, int Tc, int steps, int r, bool ragged = false, int parts = WS_ALL) {
   Ws L{};
   WsLayout W;
+  auto in = [&](int part, size_t n) { return (parts & part) ? n : (size_t)0; };
   const size_t Me = (size_t)B * Tc, Mp = (size_t)B * steps;
   const int E = c.encoder_dims, PD = c.postnet_dims, proj_dims = E + c.speaker_embedding_size + c.gst_E;
-  L.ids = W.take<float>(Me);
-  L.emb = W.take<float>(Me * c.embed_dims);
-  L.m_enc = W.take<float>((2 * Me * E + 3) / 4 + 64);  // uint8 masks
-  L.p1 = W.take<float>(Me * E);
-  L.x0 = W.take<float>(Me * E);
-  L.bank = W.take<float>(Me * c.encoder_K * E);
-  L.pool = W.take<float>(Me * c.encoder_K * E);
-  L.pj1 = W.take<float>(Me * E);
-  L.y = W.take<float>(Me * E);
-  L.hw12 = W.take<float>(Me * 2 * E);
-  L.gi_f = W.take<float>(Me * 3 * (E / 2));
-  L.gi_b = W.take<float>(Me * 3 * (E / 2));
-  L.gh = W.take<float>((size_t)2 * B * 3 * (PD / 2));
-  L.hst = W.take<float>((size_t)2 * B * (PD / 2));
-  L.seq = W.take<float>(Me * proj_dims);
-  L.proj = W.take<float>(Me * c.decoder_dims);
-  L.style_q = W.take<float>((size_t)B * c.gst_E);
-  L.style = W.take<float>((size_t)B * c.gst_E);
-  L.attn_h = W.take<float>((size_t)B * c.decoder_dims);
-  L.h1 = W.take<float>((size_t)B * c.lstm_dims);
-  L.c1 = W.take<float>((size_t)B * c.lstm_dims);
-  L.h2 = W.take<float>((size_t)B * c.lstm_dims);
-  L.c2 = W.take<float>((size_t)B * c.lstm_dims);
-  L.ctx = W.take<float>((size_t)B * proj_dims);
-  L.cum = W.take<float>(Me);
-  L.dp1 = W.take<float>((size_t)B * 2 * c.decoder_dims);
-  L.dp2 = W.take<float>((size_t)B * 2 * c.decoder_dims);
-  L.dgi = W.take<float>((size_t)B * 3 * c.decoder_dims);
-  L.dgh = W.take<float>((size_t)B * 3 * c.decoder_dims);
-  L.pq = W.take<float>((size_t)B * c.decoder_dims);
-  L.x = W.take<float>((size_t)B * c.lstm_dims);
-  L.gates = W.take<float>((size_t)B * 4 * c.lstm_dims);
+  L.ids = W.take<float>(in(WS_DEC, Me));  // int32 characters of the rows (streams; generate reads the caller's)
+  L.emb = W.take<float>(in(WS_ENC, Me * c.embed_dims));
+  L.m_enc = W.take<float>(in(WS_ENC, (2 * Me * E + 3) / 4 + 64));  // uint8 masks
+  L.p1 = W.take<float>(in(WS_ENC, Me * E));
+  L.x0 = W.take<float>(in(WS_ENC, Me * E));
+  L.bank = W.take<float>(in(WS_ENC, Me * c.encoder_K * E));
+  L.pool = W.take<float>(in(WS_ENC, Me * c.encoder_K * E));
+  L.pj1 = W.take<float>(in(WS_ENC, Me * E));
+  L.y = W.take<float>(in(WS_ENC, Me * E));
+  L.hw12 = W.take<float>(in(WS_ENC, Me * 2 * E));
+  L.gi_f = W.take<float>(in(WS_ENC, Me * 3 * (E / 2)));
+  L.gi_b = W.take<float>(in(WS_ENC, Me * 3 * (E / 2)));
+  L.gh = W.take<float>(in(WS_ENC | WS_POST, (size_t)2 * B * 3 * (PD / 2)));
+  L.hst = W.take<float>(in(WS_ENC | WS_POST, (size_t)2 * B * (PD / 2)));
+  L.seq = W.take<float>(in(WS_DEC, Me * proj_dims));
+  L.proj = W.take<float>(in(WS_DEC, Me * c.decoder_dims));
+  L.style_q = W.take<float>(in(WS_ENC, (size_t)B * c.gst_E));
+  L.style = W.take<float>(in(WS_ENC, (size_t)B * c.gst_E));
+  L.attn_h = W.take<float>(in(WS_DEC, (size_t)B * c.decoder_dims));
+  L.h1 = W.take<float>(in(WS_DEC, (size_t)B * c.lstm_dims));
+  L.c1 = W.take<float>(in(WS_DEC, (size_t)B * c.lstm_dims));
+  L.h2 = W.take<float>(in(WS_DEC, (size_t)B * c.lstm_dims));
+  L.c2 = W.take<float>(in(WS_DEC, (size_t)B * c.lstm_dims));
+  L.ctx = W.take<float>(in(WS_DEC, (size_t)B * proj_dims));
+  L.cum = W.take<float>(in(WS_DEC, Me));
+  L.dp1 = W.take<float>(in(WS_DEC, (size_t)B * 2 * c.decoder_dims));
+  L.dp2 = W.take<float>(in(WS_DEC, (size_t)B * 2 * c.decoder_dims));
+  L.dgi = W.take<float>(in(WS_DEC, (size_t)B * 3 * c.decoder_dims));
+  L.dgh = W.take<float>(in(WS_DEC, (size_t)B * 3 * c.decoder_dims));
+  L.pq = W.take<float>(in(WS_DEC, (size_t)B * c.decoder_dims));
+  L.x = W.take<float>(in(WS_DEC, (size_t)B * c.lstm_dims));
+  L.gates = W.take<float>(in(WS_DEC, (size_t)B * 4 * c.lstm_dims));
   L.a_hi = W.take<float>(tc_skinny_act_bytes(B > 128 ? 128 : B, 2 * c.lstm_dims) / 4);
   L.a_lo = W.take<float>(tc_skinny_act_bytes(B > 128 ? 128 : B, 2 * c.lstm_dims) / 4);
-  L.ah_hi = W.take<float>(2 * tc_skinny_act_bytes(B > 128 ? 128 : B, c.decoder_dims) / 4);  // attention-GRU state tiles, 2 parities
-  L.ah_lo = W.take<float>(2 * tc_skinny_act_bytes(B > 128 ? 128 : B, c.decoder_dims) / 4);
+  L.ah_hi = W.take<float>(in(WS_DEC, 2 * tc_skinny_act_bytes(B > 128 ? 128 : B, c.decoder_dims) / 4));  // attention-GRU state tiles, 2 parities
+  L.ah_lo = W.take<float>(in(WS_DEC, 2 * tc_skinny_act_bytes(B > 128 ? 128 : B, c.decoder_dims) / 4));
   {
     // operand tiles written by the producing kernels (fused act_split): P1 [ctx | prenet], P2 [ctx | attn_h], P3 / P4 [x | h] of the
     // two LSTMs (two step parities each), P5 [x]; hi and lo of each; zeroed with the attention-GRU tiles at the start of generate()
     const int Bc = B > 128 ? 128 : B;
     const FusedSplit f = fused_split_layout(Bc, proj_dims, c.decoder_dims, c.lstm_dims);
-    L.fsp = W.take<float>(f.total / 4);
+    L.fsp = W.take<float>(in(WS_DEC, f.total / 4));
   }
   // partial GEMM results computed a step early on the side stream: W_hh h of the two LSTMs, W_ih[:, ctx] ctx of the attention GRU
-  L.pre1 = W.take<float>((size_t)B * 4 * c.lstm_dims);
-  L.pre2 = W.take<float>((size_t)B * 4 * c.lstm_dims);
-  L.gic = W.take<float>((size_t)B * 3 * c.decoder_dims);
-  L.stopv = W.take<float>(B);
-  L.step = W.take<float>(64);
+  L.pre1 = W.take<float>(in(WS_DEC, (size_t)B * 4 * c.lstm_dims));
+  L.pre2 = W.take<float>(in(WS_DEC, (size_t)B * 4 * c.lstm_dims));
+  L.gic = W.take<float>(in(WS_DEC, (size_t)B * 3 * c.decoder_dims));
+  L.stopv = W.take<float>(in(WS_DEC, B));
+  L.step = W.take<float>(in(WS_DEC, 64));
   const int nst = (steps + r - 1) / r;
-  L.flags = W.take<float>(nst);
-  L.dmask = W.take<float>(((size_t)nst * 2 * B * 2 * c.decoder_dims + 3) / 4 + 64);  // PreNet dropout masks of every decoder step
-  L.mel_all = W.take<float>(Mp * c.n_mels + (size_t)r * c.n_mels);
-  L.scores_all = W.take<float>((size_t)B * nst * Tc);
-  L.pbank = W.take<float>(Mp * c.postnet_K * PD);
-  L.ppool = W.take<float>(Mp * c.postnet_K * PD);
-  L.ppj1 = W.take<float>(Mp * PD);
-  L.ppj2 = W.take<float>(Mp * c.n_mels);
-  L.py = W.take<float>(Mp * PD);
-  L.phw12 = W.take<float>(Mp * 2 * PD);
-  L.pgi_f = W.take<float>(Mp * 3 * (PD / 2));
-  L.pgi_b = W.take<float>(Mp * 3 * (PD / 2));
-  L.pgh = W.take<float>((size_t)2 * B * 3 * (PD / 2));
-  L.phst = W.take<float>((size_t)2 * B * (PD / 2));
-  L.pout = W.take<float>(Mp * PD);
-  L.lin = W.take<float>(Mp * c.n_mels);
+  L.flags = W.take<float>(in(WS_DEC, nst));
+  L.dmask = W.take<float>(in(WS_DEC, ((size_t)nst * 2 * B * 2 * c.decoder_dims + 3) / 4 + 64));  // PreNet dropout masks of every decoder step
+  L.mel_all = W.take<float>(in(WS_DEC, Mp * c.n_mels + (size_t)r * c.n_mels));
+  L.scores_all = W.take<float>(in(WS_DEC, (size_t)B * nst * Tc));
+  L.pbank = W.take<float>(in(WS_POST, Mp * c.postnet_K * PD));
+  L.ppool = W.take<float>(in(WS_POST, Mp * c.postnet_K * PD));
+  L.ppj1 = W.take<float>(in(WS_POST, Mp * PD));
+  L.ppj2 = W.take<float>(in(WS_POST, Mp * c.n_mels));
+  L.py = W.take<float>(in(WS_POST, Mp * PD));
+  L.phw12 = W.take<float>(in(WS_POST, Mp * 2 * PD));
+  L.pgi_f = W.take<float>(in(WS_POST, Mp * 3 * (PD / 2)));
+  L.pgi_b = W.take<float>(in(WS_POST, Mp * 3 * (PD / 2)));
+  L.pgh = W.take<float>(in(WS_POST, (size_t)2 * B * 3 * (PD / 2)));
+  L.phst = W.take<float>(in(WS_POST, (size_t)2 * B * (PD / 2)));
+  L.pout = W.take<float>(in(WS_POST, Mp * PD));
+  L.lin = W.take<float>(in(WS_POST, Mp * c.n_mels));
   {  // im2col operand planes of the large-M tensor-core GEMMs: the widest layer is conv_project1 (3 taps x K * ch)
-    const size_t enc = tc_big_act_bytes((int)Me, 3, c.encoder_K * E), post = tc_big_act_bytes((int)Mp, 3, c.postnet_K * PD);
+    const size_t enc = in(WS_ENC, tc_big_act_bytes((int)Me, 3, c.encoder_K * E)), post = in(WS_POST, tc_big_act_bytes((int)Mp, 3, c.postnet_K * PD));
     L.big_bytes = enc > post ? enc : post;
     L.big_hi = W.take<float>(L.big_bytes / 4);
     L.big_lo = W.take<float>(L.big_bytes / 4);
   }
-  if (ragged) L.rows = W.take<float>((size_t)6 * B);
+  if (ragged) L.rows = W.take<float>(in(WS_DEC, (size_t)6 * B));
   L.total = W.total();
   return L;
 }
@@ -1120,6 +1218,651 @@ struct RaggedRows {
   int32_t* frames;        // out: frames of each row
 };
 
+// the handle's internal streams and events (created at the first decoder loop)
+int ensure_streams(mb_tacotron* h) {
+  if (!h->own_stream) {
+    MB_CUDA_CHECK(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
+    MB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
+    MB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_out, cudaEventDisableTiming));
+    MB_CUDA_CHECK(cudaStreamCreateWithFlags(&h->side_stream, cudaStreamNonBlocking));
+    for (cudaEvent_t& e : h->ev_side) MB_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  }
+  return MB_OK;
+}
+
+// the mel projection's packed rows and tensor-core image for reduction factor r (re-packed when r changes)
+int prepare_mel_proj(mb_tacotron* h, int r, cudaStream_t st) {
+  const mb_tacotron_config& c = h->cfg;
+  const int NM = c.n_mels, LD = c.lstm_dims;
+  if (h->packed_r == r) return MB_OK;
+  const size_t n = (size_t)r * NM * LD;
+  pack_melproj_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(P(h, "decoder.mel_proj.weight"), P(h, "decoder.mel_proj.packed"),
+                                                                   NM, c.max_r, r, LD);
+  MB_LAUNCH_CHECK("pack_melproj_kernel");
+  int rc = tc_prepare(h, "decoder.mel_proj", P(h, "decoder.mel_proj.packed"), LD, nullptr, 0, nullptr, nullptr, r * NM, 0, st);
+  if (rc != MB_OK) return rc;
+  h->packed_r = r;
+  return MB_OK;
+}
+
+// the encoder (embedding, PreNet, CBHG), speaker and style columns and encoder_proj of B rows of Tc characters: seq [B][Tc][proj_dims]
+// and proj [B][Tc][decoder_dims].  Ragged rows (d_lens) take the routes whose arithmetic per row does not depend on the batch.
+int run_encoder(mb_tacotron* h, const Ws& L, float* ws, const int32_t* chars, const float* spk, int B, int Tc, int style_idx,
+                const uint8_t* enc_masks, uint64_t seed, bool ragged, const int* d_lens, const uint64_t* d_seeds, bool use_tc,
+                float* seq, float* proj, cudaStream_t st) {
+  const mb_tacotron_config& c = h->cfg;
+  const int E = c.encoder_dims, D = c.decoder_dims, LD = c.lstm_dims, SE = c.speaker_embedding_size, proj_dims = E + SE + c.gst_E;
+  const int Me = B * Tc;
+  BigWs bw;
+  bw.hi = ws + L.big_hi;
+  bw.lo = ws + L.big_lo;
+  bw.bytes = L.big_bytes;
+  TK(launch_embedding(chars, P(h, "encoder.embedding.weight"), ws + L.emb, Me, c.embed_dims, st));
+  uint8_t* em = reinterpret_cast<uint8_t*>(ws + L.m_enc);
+  const size_t enc_mask_n = (size_t)Me * E;
+  if (enc_masks) {
+    MB_CUDA_CHECK(cudaMemcpyAsync(em, enc_masks, 2 * enc_mask_n, cudaMemcpyDeviceToDevice, st));
+  } else if (ragged) {
+    fill_masks_seeded_kernel<<<(unsigned)((2 * enc_mask_n + 255) / 256), 256, 0, st>>>(em, B, Tc, E, d_seeds, 0);
+    MB_LAUNCH_CHECK("fill_masks_seeded_kernel");
+  } else {
+    fill_masks_kernel<<<(unsigned)((2 * enc_mask_n + 255) / 256), 256, 0, st>>>(em, 2 * enc_mask_n, seed, 0xffffffffu);
+    MB_LAUNCH_CHECK("fill_masks_kernel");
+  }
+  {
+    GemmArgs a = gemm1(ws + L.emb, c.embed_dims, c.embed_dims, P(h, "encoder.pre_net.fc1.weight"), c.embed_dims,
+                       P(h, "encoder.pre_net.fc1.bias"), Me, E, ws + L.p1, E, ACT_RELU);
+    a.mask = em;
+    a.fma_chain = ragged;
+    TK(launch_gemm(a, st));
+    GemmArgs b = gemm1(ws + L.p1, E, E, P(h, "encoder.pre_net.fc2.weight"), E, P(h, "encoder.pre_net.fc2.bias"), Me, E,
+                       ws + L.x0, E, ACT_RELU);
+    b.mask = em + enc_mask_n;
+    b.fma_chain = ragged;
+    TK(launch_gemm(b, st));
+  }
+  int rc = run_cbhg(h, "encoder.cbhg", c.encoder_K, E, E, E, E, c.num_highways, ws + L.x0, B, Tc, ws + L.bank, ws + L.pool,
+                    ws + L.pj1, ws + L.y, ws + L.hw12, ws + L.gi_f, ws + L.gi_b, ws + L.gh, ws + L.hst, seq, proj_dims, st,
+                    use_tc ? ws + L.a_hi : nullptr, use_tc ? ws + L.a_lo : nullptr, tc_skinny_act_bytes(B > 128 ? 128 : B, 2 * LD), bw,
+                    d_lens);
+  if (rc != MB_OK) return rc;
+  // speaker embedding per char (tacotron.py:236), style embedding (tacotron.py:238-253)
+  TK(launch_copy_cols(spk, SE, Tc, seq, proj_dims, E, Me, SE, st));
+  if (style_idx >= 0 && style_idx < c.gst_tokens) {
+    // zero query over a single token: softmax over one key == 1  ->  style = W_value tanh(embed[idx])
+    TK(launch_copy_cols(P(h, "gst.values") + (size_t)style_idx * c.gst_E, c.gst_E, Me, seq, proj_dims, E + SE, Me, c.gst_E, st));
+  } else {
+    GemmArgs a;
+    memset(&a, 0, sizeof(a));
+    a.nseg = 2;
+    a.seg[0] = {P(h, "gst.const_enc"), c.gst_E / 2, 0, 0, 0, 1};  // ld 0: the same row for every batch element
+    a.seg[1] = {spk, SE, SE, 0, c.gst_E / 2, 1};
+    a.W = P(h, "gst.stl.attention.W_query.weight");
+    a.ldw = c.gst_E / 2 + SE;
+    a.M = B;
+    a.N = c.gst_E;
+    a.T = 1;
+    a.Y = ws + L.style_q;
+    a.ldy = c.gst_E;
+    a.fma_chain = ragged;
+    TK(launch_gemm(a, st));
+    const int dk = c.gst_E / c.gst_heads;
+    gst_attention_kernel<<<B, 256, 0, st>>>(ws + L.style_q, P(h, "gst.keys"), P(h, "gst.values"), c.gst_tokens,
+                                            ws + L.style, c.gst_E, c.gst_heads, 1.0f / sqrtf((float)dk));
+    MB_LAUNCH_CHECK("gst_attention_kernel");
+    TK(launch_copy_cols(ws + L.style, c.gst_E, Tc, seq, proj_dims, E + SE, Me, c.gst_E, st));
+  }
+  {
+    GemmArgs a = gemm1(seq, proj_dims, proj_dims, P(h, "encoder_proj.weight"), proj_dims, nullptr, Me, D, proj, D);
+    a.fma_chain = ragged;
+    TK(launch_gemm(a, st));
+  }
+
+  return MB_OK;
+}
+
+// the postnet CBHG and post_proj over B rows of `frames` mel frames (melc [B][frames][n_mels]; ragged rows: d_flen) -> ws + L.lin
+int run_postnet(mb_tacotron* h, const Ws& L, float* ws, const float* melc, int B, int frames, const int* d_flen, bool use_tc,
+                cudaStream_t st) {
+  const mb_tacotron_config& c = h->cfg;
+  const int PD = c.postnet_dims, NM = c.n_mels, LD = c.lstm_dims;
+  BigWs bw;
+  bw.hi = ws + L.big_hi;
+  bw.lo = ws + L.big_lo;
+  bw.bytes = L.big_bytes;
+  int rc = run_cbhg(h, "postnet", c.postnet_K, NM, PD, PD, NM, c.num_highways, melc, B, frames, ws + L.pbank, ws + L.ppool,
+                ws + L.ppj1, ws + L.py, ws + L.phw12, ws + L.pgi_f, ws + L.pgi_b, ws + L.pgh, ws + L.phst, ws + L.pout, PD, st,
+                use_tc ? ws + L.a_hi : nullptr, use_tc ? ws + L.a_lo : nullptr, tc_skinny_act_bytes(B > 128 ? 128 : B, 2 * LD), bw,
+                d_flen);
+  if (rc != MB_OK) return rc;
+  {
+    GemmArgs a = gemm1(ws + L.pout, PD, PD, P(h, "post_proj.weight"), PD, nullptr, B * frames, NM, ws + L.lin, NM);
+    int rc2 = cbhg_gemm(h, "post_proj", a, st, bw, d_flen);
+    if (rc2 != MB_OK) return rc2;
+  }
+  return MB_OK;
+}
+
+// One decoder step of B rows (tacotron.py:71-138), launched on st (+ the side stream sd of the step DAG).  The step index is
+// (sp ? *sp : 0) + sj, resolved ON THE DEVICE by the few kernels that need it (PreNet input frame and dropout masks, alignment row,
+// mel output frames, stop rule), so the same launch sequence can be captured once into a CUDA graph and replayed for every group
+// of steps.  With a per-row step origin (d_start) each row reads and writes its per-step buffers (nst steps: alignment rows, mel
+// frames, masks) at its own step modulo nst.
+// Fused operand split (MB_TACO_SPLIT_FUSED, default 1): the five act_split launches of a step disappear - every kernel that
+// produces an input of a tensor-core GEMM (PreNet, context, attention GRU, rnn_input, the two LSTM cells) writes the fp16 hi / lo
+// operand chunks itself, into per-consumer tiles (the LSTM tiles ping-pong on the step parity: a cell writes h' for the next step
+// while other CTAs of the same launch still read this step's tiles).
+// Step DAG (MB_TACO_DAG, default 1, needs the fused split): a step's critical path is a chain of ~10 latency-bound kernels.  Three
+// of its GEMMs have a K segment that is known a whole step early - W_hh h_{t-1} of both LSTM cells and the context half of the
+// attention GRU's input projection - so those halves run on a side stream (TCS_PLAIN over a k-block range, result added to the
+// accumulator of the short main-path GEMM), and so does the stop projection / stop rule, which nothing in the next step needs.
+// The side stream forks from / joins the main one with events, inside the captured graph as well.
+struct DecoderLoop {
+  mb_tacotron* h;
+  Ws L;
+  float* ws;
+  int B, Tc, r, nst, steps_alloc;  // nst: steps the per-step buffers hold (steps_alloc = nst * r frames per row)
+  const int32_t* chars;
+  float* seq;
+  float* mel_all;
+  const uint8_t* dec_masks;  // injected masks [nst][2][B][2D], else dm (drawn before the loop / written at admission)
+  uint8_t* dm;
+  float min_stop_token;
+  int* flags;                // [nst] stop flags of the padded / ragged loop, or null (per-row step origin)
+  const int* d_lens;         // ragged rows: characters, caps, done steps; or null
+  const int* d_caps;
+  int* d_done;
+  const int* d_start;        // per-row step origin, or null
+  bool use_tc;
+  // derived by init()
+  int NM, D, LD, proj_dims, f_rows_pad;
+  size_t dmask_n, lsa_smem;
+  bool prenet_fused_env, fsplit, dag;
+  FusedSplit fs;
+  char* fbase;
+  cudaStream_t st, sd;
+  bool have_gic = false, have_p1 = false, have_p2 = false, have_stop = false, side_open = false;
+
+  void init(cudaStream_t main_stream) {
+    const mb_tacotron_config& c = h->cfg;
+    NM = c.n_mels;
+    D = c.decoder_dims;
+    LD = c.lstm_dims;
+    proj_dims = c.encoder_dims + c.speaker_embedding_size + c.gst_E;
+    dmask_n = (size_t)B * 2 * D;
+    lsa_smem = lsa_step_smem_bytes(Tc);
+    static const bool split_fused_env = [] {
+      const char* e = getenv("MB_TACO_SPLIT_FUSED");
+      return e ? atoi(e) != 0 : true;
+    }();
+    static const bool prenet_env = [] {
+      const char* e = getenv("MB_TACO_PRENET_FUSED");
+      return e ? atoi(e) != 0 : true;
+    }();
+    prenet_fused_env = prenet_env;
+    fsplit = split_fused_env && prenet_fused_env && use_tc && D % 64 == 0 && proj_dims % 256 == 0 && LD % 64 == 0 &&
+             (r * NM) % 4 == 0 && NM <= 128 && 2 * D <= 256 && B <= 128;
+    fs = fused_split_layout(B > 128 ? 128 : B, proj_dims, D, LD);
+    fbase = reinterpret_cast<char*>(ws + L.fsp);
+    f_rows_pad = B <= 64 ? 64 : 128;
+    static const bool dag_env = [] {
+      const char* e = getenv("MB_TACO_DAG");
+      return e ? atoi(e) != 0 : true;
+    }();
+    dag = dag_env && fsplit && proj_dims % 64 == 0;
+    st = main_stream;
+    sd = h->side_stream;
+  }
+  __half* fhi(size_t off) const { return reinterpret_cast<__half*>(fbase + off); }
+  // fork: side stream waits for everything enqueued on the main stream so far
+  int side_after_main(cudaEvent_t ev) {
+    MB_CUDA_CHECK(cudaEventRecord(ev, st));
+    MB_CUDA_CHECK(cudaStreamWaitEvent(sd, ev, 0));
+    side_open = true;
+    return MB_OK;
+  }
+  int main_after_side(cudaEvent_t ev) {
+    MB_CUDA_CHECK(cudaEventRecord(ev, sd));
+    MB_CUDA_CHECK(cudaStreamWaitEvent(st, ev, 0));
+    return MB_OK;
+  }
+  // join everything outstanding on the side stream (end of a captured group / of a directly launched step)
+  int join_side() {
+    if (side_open) {
+      int rcj = main_after_side(h->ev_side[7]);
+      if (rcj != MB_OK) return rcj;
+    }
+    side_open = have_gic = have_p1 = have_p2 = have_stop = false;
+    return MB_OK;
+  }
+  int emit_step(const int* sp, int sj);
+};
+
+int DecoderLoop::emit_step(const int* sp, int sj) {
+  // PreNet on the last frame of the previous step (go frame = zeros)
+  const uint8_t* m1;
+  const uint8_t* m2;
+  long long mstep = 0;
+  if (dec_masks) {
+    m1 = dec_masks;
+    m2 = m1 + dmask_n;
+    mstep = (long long)(2 * dmask_n);
+  } else {  // generated for all steps before the loop (fill_masks_steps_kernel)
+    m1 = dm;
+    m2 = dm + dmask_n;
+    mstep = (long long)(2 * dmask_n);
+  }
+  const bool prenet_fused = prenet_fused_env;  // A/B switch MB_TACO_PRENET_FUSED: 0 = two skinny GEMM launches (round 1)
+  const int par = sj & 1;  // graph groups start at even steps, so the parity of (base + sj) is that of sj
+  if (prenet_fused && NM <= 128 && 2 * D <= 256) {
+    // both PreNet layers in one launch; frame (step * r - 1) of every utterance, step 0 = the all-zero go frame
+    PrenetArgs pa;
+    memset(&pa, 0, sizeof(pa));
+    pa.x = mel_all - NM;
+    pa.x_ld = (long long)steps_alloc * NM;
+    pa.x_step = (long long)r * NM;
+    pa.x_first = mel_all + (size_t)B * steps_alloc * NM;
+    pa.W1 = P(h, "decoder.prenet.fc1.weight");
+    pa.b1 = P(h, "decoder.prenet.fc1.bias");
+    pa.W2 = P(h, "decoder.prenet.fc2.weight");
+    pa.b2 = P(h, "decoder.prenet.fc2.bias");
+    pa.m1 = m1;
+    pa.m2 = m2;
+    pa.mask_step = mstep;
+    pa.step_ptr = sp;
+    pa.step_j = sj;
+    pa.row_start = d_start;
+    pa.ring = nst;
+    pa.B = B;
+    pa.K = NM;
+    pa.H = 2 * D;
+    pa.y = ws + L.dp2;
+    pa.ldy = 2 * D;
+    if (fsplit) {  // [ctx | prenet] tiles of the attention GRU's input GEMM
+      pa.s_hi = fhi(fs.p1);
+      pa.s_lo = fhi(fs.p1 + fs.b1);
+      pa.s_k0 = proj_dims;
+      pa.s_rows_pad = f_rows_pad;
+    }
+    TK(launch_prenet_fused(pa, st));
+  } else {
+    // frame (step * r - 1) of every utterance; step 0 reads the zero block behind mel_all with row stride 0
+    GemmArgs a = gemm1(mel_all - NM, NM, steps_alloc * NM, P(h, "decoder.prenet.fc1.weight"), NM,
+                       P(h, "decoder.prenet.fc1.bias"), B, 2 * D, ws + L.dp1, 2 * D, ACT_RELU);
+    a.mask = m1;
+    a.step_mode = 1;
+    a.step_ptr = sp;
+    a.step_j = sj;
+    a.x_step = (long long)r * NM;
+    a.x_first = mel_all + (size_t)B * steps_alloc * NM;
+    a.mask_step = mstep;
+    TK(launch_gemm(a, st));
+    GemmArgs b = gemm1(ws + L.dp1, 2 * D, 2 * D, P(h, "decoder.prenet.fc2.weight"), 2 * D, P(h, "decoder.prenet.fc2.bias"),
+                       B, 2 * D, ws + L.dp2, 2 * D, ACT_RELU);
+    b.mask = m2;
+    b.step_mode = 1;
+    b.step_ptr = sp;
+    b.step_j = sj;
+    b.mask_step = mstep;
+    TK(launch_gemm(b, st));
+  }
+  if (use_tc && D % 64 == 0) {  // attention GRU on [context, prenet]: input projection + recurrent step on tensor cores
+    __half* a_hi = reinterpret_cast<__half*>(ws + L.a_hi);
+    __half* a_lo = reinterpret_cast<__half*>(ws + L.a_lo);
+    if (fsplit) {
+      a_hi = fhi(fs.p1);
+      a_lo = fhi(fs.p1 + fs.b1);
+    } else {
+      TK(launch_act_split(ws + L.ctx, proj_dims, proj_dims, ws + L.dp2, 2 * D, 2 * D, B, a_hi, a_lo, st));
+    }
+    TcSkinnyArgs ta;
+    memset(&ta, 0, sizeof(ta));
+    ta.a_hi = a_hi;
+    ta.a_lo = a_lo;
+    ta.w = reinterpret_cast<const __half*>(P(h, "decoder.attn_rnn.ih.tcw"));
+    ta.bias = P(h, "decoder.attn_rnn.ih.tcb");
+    ta.KB = (proj_dims + 2 * D + 63) / 64;
+    if (dag) {  // the context half was multiplied on the side stream after the previous step's attention (zero at step 0)
+      if (have_gic) {
+        MB_CUDA_CHECK(cudaStreamWaitEvent(st, h->ev_side[1], 0));
+        have_gic = false;
+      }
+      ta.KBw = ta.KB;
+      ta.kb0 = proj_dims / 64;
+      ta.KB = ta.KBw - ta.kb0;
+      ta.pre = ws + L.gic;
+      ta.ldpre = 3 * D;
+    }
+    ta.M = B;
+    ta.N = 3 * D;
+    ta.mode = TCS_PLAIN;
+    ta.inv_scale = h->tc_inv_scale["decoder.attn_rnn.ih"];
+    ta.y = ws + L.dgi;
+    ta.ldy = 3 * D;
+    TK(launch_tc_skinny(ta, st));
+    const size_t tb = tc_skinny_act_bytes(B, D);
+    TcGruArgs g;
+    memset(&g, 0, sizeof(g));
+    if (fsplit) {  // attn_h is the trailing K segment of rnn_input's [ctx | attn_h] tiles
+      g.s_hi = fhi(fs.p2);
+      g.s_lo = fhi(fs.p2 + fs.b2);
+      g.s_k0 = proj_dims;
+    }
+    g.a_hi[0] = reinterpret_cast<const __half*>(reinterpret_cast<const char*>(ws + L.ah_hi) + par * tb);
+    g.a_lo[0] = reinterpret_cast<const __half*>(reinterpret_cast<const char*>(ws + L.ah_lo) + par * tb);
+    g.nxt_hi[0] = reinterpret_cast<__half*>(reinterpret_cast<char*>(ws + L.ah_hi) + (par ^ 1) * tb);
+    g.nxt_lo[0] = reinterpret_cast<__half*>(reinterpret_cast<char*>(ws + L.ah_lo) + (par ^ 1) * tb);
+    g.w[0] = reinterpret_cast<const __half*>(P(h, "decoder.attn_rnn.hh.tcw"));
+    g.bias[0] = P(h, "decoder.attn_rnn.hh.tcb");
+    g.gi[0] = ws + L.dgi;
+    g.h[0] = ws + L.attn_h;
+    g.out[0] = ws + L.attn_h;
+    g.inv_scale[0] = h->tc_inv_scale["decoder.attn_rnn.hh"];
+    g.ldgi = 3 * D;
+    g.ldout = D;
+    g.KB = D / 64;
+    g.M = B;
+    g.H = D;
+    g.ndir = 1;
+    TK(launch_tc_gru(g, st));
+  } else {  // attention GRU on [context, prenet]
+    GemmArgs a;
+    memset(&a, 0, sizeof(a));
+    a.nseg = 2;
+    a.seg[0] = {ws + L.ctx, proj_dims, proj_dims, 0, 0, 1};
+    a.seg[1] = {ws + L.dp2, 2 * D, 2 * D, 0, proj_dims, 1};
+    a.W = P(h, "decoder.attn_rnn.weight_ih");
+    a.ldw = proj_dims + 2 * D;
+    a.bias = P(h, "decoder.attn_rnn.bias_ih");
+    a.M = B;
+    a.N = 3 * D;
+    a.T = 1;
+    a.Y = ws + L.dgi;
+    a.ldy = 3 * D;
+    TK(launch_gemm(a, st));
+    GemmArgs b = gemm1(ws + L.attn_h, D, D, P(h, "decoder.attn_rnn.weight_hh"), D, P(h, "decoder.attn_rnn.bias_hh"), B, 3 * D,
+                       ws + L.dgh, 3 * D);
+    TK(launch_gemm(b, st));
+    TK(launch_gru_cell(ws + L.dgi, 3 * D, ws + L.dgh, ws + L.attn_h, D, nullptr, 0, B, D, st));
+  }
+  {  // location sensitive attention + context
+    // MB_TACO_LSA_FUSED (default 1): 512 threads per batch row (4 time-step groups in the energy phase) and the query
+    // projection W q + b inside the kernel; 0 = round-2 shape (256 threads, separate GEMM launch)
+    static const bool lsa_fused = [] {
+      const char* e = getenv("MB_TACO_LSA_FUSED");
+      return e ? atoi(e) != 0 : true;
+    }();
+    const bool qf = lsa_fused && D == ATT_D;
+    if (!qf) {
+      GemmArgs a = gemm1(ws + L.attn_h, D, D, P(h, "decoder.attn_net.W.weight"), D, P(h, "decoder.attn_net.W.bias"), B, D,
+                         ws + L.pq, D);
+      TK(launch_gemm(a, st));
+    }
+    MB_CUDA_CHECK(launch_pdl2(lsa_step_kernel, dim3(B), dim3(lsa_fused ? 512 : 256), lsa_smem, st, ws + L.pq, ws + L.proj, seq,
+                              proj_dims, chars, ws + L.cum, P(h, "decoder.attn_net.conv.weight"),
+                              P(h, "decoder.attn_net.conv.bias"), P(h, "decoder.attn_net.L.weight"),
+                              P(h, "decoder.attn_net.v.weight"), ws + L.scores_all, nst * Tc,
+                              (proj_dims % 256 == 0) ? nullptr : ws + L.ctx, Tc, sp, sj, qf ? ws + L.attn_h : nullptr,
+                              P(h, "decoder.attn_net.W.weight"), P(h, "decoder.attn_net.W.bias"), d_lens, d_start, nst));
+    MB_LAUNCH_CHECK("lsa_step_kernel");
+    if (proj_dims % 256 == 0) {
+      if (have_stop) {  // the previous step's stop projection (side stream) still reads ctx and x, which are rewritten from here on
+        MB_CUDA_CHECK(cudaStreamWaitEvent(st, h->ev_side[6], 0));
+        have_stop = false;
+      }
+      MB_CUDA_CHECK(launch_pdl2(lsa_ctx_kernel, dim3(proj_dims / 256, B), dim3(256), sizeof(float) * Tc, st, ws + L.scores_all,
+                                nst * Tc, seq, proj_dims, Tc, ws + L.ctx, sp, sj, fsplit ? fhi(fs.p1) : nullptr,
+                                fsplit ? fhi(fs.p1 + fs.b1) : nullptr, fsplit ? fhi(fs.p2) : nullptr,
+                                fsplit ? fhi(fs.p2 + fs.b2) : nullptr, f_rows_pad, d_lens, d_start, nst));
+      MB_LAUNCH_CHECK("lsa_ctx_kernel");
+    }
+    if (dag) {  // side stream: context half of the NEXT step's attention-GRU input projection
+      int rcs = side_after_main(h->ev_side[0]);
+      if (rcs != MB_OK) return rcs;
+      TcSkinnyArgs tp;
+      memset(&tp, 0, sizeof(tp));
+      tp.a_hi = fhi(fs.p1);
+      tp.a_lo = fhi(fs.p1 + fs.b1);
+      tp.w = reinterpret_cast<const __half*>(P(h, "decoder.attn_rnn.ih.tcw"));
+      tp.KBw = (proj_dims + 2 * D + 63) / 64;
+      tp.kb0 = 0;
+      tp.KB = proj_dims / 64;
+      tp.M = B;
+      tp.N = 3 * D;
+      tp.mode = TCS_PLAIN;
+      tp.inv_scale = h->tc_inv_scale["decoder.attn_rnn.ih"];
+      tp.y = ws + L.gic;
+      tp.ldy = 3 * D;
+      TK(launch_tc_skinny(tp, sd));
+      MB_CUDA_CHECK(cudaEventRecord(h->ev_side[1], sd));
+      have_gic = true;
+    }
+  }
+  if (use_tc) {  // rnn_input on [context, attn_hidden] (tensor cores)
+    __half* a_hi = reinterpret_cast<__half*>(ws + L.a_hi);
+    __half* a_lo = reinterpret_cast<__half*>(ws + L.a_lo);
+    if (fsplit) {
+      a_hi = fhi(fs.p2);
+      a_lo = fhi(fs.p2 + fs.b2);
+    } else {
+      TK(launch_act_split(ws + L.ctx, proj_dims, proj_dims, ws + L.attn_h, D, D, B, a_hi, a_lo, st));
+    }
+    TcSkinnyArgs ta;
+    memset(&ta, 0, sizeof(ta));
+    ta.a_hi = a_hi;
+    ta.a_lo = a_lo;
+    if (fsplit) {  // x is the leading K segment of the first LSTM's [x | h1] tiles of this step
+      ta.s_hi[0] = fhi(fs.p3[par]);
+      ta.s_lo[0] = fhi(fs.p3[par] + fs.b3);
+      ta.s_k0[0] = 0;
+    }
+    ta.w = reinterpret_cast<const __half*>(P(h, "decoder.rnn_input.tcw"));
+    ta.bias = P(h, "decoder.rnn_input.tcb");
+    ta.KB = (proj_dims + D + 63) / 64;
+    ta.M = B;
+    ta.N = LD;
+    ta.mode = TCS_PLAIN;
+    ta.inv_scale = h->tc_inv_scale["decoder.rnn_input"];
+    ta.y = ws + L.x;
+    ta.ldy = LD;
+    TK(launch_tc_skinny(ta, st));
+  } else {  // rnn_input on [context, attn_hidden]
+    GemmArgs a;
+    memset(&a, 0, sizeof(a));
+    a.nseg = 2;
+    a.seg[0] = {ws + L.ctx, proj_dims, proj_dims, 0, 0, 1};
+    a.seg[1] = {ws + L.attn_h, D, D, 0, proj_dims, 1};
+    a.W = P(h, "decoder.rnn_input.weight");
+    a.ldw = proj_dims + D;
+    a.bias = P(h, "decoder.rnn_input.bias");
+    a.M = B;
+    a.N = LD;
+    a.T = 1;
+    a.Y = ws + L.x;
+    a.ldy = LD;
+    TK(launch_gemm(a, st));
+  }
+  for (int l = 0; l < 2; ++l) {  // residual LSTMs
+    const std::string n = l == 0 ? "decoder.res_rnn1" : "decoder.res_rnn2";
+    float* hh = ws + (l == 0 ? L.h1 : L.h2);
+    float* cc = ws + (l == 0 ? L.c1 : L.c2);
+    if (use_tc) {
+      // gates GEMM on the tensor cores (3-term fp16 split, FP32 accumulate) with the cell update fused
+      __half* a_hi = reinterpret_cast<__half*>(ws + L.a_hi);
+      __half* a_lo = reinterpret_cast<__half*>(ws + L.a_lo);
+      TcSkinnyArgs ta;
+      memset(&ta, 0, sizeof(ta));
+      if (fsplit) {
+        // this step's [x | h] tiles; x' (residual stream) goes to the next consumer's tiles, h' to this cell's tiles of the
+        // NEXT step (other parity)
+        const size_t* mine = l == 0 ? fs.p3 : fs.p4;
+        a_hi = fhi(mine[par]);
+        a_lo = fhi(mine[par] + fs.b3);
+        ta.s_hi[1] = fhi(mine[par ^ 1]);
+        ta.s_lo[1] = fhi(mine[par ^ 1] + fs.b3);
+        ta.s_k0[1] = LD;
+        ta.s_hi[0] = l == 0 ? fhi(fs.p4[par]) : fhi(fs.p5);
+        ta.s_lo[0] = l == 0 ? fhi(fs.p4[par] + fs.b3) : fhi(fs.p5 + fs.b5);
+        ta.s_k0[0] = 0;
+      } else {
+        TK(launch_act_split(ws + L.x, LD, LD, hh, LD, LD, B, a_hi, a_lo, st));
+      }
+      ta.a_hi = a_hi;
+      ta.a_lo = a_lo;
+      ta.w = reinterpret_cast<const __half*>(P(h, n + ".tcw"));
+      ta.bias = P(h, n + ".tcb");
+      ta.KB = 2 * LD / 64;
+      if (dag) {  // W_hh h_{t-1} was multiplied on the side stream right after the previous step's cell (zero at step 0)
+        bool& have = l == 0 ? have_p1 : have_p2;
+        if (have) {
+          MB_CUDA_CHECK(cudaStreamWaitEvent(st, h->ev_side[l == 0 ? 3 : 5], 0));
+          have = false;
+        }
+        ta.KBw = ta.KB;
+        ta.kb0 = 0;
+        ta.KB = LD / 64;
+        ta.pre = ws + (l == 0 ? L.pre1 : L.pre2);
+        ta.ldpre = 4 * LD;
+      }
+      ta.M = B;
+      ta.N = 4 * LD;
+      ta.mode = TCS_LSTM;
+      ta.inv_scale = h->tc_inv_scale[n];
+      ta.c = cc;
+      ta.h = hh;
+      ta.x = ws + L.x;
+      ta.H = LD;
+      TK(launch_tc_skinny(ta, st));
+      if (dag) {  // side stream: W_hh h_t for the next step, from the h tiles this launch just wrote (other parity)
+        int rcs = side_after_main(h->ev_side[l == 0 ? 2 : 4]);
+        if (rcs != MB_OK) return rcs;
+        const size_t* mine = l == 0 ? fs.p3 : fs.p4;
+        TcSkinnyArgs tp;
+        memset(&tp, 0, sizeof(tp));
+        tp.a_hi = fhi(mine[par ^ 1]);
+        tp.a_lo = fhi(mine[par ^ 1] + fs.b3);
+        tp.w = reinterpret_cast<const __half*>(P(h, n + ".tcw"));
+        tp.KBw = 2 * LD / 64;
+        tp.kb0 = LD / 64;
+        tp.KB = LD / 64;
+        tp.M = B;
+        tp.N = 4 * LD;
+        tp.mode = TCS_PLAIN;
+        tp.inv_scale = h->tc_inv_scale[n];
+        tp.y = ws + (l == 0 ? L.pre1 : L.pre2);
+        tp.ldy = 4 * LD;
+        TK(launch_tc_skinny(tp, sd));
+        MB_CUDA_CHECK(cudaEventRecord(h->ev_side[l == 0 ? 3 : 5], sd));
+        (l == 0 ? have_p1 : have_p2) = true;
+      }
+      continue;
+    }
+    GemmArgs a;
+    memset(&a, 0, sizeof(a));
+    // gates = linear_hh(h) + linear_ih(x): two GEMMs chained through the residual input of the second
+    GemmArgs g1 = gemm1(hh, LD, LD, P(h, n + ".weight_hh"), LD, P(h, n + ".bias_hh"), B, 4 * LD, ws + L.gates, 4 * LD);
+    TK(launch_gemm(g1, st));
+    GemmArgs g2 = gemm1(ws + L.x, LD, LD, P(h, n + ".weight_ih"), LD, P(h, n + ".bias_ih"), B, 4 * LD, ws + L.gates, 4 * LD);
+    g2.res = ws + L.gates;
+    g2.ldres = 4 * LD;
+    TK(launch_gemm(g2, st));
+    TK(launch_lstm_cell(ws + L.gates, cc, hh, ws + L.x, B, LD, st));
+  }
+  {  // mel frames of this step, written straight into mel_all[b][t..t+r)[:]
+    if (use_tc && (r * NM) % 4 == 0) {
+      __half* a_hi = reinterpret_cast<__half*>(ws + L.a_hi);
+      __half* a_lo = reinterpret_cast<__half*>(ws + L.a_lo);
+      if (fsplit) {
+        a_hi = fhi(fs.p5);
+        a_lo = fhi(fs.p5 + fs.b5);
+      } else {
+        TK(launch_act_split(ws + L.x, LD, LD, nullptr, 0, 0, B, a_hi, a_lo, st));
+      }
+      TcSkinnyArgs ta;
+      memset(&ta, 0, sizeof(ta));
+      ta.a_hi = a_hi;
+      ta.a_lo = a_lo;
+      ta.w = reinterpret_cast<const __half*>(P(h, "decoder.mel_proj.tcw"));
+      ta.bias = nullptr;
+      ta.KB = LD / 64;
+      ta.M = B;
+      ta.N = r * NM;
+      ta.mode = TCS_PLAIN;
+      ta.inv_scale = h->tc_inv_scale["decoder.mel_proj"];
+      ta.y = mel_all;
+      ta.ldy = steps_alloc * NM;
+      ta.step_ptr = sp;
+      ta.step_j = sj;
+      ta.y_step = (long long)r * NM;
+      ta.row_start = d_start;
+      ta.ring = nst;
+      TK(launch_tc_skinny(ta, st));
+    } else {
+      if (sp) return fail(MB_ERR_STATE, "mb_tacotron_generate: graph replay needs the tensor-core mel projection");
+      GemmArgs a = gemm1(ws + L.x, LD, LD, P(h, "decoder.mel_proj.packed"), LD, nullptr, B, r * NM,
+                         mel_all + (size_t)sj * r * NM, steps_alloc * NM);
+      TK(launch_gemm(a, st));
+    }
+    GemmArgs s;
+    memset(&s, 0, sizeof(s));
+    s.nseg = 2;
+    s.seg[0] = {ws + L.x, LD, LD, 0, 0, 1};
+    s.seg[1] = {ws + L.ctx, proj_dims, proj_dims, 0, LD, 1};
+    s.W = P(h, "decoder.stop_proj.weight");
+    s.ldw = LD + proj_dims;
+    s.bias = P(h, "decoder.stop_proj.bias");
+    s.M = B;
+    s.N = 1;
+    s.T = 1;
+    s.act = ACT_SIGMOID;
+    s.Y = ws + L.stopv;
+    s.ldy = 1;
+    static const bool stop_fused = [] {
+      const char* e = getenv("MB_TACO_STOP_FUSED");  // 0 = stop projection and stop rule as two launches (round 2)
+      return e ? atoi(e) != 0 : true;
+    }();
+    if (stop_fused) {
+      // the CTA that finishes last applies the stop rule (ticket counter behind the step counter, reset by that CTA).
+      // With the step DAG it runs on the side stream (after the second LSTM's fork): the next step does not need it.
+      stop_step_kernel<<<B, 256, 0, dag ? sd : st>>>(s, B, min_stop_token, r, flags, sp, sj,
+                                                     reinterpret_cast<unsigned int*>(ws + L.step) + 16, d_done, d_caps,
+                                                     d_start);
+      MB_LAUNCH_CHECK("stop_step_kernel");
+      if (dag) {
+        MB_CUDA_CHECK(cudaEventRecord(h->ev_side[6], sd));
+        have_stop = true;
+      }
+    } else {
+      TK(launch_gemm(s, st));
+      stop_flag_kernel<<<1, 32, 0, st>>>(ws + L.stopv, B, min_stop_token, r, flags, sp, sj, d_done, d_caps, d_start);
+      MB_LAUNCH_CHECK("stop_flag_kernel");
+    }
+  }
+  return MB_OK;
+}
+
+// Groups of kGraphSteps decoder steps are captured once and replayed (the loop is launch-bound: ~20 kernels of a few
+// microseconds per step); MB_TACO_GRAPH=0 or a capture failure falls back to direct launches.  The group ends by advancing the
+// device step counter.  false (error cleared): no graph.
+constexpr int kGraphSteps = 8;
+bool capture_group(DecoderLoop& dl, int* step_dev, cudaGraph_t* graph, cudaGraphExec_t* exec, int* per_graph) {
+  cudaStream_t st = dl.st;
+  const uint64_t launches_before = mb_launch_count();
+  bool ok = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
+  int rc_cap = MB_OK;
+  if (ok) {
+    for (int j = 0; j < kGraphSteps && rc_cap == MB_OK; ++j) rc_cap = dl.emit_step(step_dev, j);
+    if (rc_cap == MB_OK) rc_cap = dl.join_side();
+    if (rc_cap == MB_OK) step_advance_kernel<<<1, 32, 0, st>>>(step_dev, kGraphSteps);
+    ok = cudaStreamEndCapture(st, graph) == cudaSuccess && rc_cap == MB_OK && *graph != nullptr;
+  }
+  if (ok) ok = cudaGraphInstantiate(exec, *graph, 0) == cudaSuccess;
+  *per_graph = (int)(mb_launch_count() - launches_before);
+  count_launch(-*per_graph);  // captured, not launched; every replay counts them
+  if (!ok) cudaGetLastError();
+  return ok;
+}
+
 // Tacotron.generate of one padded batch (rg == nullptr) or of B ragged rows, each computed as that utterance alone (rg)
 int generate_impl(mb_tacotron* h, const int32_t* chars, const float* spk, int32_t B, int32_t Tc, int32_t steps,
                   int32_t r, int32_t style_idx, float min_stop_token, const uint8_t* enc_masks,
@@ -1140,13 +1883,7 @@ int generate_impl(mb_tacotron* h, const int32_t* chars, const float* spk, int32_
   float* ws;
   if (int rc = bind("mb_tacotron_generate", workspace, workspace_bytes, L.total, &ws)) return rc;
   cudaStream_t caller = (cudaStream_t)stream;
-  if (!h->own_stream) {
-    MB_CUDA_CHECK(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
-    MB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
-    MB_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_out, cudaEventDisableTiming));
-    MB_CUDA_CHECK(cudaStreamCreateWithFlags(&h->side_stream, cudaStreamNonBlocking));
-    for (cudaEvent_t& e : h->ev_side) MB_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  }
+  if (int rc = ensure_streams(h)) return rc;
   cudaStream_t st = h->own_stream;
   MB_CUDA_CHECK(cudaEventRecord(h->ev_in, caller));
   MB_CUDA_CHECK(cudaStreamWaitEvent(st, h->ev_in, 0));
@@ -1187,78 +1924,11 @@ int generate_impl(mb_tacotron* h, const int32_t* chars, const float* spk, int32_
     d_seeds = reinterpret_cast<const uint64_t*>(base + 4 * B);
   }
 
-  if (h->packed_r != r) {
-    const size_t n = (size_t)r * NM * LD;
-    pack_melproj_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(P(h, "decoder.mel_proj.weight"),
-                                                                     P(h, "decoder.mel_proj.packed"), NM, c.max_r, r, LD);
-    MB_LAUNCH_CHECK("pack_melproj_kernel");
-    int rc = tc_prepare(h, "decoder.mel_proj", P(h, "decoder.mel_proj.packed"), LD, nullptr, 0, nullptr, nullptr, r * NM, 0, st);
-    if (rc != MB_OK) return rc;
-    h->packed_r = r;
-  }
+  if (int rc = prepare_mel_proj(h, r, st)) return rc;
 
-  // ------------------------------------------------------------------ encoder (tacotron.py:31-44)
-  TK(launch_embedding(chars, P(h, "encoder.embedding.weight"), ws + L.emb, Me, c.embed_dims, st));
-  uint8_t* em = reinterpret_cast<uint8_t*>(ws + L.m_enc);
-  const size_t enc_mask_n = (size_t)Me * E;
-  if (enc_masks) {
-    MB_CUDA_CHECK(cudaMemcpyAsync(em, enc_masks, 2 * enc_mask_n, cudaMemcpyDeviceToDevice, st));
-  } else if (rg) {
-    fill_masks_seeded_kernel<<<(unsigned)((2 * enc_mask_n + 255) / 256), 256, 0, st>>>(em, B, Tc, E, d_seeds, 0);
-    MB_LAUNCH_CHECK("fill_masks_seeded_kernel");
-  } else {
-    fill_masks_kernel<<<(unsigned)((2 * enc_mask_n + 255) / 256), 256, 0, st>>>(em, 2 * enc_mask_n, seed, 0xffffffffu);
-    MB_LAUNCH_CHECK("fill_masks_kernel");
-  }
-  {
-    GemmArgs a = gemm1(ws + L.emb, c.embed_dims, c.embed_dims, P(h, "encoder.pre_net.fc1.weight"), c.embed_dims,
-                       P(h, "encoder.pre_net.fc1.bias"), Me, E, ws + L.p1, E, ACT_RELU);
-    a.mask = em;
-    a.fma_chain = rg != nullptr;
-    TK(launch_gemm(a, st));
-    GemmArgs b = gemm1(ws + L.p1, E, E, P(h, "encoder.pre_net.fc2.weight"), E, P(h, "encoder.pre_net.fc2.bias"), Me, E,
-                       ws + L.x0, E, ACT_RELU);
-    b.mask = em + enc_mask_n;
-    b.fma_chain = rg != nullptr;
-    TK(launch_gemm(b, st));
-  }
   float* seq = ws + L.seq;
-  int rc = run_cbhg(h, "encoder.cbhg", c.encoder_K, E, E, E, E, c.num_highways, ws + L.x0, B, Tc, ws + L.bank, ws + L.pool,
-                    ws + L.pj1, ws + L.y, ws + L.hw12, ws + L.gi_f, ws + L.gi_b, ws + L.gh, ws + L.hst, seq, proj_dims, st,
-                    use_tc ? ws + L.a_hi : nullptr, use_tc ? ws + L.a_lo : nullptr, tc_skinny_act_bytes(B > 128 ? 128 : B, 2 * LD), bw,
-                    d_lens);
+  int rc = run_encoder(h, L, ws, chars, spk, B, Tc, style_idx, enc_masks, seed, rg != nullptr, d_lens, d_seeds, use_tc, seq, ws + L.proj, st);
   if (rc != MB_OK) return rc;
-  // speaker embedding per char (tacotron.py:236), style embedding (tacotron.py:238-253)
-  TK(launch_copy_cols(spk, SE, Tc, seq, proj_dims, E, Me, SE, st));
-  if (style_idx >= 0 && style_idx < c.gst_tokens) {
-    // zero query over a single token: softmax over one key == 1  ->  style = W_value tanh(embed[idx])
-    TK(launch_copy_cols(P(h, "gst.values") + (size_t)style_idx * c.gst_E, c.gst_E, Me, seq, proj_dims, E + SE, Me, c.gst_E, st));
-  } else {
-    GemmArgs a;
-    memset(&a, 0, sizeof(a));
-    a.nseg = 2;
-    a.seg[0] = {P(h, "gst.const_enc"), c.gst_E / 2, 0, 0, 0, 1};  // ld 0: the same row for every batch element
-    a.seg[1] = {spk, SE, SE, 0, c.gst_E / 2, 1};
-    a.W = P(h, "gst.stl.attention.W_query.weight");
-    a.ldw = c.gst_E / 2 + SE;
-    a.M = B;
-    a.N = c.gst_E;
-    a.T = 1;
-    a.Y = ws + L.style_q;
-    a.ldy = c.gst_E;
-    a.fma_chain = rg != nullptr;
-    TK(launch_gemm(a, st));
-    const int dk = c.gst_E / c.gst_heads;
-    gst_attention_kernel<<<B, 256, 0, st>>>(ws + L.style_q, P(h, "gst.keys"), P(h, "gst.values"), c.gst_tokens,
-                                            ws + L.style, c.gst_E, c.gst_heads, 1.0f / sqrtf((float)dk));
-    MB_LAUNCH_CHECK("gst_attention_kernel");
-    TK(launch_copy_cols(ws + L.style, c.gst_E, Tc, seq, proj_dims, E + SE, Me, c.gst_E, st));
-  }
-  {
-    GemmArgs a = gemm1(seq, proj_dims, proj_dims, P(h, "encoder_proj.weight"), proj_dims, nullptr, Me, D, ws + L.proj, D);
-    a.fma_chain = rg != nullptr;
-    TK(launch_gemm(a, st));
-  }
 
   // ------------------------------------------------------------------ decoder loop (tacotron.py:264-275)
   MB_CUDA_CHECK(cudaMemsetAsync(ws + L.attn_h, 0, sizeof(float) * (L.dp1 - L.attn_h), st));  // states, ctx, cum
@@ -1270,7 +1940,6 @@ int generate_impl(mb_tacotron* h, const int32_t* chars, const float* spk, int32_
   MB_CUDA_CHECK(cudaMemsetAsync(flags, 0, sizeof(int) * nst, st));
   uint8_t* dm = reinterpret_cast<uint8_t*>(ws + L.dmask);
   const size_t dmask_n = (size_t)B * 2 * D;
-  const size_t lsa_smem = lsa_step_smem_bytes(Tc);
   MB_CUDA_CHECK(lsa_step_prepare(Tc));
   if (!dec_masks && rg) {
     fill_masks_seeded_kernel<<<(unsigned)((2 * dmask_n * (size_t)nst + 255) / 256), 256, 0, st>>>(dm, B, nst, 2 * D, d_seeds, 1);
@@ -1283,457 +1952,30 @@ int generate_impl(mb_tacotron* h, const int32_t* chars, const float* spk, int32_
   int done_step = -1;
   std::vector<int> hflags(nst, 0);
   int checked = 0;
-  // One decoder step.  The step index is (sp ? *sp : 0) + sj, resolved ON THE DEVICE by the few kernels that
-  // need it (PreNet input frame and dropout masks, alignment row, mel output frames, stop flag), so the same
-  // launch sequence can be captured once into a CUDA graph and replayed for every group of steps.
-  // Fused operand split (MB_TACO_SPLIT_FUSED, default 1): the five act_split launches of a step disappear - every kernel that
-  // produces an input of a tensor-core GEMM (PreNet, context, attention GRU, rnn_input, the two LSTM cells) writes the fp16 hi / lo
-  // operand chunks itself, into per-consumer tiles (the LSTM tiles ping-pong on the step parity: a cell writes h' for the next step
-  // while other CTAs of the same launch still read this step's tiles).
-  static const bool split_fused_env = [] {
-    const char* e = getenv("MB_TACO_SPLIT_FUSED");
-    return e ? atoi(e) != 0 : true;
-  }();
-  static const bool prenet_fused_env = [] {
-    const char* e = getenv("MB_TACO_PRENET_FUSED");
-    return e ? atoi(e) != 0 : true;
-  }();
-  const bool fsplit = split_fused_env && prenet_fused_env && use_tc && D % 64 == 0 && proj_dims % 256 == 0 && LD % 64 == 0 &&
-                      (r * NM) % 4 == 0 && NM <= 128 && 2 * D <= 256 && B <= 128;
-  const FusedSplit fs = fused_split_layout(B > 128 ? 128 : B, proj_dims, D, LD);
-  char* fbase = reinterpret_cast<char*>(ws + L.fsp);
-  auto fhi = [&](size_t off) { return reinterpret_cast<__half*>(fbase + off); };
-  const int f_rows_pad = B <= 64 ? 64 : 128;
-  // Step DAG (MB_TACO_DAG, default 1, needs the fused split): a step's critical path is a chain of ~10 latency-bound kernels.  Three
-  // of its GEMMs have a K segment that is known a whole step early - W_hh h_{t-1} of both LSTM cells and the context half of the
-  // attention GRU's input projection - so those halves run on a side stream (TCS_PLAIN over a k-block range, result added to the
-  // accumulator of the short main-path GEMM), and so does the stop projection / stop rule, which nothing in the next step needs.
-  // The side stream forks from / joins the main one with events, inside the captured graph as well.
-  static const bool dag_env = [] {
-    const char* e = getenv("MB_TACO_DAG");
-    return e ? atoi(e) != 0 : true;
-  }();
-  const bool dag = dag_env && fsplit && proj_dims % 64 == 0;
-  cudaStream_t sd = h->side_stream;
-  bool have_gic = false, have_p1 = false, have_p2 = false, have_stop = false, side_open = false;
-  // fork: side stream waits for everything enqueued on the main stream so far
-  auto side_after_main = [&](cudaEvent_t ev) -> int {
-    MB_CUDA_CHECK(cudaEventRecord(ev, st));
-    MB_CUDA_CHECK(cudaStreamWaitEvent(sd, ev, 0));
-    side_open = true;
-    return MB_OK;
-  };
-  auto main_after_side = [&](cudaEvent_t ev) -> int {
-    MB_CUDA_CHECK(cudaEventRecord(ev, sd));
-    MB_CUDA_CHECK(cudaStreamWaitEvent(st, ev, 0));
-    return MB_OK;
-  };
-  // join everything outstanding on the side stream (end of a captured group / of a directly launched step)
-  auto join_side = [&]() -> int {
-    if (side_open) {
-      int rcj = main_after_side(h->ev_side[7]);
-      if (rcj != MB_OK) return rcj;
-    }
-    side_open = have_gic = have_p1 = have_p2 = have_stop = false;
-    return MB_OK;
-  };
-  auto emit_step = [&](const int* sp, int sj) -> int {
-    // PreNet on the last frame of the previous step (go frame = zeros)
-    const uint8_t* m1;
-    const uint8_t* m2;
-    long long mstep = 0;
-    if (dec_masks) {
-      m1 = dec_masks;
-      m2 = m1 + dmask_n;
-      mstep = (long long)(2 * dmask_n);
-    } else {  // generated for all steps before the loop (fill_masks_steps_kernel)
-      m1 = dm;
-      m2 = dm + dmask_n;
-      mstep = (long long)(2 * dmask_n);
-    }
-    const bool prenet_fused = prenet_fused_env;  // A/B switch MB_TACO_PRENET_FUSED: 0 = two skinny GEMM launches (round 1)
-    const int par = sj & 1;  // graph groups start at even steps, so the parity of (base + sj) is that of sj
-    if (prenet_fused && NM <= 128 && 2 * D <= 256) {
-      // both PreNet layers in one launch; frame (step * r - 1) of every utterance, step 0 = the all-zero go frame
-      PrenetArgs pa;
-      memset(&pa, 0, sizeof(pa));
-      pa.x = mel_all - NM;
-      pa.x_ld = (long long)steps_alloc * NM;
-      pa.x_step = (long long)r * NM;
-      pa.x_first = mel_all + (size_t)B * steps_alloc * NM;
-      pa.W1 = P(h, "decoder.prenet.fc1.weight");
-      pa.b1 = P(h, "decoder.prenet.fc1.bias");
-      pa.W2 = P(h, "decoder.prenet.fc2.weight");
-      pa.b2 = P(h, "decoder.prenet.fc2.bias");
-      pa.m1 = m1;
-      pa.m2 = m2;
-      pa.mask_step = mstep;
-      pa.step_ptr = sp;
-      pa.step_j = sj;
-      pa.B = B;
-      pa.K = NM;
-      pa.H = 2 * D;
-      pa.y = ws + L.dp2;
-      pa.ldy = 2 * D;
-      if (fsplit) {  // [ctx | prenet] tiles of the attention GRU's input GEMM
-        pa.s_hi = fhi(fs.p1);
-        pa.s_lo = fhi(fs.p1 + fs.b1);
-        pa.s_k0 = proj_dims;
-        pa.s_rows_pad = f_rows_pad;
-      }
-      TK(launch_prenet_fused(pa, st));
-    } else {
-      // frame (step * r - 1) of every utterance; step 0 reads the zero block behind mel_all with row stride 0
-      GemmArgs a = gemm1(mel_all - NM, NM, steps_alloc * NM, P(h, "decoder.prenet.fc1.weight"), NM,
-                         P(h, "decoder.prenet.fc1.bias"), B, 2 * D, ws + L.dp1, 2 * D, ACT_RELU);
-      a.mask = m1;
-      a.step_mode = 1;
-      a.step_ptr = sp;
-      a.step_j = sj;
-      a.x_step = (long long)r * NM;
-      a.x_first = mel_all + (size_t)B * steps_alloc * NM;
-      a.mask_step = mstep;
-      TK(launch_gemm(a, st));
-      GemmArgs b = gemm1(ws + L.dp1, 2 * D, 2 * D, P(h, "decoder.prenet.fc2.weight"), 2 * D, P(h, "decoder.prenet.fc2.bias"),
-                         B, 2 * D, ws + L.dp2, 2 * D, ACT_RELU);
-      b.mask = m2;
-      b.step_mode = 1;
-      b.step_ptr = sp;
-      b.step_j = sj;
-      b.mask_step = mstep;
-      TK(launch_gemm(b, st));
-    }
-    if (use_tc && D % 64 == 0) {  // attention GRU on [context, prenet]: input projection + recurrent step on tensor cores
-      __half* a_hi = reinterpret_cast<__half*>(ws + L.a_hi);
-      __half* a_lo = reinterpret_cast<__half*>(ws + L.a_lo);
-      if (fsplit) {
-        a_hi = fhi(fs.p1);
-        a_lo = fhi(fs.p1 + fs.b1);
-      } else {
-        TK(launch_act_split(ws + L.ctx, proj_dims, proj_dims, ws + L.dp2, 2 * D, 2 * D, B, a_hi, a_lo, st));
-      }
-      TcSkinnyArgs ta;
-      memset(&ta, 0, sizeof(ta));
-      ta.a_hi = a_hi;
-      ta.a_lo = a_lo;
-      ta.w = reinterpret_cast<const __half*>(P(h, "decoder.attn_rnn.ih.tcw"));
-      ta.bias = P(h, "decoder.attn_rnn.ih.tcb");
-      ta.KB = (proj_dims + 2 * D + 63) / 64;
-      if (dag) {  // the context half was multiplied on the side stream after the previous step's attention (zero at step 0)
-        if (have_gic) {
-          MB_CUDA_CHECK(cudaStreamWaitEvent(st, h->ev_side[1], 0));
-          have_gic = false;
-        }
-        ta.KBw = ta.KB;
-        ta.kb0 = proj_dims / 64;
-        ta.KB = ta.KBw - ta.kb0;
-        ta.pre = ws + L.gic;
-        ta.ldpre = 3 * D;
-      }
-      ta.M = B;
-      ta.N = 3 * D;
-      ta.mode = TCS_PLAIN;
-      ta.inv_scale = h->tc_inv_scale["decoder.attn_rnn.ih"];
-      ta.y = ws + L.dgi;
-      ta.ldy = 3 * D;
-      TK(launch_tc_skinny(ta, st));
-      const size_t tb = tc_skinny_act_bytes(B, D);
-      TcGruArgs g;
-      memset(&g, 0, sizeof(g));
-      if (fsplit) {  // attn_h is the trailing K segment of rnn_input's [ctx | attn_h] tiles
-        g.s_hi = fhi(fs.p2);
-        g.s_lo = fhi(fs.p2 + fs.b2);
-        g.s_k0 = proj_dims;
-      }
-      g.a_hi[0] = reinterpret_cast<const __half*>(reinterpret_cast<const char*>(ws + L.ah_hi) + par * tb);
-      g.a_lo[0] = reinterpret_cast<const __half*>(reinterpret_cast<const char*>(ws + L.ah_lo) + par * tb);
-      g.nxt_hi[0] = reinterpret_cast<__half*>(reinterpret_cast<char*>(ws + L.ah_hi) + (par ^ 1) * tb);
-      g.nxt_lo[0] = reinterpret_cast<__half*>(reinterpret_cast<char*>(ws + L.ah_lo) + (par ^ 1) * tb);
-      g.w[0] = reinterpret_cast<const __half*>(P(h, "decoder.attn_rnn.hh.tcw"));
-      g.bias[0] = P(h, "decoder.attn_rnn.hh.tcb");
-      g.gi[0] = ws + L.dgi;
-      g.h[0] = ws + L.attn_h;
-      g.out[0] = ws + L.attn_h;
-      g.inv_scale[0] = h->tc_inv_scale["decoder.attn_rnn.hh"];
-      g.ldgi = 3 * D;
-      g.ldout = D;
-      g.KB = D / 64;
-      g.M = B;
-      g.H = D;
-      g.ndir = 1;
-      TK(launch_tc_gru(g, st));
-    } else {  // attention GRU on [context, prenet]
-      GemmArgs a;
-      memset(&a, 0, sizeof(a));
-      a.nseg = 2;
-      a.seg[0] = {ws + L.ctx, proj_dims, proj_dims, 0, 0, 1};
-      a.seg[1] = {ws + L.dp2, 2 * D, 2 * D, 0, proj_dims, 1};
-      a.W = P(h, "decoder.attn_rnn.weight_ih");
-      a.ldw = proj_dims + 2 * D;
-      a.bias = P(h, "decoder.attn_rnn.bias_ih");
-      a.M = B;
-      a.N = 3 * D;
-      a.T = 1;
-      a.Y = ws + L.dgi;
-      a.ldy = 3 * D;
-      TK(launch_gemm(a, st));
-      GemmArgs b = gemm1(ws + L.attn_h, D, D, P(h, "decoder.attn_rnn.weight_hh"), D, P(h, "decoder.attn_rnn.bias_hh"), B, 3 * D,
-                         ws + L.dgh, 3 * D);
-      TK(launch_gemm(b, st));
-      TK(launch_gru_cell(ws + L.dgi, 3 * D, ws + L.dgh, ws + L.attn_h, D, nullptr, 0, B, D, st));
-    }
-    {  // location sensitive attention + context
-      // MB_TACO_LSA_FUSED (default 1): 512 threads per batch row (4 time-step groups in the energy phase) and the query
-      // projection W q + b inside the kernel; 0 = round-2 shape (256 threads, separate GEMM launch)
-      static const bool lsa_fused = [] {
-        const char* e = getenv("MB_TACO_LSA_FUSED");
-        return e ? atoi(e) != 0 : true;
-      }();
-      const bool qf = lsa_fused && D == ATT_D;
-      if (!qf) {
-        GemmArgs a = gemm1(ws + L.attn_h, D, D, P(h, "decoder.attn_net.W.weight"), D, P(h, "decoder.attn_net.W.bias"), B, D,
-                           ws + L.pq, D);
-        TK(launch_gemm(a, st));
-      }
-      MB_CUDA_CHECK(launch_pdl2(lsa_step_kernel, dim3(B), dim3(lsa_fused ? 512 : 256), lsa_smem, st, ws + L.pq, ws + L.proj, seq,
-                                proj_dims, chars, ws + L.cum, P(h, "decoder.attn_net.conv.weight"),
-                                P(h, "decoder.attn_net.conv.bias"), P(h, "decoder.attn_net.L.weight"),
-                                P(h, "decoder.attn_net.v.weight"), ws + L.scores_all, nst * Tc,
-                                (proj_dims % 256 == 0) ? nullptr : ws + L.ctx, Tc, sp, sj, qf ? ws + L.attn_h : nullptr,
-                                P(h, "decoder.attn_net.W.weight"), P(h, "decoder.attn_net.W.bias"), d_lens));
-      MB_LAUNCH_CHECK("lsa_step_kernel");
-      if (proj_dims % 256 == 0) {
-        if (have_stop) {  // the previous step's stop projection (side stream) still reads ctx and x, which are rewritten from here on
-          MB_CUDA_CHECK(cudaStreamWaitEvent(st, h->ev_side[6], 0));
-          have_stop = false;
-        }
-        MB_CUDA_CHECK(launch_pdl2(lsa_ctx_kernel, dim3(proj_dims / 256, B), dim3(256), sizeof(float) * Tc, st, ws + L.scores_all,
-                                  nst * Tc, seq, proj_dims, Tc, ws + L.ctx, sp, sj, fsplit ? fhi(fs.p1) : nullptr,
-                                  fsplit ? fhi(fs.p1 + fs.b1) : nullptr, fsplit ? fhi(fs.p2) : nullptr,
-                                  fsplit ? fhi(fs.p2 + fs.b2) : nullptr, f_rows_pad, d_lens));
-        MB_LAUNCH_CHECK("lsa_ctx_kernel");
-      }
-      if (dag) {  // side stream: context half of the NEXT step's attention-GRU input projection
-        int rcs = side_after_main(h->ev_side[0]);
-        if (rcs != MB_OK) return rcs;
-        TcSkinnyArgs tp;
-        memset(&tp, 0, sizeof(tp));
-        tp.a_hi = fhi(fs.p1);
-        tp.a_lo = fhi(fs.p1 + fs.b1);
-        tp.w = reinterpret_cast<const __half*>(P(h, "decoder.attn_rnn.ih.tcw"));
-        tp.KBw = (proj_dims + 2 * D + 63) / 64;
-        tp.kb0 = 0;
-        tp.KB = proj_dims / 64;
-        tp.M = B;
-        tp.N = 3 * D;
-        tp.mode = TCS_PLAIN;
-        tp.inv_scale = h->tc_inv_scale["decoder.attn_rnn.ih"];
-        tp.y = ws + L.gic;
-        tp.ldy = 3 * D;
-        TK(launch_tc_skinny(tp, sd));
-        MB_CUDA_CHECK(cudaEventRecord(h->ev_side[1], sd));
-        have_gic = true;
-      }
-    }
-    if (use_tc) {  // rnn_input on [context, attn_hidden] (tensor cores)
-      __half* a_hi = reinterpret_cast<__half*>(ws + L.a_hi);
-      __half* a_lo = reinterpret_cast<__half*>(ws + L.a_lo);
-      if (fsplit) {
-        a_hi = fhi(fs.p2);
-        a_lo = fhi(fs.p2 + fs.b2);
-      } else {
-        TK(launch_act_split(ws + L.ctx, proj_dims, proj_dims, ws + L.attn_h, D, D, B, a_hi, a_lo, st));
-      }
-      TcSkinnyArgs ta;
-      memset(&ta, 0, sizeof(ta));
-      ta.a_hi = a_hi;
-      ta.a_lo = a_lo;
-      if (fsplit) {  // x is the leading K segment of the first LSTM's [x | h1] tiles of this step
-        ta.s_hi[0] = fhi(fs.p3[par]);
-        ta.s_lo[0] = fhi(fs.p3[par] + fs.b3);
-        ta.s_k0[0] = 0;
-      }
-      ta.w = reinterpret_cast<const __half*>(P(h, "decoder.rnn_input.tcw"));
-      ta.bias = P(h, "decoder.rnn_input.tcb");
-      ta.KB = (proj_dims + D + 63) / 64;
-      ta.M = B;
-      ta.N = LD;
-      ta.mode = TCS_PLAIN;
-      ta.inv_scale = h->tc_inv_scale["decoder.rnn_input"];
-      ta.y = ws + L.x;
-      ta.ldy = LD;
-      TK(launch_tc_skinny(ta, st));
-    } else {  // rnn_input on [context, attn_hidden]
-      GemmArgs a;
-      memset(&a, 0, sizeof(a));
-      a.nseg = 2;
-      a.seg[0] = {ws + L.ctx, proj_dims, proj_dims, 0, 0, 1};
-      a.seg[1] = {ws + L.attn_h, D, D, 0, proj_dims, 1};
-      a.W = P(h, "decoder.rnn_input.weight");
-      a.ldw = proj_dims + D;
-      a.bias = P(h, "decoder.rnn_input.bias");
-      a.M = B;
-      a.N = LD;
-      a.T = 1;
-      a.Y = ws + L.x;
-      a.ldy = LD;
-      TK(launch_gemm(a, st));
-    }
-    for (int l = 0; l < 2; ++l) {  // residual LSTMs
-      const std::string n = l == 0 ? "decoder.res_rnn1" : "decoder.res_rnn2";
-      float* hh = ws + (l == 0 ? L.h1 : L.h2);
-      float* cc = ws + (l == 0 ? L.c1 : L.c2);
-      if (use_tc) {
-        // gates GEMM on the tensor cores (3-term fp16 split, FP32 accumulate) with the cell update fused
-        __half* a_hi = reinterpret_cast<__half*>(ws + L.a_hi);
-        __half* a_lo = reinterpret_cast<__half*>(ws + L.a_lo);
-        TcSkinnyArgs ta;
-        memset(&ta, 0, sizeof(ta));
-        if (fsplit) {
-          // this step's [x | h] tiles; x' (residual stream) goes to the next consumer's tiles, h' to this cell's tiles of the
-          // NEXT step (other parity)
-          const size_t* mine = l == 0 ? fs.p3 : fs.p4;
-          a_hi = fhi(mine[par]);
-          a_lo = fhi(mine[par] + fs.b3);
-          ta.s_hi[1] = fhi(mine[par ^ 1]);
-          ta.s_lo[1] = fhi(mine[par ^ 1] + fs.b3);
-          ta.s_k0[1] = LD;
-          ta.s_hi[0] = l == 0 ? fhi(fs.p4[par]) : fhi(fs.p5);
-          ta.s_lo[0] = l == 0 ? fhi(fs.p4[par] + fs.b3) : fhi(fs.p5 + fs.b5);
-          ta.s_k0[0] = 0;
-        } else {
-          TK(launch_act_split(ws + L.x, LD, LD, hh, LD, LD, B, a_hi, a_lo, st));
-        }
-        ta.a_hi = a_hi;
-        ta.a_lo = a_lo;
-        ta.w = reinterpret_cast<const __half*>(P(h, n + ".tcw"));
-        ta.bias = P(h, n + ".tcb");
-        ta.KB = 2 * LD / 64;
-        if (dag) {  // W_hh h_{t-1} was multiplied on the side stream right after the previous step's cell (zero at step 0)
-          bool& have = l == 0 ? have_p1 : have_p2;
-          if (have) {
-            MB_CUDA_CHECK(cudaStreamWaitEvent(st, h->ev_side[l == 0 ? 3 : 5], 0));
-            have = false;
-          }
-          ta.KBw = ta.KB;
-          ta.kb0 = 0;
-          ta.KB = LD / 64;
-          ta.pre = ws + (l == 0 ? L.pre1 : L.pre2);
-          ta.ldpre = 4 * LD;
-        }
-        ta.M = B;
-        ta.N = 4 * LD;
-        ta.mode = TCS_LSTM;
-        ta.inv_scale = h->tc_inv_scale[n];
-        ta.c = cc;
-        ta.h = hh;
-        ta.x = ws + L.x;
-        ta.H = LD;
-        TK(launch_tc_skinny(ta, st));
-        if (dag) {  // side stream: W_hh h_t for the next step, from the h tiles this launch just wrote (other parity)
-          int rcs = side_after_main(h->ev_side[l == 0 ? 2 : 4]);
-          if (rcs != MB_OK) return rcs;
-          const size_t* mine = l == 0 ? fs.p3 : fs.p4;
-          TcSkinnyArgs tp;
-          memset(&tp, 0, sizeof(tp));
-          tp.a_hi = fhi(mine[par ^ 1]);
-          tp.a_lo = fhi(mine[par ^ 1] + fs.b3);
-          tp.w = reinterpret_cast<const __half*>(P(h, n + ".tcw"));
-          tp.KBw = 2 * LD / 64;
-          tp.kb0 = LD / 64;
-          tp.KB = LD / 64;
-          tp.M = B;
-          tp.N = 4 * LD;
-          tp.mode = TCS_PLAIN;
-          tp.inv_scale = h->tc_inv_scale[n];
-          tp.y = ws + (l == 0 ? L.pre1 : L.pre2);
-          tp.ldy = 4 * LD;
-          TK(launch_tc_skinny(tp, sd));
-          MB_CUDA_CHECK(cudaEventRecord(h->ev_side[l == 0 ? 3 : 5], sd));
-          (l == 0 ? have_p1 : have_p2) = true;
-        }
-        continue;
-      }
-      GemmArgs a;
-      memset(&a, 0, sizeof(a));
-      // gates = linear_hh(h) + linear_ih(x): two GEMMs chained through the residual input of the second
-      GemmArgs g1 = gemm1(hh, LD, LD, P(h, n + ".weight_hh"), LD, P(h, n + ".bias_hh"), B, 4 * LD, ws + L.gates, 4 * LD);
-      TK(launch_gemm(g1, st));
-      GemmArgs g2 = gemm1(ws + L.x, LD, LD, P(h, n + ".weight_ih"), LD, P(h, n + ".bias_ih"), B, 4 * LD, ws + L.gates, 4 * LD);
-      g2.res = ws + L.gates;
-      g2.ldres = 4 * LD;
-      TK(launch_gemm(g2, st));
-      TK(launch_lstm_cell(ws + L.gates, cc, hh, ws + L.x, B, LD, st));
-    }
-    {  // mel frames of this step, written straight into mel_all[b][t..t+r)[:]
-      if (use_tc && (r * NM) % 4 == 0) {
-        __half* a_hi = reinterpret_cast<__half*>(ws + L.a_hi);
-        __half* a_lo = reinterpret_cast<__half*>(ws + L.a_lo);
-        if (fsplit) {
-          a_hi = fhi(fs.p5);
-          a_lo = fhi(fs.p5 + fs.b5);
-        } else {
-          TK(launch_act_split(ws + L.x, LD, LD, nullptr, 0, 0, B, a_hi, a_lo, st));
-        }
-        TcSkinnyArgs ta;
-        memset(&ta, 0, sizeof(ta));
-        ta.a_hi = a_hi;
-        ta.a_lo = a_lo;
-        ta.w = reinterpret_cast<const __half*>(P(h, "decoder.mel_proj.tcw"));
-        ta.bias = nullptr;
-        ta.KB = LD / 64;
-        ta.M = B;
-        ta.N = r * NM;
-        ta.mode = TCS_PLAIN;
-        ta.inv_scale = h->tc_inv_scale["decoder.mel_proj"];
-        ta.y = mel_all;
-        ta.ldy = steps_alloc * NM;
-        ta.step_ptr = sp;
-        ta.step_j = sj;
-        ta.y_step = (long long)r * NM;
-        TK(launch_tc_skinny(ta, st));
-      } else {
-        if (sp) return fail(MB_ERR_STATE, "mb_tacotron_generate: graph replay needs the tensor-core mel projection");
-        GemmArgs a = gemm1(ws + L.x, LD, LD, P(h, "decoder.mel_proj.packed"), LD, nullptr, B, r * NM,
-                           mel_all + (size_t)sj * r * NM, steps_alloc * NM);
-        TK(launch_gemm(a, st));
-      }
-      GemmArgs s;
-      memset(&s, 0, sizeof(s));
-      s.nseg = 2;
-      s.seg[0] = {ws + L.x, LD, LD, 0, 0, 1};
-      s.seg[1] = {ws + L.ctx, proj_dims, proj_dims, 0, LD, 1};
-      s.W = P(h, "decoder.stop_proj.weight");
-      s.ldw = LD + proj_dims;
-      s.bias = P(h, "decoder.stop_proj.bias");
-      s.M = B;
-      s.N = 1;
-      s.T = 1;
-      s.act = ACT_SIGMOID;
-      s.Y = ws + L.stopv;
-      s.ldy = 1;
-      static const bool stop_fused = [] {
-        const char* e = getenv("MB_TACO_STOP_FUSED");  // 0 = stop projection and stop rule as two launches (round 2)
-        return e ? atoi(e) != 0 : true;
-      }();
-      if (stop_fused) {
-        // the CTA that finishes last applies the stop rule (ticket counter behind the step counter, reset by that CTA).
-        // With the step DAG it runs on the side stream (after the second LSTM's fork): the next step does not need it.
-        stop_step_kernel<<<B, 256, 0, dag ? sd : st>>>(s, B, min_stop_token, r, flags, sp, sj,
-                                                       reinterpret_cast<unsigned int*>(ws + L.step) + 16, d_done, d_caps);
-        MB_LAUNCH_CHECK("stop_step_kernel");
-        if (dag) {
-          MB_CUDA_CHECK(cudaEventRecord(h->ev_side[6], sd));
-          have_stop = true;
-        }
-      } else {
-        TK(launch_gemm(s, st));
-        stop_flag_kernel<<<1, 32, 0, st>>>(ws + L.stopv, B, min_stop_token, r, flags, sp, sj, d_done, d_caps);
-        MB_LAUNCH_CHECK("stop_flag_kernel");
-      }
-    }
-    return MB_OK;
-  };
+  DecoderLoop dl;
+  dl.h = h;
+  dl.L = L;
+  dl.ws = ws;
+  dl.B = B;
+  dl.Tc = Tc;
+  dl.r = r;
+  dl.nst = nst;
+  dl.steps_alloc = steps_alloc;
+  dl.chars = chars;
+  dl.seq = seq;
+  dl.mel_all = mel_all;
+  dl.dec_masks = dec_masks;
+  dl.dm = dm;
+  dl.min_stop_token = min_stop_token;
+  dl.flags = flags;
+  dl.d_lens = d_lens;
+  dl.d_caps = d_caps;
+  dl.d_done = d_done;
+  dl.d_start = nullptr;
+  dl.use_tc = use_tc;
+  dl.init(st);
+  auto emit_step = [&](const int* sp, int sj) { return dl.emit_step(sp, sj); };
+  auto join_side = [&]() { return dl.join_side(); };
 
   // poll the early-stop rule (tacotron.py:275) after every group of 16 decoder steps
   auto poll = [&](int upto) -> int {
@@ -1745,9 +1987,6 @@ int generate_impl(mb_tacotron* h, const int32_t* chars, const float* spk, int32_
     checked = upto + 1;
     return MB_OK;
   };
-  // Groups of kGraphSteps steps are captured once and replayed (the loop is launch-bound: ~20 kernels of a few
-  // microseconds per step); MB_TACO_GRAPH=0 or a capture failure falls back to direct launches.
-  constexpr int kGraphSteps = 8;
   static const bool graph_env = [] {
     const char* e = getenv("MB_TACO_GRAPH");
     return e ? atoi(e) != 0 : true;
@@ -1758,18 +1997,8 @@ int generate_impl(mb_tacotron* h, const int32_t* chars, const float* spk, int32_
     MB_CUDA_CHECK(cudaMemsetAsync(step_dev, 0, sizeof(int), st));
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
-    const uint64_t launches_before = mb_launch_count();
-    bool ok = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
-    int rc_cap = MB_OK;
-    if (ok) {
-      for (int j = 0; j < kGraphSteps && rc_cap == MB_OK; ++j) rc_cap = emit_step(step_dev, j);
-      if (rc_cap == MB_OK) rc_cap = join_side();
-      if (rc_cap == MB_OK) step_advance_kernel<<<1, 32, 0, st>>>(step_dev, kGraphSteps);
-      ok = cudaStreamEndCapture(st, &graph) == cudaSuccess && rc_cap == MB_OK && graph != nullptr;
-    }
-    if (ok) ok = cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess;
-    const int per_graph = (int)(mb_launch_count() - launches_before);
-    count_launch(-per_graph);  // captured, not launched; every replay below counts them
+    int per_graph = 0;
+    const bool ok = capture_group(dl, step_dev, &graph, &exec, &per_graph);
     if (ok) {
       while (si + kGraphSteps <= nst && done_step < 0) {
         if (cudaGraphLaunch(exec, st) != cudaSuccess) {
@@ -1784,8 +2013,6 @@ int generate_impl(mb_tacotron* h, const int32_t* chars, const float* spk, int32_
           if (rc2 != MB_OK) return rc2;
         }
       }
-    } else {
-      cudaGetLastError();  // clear the capture error; direct launches below
     }
     if (exec) cudaGraphExecDestroy(exec);
     if (graph) cudaGraphDestroy(graph);
@@ -1828,16 +2055,8 @@ int generate_impl(mb_tacotron* h, const int32_t* chars, const float* spk, int32_
   } else {
     melc = mel_all;
   }
-  rc = run_cbhg(h, "postnet", c.postnet_K, NM, PD, PD, NM, c.num_highways, melc, B, frames, ws + L.pbank, ws + L.ppool,
-                ws + L.ppj1, ws + L.py, ws + L.phw12, ws + L.pgi_f, ws + L.pgi_b, ws + L.pgh, ws + L.phst, ws + L.pout, PD, st,
-                use_tc ? ws + L.a_hi : nullptr, use_tc ? ws + L.a_lo : nullptr, tc_skinny_act_bytes(B > 128 ? 128 : B, 2 * LD), bw,
-                d_flen);
+  rc = run_postnet(h, L, ws, melc, B, frames, d_flen, use_tc, st);
   if (rc != MB_OK) return rc;
-  {
-    GemmArgs a = gemm1(ws + L.pout, PD, PD, P(h, "post_proj.weight"), PD, nullptr, B * frames, NM, ws + L.lin, NM);
-    int rc2 = cbhg_gemm(h, "post_proj", a, st, bw, d_flen);
-    if (rc2 != MB_OK) return rc2;
-  }
   // outputs in the reference's layouts: mel [B][80][frames], linear [B][80][frames], attn [B][nsteps][Tc]
   {
     const size_t n = (size_t)B * NM * frames;
@@ -1896,6 +2115,485 @@ int32_t mb_tacotron_max_chars(void) { return lsa_max_chars(); }
 
 }  // extern "C"
 
+namespace {
+
+// ---- streamed decoding (mb_tacotron_stream_*) ----------------------------------------------------------------------------------
+// A decoder loop over a fixed set of slots.  A text enters a free slot between graph replays (admission) and leaves when its row
+// stops; its frames and alignment rows are then copied to a pool the postnet reads from its own stream.  Each row's step is the
+// global step minus its start step (DecoderLoop::d_start), and its per-step buffers are rings of kStreamRing steps beyond its cap,
+// so a row finished at its last step still has its frames when the next poll (at most 15 steps later) finds it.
+constexpr int kStreamPoll = 16;
+
+struct StreamLayout {
+  Ws enc, dec, post;
+  // byte offsets
+  size_t enc_at, dec_at, post_at, pool_seq, pool_proj, pool_chars, pool_tab, post_mel, post_attn, post_flen, admit_tab, start, total;
+};
+
+StreamLayout stream_layout(const mb_tacotron_config& c, int S, int Tc, int nst, int r) {
+  StreamLayout L{};
+  const int ring = nst + kStreamPoll, proj_dims = c.encoder_dims + c.speaker_embedding_size + c.gst_E;
+  L.enc = ws_layout(c, S, Tc, r, r, true, WS_ENC);
+  L.dec = ws_layout(c, S, Tc, ring * r, r, true, WS_DEC);
+  L.post = ws_layout(c, S, Tc, nst * r, r, true, WS_POST);
+  WsLayout W;
+  L.enc_at = W.take(L.enc.total);
+  L.dec_at = W.take(L.dec.total);
+  L.post_at = W.take(L.post.total);
+  L.pool_seq = W.take(sizeof(float) * (size_t)2 * S * Tc * proj_dims);
+  L.pool_proj = W.take(sizeof(float) * (size_t)2 * S * Tc * c.decoder_dims);
+  L.pool_chars = W.take(sizeof(int32_t) * (size_t)2 * S * Tc);
+  L.pool_tab = W.take(sizeof(int32_t) * (size_t)2 * S * 3);  // characters [2S] | seeds (u64) [2S] of each staging-pool row
+  L.post_mel = W.take(sizeof(float) * (size_t)2 * S * nst * r * c.n_mels);
+  L.post_attn = W.take(sizeof(float) * (size_t)2 * S * nst * Tc);
+  L.post_flen = W.take(sizeof(int32_t) * S);
+  L.admit_tab = W.take(sizeof(AdmitRow) * S);
+  L.start = W.take(sizeof(int32_t) * S);
+  L.total = W.total();
+  return L;
+}
+
+}  // namespace
+
+struct mb_taco_stream {
+  mb_tacotron* h = nullptr;
+  int S = 0, Tc = 0, nst = 0, ring = 0, r = 0, style_idx = 0;
+  StreamLayout L;
+  char* base = nullptr;
+  float *we = nullptr, *wd = nullptr, *wp = nullptr;
+  int* d_done = nullptr;
+  DecoderLoop dl;
+  cudaGraph_t graph = nullptr;
+  cudaGraphExec_t exec = nullptr;
+  int per_graph = 0;
+  cudaStream_t enc_st = nullptr;
+  cudaEvent_t ev_enc[2] = {nullptr, nullptr}, ev_admit = nullptr, ev_copied = nullptr, ev_post = nullptr, ev_in = nullptr;
+  int global = 0;                     // decoder steps run so far (the device step counter)
+  long long steps_run = 0;
+  std::vector<int64_t> occupant;      // text in each slot, -1: free
+  std::vector<int> pool;              // postnet pool rows: 0 free, 1 finished and waiting, 2 read by a postnet in flight
+  std::vector<int64_t> pool_id;
+  std::vector<int> pool_frames;
+  std::vector<int> pending;           // pool rows in the order their rows finished
+  std::vector<int32_t> hdone;
+  // releases the stream's graph, events and encoder stream (mb_tacotron_stream_close first waits for their work)
+  ~mb_taco_stream() {
+    if (exec) cudaGraphExecDestroy(exec);
+    if (graph) cudaGraphDestroy(graph);
+    for (cudaEvent_t e : {ev_enc[0], ev_enc[1], ev_admit, ev_copied, ev_post, ev_in})
+      if (e) cudaEventDestroy(e);
+    if (enc_st) cudaStreamDestroy(enc_st);
+  }
+};
+
+namespace {
+
+int stream_check(const char* fn, mb_taco_stream* s) {
+  if (!s || !s->h) return fail(MB_ERR_INVALID, "%s: null stream", fn);
+  return MB_OK;
+}
+
+int caller_to(mb_taco_stream* s, cudaStream_t caller, cudaStream_t to) {
+  MB_CUDA_CHECK(cudaEventRecord(s->ev_in, caller));
+  MB_CUDA_CHECK(cudaStreamWaitEvent(to, s->ev_in, 0));
+  return MB_OK;
+}
+
+// A few host bytes into device memory in stream order, carried as a kernel argument.  A copy from pageable host memory would
+// first wait for the stream, which would block the host behind an encode or a postnet that is still running.
+int upload(void* dst, const void* src, size_t n, cudaStream_t st) {
+  if (n > (size_t)kUploadBytes) return fail(MB_ERR_INVALID, "upload of %zu bytes (at most %d)", n, kUploadBytes);
+  UploadBlob b;
+  memcpy(b.b, src, n);
+  upload_kernel<<<1, 256, 0, st>>>(b, reinterpret_cast<unsigned char*>(dst), (int)n);
+  MB_LAUNCH_CHECK("upload_kernel");
+  return MB_OK;
+}
+
+// The per-slot regions of a stream's decoder loop and its staging pool.  Admission zeroes the rows of the `reset` regions (the
+// state a fresh row starts from, as generate zeroes it) and fills the rest of a slot's rows; mb_tacotron_stream_regions hands the
+// same list to tests.
+void stream_regions(const mb_taco_stream* s, std::vector<mb_taco_stream_region>& out) {
+  const mb_tacotron_config& c = s->h->cfg;
+  const Ws& D = s->L.dec;
+  float* wd = s->wd;
+  const int S = s->S, Dd = c.decoder_dims, LD = c.lstm_dims, proj_dims = c.encoder_dims + c.speaker_embedding_size + c.gst_E;
+  const int rows_pad = S <= 64 ? 64 : 128;
+  auto add = [&](const char* name, void* p, int kind, int rows, int width, int depth, int reset) {
+    mb_taco_stream_region r;
+    memset(&r, 0, sizeof(r));
+    snprintf(r.name, sizeof(r.name), "%s", name);
+    r.ptr = p;
+    r.kind = kind;
+    r.rows = rows;
+    r.width = width;
+    r.depth = depth;
+    r.reset = reset;
+    out.push_back(r);
+  };
+  add("attn_h", wd + D.attn_h, MB_TACO_REGION_F32, S, Dd, 1, 1);
+  add("h1", wd + D.h1, MB_TACO_REGION_F32, S, LD, 1, 1);
+  add("c1", wd + D.c1, MB_TACO_REGION_F32, S, LD, 1, 1);
+  add("h2", wd + D.h2, MB_TACO_REGION_F32, S, LD, 1, 1);
+  add("c2", wd + D.c2, MB_TACO_REGION_F32, S, LD, 1, 1);
+  add("ctx", wd + D.ctx, MB_TACO_REGION_F32, S, proj_dims, 1, 1);
+  add("cum", wd + D.cum, MB_TACO_REGION_F32, S, s->Tc, 1, 1);
+  add("pre1", wd + D.pre1, MB_TACO_REGION_F32, S, 4 * LD, 1, 1);
+  add("pre2", wd + D.pre2, MB_TACO_REGION_F32, S, 4 * LD, 1, 1);
+  add("gic", wd + D.gic, MB_TACO_REGION_F32, S, 3 * Dd, 1, 1);
+  const size_t tb = tc_skinny_act_bytes(S, Dd);
+  for (int par = 0; par < 2; ++par) {
+    add(par ? "ah_hi.1" : "ah_hi.0", reinterpret_cast<char*>(wd + D.ah_hi) + par * tb, MB_TACO_REGION_TILE, rows_pad, Dd, 1, 1);
+    add(par ? "ah_lo.1" : "ah_lo.0", reinterpret_cast<char*>(wd + D.ah_lo) + par * tb, MB_TACO_REGION_TILE, rows_pad, Dd, 1, 1);
+  }
+  const FusedSplit& fs = s->dl.fs;
+  char* fb = s->dl.fbase;
+  auto pair = [&](const char* hi, const char* lo, size_t off, size_t bytes, int K) {
+    add(hi, fb + off, MB_TACO_REGION_TILE, rows_pad, K, 1, 1);
+    add(lo, fb + off + bytes, MB_TACO_REGION_TILE, rows_pad, K, 1, 1);
+  };
+  pair("p1_hi", "p1_lo", fs.p1, fs.b1, proj_dims + 2 * Dd);
+  pair("p2_hi", "p2_lo", fs.p2, fs.b2, proj_dims + Dd);
+  pair("p3_hi.0", "p3_lo.0", fs.p3[0], fs.b3, 2 * LD);
+  pair("p3_hi.1", "p3_lo.1", fs.p3[1], fs.b3, 2 * LD);
+  pair("p4_hi.0", "p4_lo.0", fs.p4[0], fs.b3, 2 * LD);
+  pair("p4_hi.1", "p4_lo.1", fs.p4[1], fs.b3, 2 * LD);
+  pair("p5_hi", "p5_lo", fs.p5, fs.b5, LD);
+  add("seq", wd + D.seq, MB_TACO_REGION_F32, S, s->Tc * proj_dims, 1, 0);
+  add("proj", wd + D.proj, MB_TACO_REGION_F32, S, s->Tc * Dd, 1, 0);
+  add("chars", wd + D.ids, MB_TACO_REGION_I32, S, s->Tc, 1, 0);
+  int32_t* drows = reinterpret_cast<int32_t*>(wd + D.rows);
+  add("lens", drows, MB_TACO_REGION_I32, S, 1, 1, 0);
+  add("caps", drows + S, MB_TACO_REGION_I32, S, 1, 1, 0);
+  add("done", drows + 2 * S, MB_TACO_REGION_I32, S, 1, 1, 0);
+  add("start", s->base + s->L.start, MB_TACO_REGION_I32, S, 1, 1, 0);
+  add("dmask", wd + D.dmask, MB_TACO_REGION_U8, S, 2 * Dd, s->ring, 0);
+  add("pool_seq", s->base + s->L.pool_seq, MB_TACO_REGION_F32, 2 * S, s->Tc * proj_dims, 1, 0);
+  add("pool_proj", s->base + s->L.pool_proj, MB_TACO_REGION_F32, 2 * S, s->Tc * Dd, 1, 0);
+  add("pool_chars", s->base + s->L.pool_chars, MB_TACO_REGION_I32, 2 * S, s->Tc, 1, 0);
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t mb_tacotron_stream_workspace_bytes(const mb_tacotron* h, int32_t slots, int32_t n_chars, int32_t max_steps, int32_t r) {
+  if (!h || slots < 1 || slots > 128 || !mb_tacotron_workspace_bytes(h, slots, n_chars, max_steps, r)) return 0;
+  return stream_layout(h->cfg, slots, n_chars, (max_steps + r - 1) / r, r).total;
+}
+
+int mb_tacotron_stream_open(mb_tacotron* h, int32_t slots, int32_t n_chars, int32_t max_steps, int32_t r, int32_t style_idx,
+                            float min_stop_token, void* workspace, size_t workspace_bytes, void* stream, mb_taco_stream** out) {
+  const char* me = "mb_tacotron_stream_open";
+  if (!h || !out) return fail(MB_ERR_INVALID, "%s: null argument", me);
+  if (!h->finalized) return fail(MB_ERR_STATE, "%s: weights not finalized", me);
+  const mb_tacotron_config& c = h->cfg;
+  if (slots < 1 || slots > 128 || n_chars < 1 || max_steps < 1 || r < 1 || r > c.max_r)
+    return fail(MB_ERR_INVALID, "%s: %d slots (1 to 128), %d characters, %d frames, r = %d", me, slots, n_chars, max_steps, r);
+  if (n_chars > lsa_max_chars())
+    return fail(MB_ERR_INVALID, "%s: %d characters exceed the limit of %d (the attention step's shared memory)", me, n_chars,
+                lsa_max_chars());
+  const size_t need = mb_tacotron_stream_workspace_bytes(h, slots, n_chars, max_steps, r);
+  char* base;
+  if (int rc = bind(me, workspace, workspace_bytes, need, &base)) return rc;
+  if (int rc = ensure_streams(h)) return rc;
+  cudaStream_t st = h->own_stream;
+  std::unique_ptr<mb_taco_stream> s(new mb_taco_stream());
+  s->h = h;
+  s->S = slots;
+  s->Tc = n_chars;
+  s->r = r;
+  s->nst = (max_steps + r - 1) / r;
+  s->ring = s->nst + kStreamPoll;
+  s->style_idx = style_idx;
+  s->L = stream_layout(c, slots, n_chars, s->nst, r);
+  s->base = base;
+  s->we = reinterpret_cast<float*>(base + s->L.enc_at);
+  s->wd = reinterpret_cast<float*>(base + s->L.dec_at);
+  s->wp = reinterpret_cast<float*>(base + s->L.post_at);
+  s->occupant.assign(slots, -1);
+  s->pool.assign(2 * slots, 0);
+  s->pool_id.assign(2 * slots, -1);
+  s->pool_frames.assign(2 * slots, 0);
+  s->hdone.assign(slots, 0);
+  MB_CUDA_CHECK(cudaStreamCreateWithFlags(&s->enc_st, cudaStreamNonBlocking));
+  for (cudaEvent_t* e : {&s->ev_enc[0], &s->ev_enc[1], &s->ev_admit, &s->ev_copied, &s->ev_post, &s->ev_in})
+    MB_CUDA_CHECK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+  if (int rc = caller_to(s.get(), (cudaStream_t)stream, st)) return rc;
+  if (int rc = prepare_mel_proj(h, r, st)) return rc;
+  MB_CUDA_CHECK(lsa_step_prepare(n_chars));
+  const Ws& D = s->L.dec;
+  float* wd = s->wd;
+  // every slot starts empty: zero state, one character, done at step 0 (a finished row that is never reported)
+  MB_CUDA_CHECK(cudaMemsetAsync(wd, 0, D.total, st));
+  int32_t* rows = reinterpret_cast<int32_t*>(wd + D.rows);
+  std::vector<int32_t> init((size_t)3 * slots, 0);
+  for (int b = 0; b < slots; ++b) init[b] = init[slots + b] = 1;
+  MB_CUDA_CHECK(cudaMemcpyAsync(rows, init.data(), sizeof(int32_t) * init.size(), cudaMemcpyHostToDevice, st));
+  MB_CUDA_CHECK(cudaMemsetAsync(base + s->L.start, 0, sizeof(int32_t) * slots, st));
+  s->d_done = rows + 2 * slots;
+  DecoderLoop& dl = s->dl;
+  dl.h = h;
+  dl.L = D;
+  dl.ws = wd;
+  dl.B = slots;
+  dl.Tc = n_chars;
+  dl.r = r;
+  dl.nst = s->ring;
+  dl.steps_alloc = s->ring * r;
+  dl.chars = reinterpret_cast<const int32_t*>(wd + D.ids);
+  dl.seq = wd + D.seq;
+  dl.mel_all = wd + D.mel_all;
+  dl.dec_masks = nullptr;
+  dl.dm = reinterpret_cast<uint8_t*>(wd + D.dmask);
+  dl.min_stop_token = min_stop_token;
+  dl.flags = nullptr;
+  dl.d_lens = rows;
+  dl.d_caps = rows + slots;
+  dl.d_done = s->d_done;
+  dl.d_start = reinterpret_cast<const int*>(base + s->L.start);
+  dl.use_tc = true;
+  dl.init(st);
+  if (!dl.fsplit || (r * c.n_mels) % 4)
+    return fail(MB_ERR_STATE, "%s: streaming needs the fused decoder step (MB_TACO_SPLIT_FUSED, MB_TACO_PRENET_FUSED)", me);
+  if (!capture_group(dl, reinterpret_cast<int*>(wd + D.step), &s->graph, &s->exec, &s->per_graph))
+    return fail(MB_ERR_CUDA, "%s: capturing the decoder step graph failed", me);
+  MB_CUDA_CHECK(cudaEventRecord(s->ev_admit, st));
+  MB_CUDA_CHECK(cudaEventRecord(s->ev_enc[0], st));
+  MB_CUDA_CHECK(cudaEventRecord(s->ev_enc[1], st));
+  MB_CUDA_CHECK(cudaEventRecord(s->ev_post, st));
+  MB_CUDA_CHECK(cudaEventRecord(h->ev_out, st));
+  MB_CUDA_CHECK(cudaStreamWaitEvent((cudaStream_t)stream, h->ev_out, 0));
+  *out = s.release();
+  return MB_OK;
+}
+
+int mb_tacotron_stream_encode(mb_taco_stream* s, int32_t pool_row, int32_t n, const int32_t* chars, const float* spk,
+                              const int32_t* row_chars, const uint64_t* row_seeds, const uint8_t* enc_masks, void* stream) {
+  const char* me = "mb_tacotron_stream_encode";
+  if (int rc = stream_check(me, s)) return rc;
+  if (!chars || !spk || !row_chars || !row_seeds) return fail(MB_ERR_INVALID, "%s: null argument", me);
+  if (n < 1 || pool_row < 0 || pool_row / s->S != (pool_row + n - 1) / s->S || pool_row + n > 2 * s->S)
+    return fail(MB_ERR_INVALID, "%s: rows [%d, %d) are not inside one half of the staging pool (2 x %d rows)", me, pool_row,
+                pool_row + n, s->S);
+  for (int i = 0; i < n; ++i)
+    if (row_chars[i] < 1 || row_chars[i] > s->Tc)
+      return fail(MB_ERR_INVALID, "%s: row %d has %d characters, outside [1, %d]", me, i, row_chars[i], s->Tc);
+  mb_tacotron* h = s->h;
+  const mb_tacotron_config& c = h->cfg;
+  const int proj_dims = c.encoder_dims + c.speaker_embedding_size + c.gst_E, Tc = s->Tc, S2 = 2 * s->S;
+  cudaStream_t st = s->enc_st;
+  if (int rc = caller_to(s, (cudaStream_t)stream, st)) return rc;
+  MB_CUDA_CHECK(cudaStreamWaitEvent(st, s->ev_admit, 0));  // the rows it overwrites have been admitted
+  int32_t* tab = reinterpret_cast<int32_t*>(s->base + s->L.pool_tab);
+  uint64_t* seeds = reinterpret_cast<uint64_t*>(tab + S2);
+  if (int rc = upload(tab + pool_row, row_chars, sizeof(int32_t) * n, st)) return rc;
+  if (int rc = upload(seeds + pool_row, row_seeds, sizeof(uint64_t) * n, st)) return rc;
+  MB_CUDA_CHECK(cudaMemcpyAsync(reinterpret_cast<int32_t*>(s->base + s->L.pool_chars) + (size_t)pool_row * Tc, chars,
+                                sizeof(int32_t) * n * Tc, cudaMemcpyDeviceToDevice, st));
+  float* seq = reinterpret_cast<float*>(s->base + s->L.pool_seq) + (size_t)pool_row * Tc * proj_dims;
+  float* proj = reinterpret_cast<float*>(s->base + s->L.pool_proj) + (size_t)pool_row * Tc * c.decoder_dims;
+  if (int rc = run_encoder(h, s->L.enc, s->we, chars, spk, n, Tc, s->style_idx, enc_masks, 0, true, tab + pool_row, seeds + pool_row,
+                           true, seq, proj, st))
+    return rc;
+  // only the admissions that copy these rows wait for them (mb_tacotron_stream_admit): the caller's stream does not, so the
+  // decoder keeps running while the encoder works; the inputs must stay allocated until the stream is closed
+  MB_CUDA_CHECK(cudaEventRecord(s->ev_enc[pool_row / s->S], st));
+  return MB_OK;
+}
+
+int mb_tacotron_stream_admit(mb_taco_stream* s, int32_t n, const int32_t* slot, const int32_t* pool_row, const int64_t* text_id,
+                             const int32_t* row_chars, const int32_t* row_steps, const uint64_t* row_seeds,
+                             const uint8_t* const* dec_masks, void* stream) {
+  const char* me = "mb_tacotron_stream_admit";
+  if (int rc = stream_check(me, s)) return rc;
+  if (!slot || !pool_row || !text_id || !row_chars || !row_steps || !row_seeds) return fail(MB_ERR_INVALID, "%s: null argument", me);
+  if (n < 1 || n > s->S) return fail(MB_ERR_INVALID, "%s: %d rows (1 to %d)", me, n, s->S);
+  std::vector<AdmitRow> rows(n);
+  std::vector<int> seen(s->S, 0);
+  for (int i = 0; i < n; ++i) {
+    if (slot[i] < 0 || slot[i] >= s->S || s->occupant[slot[i]] >= 0 || seen[slot[i]]++)
+      return fail(MB_ERR_INVALID, "%s: slot %d is not free", me, slot[i]);
+    if (pool_row[i] < 0 || pool_row[i] >= 2 * s->S) return fail(MB_ERR_INVALID, "%s: pool row %d", me, pool_row[i]);
+    if (row_chars[i] < 1 || row_chars[i] > s->Tc)
+      return fail(MB_ERR_INVALID, "%s: row %d has %d characters, outside [1, %d]", me, i, row_chars[i], s->Tc);
+    if (row_steps[i] < 1 || row_steps[i] > s->nst * s->r)
+      return fail(MB_ERR_INVALID, "%s: frame cap %d outside [1, %d]", me, row_steps[i], s->nst * s->r);
+  }
+  mb_tacotron* h = s->h;
+  const mb_tacotron_config& c = h->cfg;
+  cudaStream_t st = h->own_stream;
+  if (int rc = caller_to(s, (cudaStream_t)stream, st)) return rc;
+  bool half[2] = {false, false};
+  for (int i = 0; i < n; ++i) half[pool_row[i] / s->S] = true;
+  for (int q = 0; q < 2; ++q)  // the encoder rows this admission copies
+    if (half[q]) MB_CUDA_CHECK(cudaStreamWaitEvent(st, s->ev_enc[q], 0));
+  for (int i = 0; i < n; ++i) {
+    rows[i] = AdmitRow{slot[i], pool_row[i], row_chars[i], (row_steps[i] + s->r - 1) / s->r, row_seeds[i],
+                       dec_masks ? dec_masks[i] : nullptr};
+    s->occupant[slot[i]] = text_id[i];
+  }
+  AdmitRow* d_rows = reinterpret_cast<AdmitRow*>(s->base + s->L.admit_tab);
+  if (int rc = upload(d_rows, rows.data(), sizeof(AdmitRow) * n, st)) return rc;
+  const Ws& D = s->L.dec;
+  float* wd = s->wd;
+  const int Dd = c.decoder_dims, proj_dims = c.encoder_dims + c.speaker_embedding_size + c.gst_E, S = s->S;
+  AdmitArgs a;
+  memset(&a, 0, sizeof(a));
+  a.rows = d_rows;
+  a.start = s->global;
+  std::vector<mb_taco_stream_region> regs;
+  stream_regions(s, regs);
+  for (const mb_taco_stream_region& g : regs) {
+    if (!g.reset) continue;
+    if (a.nzero == kMaxZero) return fail(MB_ERR_STATE, "%s: more than %d regions to reset", me, kMaxZero);
+    char* p = reinterpret_cast<char*>(g.ptr);
+    if (g.kind == MB_TACO_REGION_TILE)  // the slot's 128 bytes in every k-block of a plane [K/64][rows_pad][64] halves
+      a.zero[a.nzero++] = RowZero{p, 128, (long long)g.rows * 128, (g.width + 63) / 64, 128};
+    else
+      a.zero[a.nzero++] = RowZero{p, (long long)g.width * 4, 0, 1, g.width * 4};
+  }
+  a.src_seq = reinterpret_cast<const float*>(s->base + s->L.pool_seq);
+  a.seq = wd + D.seq;
+  a.seq_row = (long long)s->Tc * proj_dims;
+  a.src_proj = reinterpret_cast<const float*>(s->base + s->L.pool_proj);
+  a.proj = wd + D.proj;
+  a.proj_row = (long long)s->Tc * Dd;
+  a.src_chars = reinterpret_cast<const int32_t*>(s->base + s->L.pool_chars);
+  a.chars = reinterpret_cast<int32_t*>(wd + D.ids);
+  a.Tc = s->Tc;
+  int32_t* drows = reinterpret_cast<int32_t*>(wd + D.rows);
+  a.lens = drows;
+  a.caps = drows + S;
+  a.done = drows + 2 * S;
+  a.starts = reinterpret_cast<int*>(s->base + s->L.start);
+  a.dmask = reinterpret_cast<uint8_t*>(wd + D.dmask);
+  a.S = S;
+  a.units = 2 * Dd;
+  admit_rows_kernel<<<dim3(16, n), 256, 0, st>>>(a);
+  MB_LAUNCH_CHECK("admit_rows_kernel");
+  MB_CUDA_CHECK(cudaEventRecord(s->ev_admit, st));
+  MB_CUDA_CHECK(cudaStreamWaitEvent((cudaStream_t)stream, s->ev_admit, 0));
+  return MB_OK;
+}
+
+int mb_tacotron_stream_run(mb_taco_stream* s, int32_t* n_done, int64_t* done_ids, int32_t* done_frames, int64_t* steps_run) {
+  const char* me = "mb_tacotron_stream_run";
+  if (int rc = stream_check(me, s)) return rc;
+  if (!n_done || !done_ids || !done_frames) return fail(MB_ERR_INVALID, "%s: null argument", me);
+  *n_done = 0;
+  const int S = s->S;
+  int busy = 0;
+  for (int b = 0; b < S; ++b) busy += s->occupant[b] >= 0;
+  cudaStream_t st = s->h->own_stream;
+  std::vector<int> fin;
+  while (busy && fin.empty()) {
+    for (int g = 0; g < kStreamPoll / kGraphSteps; ++g) {
+      if (cudaGraphLaunch(s->exec, st) != cudaSuccess) return fail(MB_ERR_CUDA, "%s: cudaGraphLaunch failed", me);
+      count_launch(s->per_graph + 1);
+    }
+    s->global += kStreamPoll;
+    s->steps_run += kStreamPoll;
+    MB_CUDA_CHECK(cudaMemcpyAsync(s->hdone.data(), s->d_done, sizeof(int32_t) * S, cudaMemcpyDeviceToHost, st));
+    MB_CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int b = 0; b < S; ++b)
+      if (s->occupant[b] >= 0 && s->hdone[b] >= 0) fin.push_back(b);
+  }
+  int nfree = 0;
+  for (int v : s->pool) nfree += v == 0;
+  if (nfree < (int)fin.size()) {  // rows a postnet still reads come back once it has finished
+    MB_CUDA_CHECK(cudaStreamWaitEvent(st, s->ev_post, 0));
+    for (int& v : s->pool)
+      if (v == 2) v = 0, ++nfree;
+  }
+  if (nfree < (int)fin.size())
+    return fail(MB_ERR_STATE, "%s: %zu finished rows wait for the postnet: harvest them first", me, s->pending.size());
+  const mb_tacotron_config& c = s->h->cfg;
+  const int NM = c.n_mels, r = s->r;
+  const Ws& D = s->L.dec;
+  float* pmel = reinterpret_cast<float*>(s->base + s->L.post_mel);
+  float* pattn = reinterpret_cast<float*>(s->base + s->L.post_attn);
+  int p = 0;
+  for (int b : fin) {
+    while (s->pool[p]) ++p;
+    const int steps = s->hdone[b] + 1;
+    MB_CUDA_CHECK(cudaMemcpyAsync(pmel + (size_t)p * s->nst * r * NM, s->wd + D.mel_all + (size_t)b * s->ring * r * NM,
+                                  sizeof(float) * steps * r * NM, cudaMemcpyDeviceToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(pattn + (size_t)p * s->nst * s->Tc, s->wd + D.scores_all + (size_t)b * s->ring * s->Tc,
+                                  sizeof(float) * steps * s->Tc, cudaMemcpyDeviceToDevice, st));
+    s->pool[p] = 1;
+    s->pool_id[p] = s->occupant[b];
+    s->pool_frames[p] = steps * r;
+    s->pending.push_back(p);
+    done_ids[*n_done] = s->occupant[b];
+    done_frames[*n_done] = steps * r;
+    ++*n_done;
+    s->occupant[b] = -1;
+  }
+  MB_CUDA_CHECK(cudaEventRecord(s->ev_copied, st));
+  if (steps_run) *steps_run = s->steps_run;
+  return MB_OK;
+}
+
+int mb_tacotron_stream_harvest(mb_taco_stream* s, int32_t n, int32_t frames, float* mel, float* linear, float* attn, void* stream) {
+  const char* me = "mb_tacotron_stream_harvest";
+  if (int rc = stream_check(me, s)) return rc;
+  if (!mel || !linear || !attn) return fail(MB_ERR_INVALID, "%s: null argument", me);
+  if (n < 1 || n > s->S || n > (int)s->pending.size())
+    return fail(MB_ERR_INVALID, "%s: %d rows (1 to %d, %zu finished)", me, n, s->S, s->pending.size());
+  std::vector<int32_t> flen(n);
+  int fmax = 0;
+  for (int i = 0; i < n; ++i) fmax = std::max(fmax, flen[i] = s->pool_frames[s->pending[i]]);
+  if (frames != fmax) return fail(MB_ERR_INVALID, "%s: frames %d, the longest of these rows has %d", me, frames, fmax);
+  mb_tacotron* h = s->h;
+  const mb_tacotron_config& c = h->cfg;
+  const int NM = c.n_mels, r = s->r, Tc = s->Tc;
+  cudaStream_t st = (cudaStream_t)stream;
+  MB_CUDA_CHECK(cudaStreamWaitEvent(st, s->ev_copied, 0));
+  const Ws& Lp = s->L.post;
+  float* wp = s->wp;
+  float* melc = wp + Lp.ppj2;
+  const float* pmel = reinterpret_cast<const float*>(s->base + s->L.post_mel);
+  const float* pattn = reinterpret_cast<const float*>(s->base + s->L.post_attn);
+  for (int i = 0; i < n; ++i) {
+    const int p = s->pending[i];
+    MB_CUDA_CHECK(cudaMemcpyAsync(melc + (size_t)i * frames * NM, pmel + (size_t)p * s->nst * r * NM, sizeof(float) * frames * NM,
+                                  cudaMemcpyDeviceToDevice, st));
+    MB_CUDA_CHECK(cudaMemcpyAsync(attn + (size_t)i * (frames / r) * Tc, pattn + (size_t)p * s->nst * Tc,
+                                  sizeof(float) * (frames / r) * Tc, cudaMemcpyDeviceToDevice, st));
+  }
+  int32_t* d_flen = reinterpret_cast<int32_t*>(s->base + s->L.post_flen);
+  if (int rc = upload(d_flen, flen.data(), sizeof(int32_t) * n, st)) return rc;
+  if (int rc = run_postnet(h, Lp, wp, melc, n, frames, d_flen, true, st)) return rc;
+  const size_t cnt = (size_t)n * NM * frames;
+  to_ncl_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, st>>>(melc, frames, mel, n, NM, frames);
+  MB_LAUNCH_CHECK("to_ncl_kernel");
+  to_ncl_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, st>>>(wp + Lp.lin, frames, linear, n, NM, frames);
+  MB_LAUNCH_CHECK("to_ncl_kernel");
+  MB_CUDA_CHECK(cudaEventRecord(s->ev_post, st));
+  for (int i = 0; i < n; ++i) s->pool[s->pending[i]] = 2;
+  s->pending.erase(s->pending.begin(), s->pending.begin() + n);
+  return MB_OK;
+}
+
+int32_t mb_tacotron_stream_regions(const mb_taco_stream* s, mb_taco_stream_region* out, int32_t max) {
+  if (!s || !s->h) return fail(MB_ERR_INVALID, "mb_tacotron_stream_regions: null stream");
+  std::vector<mb_taco_stream_region> regs;
+  stream_regions(s, regs);
+  for (int i = 0; out && i < max && i < (int)regs.size(); ++i) out[i] = regs[i];
+  return (int32_t)regs.size();
+}
+
+void mb_tacotron_stream_close(mb_taco_stream* s) {
+  if (!s) return;
+  if (s->h && s->h->own_stream) cudaStreamSynchronize(s->h->own_stream);
+  if (s->enc_st) cudaStreamSynchronize(s->enc_st);
+  if (s->ev_post) cudaEventSynchronize(s->ev_post);
+  delete s;
+}
+
+}  // extern "C"
+
 // ---- mb_taco_debug: one FP32 kernel of this path per call, launched as the forward launches it ----------------------------
 namespace {
 
@@ -1932,13 +2630,16 @@ int debug_check(const mb_taco_debug_spec& s) {
   const char* me = "mb_taco_debug";
   if (s.kind < MB_TACO_DBG_GEMM || s.kind > MB_TACO_DBG_FILL_MASKS_SEEDED) return fail(MB_ERR_INVALID, "%s: bad kind %d", me, s.kind);
   if ((s.row_done == nullptr) != (s.row_caps == nullptr)) return fail(MB_ERR_INVALID, "%s: row_done and row_caps go together", me);
+  if (s.row_start && s.ring < 1) return fail(MB_ERR_INVALID, "%s: row_start needs a ring of at least one step", me);
+  if (s.row_start && (s.kind == MB_TACO_DBG_STOP_STEP || s.kind == MB_TACO_DBG_STOP_FLAG) && (!s.row_done || s.out[0]))
+    return fail(MB_ERR_INVALID, "%s: with row_start the stop rule is per row (row_done, row_caps) and writes no flags", me);
   if (s.kind == MB_TACO_DBG_GEMM || s.kind == MB_TACO_DBG_STOP_STEP) {
     if (s.nseg < 1 || s.nseg > kMaxSeg || !s.W || !s.y || s.M <= 0 || s.N <= 0)
       return fail(MB_ERR_INVALID, "%s: GEMM nseg %d, M %d, N %d or a null operand", me, s.nseg, s.M, s.N);
     for (int j = 0; j < s.nseg; ++j)
       if (!s.x[j] || s.K[j] <= 0) return fail(MB_ERR_INVALID, "%s: segment %d empty", me, j);
-    if (s.kind == MB_TACO_DBG_STOP_STEP && (s.N != 1 || !s.out[0] || !s.out[1] || s.n[0] != s.M))
-      return fail(MB_ERR_INVALID, "%s: STOP_STEP needs N = 1, flags, ticket and B = M", me);
+    if (s.kind == MB_TACO_DBG_STOP_STEP && (s.N != 1 || (!s.out[0] && !s.row_start) || !s.out[1] || s.n[0] != s.M))
+      return fail(MB_ERR_INVALID, "%s: STOP_STEP needs N = 1, flags (unless row_start), ticket and B = M", me);
     return MB_OK;
   }
   for (int i = 0; i < 10; ++i)
@@ -2007,6 +2708,8 @@ int mb_taco_debug(const mb_taco_debug_spec* spec, void* workspace, size_t worksp
       pa.s_rows_pad = (int)n[8];
       pa.step_ptr = s.step_ptr;
       pa.step_j = s.step_j;
+      pa.row_start = s.row_start;
+      pa.ring = s.ring;
       TK(launch_prenet_fused(pa, st));
       info = {"prenet_fused", (pa.B + 3) / 4, 1, 512, 0};
       break;
@@ -2041,7 +2744,8 @@ int mb_taco_debug(const mb_taco_debug_spec* spec, void* workspace, size_t worksp
       MB_CUDA_CHECK(lsa_step_prepare(Tc));
       MB_CUDA_CHECK(launch_pdl2(lsa_step_kernel, dim3(B), dim3(threads), smem, st, fin(0), fin(1), fin(2), (int)n[2],
                                 reinterpret_cast<const int32_t*>(s.in[3]), fout(0), fin(4), fin(5), fin(6), fin(7), fout(1),
-                                (int)n[3], fout(2), Tc, s.step_ptr, s.step_j, fin(8), fin(9), fin(10), s.row_len));
+                                (int)n[3], fout(2), Tc, s.step_ptr, s.step_j, fin(8), fin(9), fin(10), s.row_len, s.row_start,
+                                s.ring));
       MB_LAUNCH_CHECK("lsa_step_kernel");
       info = {"lsa_step", B, 1, threads, smem};
       break;
@@ -2050,7 +2754,8 @@ int mb_taco_debug(const mb_taco_debug_spec* spec, void* workspace, size_t worksp
       const int B = (int)n[0], Tc = (int)n[1], seq_dim = (int)n[2];
       const size_t smem = sizeof(float) * Tc;
       MB_CUDA_CHECK(launch_pdl2(lsa_ctx_kernel, dim3(seq_dim / 256, B), dim3(256), smem, st, fin(0), (int)n[3], fin(1), seq_dim, Tc,
-                                fout(0), s.step_ptr, s.step_j, hout(1), hout(2), hout(3), hout(4), (int)n[4], s.row_len));
+                                fout(0), s.step_ptr, s.step_j, hout(1), hout(2), hout(3), hout(4), (int)n[4], s.row_len, s.row_start,
+                                s.ring));
       MB_LAUNCH_CHECK("lsa_ctx_kernel");
       info = {"lsa_ctx", seq_dim / 256, B, 256, smem};
       break;
@@ -2065,14 +2770,14 @@ int mb_taco_debug(const mb_taco_debug_spec* spec, void* workspace, size_t worksp
     case MB_TACO_DBG_STOP_STEP: {
       const int B = (int)n[0];
       stop_step_kernel<<<B, 256, 0, st>>>(debug_gemm_args(s), B, s.fval, (int)n[1], reinterpret_cast<int*>(s.out[0]), s.step_ptr,
-                                          s.step_j, reinterpret_cast<unsigned int*>(s.out[1]), s.row_done, s.row_caps);
+                                          s.step_j, reinterpret_cast<unsigned int*>(s.out[1]), s.row_done, s.row_caps, s.row_start);
       MB_LAUNCH_CHECK("stop_step_kernel");
       info = {"stop_step", B, 1, 256, 0};
       break;
     }
     case MB_TACO_DBG_STOP_FLAG:
       stop_flag_kernel<<<1, 32, 0, st>>>(fin(0), (int)n[0], s.fval, (int)n[1], reinterpret_cast<int*>(s.out[0]), s.step_ptr, s.step_j,
-                                         s.row_done, s.row_caps);
+                                         s.row_done, s.row_caps, s.row_start);
       MB_LAUNCH_CHECK("stop_flag_kernel");
       info = {"stop_flag", 1, 1, 32, 0};
       break;

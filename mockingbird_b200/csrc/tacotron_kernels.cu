@@ -430,7 +430,8 @@ constexpr int kPrenetOut = 8;      // outputs per warp and pass: 16 warps x 8 = 
 // in flight (8 outputs x 2 k: 12 dependent round trips per step instead of 22); the per-lane accumulation order (k = lane, lane + 32, ...) is that of the 4-output version.
 template <int KMAX>
 __device__ __forceinline__ void prenet_layer(const float* __restrict__ W, const float* __restrict__ bias, int K, int H,
-                                             const float (*in)[KMAX], const uint8_t* __restrict__ mask, int b0, int B, int warp, int lane,
+                                             const float (*in)[KMAX], const uint8_t* __restrict__ mask, const long long* moff, int b0,
+                                             int B, int warp, int lane,
                                              float (*out_s)[256], float* out_g, int ldy, __half* s_hi = nullptr,
                                              __half* s_lo = nullptr, int s_k0 = 0, int s_rows_pad = 0) {
   for (int n0 = warp * kPrenetOut; n0 < H; n0 += kPrenetWarps * kPrenetOut) {
@@ -481,7 +482,7 @@ __device__ __forceinline__ void prenet_layer(const float* __restrict__ W, const 
       if (n < H) {
         v += bias[n];
         v = v > 0.f ? v : 0.f;
-        if (b < B) v = mask[(size_t)b * H + n] ? v * 2.f : 0.f;
+        if (b < B) v = mask[(moff ? moff[r] : 0) + (long long)b * H + n] ? v * 2.f : 0.f;
         if (out_s) out_s[r][n] = v;
         if (out_g && b < B) out_g[(size_t)b * ldy + n] = v;
         if (s_hi && b < B) store_split_scalar(v, b, s_rows_pad, s_k0 + n, s_hi, s_lo);
@@ -496,24 +497,38 @@ __global__ void __launch_bounds__(32 * kPrenetWarps) prenet_fused_kernel(const P
   const int b0 = blockIdx.x * kPrenetRows;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int si = step_index(a.step_ptr, a.step_j);
+  // with a per-row step origin each row reads at its own step (row_step): the go frame at its step 0, else the last frame of its
+  // previous step, and the masks of its step; without one every row is at step si
+  const bool per_row = a.row_start != nullptr;
+  __shared__ long long moff[kPrenetRows];
+  if (per_row && threadIdx.x < kPrenetRows) {
+    const int b = b0 + threadIdx.x;
+    moff[threadIdx.x] = b < a.B ? (long long)ring_slot(row_step(si, a.row_start, b), a.row_start, a.ring) * a.mask_step : 0;
+  }
   const bool go = (si == 0 && a.x_first != nullptr);
   for (int i = threadIdx.x; i < kPrenetRows * a.K; i += blockDim.x) {
     const int r = i / a.K, k = i - r * a.K;
     const int b = b0 + r;
     float v = 0.f;
-    if (b < a.B) v = go ? a.x_first[k] : a.x[(long long)b * a.x_ld + (long long)si * a.x_step + k];
+    if (b < a.B && !per_row) {
+      v = go ? a.x_first[k] : a.x[(long long)b * a.x_ld + (long long)si * a.x_step + k];
+    } else if (b < a.B) {
+      const int s = row_step(si, a.row_start, b);
+      // x + s * x_step is frame s * r - 1; in a ring, step s - 1's frames sit at slot (s - 1) % ring
+      v = (s == 0 && a.x_first != nullptr) ? a.x_first[k] : a.x[(long long)b * a.x_ld + ((long long)((s - 1) % a.ring) + 1) * a.x_step + k];
+    }
     xs[r][k] = v;
   }
   __syncthreads();
-  const uint8_t* m1 = a.m1 + (size_t)si * (size_t)a.mask_step;
-  const uint8_t* m2 = a.m2 + (size_t)si * (size_t)a.mask_step;
-  prenet_layer<128>(a.W1, a.b1, a.K, a.H, xs, m1, b0, a.B, warp, lane, hs, nullptr, 0);
+  const uint8_t* m1 = per_row ? a.m1 : a.m1 + (size_t)si * (size_t)a.mask_step;
+  const uint8_t* m2 = per_row ? a.m2 : a.m2 + (size_t)si * (size_t)a.mask_step;
+  prenet_layer<128>(a.W1, a.b1, a.K, a.H, xs, m1, per_row ? moff : nullptr, b0, a.B, warp, lane, hs, nullptr, 0);
   __syncthreads();
-  prenet_layer<256>(a.W2, a.b2, a.H, a.H, hs, m2, b0, a.B, warp, lane, nullptr, a.y, a.ldy, a.s_hi, a.s_lo, a.s_k0, a.s_rows_pad);
+  prenet_layer<256>(a.W2, a.b2, a.H, a.H, hs, m2, per_row ? moff : nullptr, b0, a.B, warp, lane, nullptr, a.y, a.ldy, a.s_hi, a.s_lo, a.s_k0, a.s_rows_pad);
 }
 
 cudaError_t launch_prenet_fused(const PrenetArgs& a, cudaStream_t st) {
-  if (a.K > 128 || a.H > 256 || a.B <= 0) return cudaErrorInvalidValue;
+  if (a.K > 128 || a.H > 256 || a.B <= 0 || (a.row_start && a.ring <= 0)) return cudaErrorInvalidValue;
   prenet_fused_kernel<<<(a.B + kPrenetRows - 1) / kPrenetRows, 32 * kPrenetWarps, 0, st>>>(a);
   return cudaGetLastError();
 }

@@ -87,6 +87,13 @@ struct GemmArgs {
 
 __device__ __forceinline__ int step_index(const int* step_ptr, int step_j) { return (step_ptr ? *step_ptr : 0) + step_j; }
 
+// Per-row step origin (streamed decoding, mb_tacotron_stream_*): row m entered the loop at global step row_start[m], so its own
+// decoder step is the global step minus that start, and what a step writes for the row lands at that step modulo `ring` in the
+// row's per-step buffers.  row_start == nullptr: every row's step is the global step and the buffers are indexed by it directly
+// (padded and ragged batches, whose buffers hold every step).
+__device__ __forceinline__ int row_step(int si, const int* row_start, int m) { return row_start ? si - row_start[m] : si; }
+__device__ __forceinline__ int ring_slot(int s, const int* row_start, int ring) { return row_start ? s % ring : s; }
+
 // which kernel launch_gemm chose and its launch shape (filled when asked; mb_taco_debug reports it)
 struct GemmLaunchInfo {
   const char* kernel;
@@ -117,6 +124,8 @@ struct PrenetArgs {
   __half* s_hi;            // optional: y also goes, split into fp16 hi / lo, into the operand tiles of the next tensor-core GEMM
   __half* s_lo;            //   (columns [s_k0, s_k0 + H) of tiles [KB][s_rows_pad][64], the layout of launch_act_split)
   int s_k0, s_rows_pad;
+  const int* row_start;    // optional per-row step origin (row_step / ring_slot): x and the masks are read at the row's own step
+  int ring;                //   modulo `ring` steps, the go frame at its step 0
 };
 cudaError_t launch_prenet_fused(const PrenetArgs& a, cudaStream_t st);
 
@@ -166,6 +175,8 @@ struct TcSkinnyArgs {
   const float* pre;
   int ldpre;
   int compact;          // set by launch_tc_skinny: 8 KB activation slots, 8-stage ring (rows_pad == 64)
+  const int* row_start; // optional TCS_PLAIN per-row step origin: row m writes at y + ring_slot(row_step(step, row_start, m)) * y_step
+  int ring;
 };
 // one recurrent GRU step for 1 or 2 directions (blockIdx.y); pointers per direction
 struct TcGruArgs {

@@ -261,7 +261,8 @@ __global__ void __launch_bounds__(kThreads, 1) tc_skinny_kernel(const __grid_con
       if (p.s_hi[0]) store_split_chunk(xn, m, p.rows_pad, p.s_k0[0] + tile * 8, p.s_hi[0], p.s_lo[0]);
       if (p.s_hi[1]) store_split_chunk(hn, m, p.rows_pad, p.s_k0[1] + tile * 8, p.s_hi[1], p.s_lo[1]);
     } else {
-      float* y = p.y + (long long)step_index(p.step_ptr, p.step_j) * p.y_step + (size_t)m * p.ldy + (size_t)tile * 32;
+      const int sm = row_step(step_index(p.step_ptr, p.step_j), p.row_start, m);
+      float* y = p.y + (long long)ring_slot(sm, p.row_start, p.ring) * p.y_step + (size_t)m * p.ldy + (size_t)tile * 32;
 #pragma unroll
       for (int i = 0; i < 32; i += 4) {
         if (tile * 32 + i < p.N) *reinterpret_cast<float4*>(y + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
@@ -682,7 +683,7 @@ cudaError_t launch_tc_gru(const TcGruArgs& a, cudaStream_t st, int pdl, TcLaunch
 cudaError_t launch_tc_gru(const TcGruArgs& a, cudaStream_t st) { return launch_tc_gru(a, st, -1); }
 
 cudaError_t launch_tc_skinny(const TcSkinnyArgs& a, cudaStream_t st, int ring8, int mc, int pdl, TcLaunchInfo* info) {
-  if (a.M <= 0 || a.M > 128 || a.N <= 0 || a.KB <= 0) return cudaErrorInvalidValue;
+  if (a.M <= 0 || a.M > 128 || a.N <= 0 || a.KB <= 0 || (a.row_start && a.ring <= 0)) return cudaErrorInvalidValue;
   TcSkinnyArgs p = a;
   p.rows_pad = a.M <= 64 ? 64 : 128;
   p.compact = (ring8 && p.rows_pad == 64) ? 1 : 0;

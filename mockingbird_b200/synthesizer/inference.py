@@ -105,6 +105,32 @@ class Synthesizer:
             alignments.append(attn.cpu().numpy())
         return (specs, alignments) if return_alignments else specs
 
+    def synthesize_spectrograms_stream(self, texts: List[str], embeddings: Union[np.ndarray, List[np.ndarray]], style_idx=0,
+                                       min_stop_token=5, steps=2000, seeds=None, slots=128):
+        """synthesize_spectrograms_many as an iterator that yields each text's spectrogram as soon as it is done
+        (Tacotron.generate_stream): ``(i, [80, f_i] host array)`` in the order the texts finish, each equal to
+        synthesize_spectrograms_many's i-th.  Same text front-end, postnet output and trailing trim."""
+        if not self.is_loaded():
+            self.load()
+        if lazy_pinyin is not None:
+            texts = [" ".join(lazy_pinyin(v, style=Style.TONE3, neutral_tone_with_five=True)) for v in texts]
+        inputs = [text_to_sequence(text, hparams.tts_cleaner_names) for text in texts]
+        emb = np.stack([np.asarray(e, dtype=np.float32) for e in embeddings]) if len(embeddings) else np.zeros((0, 256), np.float32)
+        if emb.shape[0] != len(inputs):
+            raise ValueError(f"{emb.shape[0]} speaker embeddings for {len(inputs)} texts")
+        outs = self._model.generate_stream(inputs, torch.from_numpy(emb), steps=steps, style_idx=style_idx,
+                                           min_stop_token=min_stop_token, seeds=seeds, slots=slots)
+        return self._trimmed(outs)
+
+    @staticmethod
+    def _trimmed(outs):
+        for i, _, lin, _ in outs:
+            m = lin.cpu().numpy()
+            # Trim silence from end of each spectrogram (inference.py:135-138)
+            while m.shape[1] > 0 and np.max(m[:, -1]) < hparams.tts_stop_threshold:
+                m = m[:, :-1]
+            yield i, m
+
     @staticmethod
     def load_preprocess_wav(fpath):
         """inference.py:143-158 (host utility): load at the synthesizer rate and rescale.  The reference additionally

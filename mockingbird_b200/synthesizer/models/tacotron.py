@@ -33,6 +33,54 @@ def many_plan(lengths, chunk_rows):
     return [order[k:k + int(chunk_rows)] for k in range(0, len(order), int(chunk_rows))]
 
 
+class StreamSchedule:
+    """The host side of ``Tacotron.generate_stream``: which text enters which slot, and when each batch of texts is encoded.
+
+    Texts are admitted longest first, ties in input order (``many_plan``'s order), each into the lowest free slot.  They are
+    encoded in batches of ``slots`` texts in that order into a staging pool of two halves of ``slots`` rows: batch k goes to
+    half k % 2, so it can be encoded once every text of batch k - 2 has been admitted."""
+
+    def __init__(self, lengths, slots):
+        if not 1 <= int(slots) <= 128:
+            raise ValueError(f"slots must be in [1, 128], got {slots}")
+        self.slots = int(slots)
+        self.order = [i for chunk in many_plan(lengths, self.slots) for i in chunk]
+        self.batches = [self.order[k:k + self.slots] for k in range(0, len(self.order), self.slots)]
+        self.free = list(range(self.slots))
+        self.pos = 0      # texts admitted so far (a position in `order`)
+        self.encoded = 0  # batches handed to the encoder so far
+
+    def pool_row(self, q):
+        """staging-pool row of the text at position q of the admission order"""
+        return (q // self.slots) % 2 * self.slots + q % self.slots
+
+    def to_encode(self):
+        """batches whose pool half is free now: list of (pool row of the first text, texts)"""
+        out = []
+        while self.encoded < len(self.batches) and self.pos >= (self.encoded - 1) * self.slots:
+            out.append((self.pool_row(self.encoded * self.slots), self.batches[self.encoded]))
+            self.encoded += 1
+        return out
+
+    def admit(self):
+        """texts for the free slots: list of (slot, text, pool row); only texts whose batch has been encoded"""
+        out = []
+        self.free.sort(reverse=True)
+        while self.free and self.pos < len(self.order) and self.pos // self.slots < self.encoded:
+            out.append((self.free.pop(), self.order[self.pos], self.pool_row(self.pos)))
+            self.pos += 1
+        return out
+
+    def finish(self, slot):
+        self.free.append(int(slot))
+
+    def busy(self):
+        return self.slots - len(self.free)
+
+    def done(self):
+        return self.pos == len(self.order) and not self.busy()
+
+
 class Tacotron:
     def __init__(self, embed_dims, num_chars, encoder_dims, decoder_dims, n_mels, fft_bins, postnet_dims, encoder_K,
                  lstm_dims, postnet_K, num_highways, dropout, stop_threshold, speaker_embedding_size):
@@ -197,21 +245,10 @@ class Tacotron:
         attn = attn[: B * (f // r) * Tc].view(B, f // r, Tc)
         return mel, lin, attn
 
-    def generate_many(self, seqs, speaker_embeddings, steps=2000, style_idx=0, min_stop_token=5, seeds=None,
-                      dropout_masks=None, chunk_rows=None):
-        """Many texts, each computed as its own B = 1 ``generate`` -> list of N ``(mel [80, f_i], linear [80, f_i],
-        attn [f_i / r, Tc_i])`` device tensors in input order.
-
-        ``seqs``: N unpadded int sequences; ``speaker_embeddings`` [N, 256]; ``steps``: one frame cap or N of them.  Each
-        utterance stops at its own stop rule or cap.  Utterances are sorted longest first and run in ragged batches of at
-        most ``chunk_rows`` (default ``MANY_CHUNK_ROWS``) rows; a result is bitwise the same whatever the list around it.
-        Dropout is drawn from ``seeds[i]`` (default ``self.seed + i``) or injected per utterance as
-        ``dropout_masks = (enc, dec)`` with enc[i] [2, Tc_i, 256] and dec[i] [>= ceil(steps_i / r), 2, 256]."""
-        self.eval()
+    def _many_args(self, seqs, speaker_embeddings, steps, seeds, dropout_masks):
+        """generate_many's argument checks -> (int32 rows, speaker embeddings [N, 256], frame caps, seeds)"""
         N = len(seqs)
         rows = [torch.as_tensor(s).reshape(-1).to(torch.int32) for s in seqs]
-        if N == 0:
-            return []
         L = _lib.lib()
         with torch.cuda.device(self._device or _lib.require_cuda()):
             max_chars = int(L.mb_tacotron_max_chars())
@@ -243,6 +280,28 @@ class Tacotron:
                 nst_i = -(-caps[i] // r)
                 if enc_l[i].dim() != 3 or dec_l[i].dim() != 3 or dec_l[i].shape[0] < nst_i or tuple(dec_l[i].shape[1:]) != (2, D2):
                     raise ValueError(f"decoder mask {i} has shape {tuple(dec_l[i].shape)}, expected ({nst_i}, 2, {D2})")
+        return rows, spk_all, caps, seeds
+
+    def generate_many(self, seqs, speaker_embeddings, steps=2000, style_idx=0, min_stop_token=5, seeds=None,
+                      dropout_masks=None, chunk_rows=None):
+        """Many texts, each computed as its own B = 1 ``generate`` -> list of N ``(mel [80, f_i], linear [80, f_i],
+        attn [f_i / r, Tc_i])`` device tensors in input order.
+
+        ``seqs``: N unpadded int sequences; ``speaker_embeddings`` [N, 256]; ``steps``: one frame cap or N of them.  Each
+        utterance stops at its own stop rule or cap.  Utterances are sorted longest first and run in ragged batches of at
+        most ``chunk_rows`` (default ``MANY_CHUNK_ROWS``) rows; a result is bitwise the same whatever the list around it.
+        Dropout is drawn from ``seeds[i]`` (default ``self.seed + i``) or injected per utterance as
+        ``dropout_masks = (enc, dec)`` with enc[i] [2, Tc_i, 256] and dec[i] [>= ceil(steps_i / r), 2, 256]."""
+        self.eval()
+        N = len(seqs)
+        if N == 0:
+            return []
+        rows, spk_all, caps, seeds = self._many_args(seqs, speaker_embeddings, steps, seeds, dropout_masks)
+        L = _lib.lib()
+        r = self._r
+        E, D2 = self.encoder_dims, 2 * self.decoder_dims
+        if dropout_masks is not None:
+            enc_l, dec_l = dropout_masks
         if not self._ready:
             self._upload()
         dev = self._device
@@ -294,6 +353,132 @@ class Tacotron:
                 f = row_frames[b]
                 out[i] = (mel[b, :, :f].clone(), lin[b, :, :f].clone(), attn[b, : f // r, : lens[b]].clone())
         return out
+
+    def generate_stream(self, seqs, speaker_embeddings, steps=2000, style_idx=0, min_stop_token=5, seeds=None,
+                        dropout_masks=None, slots=MANY_CHUNK_ROWS):
+        """Many texts through one decoder loop of ``slots`` rows (1..128): a text enters a free row as soon as one is free,
+        and its result comes back as soon as its postnet has run -> iterator of ``(i, mel [80, f_i], linear [80, f_i],
+        attn [f_i / r, Tc_i])`` device tensors in the order the texts finish, each bitwise what ``generate_many`` returns for
+        text i.  Same arguments and checks as ``generate_many`` (checked before this returns).  Texts are admitted longest
+        first, ties in input order, and encoded a batch of ``slots`` ahead on a stream of their own; the postnet runs on
+        another stream over every row that finished since the previous postnet started.  Stopping early is allowed: the
+        model stays usable.  ``self.stream_steps`` holds the decoder steps the loop has run."""
+        self.eval()
+        if not 1 <= int(slots) <= 128:
+            raise ValueError(f"slots must be in [1, 128], got {slots}")
+        N = len(seqs)
+        if N == 0:
+            return iter(())
+        rows, spk_all, caps, seeds = self._many_args(seqs, speaker_embeddings, steps, seeds, dropout_masks)
+        if not self._ready:
+            self._upload()
+        return self._stream(rows, spk_all, caps, seeds, int(style_idx), float(min_stop_token), dropout_masks, int(slots))
+
+    def _stream(self, rows, spk_all, caps, seeds, style_idx, min_stop_token, dropout_masks, slots):
+        L = _lib.lib()
+        dev = self._device
+        r, E = self._r, self.encoder_dims
+        N = len(rows)
+        lens = [s.numel() for s in rows]
+        Tc, max_steps = max(lens), max(caps)
+        sched = StreamSchedule(lens, slots)
+        dec = None
+        if dropout_masks is not None:  # each text's decoder masks for its steps, on the device while it may be admitted
+            dec = [dropout_masks[1][i][: -(-caps[i] // r)].to(device=dev, dtype=torch.uint8).contiguous() for i in range(N)]
+        with torch.cuda.device(dev):
+            need = int(L.mb_tacotron_stream_workspace_bytes(self._handle, slots, Tc, max_steps, r))
+            if need == 0:
+                raise ValueError(f"no stream of {slots} rows for texts of {Tc} characters and {max_steps} frames")
+            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            cur = torch.cuda.current_stream(dev)
+            post = torch.cuda.Stream(dev)
+            post.wait_stream(cur)
+            handle = C.c_void_p()
+            _lib.check(L.mb_tacotron_stream_open(self._handle, slots, Tc, max_steps, r, style_idx, C.c_float(min_stop_token),
+                                                 C.c_void_p(ws.data_ptr()), need, C.c_void_p(cur.cuda_stream), C.byref(handle)))
+        keep = []          # device inputs of calls that may still be running (released at close)
+        finished = []      # (text, frames) of rows run() reported and no postnet has taken yet
+        flights = []       # postnets launched: (event, [(text, frames)], mel, linear, attn)
+        slot_of = {}       # text -> slot while it decodes
+        n_done = C.c_int32(0)
+        ids = (C.c_int64 * slots)()
+        frames = (C.c_int32 * slots)()
+        steps_run = C.c_int64(0)
+        self.stream_steps = 0
+        try:
+            while not sched.done() or finished or flights:
+                with torch.cuda.device(dev):
+                    for row0, batch in sched.to_encode():
+                        n = len(batch)
+                        chars = torch.zeros(n, Tc, dtype=torch.int32)
+                        for b, i in enumerate(batch):
+                            chars[b, : lens[i]] = rows[i]
+                        chars = chars.to(dev)
+                        spk = spk_all[batch].to(dev).contiguous()
+                        enc_p = None
+                        if dropout_masks is not None:
+                            enc_m = torch.zeros(2, n, Tc, E, dtype=torch.uint8)
+                            for b, i in enumerate(batch):
+                                enc_m[:, b, : lens[i]] = dropout_masks[0][i].to(torch.uint8)
+                            enc_m = enc_m.to(dev)
+                            keep.append(enc_m)
+                            enc_p = C.c_void_p(enc_m.data_ptr())
+                        keep += [chars, spk]
+                        _lib.check(L.mb_tacotron_stream_encode(
+                            handle, row0, n, C.c_void_p(chars.data_ptr()), C.c_void_p(spk.data_ptr()),
+                            (C.c_int32 * n)(*[lens[i] for i in batch]),
+                            (C.c_uint64 * n)(*[seeds[i] & 0xFFFFFFFFFFFFFFFF for i in batch]), enc_p, C.c_void_p(cur.cuda_stream)))
+                    adm = sched.admit()
+                    if adm:
+                        n = len(adm)
+                        masks = None
+                        if dec is not None:
+                            masks = (C.c_void_p * n)(*[dec[i].data_ptr() for _, i, _ in adm])
+                        _lib.check(L.mb_tacotron_stream_admit(
+                            handle, n, (C.c_int32 * n)(*[s for s, _, _ in adm]), (C.c_int32 * n)(*[p for _, _, p in adm]),
+                            (C.c_int64 * n)(*[i for _, i, _ in adm]), (C.c_int32 * n)(*[lens[i] for _, i, _ in adm]),
+                            (C.c_int32 * n)(*[caps[i] for _, i, _ in adm]),
+                            (C.c_uint64 * n)(*[seeds[i] & 0xFFFFFFFFFFFFFFFF for _, i, _ in adm]), masks,
+                            C.c_void_p(cur.cuda_stream)))
+                        for slot, i, _ in adm:
+                            slot_of[i] = slot
+                    if sched.busy():
+                        _lib.check(L.mb_tacotron_stream_run(handle, C.byref(n_done), ids, frames, C.byref(steps_run)))
+                        self.stream_steps = steps_run.value
+                        for k in range(n_done.value):
+                            finished.append((int(ids[k]), int(frames[k])))
+                            sched.finish(slot_of.pop(int(ids[k])))
+                    # one postnet over every row finished since the previous one started, once that one is done (or when
+                    # nothing else is left to overlap with, or the finished rows would fill their pool)
+                    idle = not flights or flights[-1][0].query()
+                    if finished and (idle or len(finished) >= slots or sched.done()):
+                        take, finished = finished[:slots], finished[slots:]
+                        F = max(f for _, f in take)
+                        n = len(take)
+                        with torch.cuda.stream(post):
+                            mel = torch.empty(n, self.n_mels, F, dtype=torch.float32, device=dev)
+                            lin = torch.empty(n, self.n_mels, F, dtype=torch.float32, device=dev)
+                            att = torch.empty(n, F // r, Tc, dtype=torch.float32, device=dev)
+                        _lib.check(L.mb_tacotron_stream_harvest(handle, n, F, C.c_void_p(mel.data_ptr()),
+                                                                C.c_void_p(lin.data_ptr()), C.c_void_p(att.data_ptr()),
+                                                                C.c_void_p(post.cuda_stream)))
+                        ev = torch.cuda.Event()
+                        ev.record(post)
+                        flights.append((ev, take, mel, lin, att))
+                    ready = []
+                    while flights and (flights[0][0].query() or (sched.done() and not finished)):
+                        ev, take, mel, lin, att = flights.pop(0)
+                        ev.synchronize()
+                        cur.wait_event(ev)
+                        for t in (mel, lin, att):
+                            t.record_stream(cur)
+                        for b, (i, f) in enumerate(take):
+                            ready.append((i, mel[b, :, :f].clone(), lin[b, :, :f].clone(), att[b, : f // r, : lens[i]].clone()))
+                yield from ready
+        finally:
+            with torch.cuda.device(dev):
+                L.mb_tacotron_stream_close(handle)
+                cur.wait_stream(post)
 
     def __del__(self):
         try:

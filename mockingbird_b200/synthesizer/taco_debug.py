@@ -21,10 +21,12 @@ def taco_debug(kind: str, *, segs: Sequence[dict] = (), W=None, ldw: int = 0, bi
                act: int = 0, bn_scale=None, bn_shift=None, mask=None, res=None, ldres: int = 0, y=None, ldy: int = 0,
                step_mode: int = 0, step_ptr=None, step_j: int = 0, x_step: int = 0, x_first=None, mask_step: int = 0,
                ins: Sequence = (), outs: Sequence = (), n: Sequence[int] = (), fval: float = 0.0, seed: int = 0,
-               row_len=None, row_done=None, row_caps=None, row_seeds=None, fma_chain: int = 0, stream=None) -> str:
+               row_len=None, row_done=None, row_caps=None, row_seeds=None, fma_chain: int = 0, row_start=None, ring: int = 0,
+               stream=None) -> str:
     """Enqueues one launch, synchronises and returns the report line.  `segs`: GemmArgs segments as dicts with keys
     x, K, ld, shift, w_off, w_stride (x may be an int device address, e.g. a pointer offset by one float).  row_len,
-    row_done, row_caps (int32) and row_seeds (int64 holding the uint64 seeds) are the per-row arrays of ragged batches."""
+    row_done, row_caps (int32) and row_seeds (int64 holding the uint64 seeds) are the per-row arrays of ragged batches;
+    row_start (int32) and ring the per-row step origin of streamed decoding."""
     s = _lib.TacoDebugSpec()
     s.kind = _lib.MB_TACO_DBG[kind]
     s.nseg = len(segs)
@@ -45,6 +47,7 @@ def taco_debug(kind: str, *, segs: Sequence[dict] = (), W=None, ldw: int = 0, bi
     s.fval, s.seed = fval, seed
     s.row_len, s.row_done, s.row_caps, s.row_seeds = _p(row_len), _p(row_done), _p(row_caps), _p(row_seeds)
     s.fma_chain = fma_chain
+    s.row_start, s.ring = _p(row_start), ring
     lib = _lib.lib()
     need = lib.mb_taco_debug_workspace_bytes(C.byref(s))
     if need == 0:

@@ -29,7 +29,8 @@ def tc_debug(kind: str, *, M: int, N: int = 0, H: int = 0, K0: int = 0, K1: int 
              gi: Sequence[Optional[torch.Tensor]] = (), ldgi: int = 0, hst: Sequence = (), out: Sequence = (), ldout: int = 0,
              ndir: int = 1, s_hi: Sequence = (), s_lo: Sequence = (), s_k0: Sequence[int] = (), nxt_hi: Sequence = (),
              nxt_lo: Sequence = (), act: int = 0, bn_scale=None, bn_shift=None, res=None, ldres: int = 0, compact: int = -1,
-             cluster: int = 0, pdl: int = -1, a_tiles=None, w_tiles=None, len=None, t1: int = 0, stream=None) -> str:
+             cluster: int = 0, pdl: int = -1, a_tiles=None, w_tiles=None, len=None, t1: int = 0, row_start=None, ring: int = 0,
+             stream=None) -> str:
     """Runs one launch (synchronising the stream) and returns the report line.  Pointers are taken as given: sub-views such as
     strided gi / out slices pass their base pointer with the row stride in ld*.  `len` (int32, device): valid length of each
     sequence (big) or row (gru, with `t1` the backward direction's time index) of a ragged batch."""
@@ -58,6 +59,7 @@ def tc_debug(kind: str, *, M: int, N: int = 0, H: int = 0, K0: int = 0, K1: int 
     s.compact, s.cluster, s.pdl = compact, cluster, pdl
     s.a_tiles, s.w_tiles = _p(a_tiles), _p(w_tiles)
     s.len, s.t1 = _p(len), t1
+    s.row_start, s.ring = _p(row_start), ring  # PLAIN: per-row step origin (int32 device [M])
     lib = _lib.lib()
     need = lib.mb_taco_tc_debug_workspace_bytes(C.byref(s))
     if need == 0:
