@@ -876,6 +876,48 @@ int mb_logmmse_denoise(mb_logmmse* h, const float* x, const int32_t* lengths_hos
 /* E1(x) = expint(1, x) for x > 0, the device function the gains use: x, y float64 [n] (device) */
 int mb_logmmse_exp1(const double* x, double* y, int64_t n, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Harvest F0 tracking (DESIGN.md section 4n; csrc/f0.cu)
+ *   replaces  pyworld.harvest(wav, 16000, frame_period=10, f0_floor=80, f0_ceil=600), as utils/f0_utils.py:14-20
+ *             (compute_f0) calls it
+ * The contract is oracle/harvest_oracle.py: 16 kHz float64 input decimated by 2, 128 band-pass channels, events and
+ * official candidates per 1 ms frame, refinement, FixStep1-4 and smoothing, then every 10th frame.  All float64.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct mb_f0 mb_f0;
+
+/* Optional outputs for tests, per 1 ms frame of every clip back to back (T_b = int(1000 L_b / 16000) + 1 frames); any
+ * member may be NULL:
+ *   raw_count int32 [sum T_b]: channels with a raw candidate
+ *   official_count int32 [sum T_b]: official candidates of the frame itself
+ *   refined, scores float64 [sum T_b][91]: slot s < 7 nc_b (nc_b the clip's largest official count) after refinement,
+ *     before the unreliable-candidate removal; 0 in the other slots
+ *   contour float64 [sum T_b]: after FixStep4, before smoothing */
+typedef struct mb_f0_debug {
+  int32_t* raw_count;
+  int32_t* official_count;
+  double* refined;
+  double* scores;
+  double* contour;
+} mb_f0_debug;
+
+int mb_f0_create(mb_f0** out);
+void mb_f0_destroy(mb_f0* h);
+/* the handle holds no checkpoint tensor: its arena is the channel table, the band-pass taps and the DFT twiddles (float64,
+ * computed on the host at create), which finalize writes and then synchronises `stream` */
+size_t mb_f0_arena_bytes(const mb_f0* h);
+int mb_f0_set_arena(mb_f0* h, void* arena, size_t bytes);
+int mb_f0_finalize(mb_f0* h, void* stream);
+/* lengths_host int32 [batch] (host); 0 when batch < 1 or a length is outside 1 .. 2^28.  About 8 MB per second of audio. */
+size_t mb_f0_workspace_bytes(const mb_f0* h, int32_t batch, const int32_t* lengths_host);
+/* Harvest of `batch` clips in one sequence of five launches:
+ *   x float64: the 16 kHz clips back to back (device), lengths_host[b] samples each (host)
+ *   f0_out float64 [sum_b int(L_b / 160) + 1] (device): each clip's F0 every 10 ms, 0 where unvoiced
+ * Each clip's outputs are bitwise what a batch of that clip alone gives.  MB_ERR_INVALID before anything is queued for an
+ * empty clip or one longer than 2^28 samples; the message names the clip.  The clip table is copied from pageable host
+ * memory into the workspace. */
+int mb_f0_harvest(mb_f0* h, const double* x, const int32_t* lengths_host, int32_t batch, double* f0_out,
+                  const mb_f0_debug* debug, void* workspace, size_t workspace_bytes, void* stream);
+
 /* The shared Stockham FFT of Griffin-Lim and log-MMSE (csrc/mb_fft.cuh) on its own, for tests: y[r] = sum_j x[r][j]
  * exp(-+2 pi i j k / n) for each of `rows` rows of n complex points, unscaled in both directions, over the handles' twiddle
  * table.  x, y [rows][n] (device) of float2 (dtype 0) or double2 (dtype 1); inverse != 0 takes the + sign.  n is 2^a or 5 * 2^a

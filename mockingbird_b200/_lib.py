@@ -223,6 +223,11 @@ class LogMmseConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("window_size", "len1", "len2", "n_fft")]
 
 
+class F0Debug(C.Structure):
+    _fields_ = [("raw_count", C.c_void_p), ("official_count", C.c_void_p), ("refined", C.c_void_p), ("scores", C.c_void_p),
+                ("contour", C.c_void_p)]
+
+
 class VitsConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("n_vocab", "inter_channels", "hidden_channels", "filter_channels", "n_heads", "n_layers",
                                          "kernel_size", "resblock_type", "num_kernels")] + [
@@ -402,6 +407,14 @@ SIGNATURES = {
     "mb_logmmse_denoise": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p,
                                      C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_logmmse_exp1": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "mb_f0_create": (C.c_int, [C.POINTER(C.c_void_p)]),
+    "mb_f0_destroy": (None, [C.c_void_p]),
+    "mb_f0_arena_bytes": (C.c_size_t, [C.c_void_p]),
+    "mb_f0_set_arena": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "mb_f0_finalize": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "mb_f0_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]),
+    "mb_f0_harvest": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.POINTER(F0Debug),
+                                C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_fft_debug": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "mb_resample_create": (C.c_int, [C.c_int32, C.POINTER(C.c_void_p)]),
     "mb_resample_destroy": (None, [C.c_void_p]),
