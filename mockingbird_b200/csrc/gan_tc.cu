@@ -71,6 +71,8 @@ struct TcParams {
   int y_nchunks, y_cw, y_c0;           // fp16 destination plane: row chunks per utterance, channels per row chunk, first channel
                                        // this launch writes
   int y_lo_c;                          // >= 0: hi/lo destination plane - lo = fp16(v - fp16(v)) goes to channel + y_lo_c
+  int res_win;                         // fused pair whose res16 plane is its x16 plane: the residual rows are read from the item's
+                                       // operand window in shared memory instead of global memory
   int x_pchunks;                       // 64-channel chunks of the INPUT plane per utterance (K-chunk c reads chunk c % x_pchunks)
   float acc_scale;                     // accumulator -> value (1, or 1/kX3WScale for 3-term-split layers)
   float out_slope;
@@ -132,7 +134,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(const __grid_con
   if (threadIdx.x == 0) {
     for (int i = 0; i < kAStages; ++i) {
       mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], kMmaGroups);
+      mbar_init(&a_empty[i], p.res_win ? 4 * kMmaGroups : kMmaGroups);  // res_win: every MMA warp releases after its epilogue
     }
     for (int i = 0; i < kMaxWStages; ++i) {
       mbar_init(&w_full[i], 1);
@@ -266,9 +268,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(const __grid_con
       wgmma_wait<0>();
 #pragma unroll
       for (int mt = 0; mt < MT; ++mt) fence_acc(acc[mt]);
+      // res_win (pairs only, one K-chunk): the epilogue still reads the residual from the last A stage, which is released after it
+      const int win_a = (PAIR && p.res_win) ? pend_a : -1;
       if (leader) {
         if (pend_w >= 0) mbar_arrive(&w_empty[pend_w]);
-        if (pend_a >= 0) mbar_arrive(&a_empty[pend_a]);
+        if (pend_a >= 0 && win_a < 0) mbar_arrive(&a_empty[pend_a]);
       }
       if constexpr (PAIR) {
         // ---- c1 epilogue -> mid (fp16, swizzled like the operand planes); rows outside [0, valid) are c2's zero padding
@@ -321,10 +325,12 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(const __grid_con
 #pragma unroll
         for (int mt = 0; mt < MT; ++mt) fence_acc(acc[mt]);
       }
-      // ---- epilogue: per (row tile, 32-column unit) the slice goes through shared memory so that a thread owns one row and
-      // 16 consecutive columns (the fp16 plane stores 8 channels and the F32B plane 4 channels per 16-byte access)
+      // ---- epilogue: per (row tile, 32-column unit) the slice goes through shared memory so that a lane owns one row and
+      // 16 consecutive columns (the fp16 plane stores 8 channels and the F32B plane 4 channels per 16-byte access).  Each warp
+      // stages and reads back only its own 16 fragment rows, so the round trip is ordered by __syncwarp alone.
       const int valid_out = p.lengths ? min(p.Lout, p.lengths[wi.b] * p.len_mul_out) : p.Lout;
-      const int row_in_tile = tid & 63;
+      const int row_in_tile = 16 * (warp & 3) + (lane >> 1);
+      const int col_half = (lane & 1) * UC;
       // global reads of unit k: residual (rv / rh) and running sum (ov).  Where the accumulators leave room for a second register
       // set (MT x N / 2 <= 64 of them; 128 spill), they are issued one unit ahead, before the previous unit goes through shared
       // memory.
@@ -334,7 +340,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(const __grid_con
       uint4 rh[kSets][UC / 8];
       auto load_unit = [&](int k, float4 (&rv)[UC / 4], float4 (&ov)[UC / 4], uint4 (&rh)[UC / 8]) {
         const int mt = k / (N / 32);
-        const int col0 = (k % (N / 32)) * 32 + (tid >> 6) * UC;
+        const int col0 = (k % (N / 32)) * 32 + col_half;
         const int q = wi.m0 + (g * MT + mt) * 64 + row_in_tile;
         const int lo = q * p.stride + wi.r;
         const bool inb = q < p.Lin && (g * MT + mt) * 64 + row_in_tile < p.rows_item;
@@ -345,7 +351,15 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(const __grid_con
         }
         if (inb && p.res16) {  // (the lo halves of a hi/lo residual share rv's registers: res32 and res16 are exclusive)
           const int rr = kPadRows + lo;
-          if (!p.res_hilo) {
+          if (PAIR && win_a >= 0) {
+            // plane row rr is window row rr - floor8(kPadRows + m0 + omin); the window starts on a multiple of 8 rows, so the
+            // row keeps the plane's swizzle phase
+            const int wr = delta - p.omin + (q - wi.m0);
+            const uint8_t* wrow = a_base + (size_t)win_a * p.a_stage_bytes + (size_t)wr * ROWB;
+            const int c0 = col0 >> 3, sw = f16_swz(CW, wr);
+#pragma unroll
+            for (int j = 0; j < UC / 8; ++j) rh[j] = *reinterpret_cast<const uint4*>(wrow + (((c0 + j) ^ sw) << 4));
+          } else if (!p.res_hilo) {
             const size_t rbase = (((size_t)wi.b * (p.Cout / ocw) + col0 / ocw) * p.res_Lp + rr) * (size_t)(ocw >> 3);
             const int c0 = (col0 & (ocw - 1)) >> 3, sw = f16_swz(ocw, rr);
 #pragma unroll
@@ -371,7 +385,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(const __grid_con
       for (int k = 0; k < kUnits; ++k) {
         {
           const int mt = k / (N / 32), u = k % (N / 32);
-          const int col0 = u * 32 + (tid >> 6) * UC;
+          const int col0 = u * 32 + col_half;
           const int q = wi.m0 + (g * MT + mt) * 64 + row_in_tile;
           const int lo = q * p.stride + wi.r;
           const bool inb = q < p.Lin && (g * MT + mt) * 64 + row_in_tile < p.rows_item;
@@ -382,14 +396,20 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(const __grid_con
           const float4(&rvk)[UC / 4] = rv[k % kSets];
           const float4(&ovk)[UC / 4] = ov[k % kSets];
           const uint4(&rhk)[UC / 8] = rh[k % kSets];
-          group_sync(1 + g, 128);  // the previous unit's rows have been read
+          __syncwarp();  // this warp has read back the previous unit's rows (lanes that skipped a unit still arrive here)
           stage_acc32(stage, &acc[mt][u * 16], tid);
-          group_sync(1 + g, 128);
+          __syncwarp();
           if (!inb) continue;
           float v[UC];
-          const float* srow = stage + row_in_tile * kStageLd + (tid >> 6) * UC;
+          const float4* srow = reinterpret_cast<const float4*>(stage + row_in_tile * kStageLd + col_half);
 #pragma unroll
-          for (int i = 0; i < UC; ++i) v[i] = srow[i] * p.acc_scale + bias_s[col0 + i];
+          for (int j = 0; j < UC / 4; ++j) {
+            const float4 s = srow[j];
+            v[4 * j + 0] = s.x * p.acc_scale + bias_s[col0 + 4 * j + 0];
+            v[4 * j + 1] = s.y * p.acc_scale + bias_s[col0 + 4 * j + 1];
+            v[4 * j + 2] = s.z * p.acc_scale + bias_s[col0 + 4 * j + 2];
+            v[4 * j + 3] = s.w * p.acc_scale + bias_s[col0 + 4 * j + 3];
+          }
           if (p.res32) {
 #pragma unroll
             for (int j = 0; j < UC / 4; ++j) {
@@ -470,6 +490,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(const __grid_con
             }
           }
         }
+      }
+      if (win_a >= 0) {  // every lane of this warp is done with the operand window
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&a_empty[win_a]);
       }
     }
   }
@@ -857,6 +881,14 @@ int launch_tc(const TcOp& op, const char* tc_arena, const TRef& x16, const TRef&
     p.div = u.div;
     p.len_mul_out = u.len_mul_out;
     p.red_add = (p.mode == EPI_ADD && !y16.p && y32.p && red_add) ? 1 : 0;
+    // the residual is c1's own input plane (the resblock's x): its rows are already in the item's operand window
+    p.res_win = (res16.p == x16.p && !res16.hilo && !x16.hilo && p.res_Lp == p.x_Lp && p.stride == 1 && p.n_cchunks == 1 &&
+                 f16_cw(t.Cout) == p.cw)
+                    ? 1
+                    : 0;
+    // the epilogue reads window rows delta - omin + i (0 <= delta <= 7) for output rows 0 <= i < rows_item
+    if (p.res_win && (p.omin > 0 || 7 - p.omin + p.rows_item > p.W))
+      return fail(MB_ERR_INVALID, "tc_pair(%s): residual rows outside the operand window", op.name);
   }
   if (res16.p && !res16.hilo && res16.C != t.Cout) return fail(MB_ERR_INVALID, "tc_conv(%s): fp16 residual plane geometry", op.name);
   if (res16.p && res16.hilo && res16.C != (t.Cout >= 64 ? 2 * t.Cout : 64)) return fail(MB_ERR_INVALID, "tc_conv(%s): hi/lo residual plane geometry", op.name);

@@ -132,7 +132,9 @@ __device__ __forceinline__ void group_sync(int id, int threads) {
 }
 
 // one 64-row x 32-column slice of a wgmma accumulator -> shared memory rows of kStageLd floats (row = accumulator row),
-// so that the epilogue reads whole rows; `d` points at the 16 registers of that slice (columns 8 j .. 8 j + 31)
+// so that the epilogue reads whole rows; `d` points at the 16 registers of that slice (columns 8 j .. 8 j + 31).
+// Warp w writes only its own fragment rows 16 w .. 16 w + 15, so a warp that reads back rows of that band needs no barrier
+// beyond __syncwarp.  With kStageLd = 36, 16-byte reads by lanes (row 16 w + l / 2, columns 16 (l & 1) ..) are conflict-free.
 constexpr int kStageLd = 36;
 __device__ __forceinline__ void stage_acc32(float* stage, const float* d, int tid) {
   const int w = tid >> 5, l = tid & 31;
