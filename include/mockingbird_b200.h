@@ -256,7 +256,8 @@ int mb_wavernn_condition(mb_wavernn* h, const float* mel, int32_t frames, void* 
 
 /* The sample loop (fatchord_version.py:190-234) over `folds` independent rows, each `steps` long,
  * row r starting at upsampled-time offset fold_starts[r] (fold_with_overlap, :288-338; positions
- * past the end of the conditioning read zeros like the reference's zero padding).
+ * past the end of the conditioning read zeros like the reference's zero padding).  A fold start must be
+ * >= 0 and fold_starts[r] + steps must fit in int32; otherwise the call is refused with MB_ERR_INVALID.
  *   noise  : Exp(1) draws, fp32 [steps_in_call, folds, 512] in the reference's draw order
  *            (Categorical.sample == argmax(p/q), SURVEY.md fact 5), or NULL to use the built-in
  *            counter-based generator seeded by `seed`.

@@ -17,7 +17,6 @@
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 
-#include <cstdlib>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -151,41 +150,18 @@ __global__ void k_aux_table(const float* __restrict__ W, int ld, int K0, const f
 
 // per-chunk conditioning of the I layer in the exchange layout:
 //   condI[i][u][r] = dot_seq(I_w[u][1:113], [melup[t]; aux[t/200][0:32]]) + I_b[u],  t = start[r] + step0 + i
+// row r is described by rowc[r] = {start, T_u, table base, frame base}; only the W = 64 * (live row blocks) leading rows are
+// written, and the dot product is skipped for the padding rows past the table (T_u == 0: most of a row block when there are
+// only a few rows)
 __global__ void __launch_bounds__(256) k_condI(const float* __restrict__ I_w, const float* __restrict__ I_b,
                                                const float* __restrict__ melup, const float* __restrict__ aux,
-                                               int T, const int* __restrict__ starts, int B, int Bpad, int step0,
-                                               int nsteps, float* __restrict__ out) {
-  __shared__ float c[FEAT + AUXD];
-  const int r = blockIdx.x % Bpad;
-  const int i = blockIdx.x / Bpad;
-  if (i >= nsteps) return;
-  const int t = (r < B) ? starts[r] + step0 + i : -1;
-  const bool live = (t >= 0 && t < HOP * T);
-  for (int j = threadIdx.x; j < FEAT + AUXD; j += blockDim.x) {
-    float v = 0.0f;
-    if (live) v = (j < FEAT) ? melup[(size_t)t * FEAT + j] : aux[(size_t)(t / HOP) * CDIM + (j - FEAT)];
-    c[j] = v;
-  }
-  __syncthreads();
-  for (int u = threadIdx.x; u < RNN; u += blockDim.x) {
-    float acc = 0.0f;
-    const float* wr = I_w + (size_t)u * 113 + 1;
-    for (int j = 0; j < FEAT + AUXD; ++j) acc = fmaf(wr[j], c[j], acc);
-    out[((size_t)i * RNN + u) * Bpad + r] = (r < B) ? acc + I_b[u] : 0.0f;
-  }
-}
-
-// the same for the multi-utterance loop: row r is described by rowc[r] = {start, T_u, table base, frame base}; only the
-// W = 64 * (live row blocks) leading rows are computed
-__global__ void __launch_bounds__(256) k_condI_multi(const float* __restrict__ I_w, const float* __restrict__ I_b,
-                                                     const float* __restrict__ melup, const float* __restrict__ aux,
-                                                     const int4* __restrict__ rowc, int W, int Bpad, int step0, int nsteps,
-                                                     float* __restrict__ out) {
+                                               const int4* __restrict__ rowc, int W, int Bpad, int step0, int nsteps,
+                                               float* __restrict__ out) {
   __shared__ float c[FEAT + AUXD];
   const int r = blockIdx.x % W;
   const int i = blockIdx.x / W;
   if (i >= nsteps) return;
-  const int4 d = rowc[r];  // rows past the table: T_u == 0, never live
+  const int4 d = rowc[r];
   const int t = d.x + step0 + i;
   const bool live = t < HOP * d.y;
   for (int j = threadIdx.x; j < FEAT + AUXD; j += blockDim.x) {
@@ -197,7 +173,8 @@ __global__ void __launch_bounds__(256) k_condI_multi(const float* __restrict__ I
   for (int u = threadIdx.x; u < RNN; u += blockDim.x) {
     float acc = 0.0f;
     const float* wr = I_w + (size_t)u * 113 + 1;
-    for (int j = 0; j < FEAT + AUXD; ++j) acc = fmaf(wr[j], c[j], acc);
+    if (d.y > 0)
+      for (int j = 0; j < FEAT + AUXD; ++j) acc = fmaf(wr[j], c[j], acc);
     out[((size_t)i * RNN + u) * Bpad + r] = acc + I_b[u];
   }
 }
@@ -214,8 +191,7 @@ struct LoopParams {
   const float* aux3P;       // [T+1][512]
   const float* aux4P;       // [T+1][512]
   const float* condI;       // [nsteps][512][Bpad]
-  const int* starts;        // [B]
-  int T, B, Bpad, step0, nsteps, steps_total;
+  int B, Bpad, step0, nsteps, steps_total;  // B: live rows, a prefix (rows are ordered longest first); steps_total: row 0's
   // state / exchange buffers (global, [unit][Bpad])
   float* h1;                // [2][512][Bpad]
   float* h2;                // [2][512][Bpad]
@@ -223,19 +199,16 @@ struct LoopParams {
   float* f2;                // [512][Bpad]
   float* logits;            // [512][Bpad]
   float* xprev;             // [Bpad]
-  const float* noise;       // RAW: [nsteps][noise_B][512] Exp(1); MOL: [nsteps][noise_B*10 mixture | noise_B logistic]
-                            // uniforms; or nullptr (this call's rows are noise rows row0 .. row0+B)
-  int noise_B, row0;        // row0: global fold index of local row 0 (fold sharding across GPUs)
-  uint64_t seed;
+  const float* noise;       // RAW: [nsteps][noise_B][512] Exp(1), row r at noise row rown.z + rown.y; MOL: per step, every
+                            // block of n noise rows from rown.z holds its [n*10 mixture | n logistic] uniforms; or nullptr
+  int noise_B;              // noise rows per step
   int16_t* out_idx;         // RAW: class indices [B][steps_total]
   float* out_x;             // MOL: float samples [B][steps_total]
-  unsigned int* barrier;    // grid barrier counter / per-CTA epoch flags [NCTA] (zeroed by the host before launch)
-  int flagbar;              // 1: flag barrier, 0: single atomic counter
-  // multi-utterance loop (k_sample_loop<MOL, true>): per-row descriptors [Bpad] replace starts / T / row0 / seed; B is the
-  // number of live rows (a prefix: rows are ordered longest first), noise_B == B, steps_total the longest row's steps
+  unsigned int* barrier;    // grid barrier counter (zeroed by the host before launch)
+  // per-row descriptors [Bpad]
   const int4* rowc;         // {start, T_u, first table row of its utterance, first frame of its utterance}
-  const int4* rown;         // {steps, fold index in its utterance, first row of its utterance, folds of its utterance}
-  const uint64_t* rowseed;  // seed of its utterance (built-in generator: keyed by (seed, step, fold index, slot))
+  const int4* rown;         // {steps, noise / generator key, first noise row of its block, rows in that block}
+  const uint64_t* rowseed;  // built-in generator: keyed by (seed, step, key, slot)
 };
 
 // per-CTA weight pack (floats):
@@ -297,26 +270,7 @@ __global__ void k_pack(PackSrc s, float* __restrict__ wpack) {
   }
 }
 
-// Flag barrier (p.flagbar): every CTA publishes its epoch in its own word, threads 0..gridDim-1 of every CTA each poll one
-// word - no 128-way serialised atomic on a single L2 line, the polls run in parallel.  The counter variant is kept for A/B.
-__device__ __forceinline__ void grid_barrier_flags(unsigned int* flags, unsigned int& epoch) {
-  __syncthreads();
-  epoch += 1;
-  if (threadIdx.x == 0) {
-    __threadfence();
-    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(flags + blockIdx.x), "r"(epoch) : "memory");
-  }
-  if (threadIdx.x < gridDim.x) {
-    unsigned int v;
-    do {
-      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(flags + threadIdx.x) : "memory");
-    } while (v < epoch);
-    __threadfence();
-  }
-  __syncthreads();
-}
-
-__device__ __forceinline__ void grid_barrier_counter(unsigned int* counter, unsigned int& target) {
+__device__ __forceinline__ void grid_barrier(unsigned int* counter, unsigned int& target) {
   __syncthreads();
   if (threadIdx.x == 0) {
     target += gridDim.x;
@@ -331,9 +285,11 @@ __device__ __forceinline__ void grid_barrier_counter(unsigned int* counter, unsi
   __syncthreads();
 }
 
-__device__ __forceinline__ void grid_barrier(const LoopParams& p, unsigned int& target) {
-  if (p.flagbar) grid_barrier_flags(p.barrier, target);
-  else grid_barrier_counter(p.barrier, target);
+// the aux-table row that `row` reads at step gstep: its frame, or its utterance's "past the end" row
+__device__ __forceinline__ int table_row(const LoopParams& p, int row, int gstep) {
+  const int4 d = p.rowc[row];
+  const int t = d.x + gstep;
+  return d.z + (t < HOP * d.y ? t / HOP : d.y);
 }
 
 // 4 rows x NC columns register tile over the k-range [k0, k0+klen) of one matrix:
@@ -365,10 +321,10 @@ __device__ __forceinline__ void tile_gemv(const float* __restrict__ wsm /*[512][
 
 __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 
+// Rows of one or several utterances with their own lengths (LoopParams::rowc / rown / rowseed); only the row blocks that hold
+// a live row run, and a row stores nothing past its own last step.
 // MOL: fc3 has 30 outputs (units of CTAs 0..7; the other CTAs skip phase E) and phase F is the mixture-of-logistics draw
-// MULTI: rows of several utterances with their own lengths (LoopParams::rowc / rown / rowseed); only the row blocks that
-// hold a live row run, and a row stores nothing past its own last step
-template <bool MOL, bool MULTI>
+template <bool MOL>
 __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p) {
   extern __shared__ __align__(16) float sm[];
   float* wsm = sm;
@@ -382,13 +338,21 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
   const int kh = lane >> 4;   // k half within the warp's slice
   const int cta = blockIdx.x;
   const int Bpad = p.Bpad;
-  const int nrb = MULTI ? (p.B + RB - 1) / RB : Bpad / RB;
+  const int nrb = (p.B + RB - 1) / RB;
+  // descriptors of this CTA's own row (the first row of phase F): the same at every step, so read once and kept in shared
+  // memory (in registers they would add spills to the GEMV phases)
+  __shared__ int4 own;
+  __shared__ uint64_t own_seed;
 
   {  // one-time: weights -> shared memory
     const float4* src = reinterpret_cast<const float4*>(p.wpack + (size_t)cta * WPACK_FLOATS);
     float4* dst = reinterpret_cast<float4*>(wsm);
     for (int i = tid; i < WPACK_FLOATS / 4; i += kThreads) dst[i] = src[i];
     for (int i = tid; i < RNN; i += kThreads) I0[i] = p.I0[i];
+    if (tid == 0) {
+      own = cta < p.B ? p.rown[cta] : make_int4(0, 0, 0, 0);
+      own_seed = cta < p.B ? p.rowseed[cta] : 0;
+    }
   }
   __syncthreads();
 
@@ -407,7 +371,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
     // into shared memory now (cp.async: no registers), so that their HBM/L2 latency hides behind phases A-E instead of sitting
     // on the dependent chain (measured: +2 us per step with noise in global memory).
     if (!MOL && p.noise && cta < p.B && tid < NCLS / 4) {
-      const float* src = p.noise + ((size_t)i * p.noise_B + (size_t)(p.row0 + cta)) * NCLS + tid * 4;
+      const float* src = p.noise + ((size_t)i * p.noise_B + (size_t)(own.z + own.y)) * NCLS + tid * 4;
       const uint32_t dst = (uint32_t)__cvta_generic_to_shared(qsm + tid * 4);
       asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
     }
@@ -416,20 +380,11 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
     float mol_pre = 0.0f;
     if (MOL && p.noise && cta < p.B && warp == 0 && lane < MB_MOL_UNIFORMS) {
       const size_t base = (size_t)i * MB_MOL_UNIFORMS * p.noise_B;
-      if constexpr (MULTI) {  // per utterance block of nf rows starting at row r0: [nf x 10 mixture | nf logistic]
-        const int4 d = p.rown[cta];
-        mol_pre = p.noise[base + (size_t)MB_MOL_UNIFORMS * d.z +
-                          (lane < MB_MOL_NMIX ? d.y * MB_MOL_NMIX + lane : MB_MOL_NMIX * d.w + d.y)];
-      } else {
-        mol_pre = p.noise[base + (lane < MB_MOL_NMIX ? (size_t)(p.row0 + cta) * MB_MOL_NMIX + lane
-                                                     : (size_t)MB_MOL_NMIX * p.noise_B + (p.row0 + cta))];
-      }
+      mol_pre = p.noise[base + (size_t)MB_MOL_UNIFORMS * own.z +
+                        (lane < MB_MOL_NMIX ? own.y * MB_MOL_NMIX + lane : MB_MOL_NMIX * own.w + own.y)];
     }
     // built-in generator: the same 512 values, one per thread, computed here instead of inside the sampling phase
-    if (!MOL && !p.noise && cta < p.B && tid < NCLS) {
-      if constexpr (MULTI) qsm[tid] = mb_exp1_noise(p.rowseed[cta], (uint32_t)gstep, (uint32_t)p.rown[cta].y, (uint32_t)tid);
-      else qsm[tid] = mb_exp1_noise(p.seed, (uint32_t)gstep, (uint32_t)(p.row0 + cta), (uint32_t)tid);
-    }
+    if (!MOL && !p.noise && cta < p.B && tid < NCLS) qsm[tid] = mb_exp1_noise(own_seed, (uint32_t)gstep, (uint32_t)own.y, (uint32_t)tid);
 
     // ================= phase A: rnn1 =================
     for (int rb = 0; rb < nrb; ++rb) {
@@ -488,7 +443,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
       }
       __syncthreads();
     }
-    grid_barrier(p, bar_target);
+    grid_barrier(p.barrier, bar_target);
 
     // ================= phase B: rnn2 =================
     for (int rb = 0; rb < nrb; ++rb) {
@@ -529,15 +484,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
         const int r = tid & (RB - 1), j = tid >> 6;
         const int row = rb * RB + r;
         const int unit = cta * UPC + j;
-        int frame = p.T;  // "past the end" row of the tables
-        if constexpr (MULTI) {
-          const int4 d = p.rowc[row];
-          const int t = d.x + gstep;
-          frame = d.z + (t < HOP * d.y ? t / HOP : d.y);
-        } else if (row < p.B) {
-          const int t = p.starts[row] + gstep;
-          if (t < HOP * p.T) frame = t / HOP;
-        }
+        const int frame = table_row(p, row, gstep);
         float g[2][3];
 #pragma unroll
         for (int m = 0; m < 2; ++m)
@@ -557,7 +504,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
       }
       __syncthreads();
     }
-    grid_barrier(p, bar_target);
+    grid_barrier(p.barrier, bar_target);
 
     // ================= phases C, D, E: fc1, fc2, fc3 =================
 #pragma unroll 1
@@ -609,15 +556,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
             for (int q = 0; q < n; ++q) s[q] = s[2 * q] + s[2 * q + 1];
           float v = s[0];
           if (layer < 2) {
-            int frame = p.T;
-            if constexpr (MULTI) {
-              const int4 d = p.rowc[row];
-              const int t = d.x + gstep;
-              frame = d.z + (t < HOP * d.y ? t / HOP : d.y);
-            } else if (row < p.B) {
-              const int t = p.starts[row] + gstep;
-              if (t < HOP * p.T) frame = t / HOP;
-            }
+            const int frame = table_row(p, row, gstep);
             v = v + (layer == 0 ? p.aux3P : p.aux4P)[(size_t)frame * RNN + unit];
             v = v > 0.0f ? v : 0.0f;
             (layer == 0 ? p.f1 : p.f2)[(size_t)unit * Bpad + row] = v;
@@ -628,7 +567,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
         __syncthreads();
       }
       asm volatile("cp.async.wait_group 0;" ::: "memory");  // this step's noise row has landed (issued at the top of the step)
-      grid_barrier(p, bar_target);
+      grid_barrier(p.barrier, bar_target);
     }
 
     if constexpr (MOL) {
@@ -637,19 +576,16 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
       if (warp == 0) {
         const size_t base = (size_t)i * MB_MOL_UNIFORMS * p.noise_B;
         for (int row = cta; row < p.B; row += gridDim.x) {
-          int4 dn = make_int4(0, 0, 0, 0);
-          if constexpr (MULTI) dn = p.rown[row];
-          const uint32_t grow = MULTI ? (uint32_t)dn.y : (uint32_t)(p.row0 + row);  // noise row key
-          const uint64_t seed = MULTI ? p.rowseed[row] : p.seed;
+          const int4 dn = row == cta ? own : p.rown[row];
+          const uint64_t seed = row == cta ? own_seed : p.rowseed[row];
           // element offsets of the row's mixture uniforms and of its logistic uniform within the step
-          const size_t mix0 = MULTI ? (size_t)MB_MOL_UNIFORMS * dn.z + (size_t)dn.y * MB_MOL_NMIX : (size_t)grow * MB_MOL_NMIX;
-          const size_t log0 = MULTI ? (size_t)MB_MOL_UNIFORMS * dn.z + (size_t)MB_MOL_NMIX * dn.w + dn.y
-                                    : (size_t)MB_MOL_NMIX * p.noise_B + grow;
+          const size_t mix0 = (size_t)MB_MOL_UNIFORMS * dn.z + (size_t)dn.y * MB_MOL_NMIX;
+          const size_t log0 = (size_t)MB_MOL_UNIFORMS * dn.z + (size_t)MB_MOL_NMIX * dn.w + dn.y;
           float sc = -3.0e38f;
           if (lane < MB_MOL_NMIX) {
             const float t = (row == cta && p.noise) ? mol_pre
                             : (p.noise ? p.noise[base + mix0 + lane]
-                                       : mb_mol_uniform(seed, (uint32_t)gstep, grow, (uint32_t)lane));
+                                       : mb_mol_uniform(seed, (uint32_t)gstep, (uint32_t)dn.y, (uint32_t)lane));
             sc = mb_mol_score(p.logits[(size_t)lane * Bpad + row], t);
           }
           int best = lane;
@@ -666,10 +602,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
           if (lane == 0) {
             const float u = (row == cta && p.noise) ? u_pre
                             : (p.noise ? p.noise[base + log0]
-                                       : mb_mol_uniform(seed, (uint32_t)gstep, grow, MB_MOL_NMIX));
+                                       : mb_mol_uniform(seed, (uint32_t)gstep, (uint32_t)dn.y, MB_MOL_NMIX));
             const float x = mb_mol_sample(p.logits[(size_t)(MB_MOL_NMIX + best) * Bpad + row],
                                           p.logits[(size_t)(2 * MB_MOL_NMIX + best) * Bpad + row], u);
-            if (!MULTI || gstep < dn.x) p.out_x[(size_t)row * p.steps_total + gstep] = x;
+            if (gstep < dn.x) p.out_x[(size_t)row * p.steps_total + gstep] = x;
             p.xprev[row] = x;
           }
         }
@@ -678,6 +614,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
     // ================= phase F: softmax + Categorical sample (one warp per row) =================
     // (the copies issued at the top of the step were waited for before the grid barrier above: qsm is complete and visible)
       for (int row = cta; row < p.B; row += gridDim.x) {
+        const int4 dn = row == cta ? own : p.rown[row];
         float lg[16], e[16];
         float m = -3.0e38f;
 #pragma unroll
@@ -714,9 +651,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
         for (int jj = 0; jj < 16; ++jj) {
           const int cls = lane + 32 * jj;
           const float q = (row == cta) ? qsm[cls]
-                          : (p.noise ? p.noise[((size_t)i * p.noise_B + (size_t)(p.row0 + row)) * NCLS + cls]
-                             : MULTI ? mb_exp1_noise(p.rowseed[row], (uint32_t)gstep, (uint32_t)p.rown[row].y, (uint32_t)cls)
-                                     : mb_exp1_noise(p.seed, (uint32_t)gstep, (uint32_t)(p.row0 + row), (uint32_t)cls));
+                          : (p.noise ? p.noise[((size_t)i * p.noise_B + (size_t)(dn.z + dn.y)) * NCLS + cls]
+                                     : mb_exp1_noise(p.rowseed[row], (uint32_t)gstep, (uint32_t)dn.y, (uint32_t)cls));
           const float v = (e[jj] / S2) / q;
           if (v > bestv) {  // ascending class order within the lane: first maximum wins
             bestv = v;
@@ -733,12 +669,12 @@ __global__ void __launch_bounds__(kThreads, 1) k_sample_loop(const LoopParams p)
           }
         }
         if (lane == 0) {
-          if (!MULTI || gstep < p.rown[row].x) p.out_idx[(size_t)row * p.steps_total + gstep] = (int16_t)best;
+          if (gstep < dn.x) p.out_idx[(size_t)row * p.steps_total + gstep] = (int16_t)best;
           p.xprev[row] = (2.0f * (float)best) / 511.0f - 1.0f;
         }
       }
     }
-    grid_barrier(p, bar_target);
+    grid_barrier(p.barrier, bar_target);
   }
 }
 
@@ -769,13 +705,13 @@ namespace {
 const float* W(const mb_wavernn* h, const std::string& name) { return h->w.ptr(name); }
 
 struct Ws {
-  size_t aux, melup, aux2P, aux3P, aux4P, tmpA, tmpB, tmpR, padP, lad5, lad25, lad200, segs, starts, condI, h1, h2, f1, f2, logits,
+  size_t aux, melup, aux2P, aux3P, aux4P, tmpA, tmpB, tmpR, padP, lad5, lad25, lad200, segs, condI, h1, h2, f1, f2, logits,
       xprev, barrier, rowdesc;  // floats
   size_t total;                 // bytes
 };
 
 // T frames of U utterances in all (each utterance has its own "past the end" table row and its own 4 frames of ladder padding);
-// the segment tables of the conditioning kernels and the row descriptors of the multi-utterance loop are always laid out
+// the segment tables of the conditioning kernels and the row descriptors of the sample loop are always laid out
 Ws ws_layout(int T, int Bpad, int chunk_steps, int U) {
   Ws L{};
   WsLayout W;
@@ -792,7 +728,6 @@ Ws ws_layout(int T, int Bpad, int chunk_steps, int U) {
   L.lad25 = W.take<float>((size_t)FEAT * (T + 4 * U) * 25);
   L.lad200 = W.take<float>((size_t)FEAT * (T + 4 * U) * HOP);
   L.segs = W.take<float>((size_t)3 * T + 7 * U);  // int32: fseg[T] pseg[T+4U] tsrc[T+U] segF[U] segT[U]
-  L.starts = W.take<float>((size_t)Bpad);
   L.condI = W.take<float>((size_t)chunk_steps * RNN * Bpad);
   L.h1 = W.take<float>((size_t)2 * RNN * Bpad);
   L.h2 = W.take<float>((size_t)2 * RNN * Bpad);
@@ -800,7 +735,7 @@ Ws ws_layout(int T, int Bpad, int chunk_steps, int U) {
   L.f2 = W.take<float>((size_t)RNN * Bpad);
   L.logits = W.take<float>((size_t)RNN * Bpad);
   L.xprev = W.take<float>((size_t)Bpad);
-  L.barrier = W.take<float>(256);  // 1 KB: counter, or one epoch word per CTA
+  L.barrier = W.take<float>(1);  // the grid barrier's counter
   L.rowdesc = W.take<float>((size_t)10 * Bpad);  // int4 rowc[Bpad] | int4 rown[Bpad] | uint64 rowseed[Bpad]
   L.total = W.total();
   return L;
@@ -1044,99 +979,76 @@ int mb_wavernn_condition_multi(mb_wavernn* h, const float* mel_concat, const int
   return condition_impl("mb_wavernn_condition_multi", h, mel_concat, frames, n_utts, workspace, workspace_bytes, stream);
 }
 
-int mb_wavernn_generate(mb_wavernn* h, const int32_t* fold_starts_host, int32_t B, int32_t steps, int32_t step0,
-                        int32_t nsteps, const float* noise, uint64_t seed, int16_t* out_idx, void* workspace,
-                        size_t workspace_bytes, void* stream) {
-  return mb_wavernn_generate_rows(h, fold_starts_host, B, steps, step0, nsteps, noise, B, 0, seed, out_idx, workspace,
-                                  workspace_bytes, stream);
-}
-
 }  // extern "C"
 
 namespace {
 
-int launch_sample_loop(mb_wavernn* h, LoopParams& p, const Ws& L, float* ws, bool multi, cudaStream_t st);
-
-// one chunk of the sample loop; exactly one of out_idx (RAW handle) / out_x (MOL handle) is given
-int generate_rows_impl(mb_wavernn* h, const int32_t* fold_starts_host, int32_t B, int32_t steps, int32_t step0,
-                       int32_t nsteps, const float* noise, int32_t noise_folds, int32_t row0, uint64_t seed,
-                       int16_t* out_idx, float* out_x, void* workspace, size_t workspace_bytes, void* stream) {
-  if (row0 < 0 || (noise && row0 + B > noise_folds))
-    return fail(MB_ERR_INVALID, "mb_wavernn_generate_rows: rows [%d, %d) outside the %d noise rows", row0, row0 + B, noise_folds);
-  if (!h->finalized) return fail(MB_ERR_STATE, "mb_wavernn_generate: weights not finalized");
-  if (h->cond_frames.size() != 1 || h->cond_ws != workspace)
-    return fail(MB_ERR_STATE, "mb_wavernn_generate: call mb_wavernn_condition on this workspace first");
-  if (B <= 0 || nsteps <= 0 || nsteps > kChunkMax || step0 < 0 || step0 + nsteps > steps)
-    return fail(MB_ERR_INVALID, "mb_wavernn_generate: bad step range (at most %d steps per call)", kChunkMax);
-  const int T = h->cond_frames[0];
-  const int Bpad = bpad_of(B);
-  const Ws L = ws_layout(T, Bpad, kChunkMax, 1);
+// One chunk of the sample loop over a row table the caller has checked: `rows` rows, of which the first n_live are alive, and
+// `noise_rows` rows of injected noise per step.  At step0 == 0 the state is reset and the row descriptors are uploaded, as
+// describe(rowc, rown, rowseed) writes them for the `rows` rows (int32 [4] per row for rowc and rown; LoopParams).  Exactly one
+// of out_idx (RAW handle) / out_x (MOL handle) is given.
+template <class Describe>
+int sample_chunk(const char* fn, mb_wavernn* h, int rows, int n_live, int noise_rows, int max_steps, int step0, int nsteps,
+                 const float* noise, int16_t* out_idx, float* out_x, void* workspace, size_t workspace_bytes, void* stream,
+                 Describe describe) {
+  int Ttot = 0;
+  for (int t : h->cond_frames) Ttot += t;
+  const int Bpad = bpad_of(rows);
+  const Ws L = ws_layout(Ttot, Bpad, kChunkMax, (int)h->cond_frames.size());
   float* ws;
-  if (int rc = bind("mb_wavernn_generate", workspace, workspace_bytes, L.total, &ws)) return rc;
+  if (int rc = bind(fn, workspace, workspace_bytes, L.total, &ws)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
+  int4* rowc = reinterpret_cast<int4*>(ws + L.rowdesc);
+  int4* rown = rowc + Bpad;
+  uint64_t* rowseed = reinterpret_cast<uint64_t*>(rown + Bpad);
   if (step0 == 0) {
-    // zero initial state (fatchord_version.py:178-185) and upload the fold starts
+    // zero initial state (fatchord_version.py:178-185) and upload the row descriptors (rows past the table: T_u == 0, never
+    // live)
     MB_CUDA_CHECK(cudaMemsetAsync(ws + L.h1, 0, sizeof(float) * (L.xprev + align_up((size_t)Bpad, 64) - L.h1), st));
-    std::vector<int32_t> tmp(Bpad, 0);
-    memcpy(tmp.data(), fold_starts_host, sizeof(int32_t) * B);
-    MB_CUDA_CHECK(cudaMemcpyAsync(ws + L.starts, tmp.data(), sizeof(int32_t) * Bpad, cudaMemcpyHostToDevice, st));
+    std::vector<int32_t> tmp((size_t)10 * Bpad, 0);
+    describe(tmp.data(), tmp.data() + 4 * Bpad, reinterpret_cast<uint64_t*>(tmp.data() + 8 * Bpad));
+    MB_CUDA_CHECK(cudaMemcpyAsync(rowc, tmp.data(), sizeof(int32_t) * tmp.size(), cudaMemcpyHostToDevice, st));
     MB_CUDA_CHECK(cudaStreamSynchronize(st));  // tmp goes out of scope
   }
-  const int* starts = reinterpret_cast<const int*>(ws + L.starts);
-  k_condI<<<nsteps * Bpad, 256, 0, st>>>(W(h, "I.weight"), W(h, "I.bias"), ws + L.melup, ws + L.aux, T, starts, B, Bpad,
-                                         step0, nsteps, ws + L.condI);
+  const int Wl = bpad_of(n_live);  // rows of the live row blocks
+  k_condI<<<nsteps * Wl, 256, 0, st>>>(W(h, "I.weight"), W(h, "I.bias"), ws + L.melup, ws + L.aux, rowc, Wl, Bpad, step0, nsteps,
+                                       ws + L.condI);
   MB_LAUNCH_CHECK("k_condI");
+  MB_CUDA_CHECK(cudaMemsetAsync(ws + L.barrier, 0, sizeof(unsigned int), st));
   LoopParams p;
   memset(&p, 0, sizeof(p));
-  p.starts = starts;
-  p.T = T;
-  p.B = B;
-  p.Bpad = Bpad;
-  p.step0 = step0;
-  p.nsteps = nsteps;
-  p.steps_total = steps;
-  p.noise = noise;
-  p.noise_B = noise_folds;
-  p.row0 = row0;
-  p.seed = seed;
-  p.out_idx = out_idx;
-  p.out_x = out_x;
-  return launch_sample_loop(h, p, L, ws, false, st);
-}
-
-// fills the workspace pointers of `p` and launches the loop instance of the handle's sampler
-int launch_sample_loop(mb_wavernn* h, LoopParams& p, const Ws& L, float* ws, bool multi, cudaStream_t st) {
-  const bool mol = h->mode == MB_WAVERNN_MOL;
-  MB_CUDA_CHECK(cudaMemsetAsync(ws + L.barrier, 0, 1024, st));
   p.wpack = h->arena + h->pack_off;
   p.I0 = h->arena + h->pack_off + (size_t)NCTA * WPACK_FLOATS;
   p.aux2P = ws + L.aux2P;
   p.aux3P = ws + L.aux3P;
   p.aux4P = ws + L.aux4P;
   p.condI = ws + L.condI;
+  p.B = n_live;
+  p.Bpad = Bpad;
+  p.step0 = step0;
+  p.nsteps = nsteps;
+  p.steps_total = max_steps;
   p.h1 = ws + L.h1;
   p.h2 = ws + L.h2;
   p.f1 = ws + L.f1;
   p.f2 = ws + L.f2;
   p.logits = ws + L.logits;
   p.xprev = ws + L.xprev;
+  p.noise = noise;
+  p.noise_B = noise_rows;
+  p.out_idx = out_idx;
+  p.out_x = out_x;
   p.barrier = reinterpret_cast<unsigned int*>(ws + L.barrier);
-  static const int flagbar = [] {
-    // A/B switch.  Measured: the flag barrier is much SLOWER (604 vs 428 ms per cfg-3 call: 128 x 128 polling threads swamp the
-    // four flag lines); the single-counter barrier stays the default.
-    const char* e = getenv("MB_WAVERNN_FLAGBAR");
-    return e ? atoi(e) : 0;
-  }();
-  p.flagbar = flagbar;
+  p.rowc = rowc;
+  p.rown = rown;
+  p.rowseed = rowseed;
+  const bool mol = h->mode == MB_WAVERNN_MOL;
+  const void* kern = mol ? (const void*)k_sample_loop<true> : (const void*)k_sample_loop<false>;
   const size_t smem = sizeof(float) * SMEM_FLOATS;
-  static bool attr[4] = {false, false, false, false};
-  const void* kerns[4] = {(const void*)k_sample_loop<false, false>, (const void*)k_sample_loop<true, false>,
-                          (const void*)k_sample_loop<false, true>, (const void*)k_sample_loop<true, true>};
-  const int which = (multi ? 2 : 0) + (mol ? 1 : 0);
-  const void* kern = kerns[which];
-  if (!attr[which]) {
+  static bool attr[2] = {false, false};
+  if (!attr[mol]) {
     MB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr[which] = true;
+    attr[mol] = true;
   }
   void* args[] = {(void*)&p};
   MB_CUDA_CHECK(cudaLaunchCooperativeKernel(kern, dim3(NCTA), dim3(kThreads), args, smem, st));
@@ -1144,17 +1056,108 @@ int launch_sample_loop(mb_wavernn* h, LoopParams& p, const Ws& L, float* ws, boo
   return MB_OK;
 }
 
+// mb_wavernn_generate_rows[_mol]: the folds of the one conditioned utterance as a one-utterance row table.  Row r is fold
+// row0 + r of a block of noise_folds noise rows, which is also its generator key, so a fold draws the same noise however the
+// folds are dealt to calls.
+int generate_folds(mb_wavernn* h, const int32_t* fold_starts_host, int32_t B, int32_t steps, int32_t step0, int32_t nsteps,
+                   const float* noise, int32_t noise_folds, int32_t row0, uint64_t seed, int16_t* out_idx, float* out_x,
+                   void* workspace, size_t workspace_bytes, void* stream) {
+  if (row0 < 0 || (noise && row0 + B > noise_folds))
+    return fail(MB_ERR_INVALID, "mb_wavernn_generate_rows: rows [%d, %d) outside the %d noise rows", row0, row0 + B, noise_folds);
+  if (B <= 0 || nsteps <= 0 || nsteps > kChunkMax || step0 < 0 || step0 + nsteps > steps)
+    return fail(MB_ERR_INVALID, "mb_wavernn_generate: bad step range (at most %d steps per call)", kChunkMax);
+  for (int r = 0; r < B; ++r)
+    if (fold_starts_host[r] < 0 || fold_starts_host[r] > INT32_MAX - steps)
+      return fail(MB_ERR_INVALID, "mb_wavernn_generate: fold start %d of row %d outside [0, %d]", fold_starts_host[r], r,
+                  INT32_MAX - steps);
+  if (!h->finalized) return fail(MB_ERR_STATE, "mb_wavernn_generate: weights not finalized");
+  if (h->cond_frames.size() != 1 || h->cond_ws != workspace)
+    return fail(MB_ERR_STATE, "mb_wavernn_generate: call mb_wavernn_condition on this workspace first");
+  const int T = h->cond_frames[0];
+  return sample_chunk("mb_wavernn_generate", h, B, B, noise_folds, steps, step0, nsteps, noise, out_idx, out_x, workspace,
+                      workspace_bytes, stream, [&](int32_t* c, int32_t* n, uint64_t* sd) {
+                        for (int r = 0; r < B; ++r) {
+                          c[4 * r + 0] = fold_starts_host[r];
+                          c[4 * r + 1] = T;
+                          n[4 * r + 0] = steps;
+                          n[4 * r + 1] = row0 + r;
+                          n[4 * r + 3] = noise_folds;
+                          sd[r] = seed;
+                        }
+                      });
+}
+
+// mb_wavernn_generate_multi[_mol]: whole utterances side by side (folds 0 .. n-1 of one utterance, all of one length), longest
+// rows first.  Row r is fold row_fold[r] of its utterance's block of noise rows.
+int generate_multi_impl(const char* fn, mb_wavernn* h, const int32_t* row_utt, const int32_t* row_start,
+                        const int32_t* row_steps, const int32_t* row_fold, int32_t rows, const uint64_t* utt_seeds,
+                        int32_t max_steps, int32_t step0, int32_t nsteps, int32_t n_live, const float* noise, int16_t* out_idx,
+                        float* out_x, void* workspace, size_t workspace_bytes, void* stream) {
+  if (rows <= 0 || max_steps <= 0 || nsteps <= 0 || nsteps > kChunkMax || step0 < 0 || step0 + nsteps > max_steps)
+    return fail(MB_ERR_INVALID, "%s: bad row count or step range (at most %d steps per call)", fn, kChunkMax);
+  int alive = 0;
+  for (int r = 0; r < rows; ++r) {
+    if (row_utt[r] < 0 || row_start[r] < 0 || row_start[r] > INT32_MAX - max_steps || row_steps[r] <= 0 ||
+        row_steps[r] > max_steps || row_fold[r] < 0)
+      return fail(MB_ERR_INVALID, "%s: row %d (utterance %d, start %d, steps %d, fold %d) outside the table", fn, r, row_utt[r],
+                  row_start[r], row_steps[r], row_fold[r]);
+    if (r > 0 && row_steps[r] > row_steps[r - 1]) return fail(MB_ERR_INVALID, "%s: rows must be ordered longest first (row %d)", fn, r);
+    const bool cont = r > 0 && row_utt[r] == row_utt[r - 1];
+    if (cont ? (row_fold[r] != row_fold[r - 1] + 1 || row_steps[r] != row_steps[r - 1]) : row_fold[r] != 0)
+      return fail(MB_ERR_INVALID, "%s: the folds of an utterance must be adjacent rows 0, 1, .. of one length (row %d)", fn, r);
+    alive += row_steps[r] > step0;
+  }
+  if (n_live != alive)
+    return fail(MB_ERR_INVALID, "%s: %d rows are alive at step %d, the call says %d", fn, alive, step0, n_live);
+  if (n_live < rows && row_utt[n_live] == row_utt[n_live - 1])
+    return fail(MB_ERR_INVALID, "%s: the live rows end inside utterance %d", fn, row_utt[n_live]);
+  if (!h->finalized) return fail(MB_ERR_STATE, "%s: weights not finalized", fn);
+  if (h->cond_frames.empty() || h->cond_ws != workspace)
+    return fail(MB_ERR_STATE, "%s: call mb_wavernn_condition_multi on this workspace first", fn);
+  const int U = (int)h->cond_frames.size();
+  for (int r = 0; r < rows; ++r)
+    if (row_utt[r] >= U) return fail(MB_ERR_INVALID, "%s: row %d names utterance %d of %d", fn, r, row_utt[r], U);
+  return sample_chunk(fn, h, rows, n_live, n_live, max_steps, step0, nsteps, noise, out_idx, out_x, workspace, workspace_bytes,
+                      stream, [&](int32_t* c, int32_t* n, uint64_t* sd) {
+                        std::vector<int32_t> fbase(U);
+                        for (int u = 0, f = 0; u < U; f += h->cond_frames[u], ++u) fbase[u] = f;
+                        for (int r = 0, first = 0; r < rows; ++r) {
+                          const int u = row_utt[r];
+                          if (row_fold[r] == 0) first = r;
+                          c[4 * r + 0] = row_start[r];
+                          c[4 * r + 1] = h->cond_frames[u];
+                          c[4 * r + 2] = fbase[u] + u;
+                          c[4 * r + 3] = fbase[u];
+                          n[4 * r + 0] = row_steps[r];
+                          n[4 * r + 1] = row_fold[r];
+                          n[4 * r + 2] = first;
+                          sd[r] = utt_seeds ? utt_seeds[u] : 0;
+                        }
+                        for (int r = rows - 1, nf = 0; r >= 0; --r) {  // folds of the row's utterance
+                          if (r == rows - 1 || row_fold[r + 1] == 0) nf = row_fold[r] + 1;
+                          n[4 * r + 3] = nf;
+                        }
+                      });
+}
+
 }  // namespace
 
 extern "C" {
+
+int mb_wavernn_generate(mb_wavernn* h, const int32_t* fold_starts_host, int32_t B, int32_t steps, int32_t step0,
+                        int32_t nsteps, const float* noise, uint64_t seed, int16_t* out_idx, void* workspace,
+                        size_t workspace_bytes, void* stream) {
+  return mb_wavernn_generate_rows(h, fold_starts_host, B, steps, step0, nsteps, noise, B, 0, seed, out_idx, workspace,
+                                  workspace_bytes, stream);
+}
 
 int mb_wavernn_generate_rows(mb_wavernn* h, const int32_t* fold_starts_host, int32_t B, int32_t steps, int32_t step0,
                              int32_t nsteps, const float* noise, int32_t noise_folds, int32_t row0, uint64_t seed,
                              int16_t* out_idx, void* workspace, size_t workspace_bytes, void* stream) {
   if (!h || !fold_starts_host || !out_idx || !workspace) return fail(MB_ERR_INVALID, "mb_wavernn_generate: null argument");
   if (h->mode != MB_WAVERNN_RAW) return fail(MB_ERR_INVALID, "mb_wavernn_generate_rows: a MOL handle samples floats (mb_wavernn_generate_rows_mol)");
-  return generate_rows_impl(h, fold_starts_host, B, steps, step0, nsteps, noise, noise_folds, row0, seed, out_idx, nullptr,
-                            workspace, workspace_bytes, stream);
+  return generate_folds(h, fold_starts_host, B, steps, step0, nsteps, noise, noise_folds, row0, seed, out_idx, nullptr, workspace,
+                        workspace_bytes, stream);
 }
 
 int mb_wavernn_generate_rows_mol(mb_wavernn* h, const int32_t* fold_starts_host, int32_t B, int32_t steps, int32_t step0,
@@ -1162,8 +1165,8 @@ int mb_wavernn_generate_rows_mol(mb_wavernn* h, const int32_t* fold_starts_host,
                                  float* out_x, void* workspace, size_t workspace_bytes, void* stream) {
   if (!h || !fold_starts_host || !out_x || !workspace) return fail(MB_ERR_INVALID, "mb_wavernn_generate_rows_mol: null argument");
   if (h->mode != MB_WAVERNN_MOL) return fail(MB_ERR_INVALID, "mb_wavernn_generate_rows_mol: the handle was not created in MOL mode");
-  return generate_rows_impl(h, fold_starts_host, B, steps, step0, nsteps, uniforms, noise_folds, row0, seed, nullptr, out_x,
-                            workspace, workspace_bytes, stream);
+  return generate_folds(h, fold_starts_host, B, steps, step0, nsteps, uniforms, noise_folds, row0, seed, nullptr, out_x, workspace,
+                        workspace_bytes, stream);
 }
 
 int mb_wavernn_last_logits(mb_wavernn* h, float* logits, int32_t B, void* workspace, void* stream) {
@@ -1182,104 +1185,6 @@ int mb_wavernn_last_logits(mb_wavernn* h, float* logits, int32_t B, void* worksp
                                     sizeof(float), ncls, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return MB_OK;
 }
-
-}  // extern "C"
-
-// =================================================================================================
-// several utterances in one sample loop
-// =================================================================================================
-namespace {
-
-int generate_multi_impl(const char* fn, mb_wavernn* h, const int32_t* row_utt, const int32_t* row_start,
-                        const int32_t* row_steps, const int32_t* row_fold, int32_t rows, const uint64_t* utt_seeds,
-                        int32_t max_steps, int32_t step0, int32_t nsteps, int32_t n_live, const float* noise, int16_t* out_idx,
-                        float* out_x, void* workspace, size_t workspace_bytes, void* stream) {
-  if (rows <= 0 || max_steps <= 0 || nsteps <= 0 || nsteps > kChunkMax || step0 < 0 || step0 + nsteps > max_steps)
-    return fail(MB_ERR_INVALID, "%s: bad row count or step range (at most %d steps per call)", fn, kChunkMax);
-  // the row table: whole utterances side by side (folds 0 .. n-1 of one utterance, all of one length), longest rows first
-  int alive = 0;
-  for (int r = 0; r < rows; ++r) {
-    if (row_utt[r] < 0 || row_start[r] < 0 || row_steps[r] <= 0 || row_steps[r] > max_steps || row_fold[r] < 0)
-      return fail(MB_ERR_INVALID, "%s: row %d (utterance %d, start %d, steps %d, fold %d) outside the table", fn, r, row_utt[r],
-                  row_start[r], row_steps[r], row_fold[r]);
-    if (r > 0 && row_steps[r] > row_steps[r - 1]) return fail(MB_ERR_INVALID, "%s: rows must be ordered longest first (row %d)", fn, r);
-    const bool cont = r > 0 && row_utt[r] == row_utt[r - 1];
-    if (cont ? (row_fold[r] != row_fold[r - 1] + 1 || row_steps[r] != row_steps[r - 1]) : row_fold[r] != 0)
-      return fail(MB_ERR_INVALID, "%s: the folds of an utterance must be adjacent rows 0, 1, .. of one length (row %d)", fn, r);
-    alive += row_steps[r] > step0;
-  }
-  if (n_live != alive)
-    return fail(MB_ERR_INVALID, "%s: %d rows are alive at step %d, the call says %d", fn, alive, step0, n_live);
-  if (n_live < rows && row_utt[n_live] == row_utt[n_live - 1])
-    return fail(MB_ERR_INVALID, "%s: the live rows end inside utterance %d", fn, row_utt[n_live]);
-  if (!h->finalized) return fail(MB_ERR_STATE, "%s: weights not finalized", fn);
-  if (h->cond_frames.empty() || h->cond_ws != workspace)
-    return fail(MB_ERR_STATE, "%s: call mb_wavernn_condition_multi on this workspace first", fn);
-  const int U = (int)h->cond_frames.size();
-  int Ttot = 0;
-  for (int t : h->cond_frames) Ttot += t;
-  for (int r = 0; r < rows; ++r)
-    if (row_utt[r] >= U) return fail(MB_ERR_INVALID, "%s: row %d names utterance %d of %d", fn, r, row_utt[r], U);
-  const int Bpad = bpad_of(rows);
-  const Ws L = ws_layout(Ttot, Bpad, kChunkMax, U);
-  float* ws;
-  if (int rc = bind(fn, workspace, workspace_bytes, L.total, &ws)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  int4* rowc = reinterpret_cast<int4*>(ws + L.rowdesc);
-  int4* rown = rowc + Bpad;
-  uint64_t* rowseed = reinterpret_cast<uint64_t*>(rown + Bpad);
-  if (step0 == 0) {
-    // zero initial state and upload the row descriptors (rows past the table: T_u == 0, never live)
-    MB_CUDA_CHECK(cudaMemsetAsync(ws + L.h1, 0, sizeof(float) * (L.xprev + align_up((size_t)Bpad, 64) - L.h1), st));
-    std::vector<int32_t> fbase(U);
-    for (int u = 0, f = 0; u < U; f += h->cond_frames[u], ++u) fbase[u] = f;
-    std::vector<int32_t> tmp((size_t)10 * Bpad, 0);
-    int32_t* c = tmp.data();
-    int32_t* n = c + 4 * Bpad;
-    uint64_t* sd = reinterpret_cast<uint64_t*>(n + 4 * Bpad);
-    for (int r = 0, first = 0; r < rows; ++r) {
-      const int u = row_utt[r];
-      if (row_fold[r] == 0) first = r;
-      c[4 * r + 0] = row_start[r];
-      c[4 * r + 1] = h->cond_frames[u];
-      c[4 * r + 2] = fbase[u] + u;
-      c[4 * r + 3] = fbase[u];
-      n[4 * r + 0] = row_steps[r];
-      n[4 * r + 1] = row_fold[r];
-      n[4 * r + 2] = first;
-      sd[r] = utt_seeds ? utt_seeds[u] : 0;
-    }
-    for (int r = rows - 1, nf = 0; r >= 0; --r) {  // folds of the row's utterance
-      if (r == rows - 1 || row_fold[r + 1] == 0) nf = row_fold[r] + 1;
-      n[4 * r + 3] = nf;
-    }
-    MB_CUDA_CHECK(cudaMemcpyAsync(rowc, tmp.data(), sizeof(int32_t) * tmp.size(), cudaMemcpyHostToDevice, st));
-    MB_CUDA_CHECK(cudaStreamSynchronize(st));  // tmp goes out of scope
-  }
-  const int Wl = bpad_of(n_live);  // rows of the live row blocks
-  k_condI_multi<<<nsteps * Wl, 256, 0, st>>>(W(h, "I.weight"), W(h, "I.bias"), ws + L.melup, ws + L.aux, rowc, Wl, Bpad, step0,
-                                             nsteps, ws + L.condI);
-  MB_LAUNCH_CHECK("k_condI_multi");
-  LoopParams p;
-  memset(&p, 0, sizeof(p));
-  p.B = n_live;
-  p.Bpad = Bpad;
-  p.step0 = step0;
-  p.nsteps = nsteps;
-  p.steps_total = max_steps;
-  p.noise = noise;
-  p.noise_B = n_live;
-  p.out_idx = out_idx;
-  p.out_x = out_x;
-  p.rowc = rowc;
-  p.rown = rown;
-  p.rowseed = rowseed;
-  return launch_sample_loop(h, p, L, ws, true, st);
-}
-
-}  // namespace
-
-extern "C" {
 
 int mb_wavernn_generate_multi(mb_wavernn* h, const int32_t* row_utt, const int32_t* row_start, const int32_t* row_steps,
                               const int32_t* row_fold, int32_t rows, const uint64_t* utt_seeds, int32_t max_steps,

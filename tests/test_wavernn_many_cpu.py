@@ -97,11 +97,46 @@ def test_abi_argument_checks():
     refused(gen(G, raw._handle, [0], [0], [200], [0], 200, 150, 100, 1), "step range")
     refused(gen(G, raw._handle, [0], [0], [200], [0], 200, 0, 129, 1), "step range")
     refused(gen(G, raw._handle, [0, -1], [0, 0], [200, 200], [0, 0], 200, 0, 100, 2), "outside the table")
+    refused(gen(G, raw._handle, [0], [2 ** 31 - 100], [200], [0], 200, 0, 100, 1), "outside the table")  # start + step overflows
     refused(gen(G, raw._handle, [0, 1], [0, 0], [200, 400], [0, 0], 400, 0, 100, 2), "longest first")
     refused(gen(G, raw._handle, [0, 0], [0, 340], [380, 380], [0, 2], 380, 0, 100, 2), "folds of an utterance")
     refused(gen(G, raw._handle, [0, 1], [0, 0], [400, 200], [0, 0], 400, 200, 100, 2), "rows are alive")
     refused(gen(G, raw._handle, [0, 1], [0, 0], [400, 200], [0, 0], 400, 200, 100, 1, noise=None, seeds=u64(1, 2)),
             "weights not finalized")
+
+
+def test_single_abi_argument_checks():
+    """mb_wavernn_generate_rows[_mol] on an unfinalized handle: each bad argument is refused with its own message, before
+    "weights not finalized" and before any launch"""
+    raw, mol = WaveRNN(*ARGS), WaveRNN(*ARGS, mode="MOL")
+    L = _lib.lib()
+    i32 = lambda *a: (C.c_int32 * len(a))(*a)
+    p = C.c_void_p(256)  # never dereferenced: every call below is refused first
+    launches = L.mb_launch_count()
+
+    def gen(m, starts, steps=200, step0=0, n=100, noise=p, noise_folds=None, row0=0):
+        fn = L.mb_wavernn_generate_rows_mol if m.mode == "MOL" else L.mb_wavernn_generate_rows
+        folds = len(starts) if noise_folds is None else noise_folds
+        return fn(m._handle, i32(*starts), len(starts), steps, step0, n, noise, folds, row0, 0, p, p, 1 << 30, None)
+
+    def refused(status, code, text):
+        assert status == code, L.mb_last_error()
+        assert text in L.mb_last_error().decode()
+
+    for m in (raw, mol):
+        refused(gen(m, [0, -1]), 1, "fold start -1 of row 1")
+        refused(gen(m, [0, 2 ** 31 - 150]), 1, "fold start")
+        refused(gen(m, [0, 340], noise_folds=3, row0=2), 1, "outside the 3 noise rows")
+        refused(gen(m, [0], row0=-1, noise=None), 1, "outside the")
+        refused(gen(m, [0], n=129), 1, "bad step range")
+        refused(gen(m, [0], step0=150, n=100), 1, "bad step range")
+        refused(gen(m, [0, 340], noise_folds=5, row0=3), 2, "weights not finalized")
+    other = L.mb_wavernn_generate_rows_mol(raw._handle, i32(0), 1, 200, 0, 100, p, 1, 0, 0, p, p, 1 << 30, None)
+    refused(other, 1, "not created in MOL mode")
+    refused(L.mb_wavernn_generate_rows(mol._handle, i32(0), 1, 200, 0, 100, p, 1, 0, 0, p, p, 1 << 30, None), 1,
+            "MOL handle samples floats")
+    refused(L.mb_wavernn_generate(raw._handle, i32(-5), 1, 200, 0, 100, p, 0, p, p, 1 << 30, None), 1, "fold start -5")
+    assert L.mb_launch_count() == launches
 
 
 def _draw_reference(model, B, steps):

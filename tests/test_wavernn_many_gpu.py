@@ -1,5 +1,5 @@
 """GPU tests of the multi-utterance WaveRNN sample loop (WaveRNN.generate_many, mb_wavernn_condition_multi /
-mb_wavernn_generate_multi[_mol], k_sample_loop<MOL, true>): every utterance of a batch is bit for bit what the
+mb_wavernn_generate_multi[_mol], k_sample_loop<MOL>): every utterance of a batch is bit for bit what the
 single-utterance call returns for it alone - conditioning tables, ragged lengths, per-utterance noise, RAW and MOL."""
 import ctypes as C
 import json
