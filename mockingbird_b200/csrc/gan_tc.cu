@@ -335,6 +335,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(const __grid_con
       // set (MT x N / 2 <= 64 of them; 128 spill), they are issued one unit ahead, before the previous unit goes through shared
       // memory.
       constexpr bool kLoadAhead = MT * N / 2 <= 64;
+      static_assert(!kLoadAhead || kUnits % 2 == 0, "the load-ahead loop runs units in pairs");
       constexpr int kSets = kLoadAhead ? 2 : 1;
       float4 rv[kSets][UC / 4], ov[kSets][UC / 4];
       uint4 rh[kSets][UC / 8];
@@ -380,115 +381,126 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(const __grid_con
           for (int j = 0; j < UC / 4; ++j) ov[j] = reinterpret_cast<const float4*>(p.y32)[i32 + (size_t)j * p.Lout];
         }
       };
-      if constexpr (kLoadAhead) load_unit(0, rv[0], ov[0], rh[0]);
+      // unit k: staging, bias, residual, running sum, length mask, outputs.  The unit loops below stay rolled (k is a run-time
+      // index): unrolled, the epilogue's copies of this body made the hot loop of an instance overflow the instruction cache.
+      auto unit = [&](int k, const float4 (&rvk)[UC / 4], const float4 (&ovk)[UC / 4], const uint4 (&rhk)[UC / 8]) {
+        const int mt = k / (N / 32), u = k % (N / 32);
+        const int col0 = u * 32 + col_half;
+        const int q = wi.m0 + (g * MT + mt) * 64 + row_in_tile;
+        const int lo = q * p.stride + wi.r;
+        const bool inb = q < p.Lin && (g * MT + mt) * 64 + row_in_tile < p.rows_item;
+        const bool live = inb && lo < valid_out;
+        const size_t i32 = ((size_t)wi.b * C4 + (col0 >> 2)) * p.Lout + lo;  // + g * Lout per 4 channels
+        __syncwarp();  // this warp has read back the previous unit's rows (lanes that skipped a unit still arrive here)
 #pragma unroll
-      for (int k = 0; k < kUnits; ++k) {
-        {
-          const int mt = k / (N / 32), u = k % (N / 32);
-          const int col0 = u * 32 + col_half;
-          const int q = wi.m0 + (g * MT + mt) * 64 + row_in_tile;
-          const int lo = q * p.stride + wi.r;
-          const bool inb = q < p.Lin && (g * MT + mt) * 64 + row_in_tile < p.rows_item;
-          const bool live = inb && lo < valid_out;
-          const size_t i32 = ((size_t)wi.b * C4 + (col0 >> 2)) * p.Lout + lo;  // + g * Lout per 4 channels
-          if (!kLoadAhead) load_unit(k, rv[0], ov[0], rh[0]);
-          else if (k + 1 < kUnits) load_unit(k + 1, rv[(k + 1) % kSets], ov[(k + 1) % kSets], rh[(k + 1) % kSets]);
-          const float4(&rvk)[UC / 4] = rv[k % kSets];
-          const float4(&ovk)[UC / 4] = ov[k % kSets];
-          const uint4(&rhk)[UC / 8] = rh[k % kSets];
-          __syncwarp();  // this warp has read back the previous unit's rows (lanes that skipped a unit still arrive here)
-          stage_acc32(stage, &acc[mt][u * 16], tid);
-          __syncwarp();
-          if (!inb) continue;
-          float v[UC];
-          const float4* srow = reinterpret_cast<const float4*>(stage + row_in_tile * kStageLd + col_half);
+        for (int kk = 0; kk < kUnits; ++kk)  // k is a run-time index: the slice's registers are picked by comparison
+          if (kk == k) stage_acc32(stage, &acc[kk / (N / 32)][(kk % (N / 32)) * 16], tid);
+        __syncwarp();
+        if (!inb) return;
+        float v[UC];
+        const float4* srow = reinterpret_cast<const float4*>(stage + row_in_tile * kStageLd + col_half);
+#pragma unroll
+        for (int j = 0; j < UC / 4; ++j) {
+          const float4 s = srow[j];
+          v[4 * j + 0] = s.x * p.acc_scale + bias_s[col0 + 4 * j + 0];
+          v[4 * j + 1] = s.y * p.acc_scale + bias_s[col0 + 4 * j + 1];
+          v[4 * j + 2] = s.z * p.acc_scale + bias_s[col0 + 4 * j + 2];
+          v[4 * j + 3] = s.w * p.acc_scale + bias_s[col0 + 4 * j + 3];
+        }
+        if (p.res32) {
 #pragma unroll
           for (int j = 0; j < UC / 4; ++j) {
-            const float4 s = srow[j];
-            v[4 * j + 0] = s.x * p.acc_scale + bias_s[col0 + 4 * j + 0];
-            v[4 * j + 1] = s.y * p.acc_scale + bias_s[col0 + 4 * j + 1];
-            v[4 * j + 2] = s.z * p.acc_scale + bias_s[col0 + 4 * j + 2];
-            v[4 * j + 3] = s.w * p.acc_scale + bias_s[col0 + 4 * j + 3];
+            v[4 * j + 0] += rvk[j].x; v[4 * j + 1] += rvk[j].y; v[4 * j + 2] += rvk[j].z; v[4 * j + 3] += rvk[j].w;
           }
-          if (p.res32) {
+        }
+        if (p.res16) {
 #pragma unroll
-            for (int j = 0; j < UC / 4; ++j) {
-              v[4 * j + 0] += rvk[j].x; v[4 * j + 1] += rvk[j].y; v[4 * j + 2] += rvk[j].z; v[4 * j + 3] += rvk[j].w;
-            }
+          for (int j = 0; j < UC / 8; ++j) {
+            if (p.res_hilo) add_res16_hilo(&v[8 * j], rhk[j], *reinterpret_cast<const uint4*>(&rvk[j]), p.res_inv);
+            else add_res16(&v[8 * j], rhk[j], p.res_inv);
           }
-          if (p.res16) {
+        }
+        if (p.mode != EPI_STORE && !p.red_add) {
 #pragma unroll
-            for (int j = 0; j < UC / 8; ++j) {
-              if (p.res_hilo) add_res16_hilo(&v[8 * j], rhk[j], *reinterpret_cast<const uint4*>(&rvk[j]), p.res_inv);
-              else add_res16(&v[8 * j], rhk[j], p.res_inv);
-            }
+          for (int j = 0; j < UC / 4; ++j) {
+            v[4 * j + 0] += ovk[j].x; v[4 * j + 1] += ovk[j].y; v[4 * j + 2] += ovk[j].z; v[4 * j + 3] += ovk[j].w;
           }
-          if (p.mode != EPI_STORE && !p.red_add) {
+          if (p.mode == EPI_ADD_DIV) {
 #pragma unroll
-            for (int j = 0; j < UC / 4; ++j) {
-              v[4 * j + 0] += ovk[j].x; v[4 * j + 1] += ovk[j].y; v[4 * j + 2] += ovk[j].z; v[4 * j + 3] += ovk[j].w;
-            }
-            if (p.mode == EPI_ADD_DIV) {
-#pragma unroll
-              for (int i = 0; i < UC; ++i) v[i] /= p.div;
-            }
+            for (int i = 0; i < UC; ++i) v[i] /= p.div;
           }
-          if (!live) {
+        }
+        if (!live) {
 #pragma unroll
-            for (int i = 0; i < UC; ++i) v[i] = 0.f;
-          }
-          if (p.red_add) {  // MRF sum of a middle resblock: S += v by vector reductions in L2 (rows past the length add nothing)
-            if (live) {
-#pragma unroll
-              for (int j = 0; j < UC / 4; ++j)
-                red_add_f32x4(p.y32 + (i32 + (size_t)j * p.Lout) * 4, v[4 * j + 0], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-            }
-          } else if (p.y32) {
+          for (int i = 0; i < UC; ++i) v[i] = 0.f;
+        }
+        if (p.red_add) {  // MRF sum of a middle resblock: S += v by vector reductions in L2 (rows past the length add nothing)
+          if (live) {
 #pragma unroll
             for (int j = 0; j < UC / 4; ++j)
-              reinterpret_cast<float4*>(p.y32)[i32 + (size_t)j * p.Lout] =
-                  make_float4(v[4 * j + 0], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+              red_add_f32x4(p.y32 + (i32 + (size_t)j * p.Lout) * 4, v[4 * j + 0], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
           }
-          if (p.y16) {
-            const int rr = kPadRows + lo;
-            const int ysw = f16_swz(p.y_cw, rr);
-            const int ycw8 = p.y_cw >> 3;
+        } else if (p.y32) {
 #pragma unroll
-            for (int j = 0; j < UC / 8; ++j) {
-              float a[8];
+          for (int j = 0; j < UC / 4; ++j)
+            reinterpret_cast<float4*>(p.y32)[i32 + (size_t)j * p.Lout] =
+                make_float4(v[4 * j + 0], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+        }
+        if (p.y16) {
+          const int rr = kPadRows + lo;
+          const int ysw = f16_swz(p.y_cw, rr);
+          const int ycw8 = p.y_cw >> 3;
 #pragma unroll
-              for (int e = 0; e < 8; ++e) a[e] = lrelu(v[8 * j + e], p.out_slope);
-              __half2 h[4];
+          for (int j = 0; j < UC / 8; ++j) {
+            float a[8];
 #pragma unroll
-              for (int e = 0; e < 4; ++e) h[e] = __floats2half2_rn(a[2 * e], a[2 * e + 1]);
-              uint4 pk;
-              pk.x = *reinterpret_cast<uint32_t*>(&h[0]);
-              pk.y = *reinterpret_cast<uint32_t*>(&h[1]);
-              pk.z = *reinterpret_cast<uint32_t*>(&h[2]);
-              pk.w = *reinterpret_cast<uint32_t*>(&h[3]);
-              const int ct = p.y_c0 + col0 + 8 * j;  // channel of the (hi) block
-              const int chunk = ct / p.y_cw, cc = ct - chunk * p.y_cw;
-              const size_t i16 = (((size_t)wi.b * p.y_nchunks + chunk) * p.y_Lp + rr) * (size_t)ycw8 + (size_t)((cc >> 3) ^ ysw);
-              reinterpret_cast<uint4*>(p.y16)[i16] = pk;
-              if (p.y_lo_c >= 0) {
-                __half2 l2[4];
+            for (int e = 0; e < 8; ++e) a[e] = lrelu(v[8 * j + e], p.out_slope);
+            __half2 h[4];
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const float2 hf = __half22float2(h[e]);
-                  l2[e] = __floats2half2_rn(a[2 * e] - hf.x, a[2 * e + 1] - hf.y);
-                }
-                uint4 pl;
-                pl.x = *reinterpret_cast<uint32_t*>(&l2[0]);
-                pl.y = *reinterpret_cast<uint32_t*>(&l2[1]);
-                pl.z = *reinterpret_cast<uint32_t*>(&l2[2]);
-                pl.w = *reinterpret_cast<uint32_t*>(&l2[3]);
-                const int ctl = ct + p.y_lo_c;
-                const int chl = ctl / p.y_cw, ccl = ctl - chl * p.y_cw;
-                const size_t j16 = (((size_t)wi.b * p.y_nchunks + chl) * p.y_Lp + rr) * (size_t)ycw8 + (size_t)((ccl >> 3) ^ ysw);
-                reinterpret_cast<uint4*>(p.y16)[j16] = pl;
+            for (int e = 0; e < 4; ++e) h[e] = __floats2half2_rn(a[2 * e], a[2 * e + 1]);
+            uint4 pk;
+            pk.x = *reinterpret_cast<uint32_t*>(&h[0]);
+            pk.y = *reinterpret_cast<uint32_t*>(&h[1]);
+            pk.z = *reinterpret_cast<uint32_t*>(&h[2]);
+            pk.w = *reinterpret_cast<uint32_t*>(&h[3]);
+            const int ct = p.y_c0 + col0 + 8 * j;  // channel of the (hi) block
+            const int chunk = ct / p.y_cw, cc = ct - chunk * p.y_cw;
+            const size_t i16 = (((size_t)wi.b * p.y_nchunks + chunk) * p.y_Lp + rr) * (size_t)ycw8 + (size_t)((cc >> 3) ^ ysw);
+            reinterpret_cast<uint4*>(p.y16)[i16] = pk;
+            if (p.y_lo_c >= 0) {
+              __half2 l2[4];
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const float2 hf = __half22float2(h[e]);
+                l2[e] = __floats2half2_rn(a[2 * e] - hf.x, a[2 * e + 1] - hf.y);
               }
+              uint4 pl;
+              pl.x = *reinterpret_cast<uint32_t*>(&l2[0]);
+              pl.y = *reinterpret_cast<uint32_t*>(&l2[1]);
+              pl.z = *reinterpret_cast<uint32_t*>(&l2[2]);
+              pl.w = *reinterpret_cast<uint32_t*>(&l2[3]);
+              const int ctl = ct + p.y_lo_c;
+              const int chl = ctl / p.y_cw, ccl = ctl - chl * p.y_cw;
+              const size_t j16 = (((size_t)wi.b * p.y_nchunks + chl) * p.y_Lp + rr) * (size_t)ycw8 + (size_t)((ccl >> 3) ^ ysw);
+              reinterpret_cast<uint4*>(p.y16)[j16] = pl;
             }
           }
+        }
+      };
+      if constexpr (kLoadAhead) {
+        load_unit(0, rv[0], ov[0], rh[0]);
+#pragma unroll 1
+        for (int k = 0; k < kUnits; k += 2) {
+          load_unit(k + 1, rv[1], ov[1], rh[1]);
+          unit(k, rv[0], ov[0], rh[0]);
+          if (k + 2 < kUnits) load_unit(k + 2, rv[0], ov[0], rh[0]);
+          unit(k + 1, rv[1], ov[1], rh[1]);
+        }
+      } else {
+#pragma unroll 1
+        for (int k = 0; k < kUnits; ++k) {
+          load_unit(k, rv[0], ov[0], rh[0]);
+          unit(k, rv[0], ov[0], rh[0]);
         }
       }
       if (win_a >= 0) {  // every lane of this warp is done with the operand window
