@@ -24,7 +24,7 @@ sys.path.insert(0, str(ROOT / "synth_weights"))
 sys.path.insert(0, str(ROOT / "oracle"))
 
 from bench_ppg2mel import card  # noqa: E402
-from bench_vc import cuda_timed, vocode_on_device, vocoder  # noqa: E402
+from bench_vc import cuda_timed, vocoder  # noqa: E402
 
 SR = 16000
 
@@ -78,6 +78,7 @@ def main():
         import ref_init as ri
         from mockingbird_b200.ppg2mel import MelDecoderMOLv2
         from mockingbird_b200.ppg_extractor import build_model
+        from mockingbird_b200.vocoder._gan import infer_waveforms_batched
 
         m = build_model(ri.PPGX_CONFIG)
         m.load_state_dict(ri.ppg_extractor_state_dict(ri.PPGX_CONFIG, 0))
@@ -98,7 +99,7 @@ def main():
                 n = min(p.shape[0], len(l))  # as run.py and the toolbox trim them
                 utts.append((p[:n], torch.from_numpy(l[:n]).float().cuda()))
             outs = dec.inference_batch(utts, spk, seed=3)
-            return vocode_on_device(voc, [o[1].t() for o in outs])
+            return infer_waveforms_batched(voc, "cuda", [o[1].t() for o in outs])
 
         with torch.no_grad():
             ms_c, wavs = cuda_timed(chain, 2, 1)

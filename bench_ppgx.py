@@ -25,7 +25,7 @@ sys.path.insert(0, str(ROOT))
 sys.path.insert(0, str(ROOT / "synth_weights"))
 
 from bench_ppg2mel import card  # noqa: E402
-from bench_vc import cuda_timed, vocode_on_device, vocoder  # noqa: E402
+from bench_vc import cuda_timed, vocoder  # noqa: E402
 
 SR = 16000
 
@@ -51,6 +51,7 @@ def main():
     import ref_init as ri
     from mockingbird_b200.ppg2mel import MelDecoderMOLv2
     from mockingbird_b200.ppg_extractor import build_model
+    from mockingbird_b200.vocoder._gan import infer_waveforms_batched
 
     if not torch.cuda.is_available():
         raise SystemExit("bench_ppgx.py needs a CUDA device")
@@ -125,7 +126,7 @@ def main():
             utts.append((p, lf0))
         outs = dec.inference_batch(utts, spk, seed=3)
         mels = [o[1].t() for o in outs]
-        return feats, vocode_on_device(voc, mels)
+        return feats, infer_waveforms_batched(voc, "cuda", mels)
 
     with torch.no_grad():
         ms_c, (feats, outw) = cuda_timed(chain, max(1, a.iters // 2), 1)

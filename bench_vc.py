@@ -59,25 +59,6 @@ def vocoder(cfg, sd, precision):
     return g
 
 
-def vocode_on_device(g, mels, batch=32):
-    """[80, T_i] device mels -> list of [T_i * hop] device waveforms, as length-sorted padded batches with per-row lengths"""
-    import torch
-
-    order = sorted(range(len(mels)), key=lambda i: -mels[i].shape[1])
-    out = [None] * len(mels)
-    for s in range(0, len(order), batch):
-        idx = order[s:s + batch]
-        tmax = mels[idx[0]].shape[1]
-        x = torch.zeros(len(idx), 80, tmax, device="cuda")
-        for r, i in enumerate(idx):
-            x[r, :, : mels[i].shape[1]] = mels[i]
-        lens = torch.tensor([mels[i].shape[1] for i in idx], dtype=torch.int32, device="cuda")
-        wav = g(x, lengths=lens)
-        for r, i in enumerate(idx):
-            out[i] = wav[r, 0, : mels[i].shape[1] * g.hop]
-    return out
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=10)
@@ -88,6 +69,7 @@ def main():
 
     import ref_init as ri
     from mockingbird_b200.ppg2mel import MelDecoderMOLv2
+    from mockingbird_b200.vocoder._gan import infer_waveforms_batched
 
     if not torch.cuda.is_available():
         raise SystemExit("bench_vc.py needs a CUDA device")
@@ -142,7 +124,7 @@ def main():
     def vc():
         outs = model.inference_batch(utts, spk, seed=3)
         mels = [o[1].t() if o[1].shape[-1] == 80 else o[1] for o in outs]  # postnet mel as [80, T]
-        return mels, vocode_on_device(g_auto, mels)
+        return mels, infer_waveforms_batched(g_auto, "cuda", mels)
 
     with torch.no_grad():
         ms, (mels, wavs) = cuda_timed(vc, max(1, a.iters // 2), 1)

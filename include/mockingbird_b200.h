@@ -1041,6 +1041,17 @@ int mb_ppg2mel_inference(mb_ppg2mel* h, const float* ppg, const float* lf0_uv, c
                          float* mel, float* mel_post, float* align, float* stop, int32_t* steps_host, void* workspace,
                          size_t workspace_bytes, void* stream);
 
+/* mb_ppg2mel_inference with one dropout stream per row, so that a row's result does not depend on the batch around it:
+ *   seeds uint64 [B] (device): row b draws its PreNet keep flags exactly as the only row of a B = 1 mb_ppg2mel_inference
+ *     call with seed = seeds[b] (Philox keyed by step, row 0 and unit).  The table is copied into the workspace before
+ *     the decoder runs (the workspace holds room for it: mb_ppg2mel_workspace_bytes counts B seeds); the captured decoder
+ *     steps read it from there.
+ * Every other argument, output and error is mb_ppg2mel_inference's; a NULL seed table is MB_ERR_INVALID. */
+int mb_ppg2mel_inference_rows(mb_ppg2mel* h, const float* ppg, const float* lf0_uv, const float* spk,
+                              const int32_t* lengths, int32_t batch, int32_t frames, const uint64_t* seeds, float* mel,
+                              float* mel_post, float* align, float* stop, int32_t* steps_host, void* workspace,
+                              size_t workspace_bytes, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Voice-conversion PPG extractor (Conformer ASR encoder)
  *   replaces  models/ppg_extractor/__init__.py:25-39 (PPGModel.forward: DefaultFrontend STFT + log-mel, UtteranceMVN,

@@ -446,6 +446,9 @@ SIGNATURES = {
     "mb_ppg2mel_inference": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32,
                                        C.c_int32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mb_ppg2mel_inference_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32,
+                                            C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.POINTER(C.c_int32), C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_ppgx_create": (C.c_int, [C.POINTER(PpgxConfig), C.POINTER(C.c_void_p)]),
     "mb_ppgx_destroy": (None, [C.c_void_p]),
     "mb_ppgx_arena_bytes": (C.c_size_t, [C.c_void_p]),

@@ -47,11 +47,13 @@ __device__ __forceinline__ float softplusf_(float x) { return x > 20.0f ? x : lo
 
 __device__ __forceinline__ bool row_active(const int* done_at, int b, int step) { return step < done_at[b]; }
 
+// key_row is the row index in the Philox counter: b for one stream per call, 0 for per-row streams (a row then draws
+// as the only row of a B = 1 call with its own seed)
 __device__ __forceinline__ bool keep_flag(const uint8_t* masks, int width, int B, int b, int step, int unit, int layer,
-                                          uint64_t seed) {
+                                          int key_row, uint64_t seed) {
   if (masks) return masks[((size_t)step * B + b) * width + unit] != 0;
   uint32_t o[4];
-  mb_philox4x32((uint32_t)unit >> 2, (uint32_t)b, (uint32_t)step, 0x70326d00u + (uint32_t)layer, (uint32_t)seed,
+  mb_philox4x32((uint32_t)unit >> 2, (uint32_t)key_row, (uint32_t)step, 0x70326d00u + (uint32_t)layer, (uint32_t)seed,
                 (uint32_t)(seed >> 32), o);
   return ((o[unit & 3] >> 16) & 1u) != 0;
 }
@@ -321,25 +323,30 @@ __device__ __forceinline__ void rows_active(int B, const int* done_at, int step,
 }
 
 // PreNet: Linear 80->256 (no bias) -> ReLU -> dropout(0.5, always on) -> Linear 256->128 -> ReLU -> dropout.
-// Weights transposed ([in][out]) so that the per-unit loops read coalesced.  grid B, block 256
+// Weights transposed ([in][out]) so that the per-unit loops read coalesced.  Drawn keep flags come from one stream per
+// call (`seed`, keyed by row) or, when row_seeds is given, from row b's own seed row_seeds[b] keyed as row 0.  The table
+// is read at run time, so a captured graph serves any seeds.  grid B, block 256
 __global__ void __launch_bounds__(256) prenet_kernel(const float* frame, const float* W1t, const float* W2t,
-                                                     const uint8_t* m1, const uint8_t* m2, uint64_t seed, int B,
-                                                     const int* done_at, const int* g_step, float* out) {
+                                                     const uint8_t* m1, const uint8_t* m2, uint64_t seed,
+                                                     const uint64_t* row_seeds, int B, const int* done_at,
+                                                     const int* g_step, float* out) {
   __shared__ float x[kNM], h1[kP1];
   const int b = blockIdx.x, tid = threadIdx.x, step = *g_step;
   if (!row_active(done_at, b, step)) return;
+  const int key_row = row_seeds ? 0 : b;
+  if (row_seeds) seed = row_seeds[b];
   if (tid < kNM) x[tid] = frame[(size_t)b * kNM + tid];
   __syncthreads();
   float a = 0.0f;
   for (int k = 0; k < kNM; ++k) a += W1t[k * kP1 + tid] * x[k];
   a = a > 0.0f ? a : 0.0f;
-  h1[tid] = keep_flag(m1, kP1, B, b, step, tid, 1, seed) ? a * 2.0f : 0.0f;
+  h1[tid] = keep_flag(m1, kP1, B, b, step, tid, 1, key_row, seed) ? a * 2.0f : 0.0f;
   __syncthreads();
   if (tid < kP2) {
     float c = 0.0f;
     for (int k = 0; k < kP1; ++k) c += W2t[k * kP2 + tid] * h1[k];
     c = c > 0.0f ? c : 0.0f;
-    out[(size_t)b * kP2 + tid] = keep_flag(m2, kP2, B, b, step, tid, 2, seed) ? c * 2.0f : 0.0f;
+    out[(size_t)b * kP2 + tid] = keep_flag(m2, kP2, B, b, step, tid, 2, key_row, seed) ? c * 2.0f : 0.0f;
   }
 }
 
@@ -595,7 +602,7 @@ void build_specs(mb_ppg2mel* h) {
 
 // per-call workspace layout (byte offsets)
 struct Ws {
-  size_t ints, rowbias, x0, x1, e1, e2, mem, ah, ac, dh, dc, ctx, mu, frame, pre, q, p0, p1, total;
+  size_t ints, rowbias, x0, x1, e1, e2, mem, ah, ac, dh, dc, ctx, mu, frame, pre, q, p0, p1, seeds, total;
 };
 
 Ws ws_layout(int B, int T) {
@@ -620,6 +627,7 @@ Ws ws_layout(int B, int T) {
   L.q = W.take(sizeof(float) * (size_t)B * kQ);
   L.p0 = W.take(sizeof(float) * (size_t)B * 2 * S * 512);
   L.p1 = W.take(sizeof(float) * (size_t)B * 2 * S * 512);
+  L.seeds = W.take(sizeof(uint64_t) * (size_t)B);  // per-row dropout seeds (mb_ppg2mel_inference_rows)
   L.total = W.total();
   return L;
 }
@@ -790,32 +798,37 @@ size_t mb_ppg2mel_workspace_bytes(const mb_ppg2mel* h, int32_t batch, int32_t fr
   return ws_layout(batch, frames).total;
 }
 
-int mb_ppg2mel_inference(mb_ppg2mel* h, const float* ppg, const float* lf0_uv, const float* spk, const int32_t* lengths,
-                         int32_t batch, int32_t frames, const uint8_t* mask1, const uint8_t* mask2, uint64_t seed,
-                         float* mel, float* mel_post, float* align, float* stop, int32_t* steps_host, void* workspace,
-                         size_t workspace_bytes, void* stream) {
-  if (!h) return fail(MB_ERR_INVALID, "mb_ppg2mel_inference: null handle");
-  if (!h->finalized) return fail(MB_ERR_STATE, "mb_ppg2mel_inference: weights not finalized");
-  if (batch < 1 || batch > kMaxRows) return fail(MB_ERR_INVALID, "mb_ppg2mel_inference: batch %d outside 1..%d", batch, kMaxRows);
-  if (frames < 4) return fail(MB_ERR_INVALID, "mb_ppg2mel_inference: frames %d < 4", frames);
+}  // extern "C"
+
+namespace {
+
+// both entry points: `seeds` (device, one per row) selects per-row dropout streams; `fn` names the entry in messages
+int ppg2mel_run(const char* fn, mb_ppg2mel* h, const float* ppg, const float* lf0_uv, const float* spk,
+                const int32_t* lengths, int32_t batch, int32_t frames, const uint8_t* mask1, const uint8_t* mask2,
+                uint64_t seed, const uint64_t* seeds, float* mel, float* mel_post, float* align, float* stop,
+                int32_t* steps_host, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!h) return fail(MB_ERR_INVALID, "%s: null handle", fn);
+  if (!h->finalized) return fail(MB_ERR_STATE, "%s: weights not finalized", fn);
+  if (batch < 1 || batch > kMaxRows) return fail(MB_ERR_INVALID, "%s: batch %d outside 1..%d", fn, batch, kMaxRows);
+  if (frames < 4) return fail(MB_ERR_INVALID, "%s: frames %d < 4", fn, frames);
   const int te_max = max_att_tenc();
   if (te_max == 0) return MB_ERR_CUDA;
   if (frames / 4 > te_max)
-    return fail(MB_ERR_INVALID, "mb_ppg2mel_inference: frames %d gives T_enc %d > %d, the most the MoL attention's shared "
-                "memory holds (frames <= %d)", frames, frames / 4, te_max, 4 * te_max + 3);
+    return fail(MB_ERR_INVALID, "%s: frames %d gives T_enc %d > %d, the most the MoL attention's shared "
+                "memory holds (frames <= %d)", fn, frames, frames / 4, te_max, 4 * te_max + 3);
   if (!ppg || !lf0_uv || !spk || !lengths || !mel || !mel_post || !align || !steps_host)
-    return fail(MB_ERR_INVALID, "mb_ppg2mel_inference: null argument");
+    return fail(MB_ERR_INVALID, "%s: null argument", fn);
   if ((mask1 == nullptr) != (mask2 == nullptr))
-    return fail(MB_ERR_INVALID, "mb_ppg2mel_inference: pass both dropout masks or neither");
+    return fail(MB_ERR_INVALID, "%s: pass both dropout masks or neither", fn);
   Lens lens{};
   for (int b = 0; b < batch; ++b) {
     if (lengths[b] < 4 || lengths[b] > frames)
-      return fail(MB_ERR_INVALID, "mb_ppg2mel_inference: lengths[%d] = %d outside 4..%d", b, lengths[b], frames);
+      return fail(MB_ERR_INVALID, "%s: lengths[%d] = %d outside 4..%d", fn, b, lengths[b], frames);
     lens.v[b] = lengths[b];
   }
   const Ws L = ws_layout(batch, frames);
   char* ws;
-  if (int rc = mb::bind("mb_ppg2mel_inference", workspace, workspace_bytes, L.total, &ws)) return rc;
+  if (int rc = mb::bind(fn, workspace, workspace_bytes, L.total, &ws)) return rc;
   const int B = batch, T = frames, T1 = T / 2, T2 = T1 / 2, S = 2 * T2;
   const int Dp = h->cfg.bottle_neck_feature_dim, Ds = h->cfg.spk_embed_dim;
   auto F = [&](size_t off) { return reinterpret_cast<float*>(ws + off); };
@@ -839,6 +852,10 @@ int mb_ppg2mel_inference(mb_ppg2mel* h, const float* ppg, const float* lf0_uv, c
   MB_CUDA_CHECK(cudaMemsetAsync(align, 0, sizeof(float) * B * S * T2, st));
   if (stop) MB_CUDA_CHECK(cudaMemsetAsync(stop, 0, sizeof(float) * B * S, st));
   MB_CUDA_CHECK(cudaMemsetAsync(ws + L.ah, 0, L.p0 - L.ah, st));
+  // the caller's seed table is copied into the workspace, which is what the captured decoder steps read
+  const uint64_t* row_seeds = seeds ? reinterpret_cast<const uint64_t*>(ws + L.seeds) : nullptr;
+  if (seeds)
+    MB_CUDA_CHECK(cudaMemcpyAsync(ws + L.seeds, seeds, sizeof(uint64_t) * B, cudaMemcpyDeviceToDevice, st));
   init_state_kernel<<<1, kMaxRows, 0, st>>>(lens, B, s);
   MB_LAUNCH_CHECK("init_state_kernel");
 
@@ -896,8 +913,8 @@ int mb_ppg2mel_inference(mb_ppg2mel* h, const float* ppg, const float* lf0_uv, c
     float* ah_out = ah[parity ^ 1];
     const float* dh_in = dh[parity];
     float* dh_out = dh[parity ^ 1];
-    prenet_kernel<<<B, 256, 0, st>>>(F(L.frame), A + h->d_w1t, A + h->d_w2t, mask1, mask2, seed, B, s.done_at, s.g_step,
-                                     F(L.pre));
+    prenet_kernel<<<B, 256, 0, st>>>(F(L.frame), A + h->d_w1t, A + h->d_w2t, mask1, mask2, seed, row_seeds, B,
+                                     s.done_at, s.g_step, F(L.pre));
     MB_LAUNCH_CHECK("prenet_kernel");
     Segs a{};
     a.s[0] = {F(L.pre), kP2, kP2, h->p("decoder.attention_rnn.weight_ih"), kP2 + kE};
@@ -950,25 +967,25 @@ int mb_ppg2mel_inference(mb_ppg2mel* h, const float* ppg, const float* lf0_uv, c
     if (graph) cudaGraphDestroy(graph);
     return rc;
   }
-  if (ec != cudaSuccess || !graph) return fail(MB_ERR_CUDA, "mb_ppg2mel_inference: graph capture failed: %s", cudaGetErrorString(ec));
+  if (ec != cudaSuccess || !graph) return fail(MB_ERR_CUDA, "%s: graph capture failed: %s", fn, cudaGetErrorString(ec));
   if (cudaGraphInstantiate(&exec, graph, 0) != cudaSuccess) {
     cudaGraphDestroy(graph);
-    return fail(MB_ERR_CUDA, "mb_ppg2mel_inference: cudaGraphInstantiate failed");
+    return fail(MB_ERR_CUDA, "%s: cudaGraphInstantiate failed", fn);
   }
   int flag = 0;
   const int groups = (S + kGroup - 1) / kGroup;
   for (int g = 0; g < groups && !flag && rc == MB_OK; ++g) {
-    if (cudaGraphLaunch(exec, st) != cudaSuccess) rc = fail(MB_ERR_CUDA, "mb_ppg2mel_inference: cudaGraphLaunch failed");
+    if (cudaGraphLaunch(exec, st) != cudaSuccess) rc = fail(MB_ERR_CUDA, "%s: cudaGraphLaunch failed", fn);
     mb::count_launch(per_graph);
     if (rc == MB_OK && cudaMemcpyAsync(&flag, s.flag, sizeof(int), cudaMemcpyDeviceToHost, st) != cudaSuccess)
-      rc = fail(MB_ERR_CUDA, "mb_ppg2mel_inference: flag copy failed");
+      rc = fail(MB_ERR_CUDA, "%s: flag copy failed", fn);
     if (rc == MB_OK && cudaStreamSynchronize(st) != cudaSuccess)
-      rc = fail(MB_ERR_CUDA, "mb_ppg2mel_inference: decoder step failed: %s", cudaGetErrorString(cudaGetLastError()));
+      rc = fail(MB_ERR_CUDA, "%s: decoder step failed: %s", fn, cudaGetErrorString(cudaGetLastError()));
   }
   cudaGraphExecDestroy(exec);
   cudaGraphDestroy(graph);
   if (rc != MB_OK) return rc;
-  if (!flag) return fail(MB_ERR_STATE, "mb_ppg2mel_inference: rows still running after the step limit");
+  if (!flag) return fail(MB_ERR_STATE, "%s: rows still running after the step limit", fn);
   MB_CUDA_CHECK(cudaMemcpy(steps_host, s.steps, sizeof(int) * B, cudaMemcpyDeviceToHost));
   int nmax = 0;
   for (int b = 0; b < B; ++b) nmax = steps_host[b] > nmax ? steps_host[b] : nmax;
@@ -996,6 +1013,27 @@ int mb_ppg2mel_inference(mb_ppg2mel* h, const float* ppg, const float* lf0_uv, c
   MB_CUDA_CHECK(cudaEventRecord(h->ev_out, st));
   MB_CUDA_CHECK(cudaStreamWaitEvent(caller, h->ev_out, 0));
   return MB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mb_ppg2mel_inference(mb_ppg2mel* h, const float* ppg, const float* lf0_uv, const float* spk, const int32_t* lengths,
+                         int32_t batch, int32_t frames, const uint8_t* mask1, const uint8_t* mask2, uint64_t seed,
+                         float* mel, float* mel_post, float* align, float* stop, int32_t* steps_host, void* workspace,
+                         size_t workspace_bytes, void* stream) {
+  return ppg2mel_run("mb_ppg2mel_inference", h, ppg, lf0_uv, spk, lengths, batch, frames, mask1, mask2, seed, nullptr,
+                     mel, mel_post, align, stop, steps_host, workspace, workspace_bytes, stream);
+}
+
+int mb_ppg2mel_inference_rows(mb_ppg2mel* h, const float* ppg, const float* lf0_uv, const float* spk,
+                              const int32_t* lengths, int32_t batch, int32_t frames, const uint64_t* seeds, float* mel,
+                              float* mel_post, float* align, float* stop, int32_t* steps_host, void* workspace,
+                              size_t workspace_bytes, void* stream) {
+  if (!seeds) return fail(MB_ERR_INVALID, "mb_ppg2mel_inference_rows: null seed table");
+  return ppg2mel_run("mb_ppg2mel_inference_rows", h, ppg, lf0_uv, spk, lengths, batch, frames, nullptr, nullptr, 0, seeds,
+                     mel, mel_post, align, stop, steps_host, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

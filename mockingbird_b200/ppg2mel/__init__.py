@@ -7,6 +7,8 @@ for one utterance (B = 1), exactly as the reference returns them.  All layers ru
 The reference's decoder PreNet dropout is always on (rnn_decoder_mol.py:20), so inference is stochastic.
 ``dropout_masks=(keep1, keep2)`` injects the keep masks (bool / uint8, keep1 [steps, 256], keep2 [steps, 128], at least
 2 * (T // 4) steps) for reproducible comparisons; otherwise they are drawn on the device from ``seed``.
+``inference_batch(..., seeds=[s_i])`` gives every utterance its own dropout stream: utterance i is bitwise
+``inference(..., seed=s_i)`` whatever else is in the call (with ``seed=`` the draws of a row depend on its position).
 
 The reference's ``inference`` with B > 1 calls ``Decoder.inference_batched``, which concatenates every row's frames
 into one output and raises IndexError for a row whose stop token never fires, so no caller can depend on it; here B > 1
@@ -15,6 +17,7 @@ through ``inference`` is an error and ``inference_batch`` runs many utterances, 
 from __future__ import annotations
 
 import ctypes as C
+import numbers
 from pathlib import Path
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -100,8 +103,9 @@ class MelDecoderMOLv2:
 
     # -- inference -----------------------------------------------------------------------------------------------------
     def _run(self, ppg: torch.Tensor, lf0_uv: torch.Tensor, spk: torch.Tensor, lengths: List[int], masks=None,
-             seed: Optional[int] = None, return_stop: bool = False):
-        """one padded batch of <= MAX_ROWS rows -> per-row (mel, mel_postnet, alignments[, stop])"""
+             seed: Optional[int] = None, return_stop: bool = False, row_seeds: Optional[torch.Tensor] = None):
+        """one padded batch of <= MAX_ROWS rows -> per-row (mel, mel_postnet, alignments[, stop]); row_seeds (int64 [B]
+        on the device, the seeds' 64 bits) selects per-row dropout streams (mb_ppg2mel_inference_rows)"""
         dev = self._device
         L = _lib.lib()
         B, T, _ = ppg.shape
@@ -125,12 +129,16 @@ class MelDecoderMOLv2:
             lens = (C.c_int32 * B)(*lengths)
             steps = (C.c_int32 * B)()
             stream = torch.cuda.current_stream(dev).cuda_stream
-            _lib.check(L.mb_ppg2mel_inference(
-                self._handle, C.c_void_p(ppg.data_ptr()), C.c_void_p(lf0_uv.data_ptr()), C.c_void_p(spk.data_ptr()), lens,
-                B, T, C.c_void_p(m1.data_ptr()) if m1 is not None else None,
-                C.c_void_p(m2.data_ptr()) if m2 is not None else None, C.c_uint64(self.seed if seed is None else seed),
-                C.c_void_p(mel.data_ptr()), C.c_void_p(post.data_ptr()), C.c_void_p(align.data_ptr()),
-                C.c_void_p(stop.data_ptr()), steps, C.c_void_p(self._ws.data_ptr()), self._ws.numel(), C.c_void_p(stream)))
+            io = (C.c_void_p(ppg.data_ptr()), C.c_void_p(lf0_uv.data_ptr()), C.c_void_p(spk.data_ptr()), lens, B, T)
+            outs = (C.c_void_p(mel.data_ptr()), C.c_void_p(post.data_ptr()), C.c_void_p(align.data_ptr()),
+                    C.c_void_p(stop.data_ptr()), steps, C.c_void_p(self._ws.data_ptr()), self._ws.numel(), C.c_void_p(stream))
+            if row_seeds is not None:
+                _lib.check(L.mb_ppg2mel_inference_rows(self._handle, *io, C.c_void_p(row_seeds.data_ptr()), *outs))
+            else:
+                _lib.check(L.mb_ppg2mel_inference(
+                    self._handle, *io, C.c_void_p(m1.data_ptr()) if m1 is not None else None,
+                    C.c_void_p(m2.data_ptr()) if m2 is not None else None, C.c_uint64(self.seed if seed is None else seed),
+                    *outs))
         out = []
         for b in range(B):
             n, te = steps[b], lengths[b] // 4
@@ -181,14 +189,22 @@ class MelDecoderMOLv2:
         return self._run(*args, [T], masks, seed)[0]
 
     def inference_batch(self, utterances: Sequence[Tuple[torch.Tensor, torch.Tensor]], spembs: torch.Tensor,
-                        dropout_masks=None, seed: Optional[int] = None, return_stop: bool = False):
+                        dropout_masks=None, seed: Optional[int] = None, return_stop: bool = False,
+                        seeds: Optional[Sequence[int]] = None):
         """many utterances [(ppg [T_i, 144], lf0_uv [T_i, 2])] with spembs [N, 256] -> a list of per-utterance
         (mel, mel_postnet, alignments) as ``inference`` returns them.  Rows are length-sorted into padded batches of
         <= 128; each result equals the utterance's own B = 1 call with the same masks.
-        ``dropout_masks``: a list of per-utterance (keep1 [S_i, 256], keep2 [S_i, 128]) pairs."""
+        ``dropout_masks``: a list of per-utterance (keep1 [S_i, 256], keep2 [S_i, 128]) pairs.
+        ``seeds``: one dropout seed per utterance (integers in [0, 2**64)); utterance i is then bitwise
+        ``inference(..., seed=seeds[i])``, whatever the other utterances are.  Not combined with ``seed`` or ``dropout_masks``."""
         n = len(utterances)
         if spembs.dim() != 2 or spembs.shape[0] != n or spembs.shape[1] != self.spk_embed_dim:
             raise ValueError(f"spembs must be [{n}, {self.spk_embed_dim}]")
+        table = None
+        if seeds is not None:
+            if seed is not None or dropout_masks is not None:
+                raise ValueError("pass seeds alone: not together with seed or dropout_masks")
+            table = seed_table(seeds, n)
         for ppg, lf0 in utterances:
             self._check_inputs(ppg, lf0)
         self._prepare()
@@ -216,7 +232,10 @@ class MelDecoderMOLv2:
                     m1[:s_i, r] = torch.as_tensor(dropout_masks[i][0])[:s_i].to(torch.uint8)
                     m2[:s_i, r] = torch.as_tensor(dropout_masks[i][1])[:s_i].to(torch.uint8)
                 masks = (m1, m2)
-            for r, res in zip(idx, self._run(ppg, lf0, spk, lens, masks, seed, return_stop)):
+            rs = None
+            if table is not None:
+                rs = torch.tensor([table[i] for i in idx], dtype=torch.int64).to(dev)
+            for r, res in zip(idx, self._run(ppg, lf0, spk, lens, masks, seed, return_stop, rs)):
                 results[r] = res
         return results
 
@@ -227,6 +246,19 @@ class MelDecoderMOLv2:
                 self._handle = C.c_void_p()
         except Exception:
             pass
+
+
+def seed_table(seeds: Sequence[int], n: int) -> List[int]:
+    """per-utterance dropout seeds as the int64 values whose 64 bits are the seeds (the library reads them as uint64)"""
+    seeds = list(seeds)
+    if len(seeds) != n:
+        raise ValueError(f"{len(seeds)} seeds for {n} utterances")
+    out = []
+    for i, s in enumerate(seeds):
+        if isinstance(s, bool) or not isinstance(s, numbers.Integral) or not 0 <= int(s) < 1 << 64:
+            raise ValueError(f"seeds[{i}] = {s!r} is not an integer in [0, 2**64)")
+        out.append(int(s) - (1 << 64) if int(s) >= 1 << 63 else int(s))
+    return out
 
 
 def load_model(model_file, device=None):

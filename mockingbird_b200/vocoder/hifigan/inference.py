@@ -101,7 +101,8 @@ def infer_waveform(mel, progress_callback=None):
 
 def infer_waveforms(mels: Sequence[np.ndarray], batch_size: int = 32) -> List[np.ndarray]:
     """Vocode many utterances as length-sorted padded batches; each result equals the per-utterance
-    call (padding is masked at every layer on the device).  See ``_gan.infer_waveforms_batched``."""
+    call (padding is masked at every layer on the device).  Host mels give host waveforms; CUDA mels [80, T_i] give
+    CUDA waveforms without a host round trip.  See ``_gan.infer_waveforms_batched``."""
     if generator is None:
         raise Exception("Please load hifi-gan in memory before using it")
     return infer_waveforms_batched(generator, _device, mels, batch_size)
