@@ -984,6 +984,17 @@ int mb_resample_scale(const float* x, const int32_t* lengths_host, int32_t batch
 /* y = (x / max |x|) * peak per clip (two rounded fp32 operations); y may be x */
 int mb_resample_rescale(const float* x, const int32_t* lengths_host, int32_t batch, float peak, float* y, void* workspace,
                         size_t workspace_bytes, void* stream);
+/* The same three calls on float64 clips (the text-to-speech chain's levelling, gen_voice.py), same workspace:
+ *   sumsq_f64    the float64 sum of x * x in numpy's pairwise order, bitwise np.add.reduce(x ** 2) on float64
+ *   scale_f64    y = x * gains[b] (one rounded fp64 multiply; gains fp64 [batch], device); y may be x
+ *   rescale_f64  y = (x / max |x|) * peak (two rounded fp64 operations); a NaN sample makes max |x| NaN, as np.abs(x).max()
+ *                does, so the clip comes out all NaN; y may be x */
+int mb_resample_sumsq_f64(const double* x, const int32_t* lengths_host, int32_t batch, double* sumsq, void* workspace,
+                          size_t workspace_bytes, void* stream);
+int mb_resample_scale_f64(const double* x, const int32_t* lengths_host, int32_t batch, const double* gains, double* y,
+                          void* workspace, size_t workspace_bytes, void* stream);
+int mb_resample_rescale_f64(const double* x, const int32_t* lengths_host, int32_t batch, double peak, double* y,
+                            void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Voice-conversion mel decoder (ppg2mel)
@@ -1317,6 +1328,39 @@ typedef struct mb_emo_debug_spec {
 } mb_emo_debug_spec;
 size_t mb_emo_debug_workspace_bytes(const mb_emo_debug_spec* spec);
 int mb_emo_debug(const mb_emo_debug_spec* spec, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Text-to-speech chain (gen_voice.py): DESIGN.md section 4p
+ * ------------------------------------------------------------------------------------------- */
+/* device workspace of mb_tacotron_trim_frames (its row table); 0 when batch < 1 */
+size_t mb_tacotron_trim_workspace_bytes(int32_t batch);
+/* The trailing-silence trim of Tacotron rows (synthesizer/inference.py:135-138) in one launch:
+ *   linear fp32 [batch][n_mels][frames] (device): a ragged chunk's postnet output, row b valid for row_frames_host[b] frames
+ *   (host, 0 <= row_frames_host[b] <= frames)
+ *   trimmed int32 [batch] (device): the largest t <= row_frames_host[b] for which max_c linear[b][c][t - 1] < threshold is
+ *   false (0 when every frame is silent).  A frame holding a NaN is not silent.  Exact.
+ * MB_ERR_INVALID before anything is queued for a row length out of range. */
+int mb_tacotron_trim_frames(const float* linear, int32_t batch, int32_t n_mels, int32_t frames, const int32_t* row_frames_host,
+                            float threshold, int32_t* trimmed, void* workspace, size_t workspace_bytes, void* stream);
+
+/* One piece of a document: the slice src[start:end] of a vocoder row of src_len samples, with numpy's clamping
+ * (start and end are cut to src_len; 0 <= start <= end), followed by `zeros` zeros. */
+typedef struct mb_tts_piece {
+  const float* src; /* device: the row's first sample (may be NULL when src_len is 0) */
+  int64_t src_len;
+  int64_t start, end;
+  int32_t zeros;
+  int32_t pad;
+} mb_tts_piece;
+/* offsets_host int64 [n_pieces + 1] (host): the first output sample of every piece of mb_tts_join and the total.
+ * MB_ERR_INVALID for a malformed piece (the message names it). */
+int mb_tts_join_plan(const mb_tts_piece* pieces_host, int32_t n_pieces, int64_t* offsets_host);
+/* device workspace of mb_tts_join (its piece table); 0 when n_pieces < 1 */
+size_t mb_tts_join_workspace_bytes(int32_t n_pieces);
+/* gen_one_wav's break assembly (gen_voice.py:30-34) for every piece of pieces_host in one launch: out fp64 (device) receives
+ * the pieces back to back at mb_tts_join_plan's offsets, each one's float32 samples widened exactly, then its zeros. */
+int mb_tts_join(const mb_tts_piece* pieces_host, int32_t n_pieces, double* out, void* workspace, size_t workspace_bytes,
+                void* stream);
 
 #ifdef __cplusplus
 }

@@ -244,6 +244,11 @@ class VitsDebugSpec(C.Structure):
         (n, C.c_void_p) for n in ("lengths", "x", "x2", "x3", "y", "y2")]
 
 
+class TtsPiece(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("src_len", C.c_int64), ("start", C.c_int64), ("end", C.c_int64), ("zeros", C.c_int32),
+                ("pad", C.c_int32)]
+
+
 # name -> (restype, argtypes); every symbol include/mockingbird_b200.h declares
 SIGNATURES = {
     "mb_last_error": (C.c_char_p, []),
@@ -436,6 +441,12 @@ SIGNATURES = {
                                     C.c_size_t, C.c_void_p]),
     "mb_resample_rescale": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_float, C.c_void_p, C.c_void_p,
                                       C.c_size_t, C.c_void_p]),
+    "mb_resample_sumsq_f64": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p, C.c_size_t,
+                                        C.c_void_p]),
+    "mb_resample_scale_f64": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_size_t, C.c_void_p]),
+    "mb_resample_rescale_f64": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_double, C.c_void_p, C.c_void_p,
+                                          C.c_size_t, C.c_void_p]),
     "mb_ppg2mel_create": (C.c_int, [C.POINTER(Ppg2MelConfig), C.POINTER(C.c_void_p)]),
     "mb_ppg2mel_destroy": (None, [C.c_void_p]),
     "mb_ppg2mel_arena_bytes": (C.c_size_t, [C.c_void_p]),
@@ -491,6 +502,12 @@ SIGNATURES = {
                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mb_vits_debug_workspace_bytes": (C.c_size_t, [C.c_void_p, C.POINTER(VitsDebugSpec)]),
     "mb_vits_debug": (C.c_int, [C.c_void_p, C.POINTER(VitsDebugSpec), C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mb_tacotron_trim_workspace_bytes": (C.c_size_t, [C.c_int32]),
+    "mb_tacotron_trim_frames": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.c_float,
+                                          C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mb_tts_join_plan": (C.c_int, [C.POINTER(TtsPiece), C.c_int32, C.POINTER(C.c_int64)]),
+    "mb_tts_join_workspace_bytes": (C.c_size_t, [C.c_int32]),
+    "mb_tts_join": (C.c_int, [C.POINTER(TtsPiece), C.c_int32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 _lib: Optional[C.CDLL] = None

@@ -1,6 +1,7 @@
-// numpy's float32 pairwise summation (numpy/_core/src/umath/loops_utils.h.src, the order np.add.reduce takes over a contiguous
-// float32 array) of an element function f(i), i in [0, n).  Shared by the resampler's levelling (f = x * x) and the wav2vec2
-// feature extractor's normalisation (f = x, then f = (x - mean)^2).
+// numpy's pairwise summation (numpy/_core/src/umath/loops_utils.h.src, the order np.add.reduce takes over a contiguous
+// float32 or float64 array: the same 8-accumulator, 128-element blocks for both) of an element function f(i), i in [0, n),
+// in the element type T (float or double), every addition rounded once.  Shared by the resampler's levelling (f = x * x,
+// float32 and float64) and the wav2vec2 feature extractor's normalisation (f = x, then f = (x - mean)^2).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -10,35 +11,42 @@
 
 namespace mb {
 
-template <class F>
-__device__ float pairwise_sum(const F& f, int64_t i0, int64_t n) {
+// rounded arithmetic by element type: never contracted into an FMA
+__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
+__device__ __forceinline__ double div_rn(double a, double b) { return __ddiv_rn(a, b); }
+
+template <class T, class F>
+__device__ T pairwise_sum(const F& f, int64_t i0, int64_t n) {
   if (n < 8) {
-    float r = -0.0f;
-    for (int64_t i = 0; i < n; ++i) r = __fadd_rn(r, f(i0 + i));
+    T r = (T)-0.0;
+    for (int64_t i = 0; i < n; ++i) r = add_rn(r, (T)f(i0 + i));
     return r;
   }
   if (n <= 128) {
-    float r[8];
+    T r[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) r[k] = f(i0 + k);
     int64_t i = 8;
     for (; i < n - (n % 8); i += 8)
 #pragma unroll
-      for (int k = 0; k < 8; ++k) r[k] = __fadd_rn(r[k], f(i0 + i + k));
-    float res = __fadd_rn(__fadd_rn(__fadd_rn(r[0], r[1]), __fadd_rn(r[2], r[3])),
-                          __fadd_rn(__fadd_rn(r[4], r[5]), __fadd_rn(r[6], r[7])));
-    for (; i < n; ++i) res = __fadd_rn(res, f(i0 + i));
+      for (int k = 0; k < 8; ++k) r[k] = add_rn(r[k], (T)f(i0 + i + k));
+    T res = add_rn(add_rn(add_rn(r[0], r[1]), add_rn(r[2], r[3])), add_rn(add_rn(r[4], r[5]), add_rn(r[6], r[7])));
+    for (; i < n; ++i) res = add_rn(res, (T)f(i0 + i));
     return res;
   }
   int64_t n2 = n / 2;
   n2 -= n2 % 8;
-  return __fadd_rn(pairwise_sum(f, i0, n2), pairwise_sum(f, i0 + n2, n - n2));
+  return add_rn(pairwise_sum<T>(f, i0, n2), pairwise_sum<T>(f, i0 + n2, n - n2));
 }
 
 // The same sum by one CTA: the tree is split into 2^depth subtrees (depth from pairwise_depth), one per thread, and the levels
-// above them are added bottom up in shared memory `part` (at least 2^depth floats).  Every thread returns the sum.
-template <class F>
-__device__ float pairwise_sum_block(const F& f, int64_t n, int depth, float* part) {
+// above them are added bottom up in shared memory `part` (at least 2^depth elements of T).  Every thread returns the sum.
+template <class F, class T>
+__device__ T pairwise_sum_block(const F& f, int64_t n, int depth, T* part) {
   const int nsub = 1 << depth;
   if ((int)threadIdx.x < nsub) {
     int64_t off = 0, m = n;
@@ -48,17 +56,17 @@ __device__ float pairwise_sum_block(const F& f, int64_t n, int depth, float* par
       if ((threadIdx.x >> d) & 1) off += n2, m -= n2;
       else m = n2;
     }
-    part[threadIdx.x] = pairwise_sum(f, off, m);
+    part[threadIdx.x] = pairwise_sum<T>(f, off, m);
   }
   __syncthreads();
   for (int w = nsub >> 1; w >= 1; w >>= 1) {
-    float v = 0.0f;
-    if ((int)threadIdx.x < w) v = __fadd_rn(part[2 * threadIdx.x], part[2 * threadIdx.x + 1]);
+    T v = 0;
+    if ((int)threadIdx.x < w) v = add_rn(part[2 * threadIdx.x], part[2 * threadIdx.x + 1]);
     __syncthreads();
     if ((int)threadIdx.x < w) part[threadIdx.x] = v;
     __syncthreads();
   }
-  const float s = part[0];
+  const T s = part[0];
   __syncthreads();  // part may be reused by the caller's next sum
   return s;
 }

@@ -15,9 +15,11 @@
 //                      of the tile plus the filter halo is staged in shared memory by a bulk copy (the 16-byte aligned
 //                      interior) and plain loads (the unaligned ends); the polyphase table [up][taps] is staged the same way
 //                      when it fits under the handle's limit, else read through L2
-// rs_sumsq_kernel      one CTA per clip: the float32 sum of x * x in numpy's pairwise order (np.add.reduce on float32)
+// rs_sumsq_kernel      one CTA per clip: the sum of x * x in numpy's pairwise order (np.add.reduce on float32 or float64)
 // rs_scale_kernel      y = x * gain[b] (one rounded multiply)
 // rs_rescale_kernel    one CTA per clip: m = max |x| (exact), y = (x / m) * peak (two rounded operations)
+// The three levelling kernels are instantiated for float (mb_resample_sumsq / _scale / _rescale) and for double (the _f64
+// entries, the text-to-speech chain's float64 post-processing, gen_voice.py).
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -139,36 +141,47 @@ struct LvClip {
   int32_t depth;  // the pairwise tree is split into 2^depth subtrees, one per thread; every node above them is internal
 };
 
-__global__ void __launch_bounds__(kLevelThreads) rs_sumsq_kernel(const float* __restrict__ x, const LvClip* clips,
-                                                                 float* __restrict__ sumsq) {
-  __shared__ float part[kLevelThreads];
+// numpy's max of |x| as the levelling reads it: the float32 kernels keep fmaxf (a NaN sample is skipped); the float64 kernel
+// propagates NaN as np.abs(x).max() does, so a NaN anywhere makes the clip all NaN
+__device__ __forceinline__ float max_abs(float m, float v) { return fmaxf(m, fabsf(v)); }
+__device__ __forceinline__ double max_abs(double m, double v) {
+  const double a = fabs(v);
+  return (a > m || a != a) ? a : m;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kLevelThreads) rs_sumsq_kernel(const T* __restrict__ x, const LvClip* clips,
+                                                                 T* __restrict__ sumsq) {
+  __shared__ T part[kLevelThreads];
   const LvClip c = clips[blockIdx.x];
-  const float* a = x + c.off;
-  const float s = pairwise_sum_block([a](int64_t i) { return __fmul_rn(a[i], a[i]); }, c.n, c.depth, part);
+  const T* a = x + c.off;
+  const T s = pairwise_sum_block([a](int64_t i) { return mul_rn(a[i], a[i]); }, c.n, c.depth, part);
   if (threadIdx.x == 0) sumsq[blockIdx.x] = s;
 }
 
-__global__ void __launch_bounds__(kLevelThreads) rs_scale_kernel(const float* __restrict__ x, const LvClip* clips,
-                                                                 const float* __restrict__ gains, float* __restrict__ y) {
+template <typename T>
+__global__ void __launch_bounds__(kLevelThreads) rs_scale_kernel(const T* __restrict__ x, const LvClip* clips,
+                                                                 const T* __restrict__ gains, T* __restrict__ y) {
   const LvClip c = clips[blockIdx.y];
-  const float g = gains[blockIdx.y];
+  const T g = gains[blockIdx.y];
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < c.n; i += (int64_t)gridDim.x * blockDim.x)
-    y[c.off + i] = __fmul_rn(x[c.off + i], g);
+    y[c.off + i] = mul_rn(x[c.off + i], g);
 }
 
-__global__ void __launch_bounds__(kLevelThreads) rs_rescale_kernel(const float* __restrict__ x, const LvClip* clips, float peak,
-                                                                   float* __restrict__ y) {
-  __shared__ float red[kLevelThreads / 32];
+template <typename T>
+__global__ void __launch_bounds__(kLevelThreads) rs_rescale_kernel(const T* __restrict__ x, const LvClip* clips, T peak,
+                                                                   T* __restrict__ y) {
+  __shared__ T red[kLevelThreads / 32];
   const LvClip c = clips[blockIdx.x];
-  const float* xc = x + c.off;
-  float m = 0.0f;
-  for (int64_t i = threadIdx.x; i < c.n; i += blockDim.x) m = fmaxf(m, fabsf(xc[i]));
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  const T* xc = x + c.off;
+  T m = 0;
+  for (int64_t i = threadIdx.x; i < c.n; i += blockDim.x) m = max_abs(m, xc[i]);
+  for (int o = 16; o > 0; o >>= 1) m = max_abs(m, __shfl_xor_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
   __syncthreads();
   m = red[0];
-  for (int w = 1; w < kLevelThreads / 32; ++w) m = fmaxf(m, red[w]);
-  for (int64_t i = threadIdx.x; i < c.n; i += blockDim.x) y[c.off + i] = __fmul_rn(__fdiv_rn(xc[i], m), peak);
+  for (int w = 1; w < kLevelThreads / 32; ++w) m = max_abs(m, red[w]);
+  for (int64_t i = threadIdx.x; i < c.n; i += blockDim.x) y[c.off + i] = mul_rn(div_rn(xc[i], m), peak);
 }
 
 
@@ -382,41 +395,78 @@ static int level_table(const char* fn, const int32_t* lengths_host, int32_t batc
   return MB_OK;
 }
 
-int mb_resample_sumsq(const float* x, const int32_t* lengths_host, int32_t batch, float* sumsq, void* workspace,
-                      size_t workspace_bytes, void* stream) {
-  if (!x || !lengths_host || !sumsq) return fail(MB_ERR_INVALID, "mb_resample_sumsq: null argument");
+}  // extern "C"
+
+template <typename T>
+static int level_sumsq(const char* fn, const T* x, const int32_t* lengths_host, int32_t batch, T* sumsq, void* workspace,
+                       size_t workspace_bytes, void* stream) {
+  if (!x || !lengths_host || !sumsq) return fail(MB_ERR_INVALID, "%s: null argument", fn);
   cudaStream_t st = (cudaStream_t)stream;
   const LvClip* t;
   int32_t n_max;
-  if (int rc = level_table("mb_resample_sumsq", lengths_host, batch, workspace, workspace_bytes, st, &t, &n_max)) return rc;
-  rs_sumsq_kernel<<<batch, kLevelThreads, 0, st>>>(x, t, sumsq);
+  if (int rc = level_table(fn, lengths_host, batch, workspace, workspace_bytes, st, &t, &n_max)) return rc;
+  rs_sumsq_kernel<T><<<batch, kLevelThreads, 0, st>>>(x, t, sumsq);
   MB_LAUNCH_CHECK("rs_sumsq_kernel");
   return MB_OK;
 }
 
-int mb_resample_scale(const float* x, const int32_t* lengths_host, int32_t batch, const float* gains, float* y, void* workspace,
-                      size_t workspace_bytes, void* stream) {
-  if (!x || !lengths_host || !gains || !y) return fail(MB_ERR_INVALID, "mb_resample_scale: null argument");
+template <typename T>
+static int level_scale(const char* fn, const T* x, const int32_t* lengths_host, int32_t batch, const T* gains, T* y,
+                       void* workspace, size_t workspace_bytes, void* stream) {
+  if (!x || !lengths_host || !gains || !y) return fail(MB_ERR_INVALID, "%s: null argument", fn);
   cudaStream_t st = (cudaStream_t)stream;
   const LvClip* t;
   int32_t n_max;
-  if (int rc = level_table("mb_resample_scale", lengths_host, batch, workspace, workspace_bytes, st, &t, &n_max)) return rc;
+  if (int rc = level_table(fn, lengths_host, batch, workspace, workspace_bytes, st, &t, &n_max)) return rc;
   const dim3 grid((unsigned)std::min<int64_t>(64, ((int64_t)n_max + kLevelThreads - 1) / kLevelThreads), (unsigned)batch);
-  rs_scale_kernel<<<grid, kLevelThreads, 0, st>>>(x, t, gains, y);
+  rs_scale_kernel<T><<<grid, kLevelThreads, 0, st>>>(x, t, gains, y);
   MB_LAUNCH_CHECK("rs_scale_kernel");
   return MB_OK;
 }
 
-int mb_resample_rescale(const float* x, const int32_t* lengths_host, int32_t batch, float peak, float* y, void* workspace,
-                        size_t workspace_bytes, void* stream) {
-  if (!x || !lengths_host || !y) return fail(MB_ERR_INVALID, "mb_resample_rescale: null argument");
+template <typename T>
+static int level_rescale(const char* fn, const T* x, const int32_t* lengths_host, int32_t batch, T peak, T* y, void* workspace,
+                         size_t workspace_bytes, void* stream) {
+  if (!x || !lengths_host || !y) return fail(MB_ERR_INVALID, "%s: null argument", fn);
   cudaStream_t st = (cudaStream_t)stream;
   const LvClip* t;
   int32_t n_max;
-  if (int rc = level_table("mb_resample_rescale", lengths_host, batch, workspace, workspace_bytes, st, &t, &n_max)) return rc;
-  rs_rescale_kernel<<<batch, kLevelThreads, 0, st>>>(x, t, peak, y);
+  if (int rc = level_table(fn, lengths_host, batch, workspace, workspace_bytes, st, &t, &n_max)) return rc;
+  rs_rescale_kernel<T><<<batch, kLevelThreads, 0, st>>>(x, t, peak, y);
   MB_LAUNCH_CHECK("rs_rescale_kernel");
   return MB_OK;
+}
+
+extern "C" {
+
+int mb_resample_sumsq(const float* x, const int32_t* lengths_host, int32_t batch, float* sumsq, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+  return level_sumsq("mb_resample_sumsq", x, lengths_host, batch, sumsq, workspace, workspace_bytes, stream);
+}
+
+int mb_resample_scale(const float* x, const int32_t* lengths_host, int32_t batch, const float* gains, float* y, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+  return level_scale("mb_resample_scale", x, lengths_host, batch, gains, y, workspace, workspace_bytes, stream);
+}
+
+int mb_resample_rescale(const float* x, const int32_t* lengths_host, int32_t batch, float peak, float* y, void* workspace,
+                        size_t workspace_bytes, void* stream) {
+  return level_rescale("mb_resample_rescale", x, lengths_host, batch, peak, y, workspace, workspace_bytes, stream);
+}
+
+int mb_resample_sumsq_f64(const double* x, const int32_t* lengths_host, int32_t batch, double* sumsq, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+  return level_sumsq("mb_resample_sumsq_f64", x, lengths_host, batch, sumsq, workspace, workspace_bytes, stream);
+}
+
+int mb_resample_scale_f64(const double* x, const int32_t* lengths_host, int32_t batch, const double* gains, double* y,
+                          void* workspace, size_t workspace_bytes, void* stream) {
+  return level_scale("mb_resample_scale_f64", x, lengths_host, batch, gains, y, workspace, workspace_bytes, stream);
+}
+
+int mb_resample_rescale_f64(const double* x, const int32_t* lengths_host, int32_t batch, double peak, double* y,
+                            void* workspace, size_t workspace_bytes, void* stream) {
+  return level_rescale("mb_resample_rescale_f64", x, lengths_host, batch, peak, y, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -11,9 +11,10 @@ ValueError naming the clip, before anything is queued: an empty or non-1-D clip,
 float64 samples (the host computes those in float64; this path is float32 only) or any other dtype.
 
 ``normalize_volume_device`` is ``normalize_volume(wav, target_dBFS, increase_only=True)``: the mean square is summed on
-the device in numpy's pairwise order, the gain is computed on the host with numpy's own float32 scalar functions from the
-B mean squares (one copy of B floats), and the clips are scaled on the device.  ``rescale_device`` is
-``wav / np.abs(wav).max() * peak``."""
+the device in numpy's pairwise order, the gain is computed on the host with numpy's own scalar functions from the B mean
+squares (one copy of B values), and the clips are scaled on the device.  ``rescale_device`` is
+``wav / np.abs(wav).max() * peak``.  Both level float32 clips in float32 and float64 clips (the text-to-speech chain's
+documents, gen_voice.py) in float64, each as numpy does for that dtype; resampling itself takes float32 only."""
 from __future__ import annotations
 
 import ctypes as C
@@ -28,16 +29,17 @@ from . import _lib
 
 
 class DeviceClips:
-    """Clips on the device: ``data`` holds clip i's ``lengths[i]`` float32 samples after those of clips 0 .. i-1.  Indexing
-    and iteration give 1-D views of ``data``; ``numpy()`` copies every clip to the host in one transfer."""
+    """Clips on the device: ``data`` holds clip i's ``lengths[i]`` samples (float32, or float64 for levelling only) after
+    those of clips 0 .. i-1.  Indexing and iteration give 1-D views of ``data``; ``numpy()`` copies every clip to the host
+    in one transfer."""
 
     def __init__(self, data: torch.Tensor, lengths, sample_rate: int):
         self.data = data
         self.lengths = [int(n) for n in lengths]
         self.sample_rate = int(sample_rate)
         self.offsets = np.concatenate([[0], np.cumsum(self.lengths, dtype=np.int64)]).tolist()
-        if data.dim() != 1 or data.numel() != self.offsets[-1] or data.dtype != torch.float32:
-            raise ValueError(f"DeviceClips: data must be 1-D float32 of {self.offsets[-1]} samples")
+        if data.dim() != 1 or data.numel() != self.offsets[-1] or data.dtype not in (torch.float32, torch.float64):
+            raise ValueError(f"DeviceClips: data must be 1-D float32 or float64 of {self.offsets[-1]} samples")
 
     def __len__(self):
         return len(self.lengths)
@@ -224,51 +226,64 @@ def _level_ws(clips: DeviceClips):
     return (C.c_int32 * B)(*clips.lengths), _lib.workspace(need, clips.device)
 
 
+def _f64(clips: DeviceClips) -> bool:
+    return clips.data.dtype == torch.float64
+
+
 def mean_squares(clips: DeviceClips) -> np.ndarray:
-    """np.mean(wav ** 2) of every clip, bitwise: float32 sums of squares in numpy's pairwise order on the device, each
-    divided by the length as np.mean does (in float64, rounded once to float32)"""
+    """np.mean(wav ** 2) of every clip, bitwise: sums of squares in numpy's pairwise order on the device, each divided by
+    the length as np.mean does (float32 clips: in float64, rounded once to float32; float64 clips: in float64)"""
+    f64 = _f64(clips)
     if len(clips) == 0:
-        return np.zeros(0, np.float32)
+        return np.zeros(0, np.float64 if f64 else np.float32)
     B = len(clips)
     T, ws = _level_ws(clips)
     with torch.cuda.device(clips.device):
-        s = torch.empty(B, dtype=torch.float32, device=clips.device)
+        s = torch.empty(B, dtype=clips.data.dtype, device=clips.device)
         stream = torch.cuda.current_stream(clips.device).cuda_stream
-        _lib.check(_lib.lib().mb_resample_sumsq(C.c_void_p(clips.data.data_ptr()), T, B, C.c_void_p(s.data_ptr()),
-                                                C.c_void_p(ws.data_ptr()), ws.numel(), C.c_void_p(stream)))
+        fn = _lib.lib().mb_resample_sumsq_f64 if f64 else _lib.lib().mb_resample_sumsq
+        _lib.check(fn(C.c_void_p(clips.data.data_ptr()), T, B, C.c_void_p(s.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(),
+                      C.c_void_p(stream)))
         s = s.cpu().numpy()
+    if f64:
+        return np.array([np.float64(v) / n for v, n in zip(s, clips.lengths)], dtype=np.float64)
     return np.array([np.float32(np.float64(v) / n) for v, n in zip(s, clips.lengths)], dtype=np.float32)
 
 
 def normalize_volume_device(clips: DeviceClips, target_dBFS, increase_only=False, decrease_only=False) -> DeviceClips:
-    """normalize_volume (models/encoder/audio.py:108-117) of every float32 clip -> a new DeviceClips, each clip bitwise the
-    host call: the gain is numpy's float32 scalar arithmetic on the mean square, the scaling one float32 multiply"""
+    """normalize_volume (models/encoder/audio.py:108-117) of every clip -> a new DeviceClips, each clip bitwise the host call
+    on an array of its dtype: the gain is numpy's scalar arithmetic on the mean square (float32 clips: in float32; float64
+    clips: in float64), the scaling one rounded multiply of that dtype"""
     if increase_only and decrease_only:
         raise ValueError("Both increase only and decrease only are set")
     if len(clips) == 0:
         return clips
+    f64 = _f64(clips)
+    dt = np.float64 if f64 else np.float32
     gains = []
-    with np.errstate(divide="ignore", over="ignore"):  # a silent clip: -inf dB, as on the host (which warns)
+    # a silent clip: -inf dB, as on the host (which warns); float64 zeros then scale by inf, which gives NaN as numpy does
+    with np.errstate(divide="ignore", over="ignore", invalid="ignore"):
         for m in mean_squares(clips):
             dBFS_change = target_dBFS - 10 * np.log10(m)
             if (dBFS_change < 0 and increase_only) or (dBFS_change > 0 and decrease_only):
-                gains.append(np.float32(1.0))  # x * 1 is x
+                gains.append(dt(1.0))  # x * 1 is x
             else:
-                gains.append(np.float32(10 ** (dBFS_change / 20)))
+                gains.append(dt(10 ** (dBFS_change / 20)))
     B = len(clips)
     T, ws = _level_ws(clips)
     with torch.cuda.device(clips.device):
-        g = torch.from_numpy(np.array(gains, dtype=np.float32)).to(clips.device)
+        g = torch.from_numpy(np.array(gains, dtype=dt)).to(clips.device)
         y = torch.empty_like(clips.data)
         stream = torch.cuda.current_stream(clips.device).cuda_stream
-        _lib.check(_lib.lib().mb_resample_scale(C.c_void_p(clips.data.data_ptr()), T, B, C.c_void_p(g.data_ptr()),
-                                                C.c_void_p(y.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(),
-                                                C.c_void_p(stream)))
+        fn = _lib.lib().mb_resample_scale_f64 if f64 else _lib.lib().mb_resample_scale
+        _lib.check(fn(C.c_void_p(clips.data.data_ptr()), T, B, C.c_void_p(g.data_ptr()), C.c_void_p(y.data_ptr()),
+                      C.c_void_p(ws.data_ptr()), ws.numel(), C.c_void_p(stream)))
     return DeviceClips(y, clips.lengths, clips.sample_rate)
 
 
 def rescale_device(clips: DeviceClips, peak) -> DeviceClips:
-    """wav / np.abs(wav).max() * peak of every clip (float32; peak rounded to float32 as numpy does) -> a new DeviceClips"""
+    """wav / np.abs(wav).max() * peak of every clip -> a new DeviceClips.  float32 clips: peak rounded to float32 as numpy
+    does; float64 clips: in float64, where a NaN sample makes the clip all NaN (np.max propagates it)"""
     if len(clips) == 0:
         return clips
     B = len(clips)
@@ -276,9 +291,12 @@ def rescale_device(clips: DeviceClips, peak) -> DeviceClips:
     with torch.cuda.device(clips.device):
         y = torch.empty_like(clips.data)
         stream = torch.cuda.current_stream(clips.device).cuda_stream
-        _lib.check(_lib.lib().mb_resample_rescale(C.c_void_p(clips.data.data_ptr()), T, B, float(np.float32(peak)),
-                                                  C.c_void_p(y.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(),
-                                                  C.c_void_p(stream)))
+        if _f64(clips):
+            fn, p = _lib.lib().mb_resample_rescale_f64, float(peak)
+        else:
+            fn, p = _lib.lib().mb_resample_rescale, float(np.float32(peak))
+        _lib.check(fn(C.c_void_p(clips.data.data_ptr()), T, B, p, C.c_void_p(y.data_ptr()), C.c_void_p(ws.data_ptr()),
+                      ws.numel(), C.c_void_p(stream)))
     return DeviceClips(y, clips.lengths, clips.sample_rate)
 
 

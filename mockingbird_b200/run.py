@@ -135,12 +135,17 @@ def checkpoint_step(ppg2mel_model_file) -> str:
 
 
 def write_pcm16(path, wav: np.ndarray, sample_rate: int) -> None:
-    """a float waveform as a 16-bit PCM WAV: samples clipped to [-1, 1], scaled by 32767 in float32 and rounded to the
-    nearest integer (ties to even), as libsndfile writes float data as PCM_16"""
+    """a float waveform as a 16-bit PCM WAV, as libsndfile writes float data as PCM_16: float32 (and any other non-float64
+    input) is clipped to [-1, 1], scaled by 32767 in float32 and rounded to the nearest integer (ties to even); float64 is
+    scaled by 32767 in float64, rounded the same way and clipped to [-32767, 32767]"""
     from scipy.io import wavfile
 
-    x = np.clip(np.asarray(wav, dtype=np.float32), -1.0, 1.0) * np.float32(32767.0)
-    wavfile.write(str(path), int(sample_rate), np.rint(x).astype(np.int16))
+    wav = np.asarray(wav)
+    if wav.dtype == np.float64:
+        pcm = np.clip(np.rint(wav * 32767.0), -32767.0, 32767.0)
+    else:
+        pcm = np.rint(np.clip(np.asarray(wav, dtype=np.float32), -1.0, 1.0) * np.float32(32767.0))
+    wavfile.write(str(path), int(sample_rate), pcm.astype(np.int16))
 
 
 def _load_yaml(path):

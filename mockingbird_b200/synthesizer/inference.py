@@ -71,13 +71,25 @@ class Synthesizer:
         self._model.eval()
         return self._model
 
-    def synthesize_spectrograms(self, texts: List[str], embeddings: Union[np.ndarray, List[np.ndarray]],
-                                return_alignments=False, style_idx=0, min_stop_token=5, steps=2000):
+    def _sequences(self, texts: List[str]):
+        """the text front-end of every synthesize_* method (inference.py:97-103): the model is loaded on first use, the
+        texts are romanised with pypinyin where it is installed, then turned into symbol ids"""
         if not self.is_loaded():
             self.load()
         if lazy_pinyin is not None:
             texts = [" ".join(lazy_pinyin(v, style=Style.TONE3, neutral_tone_with_five=True)) for v in texts]
-        inputs = [text_to_sequence(text, hparams.tts_cleaner_names) for text in texts]
+        return [text_to_sequence(text, hparams.tts_cleaner_names) for text in texts]
+
+    @staticmethod
+    def _embedding_rows(embeddings, n) -> torch.Tensor:
+        emb = np.stack([np.asarray(e, dtype=np.float32) for e in embeddings]) if len(embeddings) else np.zeros((0, 256), np.float32)
+        if emb.shape[0] != n:
+            raise ValueError(f"{emb.shape[0]} speaker embeddings for {n} texts")
+        return torch.from_numpy(emb)
+
+    def synthesize_spectrograms(self, texts: List[str], embeddings: Union[np.ndarray, List[np.ndarray]],
+                                return_alignments=False, style_idx=0, min_stop_token=5, steps=2000):
+        inputs = self._sequences(texts)
         return self.synthesize_from_sequences(inputs, embeddings, return_alignments, style_idx, min_stop_token, steps)
 
     def synthesize_spectrograms_many(self, texts: List[str], embeddings: Union[np.ndarray, List[np.ndarray]],
@@ -85,16 +97,10 @@ class Synthesizer:
         """synthesize_spectrograms with every text computed as its own batch of one (Tacotron.generate_many): a text's
         spectrogram does not depend on the texts around it.  Same text front-end, postnet output and trailing trim;
         -> list of [80, f_i] host arrays in input order (plus a list of per-text alignments when return_alignments)"""
-        if not self.is_loaded():
-            self.load()
-        if lazy_pinyin is not None:
-            texts = [" ".join(lazy_pinyin(v, style=Style.TONE3, neutral_tone_with_five=True)) for v in texts]
-        inputs = [text_to_sequence(text, hparams.tts_cleaner_names) for text in texts]
-        emb = np.stack([np.asarray(e, dtype=np.float32) for e in embeddings]) if len(embeddings) else np.zeros((0, 256), np.float32)
-        if emb.shape[0] != len(inputs):
-            raise ValueError(f"{emb.shape[0]} speaker embeddings for {len(inputs)} texts")
-        outs = self._model.generate_many(inputs, torch.from_numpy(emb), steps=steps, style_idx=style_idx,
-                                         min_stop_token=min_stop_token, seeds=seeds)
+        inputs = self._sequences(texts)
+        emb = self._embedding_rows(embeddings, len(inputs))
+        outs = self._model.generate_many(inputs, emb, steps=steps, style_idx=style_idx, min_stop_token=min_stop_token,
+                                         seeds=seeds)
         specs, alignments = [], []
         for _, lin, attn in outs:
             m = lin.cpu().numpy()
@@ -105,21 +111,26 @@ class Synthesizer:
             alignments.append(attn.cpu().numpy())
         return (specs, alignments) if return_alignments else specs
 
+    def synthesize_spectrograms_device(self, texts: List[str], embeddings: Union[np.ndarray, List[np.ndarray]], style_idx=0,
+                                       min_stop_token=5, steps=2000, seeds=None) -> List[torch.Tensor]:
+        """synthesize_spectrograms_many left on the device: -> list of [80, f_i] CUDA tensors in input order, each equal to
+        synthesize_spectrograms_many's i-th.  The trailing silence is trimmed on the device (mb_tacotron_trim_frames), so
+        only the trimmed lengths reach the host."""
+        inputs = self._sequences(texts)
+        emb = self._embedding_rows(embeddings, len(inputs))
+        outs = self._model.generate_many(inputs, emb, steps=steps, style_idx=style_idx, min_stop_token=min_stop_token,
+                                         seeds=seeds, trim_threshold=hparams.tts_stop_threshold)
+        return [lin for _, lin, _ in outs]
+
     def synthesize_spectrograms_stream(self, texts: List[str], embeddings: Union[np.ndarray, List[np.ndarray]], style_idx=0,
                                        min_stop_token=5, steps=2000, seeds=None, slots=128):
         """synthesize_spectrograms_many as an iterator that yields each text's spectrogram as soon as it is done
         (Tacotron.generate_stream): ``(i, [80, f_i] host array)`` in the order the texts finish, each equal to
         synthesize_spectrograms_many's i-th.  Same text front-end, postnet output and trailing trim."""
-        if not self.is_loaded():
-            self.load()
-        if lazy_pinyin is not None:
-            texts = [" ".join(lazy_pinyin(v, style=Style.TONE3, neutral_tone_with_five=True)) for v in texts]
-        inputs = [text_to_sequence(text, hparams.tts_cleaner_names) for text in texts]
-        emb = np.stack([np.asarray(e, dtype=np.float32) for e in embeddings]) if len(embeddings) else np.zeros((0, 256), np.float32)
-        if emb.shape[0] != len(inputs):
-            raise ValueError(f"{emb.shape[0]} speaker embeddings for {len(inputs)} texts")
-        outs = self._model.generate_stream(inputs, torch.from_numpy(emb), steps=steps, style_idx=style_idx,
-                                           min_stop_token=min_stop_token, seeds=seeds, slots=slots)
+        inputs = self._sequences(texts)
+        emb = self._embedding_rows(embeddings, len(inputs))
+        outs = self._model.generate_stream(inputs, emb, steps=steps, style_idx=style_idx, min_stop_token=min_stop_token,
+                                           seeds=seeds, slots=slots)
         return self._trimmed(outs)
 
     @staticmethod

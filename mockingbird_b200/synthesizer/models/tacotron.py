@@ -102,6 +102,7 @@ class Tacotron:
         self._state: Optional[Dict[str, torch.Tensor]] = None
         self._arena = None
         self._ws = None
+        self._trim_ws = None
         self._device = None
         self._ready = False
         self._r = 1
@@ -283,7 +284,7 @@ class Tacotron:
         return rows, spk_all, caps, seeds
 
     def generate_many(self, seqs, speaker_embeddings, steps=2000, style_idx=0, min_stop_token=5, seeds=None,
-                      dropout_masks=None, chunk_rows=None):
+                      dropout_masks=None, chunk_rows=None, trim_threshold=None):
         """Many texts, each computed as its own B = 1 ``generate`` -> list of N ``(mel [80, f_i], linear [80, f_i],
         attn [f_i / r, Tc_i])`` device tensors in input order.
 
@@ -291,7 +292,10 @@ class Tacotron:
         utterance stops at its own stop rule or cap.  Utterances are sorted longest first and run in ragged batches of at
         most ``chunk_rows`` (default ``MANY_CHUNK_ROWS``) rows; a result is bitwise the same whatever the list around it.
         Dropout is drawn from ``seeds[i]`` (default ``self.seed + i``) or injected per utterance as
-        ``dropout_masks = (enc, dec)`` with enc[i] [2, Tc_i, 256] and dec[i] [>= ceil(steps_i / r), 2, 256]."""
+        ``dropout_masks = (enc, dec)`` with enc[i] [2, Tc_i, 256] and dec[i] [>= ceil(steps_i / r), 2, 256].
+        ``trim_threshold`` (a float): each linear output is cut to its trailing-silence trim, the frames up to the last one
+        whose largest channel is not below the threshold (synthesizer/inference.py:135-138), found on the device by one
+        mb_tacotron_trim_frames launch per chunk; only the trimmed lengths come back to the host."""
         self.eval()
         N = len(seqs)
         if N == 0:
@@ -346,13 +350,29 @@ class Tacotron:
                     C.c_void_p(lin.data_ptr()), C.c_void_p(attn.data_ptr()), C.byref(frames), row_frames,
                     C.c_void_p(self._ws.data_ptr()), self._ws.numel(), C.c_void_p(stream)))
             F_ = frames.value
+            keep = list(row_frames)
+            if trim_threshold is not None:
+                keep = self._trim_frames(lin, B, F_, row_frames, float(trim_threshold))
             mel = mel[: B * self.n_mels * F_].view(B, self.n_mels, F_)
             lin = lin[: B * self.n_mels * F_].view(B, self.n_mels, F_)
             attn = attn[: B * (F_ // r) * Tc].view(B, F_ // r, Tc)
             for b, i in enumerate(chunk):
                 f = row_frames[b]
-                out[i] = (mel[b, :, :f].clone(), lin[b, :, :f].clone(), attn[b, : f // r, : lens[b]].clone())
+                out[i] = (mel[b, :, :f].clone(), lin[b, :, :keep[b]].clone(), attn[b, : f // r, : lens[b]].clone())
         return out
+
+    def _trim_frames(self, lin, B, F_, row_frames, threshold):
+        """mb_tacotron_trim_frames over a chunk's postnet output [B, 80, F_] -> the B trimmed frame counts (host ints)"""
+        L = _lib.lib()
+        dev = self._device
+        with torch.cuda.device(dev):
+            kept = torch.empty(B, dtype=torch.int32, device=dev)
+            ws = _lib.workspace(int(L.mb_tacotron_trim_workspace_bytes(B)), dev, self, "_trim_ws")
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            _lib.check(L.mb_tacotron_trim_frames(C.c_void_p(lin.data_ptr()), B, self.n_mels, F_, row_frames,
+                                                 C.c_float(threshold), C.c_void_p(kept.data_ptr()), C.c_void_p(ws.data_ptr()),
+                                                 ws.numel(), C.c_void_p(stream)))
+            return kept.cpu().tolist()
 
     def generate_stream(self, seqs, speaker_embeddings, steps=2000, style_idx=0, min_stop_token=5, seeds=None,
                         dropout_masks=None, slots=MANY_CHUNK_ROWS):

@@ -192,6 +192,23 @@ class GanGenerator:
             self._upload()
         return self._arena
 
+    def frame_cap(self, budget_bytes: int, batch_size: int = 32) -> int:
+        """The largest padded-frame count (rows x longest row) whose batches of up to ``batch_size`` rows keep the forward's
+        workspace (mb_gan_workspace_bytes) within ``budget_bytes``; at least 1.  For the infer_waveforms ``max_frames``."""
+        L = _lib.lib()
+
+        def fits(n):  # B rows of ceil(n / B) frames bound every batch of at most B rows and n padded frames
+            return int(L.mb_gan_workspace_bytes(self._handle, batch_size, -(-n // batch_size))) <= budget_bytes
+
+        lo, hi = 1, 1 << 30
+        while lo < hi:
+            mid = (lo + hi + 1) // 2
+            if fits(mid):
+                lo = mid
+            else:
+                hi = mid - 1
+        return lo
+
     # -- forward ---------------------------------------------------------------------------------
     def _ensure_workspace(self, B: int, T: int) -> torch.Tensor:
         need = int(_lib.lib().mb_gan_workspace_bytes(self._handle, B, T))
@@ -431,15 +448,29 @@ def _pinned_buffer(name: str, numel: int, dtype=torch.float32) -> torch.Tensor:
     return buf
 
 
-def _infer_device(generator, mels: Sequence[torch.Tensor], order: List[int], batch_size: int) -> List[torch.Tensor]:
+def _batches(lengths: Sequence[int], order: List[int], batch_size: int, max_frames: Optional[int]) -> List[List[int]]:
+    """consecutive runs of the length-sorted order: at most batch_size rows, and with max_frames, at most max_frames padded
+    frames (rows x the first, longest row) unless a row is longer than that alone"""
+    if max_frames is None:
+        return [order[s:s + batch_size] for s in range(0, len(order), batch_size)]
+    out: List[List[int]] = []
+    for i in order:
+        if out and len(out[-1]) < batch_size and (len(out[-1]) + 1) * lengths[out[-1][0]] <= max_frames:
+            out[-1].append(i)
+        else:
+            out.append([i])
+    return out
+
+
+def _infer_device(generator, mels: Sequence[torch.Tensor], order: List[int], batch_size: int,
+                  max_frames: Optional[int] = None) -> List[torch.Tensor]:
     """infer_waveforms_batched for CUDA mels: the same padded batches, built and returned on the device"""
     for i, m in enumerate(mels):
         if m.dim() != 2 or m.shape[0] != 80:
             raise ValueError(f"mel {i} must be [80, T], got {tuple(m.shape)}")
     out: List[Optional[torch.Tensor]] = [None] * len(mels)
     dev = mels[order[0]].device
-    for s in range(0, len(order), batch_size):
-        idx = order[s:s + batch_size]
+    for idx in _batches([m.shape[1] for m in mels], order, batch_size, max_frames):
         lens = [mels[i].shape[1] for i in idx]
         if lens[0] == 0:
             for i in idx:
@@ -454,27 +485,29 @@ def _infer_device(generator, mels: Sequence[torch.Tensor], order: List[int], bat
     return out  # type: ignore[return-value]
 
 
-def infer_waveforms_batched(generator, device, mels: Sequence[np.ndarray], batch_size: int = 32) -> List[np.ndarray]:
+def infer_waveforms_batched(generator, device, mels: Sequence[np.ndarray], batch_size: int = 32,
+                            max_frames: Optional[int] = None) -> List[np.ndarray]:
     """Shared body of hifigan / fregan ``infer_waveforms``: length-sorted padded batches, each result equal to the per-utterance
     call (padding is masked at every layer on the device).  All batches are enqueued back to back (pinned H2D -> forward -> pinned
     D2H) and the host waits once at the end.  Host work is kept off the critical path (tools/time_e2e_host.py, cfg 2): the mels are
     packed into the pinned staging with numpy slice assignments (0.30 -> 0.1 ms for 32 utterances), the lengths travel in a
     pinned block too, and the copy out of the (reused) staging buffer (0.39 ms for 6.5 MB) overlaps the D2H transfer piece by piece.
     When every mel is a CUDA tensor [80, T_i] (a mel decoder's output, say), the batches are built on the mels' device and
-    the results are CUDA waveforms [T_i * hop], views of each batch's output, in the same batches with the same bits."""
+    the results are CUDA waveforms [T_i * hop], views of each batch's output, in the same batches with the same bits.
+    ``max_frames`` (default None: no cap) also bounds each batch's padded frames, rows x longest row (``frame_cap`` derives
+    it from a workspace budget); a mel longer than the cap is vocoded alone.  Every result is its B = 1 forward either way."""
     n_mels = 80  # hifigan/models.py:99, fregan/generator.py hard-code 80 mel channels
     on_device = [torch.is_tensor(m) and m.is_cuda for m in mels]
     order = sorted(range(len(mels)), key=lambda i: -mels[i].shape[1])
     if any(on_device):
         if not all(on_device):
             raise ValueError("mels must be all CUDA tensors or all host arrays")
-        return _infer_device(generator, mels, order, batch_size)
+        return _infer_device(generator, mels, order, batch_size, max_frames)
     out: List[Optional[np.ndarray]] = [None] * len(mels)
     hop = generator.hop
     batches = []
     n_in = n_out = n_len = 0
-    for s in range(0, len(order), batch_size):
-        idx = order[s:s + batch_size]
+    for idx in _batches([m.shape[1] for m in mels], order, batch_size, max_frames):
         tmax = max(mels[i].shape[1] for i in idx)
         batches.append((idx, tmax, n_in, n_out, n_len))
         n_in += len(idx) * n_mels * tmax

@@ -99,9 +99,10 @@ def infer_waveform(mel, progress_callback=None):
     return audio, output_sample_rate
 
 
-def infer_waveforms(mels: Sequence[np.ndarray], batch_size: int = 32) -> List[np.ndarray]:
+def infer_waveforms(mels: Sequence[np.ndarray], batch_size: int = 32, max_frames: Optional[int] = None) -> List[np.ndarray]:
     """Vocode many utterances as length-sorted padded batches; each result equals the per-utterance
-    call (padding is masked at every layer on the device).  See ``_gan.infer_waveforms_batched``."""
+    call (padding is masked at every layer on the device).  ``max_frames`` also bounds each batch's padded frames (rows x
+    longest row; default None: no bound).  See ``_gan.infer_waveforms_batched``."""
     if generator is None:
         raise Exception("Please load fre-gan in memory before using it")
-    return infer_waveforms_batched(generator, _device, mels, batch_size)
+    return infer_waveforms_batched(generator, _device, mels, batch_size, max_frames)
