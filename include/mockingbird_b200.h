@@ -1235,12 +1235,31 @@ int mb_vits_decode(mb_vits* h, const float* m_p, const float* logs_p, const int3
  *   WN       WN layer `sub` of coupling layer flow.flows.(2 * index): x = h [B, hidden, T], x2 = g [B, gin] or NULL;
  *            y = h after the residual update, y2 = the skip stream [B, hidden, T] (read unless sub == 0, then written)
  *   DDSCONV  DDSConv "dp.convs." (index 0) or "dp.flows.<index>.convs.": x [B, hidden, T] -> y
- *   DECODER  dec(x, g) on z = x [B, inter, T] unmasked, x2 = sid int32 [B] (multi-speaker); y = wav [B, 1, T * hop] */
+ *   DECODER  dec(x, g) on z = x [B, inter, T] unmasked, x2 = sid int32 [B] (multi-speaker); y = wav [B, 1, T * hop]
+ *   CONV     one launch of the FP32 conv kernel through its host wrapper (MB_ERR_INVALID, nothing launched, for k > 7 or
+ *            (k - 1) * dil > 14): y[b, co, t] = epi(bias[co] + bbias[b * bbs + co] + sum_{ci, j} w[co, ci, j] *
+ *            x[b * xbs + ci * T + t + j * dil - pad]), x read as 0 outside [0, T) and, with in_mask, at t >= lengths[b];
+ *            epi: relu, then mode (0 store, 1 y += v, 2 y -= v), then * mask with out_mask.  y's batch stride is ybs and
+ *            its channel stride T.  lengths, bias and bbias may be NULL
+ *   LAYERNORM y = res + act(LayerNorm_cin(x + x2) * w + bias) (* mask when lengths is given) over [B, cin, T]; x2 and
+ *            res may be NULL, act = GELU when gelu != 0
+ *   ENC_LAYER text-encoder layer `index` on x [B, hidden, T] -> y (attention, conv_o, LN 1, FFN, LN 2; the last layer
+ *            masks its output)
+ *   LOGW     the duration predictor's logw [B, 1, T] (before exp and ceil) on the encoder output x [B, hidden, T];
+ *            x2 = sid int32 [B] (NULL: no g), x3 = the SDP's unscaled noise [B, 2, T]; y2 (nullable) receives what
+ *            mb_vits_durations derives from it at length_scale: w_ceil int32 [B, T] followed by y_lengths int32 [B]
+ *   COUPLING ResidualCouplingLayer flow.flows.(2 * index) in reverse on z = x [B, inter, T] -> y, masked at lengths;
+ *            x2 = g [B, gin] or NULL (only with speakers) */
 #define MB_VITS_DBG_SPLINE 0
 #define MB_VITS_DBG_ATTN 1
 #define MB_VITS_DBG_WN 2
 #define MB_VITS_DBG_DDSCONV 3
 #define MB_VITS_DBG_DECODER 4
+#define MB_VITS_DBG_CONV 5
+#define MB_VITS_DBG_LAYERNORM 6
+#define MB_VITS_DBG_ENC_LAYER 7
+#define MB_VITS_DBG_LOGW 8
+#define MB_VITS_DBG_COUPLING 9
 typedef struct mb_vits_debug_spec {
   int32_t kind, batch, frames, index, sub, c0, c1;
   const int32_t* lengths;
@@ -1249,6 +1268,14 @@ typedef struct mb_vits_debug_spec {
   const float* x3;
   float* y;
   float* y2;
+  /* CONV / LAYERNORM operands: w = weight or gamma, bias = bias or beta */
+  const float* w;
+  const float* bias;
+  const float* bbias;
+  const float* res;
+  int64_t xbs, ybs;
+  int32_t bbs, cin, cout, k, dil, pad, in_mask, out_mask, relu, mode, gelu;
+  float noise_scale_w, length_scale; /* LOGW */
 } mb_vits_debug_spec;
 size_t mb_vits_debug_workspace_bytes(const mb_vits* h, const mb_vits_debug_spec* spec);
 int mb_vits_debug(mb_vits* h, const mb_vits_debug_spec* spec, void* workspace, size_t workspace_bytes, void* stream);

@@ -236,12 +236,16 @@ class VitsConfig(C.Structure):
         (n, C.c_int32) for n in ("upsample_initial_channel", "n_speakers", "gin_channels", "use_sdp", "precision")]
 
 
-MB_VITS_DBG = {"spline": 0, "attn": 1, "wn": 2, "ddsconv": 3, "decoder": 4}
+MB_VITS_DBG = {"spline": 0, "attn": 1, "wn": 2, "ddsconv": 3, "decoder": 4, "conv": 5, "layernorm": 6, "enc_layer": 7,
+               "logw": 8, "coupling": 9}
 
 
 class VitsDebugSpec(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("kind", "batch", "frames", "index", "sub", "c0", "c1")] + [
-        (n, C.c_void_p) for n in ("lengths", "x", "x2", "x3", "y", "y2")]
+        (n, C.c_void_p) for n in ("lengths", "x", "x2", "x3", "y", "y2", "w", "bias", "bbias", "res")] + [
+        ("xbs", C.c_int64), ("ybs", C.c_int64)] + [
+        (n, C.c_int32) for n in ("bbs", "cin", "cout", "k", "dil", "pad", "in_mask", "out_mask", "relu", "mode", "gelu")] + [
+        ("noise_scale_w", C.c_float), ("length_scale", C.c_float)]
 
 
 class TtsPiece(C.Structure):

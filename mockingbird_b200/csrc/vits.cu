@@ -289,9 +289,10 @@ __global__ void spline_flow_kernel(const float* h, const float* wp, const float*
 }
 
 // ElementwiseAffine reverse on the SDP's z (vits_modules.py:287) followed by w = exp(logw) * mask * length_scale, w_ceil =
-// ceil(w) for channel 0 (vits.py:511-513); dp_out: the DurationPredictor's logw [B, 1, T] instead (ea_m == nullptr)
+// ceil(w) for channel 0 (vits.py:511-513); z is the DurationPredictor's logw [B, 1, T] instead when ea_m == nullptr.
+// logw_out [B, T] (nullable) receives the logw the durations were taken from.
 __global__ void durations_kernel(const float* z, const float* ea_m, const float* ea_logs, int zC, float length_scale, int B,
-                                 int T, const int32_t* len, int32_t* w_ceil, int32_t* y_len) {
+                                 int T, const int32_t* len, int32_t* w_ceil, int32_t* y_len, float* logw_out) {
   const int b = blockIdx.x;
   __shared__ int tot[32];
   int s = 0;
@@ -299,6 +300,7 @@ __global__ void durations_kernel(const float* z, const float* ea_m, const float*
     const float m = t < len[b] ? 1.f : 0.f;
     float logw = z[(long long)b * zC * T + t];
     if (ea_m) logw = (logw - ea_m[0]) * expf(-ea_logs[0]) * m;
+    if (logw_out) logw_out[(long long)b * T + t] = logw;
     const float w = expf(logw) * m * length_scale;
     const int c = (int)ceilf(w);
     w_ceil[(long long)b * T + t] = c;
@@ -564,6 +566,118 @@ DecWs dec_layout(const mb_vits* h, size_t B, size_t Tx, size_t Ty, size_t Td) {
   return o;
 }
 
+// The stages below are shared by mb_vits_durations / mb_vits_decode and mb_vits_debug, so that the debug kinds run the
+// shipped code.
+
+// Text-encoder layer l (vits_modules.py:407-419) in place on X [B, H, T]: X = LN_1(X + conv_o(attn(q, k, v))), then
+// X = LN_2(X + FFN(X)), masked after the last layer.  Scratch: the q, k, v, a, y and f planes of `o` in `ws`.
+int enc_layer(const mb_vits* h, int l, float* X, const DurWs& o, char* ws, int B, int T, const int32_t* len, cudaStream_t st) {
+  auto F = [&](size_t off) { return (float*)ws + off; };
+  const int H = h->H, NH = h->NH;
+  float *Q = F(o.q), *Kb = F(o.k), *V = F(o.v), *A = F(o.a), *Y = F(o.y), *FF = F(o.f);
+  const std::string L = std::to_string(l), a = "enc_p.encoder.attn_layers." + L;
+  TRY(conv1x1("conv_q", X, H, h->p(a + ".conv_q.weight"), h->p(a + ".conv_q.bias"), Q, H, B, T, st));
+  TRY(conv1x1("conv_k", X, H, h->p(a + ".conv_k.weight"), h->p(a + ".conv_k.bias"), Kb, H, B, T, st));
+  TRY(conv1x1("conv_v", X, H, h->p(a + ".conv_v.weight"), h->p(a + ".conv_v.bias"), V, H, B, T, st));
+  rel_attn_kernel<<<dim3(T, NH, B), 128, 0, st>>>(Q, Kb, V, h->p(a + ".emb_rel_k"), h->p(a + ".emb_rel_v"), A, H, NH, T, len);
+  MB_LAUNCH_CHECK("rel_attn_kernel");
+  TRY(conv1x1("conv_o", A, H, h->p(a + ".conv_o.weight"), h->p(a + ".conv_o.bias"), Y, H, B, T, st));
+  TRY(layernorm(X, Y, h->p("enc_p.encoder.norm_layers_1." + L + ".gamma"), h->p("enc_p.encoder.norm_layers_1." + L + ".beta"),
+                nullptr, X, B, H, T, 0, nullptr, st));
+  // FFN (vits_modules.py:649-657): conv_2(relu(conv_1(x * mask)) * mask) * mask, same padding
+  const std::string f = "enc_p.encoder.ffn_layers." + L;
+  TRY(conv("ffn conv_1", X, (long long)H * T, H, h->p(f + ".conv_1.weight"), h->p(f + ".conv_1.bias"), nullptr, 0, FF,
+           (long long)h->F * T, h->F, B, T, h->K, 1, (h->K - 1) / 2, len, 1, 0, 1, EPI_STORE_, st));
+  TRY(conv("ffn conv_2", FF, (long long)h->F * T, h->F, h->p(f + ".conv_2.weight"), h->p(f + ".conv_2.bias"), nullptr, 0, Y,
+           (long long)H * T, H, B, T, h->K, 1, (h->K - 1) / 2, len, 1, 1, 0, EPI_STORE_, st));
+  return layernorm(X, Y, h->p("enc_p.encoder.norm_layers_2." + L + ".gamma"), h->p("enc_p.encoder.norm_layers_2." + L + ".beta"),
+                   nullptr, X, B, H, T, 0, l == h->NL - 1 ? len : nullptr, st);
+}
+
+// The duration predictor on the encoder output X [B, H, T] (vits.py:48-130, either kind), then w_ceil = ceil(exp(logw) *
+// mask * length_scale) and y_len = max(1, sum w_ceil).  g = emb_g[sid] conditions it when sid is given; noise [B, 2, T] is
+// the SDP's unscaled draw.  logw_out [B, T] (nullable) receives logw.  Scratch: the remaining planes of `o` in `ws`.
+int duration_predictor(const mb_vits* h, const float* X, const int32_t* sid, const float* noise, float noise_scale_w,
+                       float length_scale, int32_t* w_ceil, int32_t* y_lengths, float* logw_out, const DurWs& o, char* ws, int B,
+                       int T, const int32_t* len, cudaStream_t st) {
+  auto F = [&](size_t off) { return (float*)ws + off; };
+  const int H = h->H;
+  float* FF = F(o.f);
+  const float* gb = nullptr;
+  if (h->G && sid) {
+    gather_rows_kernel<<<blocks((long long)B * h->G), 256, 0, st>>>(h->p("emb_g.weight"), sid, F(o.g), B, h->G, h->cfg.n_speakers);
+    MB_LAUNCH_CHECK("gather_rows_kernel");
+    TRY(conv("dp.cond", F(o.g), h->G, h->G, h->p("dp.cond.weight"), h->p("dp.cond.bias"), nullptr, 0, F(o.gb), H, H, B, 1, 1, 1, 0,
+             nullptr, 0, 0, 0, EPI_STORE_, st));
+    gb = F(o.gb);
+  }
+  float *S0 = F(o.s0), *S1 = F(o.s1), *S2 = F(o.s2), *S3 = F(o.s3), *Z = F(o.z);
+  if (h->cfg.use_sdp) {
+    // StochasticDurationPredictor reverse (vits.py:48-93): x = proj(DDS(pre(x) + cond(g))) * mask
+    TRY(conv("dp.pre", X, (long long)H * T, H, h->p("dp.pre.weight"), h->p("dp.pre.bias"), gb, H, S0, (long long)H * T, H, B, T, 1,
+             1, 0, nullptr, 0, 0, 0, EPI_STORE_, st));
+    TRY(ddsconv(h, "dp.convs.", S0, S1, S2, B, H, T, len, st));
+    TRY(conv1x1("dp.proj", S0, H, h->p("dp.proj.weight"), h->p("dp.proj.bias"), S3, H, B, T, st, len, 0, 1));
+    // z = noise * noise_scale_w; flows: Flip, ConvFlow 7, Flip, ConvFlow 5, Flip, ConvFlow 3, Flip, ElementwiseAffine
+    scale_bias_kernel<<<blocks(2LL * B * T), 256, 0, st>>>(noise, noise_scale_w, nullptr, Z, B, 2, T);
+    MB_LAUNCH_CHECK("scale_bias_kernel");
+    int c0 = 1, c1 = 0;  // after the first Flip, channel 1 is x0 and channel 0 is x1
+    for (int f : {7, 5, 3}) {
+      const std::string n = "dp.flows." + std::to_string(f);
+      // ConvFlow: h = pre(x0); h = DDS(h + x); h = proj(h) * mask (fused into the spline kernel)
+      TRY(conv("convflow pre", Z + (long long)c0 * T, 2LL * T, 1, h->p(n + ".pre.weight"), h->p(n + ".pre.bias"), nullptr, 0, S0,
+               (long long)H * T, H, B, T, 1, 1, 0, nullptr, 0, 0, 0, EPI_STORE_, st));
+      add_kernel<<<blocks((long long)B * H * T), 256, 0, st>>>(S0, S3, S0, (long long)B * H * T);
+      MB_LAUNCH_CHECK("add_kernel");
+      TRY(ddsconv(h, n + ".convs.", S0, S1, S2, B, H, T, len, st));
+      spline_flow_kernel<<<blocks((long long)B * T * 32, 128), 128, 0, st>>>(S0, h->p(n + ".proj.weight"), h->p(n + ".proj.bias"),
+                                                                              Z, B, H, T, c0, c1, len);
+      MB_LAUNCH_CHECK("spline_flow_kernel");
+      std::swap(c0, c1);  // Flip
+    }
+    durations_kernel<<<B, 256, 0, st>>>(Z, h->p("dp.flows.0.m"), h->p("dp.flows.0.logs"), 2, length_scale, B, T, len, w_ceil,
+                                        y_lengths, logw_out);
+    MB_LAUNCH_CHECK("durations_kernel");
+    return MB_OK;
+  }
+  // DurationPredictor (vits.py:116-130)
+  const int D = h->DPC;
+  const float* xd = X;
+  if (gb) {
+    scale_bias_kernel<<<blocks((long long)B * H * T), 256, 0, st>>>(X, 1.f, gb, S0, B, H, T);
+    MB_LAUNCH_CHECK("scale_bias_kernel");
+    xd = S0;
+  }
+  TRY(conv("dp.conv_1", xd, (long long)H * T, H, h->p("dp.conv_1.weight"), h->p("dp.conv_1.bias"), nullptr, 0, S3,
+           (long long)D * T, D, B, T, 3, 1, 1, len, 1, 0, 1, EPI_STORE_, st));
+  TRY(layernorm(S3, nullptr, h->p("dp.norm_1.gamma"), h->p("dp.norm_1.beta"), nullptr, S3, B, D, T, 0, nullptr, st));
+  TRY(conv("dp.conv_2", S3, (long long)D * T, D, h->p("dp.conv_2.weight"), h->p("dp.conv_2.bias"), nullptr, 0, FF,
+           (long long)D * T, D, B, T, 3, 1, 1, len, 1, 0, 1, EPI_STORE_, st));
+  TRY(layernorm(FF, nullptr, h->p("dp.norm_2.gamma"), h->p("dp.norm_2.beta"), nullptr, FF, B, D, T, 0, nullptr, st));
+  TRY(conv1x1("dp.proj", FF, D, h->p("dp.proj.weight"), h->p("dp.proj.bias"), Z, 1, B, T, st, len, 1, 1));
+  durations_kernel<<<B, 256, 0, st>>>(Z, nullptr, nullptr, 1, length_scale, B, T, len, w_ceil, y_lengths, logw_out);
+  MB_LAUNCH_CHECK("durations_kernel");
+  return MB_OK;
+}
+
+// ResidualCouplingLayer flow.flows.(2f) in reverse, mean only (vits_modules.py:317-336), in place on z [B, I, T]: h =
+// pre(x0) * mask, WN (vits_modules.py:141-169) with the cond_layer(g) bias when g [B, G] is given, then x1 = (x1 -
+// post(out * mask) * mask) * mask.  Scratch: hh, acts, out [B, H, T], xin [B, 2H, T], cond [B, 2H * 4].
+int coupling_layer(const mb_vits* h, int f, float* z, const float* g, float* hh, float* xin, float* acts, float* out, float* cond,
+                   int B, int T, const int32_t* len, cudaStream_t st) {
+  const int H = h->H, Ih = h->I / 2;
+  const long long zbs = (long long)h->I * T, hbs = (long long)H * T;
+  const std::string n = "flow.flows." + std::to_string(2 * f), e = n + ".enc.";
+  TRY(conv("coupling pre", z, zbs, Ih, h->p(n + ".pre.weight"), h->p(n + ".pre.bias"), nullptr, 0, hh, hbs, H, B, T, 1, 1, 0, len,
+           0, 1, 0, EPI_STORE_, st));
+  if (g)
+    TRY(conv("cond_layer", g, h->G, h->G, h->p(e + "cond_layer.weight"), h->p(e + "cond_layer.bias"), nullptr, 0, cond,
+             2LL * H * kWnLayers, 2 * H * kWnLayers, B, 1, 1, 1, 0, nullptr, 0, 0, 0, EPI_STORE_, st));
+  for (int l = 0; l < kWnLayers; ++l) TRY(wn_layer(h, e, l, hh, xin, acts, out, g ? cond : nullptr, B, T, len, st));
+  return conv("coupling post", out, hbs, H, h->p(n + ".post.weight"), h->p(n + ".post.bias"), nullptr, 0, z + (long long)Ih * T, zbs,
+              Ih, B, T, 1, 1, 0, len, 1, 1, 0, EPI_SUB, st);
+}
+
 void declare(mb_vits* h) {
   WeightTable& w = h->w;
   const int64_t I = h->I, H = h->H, F = h->F, G = h->G, K = h->K, dk = H / h->NH;
@@ -767,92 +881,20 @@ int mb_vits_durations(mb_vits* h, const int32_t* x, const int32_t* x_lengths, in
   if (int rc = bind(fn, workspace, workspace_bytes, o.total, &ws)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   auto F = [&](size_t off) { return (float*)ws + off; };
-  const int H = h->H, I = h->I, NH = h->NH;
+  const int H = h->H, I = h->I;
   const int32_t* len = x_lengths;
-  float *X = F(o.x), *Q = F(o.q), *Kb = F(o.k), *V = F(o.v), *A = F(o.a), *Y = F(o.y), *FF = F(o.f);
+  float* X = F(o.x);
   // ---- text encoder (vits.py:167-177, vits_modules.py:407-419)
   TRY(conv("emo_proj", emo, kEmo, kEmo, h->p("enc_p.emo_proj.weight"), h->p("enc_p.emo_proj.bias"), nullptr, 0, F(o.e), H, H, B, 1,
            1, 1, 0, nullptr, 0, 0, 0, EPI_STORE_, st));
   embed_kernel<<<blocks((long long)B * H * T), 256, 0, st>>>(x, h->p("enc_p.emb.weight"), F(o.e), X, B, H, T, h->cfg.n_vocab, len);
   MB_LAUNCH_CHECK("embed_kernel");
-  for (int l = 0; l < h->NL; ++l) {
-    const std::string L = std::to_string(l), a = "enc_p.encoder.attn_layers." + L;
-    TRY(conv1x1("conv_q", X, H, h->p(a + ".conv_q.weight"), h->p(a + ".conv_q.bias"), Q, H, B, T, st));
-    TRY(conv1x1("conv_k", X, H, h->p(a + ".conv_k.weight"), h->p(a + ".conv_k.bias"), Kb, H, B, T, st));
-    TRY(conv1x1("conv_v", X, H, h->p(a + ".conv_v.weight"), h->p(a + ".conv_v.bias"), V, H, B, T, st));
-    rel_attn_kernel<<<dim3(T, NH, B), 128, 0, st>>>(Q, Kb, V, h->p(a + ".emb_rel_k"), h->p(a + ".emb_rel_v"), A, H, NH, T, len);
-    MB_LAUNCH_CHECK("rel_attn_kernel");
-    TRY(conv1x1("conv_o", A, H, h->p(a + ".conv_o.weight"), h->p(a + ".conv_o.bias"), Y, H, B, T, st));
-    TRY(layernorm(X, Y, h->p("enc_p.encoder.norm_layers_1." + L + ".gamma"), h->p("enc_p.encoder.norm_layers_1." + L + ".beta"),
-                  nullptr, X, B, H, T, 0, nullptr, st));
-    // FFN (vits_modules.py:649-657): conv_2(relu(conv_1(x * mask)) * mask) * mask, same padding
-    const std::string f = "enc_p.encoder.ffn_layers." + L;
-    TRY(conv("ffn conv_1", X, (long long)H * T, H, h->p(f + ".conv_1.weight"), h->p(f + ".conv_1.bias"), nullptr, 0, FF,
-             (long long)h->F * T, h->F, B, T, h->K, 1, (h->K - 1) / 2, len, 1, 0, 1, EPI_STORE_, st));
-    TRY(conv("ffn conv_2", FF, (long long)h->F * T, h->F, h->p(f + ".conv_2.weight"), h->p(f + ".conv_2.bias"), nullptr, 0, Y,
-             (long long)H * T, H, B, T, h->K, 1, (h->K - 1) / 2, len, 1, 1, 0, EPI_STORE_, st));
-    TRY(layernorm(X, Y, h->p("enc_p.encoder.norm_layers_2." + L + ".gamma"), h->p("enc_p.encoder.norm_layers_2." + L + ".beta"),
-                  nullptr, X, B, H, T, 0, l == h->NL - 1 ? len : nullptr, st));
-  }
+  for (int l = 0; l < h->NL; ++l) TRY(enc_layer(h, l, X, o, ws, B, T, len, st));
   TRY(conv1x1("enc_p.proj m", X, H, h->p("enc_p.proj.weight"), h->p("enc_p.proj.bias"), m_p, I, B, T, st, len, 0, 1));
   TRY(conv1x1("enc_p.proj logs", X, H, h->p("enc_p.proj.weight") + (size_t)I * H, h->p("enc_p.proj.bias") + I, logs_p, I, B, T, st,
               len, 0, 1));
   // ---- speaker embedding, duration predictor
-  const float* gb = nullptr;
-  if (h->G) {
-    gather_rows_kernel<<<blocks((long long)B * h->G), 256, 0, st>>>(h->p("emb_g.weight"), sid, F(o.g), B, h->G, h->cfg.n_speakers);
-    MB_LAUNCH_CHECK("gather_rows_kernel");
-    TRY(conv("dp.cond", F(o.g), h->G, h->G, h->p("dp.cond.weight"), h->p("dp.cond.bias"), nullptr, 0, F(o.gb), H, H, B, 1, 1, 1, 0,
-             nullptr, 0, 0, 0, EPI_STORE_, st));
-    gb = F(o.gb);
-  }
-  float *S0 = F(o.s0), *S1 = F(o.s1), *S2 = F(o.s2), *S3 = F(o.s3), *Z = F(o.z);
-  if (h->cfg.use_sdp) {
-    // StochasticDurationPredictor reverse (vits.py:48-93): x = proj(DDS(pre(x) + cond(g))) * mask
-    TRY(conv("dp.pre", X, (long long)H * T, H, h->p("dp.pre.weight"), h->p("dp.pre.bias"), gb, H, S0, (long long)H * T, H, B, T, 1,
-             1, 0, nullptr, 0, 0, 0, EPI_STORE_, st));
-    TRY(ddsconv(h, "dp.convs.", S0, S1, S2, B, H, T, len, st));
-    TRY(conv1x1("dp.proj", S0, H, h->p("dp.proj.weight"), h->p("dp.proj.bias"), S3, H, B, T, st, len, 0, 1));
-    // z = noise * noise_scale_w; flows: Flip, ConvFlow 7, Flip, ConvFlow 5, Flip, ConvFlow 3, Flip, ElementwiseAffine
-    scale_bias_kernel<<<blocks(2LL * B * T), 256, 0, st>>>(noise, noise_scale_w, nullptr, Z, B, 2, T);
-    MB_LAUNCH_CHECK("scale_bias_kernel");
-    int c0 = 1, c1 = 0;  // after the first Flip, channel 1 is x0 and channel 0 is x1
-    for (int f : {7, 5, 3}) {
-      const std::string n = "dp.flows." + std::to_string(f);
-      // ConvFlow: h = pre(x0); h = DDS(h + x); h = proj(h) * mask (fused into the spline kernel)
-      TRY(conv("convflow pre", Z + (long long)c0 * T, 2LL * T, 1, h->p(n + ".pre.weight"), h->p(n + ".pre.bias"), nullptr, 0, S0,
-               (long long)H * T, H, B, T, 1, 1, 0, nullptr, 0, 0, 0, EPI_STORE_, st));
-      add_kernel<<<blocks((long long)B * H * T), 256, 0, st>>>(S0, S3, S0, (long long)B * H * T);
-      MB_LAUNCH_CHECK("add_kernel");
-      TRY(ddsconv(h, n + ".convs.", S0, S1, S2, B, H, T, len, st));
-      spline_flow_kernel<<<blocks((long long)B * T * 32, 128), 128, 0, st>>>(S0, h->p(n + ".proj.weight"), h->p(n + ".proj.bias"),
-                                                                              Z, B, H, T, c0, c1, len);
-      MB_LAUNCH_CHECK("spline_flow_kernel");
-      std::swap(c0, c1);  // Flip
-    }
-    durations_kernel<<<B, 256, 0, st>>>(Z, h->p("dp.flows.0.m"), h->p("dp.flows.0.logs"), 2, length_scale, B, T, len, w_ceil,
-                                        y_lengths);
-    MB_LAUNCH_CHECK("durations_kernel");
-  } else {
-    // DurationPredictor (vits.py:116-130)
-    const int D = h->DPC;
-    const float* xd = X;
-    if (gb) {
-      scale_bias_kernel<<<blocks((long long)B * H * T), 256, 0, st>>>(X, 1.f, gb, S0, B, H, T);
-      MB_LAUNCH_CHECK("scale_bias_kernel");
-      xd = S0;
-    }
-    TRY(conv("dp.conv_1", xd, (long long)H * T, H, h->p("dp.conv_1.weight"), h->p("dp.conv_1.bias"), nullptr, 0, S3,
-             (long long)D * T, D, B, T, 3, 1, 1, len, 1, 0, 1, EPI_STORE_, st));
-    TRY(layernorm(S3, nullptr, h->p("dp.norm_1.gamma"), h->p("dp.norm_1.beta"), nullptr, S3, B, D, T, 0, nullptr, st));
-    TRY(conv("dp.conv_2", S3, (long long)D * T, D, h->p("dp.conv_2.weight"), h->p("dp.conv_2.bias"), nullptr, 0, FF,
-             (long long)D * T, D, B, T, 3, 1, 1, len, 1, 0, 1, EPI_STORE_, st));
-    TRY(layernorm(FF, nullptr, h->p("dp.norm_2.gamma"), h->p("dp.norm_2.beta"), nullptr, FF, B, D, T, 0, nullptr, st));
-    TRY(conv1x1("dp.proj", FF, D, h->p("dp.proj.weight"), h->p("dp.proj.bias"), Z, 1, B, T, st, len, 1, 1));
-    durations_kernel<<<B, 256, 0, st>>>(Z, nullptr, nullptr, 1, length_scale, B, T, len, w_ceil, y_lengths);
-    MB_LAUNCH_CHECK("durations_kernel");
-  }
-  return MB_OK;
+  return duration_predictor(h, X, sid, noise, noise_scale_w, length_scale, w_ceil, y_lengths, nullptr, o, ws, B, T, len, st);
 }
 
 size_t mb_vits_decode_workspace_bytes(const mb_vits* h, int32_t batch, int32_t t_x, int32_t t_y, int32_t t_dec) {
@@ -875,7 +917,7 @@ int mb_vits_decode(mb_vits* h, const float* m_p, const float* logs_p, const int3
   if (int rc = bind(fn, workspace, workspace_bytes, o.total, &ws, 1024)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   auto F = [&](size_t off) { return (float*)ws + off; };
-  const int H = h->H, I = h->I, G = h->G, Ih = h->I / 2;
+  const int I = h->I, G = h->G;
   int32_t* cum = (int32_t*)ws + o.cum;
   int32_t* ylen = (int32_t*)ws + o.ylen;
   cumsum_kernel<<<blocks(B, 64), 64, 0, st>>>(w_ceil, x_lengths, cum, ylen, B, Tx);
@@ -894,23 +936,11 @@ int mb_vits_decode(mb_vits* h, const float* m_p, const float* logs_p, const int3
   }
   // ---- reverse coupling flow (vits.py:203-210): Flip, layer 6, Flip, layer 4, Flip, layer 2, Flip, layer 0
   float *hh = F(o.hh), *xin = F(o.xin), *acts = F(o.acts), *out = F(o.out), *cond = F(o.cond);
-  const long long zbs = (long long)I * Ty, hbs = (long long)H * Ty;
   for (int f = 3; f >= 0; --f) {
-    const std::string n = "flow.flows." + std::to_string(2 * f), e = n + ".enc.";
     flip_kernel<<<blocks((long long)B * I * Ty), 256, 0, st>>>(za, zb, B, I, Ty);
     MB_LAUNCH_CHECK("flip_kernel");
     std::swap(za, zb);
-    // ResidualCouplingLayer reverse, mean only (vits_modules.py:317-336): h = pre(x0) * mask
-    TRY(conv("coupling pre", za, zbs, Ih, h->p(n + ".pre.weight"), h->p(n + ".pre.bias"), nullptr, 0, hh, hbs, H, B, Ty, 1, 1, 0,
-             ylen, 0, 1, 0, EPI_STORE_, st));
-    if (G)
-      TRY(conv("cond_layer", g, G, G, h->p(e + "cond_layer.weight"), h->p(e + "cond_layer.bias"), nullptr, 0, cond,
-               2LL * H * kWnLayers, 2 * H * kWnLayers, B, 1, 1, 1, 0, nullptr, 0, 0, 0, EPI_STORE_, st));
-    // WN (vits_modules.py:141-169)
-    for (int l = 0; l < kWnLayers; ++l) TRY(wn_layer(h, e, l, hh, xin, acts, out, G ? cond : nullptr, B, Ty, ylen, st));
-    // x1 = (x1 - post(out * mask) * mask) * mask
-    TRY(conv("coupling post", out, hbs, H, h->p(n + ".post.weight"), h->p(n + ".post.bias"), nullptr, 0, za + (long long)Ih * Ty,
-             zbs, Ih, B, Ty, 1, 1, 0, ylen, 1, 1, 0, EPI_SUB, st));
+    TRY(coupling_layer(h, f, za, g, hh, xin, acts, out, cond, B, Ty, ylen, st));
   }
   if (z) MB_CUDA_CHECK(cudaMemcpyAsync(z, za, sizeof(float) * B * I * Ty, cudaMemcpyDeviceToDevice, st));
   // ---- decoder: dec((z * y_mask)[:, :, :t_dec], g) with cond(g) folded into conv_pre over the extra g channels
@@ -923,17 +953,23 @@ int mb_vits_decode(mb_vits* h, const float* m_p, const float* logs_p, const int3
 }  // extern "C"
 
 namespace {
-// mb_vits_debug's workspace: two scratch planes (x_in / acts, DDSConv), the cond_layer output / decoder input, the generator's
+// mb_vits_debug's workspace: scratch planes (x_in / acts, DDSConv, the coupling layer's h / acts / out), the cond_layer
+// output / decoder input, the text encoder's layout (ENC_LAYER, LOGW), LOGW's w_ceil / y_len, the generator's
 struct DbgWs {
-  size_t s0, s1, s2, gan, total;
+  size_t s0, s1, s2, s3, dur, ints, gan, total;
 };
 DbgWs dbg_layout(const mb_vits* h, const mb_vits_debug_spec* s) {
   const size_t B = s->batch, T = s->frames, H = h->H;
+  const bool planes = s->kind <= MB_VITS_DBG_DECODER || s->kind == MB_VITS_DBG_COUPLING;
+  const bool dur = s->kind == MB_VITS_DBG_ENC_LAYER || s->kind == MB_VITS_DBG_LOGW;
   WsLayout L;
   DbgWs o;
-  o.s0 = L.take<float>(B * 2 * H * T);
-  o.s1 = L.take<float>(B * 2 * H * T);
-  o.s2 = L.take<float>(B * 2 * H * kWnLayers + B * (h->I + h->G) * T);
+  o.s0 = L.take<float>(planes ? B * 2 * H * T : 0);
+  o.s1 = L.take<float>(planes ? B * 2 * H * T : 0);
+  o.s2 = L.take<float>(planes ? B * 2 * H * kWnLayers + B * (h->I + h->G) * T : 0);
+  o.s3 = L.take<float>(s->kind == MB_VITS_DBG_COUPLING ? B * H * T : 0);
+  o.dur = L.take(dur ? dur_layout(h, B, T).total : 0);
+  o.ints = L.take<int32_t>(s->kind == MB_VITS_DBG_LOGW ? B * T + B : 0);
   L.align = 1024;
   o.gan = L.take(s->kind == MB_VITS_DBG_DECODER ? mb_gan_workspace_bytes(h->gan, (int32_t)B, (int32_t)T) : 0);
   o.total = L.total();
@@ -954,7 +990,8 @@ int mb_vits_debug(mb_vits* h, const mb_vits_debug_spec* s, void* workspace, size
   if (!h->finalized) return fail(MB_ERR_STATE, "%s: weights not finalized", fn);
   const int B = s->batch, T = s->frames, H = h->H;
   if (B <= 0 || T <= 0) return fail(MB_ERR_INVALID, "%s: empty batch", fn);
-  if (s->kind != MB_VITS_DBG_DECODER && !s->lengths) return fail(MB_ERR_INVALID, "%s: lengths required", fn);
+  const bool unmasked = s->kind == MB_VITS_DBG_DECODER || s->kind == MB_VITS_DBG_CONV || s->kind == MB_VITS_DBG_LAYERNORM;
+  if (!unmasked && !s->lengths) return fail(MB_ERR_INVALID, "%s: lengths required", fn);
   char* ws;
   const DbgWs o = dbg_layout(h, s);
   if (int rc = bind(fn, workspace, workspace_bytes, o.total, &ws, 1024)) return rc;
@@ -1015,6 +1052,36 @@ int mb_vits_debug(mb_vits* h, const mb_vits_debug_spec* s, void* workspace, size
       dec_input_kernel<<<blocks((long long)B * (I + G) * T), 256, 0, st>>>(s->x, g, din, B, I, G, T, T, nullptr);
       MB_LAUNCH_CHECK("dec_input_kernel");
       return mb_gan_forward(h->gan, din, nullptr, B, T, s->y, ws + o.gan, mb_gan_workspace_bytes(h->gan, B, T), stream);
+    }
+    case MB_VITS_DBG_CONV: {  // one conv1d_kernel launch through conv(), whose limits it keeps
+      if (!s->w || s->cin < 1 || s->cout < 1 || s->k < 1 || s->dil < 1 || s->pad < 0 || s->mode < EPI_STORE_ || s->mode > EPI_SUB ||
+          (s->bbias && s->bbs < s->cout))
+        return fail(MB_ERR_INVALID, "%s: conv needs a weight, cin, cout, k, dil >= 1, pad >= 0, mode 0..2, bbs >= cout", fn);
+      return conv("mb_vits_debug conv", s->x, s->xbs, s->cin, s->w, s->bias, s->bbias, s->bbs, s->y, s->ybs, s->cout, B, T, s->k,
+                  s->dil, s->pad, len, s->in_mask, s->out_mask, s->relu, s->mode, st);
+    }
+    case MB_VITS_DBG_LAYERNORM: {  // y = res + act(LN_cin(x + x2)) (* mask) with gamma = w, beta = bias
+      if (!s->w || !s->bias || s->cin < 1) return fail(MB_ERR_INVALID, "%s: layernorm needs gamma, beta and cin", fn);
+      return layernorm(s->x, s->x2, s->w, s->bias, s->res, s->y, B, s->cin, T, s->gelu, len, st);
+    }
+    case MB_VITS_DBG_ENC_LAYER: {  // y = text-encoder layer `index` on x
+      if (s->index < 0 || s->index >= h->NL || T > kMaxTokens)
+        return fail(MB_ERR_INVALID, "%s: encoder layer 0..%d and T <= %d", fn, h->NL - 1, kMaxTokens);
+      MB_CUDA_CHECK(cudaMemcpyAsync(s->y, s->x, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
+      return enc_layer(h, s->index, s->y, dur_layout(h, B, T), ws + o.dur, B, T, len, st);
+    }
+    case MB_VITS_DBG_LOGW: {  // y = logw [B, 1, T] of the duration predictor on the encoder output x, y2 = w_ceil, y_len
+      if ((h->cfg.use_sdp && !s->x3) || (s->x2 && !h->G))
+        return fail(MB_ERR_INVALID, "%s: logw needs the SDP noise in x3 (stochastic predictor) and sid only with speakers", fn);
+      int32_t* wc = s->y2 ? (int32_t*)s->y2 : (int32_t*)ws + o.ints;
+      return duration_predictor(h, s->x, (const int32_t*)s->x2, s->x3, s->noise_scale_w, s->length_scale, wc, wc + (size_t)B * T, s->y,
+                                dur_layout(h, B, T), ws + o.dur, B, T, len, st);
+    }
+    case MB_VITS_DBG_COUPLING: {  // y = coupling layer flow.flows.(2 * index) in reverse on z = x
+      if (s->index < 0 || s->index > 3 || (s->x2 && !h->G))
+        return fail(MB_ERR_INVALID, "%s: coupling index 0..3 (g only with speakers)", fn);
+      MB_CUDA_CHECK(cudaMemcpyAsync(s->y, s->x, sizeof(float) * B * h->I * T, cudaMemcpyDeviceToDevice, st));
+      return coupling_layer(h, s->index, s->y, s->x2, s1, s0, s1 + n, (float*)ws + o.s3, s2, B, T, len, st);
     }
     default:
       return fail(MB_ERR_INVALID, "%s: unknown kind %d", fn, s->kind);

@@ -59,18 +59,37 @@ def rel_attention(q, k, v, erk, erv, lengths, n_heads: int):
     qh = q.view(B, n_heads, dk, T).transpose(2, 3) / math.sqrt(dk)  # [B, nh, T, dk]
     kh = k.view(B, n_heads, dk, T).transpose(2, 3)
     vh = v.view(B, n_heads, dk, T).transpose(2, 3)
-    rel = torch.arange(T)[None, :] - torch.arange(T)[:, None]  # [t, s] = s - t
-    inside = rel.abs() <= WINDOW
-    idx = (rel.clamp(-WINDOW, WINDOW) + WINDOW)
-    rk = _d(erk)[0][idx] * inside[..., None]  # [T, T, dk]
-    rv = _d(erv)[0][idx] * inside[..., None]
-    scores = qh @ kh.transpose(2, 3) + torch.einsum("bhtd,tsd->bhts", qh, rk)
+    # the relative terms live on the 2W+1 diagonals s = t + r: scores[t, t + r] += q_t . erk[r], out_t += p[t, t + r] erv[r]
+    t = torch.arange(T)
+    band = [(r, t[(t + r >= 0) & (t + r < T)]) for r in range(-WINDOW, WINDOW + 1)]
+    rl = qh @ _d(erk)[0].T  # [B, nh, T, 2W+1]
+    scores = qh @ kh.transpose(2, 3)
+    for r, tt in band:
+        scores[:, :, tt, tt + r] += rl[:, :, tt, r + WINDOW]
     m = mask_of(lengths, T)[:, 0]
     valid = (m[:, None, :, None] * m[:, None, None, :]) > 0
     scores = torch.where(valid, scores, torch.full_like(scores, -1e4))
     p = torch.softmax(scores, -1)
-    out = p @ vh + torch.einsum("bhts,tsd->bhtd", p, rv)
+    out = p @ vh
+    rv = _d(erv)[0]
+    for r, tt in band:
+        out[:, :, tt] += p[:, :, tt, tt + r, None] * rv[r + WINDOW]
     return out.transpose(2, 3).reshape(B, H, T)
+
+
+def text_encoder_layer(sd, cfg, l: int, h, lengths, last: bool):
+    """encoder layer l on h [B, H, T]: LN_1(h + conv_o(attention)), then LN_2(h + FFN(h)); masked when it is the last"""
+    m = mask_of(lengths, h.shape[2])
+    K = cfg["kernel_size"]
+    a = f"enc_p.encoder.attn_layers.{l}"
+    y = rel_attention(conv(sd, a + ".conv_q", h), conv(sd, a + ".conv_k", h), conv(sd, a + ".conv_v", h), sd[a + ".emb_rel_k"],
+                      sd[a + ".emb_rel_v"], lengths, cfg["n_heads"])
+    h = layer_norm(sd, f"enc_p.encoder.norm_layers_1.{l}", h + conv(sd, a + ".conv_o", y))
+    f = f"enc_p.encoder.ffn_layers.{l}"
+    y = torch.relu(conv(sd, f + ".conv_1", h * m, pad=(K - 1) // 2))
+    y = conv(sd, f + ".conv_2", y * m, pad=(K - 1) // 2) * m
+    h = layer_norm(sd, f"enc_p.encoder.norm_layers_2.{l}", h + y)
+    return h * m if last else h
 
 
 def text_encoder(sd, cfg, x, lengths, emo):
@@ -79,17 +98,8 @@ def text_encoder(sd, cfg, x, lengths, emo):
     m = mask_of(lengths, T)
     e = _d(emo) @ _d(sd["enc_p.emo_proj.weight"]).T + _d(sd["enc_p.emo_proj.bias"])
     h = (_d(sd["enc_p.emb.weight"])[torch.as_tensor(x).long()] * math.sqrt(H) + e[:, None, :]).transpose(1, 2) * m
-    K = cfg["kernel_size"]
     for i in range(cfg["n_layers"]):
-        a = f"enc_p.encoder.attn_layers.{i}"
-        y = rel_attention(conv(sd, a + ".conv_q", h), conv(sd, a + ".conv_k", h), conv(sd, a + ".conv_v", h), sd[a + ".emb_rel_k"],
-                          sd[a + ".emb_rel_v"], lengths, cfg["n_heads"])
-        h = layer_norm(sd, f"enc_p.encoder.norm_layers_1.{i}", h + conv(sd, a + ".conv_o", y))
-        f = f"enc_p.encoder.ffn_layers.{i}"
-        y = torch.relu(conv(sd, f + ".conv_1", h * m, pad=(K - 1) // 2))
-        y = conv(sd, f + ".conv_2", y * m, pad=(K - 1) // 2) * m
-        h = layer_norm(sd, f"enc_p.encoder.norm_layers_2.{i}", h + y)
-    h = h * m
+        h = text_encoder_layer(sd, cfg, i, h, lengths, i == cfg["n_layers"] - 1)
     stats = conv(sd, "enc_p.proj", h) * m
     I = cfg["inter_channels"]
     return h, stats[:, :I], stats[:, I:]
@@ -153,8 +163,8 @@ def convflow_spline(sd, index, h, z, lengths, c0: int, c1: int):
     return out * m
 
 
-def durations(sd, cfg, h, lengths, g, sdp_noise, noise_scale_w, length_scale):
-    """logw of either duration predictor, then w = exp(logw) * mask * length_scale (float64)"""
+def logw(sd, cfg, h, lengths, g, sdp_noise, noise_scale_w):
+    """logw [B, 1, T] of either duration predictor on the encoder output h, conditioned on g [B, gin] when given"""
     m = mask_of(lengths, h.shape[2])
     gb = conv(sd, "dp.cond", g[:, :, None]) if g is not None else 0
     if cfg["use_sdp"]:
@@ -166,13 +176,17 @@ def durations(sd, cfg, h, lengths, g, sdp_noise, noise_scale_w, length_scale):
             hh = ddsconv(sd, f"dp.flows.{f}.convs.", conv(sd, f"dp.flows.{f}.pre", z[:, c0:c0 + 1]) + x, lengths)
             z = convflow_spline(sd, f, hh, z, lengths, c0, c1)
             c0, c1 = c1, c0
-        logw = (z[:, :1] - _d(sd["dp.flows.0.m"])[0, 0]) * torch.exp(-_d(sd["dp.flows.0.logs"])[0, 0]) * m
-    else:
-        x = h + gb
-        x = layer_norm(sd, "dp.norm_1", torch.relu(conv(sd, "dp.conv_1", x * m)))
-        x = layer_norm(sd, "dp.norm_2", torch.relu(conv(sd, "dp.conv_2", x * m)))
-        logw = conv(sd, "dp.proj", x * m) * m
-    return torch.exp(logw) * m * length_scale
+        return (z[:, :1] - _d(sd["dp.flows.0.m"])[0, 0]) * torch.exp(-_d(sd["dp.flows.0.logs"])[0, 0]) * m
+    x = h + gb
+    x = layer_norm(sd, "dp.norm_1", torch.relu(conv(sd, "dp.conv_1", x * m)))
+    x = layer_norm(sd, "dp.norm_2", torch.relu(conv(sd, "dp.conv_2", x * m)))
+    return conv(sd, "dp.proj", x * m) * m
+
+
+def durations(sd, cfg, h, lengths, g, sdp_noise, noise_scale_w, length_scale):
+    """w = exp(logw) * mask * length_scale (float64)"""
+    m = mask_of(lengths, h.shape[2])
+    return torch.exp(logw(sd, cfg, h, lengths, g, sdp_noise, noise_scale_w)) * m * length_scale
 
 
 # ---- prior expansion, flow, decoder -----------------------------------------------------------------------------------
@@ -206,19 +220,23 @@ def wn_layer(sd, e, l, h, out, cond, lengths):
     return h, out + rs
 
 
-def flow_reverse(sd, z, y_len, g):
+def coupling_reverse(sd, f: int, z, y_len, g):
+    """ResidualCouplingLayer flow.flows.(2f) in reverse on z [B, inter, T] (no flip), conditioned on g [B, gin] when given"""
     I = z.shape[1]
     m = mask_of(y_len, z.shape[2])
-    for f in (6, 4, 2, 0):
-        z = torch.flip(z, [1])
-        n = f"flow.flows.{f}"
-        h = conv(sd, n + ".pre", z[:, :I // 2]) * m
-        cond = conv(sd, n + ".enc.cond_layer", g[:, :, None])[:, :, 0] if g is not None else None
-        out = None
-        for l in range(4):
-            h, out = wn_layer(sd, n + ".enc.", l, h, out, cond, y_len)
-        stats = conv(sd, n + ".post", out * m) * m
-        z = torch.cat([z[:, :I // 2], (z[:, I // 2:] - stats) * m], 1)
+    n = f"flow.flows.{2 * f}"
+    h = conv(sd, n + ".pre", z[:, :I // 2]) * m
+    cond = conv(sd, n + ".enc.cond_layer", g[:, :, None])[:, :, 0] if g is not None else None
+    out = None
+    for l in range(4):
+        h, out = wn_layer(sd, n + ".enc.", l, h, out, cond, y_len)
+    stats = conv(sd, n + ".post", out * m) * m
+    return torch.cat([z[:, :I // 2], (z[:, I // 2:] - stats) * m], 1)
+
+
+def flow_reverse(sd, z, y_len, g):
+    for f in (3, 2, 1, 0):
+        z = coupling_reverse(sd, f, torch.flip(z, [1]), y_len, g)
     return z
 
 

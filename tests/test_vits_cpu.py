@@ -114,3 +114,66 @@ def test_float64_restatement_against_goldens(name):
         assert rel(r[k], g[k]) <= 1e-5, (k, rel(r[k], g[k]))
     assert r["o"].shape == g["o"].shape
     assert rel(r["o"], g["o"]) <= 1e-5, rel(r["o"], g["o"])
+
+
+def _golden_case(name):
+    sys.path.insert(0, str(ROOT / "oracle"))
+    import vits_oracle as vo
+
+    g = np.load(GOLDEN / f"vits_{name}.npz")
+    cfg = CASE_CFG[name]
+    return vo, g, cfg, ri.vits_state_dict(cfg, int(g["seed"]))
+
+
+@pytest.mark.parametrize("name", ["toy", "full_sdp", "full_dp", "toy_1spk"])
+def test_oracle_stages_compose_to_the_whole_chain(name):
+    """the stage functions the kernel tests call (text_encoder_layer, logw, coupling_reverse), composed by hand on the goldens'
+    inputs, give the whole-chain functions bit for bit, so the golden pin above covers them"""
+    vo, g, cfg, sd = _golden_case(name)
+    lens = torch.as_tensor(g["x_lengths"]).long()
+    x = torch.from_numpy(g["x"])
+    T = x.shape[1]
+    m = vo.mask_of(lens, T)
+    with torch.no_grad():
+        h_ref, m_p, logs_p = vo.text_encoder(sd, cfg, x, lens, g["emo"])
+        e = vo._d(g["emo"]) @ vo._d(sd["enc_p.emo_proj.weight"]).T + vo._d(sd["enc_p.emo_proj.bias"])
+        h = (vo._d(sd["enc_p.emb.weight"])[x.long()] * np.sqrt(cfg["hidden_channels"]) + e[:, None, :]).transpose(1, 2) * m
+        for l in range(cfg["n_layers"]):
+            h = vo.text_encoder_layer(sd, cfg, l, h, lens, l == cfg["n_layers"] - 1)
+        assert torch.equal(h, h_ref)
+        gv = vo._d(sd["emb_g.weight"])[torch.as_tensor(g["sid"]).long()] if cfg["n_speakers"] > 1 else None
+        lw = vo.logw(sd, cfg, h, lens, gv, g["sdp_noise"], float(g["noise_scale_w"]))
+        ls = float(g["length_scale"])
+        assert lw.shape == (x.shape[0], 1, T) and (lw * (1 - m) == 0).all()
+        assert torch.equal(torch.exp(lw) * m * ls, vo.durations(sd, cfg, h, lens, gv, g["sdp_noise"], float(g["noise_scale_w"]), ls))
+        z_p = torch.from_numpy(g["z_p"]).double()
+        y_len = torch.as_tensor(g["y_lengths"]).long()
+        z = z_p
+        for f in (3, 2, 1, 0):
+            z = vo.coupling_reverse(sd, f, torch.flip(z, [1]), y_len, gv)
+        assert torch.equal(z, vo.flow_reverse(sd, z_p, y_len, gv))
+
+
+def test_banded_attention_equals_the_dense_statement():
+    """vo.rel_attention adds the relative terms on the 2W+1 diagonals; the dense statement builds the [T, T, dk] relative
+    embeddings, zero outside the window"""
+    sys.path.insert(0, str(ROOT / "oracle"))
+    import vits_oracle as vo
+
+    g = torch.Generator().manual_seed(0)
+    for T, nh, H, lens in ((1, 2, 16, [1, 1]), (5, 2, 16, [5, 3]), (9, 3, 24, [9, 1]), (40, 1, 32, [40, 17])):
+        q, k, v = (torch.randn(2, H, T, generator=g, dtype=torch.float64) for _ in range(3))
+        erk, erv = torch.randn(1, 9, H // nh, generator=g), torch.randn(1, 9, H // nh, generator=g)
+        dk = H // nh
+        qh, kh, vh = (a.view(2, nh, dk, T).transpose(2, 3) for a in (q / np.sqrt(dk), k, v))
+        rel = torch.arange(T)[None, :] - torch.arange(T)[:, None]
+        inside = (rel.abs() <= vo.WINDOW)[..., None]
+        idx = rel.clamp(-vo.WINDOW, vo.WINDOW) + vo.WINDOW
+        rk, rv = erk.double()[0][idx] * inside, erv.double()[0][idx] * inside
+        sc = qh @ kh.transpose(2, 3) + torch.einsum("bhtd,tsd->bhts", qh, rk)
+        mk = vo.mask_of(lens, T)[:, 0]
+        sc = torch.where((mk[:, None, :, None] * mk[:, None, None, :]) > 0, sc, torch.full_like(sc, -1e4))
+        p = torch.softmax(sc, -1)
+        dense = (p @ vh + torch.einsum("bhts,tsd->bhtd", p, rv)).transpose(2, 3).reshape(2, H, T)
+        got = vo.rel_attention(q, k, v, erk, erv, torch.tensor(lens), nh)
+        assert (got - dense).abs().max() <= 1e-13 * dense.abs().max(), T
